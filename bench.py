@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py — benchmark of the B200-native DiskANN distance hot path (greedy search over a Vamana graph).
+"""bench.py — benchmark of the H100-native DiskANN distance hot path (greedy search over a Vamana graph).
 
 Headline metric (BASELINE.json): QPS at recall@10 >= 0.95 on synthetic 1M x 128 f32 L2 (R=64, max
 degree 83, L_build=100, alpha=1.2, L_search=100, batches of 10K queries, beam 1), plus the achieved
@@ -20,6 +20,8 @@ bits, result counts, cmps, hops).
 Multi-GPU: one process per GPU (torchrun); rank 0 builds the index, vectors and adjacency are
 replicated with NCCL broadcasts at load, every rank searches its own query shard with no
 collective on the search path.  --scaling weak: 10K queries per GPU; --scaling strong: 10K in total.
+--dump-outputs DIR: after the timed steps, what the last step of the timed device path returned
+(ids, dists, counts, cmps, hops of this rank's query shard) as DIR/<name>.npy, float32 / float64.
 """
 import argparse
 import ctypes as C
@@ -47,9 +49,10 @@ WORKLOADS = {
     # configs[3]: i8 rows, PQ 32 x 256 traversal (codes are the only rows read per candidate) + full-precision rerank
     "c4_10Mx128_i8_pq32": dict(n=10_000_000, dim=128, dtype="i8", metric="l2", nq=10_000, centers=4096, R=64, l_build=100,
                                l_search=100, path="pq", pq_chunks=32, pq_train=256_000, int_scale=25.0),
-    # configs[4] shape (index replicated per GPU); --n-points scales it to what the run window allows
-    "c5_100Mx96_f32_l2": dict(n=100_000_000, dim=96, dtype="f32", metric="l2", nq=10_000, centers=16384, R=64, l_build=100,
-                              l_search=100, path="fp"),
+    # configs[4] shape (index replicated per GPU), sized for one 80 GB H100: 40M rows (15.4 GB) + adjacency (13.4 GB)
+    # + the bf16 operand of the tensor-core ground-truth scan (25.6 GB); --n-points scales it
+    "c5_40Mx96_f32_l2": dict(n=40_000_000, dim=96, dtype="f32", metric="l2", nq=10_000, centers=16384, R=64, l_build=100,
+                             l_search=100, path="fp"),
     "small_100Kx128_f32_l2": dict(n=100_000, dim=128, dtype="f32", metric="l2", nq=10_000, centers=256, R=64, l_build=100,
                                   l_search=100, path="fp"),
     "small_200Kx128_i8_pq32": dict(n=200_000, dim=128, dtype="i8", metric="l2", nq=10_000, centers=256, R=64, l_build=100,
@@ -142,7 +145,7 @@ def host_cores():
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -195,7 +198,7 @@ def measured_peak_gbs():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 def ncu_traffic(workload):
@@ -344,7 +347,7 @@ def run_gpu(args):
 
     # ground truth: exhaustive scan on the device (bit-identical distances), cross-checked below
     t0 = time.time()
-    # (large indexes: the tcgen05 scan — tensor-core candidate selection + exact re-scoring, same answer)
+    # (large indexes: the wgmma scan — tensor-core candidate selection + exact re-scoring, same answer)
     flat = g.flat_knn_tc if n >= 2_000_000 else g.flat_knn
     gts = [flat(q, K)[0] for q in batches]
     t_gt = time.time() - t0
@@ -404,8 +407,8 @@ def run_gpu(args):
     # ---- batches in flight (dab_search_batch_async / dab_wait): SLOTS consecutive steps overlap, each on its own
     # slot (stream + visited tables + result buffers), so the draining tail of one batch is filled by the CTAs of
     # the next and, end to end, the copies of one batch run under the kernel of another
-    # default: two batches in flight; a strong-scaled shard smaller than half the resident workers (~3400 one-warp
-    # CTAs) keeps four, so that consecutive 10K-query steps still fill the GPU (profiles/r02_nq_sweep_strong_scaling_shares.txt)
+    # default: two batches in flight; a strong-scaled shard of fewer than 5000 queries keeps four, so that
+    # consecutive steps still fill the GPU
     in_flight = args.in_flight or (4 if nq < 5000 else 2)
     slots = 1 if is_pq else max(1, min(in_flight, dab.MAX_SLOTS))
     sd = [dict(ids=torch.empty((nq, K), dtype=torch.int32, device="cuda"), dists=torch.empty((nq, K), dtype=torch.float32, device="cuda"),
@@ -464,9 +467,13 @@ def run_gpu(args):
         sampler.start()
     if args.profile_range:  # ncu --profile-from-start off: only the timed region is captured
         torch.cuda.profiler.start()
+    def fetch(o):
+        return {name: o[name].cpu().numpy() for name in ("ids", "dists", "counts", "cmps", "hops")}
+
     step_no[0] = 0
     ms_dev_serial = timed(step_device, args.steps, args.warmup)
     launches = timed.launches
+    last_out = fetch(dict(ids=d_ids, dists=d_dists, counts=d_counts, cmps=d_cmps, hops=d_hops))
     step_no[0] = 0
     ms_e2e_serial = timed(step_e2e, args.steps, args.warmup)
     ms_dev, ms_e2e = ms_dev_serial, ms_e2e_serial
@@ -474,6 +481,7 @@ def run_gpu(args):
         step_no[0] = 0
         ms_dev = timed(step_device_async, args.steps, args.warmup, drain)
         launches = timed.launches
+        last_out = fetch(sd[(args.warmup + args.steps - 1) % slots])  # the slot the last timed step ran on
         step_no[0] = 0
         ms_e2e = timed(step_e2e_async, args.steps, args.warmup, drain)
     if args.profile_range:
@@ -550,7 +558,7 @@ def run_gpu(args):
                          + f"; seeds base {SEED_BASE:#x} queries {SEED_QUERY:#x}+97*batch; start = copy of the medoid",
             "index": "built on rank 0 by dab_build (device); vectors, adjacency (and PQ) replicated by one NCCL broadcast each inside the library",
             "parallelism": f"replica x{world}, queries sharded ({args.scaling}), no collective on the search path",
-            "l2_policy": f"no flush: index {(n * dim * ELEM[cfg['dtype']] + (n + 1) * 4 * (md + 1)) / 1e6:.0f} MB >> 126 MB L2, "
+            "l2_policy": f"no flush: index {(n * dim * ELEM[cfg['dtype']] + (n + 1) * 4 * (md + 1)) / 1e6:.0f} MB >> 50 MB L2, "
                          f"{NB} query batches rotate and each step gathers GBs of random rows",
             "batches_in_flight": slots,
             "serial": {"ms_per_step": ms_dev_serial / args.steps, "e2e_ms_per_step": ms_e2e_serial / args.steps,
@@ -581,7 +589,17 @@ def run_gpu(args):
         dist.barrier()
         dist.destroy_process_group()
     if rank == 0:
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, last_out)
         emit(result)
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes each array as <out_dir>/<name>.npy: float32 stays float32, integers become float64 (exact)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        np.save(os.path.join(out_dir, f"{name}.npy"), a if a.dtype == np.float32 else a.astype(np.float64))
 
 
 # ------------------------------------------------------------------------------------------ CPU oracle legs
@@ -793,6 +811,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-parity", action="store_true", help="skip the oracle parity gate (tuning runs only)")
     ap.add_argument("--profile-range", action="store_true", help="cudaProfilerStart/Stop around the timed region (for ncu)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write what the last timed step returned (ids, dists, counts, cmps, hops) as DIR/<name>.npy")
     ap.add_argument("--prepare-only", default="", help=argparse.SUPPRESS)
     args = ap.parse_args()
     if args.warmup < 3:

@@ -1,4 +1,4 @@
-"""diskann_b200 — B200-native (sm_100a) batched distance hot path for microsoft/DiskANN.
+"""diskann_b200 — H100-native (sm_90a) batched distance hot path for microsoft/DiskANN.
 
 The package is a thin host-side mirror of the reference interface for this path over the C ABI
 in include/diskann_b200.h (libdiskann_b200.so).  It holds no CPU implementation: importing

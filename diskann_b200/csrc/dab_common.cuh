@@ -1,5 +1,5 @@
 // dab_common.cuh — shared host-side plumbing for libdiskann_b200.so (index handle, error
-// reporting, launch accounting).  Compiled for sm_100a only.
+// reporting, launch accounting).  Compiled for sm_90a (H100) only.
 #pragma once
 
 #include <cuda_fp16.h>
@@ -68,7 +68,7 @@ struct Tuning {
     bool v2_full_grid = false;     // DAB_V2_FULL_GRID: launch every resident worker instead of balancing the rounds per worker
     int v2_slots = 0;              // DAB_V2_SLOTS: cap on the visited-table slots per warp (smaller tables, more overflow re-runs)
     int v3_table_bytes = 0;        // DAB_V3_TABLE_BYTES: visited-table bytes per warp
-    bool tc_resident = false;      // DAB_TC_RESIDENT: tensor-core scan keeps the query tile in shared memory (measured equal to streaming it)
+    bool tc_resident = false;      // DAB_TC_RESIDENT: tensor-core scan keeps the query tile in shared memory
     int pq_ctas_per_sm = 0;        // DAB_PQ_CTAS_PER_SM: resident CTAs (4 warps) per SM of the PQ traversal kernel (default 6)
     bool pq_global_lut = false;    // DAB_PQ_GLOBAL_LUT: PQ traversal with the per-warp table in global memory (search_kernel_pq) also where search_kernel_pqs fits
     bool pq_no_spec = false;       // DAB_PQ_NO_SPEC: search_kernel_pqs without the adjacency row copied one hop ahead (L2 prefetch of the row only)
@@ -91,7 +91,7 @@ struct dab_index {
     uint32_t n_start = 0;
     uint32_t max_degree = 0;
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
 
     cudaStream_t stream = nullptr;      // stream in use
     cudaStream_t own_stream = nullptr;  // library-created

@@ -617,7 +617,7 @@ int dab_pair_distances(int dtype_x, int dtype_y, int metric, uint32_t dim, const
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
         return fail(DAB_ERR_NO_DEVICE, "dab_pair_distances: no CUDA device visible (no CPU fallback)");
     DAB_CUDA(cudaSetDevice(device));
-    int sm = 148;
+    int sm = 132;
     cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, device);
     // rows are padded to 4 bytes on the device so the integer kernels can use word loads
     const size_t xb = (size_t)dim * elem_size(dtype_x), yb = (size_t)dim * elem_size(dtype_y);

@@ -1,22 +1,23 @@
-// flat_tc.cu — exhaustive scan (diskann/src/flat, ground truth for recall) on the 5th-generation
-// tensor cores: the query x base distance block is a dense contraction, so it runs as a
-// tcgen05.mma GEMM with TMA-staged tiles and a fused norm expansion + per-row candidate selection
+// flat_tc.cu — exhaustive scan (diskann/src/flat, ground truth for recall) on the Hopper tensor
+// cores: the query x base distance block is a dense contraction, so it runs as a wgmma GEMM with
+// TMA-staged tiles and a fused norm expansion + per-row candidate selection
 // (BASELINE.json north_star; SURVEY.md §8f.3).
 //
 //   * operands are bf16.  f32 / f16 rows are split x = hi + lo (hi = bf16(x), lo = bf16(x - hi)) and
 //     the three significant products are obtained from ONE GEMM over a 3x longer K:
 //     A' = [q_hi | q_hi | q_lo], B' = [b_hi | b_lo | b_hi]  =>  A'.B' = hi.hi + hi.lo + lo.hi
-//     (relative error of the dot product ~2^-16; fp32 accumulation in TMEM).  i8 / u8 rows are exact
-//     in bf16 and their products / sums are exact in fp32 (128 * 127^2 < 2^24): one segment.
+//     (relative error of the dot product ~2^-16; fp32 accumulation in registers).  i8 / u8 rows are
+//     exact in bf16 and their products / sums are exact in fp32 (128 * 127^2 < 2^24): one segment.
 //   * one CTA = 128 query rows x a range of base rows; per 128-column tile: K' / 64 pipeline stages
 //     of (A k-block, B k-block) 128 x 64 bf16 tiles loaded by TMA (128-byte swizzle) into shared
-//     memory, 4 x tcgen05.mma (M 128, N 128, K 16, cta_group::1) per stage issued by one thread,
-//     accumulators double-buffered in TMEM (2 x 128 columns) so the epilogue of tile t overlaps the
-//     MMAs of tile t + 1;
-//   * epilogue (4 warps = the 4 TMEM lane quarters, one query row per thread): tcgen05.ld the 128
-//     accumulators of the row, score = alpha[col] * dot + beta[col] (L2: ||b||^2 - 2 q.b, the ||q||^2
-//     term is constant per row; inner product: -q.b; cosine: -q.b / ||b||), keep the KP best columns of
-//     the row in a small per-thread set;
+//     memory by a producer warp, and 4 k-steps x 2 row halves of wgmma.m64n128k16 per stage issued by
+//     one consumer warpgroup, whose 128 threads hold the 128 x 128 f32 accumulator tile (2 x 64
+//     registers each); the producer runs up to a whole pipeline of stages ahead, so the loads of the
+//     next tile overlap the epilogue of this one;
+//   * epilogue (the consumer warpgroup): score = alpha[col] * dot + beta[col] (L2: ||b||^2 - 2 q.b, the
+//     ||q||^2 term is constant per row; inner product: -q.b; cosine: -q.b / ||b||), transposed through
+//     shared memory 32 columns at a time so that each thread owns one query row, which keeps the KP best
+//     columns of the row in a small per-thread set;
 //   * the KP candidates of every (query, base range) are then re-scored with the exact, reference-order
 //     distance kernel (launch_frontier) and the final top-k is taken by (distance, id) — so the
 //     returned distances are bit-identical to the exact scan and the ids are the exact scan's as long
@@ -40,7 +41,7 @@ constexpr int kBM = 128, kBN = 128, kBK = 64;  // CTA tile; one k-block = 64 bf1
 constexpr int kStages = 5;                    // streaming mode: stages of (A k-block, B k-block)
 constexpr int kStagesRes = 4;                 // A-resident mode: stages of B k-blocks only
 constexpr int kMaxResKb = 6;                  // A stays in shared memory when K' <= 6 x 64 (e.g. 3 x 128)
-constexpr int kTcThreads = 192;                // warp 0: TMA, warp 1: MMA + TMEM owner, warps 2-5: epilogue
+constexpr int kTcThreads = 160;                // warps 0-3: MMA + epilogue warpgroup, warp 4: TMA
 constexpr int kKP = 32;                        // largest candidate set per (query row, base range); k <= 10 uses 16
 constexpr uint32_t kTileBytes = kBM * kBK * 2; // 16 KB per operand tile
 
@@ -75,41 +76,42 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* ba
                  : "memory");
 }
 // K-major operand tile [rows][64 bf16] written by TMA with the 128-byte swizzle: 8-row groups of
-// 1024 bytes (SBO = 64 x 16 B), LBO = 1, descriptor version 1, layout SWIZZLE_128B
-// (cute/arch/mma_sm100_desc.hpp SmemDescriptor; cute/atom/mma_traits_sm100.hpp make_umma_desc<Major::K>)
-__device__ __forceinline__ uint64_t umma_desc(const void* tile, uint32_t k_byte_offset) {
+// 1024 bytes (SBO = 1024 B), LBO unused (1), layout type 1 = SWIZZLE_128B (PTX ISA, "Matrix Descriptor
+// Format" of wgmma); a k-step of 16 elements advances the start address by 32 bytes inside the swizzle row
+__device__ __forceinline__ uint64_t gmma_desc(const void* tile, uint32_t k_byte_offset) {
     const uint32_t addr = smem_u32(tile) + k_byte_offset;
-    return (uint64_t)((addr >> 4) & 0x3FFFu) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+    return (uint64_t)((addr >> 4) & 0x3FFFu) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-// kind::f16, A = B = bf16 (format 1), D = f32 (format 1), both K-major, M = 128, N = 128
-__device__ __forceinline__ uint32_t umma_idesc() {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(kBN >> 3) << 17) | ((uint32_t)(kBM >> 4) << 24);
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+// D[64 x 128] (+)= A[64 x 16] . B[128 x 16]^T, bf16 inputs from shared memory (both K-major), f32 accumulators.
+// Fragment of thread t of the warpgroup: d[4j + r] is row 16 (t / 32) + (t % 32) / 4 + 8 (r / 2),
+// column 8 j + 2 (t % 4) + (r % 2).
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, "
+        "%47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t"
+        "}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+          "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+          "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+          "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),
+          "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),
+          "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),
+          "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {  // arrives on `bar` when every MMA issued so far has completed
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving accesses of the accumulators across the asynchronous MMAs
+__device__ __forceinline__ void fence_operands(float (&d)[64]) {
+#pragma unroll
+    for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-          "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-          "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]),
-          "=r"(r[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ---- operand preparation --------------------------------------------------------------------
 // rows of the index dtype -> bf16 [n][kp]: f32 / f16: (hi, hi, lo) for queries, (hi, lo, hi) for base
@@ -182,17 +184,14 @@ flat_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint8_t* sa = smem;                                              // RES: kMaxResKb x 16 KB (whole A tile); else kStages x 16 KB
     uint8_t* sb = smem + (RES ? kMaxResKb : kStages) * kTileBytes;   // kSt x 16 KB
-    float* s_coef = reinterpret_cast<float*>(sb + kSt * kTileBytes);  // [2 accumulators][alpha 128 | beta 128]
-    float* s_scores = s_coef + 2 * 2 * kBN;                                      // [128 epilogue threads][33]: private scratch rows
+    float* s_coef = reinterpret_cast<float*>(sb + kSt * kTileBytes);  // [alpha 128 | beta 128] of the current tile
+    float* s_scores = s_coef + 2 * kBN;                                          // [128 query rows][33]: 32 scores per row
     float* s_cd = s_scores + 128 * 33;                                           // [KP][128]: candidate scores, entry-major (conflict-free)
     uint32_t* s_ci = reinterpret_cast<uint32_t*>(s_cd + KP * 128);               // [KP][128]: candidate ids
     uint64_t* bars = reinterpret_cast<uint64_t*>(s_ci + KP * 128);               // offsets stay 8-byte aligned
     uint64_t* full = bars;                  // [kSt] TMA -> MMA
     uint64_t* empty = bars + kSt;           // [kSt] MMA -> TMA
-    uint64_t* tfull = bars + 2 * kSt;       // [2] MMA -> epilogue
-    uint64_t* tempty = tfull + 2;           // [2] epilogue -> MMA
-    uint64_t* afull = tempty + 2;           // [1] resident A tile has landed
-    uint32_t* s_tmem = reinterpret_cast<uint32_t*>(afull + 1);
+    uint64_t* afull = bars + 2 * kSt;       // [1] resident A tile has landed
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t m0 = blockIdx.y * kBM;
@@ -204,27 +203,16 @@ flat_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     if (threadIdx.x == 0) {
         for (int s = 0; s < kSt; ++s) {
             mbar_init(full + s, 1);
-            mbar_init(empty + s, 1);
+            mbar_init(empty + s, 4);  // one arrival per consumer warp
         }
         mbar_init(afull, 1);
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(tfull + a, 1);
-            mbar_init(tempty + a, 4);  // one arrival per epilogue warp
-        }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
     }
-    if (warp == 1) {  // TMEM: 256 columns = two 128-column f32 accumulators
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(s_tmem)), "r"(256u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *s_tmem;
 
-    if (warp == 0) {
+    if (warp == 4) {
         // ===== TMA producer (one lane) =====
         if (lane == 0) {
             uint32_t stage = 0, phase = 0;
@@ -245,87 +233,72 @@ flat_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer (one lane) =====
-        if (lane == 0) {
-            const uint32_t idesc = umma_idesc();
-            uint32_t stage = 0, phase = 0;
-            if (RES) mbar_wait(afull, 0);
-            for (uint32_t t = t0; t < t1; ++t) {
-                const uint32_t acc = (t - t0) & 1, use = (t - t0) >> 1;
-                mbar_wait(tempty + acc, (use & 1) ^ 1);  // the epilogue has drained this accumulator
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t tmem_d = tmem_base + acc * kBN;
-                for (uint32_t kb = 0; kb < kblocks; ++kb) {
-                    mbar_wait(full + stage, phase);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-                    for (int k = 0; k < kBK / 16; ++k) {
-                        const uint64_t da = umma_desc(sa + (RES ? kb : stage) * kTileBytes, k * 32);
-                        const uint64_t db = umma_desc(sb + stage * kTileBytes, k * 32);
-                        umma_f16(tmem_d, da, db, idesc, (kb | (uint32_t)k) != 0 ? 1u : 0u);
-                    }
-                    umma_commit(empty + stage);  // frees the stage once these MMAs have read it
-                    if (++stage == kSt) {
-                        stage = 0;
-                        phase ^= 1;
-                    }
-                }
-                umma_commit(tfull + acc);  // accumulator complete
-            }
-        }
     } else {
-        // ===== epilogue: warps 2..5 own TMEM lane quarters (warp % 4), one query row per thread =====
-        const uint32_t quarter = (uint32_t)warp & 3u;
-        const uint32_t row = quarter * 32 + lane;  // row of the 128-row tile == TMEM lane
+        // ===== consumer warpgroup: MMAs into registers, then the epilogue with one query row per thread =====
+        const uint32_t row = threadIdx.x;  // 0..127: row of the 128-row tile this thread selects for
         const uint32_t q = m0 + row;
-        const int et = (warp - 2) * 32 + lane;     // 0..127 among the epilogue threads
-        float* my_scores = s_scores + et * 33;      // stride 33: conflict-free rows
-        float* cd = s_cd + et;        // entry e of this thread: cd[e * 128]
-        uint32_t* ci = s_ci + et;
+        float* my_scores = s_scores + row * 33;      // stride 33: conflict-free rows
+        float* cd = s_cd + row;        // entry e of this thread: cd[e * 128]
+        uint32_t* ci = s_ci + row;
         uint32_t cn = 0;
         float worst = -1.0f;   // largest kept score (valid when cn == KP)
         int worst_at = 0;
-        // per-column score coefficients (alpha, beta): tile t's are in s_coef[t & 1]; the next tile's are
-        // fetched from global memory while this tile is processed
-        auto load_coef = [&](uint32_t t, float& a, float& b) {
-            const uint32_t col = t * kBN + et;
-            a = col < p.n_base ? p.alpha[col] : 0.0f;
-            b = col < p.n_base ? p.beta[col] : __int_as_float(0x7F800000);
-        };
-        {
-            float a, b;
-            load_coef(t0, a, b);
-            s_coef[et] = a;
-            s_coef[kBN + et] = b;
-        }
+        float acc[2][64];      // rows [0, 64) and [64, 128) of the tile
+        uint32_t stage = 0, phase = 0;
+        if (RES) mbar_wait(afull, 0);
         for (uint32_t t = t0; t < t1; ++t) {
-            const uint32_t acc = (t - t0) & 1, use = (t - t0) >> 1;
-            float* coef = s_coef + acc * 2 * kBN;
-            float a_next = 0.0f, b_next = 0.0f;
-            if (t + 1 < t1) load_coef(t + 1, a_next, b_next);
-            asm volatile("bar.sync 1, 128;" ::: "memory");  // coef[acc] written by everyone; coef[acc ^ 1] no longer read
-            mbar_wait(tfull + acc, use & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t taddr = tmem_base + acc * kBN + ((quarter * 32u) << 16);
-            uint32_t rbuf[2][32];
-            tmem_ld32(taddr, rbuf[0]);
+            {  // per-column score coefficients of this tile (the previous tile's readers passed the barriers below)
+                const uint32_t col = t * kBN + row;
+                s_coef[row] = col < p.n_base ? p.alpha[col] : 0.0f;
+                s_coef[kBN + row] = col < p.n_base ? p.beta[col] : __int_as_float(0x7F800000);
+            }
+            for (uint32_t kb = 0; kb < kblocks; ++kb) {
+                mbar_wait(full + stage, phase);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < kBK / 16; ++k) {
+                    const uint64_t db = gmma_desc(sb + stage * kTileBytes, k * 32);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const uint64_t da = gmma_desc(sa + (RES ? kb : stage) * kTileBytes + h * (kTileBytes / 2), k * 32);
+                        wgmma_m64n128k16(acc[h], da, db, (kb | (uint32_t)k) != 0 ? 1u : 0u);
+                    }
+                }
+                wgmma_commit();
+                wgmma_wait_all();
+                fence_operands(acc[0]);
+                fence_operands(acc[1]);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(empty + stage);  // this warp's MMAs have read the stage
+                if (++stage == kSt) {
+                    stage = 0;
+                    phase ^= 1;
+                }
+            }
+            asm volatile("bar.sync 1, 128;" ::: "memory");  // s_coef written by everyone
 #pragma unroll
             for (int cc = 0; cc < kBN / 32; ++cc) {
                 const int c0 = cc * 32;
-                uint32_t (&r)[32] = rbuf[cc & 1];
-                tmem_ld_wait();
-                if (cc + 1 < kBN / 32) tmem_ld32(taddr + c0 + 32, rbuf[(cc + 1) & 1]);  // next chunk in flight during this one
-                // fast path, branch-free: the 32 scores go to this thread's scratch row and a bit mask
-                // marks the ones that beat the current threshold (all of them while the set fills)
+                // the scores of columns [c0, c0 + 32) of this thread's accumulator fragment, into their rows' scratch
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+#pragma unroll
+                        for (int r = 0; r < 4; ++r) {
+                            const int fr = h * 64 + warp * 16 + (lane >> 2) + 8 * (r >> 1);
+                            const int fc = 8 * j + 2 * (lane & 3) + (r & 1);
+                            s_scores[fr * 33 + fc] = fmaf(acc[h][4 * (cc * 4 + j) + r], s_coef[c0 + fc], s_coef[kBN + c0 + fc]);
+                        }
+                    }
+                }
+                asm volatile("bar.sync 1, 128;" ::: "memory");
+                // fast path, branch-free: a bit mask marks the scores that beat the current threshold (all of
+                // them while the set fills)
                 uint32_t mask = 0;
                 const float thr = cn < (uint32_t)KP ? __int_as_float(0x7F800000) : worst;
 #pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const float sc = fmaf(__uint_as_float(r[j]), coef[c0 + j], coef[kBN + c0 + j]);
-                    my_scores[j] = sc;
-                    mask |= sc < thr ? (1u << j) : 0u;
-                }
+                for (int j = 0; j < 32; ++j) mask |= my_scores[j] < thr ? (1u << j) : 0u;
                 // slow path (rare once the threshold has settled): one candidate at a time
                 while (mask) {
                     const int j = __ffs(mask) - 1;
@@ -352,14 +325,7 @@ flat_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                     for (int e = 1; e < KP; ++e)
                         if (v[e] > worst) worst = v[e], worst_at = e;
                 }
-            }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tempty + acc);
-            if (t + 1 < t1) {
-                float* nxt = s_coef + (acc ^ 1u) * 2 * kBN;
-                nxt[et] = a_next;
-                nxt[kBN + et] = b_next;
+                asm volatile("bar.sync 1, 128;" ::: "memory");  // scratch rows free for the next 32 columns
             }
         }
         if (q < p.nq) {
@@ -367,9 +333,6 @@ flat_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             for (uint32_t e = 0; e < (uint32_t)KP; ++e) out[e] = e < cn ? ci[e * 128] : kNoId;
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256u) : "memory");
 }
 
 // exact distances of the candidates -> top-k by (distance, id); one warp per query
@@ -519,11 +482,10 @@ int dab_flat_knn_tc(dab_index* idx, const void* queries, uint32_t nq, uint32_t k
     p.alpha = (const float*)idx->d_tc_coef;
     p.beta = (const float*)idx->d_tc_coef + n;
     p.cand = (uint32_t*)idx->s_ids.p;
-    // resident query tile: halves the L2 -> SM operand traffic (12.4 -> 7.1 GB for 1000 x 1M), which bounds the
-    // kernel once the epilogue is out of the way (9.3 TB/s measured in streaming mode)
+    // resident query tile (DAB_TC_RESIDENT): halves the L2 -> SM operand traffic (12.4 -> 7.1 GB for 1000 x 1M)
     const bool resident = idx->tune.tc_resident && kp / kBK <= (uint32_t)kMaxResKb;
     const size_t tiles_smem = resident ? (size_t)(kMaxResKb + kStagesRes) * kTileBytes : 2 * (size_t)kStages * kTileBytes;
-    const size_t smem = 1024 + tiles_smem + 2 * 2 * kBN * 4 + 128 * 33 * 4 + 2 * (size_t)kp_sel * 128 * 4 + (2 * (size_t)kStages + 5) * 8 + 16;
+    const size_t smem = 1024 + tiles_smem + 2 * kBN * 4 + 128 * 33 * 4 + 2 * (size_t)kp_sel * 128 * 4 + (2 * (size_t)kStages + 1) * 8;
 #define DAB_TC_LAUNCH(RES_, KP_)                                                                                        \
     do {                                                                                                                \
         DAB_CUDA(cudaFuncSetAttribute(flat_tc_kernel<RES_, KP_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \

@@ -424,7 +424,7 @@ int dab_minmax_compress(int device, float grid_scale, uint32_t dim, int nbits, c
         e = cudaFuncSetAttribute(minmax_compress_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e == cudaSuccess) {
             const uint64_t groups = (n + 31) / 32;
-            const int grid = (int)std::min<uint64_t>((groups + warps - 1) / warps, 148ull * 8);
+            const int grid = (int)std::min<uint64_t>((groups + warps - 1) / warps, 132ull * 8);
             minmax_compress_kernel<<<grid, warps * 32, smem>>>(p);
             DAB_LAUNCHED();
             e = cudaGetLastError();
@@ -475,7 +475,7 @@ int dab_minmax_distances(int device, int metric, int nbits_x, int nbits_y, uint3
         p.x = dx;
         p.y = dy;
         p.out = dout;
-        const int grid = (int)std::min<uint64_t>((n + 31) / 32, 148ull * 8);  // 8 warps x 4 pairs per CTA pass
+        const int grid = (int)std::min<uint64_t>((n + 31) / 32, 132ull * 8);  // 8 warps x 4 pairs per CTA pass
         minmax_distance_kernel<<<grid, 256>>>(p);
         DAB_LAUNCHED();
         e = cudaGetLastError();
@@ -529,7 +529,7 @@ int dab_minmax_query_distances(int device, int metric, int nbits, uint32_t dim, 
         DAB_LAUNCHED();
         const uint32_t lpp = nbits == 8 ? 1 : 8;
         const uint64_t pairs_per_cta = 256 / lpp;
-        const dim3 grid((unsigned)std::min<uint64_t>((n + pairs_per_cta - 1) / pairs_per_cta, 148ull * 8), nq);
+        const dim3 grid((unsigned)std::min<uint64_t>((n + pairs_per_cta - 1) / pairs_per_cta, 132ull * 8), nq);
         const size_t smem = (size_t)dim * 4;
         switch (nbits) {
             case 8: minmax_query_distance_kernel<8><<<grid, 256, smem>>>(p); break;

@@ -631,7 +631,7 @@ int dab_sq_compress(int device, const float* shift, float scale, uint32_t dim, i
     if (e == cudaSuccess) e = cudaMemcpy(d_vec, vectors, n * dim * 4, cudaMemcpyHostToDevice);
     int rc = DAB_OK;
     if (e == cudaSuccess) {
-        int grid = (int)std::min<uint64_t>((n + 127) / 128, 148ull * 16);
+        int grid = (int)std::min<uint64_t>((n + 127) / 128, 132ull * 16);
         sq_compress_kernel<<<grid, 128>>>(d_shift, scale, dim, nbits, d_vec, n, d_codes, d_comp);
         DAB_LAUNCHED();
         e = cudaGetLastError();
@@ -670,7 +670,7 @@ int dab_sq_distances(int device, int metric, int nbits, float scale_squared, flo
     if (e == cudaSuccess) e = cudaMemcpy(dcy, comp_y, n * 4, cudaMemcpyHostToDevice);
     int rc = DAB_OK;
     if (e == cudaSuccess) {
-        int grid = (int)std::min<uint64_t>((n + 7) / 8, 148ull * 8);
+        int grid = (int)std::min<uint64_t>((n + 7) / 8, 132ull * 8);
         sq_distance_kernel<<<grid, 256>>>(metric, nbits, scale_squared, shift_square_norm, dim, dx, dcx, dy, dcy, n, dout);
         DAB_LAUNCHED();
         e = cudaGetLastError();

@@ -177,18 +177,29 @@ __device__ __forceinline__ void merge_any(float* qd, uint32_t* qi, uint32_t cap,
 // ---- exact visited set: bucketed open addressing, 8 ids per 32-byte bucket ------------------
 // The tables are the only data of a search that is re-read (every hop probes ~R buckets of the
 // same 10-20 KB per-query table) while ~0.6 MB of vector rows stream past per query.  Bucket
-// loads therefore carry the L2 evict_last priority (one 256-bit coherent load per bucket) and
+// loads therefore carry the L2 evict_last priority (two 128-bit coherent loads per bucket) and
 // the row copies evict_first (search_kernel_v2.cu), so the streaming rows do not push the
 // tables out of L2 and every probe is an L2 hit instead of a DRAM sector.
 #ifndef DAB_L2_HINTS
 #define DAB_L2_HINTS 1
 #endif
 
+// sm_90 takes the L2 eviction priority of a 128-bit access as a cache policy operand
+__device__ __forceinline__ uint64_t l2_evict_last_policy() {
+    uint64_t pol;
+    asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+
 __device__ __forceinline__ void load_bucket(const uint32_t* bp, uint32_t (&s)[8]) {
 #if DAB_L2_HINTS
-    asm volatile("ld.relaxed.gpu.global.L2::evict_last.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(s[0]), "=r"(s[1]), "=r"(s[2]), "=r"(s[3]), "=r"(s[4]), "=r"(s[5]), "=r"(s[6]), "=r"(s[7])
-                 : "l"(bp));
+    const uint64_t pol = l2_evict_last_policy();
+    asm volatile("ld.relaxed.gpu.global.L2::cache_hint.v4.b32 {%0,%1,%2,%3}, [%4], %5;"
+                 : "=r"(s[0]), "=r"(s[1]), "=r"(s[2]), "=r"(s[3])
+                 : "l"(bp), "l"(pol));
+    asm volatile("ld.relaxed.gpu.global.L2::cache_hint.v4.b32 {%0,%1,%2,%3}, [%4], %5;"
+                 : "=r"(s[4]), "=r"(s[5]), "=r"(s[6]), "=r"(s[7])
+                 : "l"(bp + 4), "l"(pol));
 #else
     const uint4 lo = __ldcg(reinterpret_cast<const uint4*>(bp));
     const uint4 hi = __ldcg(reinterpret_cast<const uint4*>(bp) + 1);
@@ -199,7 +210,9 @@ __device__ __forceinline__ void load_bucket(const uint32_t* bp, uint32_t (&s)[8]
 // table-clear store of one 32-byte bucket, same priority as the probes
 __device__ __forceinline__ void store_empty_bucket(uint32_t* bp) {
 #if DAB_L2_HINTS
-    asm volatile("st.global.L2::evict_last.v8.b32 [%0], {%1,%1,%1,%1,%1,%1,%1,%1};" ::"l"(bp), "r"(kEmptyV2) : "memory");
+    const uint64_t pol = l2_evict_last_policy();
+    asm volatile("st.global.L2::cache_hint.v4.b32 [%0], {%1,%1,%1,%1}, %2;" ::"l"(bp), "r"(kEmptyV2), "l"(pol) : "memory");
+    asm volatile("st.global.L2::cache_hint.v4.b32 [%0], {%1,%1,%1,%1}, %2;" ::"l"(bp + 4), "r"(kEmptyV2), "l"(pol) : "memory");
 #else
     const uint4 e4 = make_uint4(kEmptyV2, kEmptyV2, kEmptyV2, kEmptyV2);
     reinterpret_cast<uint4*>(bp)[0] = e4;

@@ -33,7 +33,7 @@
 namespace dab {
 
 constexpr int kPqsMaxWarps = 16;
-constexpr size_t kPqsSmemLimit = 227 * 1024;  // opt-in dynamic shared memory of one CTA on sm_100
+constexpr size_t kPqsSmemLimit = 227 * 1024;  // opt-in dynamic shared memory of one CTA on sm_90
 
 template <int QT, int CL>
 __global__ void __launch_bounds__(kPqsMaxWarps * 32, 1) search_kernel_pqs(const SearchParamsPq p) {

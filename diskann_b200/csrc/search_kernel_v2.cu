@@ -15,11 +15,11 @@
 //     (xor 8, 16, [remainder], 4, 2, 1) — 9 shuffles per 8 rows;
 //   * the sorted candidate list lives in shared memory and a whole round of candidates is merged
 //     at once by rank (search_common.cuh), equivalent to the reference's sequential inserts;
-//   * all visited-set probes of an adjacency row are issued together (one 256-bit evict_last
-//     load per 8-id bucket); the adjacency row of the next-best unvisited candidate is copied
+//   * all visited-set probes of an adjacency row are issued together (two 128-bit evict_last
+//     loads per 8-id bucket); the adjacency row of the next-best unvisited candidate is copied
 //     into shared memory while the current hop runs, so the next hop usually starts without a
 //     global round trip;
-//   * the distance arithmetic advances two rows per instruction (packed f32x2 FADD2 / FFMA2).
+//   * the distance arithmetic is scalar f32, one row at a time (sm_90 has no packed f32x2 FADD2 / FFMA2).
 #include "dab_common.cuh"
 #include "distance_device.cuh"
 #include "search_common.cuh"
@@ -42,7 +42,7 @@ constexpr int kGroup = 8;  // rows reduced together
 #define DAB_V2_INT_BUILD 1  // i8 / u8 rows in search_kernel_v2 (exact integer distances); GPU-validated in round 2
 #endif
 #ifndef DAB_V2_F32X2
-#define DAB_V2_F32X2 1     // packed FADD2 / FFMA2 distance arithmetic
+#define DAB_V2_F32X2 0     // 1: rows advanced in pairs of 64-bit registers (same bits; no packed f32x2 arithmetic on sm_90)
 #endif
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -60,8 +60,8 @@ __device__ __forceinline__ void bfly8(float (&v)[kGroup], int lane, int bit) {
     }
 }
 
-// Packed f32x2 arithmetic (FADD2 / FFMA2 on sm_100): each half is an IEEE round-to-nearest
-// operation, so a pair of rows advances with one instruction and the same bits as two scalar ones.
+// A pair of rows carried as one 64-bit register pair.  sm_90 has no packed f32x2 arithmetic, so each
+// half is advanced by its own IEEE round-to-nearest scalar operation (the same bits as the unpaired code).
 __device__ __forceinline__ uint64_t pack2(float lo, float hi) {
     uint64_t r;
     asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
@@ -70,14 +70,19 @@ __device__ __forceinline__ uint64_t pack2(float lo, float hi) {
 __device__ __forceinline__ void unpack2(uint64_t v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
 template <int KIND>
 __device__ __forceinline__ uint64_t step2(uint64_t acc, uint64_t x2, uint64_t y2) {
+    float a0, a1, x0, x1, y0, y1;
+    unpack2(acc, a0, a1);
+    unpack2(x2, x0, x1);
+    unpack2(y2, y0, y1);
     if (KIND == KIND_L2) {
-        uint64_t c2;
-        asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(c2) : "l"(x2), "l"(y2));
-        asm("fma.rn.f32x2 %0, %1, %1, %2;" : "=l"(acc) : "l"(c2), "l"(acc));
+        const float c0 = __fsub_rn(x0, y0), c1 = __fsub_rn(x1, y1);
+        a0 = __fmaf_rn(c0, c0, a0);
+        a1 = __fmaf_rn(c1, c1, a1);
     } else {
-        asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(acc) : "l"(x2), "l"(y2), "l"(acc));
+        a0 = __fmaf_rn(x0, y0, a0);
+        a1 = __fmaf_rn(x1, y1, a1);
     }
-    return acc;
+    return pack2(a0, a1);
 }
 
 // distances of 8 staged rows (shared memory) against the query (shared memory, f32); returns on

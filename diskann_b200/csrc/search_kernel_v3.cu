@@ -4,8 +4,8 @@
 // (DiskANNIndex::search_internal, index.rs:1933-2000; NeighborPriorityQueue, queue.rs:130-318;
 // expand_beam, provider.rs:436-479, 620-690).  What changes against v2 is the number of
 // dependent GLOBAL-memory round trips a hop costs — v2 has three (bucket probe, CAS, row
-// copy), and its per-warp tables (62 MB for 3334 resident warps) do not stay in L2, so ≈3 GB of
-// the 8.8 GB a launch moves is random 32-byte table sectors (profiles/r01_table_footprint.md):
+// copy), and its per-warp tables (tens of MB for a few thousand resident warps) do not stay in
+// L2, so a large share of the bytes a launch moves is random 32-byte table sectors:
 //
 //   * the visited set of a query is an exact open-addressed table of 16-bit quotient tags in
 //     the warp's own shared memory (id -> (bucket, tag) is a bijection for ids < 2^K, so only
@@ -16,8 +16,8 @@
 //   * the only HBM round trip left on a hop's critical path is the row gather itself: rows are
 //     read straight into registers with 16-byte loads, 8 (f32) / 4 (f16) lanes per row and up
 //     to 16 rows in flight per warp, each lane running the FMA chains of the SIMD slots it
-//     loaded (the lane mapping of frontier_wide_kernel, which reaches 0.84-0.96 of the measured
-//     HBM peak) — no staging buffer, which is what makes room for the table;
+//     loaded (the lane mapping of frontier_wide_kernel) — no staging buffer, which is what makes
+//     room for the table;
 //   * i8 / u8 rows use the same structure with exact i32 dot products (dp4a);
 //   * the adjacency row of the predicted next node is copied into shared memory while the
 //     current hop runs (as in v2), so a hop normally starts without a global round trip.
@@ -39,7 +39,7 @@ namespace {
 #define DAB_V3_LP16 0  // visited set: 1 = linear-probing 16-bit slots (measured slower: dependent probe steps), 0 = buckets of 16 tags
 #endif
 #ifndef DAB_V3_FAST_ONE
-#define DAB_V3_FAST_ONE 1  // fast f32 path: one 4-row pass per step (measured best: 2.71 vs 2.90 ms on C2); 0: two passes + butterfly
+#define DAB_V3_FAST_ONE 1  // fast f32 path: one 4-row pass per step; 0: two passes + butterfly
 #endif
 
 // ---- f32 rows of 32 * nm <= 128 elements (the headline shapes: 128-d, 96-d) ------------------
@@ -413,9 +413,8 @@ __global__ void __launch_bounds__(kV3Warps * 32, DAB_V3_MIN_CTAS) search_kernel_
 // ------------------------------------------------------------------ host side
 int v3_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, uint32_t visited_need, SearchParamsV3& p, V3Launch& out) {
     if (idx->tune.disable_v3) return 1;
-    // v3 wins for short candidate lists (C2: 1.11 vs 1.67 ms at L = 15) and loses at the headline L = 100
-    // (2.94 vs 2.68 ms); the measured crossover is L ~ 25 on both the 128-d f32 and the 768-d f16 shape
-    // (profiles/r02_sweep_l.txt): longer lists go to the global-table kernel
+    // v3 is for short candidate lists (L + start points <= 24): its per-hop round trips are fewer, while at the
+    // headline L = 100 the list work dominates and v2 is faster; longer lists go to the global-table kernel
     if (l_search + idx->n_start > (uint32_t)(idx->tune.v3_max_cap ? idx->tune.v3_max_cap : 24)) return 1;
     const bool is_int = idx->dtype == DAB_I8 || idx->dtype == DAB_U8;
     const MetricPlan plan = plan_for(idx->metric, is_int);

@@ -105,7 +105,8 @@ __device__ __forceinline__ bool lp16_insert(uint32_t* table, const Lp16Map& m, u
     }
 }
 
-// Packed f32x2 arithmetic (FADD2 / FFMA2): each half is an IEEE round-to-nearest operation.
+// A pair of f32 accumulators carried as one 64-bit register pair; each half is advanced by its own IEEE
+// round-to-nearest scalar operation (sm_90 has no packed f32x2 arithmetic).
 __device__ __forceinline__ uint64_t pack2(float lo, float hi) {
     uint64_t r;
     asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
@@ -114,14 +115,19 @@ __device__ __forceinline__ uint64_t pack2(float lo, float hi) {
 __device__ __forceinline__ void unpack2(uint64_t v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
 template <int KIND>
 __device__ __forceinline__ uint64_t step2(uint64_t acc, uint64_t x2, uint64_t y2) {
+    float a0, a1, x0, x1, y0, y1;
+    unpack2(acc, a0, a1);
+    unpack2(x2, x0, x1);
+    unpack2(y2, y0, y1);
     if (KIND == KIND_L2) {
-        uint64_t c2;
-        asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(c2) : "l"(x2), "l"(y2));
-        asm("fma.rn.f32x2 %0, %1, %1, %2;" : "=l"(acc) : "l"(c2), "l"(acc));
+        const float c0 = __fsub_rn(x0, y0), c1 = __fsub_rn(x1, y1);
+        a0 = __fmaf_rn(c0, c0, a0);
+        a1 = __fmaf_rn(c1, c1, a1);
     } else {
-        asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(acc) : "l"(x2), "l"(y2), "l"(acc));
+        a0 = __fmaf_rn(x0, y0, a0);
+        a1 = __fmaf_rn(x1, y1, a1);
     }
-    return acc;
+    return pack2(a0, a1);
 }
 
 __device__ __forceinline__ uint4 ldg16(const uint8_t* p) { return __ldg(reinterpret_cast<const uint4*>(p)); }

@@ -426,7 +426,7 @@ class GpuIndex:
         return ids, dists
 
     def flat_knn_tc(self, queries, k):
-        """The exhaustive scan as a tcgen05 GEMM with fused candidate selection + exact re-scoring."""
+        """The exhaustive scan as a wgmma GEMM with fused candidate selection + exact re-scoring."""
         queries = self._queries(queries)
         ids = np.empty((queries.shape[0], k), np.uint32)
         dists = np.empty((queries.shape[0], k), np.float32)

@@ -1,4 +1,4 @@
-// Locates libdiskann_b200.so (built by `make -C diskann_b200/csrc`, nvcc sm_100a) — the library is not
+// Locates libdiskann_b200.so (built by `make -C diskann_b200/csrc`, nvcc sm_90a) — the library is not
 // compiled by cargo: it needs nvcc, and the workspace must stay buildable on machines without CUDA.
 use std::env;
 use std::path::PathBuf;

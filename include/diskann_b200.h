@@ -1,8 +1,8 @@
 /*
- * diskann_b200.h — C ABI of the B200-native distance hot path for microsoft/DiskANN (DiskANN3).
+ * diskann_b200.h — C ABI of the H100-native distance hot path for microsoft/DiskANN (DiskANN3).
  *
  * This is the drop-in boundary (SURVEY.md §8b): a plain-C shared library
- * (libdiskann_b200.so, sm_100a CUDA inside) whose entry points are what a Rust `-sys` crate
+ * (libdiskann_b200.so, sm_90a CUDA inside) whose entry points are what a Rust `-sys` crate
  * for this path binds.  Conventions mirror the reference's only FFI precedent,
  * diskann-garnet/src/lib.rs:262-630: opaque handle, (pointer, length) pairs, integer status,
  * no unwinding across the boundary, caller owns every host buffer, the library owns device
@@ -350,9 +350,9 @@ int dab_build(dab_index* idx, uint32_t pruned_degree, uint32_t l_build, float al
 int dab_flat_knn(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t* out_ids,
                  float* out_dists);
 
-/* The same scan on the tensor cores (BASELINE.json north_star: "the query x neighbour distance batch is a
- * tcgen05 tensor-core GEMM ... with TMA-staged vector tiles and fused ||x||^2 + ||y||^2 expansion"):
- * bf16 operands (f32 / f16 rows as a 3-product hi/lo split, i8 / u8 exact), fp32 accumulation in TMEM,
+/* The same scan on the tensor cores (a wgmma GEMM with TMA-staged vector tiles and fused
+ * ||x||^2 + ||y||^2 expansion): bf16 operands (f32 / f16 rows as a 3-product hi/lo split, i8 / u8 exact),
+ * fp32 accumulation in registers,
  * fused score expansion and per-row candidate selection in the epilogue; the candidates are then
  * re-scored with the exact reference-order kernel, so out_dists are bit-identical to dab_flat_knn and
  * out_ids equal it unless approximate scores (~1e-5 relative) displace a true neighbour by more than

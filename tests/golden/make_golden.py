@@ -1,8 +1,8 @@
 #!/usr/bin/env python3
 """Extracts the portable golden vectors of the reference's own tests into tests/golden/.
 
-Run in the development container (needs /root/reference, which does not exist on the GPU
-box):  python tests/golden/make_golden.py
+Run against a checkout of the reference (the tests only read the JSON files this writes):
+    python tests/golden/make_golden.py <path to the reference checkout>
 
 Sources (paths relative to the reference checkout):
   * diskann-vector/src/distance/distance_provider.rs:744-828  — 2x256 f32 literal vectors whose
@@ -23,7 +23,7 @@ import os
 import re
 import sys
 
-REF = "/root/reference"
+REF = sys.argv[1] if len(sys.argv) > 1 else "."
 OUT = os.path.dirname(os.path.abspath(__file__))
 
 

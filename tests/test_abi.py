@@ -29,10 +29,10 @@ def test_header_binding_and_library_agree():
     assert exported == declared
 
 
-def test_library_is_sm100a_and_self_contained():
+def test_library_is_sm90a_and_self_contained():
     import diskann_b200
     out = subprocess.run(["cuobjdump", "-lelf", diskann_b200.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out and "sm_90" not in out and "sm_80" not in out
+    assert "sm_90a" in out and "sm_100" not in out and "sm_80" not in out
     ldd = subprocess.run(["ldd", diskann_b200.LIB_PATH], capture_output=True, text=True).stdout
     assert "torch" not in ldd and "oracle" not in ldd  # plain C ABI, no torch types, never links the oracle
 

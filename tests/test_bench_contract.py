@@ -21,7 +21,7 @@ def test_algorithmic_bytes_follows_the_survey_formula():
     assert bench.unit_bytes(c4) == 40  # 32 code bytes + id + output
     # PQ traversal + rerank: L full-precision rows (136 B each) per query on top
     assert bench.algorithmic_bytes(c4, 1000, 100, 1, 83, rerank_rows=100) == 1000 * 40 + 100 * 336 + (128 + 80) + 100 * 136
-    assert bench.unit_bytes(bench.WORKLOADS["c5_100Mx96_f32_l2"]) == 392
+    assert bench.unit_bytes(bench.WORKLOADS["c5_40Mx96_f32_l2"]) == 392
 
 
 def test_host_cores_respects_affinity():
@@ -65,14 +65,25 @@ def test_reference_arm_prints_one_json_line_without_a_gpu():
 
 
 def test_traffic_json_is_keyed_by_workload(tmp_path, monkeypatch):
-    """roofline.traffic comes from the committed ncu capture of the workload's own search kernel."""
-    assert bench.ncu_traffic("c2_1Mx128_f32_l2") > 1e9 and bench.ncu_traffic("c4_10Mx128_i8_pq32") > 1e9
-    assert bench.ncu_traffic("c3_1Mx768_f16_ip") is None  # no capture committed under that key
-    t = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-    for entry in t.values():
-        assert os.path.exists(os.path.join(ROOT, entry["source"].split(", ")[1])), entry["source"]
-    # round-1 layout (one entry, no key) still reads as the C2 kernel
+    """roofline.traffic comes from an ncu capture of the workload's own search kernel stored as profiles/traffic.json."""
     (tmp_path / "profiles").mkdir()
-    (tmp_path / "profiles" / "traffic.json").write_text(json.dumps({"search_kernel_dram_bytes_per_launch": 7.0}))
     monkeypatch.setattr(bench, "ROOT", str(tmp_path))
+    assert bench.ncu_traffic("c2_1Mx128_f32_l2") is None  # no capture stored
+    t = {"c2_1Mx128_f32_l2": {"search_kernel_dram_bytes_per_launch": 5.0e9},
+         "c4_10Mx128_i8_pq32": {"search_kernel_dram_bytes_per_launch": 2.0e9}}
+    (tmp_path / "profiles" / "traffic.json").write_text(json.dumps(t))
+    assert bench.ncu_traffic("c2_1Mx128_f32_l2") == 5.0e9 and bench.ncu_traffic("c4_10Mx128_i8_pq32") == 2.0e9
+    assert bench.ncu_traffic("c3_1Mx768_f16_ip") is None  # no capture under that key
+    # round-1 layout (one entry, no key) still reads as the C2 kernel
+    (tmp_path / "profiles" / "traffic.json").write_text(json.dumps({"search_kernel_dram_bytes_per_launch": 7.0}))
     assert bench.ncu_traffic("c2_1Mx128_f32_l2") == 7.0 and bench.ncu_traffic("c4_10Mx128_i8_pq32") is None
+
+
+def test_dump_outputs_writes_float_arrays(tmp_path):
+    """--dump-outputs: one .npy per returned array, float32 kept, integer results widened exactly to float64."""
+    ids = np.array([[3, 1], [-1, 7]], np.int32)
+    dists = np.array([[0.5, 1.25], [np.inf, 2.0]], np.float32)
+    bench.dump_outputs(str(tmp_path / "out"), {"ids": ids, "dists": dists})
+    got_ids, got_d = np.load(tmp_path / "out" / "ids.npy"), np.load(tmp_path / "out" / "dists.npy")
+    assert got_ids.dtype == np.float64 and np.array_equal(got_ids, ids)
+    assert got_d.dtype == np.float32 and np.array_equal(got_d, dists)

@@ -864,7 +864,7 @@ def test_search_c3_shape_f16_768_inner_product(dab):
                                                (np.int8, O.L2, 30000, 128, 200), (np.float16, O.INNER_PRODUCT, 9000, 100, 64),
                                                (np.uint8, O.COSINE, 7000, 40, 50), (np.float32, O.COSINE_NORMALIZED, 3001, 33, 17)])
 def test_tensor_core_flat_scan_equals_the_exact_scan(dab, dt, metric, n, d, nq):
-    """dab_flat_knn_tc (tcgen05 GEMM over bf16 hi/lo splits, fused candidate selection, exact
+    """dab_flat_knn_tc (wgmma GEMM over bf16 hi/lo splits, fused candidate selection, exact
     re-scoring) returns the exact scan's ids and bit-identical distances."""
     rng = np.random.default_rng(n + d)
     if dt in (np.float32, np.float16):

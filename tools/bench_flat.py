@@ -1,4 +1,4 @@
-"""tuning aid: exhaustive scan, exact CUDA-core kernel vs the tcgen05 path (CUDA-event timing of the whole call
+"""tuning aid: exhaustive scan, exact CUDA-core kernel vs the tensor-core (wgmma) path (CUDA-event timing of the whole call
 minus host copies is not separated here: both go through the host API with the same copies)."""
 import os
 import sys
@@ -21,7 +21,7 @@ with dab.GpuIndex(dab.DType.f32, dab.Metric.L2, d, n, 1, 8) as g:
     for nq in (1000, 10000):
         q = centers[rng.integers(0, 1024, nq)] + np.float32(0.3) * rng.standard_normal((nq, d), dtype=np.float32)
         g.flat_knn_tc(q[:128], 10)  # builds the bf16 operand copy of the base
-        for name, fn in (("exact", g.flat_knn), ("tcgen05", g.flat_knn_tc)):
+        for name, fn in (("exact", g.flat_knn), ("wgmma", g.flat_knn_tc)):
             fn(q, 10)
             t0 = time.perf_counter()
             ids, dist = fn(q, 10)

@@ -8,7 +8,7 @@ name=$1; srcs=$(echo $2 | tr ',' ' '); shift 2
 make -C diskann_b200/csrc -j16 > /dev/null
 mkdir -p build /tmp/dab_var/$name
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
-FLAGS="-O3 -std=c++17 -lineinfo -fmad=false -gencode arch=compute_100a,code=sm_100a -Xcompiler -fPIC,-Wall -cudart static"
+FLAGS="-O3 -std=c++17 -lineinfo -fmad=false -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-Wall -cudart static"
 cd diskann_b200/csrc
 objs=""
 for o in *.o; do
@@ -19,5 +19,5 @@ for s in $srcs; do
   $NVCC $FLAGS "$@" -c -o /tmp/dab_var/$name/${s%.cu}.o $s &
 done
 wait
-$NVCC -gencode arch=compute_100a,code=sm_100a -shared -cudart static -o ../../build/lib_${name}.so $objs /tmp/dab_var/$name/*.o -ldl
+$NVCC -gencode arch=compute_90a,code=sm_90a -shared -cudart static -o ../../build/lib_${name}.so $objs /tmp/dab_var/$name/*.o -ldl
 echo "build/lib_${name}.so  ($srcs $*)"

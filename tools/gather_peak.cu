@@ -1,9 +1,9 @@
-// tools/gather_peak.cu — what the B200 memory system delivers for RANDOM row gathers (the access
+// tools/gather_peak.cu — what the H100 memory system delivers for RANDOM row gathers (the access
 // pattern of every kernel on this path): each warp reads whole rows of `row_bytes` at random
 // positions of a table much larger than the L2 with 16-byte loads, U rows in flight, and writes
 // 4 bytes per row.  This is the practical ceiling for the frontier/search kernels, to be read
 // next to the streaming-copy peak in MEASURED_PEAKS.json.
-// build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o build/gather_peak tools/gather_peak.cu
+// build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o build/gather_peak tools/gather_peak.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>

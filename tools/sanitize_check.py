@@ -62,7 +62,7 @@ for dt, ddt, metric, d in ((np.float32, dab.DType.f32, dab.Metric.L2, 100), (np.
         got = g.search_batch(base[:64], 5, 64, 1)                # search_kernel_v2 / generic
         got4 = g.search_batch(base[:64], 5, 40, 4)
         knn = g.flat_knn(base[:16], 5)
-        knn_tc = g.flat_knn_tc(base[:16], 5)                     # tcgen05 + TMA + TMEM path
+        knn_tc = g.flat_knn_tc(base[:16], 5)                     # wgmma + TMA path
         assert np.array_equal(knn[0], knn_tc[0])
         if dt != np.float16:
             g.pq_train(base[:1500].astype(np.float32), 4, 32, 2, 7)  # k-means++ / Lloyd kernels
