@@ -5,14 +5,16 @@
 // NeighborPriorityQueue, queue.rs:130-318; expand_beam, provider.rs:436-479) and bit-identical
 // results; what changes is how many dependent memory round trips a hop costs:
 //
-//   * rows of the surviving candidates of a hop are staged in shared memory with cp.async
-//     (16 B per lane, eight lanes per row: one warp instruction moves 128 B of four rows and no
-//     lane needs another lane's address; no registers tied up), a stage of
-//     rows in flight at once (a TMA bulk-copy variant was measured slower: UBLKCP takes
-//     warp-uniform operands, so per-row copies serialise);
-//   * distances are computed from shared memory (lane s <-> SIMD slot s, conflict-free) for 8
-//     rows per pass and reduced with a transpose-butterfly in the reference's association
-//     (xor 8, 16, [remainder], 4, 2, 1) — 9 shuffles per 8 rows;
+//   * f32 rows of 32..128 elements with level 1 of the visited set on (REG): every surviving row of a hop
+//     gets one bulk L2 prefetch, then the rows are read straight into registers, 8 lanes per row and
+//     4 rows per pass (wide_distances_f32_fast, the lane mapping of search_kernel_v3);
+//   * all other rows are staged in shared memory with cp.async (16 B per lane, eight lanes per row:
+//     one warp instruction moves 128 B of four rows and no lane needs another lane's address; no
+//     registers tied up), a stage of rows in flight at once (a TMA bulk-copy variant was measured
+//     slower: UBLKCP takes warp-uniform operands, so per-row copies serialise); their distances
+//     are computed from shared memory (lane s <-> SIMD slot s, conflict-free) for 8 rows per pass
+//     and reduced with a transpose-butterfly in the reference's association (xor 8, 16,
+//     [remainder], 4, 2, 1) — 9 shuffles per 8 rows;
 //   * the sorted candidate list lives in shared memory and a whole round of candidates is merged
 //     at once by rank (search_common.cuh), equivalent to the reference's sequential inserts;
 //   * all visited-set probes of an adjacency row are issued together (two 128-bit evict_last
@@ -23,6 +25,7 @@
 #include "dab_common.cuh"
 #include "distance_device.cuh"
 #include "search_common.cuh"
+#include "search_smem.cuh"
 #include "search_v2.cuh"
 
 #include <algorithm>
@@ -32,8 +35,10 @@
 namespace dab {
 
 constexpr int kGroup = 8;  // rows reduced together
-constexpr int kV2MinCtas = 21;
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+constexpr int kV2MinCtas = 21;  // staged rows: shared memory binds residency first
+// rows in registers (REG): registers bind residency.  A warp scheduler holds 16K registers, so 28 one-warp CTAs per
+// SM (7 per scheduler) leave 72 per thread.
+constexpr int kV2MinCtasReg = 28;
 
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
@@ -175,8 +180,12 @@ __device__ __forceinline__ bool global_table_insert(uint32_t* table, uint32_t nb
 // first and only an id that is neither found nor placed there goes on to the global table — for most queries never,
 // so their visited set costs no global traffic at all; the global table is cleared when its first id arrives.
 // L1 = false: the global table alone (ids too wide for 14-bit tags at the table size, or level 1 disabled).
-template <typename TD, int KIND, int POST, int QT, bool L1>
-__global__ void __launch_bounds__(kV2Warps * 32, kV2MinCtas) search_kernel_v2(const SearchParamsV2 p) {
+// REG = true (f32 rows of 32, 64, 96 or 128 elements, L1 on): a hop's candidate rows are read straight into registers
+// after one bulk L2 prefetch per row (wide_distances_f32_fast, search_smem.cuh), so all of them are on their way from
+// HBM at once and no shared memory is spent on staging them.  REG = false: rows staged in shared memory.
+template <typename TD, int KIND, int POST, int QT, bool L1, bool REG>
+__global__ void __launch_bounds__(kV2Warps * 32, REG ? kV2MinCtasReg : kV2MinCtas) search_kernel_v2(const SearchParamsV2 p) {
+    static_assert(!REG || (std::is_same<TD, float>::value && L1), "the register row path reads f32 rows, with level 1 on");
     extern __shared__ __align__(128) uint8_t smem[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     uint8_t* base = smem + (size_t)wib * p.warp_smem;
@@ -186,10 +195,8 @@ __global__ void __launch_bounds__(kV2Warps * 32, kV2MinCtas) search_kernel_v2(co
     uint32_t* cid = reinterpret_cast<uint32_t*>(base + p.off_cid);
     float* cd = reinterpret_cast<float*>(base + p.off_cd);
     uint32_t* beam_ids = reinterpret_cast<uint32_t*>(base + p.off_beam);
-    uint8_t* rows = base + p.off_rows;
-    const uint32_t rows_a = smem_u32(rows);
     uint32_t* adjbuf = reinterpret_cast<uint32_t*>(base + p.off_adj);
-    const uint32_t adjbuf_a = smem_u32(adjbuf);
+    const uint32_t adjbuf_a = smem_addr(adjbuf);
 
     uint32_t* t1 = reinterpret_cast<uint32_t*>(base + p.off_t1);
     const uint32_t nb1 = p.t1_buckets;
@@ -237,7 +244,7 @@ __global__ void __launch_bounds__(kV2Warps * 32, kV2MinCtas) search_kernel_v2(co
             if (KIND != KIND_IP) qq = warp_int_self<V2Int<TD>::is_signed>(reinterpret_cast<const uint8_t*>(qf), dim, lane);
         }
 
-        uint32_t size = 0, cursor_lo = 0, cmps = 0, hops = 0, nvisited = 0, nrec = 0;
+        uint32_t size = 0, cursor_lo = 0, cmps = 0, nvisited = 0, nrec = 0;  // nrec: expanded nodes, i.e. hops
         uint32_t n1 = 0;          // ids held by level 1 (nvisited counts those of the global table when L1 is on)
         bool closed = false;      // level 1 takes no more ids
         bool l2_used = false;     // the global table has been cleared for this query and may hold ids
@@ -271,7 +278,9 @@ __global__ void __launch_bounds__(kV2Warps * 32, kV2MinCtas) search_kernel_v2(co
 
         // stage `n` candidate rows (ids cid[c0..)) with per-lane 16 B async copies and compute
         // their distances into cd[]
-        auto distances = [&](uint32_t c0, uint32_t n) {
+        auto stage = [&](uint32_t c0, uint32_t n) {
+            uint8_t* rows = base + p.off_rows;
+            const uint32_t rows_a = smem_addr(rows);
             // eight lanes per row, 16 B each: one warp instruction moves 128 B of four different
             // rows, and every lane forms its own source address (no cross-lane traffic)
             const uint32_t sub = (uint32_t)lane >> 3, nsub = 4, off0 = ((uint32_t)lane & 7u) * 16u, offs = 128;
@@ -317,6 +326,28 @@ __global__ void __launch_bounds__(kV2Warps * 32, kV2MinCtas) search_kernel_v2(co
             __syncwarp();
         };
 
+        // distances of the candidates cid[0..n) into cd[0..n)
+        auto distances = [&](uint32_t n) {
+            if constexpr (REG) {
+                // the 16 query elements this lane multiplies, as packed pairs (re-read from shared memory per call so
+                // that they do not hold registers across the hop)
+                const int nm = dim >> 5;
+                uint64_t q2[8] = {0ull, 0ull, 0ull, 0ull, 0ull, 0ull, 0ull, 0ull};
+#pragma unroll
+                for (int m = 0; m < 4; ++m) {
+                    if (m < nm) {
+                        const float4 x = *reinterpret_cast<const float4*>(qf + 32 * m + 4 * (lane & 7));
+                        q2[2 * m] = pack2(x.x, x.y);
+                        q2[2 * m + 1] = pack2(x.z, x.w);
+                    }
+                }
+                wide_distances_f32_fast<KIND, POST>(q2, nm, p.vectors, p.row_stride, cid, n, cd, lane);
+                __syncwarp();
+            } else {
+                for (uint32_t c0 = 0; c0 < n; c0 += p.stage_rows) stage(c0, min(p.stage_rows, n - c0));
+            }
+        };
+
         // ---- start points (SearchAccessor::start_point_distances, provider.rs:406-433)
         for (uint32_t s0 = 0; s0 < p.n_start; s0 += 32) {
             const uint32_t n = min(32u, p.n_start - s0);
@@ -333,7 +364,7 @@ __global__ void __launch_bounds__(kV2Warps * 32, kV2MinCtas) search_kernel_v2(co
                 bucket_insert(table, nbk, b, bs, id);
             }
             __syncwarp();
-            for (uint32_t c0 = 0; c0 < n; c0 += p.stage_rows) distances(c0, min(p.stage_rows, n - c0));
+            distances(n);
             merge_round<QT>(qd, qi, p.cap, size, cursor_lo, cid, cd, 0, n, lane);
             if constexpr (!L1) nvisited += n;
             cmps += n;
@@ -469,13 +500,12 @@ __global__ void __launch_bounds__(kV2Warps * 32, kV2MinCtas) search_kernel_v2(co
             if (overflow) break;
             __syncwarp();
 
-            for (uint32_t c0 = 0; c0 < ncand; c0 += p.stage_rows) distances(c0, min(p.stage_rows, ncand - c0));
+            distances(ncand);
 
             // best.insert for every neighbour in adjacency order (index.rs:1986-1988)
             for (uint32_t c0 = 0; c0 < ncand; c0 += 32)
                 merge_round<QT>(qd, qi, p.cap, size, cursor_lo, cid, cd, c0, min(32u, ncand - c0), lane);
             cmps += ncand;
-            hops += nb;
         }
 
         if (overflow) {
@@ -511,7 +541,7 @@ __global__ void __launch_bounds__(kV2Warps * 32, kV2MinCtas) search_kernel_v2(co
                 atomicMax(p.counters + 2, n1 + nvisited);
                 if (p.out_counts) p.out_counts[qidx] = count;
                 if (p.out_cmps) p.out_cmps[qidx] = cmps;
-                if (p.out_hops) p.out_hops[qidx] = hops;
+                if (p.out_hops) p.out_hops[qidx] = nrec;
                 if (p.rec_counts) {
                     p.rec_counts[qidx] = min(nrec, p.rec_cap);
                     if (nrec > p.rec_cap) atomicAdd(p.counters + 3, 1u);  // expanded nodes beyond the record: reported by dab_build
@@ -519,9 +549,20 @@ __global__ void __launch_bounds__(kV2Warps * 32, kV2MinCtas) search_kernel_v2(co
             }
         }
     }
+    // without row staging nothing else drains the last speculative adjacency copy
+    if constexpr (REG) asm volatile("cp.async.wait_group 0;" ::: "memory");
 }
 
 // ------------------------------------------------------------------ host side
+// the instantiation for a level-1 choice and row path (only f32 rows with level 1 on have the register path)
+template <typename TD, int K, int P, int Q>
+static void (*pick_v2(bool l1, bool reg))(const SearchParamsV2) {
+    if constexpr (std::is_same<TD, float>::value) {
+        if (reg) return search_kernel_v2<TD, K, P, Q, true, true>;
+    }
+    return l1 ? search_kernel_v2<TD, K, P, Q, true, false> : search_kernel_v2<TD, K, P, Q, false, false>;
+}
+
 // Returns 1 when this configuration is not covered by v2 (caller falls back to v1), 0 on
 // success with `out` filled, or a negative DAB error code.
 int v2_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, bool level1, SearchParamsV2& p, V2Launch& out) {
@@ -532,7 +573,6 @@ int v2_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, bool leve
     if (cap > 256 || idx->max_degree > 1000) return 1;
     const uint32_t row_bytes = (uint32_t)round_up((size_t)idx->dim * elem_size(idx->dtype), 16);
     if (row_bytes > idx->row_stride) return 1;
-    const uint32_t row_slot = row_bytes;
     size_t off = 0;
     p.off_q = (uint32_t)off;
     off += v2_int ? round_up(round_up((size_t)idx->dim, 4), 16) : round_up((size_t)idx->dim * 4, 16);
@@ -552,16 +592,7 @@ int v2_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, bool leve
     off += cap_pad * 4;
     p.off_qi = (uint32_t)off;
     off += cap_pad * 4;
-    off = round_up(off, 128);
-    p.off_rows = (uint32_t)off;
-    const size_t fixed = off;
-    // rows staged per round: as many as fit ~6 KB per warp, a multiple of the reduce group
-    const size_t stage_bytes = 6144;
-    uint32_t stage = (uint32_t)std::max<size_t>(kGroup, (stage_bytes / row_slot) / kGroup * kGroup);
-    stage = std::min<uint32_t>(stage, 32);
-    p.stage_rows = stage;
     p.row_bytes = row_bytes;
-    p.row_slot = row_slot;
     // level-1 visited table: 4 KB of 16-bit tags per warp (2048 slots; the mean visited set of the headline
     // workload is ~1200 ids) when the ids fit 14-bit quotient tags, i.e. n_total <= 16384 * buckets
     size_t t1_bytes = idx->tune.test_visited_log2 ? 512 : 4096;  // tests: a level 1 that fills at once
@@ -578,24 +609,38 @@ int v2_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, bool leve
         p.tag_shift = K + sbits;
         p.tag_magic = (uint32_t)((((uint64_t)1 << (K + sbits)) + nb1 - 1) / nb1);
     }
-    p.off_t1 = (uint32_t)round_up(fixed + (size_t)stage * row_slot, 32);
     // level 1 pays for itself only while enough warps stay resident: at C2 (24 -> 20 one-warp CTAs per SM) it removes
     // the table traffic (8.8 -> 5.3 GB of DRAM traffic per 10K queries) and is 2 % faster, at C3 (12 -> 10) it is 11 % slower
     // ... and while batches overlap: one batch at a time is dominated by its tail, where the 4 resident warps fewer
     // cost more (2.96 vs 2.67 ms) than the traffic saves
     if (p.t1_buckets && !level1) p.t1_buckets = 0;
-    if (p.t1_buckets && (227 * 1024) / (round_up((size_t)p.off_t1 + t1_bytes, 128) * kV2Warps + 1024) * kV2Warps < 16)
-        p.t1_buckets = 0;
+    auto resident_warps = [&](size_t t1_at) {
+        return (227 * 1024) / (round_up(round_up(t1_at, 32) + t1_bytes, 128) * kV2Warps + 1024) * kV2Warps;
+    };
+    // f32 rows of 32, 64, 96 or 128 elements (C2, the C5 shape) with level 1 on are read into registers: without the
+    // staging buffer registers bind residency (28 warps per SM at C2 instead of 20).  Everything else stages its rows:
+    // with the global table alone the register path does not raise residency (registers bind both at 80), and one
+    // batch at a time at C2 measured 3.6 % slower on it.
+    const bool reg = idx->dtype == DAB_F32 && idx->dim % 32 == 0 && idx->dim <= 128 && p.t1_buckets && resident_warps(off) >= 16;
+    if (!reg) {
+        off = round_up(off, 128);
+        p.off_rows = (uint32_t)off;
+        // rows staged per round: as many as fit ~6 KB per warp, a multiple of the reduce group
+        const size_t stage_bytes = 6144;
+        uint32_t stage = (uint32_t)std::max<size_t>(kGroup, (stage_bytes / row_bytes) / kGroup * kGroup);
+        stage = std::min<uint32_t>(stage, 32);
+        p.stage_rows = stage;
+        p.row_slot = row_bytes;
+        off += (size_t)stage * row_bytes;
+    }
+    p.off_t1 = (uint32_t)round_up(off, 32);
+    if (p.t1_buckets && resident_warps(off) < 16) p.t1_buckets = 0;
     if (!p.t1_buckets) t1_bytes = 0;
     p.warp_smem = (uint32_t)round_up((size_t)p.off_t1 + t1_bytes, 128);
     out.smem_block = (size_t)p.warp_smem * kV2Warps;
     if (out.smem_block > 200 * 1024) return 1;
 
-#define PICK2(TD, K, P, Q)                                              \
-    do {                                                                \
-        if (p.t1_buckets) out.kern = search_kernel_v2<TD, K, P, Q, true>; \
-        else out.kern = search_kernel_v2<TD, K, P, Q, false>;           \
-    } while (0)
+#define PICK2(TD, K, P, Q) out.kern = pick_v2<TD, K, P, Q>(p.t1_buckets != 0, reg)
 #define PICK_Q(TD, K, P)                 \
     do {                                 \
         if (cap <= 128) PICK2(TD, K, P, 4); \

@@ -35,47 +35,6 @@ namespace dab {
 
 namespace {
 
-// ---- f32 rows of 32 * nm <= 128 elements (the headline shapes: 128-d, 96-d) ------------------
-// Same lane mapping and association as wide_distances, with the per-hop overheads removed: the
-// 16 query elements a lane ever multiplies live in registers (packed pairs), and a step covers
-// one pass of 4 rows whose nm 16-byte loads per lane are issued back to back (one pass rather
-// than two per step: 16 fewer registers).
-template <int KIND, int POST>
-__device__ __forceinline__ void wide_distances_f32_fast(const uint64_t (&q2)[8], int nm, const uint8_t* __restrict__ vectors,
-                                                        size_t row_stride, const uint32_t* __restrict__ cid, uint32_t n,
-                                                        float* __restrict__ cd, int lane) {
-    const int team = lane >> 3, tl = lane & 7;
-    if (n > 4) prefetch_rows(vectors, row_stride, cid, n, (uint32_t)nm * 128u, lane);
-    for (uint32_t j0 = 0; j0 < n; j0 += 4) {
-        const uint8_t* row0 = vectors + (size_t)cid[min(j0 + team, n - 1)] * row_stride + 16 * tl;
-        uint4 v0[4];
-#pragma unroll
-        for (int m = 0; m < 4; ++m)
-            if (m < nm) v0[m] = ldg16(row0 + m * 128);
-        uint64_t a0[2] = {0ull, 0ull};
-#pragma unroll
-        for (int m = 0; m < 4; ++m) {
-            if (m < nm) {
-                a0[0] = step2<KIND>(a0[0], q2[2 * m], pack2(__uint_as_float(v0[m].x), __uint_as_float(v0[m].y)));
-                a0[1] = step2<KIND>(a0[1], q2[2 * m + 1], pack2(__uint_as_float(v0[m].z), __uint_as_float(v0[m].w)));
-            }
-        }
-        float acc[4];
-        unpack2(a0[0], acc[0], acc[1]);
-        unpack2(a0[1], acc[2], acc[3]);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            acc[i] = __fadd_rn(acc[i], __shfl_xor_sync(kFull, acc[i], 2));
-            acc[i] = __fadd_rn(acc[i], __shfl_xor_sync(kFull, acc[i], 4));
-        }
-        float ts[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) ts[i] = __fadd_rn(acc[i], __shfl_xor_sync(kFull, acc[i], 1));
-        const float r = __fadd_rn(__fadd_rn(ts[0], ts[2]), __fadd_rn(ts[1], ts[3]));
-        if (tl == 0 && j0 + team < n) cd[j0 + team] = post_op<POST>(r);
-    }
-}
-
 template <typename T>
 struct IsInt {
     static constexpr bool value = std::is_same<T, int8_t>::value || std::is_same<T, uint8_t>::value;
@@ -338,8 +297,9 @@ __global__ void __launch_bounds__(kV3Warps * 32, kV3MinCtas) search_kernel_v3(co
 
 // ------------------------------------------------------------------ host side
 int v3_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, uint32_t visited_need, SearchParamsV3& p, V3Launch& out) {
-    // v3 is for short candidate lists (L + start points <= 24): its per-hop round trips are fewer, while at the
-    // headline L = 100 the list work dominates and v2 is faster; longer lists go to the global-table kernel
+    // v3 is for short candidate lists (L + start points <= 24), whose visited sets are small.  At the headline L = 100
+    // its whole-set tag table (~11.5 KB per warp) leaves 16 warps per SM, while v2's 4 KB level 1 with the global
+    // table behind it leaves 28 (f32 rows in registers) or 20 (staged rows), so v2 is faster there
     if (l_search + idx->n_start > 24) return 1;
     const bool is_int = idx->dtype == DAB_I8 || idx->dtype == DAB_U8;
     const MetricPlan plan = plan_for(idx->metric, is_int);

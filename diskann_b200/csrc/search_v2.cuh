@@ -43,8 +43,8 @@ struct SearchParamsV2 {
     uint32_t warp_smem, off_q, off_qd, off_qi, off_cid, off_cd, off_beam, off_rows, off_adj;
     uint32_t adj_words;   // words of an adjacency row prefetched into shared memory (0: L2 prefetch only)
     uint32_t row_bytes;   // bytes copied per row (multiple of 16)
-    uint32_t row_slot;    // bytes between staged rows
-    uint32_t stage_rows;  // rows staged per round (multiple of kGroup)
+    uint32_t row_slot;    // bytes between staged rows (REG = false only, as off_rows)
+    uint32_t stage_rows;  // rows staged per round (multiple of kGroup; REG = false only)
 };
 
 struct V2Launch {
