@@ -114,9 +114,6 @@ struct dab_index {
     uint32_t pq_hint_l = 0, pq_hint_beam = 0, pq_hint_visited = 0; int pq_hint_mode = 0;  // the same for the PQ traversal kernel
     uint32_t v3_overflow_l = 0, v3_overflow_beam = 0;      // share of queries that outgrew the shared-memory
     float v3_overflow_frac = 0.0f;                         // tables at (L, beam): search_kernel_v3 is skipped when large
-    void* l2_window_ptr = nullptr;       // current persisting-L2 window (visited tables)
-    size_t l2_window_bytes = 0;
-    cudaStream_t l2_window_stream = nullptr;
 
     uint64_t rec_truncated = 0;  // build: searches whose expanded-node record was cut at its capacity
     dab::Tuning tune;

@@ -93,11 +93,11 @@ __device__ __forceinline__ void merge_round(float* qd, uint32_t* qi, uint32_t ca
     __syncwarp();
 }
 
-// The same merge for lists longer than one register tile (QT * 32 entries): the list is walked in CH tiles from the top
+// The same merge for lists of any length: the list is walked in register tiles of QT * 32 entries from the top occupied
 // one down.  Entries only move right, by sh = #new(d_i <= d_old), which does not decrease along the sorted list, and
 // final positions are unique — so a tile's writes (all at or above its own first entry) never touch an entry a lower
 // tile still has to read, and what a lower tile writes above its own range are final positions no upper entry owns.
-template <int QT, int CH>
+template <int QT>
 __device__ __forceinline__ void merge_round_chunked(float* qd, uint32_t* qi, uint32_t cap, uint32_t& size, uint32_t& cursor_lo,
                                                     const uint32_t* cid, const float* cd, uint32_t c0, uint32_t m, int lane) {
     const uint32_t j = (uint32_t)lane;
@@ -126,9 +126,8 @@ __device__ __forceinline__ void merge_round_chunked(float* qd, uint32_t* qi, uin
     const bool keep_new = valid && pos < cap;
     __syncwarp();
 #pragma unroll 1
-    for (int c = CH - 1; c >= 0; --c) {
-        const uint32_t e0 = (uint32_t)c * QT * 32;
-        if (e0 >= size) continue;  // nothing stored in this tile yet (warp-uniform)
+    for (uint32_t c = (size + QT * 32 - 1) / (QT * 32); c-- > 0;) {
+        const uint32_t e0 = c * QT * 32;
         float od[QT];
         uint32_t oi[QT], sh[QT];
 #pragma unroll
@@ -166,11 +165,13 @@ __device__ __forceinline__ void merge_round_chunked(float* qd, uint32_t* qi, uin
     __syncwarp();
 }
 
-// QT = 4 / 8 / 16: one register tile covers the list (<= 128 / 256 / 512 entries); QT = 32: two tiles of 16 (<= 1024)
+// QT = 4 / 8 / 16: one register tile covers the list (<= 128 / 256 / 512 entries).  Lists of any length: QT = 32 in
+// tiles of 512 entries, QT = 0 in tiles of 256 (search_kernel_v2: 48 tile registers would spill at its residency)
 template <int QT>
 __device__ __forceinline__ void merge_any(float* qd, uint32_t* qi, uint32_t cap, uint32_t& size, uint32_t& cursor_lo, const uint32_t* cid,
                                           const float* cd, uint32_t c0, uint32_t m, int lane) {
-    if constexpr (QT == 32) merge_round_chunked<16, 2>(qd, qi, cap, size, cursor_lo, cid, cd, c0, m, lane);
+    if constexpr (QT == 0) merge_round_chunked<8>(qd, qi, cap, size, cursor_lo, cid, cd, c0, m, lane);
+    else if constexpr (QT == 32) merge_round_chunked<16>(qd, qi, cap, size, cursor_lo, cid, cd, c0, m, lane);
     else merge_round<QT>(qd, qi, cap, size, cursor_lo, cid, cd, c0, m, lane);
 }
 

@@ -1,9 +1,11 @@
-// search_kernel_v2.cu — latency-restructured batched greedy search for float rows
-// (f32 x f32 and f32-widened x f16; L2 / InnerProduct / CosineNormalized schemas, NA = 4).
+// search_kernel_v2.cu — batched greedy (beam) search kept entirely on the device, one warp per query, for
+// every row type (f32, f32-widened x f16, i8, u8), metric and list length.
 //
-// Same semantics as search_kernel.cu (DiskANNIndex::search_internal, index.rs:1933-2000;
-// NeighborPriorityQueue, queue.rs:130-318; expand_beam, provider.rs:436-479) and bit-identical
-// results; what changes is how many dependent memory round trips a hop costs:
+// Restates DiskANNIndex::search_internal (index.rs:1933-2000) with the reference's NeighborPriorityQueue
+// semantics (queue.rs:130-318) and the inmem expand_beam (provider.rs:436-479, 620-690), bit-identical
+// results; the sorted candidate list (capacity L + #start, scratch.rs:195-208) lives in shared memory, the
+// visited set (a HashSet in the reference) is exact, and a query whose global table would pass its load
+// limit is re-run with a larger one.  The kernel is built to keep the dependent memory round trips of a hop few:
 //
 //   * f32 rows of 32..128 elements with level 1 of the visited set on (REG): every surviving row of a hop
 //     gets one bulk L2 prefetch, then the rows are read straight into registers, 8 lanes per row and
@@ -15,8 +17,11 @@
 //     are computed from shared memory (lane s <-> SIMD slot s, conflict-free) for 8 rows per pass
 //     and reduced with a transpose-butterfly in the reference's association (xor 8, 16,
 //     [remainder], 4, 2, 1) — 9 shuffles per 8 rows;
-//   * the sorted candidate list lives in shared memory and a whole round of candidates is merged
-//     at once by rank (search_common.cuh), equivalent to the reference's sequential inserts;
+//   * lists of any length (QT = 0: L + #start > 256), the two-accumulator float cosine schema (NA = 2) and rows
+//     too wide to stage eight of them are read straight from global memory into the FMA chains of
+//     distance_device.cuh, kRowsInFlight rows per team and pass;
+//   * a whole round of candidates is merged into the list at once by rank (search_common.cuh),
+//     equivalent to the reference's sequential inserts;
 //   * all visited-set probes of an adjacency row are issued together (two 128-bit evict_last
 //     loads per 8-id bucket); the adjacency row of the next-best unvisited candidate is copied
 //     into shared memory while the current hop runs, so the next hop usually starts without a
@@ -35,7 +40,9 @@
 namespace dab {
 
 constexpr int kGroup = 8;  // rows reduced together
+constexpr int kRowsInFlight = 4;  // QT = 0: rows per team per pass
 constexpr int kV2MinCtas = 21;  // staged rows: shared memory binds residency first
+constexpr int kV2MinCtasAny = 20;  // QT = 0: 96 registers, what its merge tiles and row gathers need without a spill
 // rows in registers (REG): registers bind residency.  A warp scheduler holds 16K registers, so 28 one-warp CTAs per
 // SM (7 per scheduler) leave 72 per thread.
 constexpr int kV2MinCtasReg = 28;
@@ -183,9 +190,13 @@ __device__ __forceinline__ bool global_table_insert(uint32_t* table, uint32_t nb
 // REG = true (f32 rows of 32, 64, 96 or 128 elements, L1 on): a hop's candidate rows are read straight into registers
 // after one bulk L2 prefetch per row (wide_distances_f32_fast, search_smem.cuh), so all of them are on their way from
 // HBM at once and no shared memory is spent on staging them.  REG = false: rows staged in shared memory.
+// QT = 4 / 8: the list is one register tile of up to 128 / 256 entries in a merge.  QT = 0: lists of any length,
+// with the global table alone and the rows read straight from global memory.
 template <typename TD, int KIND, int POST, int QT, bool L1, bool REG>
-__global__ void __launch_bounds__(kV2Warps * 32, REG ? kV2MinCtasReg : kV2MinCtas) search_kernel_v2(const SearchParamsV2 p) {
+__global__ void __launch_bounds__(kV2Warps * 32, REG ? kV2MinCtasReg : QT == 0 ? kV2MinCtasAny : kV2MinCtas) search_kernel_v2(const SearchParamsV2 p) {
     static_assert(!REG || (std::is_same<TD, float>::value && L1), "the register row path reads f32 rows, with level 1 on");
+    static_assert(QT != 0 || !L1, "lists of any length run the global table alone");
+    static_assert(QT == 0 || KIND != KIND_COS || V2Int<TD>::value, "float cosine reads its rows from global memory");
     extern __shared__ __align__(128) uint8_t smem[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     uint8_t* base = smem + (size_t)wib * p.warp_smem;
@@ -343,6 +354,29 @@ __global__ void __launch_bounds__(kV2Warps * 32, REG ? kV2MinCtasReg : kV2MinCta
                 }
                 wide_distances_f32_fast<KIND, POST>(q2, nm, p.vectors, p.row_stride, cid, n, cd, lane);
                 __syncwarp();
+            } else if constexpr (QT == 0) {
+                // a team per row, kRowsInFlight rows per team and pass: the whole warp (integers, NA = 4 float
+                // schemas) or 16 lanes (float cosine, NA = 2)
+                constexpr bool INT = V2Int<TD>::value;
+                constexpr int S = KIND == KIND_COS && !INT ? 16 : 32, TEAMS = 32 / S, U = kRowsInFlight;
+                using Row = typename std::conditional<INT, uint8_t, TD>::type;
+                const int team = lane / S, slot = lane % S;
+                for (uint32_t c0 = 0; c0 < n; c0 += TEAMS * U) {
+                    float r[U];
+                    uint32_t cc[U];
+                    const Row* rows[U];
+#pragma unroll
+                    for (int u = 0; u < U; ++u) {
+                        cc[u] = c0 + u * TEAMS + team;
+                        rows[u] = reinterpret_cast<const Row*>(p.vectors + (size_t)cid[min(cc[u], n - 1)] * p.row_stride);
+                    }
+                    if constexpr (INT) warp_int_multi<V2Int<TD>::is_signed, KIND, U>(reinterpret_cast<const uint8_t*>(qf), rows, dim, lane, qq, r);
+                    else team_float_multi<S / 8, KIND, U>(qf, rows, dim, slot, r);
+#pragma unroll
+                    for (int u = 0; u < U; ++u)
+                        if (slot == 0 && cc[u] < n) cd[cc[u]] = post_op<POST>(r[u]);
+                }
+                __syncwarp();
             } else {
                 for (uint32_t c0 = 0; c0 < n; c0 += p.stage_rows) stage(c0, min(p.stage_rows, n - c0));
             }
@@ -365,7 +399,7 @@ __global__ void __launch_bounds__(kV2Warps * 32, REG ? kV2MinCtasReg : kV2MinCta
             }
             __syncwarp();
             distances(n);
-            merge_round<QT>(qd, qi, p.cap, size, cursor_lo, cid, cd, 0, n, lane);
+            merge_any<QT>(qd, qi, p.cap, size, cursor_lo, cid, cd, 0, n, lane);
             if constexpr (!L1) nvisited += n;
             cmps += n;
         }
@@ -504,7 +538,7 @@ __global__ void __launch_bounds__(kV2Warps * 32, REG ? kV2MinCtasReg : kV2MinCta
 
             // best.insert for every neighbour in adjacency order (index.rs:1986-1988)
             for (uint32_t c0 = 0; c0 < ncand; c0 += 32)
-                merge_round<QT>(qd, qi, p.cap, size, cursor_lo, cid, cd, c0, min(32u, ncand - c0), lane);
+                merge_any<QT>(qd, qi, p.cap, size, cursor_lo, cid, cd, c0, min(32u, ncand - c0), lane);
             cmps += ncand;
         }
 
@@ -563,16 +597,15 @@ static void (*pick_v2(bool l1, bool reg))(const SearchParamsV2) {
     return l1 ? search_kernel_v2<TD, K, P, Q, true, false> : search_kernel_v2<TD, K, P, Q, false, false>;
 }
 
-// Returns 1 when this configuration is not covered by v2 (caller falls back to v1), 0 on
-// success with `out` filled, or a negative DAB error code.
 int v2_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, bool level1, SearchParamsV2& p, V2Launch& out) {
     const bool v2_int = idx->dtype == DAB_I8 || idx->dtype == DAB_U8;
     const MetricPlan plan = plan_for(idx->metric, v2_int);
-    if (plan.kind == KIND_COS && !v2_int) return 1;
     const uint32_t cap = l_search + idx->n_start;
-    if (cap > 256 || idx->max_degree > 1000) return 1;
     const uint32_t row_bytes = (uint32_t)round_up((size_t)idx->dim * elem_size(idx->dtype), 16);
-    if (row_bytes > idx->row_stride) return 1;
+    auto too_big = [&] {
+        return fail(DAB_ERR_INVALID_ARGUMENT, "search: L=%u, beam=%u, dim=%u need %zu B shared memory per CTA (> 200 KB)", l_search,
+                    beam, idx->dim, out.smem_block);
+    };
     size_t off = 0;
     p.off_q = (uint32_t)off;
     off += v2_int ? round_up(round_up((size_t)idx->dim, 4), 16) : round_up((size_t)idx->dim * 4, 16);
@@ -593,6 +626,12 @@ int v2_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, bool leve
     p.off_qi = (uint32_t)off;
     off += cap_pad * 4;
     p.row_bytes = row_bytes;
+    // rows staged per round: as many as fit ~6 KB per warp, a multiple of the reduce group
+    const size_t stage_bytes = 6144;
+    const uint32_t stage = std::min<uint32_t>(32, (uint32_t)std::max<size_t>(kGroup, (stage_bytes / row_bytes) / kGroup * kGroup));
+    // QT = 0 where one register tile does not hold the list, for the float cosine schema, and for rows so wide that a
+    // stage of them does not fit: rows read straight from global memory, the global table alone
+    const bool any_len = cap > 256 || (plan.kind == KIND_COS && !v2_int) || round_up(off, 128) + (size_t)stage * row_bytes > 200 * 1024;
     // level-1 visited table: 4 KB of 16-bit tags per warp (2048 slots; the mean visited set of the headline
     // workload is ~1200 ids) when the ids fit 14-bit quotient tags, i.e. n_total <= 16384 * buckets
     size_t t1_bytes = idx->tune.test_visited_log2 ? 512 : 4096;  // tests: a level 1 that fills at once
@@ -613,7 +652,7 @@ int v2_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, bool leve
     // the table traffic (8.8 -> 5.3 GB of DRAM traffic per 10K queries) and is 2 % faster, at C3 (12 -> 10) it is 11 % slower
     // ... and while batches overlap: one batch at a time is dominated by its tail, where the 4 resident warps fewer
     // cost more (2.96 vs 2.67 ms) than the traffic saves
-    if (p.t1_buckets && !level1) p.t1_buckets = 0;
+    if (!level1 || any_len) p.t1_buckets = 0;
     auto resident_warps = [&](size_t t1_at) {
         return (227 * 1024) / (round_up(round_up(t1_at, 32) + t1_bytes, 128) * kV2Warps + 1024) * kV2Warps;
     };
@@ -622,13 +661,9 @@ int v2_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, bool leve
     // with the global table alone the register path does not raise residency (registers bind both at 80), and one
     // batch at a time at C2 measured 3.6 % slower on it.
     const bool reg = idx->dtype == DAB_F32 && idx->dim % 32 == 0 && idx->dim <= 128 && p.t1_buckets && resident_warps(off) >= 16;
-    if (!reg) {
+    if (!reg && !any_len) {
         off = round_up(off, 128);
         p.off_rows = (uint32_t)off;
-        // rows staged per round: as many as fit ~6 KB per warp, a multiple of the reduce group
-        const size_t stage_bytes = 6144;
-        uint32_t stage = (uint32_t)std::max<size_t>(kGroup, (stage_bytes / row_bytes) / kGroup * kGroup);
-        stage = std::min<uint32_t>(stage, 32);
         p.stage_rows = stage;
         p.row_slot = row_bytes;
         off += (size_t)stage * row_bytes;
@@ -638,19 +673,21 @@ int v2_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, bool leve
     if (!p.t1_buckets) t1_bytes = 0;
     p.warp_smem = (uint32_t)round_up((size_t)p.off_t1 + t1_bytes, 128);
     out.smem_block = (size_t)p.warp_smem * kV2Warps;
-    if (out.smem_block > 200 * 1024) return 1;
+    if (out.smem_block > 200 * 1024) return too_big();
 
 #define PICK2(TD, K, P, Q) out.kern = pick_v2<TD, K, P, Q>(p.t1_buckets != 0, reg)
-#define PICK_Q(TD, K, P)                 \
-    do {                                 \
-        if (cap <= 128) PICK2(TD, K, P, 4); \
-        else PICK2(TD, K, P, 8);         \
+#define PICK_Q(TD, K, P)                                                      \
+    do {                                                                      \
+        if (any_len) out.kern = search_kernel_v2<TD, K, P, 0, false, false>; \
+        else if (cap <= 128) PICK2(TD, K, P, 4);                              \
+        else PICK2(TD, K, P, 8);                                              \
     } while (0)
-#define PICK_T(TD)                                                       \
-    do {                                                                 \
-        if (plan.kind == KIND_L2) PICK_Q(TD, KIND_L2, POST_ID);           \
-        else if (plan.post == POST_NEG) PICK_Q(TD, KIND_IP, POST_NEG);    \
-        else PICK_Q(TD, KIND_IP, POST_ONE_MINUS);                         \
+#define PICK_T(TD)                                                                                              \
+    do {                                                                                                        \
+        if (plan.kind == KIND_L2) PICK_Q(TD, KIND_L2, POST_ID);                                                  \
+        else if (plan.kind == KIND_COS) out.kern = search_kernel_v2<TD, KIND_COS, POST_ONE_MINUS, 0, false, false>; \
+        else if (plan.post == POST_NEG) PICK_Q(TD, KIND_IP, POST_NEG);                                           \
+        else PICK_Q(TD, KIND_IP, POST_ONE_MINUS);                                                                \
     } while (0)
 #define PICK_I(TD)                                                       \
     do {                                                                 \
@@ -666,14 +703,11 @@ int v2_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, bool leve
 #undef PICK_T
 #undef PICK_Q
 #undef PICK2
-    if (cudaFuncSetAttribute(out.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)out.smem_block) != cudaSuccess) {
-        cudaGetLastError();
-        return 1;
-    }
     int per_sm = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, out.kern, kV2Warps * 32, out.smem_block) != cudaSuccess || per_sm < 1) {
+    if (cudaFuncSetAttribute(out.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)out.smem_block) != cudaSuccess ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, out.kern, kV2Warps * 32, out.smem_block) != cudaSuccess || per_sm < 1) {
         cudaGetLastError();
-        return 1;
+        return too_big();
     }
     out.grid = per_sm * idx->sm_count;
     return 0;

@@ -1,6 +1,6 @@
 // search_kernel_v3.cu — batched greedy search with the visited set in SHARED memory.
 //
-// Same semantics and bit-identical results as search_kernel.cu / search_kernel_v2.cu
+// Same semantics and bit-identical results as search_kernel_v2.cu
 // (DiskANNIndex::search_internal, index.rs:1933-2000; NeighborPriorityQueue, queue.rs:130-318;
 // expand_beam, provider.rs:436-479, 620-690).  What changes against v2 is the number of
 // dependent GLOBAL-memory round trips a hop costs — v2 has three (bucket probe, CAS, row
@@ -11,7 +11,7 @@
 //     the warp's own shared memory (id -> (bucket, tag) is a bijection for ids < 2^K, so only
 //     the tag is stored: 16 entries per 32-byte bucket, displacement <= 2 buckets recorded in
 //     the tag's top two bits).  A probe is two LDS.128, an insert one 32-bit shared-memory CAS;
-//     a query that outgrows its table is handed to the global-table kernel (exactness is kept,
+//     a query that outgrows its table is handed to search_kernel_v2 (exactness is kept,
 //     only speed is lost);
 //   * the only HBM round trip left on a hop's critical path is the row gather itself: rows are
 //     read straight into registers with 16-byte loads, 8 (f32) / 4 (f16) lanes per row and up
@@ -303,9 +303,9 @@ int v3_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, uint32_t 
     if (l_search + idx->n_start > 24) return 1;
     const bool is_int = idx->dtype == DAB_I8 || idx->dtype == DAB_U8;
     const MetricPlan plan = plan_for(idx->metric, is_int);
-    if (plan.kind == KIND_COS && !is_int) return 1;  // float cosine: NA = 2 schema, generic kernel
+    if (plan.kind == KIND_COS && !is_int) return 1;  // float cosine: NA = 2 schema, search_kernel_v2
     const uint32_t cap = l_search + idx->n_start;
-    if (cap > 256 || idx->max_degree > 1000) return 1;
+    if (idx->max_degree > 1000) return 1;
     if ((idx->row_stride & 15) != 0) return 1;
     // quotient tags: ids < 2^K, tag = h / n_buckets must fit 14 bits
     uint32_t K = 8;

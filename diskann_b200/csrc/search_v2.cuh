@@ -43,8 +43,8 @@ struct SearchParamsV2 {
     uint32_t warp_smem, off_q, off_qd, off_qi, off_cid, off_cd, off_beam, off_rows, off_adj;
     uint32_t adj_words;   // words of an adjacency row prefetched into shared memory (0: L2 prefetch only)
     uint32_t row_bytes;   // bytes copied per row (multiple of 16)
-    uint32_t row_slot;    // bytes between staged rows (REG = false only, as off_rows)
-    uint32_t stage_rows;  // rows staged per round (multiple of kGroup; REG = false only)
+    uint32_t row_slot;    // bytes between staged rows (staged rows only, as off_rows)
+    uint32_t stage_rows;  // rows staged per round (multiple of kGroup; staged rows only)
 };
 
 struct V2Launch {
@@ -53,8 +53,8 @@ struct V2Launch {
     int grid;
 };
 
-// Returns 1 when this configuration is not covered by v2 (caller falls back to the generic
-// kernel), 0 on success with `out` filled, or a negative DAB error code.
+// Chooses the instantiation and shared-memory layout for every dtype, metric, L and beam: returns 0 with `p`'s layout
+// and `out` filled, or DAB_ERR_INVALID_ARGUMENT when the layout does not fit one CTA.
 // `level1`: give the visited set its shared-memory level (see search_kernel_v2.cu) when the configuration allows it.
 int v2_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, bool level1, SearchParamsV2& p, V2Launch& out);
 

@@ -45,11 +45,11 @@ struct V3Launch {
     void (*kern)(const SearchParamsV3);
     size_t smem_block;
     int grid;         // resident CTAs on the device
-    uint32_t capacity;  // ids a table holds before the query is handed to the global-table kernel
+    uint32_t capacity;  // ids a table holds before the query is handed to search_kernel_v2
 };
 
-// Returns 1 when this configuration is not covered by v3 (caller uses v2 / the generic kernel),
-// 0 on success with `out` filled.  `visited_need` = ids the table should hold (0: unknown).
+// Returns 1 when this configuration is not covered by v3 (caller uses v2), 0 on success with `out` filled.
+// `visited_need` = ids the table should hold (0: unknown).
 int v3_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, uint32_t visited_need, SearchParamsV3& p, V3Launch& out);
 
 }  // namespace dab

@@ -198,6 +198,7 @@ SEARCH_CASES = [
     (np.float32, O.COSINE, 48, 3000, 16, 30),
     (np.float16, O.INNER_PRODUCT, 96, 3000, 16, 30),
     (np.float16, O.L2, 64, 3000, 16, 30),
+    (np.float16, O.COSINE, 64, 3000, 16, 30),
     (np.int8, O.L2, 128, 4000, 24, 40),
     (np.uint8, O.L2, 128, 3000, 16, 30),
     (np.uint8, O.COSINE, 40, 2000, 16, 30),
@@ -620,7 +621,7 @@ def test_device_build_graph_is_valid_and_searchable(dab, dt, metric, dim, n):
 
 
 @pytest.mark.parametrize("dt,metric,d,n,R,Lb", [(np.float32, O.L2, 32, 1500, 16, 30), (np.int8, O.L2, 64, 1200, 12, 24),
-                                                (np.float32, O.INNER_PRODUCT, 24, 1000, 8, 20)])
+                                                (np.float32, O.INNER_PRODUCT, 24, 1000, 8, 20), (np.float32, O.COSINE, 32, 1200, 16, 30)])
 def test_device_build_one_insert_at_a_time_reproduces_the_sequential_reference_build(dab, dt, metric, d, n, R, Lb):
     """dab_build with batch_size = 1 is DiskANNIndex::insert for i = 0..n (index.rs:226-341: search with
     a VisitedSearchRecord, robust_prune, set_neighbors, add_edge_and_prune per out-edge): the adjacency

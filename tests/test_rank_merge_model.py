@@ -99,11 +99,8 @@ def merge_round_in_place_by_tiles(cap, old, ids, dists, tile):
         pos = int(np.sum(od_all < d)) + sum(1 for _, e, k in new if e < d or (e == d and k > j))
         if pos < cap:
             placed.append((pos, idn, d))
-    n_tiles = (cap + tile - 1) // tile
-    for c in range(n_tiles - 1, -1, -1):
+    for c in range((size + tile - 1) // tile - 1, -1, -1):                         # from the top occupied tile down
         e0 = c * tile
-        if e0 >= size:
-            continue
         regs = [(e, qi[e], qd[e]) for e in range(e0, min(e0 + tile, size))]      # the whole tile is read first ...
         for e, i, d in regs:                                                    # ... then its moved entries are written
             sh = sum(1 for _, x, _ in new if x <= d)
@@ -117,8 +114,9 @@ def merge_round_in_place_by_tiles(cap, old, ids, dists, tile):
 
 @pytest.mark.parametrize("seed", range(16))
 def test_tile_wise_in_place_merge_equals_the_rank_merge(seed):
-    """Lists longer than one register tile (the PQ traversal with L > 512): walking the tiles from the top one down and
-    rewriting the list in place gives the list the one-tile merge (and hence the sequential inserts) gives."""
+    """Lists longer than one register tile (the PQ traversal with L > 512, search_kernel_v2 with L + start points > 256):
+    walking the tiles from the top one down and rewriting the list in place gives the list the one-tile merge (and
+    hence the sequential inserts) gives."""
     rng = np.random.default_rng(100 + seed)
     cap = int(rng.integers(5, 60))
     tile = int(rng.integers(2, 9))

@@ -1,9 +1,10 @@
-"""search_kernel_v2's two row paths against the oracle: bit-identical ids, distance bits, result counts, cmps and hops.
+"""search_kernel_v2's three row paths against the oracle: bit-identical ids, distance bits, result counts, cmps and hops.
 
 f32 rows of 32 / 64 / 96 / 128 elements are read straight into registers when level 1 of the visited set is on
-(batches in flight); other rows, and synchronous calls, stage their rows in shared memory.  Both paths run here, synchronously and in flight, at list sizes from 25 to the
-v2 limit (L + start points = 256), beam widths 1 / 2 / 4, several start points, adjacency rows longer than the
-96-word speculative buffer, and with level 1 forced to close early."""
+(batches in flight); other rows, and synchronous calls, stage their rows in shared memory, as long as the list fits one
+register tile (L + start points <= 256).  Longer lists and float Metric::Cosine read their rows from global memory.
+All paths run here, synchronously and in flight, at list sizes from 25 to 1103, beam widths 1 / 2 / 4, several start
+points, adjacency rows longer than the 96-word speculative buffer, and with level 1 forced to close early."""
 
 import numpy as np
 import pytest
@@ -29,6 +30,8 @@ def make_index(rng, metric, n, d, R, L_build, n_start=1, dt=np.float32):
         base /= np.linalg.norm(base, axis=1, keepdims=True)
     if dt == np.int8:
         base = np.clip(np.round(base * 40), -127, 127)
+    elif dt == np.uint8:
+        base = np.clip(np.round(base * 40 + 128), 0, 255)
     base = base.astype(dt)
     starts = base[rng.choice(n, n_start, replace=False)]
     vecs = np.concatenate([base, starts])
@@ -37,6 +40,8 @@ def make_index(rng, metric, n, d, R, L_build, n_start=1, dt=np.float32):
     queries = vecs[rng.integers(0, n, 160)].astype(np.float32) + 0.05 * rng.normal(size=(160, d)).astype(np.float32)
     if dt == np.int8:
         queries = np.clip(np.round(queries), -127, 127)
+    elif dt == np.uint8:
+        queries = np.clip(np.round(queries), 0, 255)
     return vecs, adj, maxdeg, queries.astype(dt)
 
 
@@ -99,19 +104,40 @@ def test_staged_rows_of_other_types(dab, dt, dim):
     check(dab, vecs, adj, maxdeg, queries, n, 1, O.L2, [(25, 1), (100, 4), (255, 2)])
 
 
+@pytest.mark.parametrize("n_start", [1, 3])
+@pytest.mark.parametrize("dt,metric", [(np.float32, O.L2), (np.float32, O.COSINE), (np.float16, O.INNER_PRODUCT), (np.int8, O.L2),
+                                       (np.uint8, O.COSINE)])
+def test_lists_longer_than_256(dab, dt, metric, n_start):
+    """L + start points from 301 to 1103: lists merged tile by tile, up to five tiles of 256 entries."""
+    rng = np.random.default_rng(int(metric) * 10 + n_start + np.dtype(dt).itemsize)
+    n = 2500
+    vecs, adj, maxdeg, queries = make_index(rng, metric, n, 64, 16, 30, n_start=n_start, dt=dt)
+    check(dab, vecs, adj, maxdeg, queries, n, n_start, metric, [(L, beam) for L in (300, 700, 1100) for beam in (1, 2)])
+
+
+def test_rows_too_wide_to_stage(dab):
+    """6000-d f32 rows: a stage of eight (192 KB) does not fit beside the rest of the layout, so they are read from
+    global memory, as for lists of any length."""
+    rng = np.random.default_rng(6000)
+    n = 400
+    vecs, adj, maxdeg, queries = make_index(rng, O.L2, n, 6000, 8, 20)
+    check(dab, vecs, adj, maxdeg, queries, n, 1, O.L2, [(40, 1), (60, 2)])
+
+
 def test_the_register_path_is_the_one_dispatched(dab):
-    """in flight, 128-d f32 launches the register instantiation and 100-d f32 the staged one; synchronous calls stage."""
+    """in flight, 128-d f32 launches the register instantiation and 100-d f32 the staged one; synchronous calls stage.
+    Float Metric::Cosine and lists longer than 256 launch the instantiation for lists of any length."""
     import torch
 
-    def kernels(g, q, in_flight):
+    def kernels(g, q, in_flight, L=100):
         with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
             if in_flight:
-                g.search_batch_async(0, q, 10, 100)
+                g.search_batch_async(0, q, 10, L)
                 g.wait(0)
             else:
-                g.search_batch(q, 10, 100)
+                g.search_batch(q, 10, L)
             torch.cuda.synchronize()
-        return {e.key for e in prof.key_averages() if "search_kernel_v2" in e.key}
+        return {e.key for e in prof.key_averages() if "search_kernel" in e.key}
 
     rng = np.random.default_rng(4)
     for dim, reg in ((128, True), (100, False)):
@@ -124,3 +150,13 @@ def test_the_register_path_is_the_one_dispatched(dab):
         assert flight and sync, (flight, sync)
         assert all(k.replace(" ", "").endswith(f"true,{'true' if reg else 'false'}>(dab::SearchParamsV2)") for k in flight), flight
         assert all(k.replace(" ", "").endswith("false,false>(dab::SearchParamsV2)") for k in sync), sync
+    for metric, dim, L in ((O.COSINE, 64, 100), (O.L2, 128, 300)):
+        n = 2000
+        vecs, adj, maxdeg, queries = make_index(rng, metric, n, dim, 16, 30)
+        with dab.GpuIndex(dab.DType.f32, metric, dim, n, 1, maxdeg) as g:
+            g.upload_vectors(vecs)
+            g.upload_graph(adj)
+            for in_flight in (True, False):
+                launched = kernels(g, queries, in_flight, L)
+                assert launched and all("search_kernel_v2<" in k for k in launched), launched
+                assert all(k.replace(" ", "").endswith(",0,false,false>(dab::SearchParamsV2)") for k in launched), launched

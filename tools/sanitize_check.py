@@ -64,7 +64,7 @@ for dt, ddt, metric, d in ((np.float32, dab.DType.f32, dab.Metric.L2, 100), (np.
         out = g.distances(base[:50], ids)                        # frontier kernels (wide for f32 / f16)
         pairs = g.row_pair_distances(ids[1, :40], ids[2, :40])
         block = g.pairwise(ids[3, :17])
-        got = g.search_batch(base[:64], 5, 64, 1)                # search_kernel_v2 / generic
+        got = g.search_batch(base[:64], 5, 64, 1)                # search_kernel_v2
         got4 = g.search_batch(base[:64], 5, 40, 4)
         knn = g.flat_knn(base[:16], 5)
         knn_tc = g.flat_knn_tc(base[:16], 5)                     # wgmma + TMA path
