@@ -420,34 +420,6 @@ __global__ void iota_kernel(uint32_t* p, uint32_t first, uint32_t n) {
 }
 
 // ------------------------------------------------------------------ host dispatch
-#define DAB_DATA_DISPATCH(idx, plan, CALL)                                                             \
-    do {                                                                                               \
-        switch ((idx)->dtype) {                                                                        \
-            case DAB_F32:                                                                              \
-                if ((plan).kind == KIND_L2) { CALL(float, 4, KIND_L2, POST_ID, false, false); }         \
-                else if ((plan).kind == KIND_IP && (plan).post == POST_NEG) { CALL(float, 4, KIND_IP, POST_NEG, false, false); } \
-                else if ((plan).kind == KIND_IP) { CALL(float, 4, KIND_IP, POST_ONE_MINUS, false, false); } \
-                else { CALL(float, 2, KIND_COS, POST_ONE_MINUS, false, false); }                        \
-                break;                                                                                 \
-            case DAB_F16: /* f16 x f16: Strategy2x4 for every schema (simd.rs:989, 1752, 2591) */      \
-                if ((plan).kind == KIND_L2) { CALL(__half, 2, KIND_L2, POST_ID, false, false); }        \
-                else if ((plan).kind == KIND_IP && (plan).post == POST_NEG) { CALL(__half, 2, KIND_IP, POST_NEG, false, false); } \
-                else if ((plan).kind == KIND_IP) { CALL(__half, 2, KIND_IP, POST_ONE_MINUS, false, false); } \
-                else { CALL(__half, 2, KIND_COS, POST_ONE_MINUS, false, false); }                       \
-                break;                                                                                 \
-            case DAB_I8:                                                                               \
-                if ((plan).kind == KIND_L2) { CALL(uint8_t, 4, KIND_L2, POST_ID, true, true); }         \
-                else if ((plan).kind == KIND_IP) { CALL(uint8_t, 4, KIND_IP, POST_NEG, true, true); }   \
-                else { CALL(uint8_t, 4, KIND_COS, POST_ONE_MINUS, true, true); }                        \
-                break;                                                                                 \
-            default:                                                                                   \
-                if ((plan).kind == KIND_L2) { CALL(uint8_t, 4, KIND_L2, POST_ID, true, false); }        \
-                else if ((plan).kind == KIND_IP) { CALL(uint8_t, 4, KIND_IP, POST_NEG, true, false); }  \
-                else { CALL(uint8_t, 4, KIND_COS, POST_ONE_MINUS, true, false); }                       \
-                break;                                                                                 \
-        }                                                                                              \
-    } while (0)
-
 static uint32_t pow2_at_least(uint32_t v) {
     uint32_t p = 2;
     while (p < v) p <<= 1;
@@ -455,8 +427,6 @@ static uint32_t pow2_at_least(uint32_t v) {
 }
 
 static int launch_prune(const dab_index* idx, PruneParams& p) {
-    const bool is_int = idx->dtype == DAB_I8 || idx->dtype == DAB_U8;
-    const MetricPlan plan = plan_for(idx->metric, is_int);
     p.vectors = idx->d_vectors;
     p.row_stride = idx->row_stride;
     p.dim = (int)idx->dim;
@@ -465,22 +435,20 @@ static int launch_prune(const dab_index* idx, PruneParams& p) {
     const size_t smem = prune_smem_bytes(p.P) * kPruneWarps;
     if (smem > 200 * 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "prune: pool capacity %u too large", p.pool_cap);
     const int grid = (int)std::min<uint64_t>(((uint64_t)p.n_pools + kPruneWarps - 1) / kPruneWarps, (uint64_t)idx->sm_count * 8);
-#define CALL(TD, NA, K, P_, II, SG)                                                                        \
-    do {                                                                                                   \
-        auto kern = prune_pools_kernel<TD, NA, K, P_, II, SG>;                                             \
-        DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));      \
-        kern<<<grid, kPruneWarps * 32, smem, idx->stream>>>(p);                                            \
-    } while (0)
-    DAB_DATA_DISPATCH(idx, plan, CALL);
-#undef CALL
+    const int rc = visit_schema<OPS_ROW>(idx->dtype, idx->metric, [&](auto s) -> int {
+        using S = decltype(s);
+        auto kern = prune_pools_kernel<KernelRow<S>, S::NA, S::KIND, S::POST, S::IS_INT, S::SIGNED>;
+        DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kern<<<grid, kPruneWarps * 32, smem, idx->stream>>>(p);
+        return DAB_OK;
+    });
+    if (rc) return rc;
     DAB_LAUNCHED();
     DAB_CUDA(cudaGetLastError());
     return DAB_OK;
 }
 
 static int launch_backedges(const dab_index* idx, BackedgeParams& p) {
-    const bool is_int = idx->dtype == DAB_I8 || idx->dtype == DAB_U8;
-    const MetricPlan plan = plan_for(idx->metric, is_int);
     p.vectors = idx->d_vectors;
     p.row_stride = idx->row_stride;
     p.dim = (int)idx->dim;
@@ -494,14 +462,14 @@ static int launch_backedges(const dab_index* idx, BackedgeParams& p) {
     if (smem > 200 * 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "build: max_degree %u too large", idx->max_degree);
     const uint32_t chunks = (p.n_pairs + 31) / 32;
     const int grid = (int)std::min<uint64_t>(((uint64_t)chunks + kPruneWarps - 1) / kPruneWarps, (uint64_t)idx->sm_count * 8);
-#define CALL(TD, NA, K, P_, II, SG)                                                                        \
-    do {                                                                                                   \
-        auto kern = backedge_kernel<TD, NA, K, P_, II, SG>;                                                \
-        DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));      \
-        kern<<<grid, kPruneWarps * 32, smem, idx->stream>>>(p);                                            \
-    } while (0)
-    DAB_DATA_DISPATCH(idx, plan, CALL);
-#undef CALL
+    const int rc = visit_schema<OPS_ROW>(idx->dtype, idx->metric, [&](auto s) -> int {
+        using S = decltype(s);
+        auto kern = backedge_kernel<KernelRow<S>, S::NA, S::KIND, S::POST, S::IS_INT, S::SIGNED>;
+        DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kern<<<grid, kPruneWarps * 32, smem, idx->stream>>>(p);
+        return DAB_OK;
+    });
+    if (rc) return rc;
     DAB_LAUNCHED();
     DAB_CUDA(cudaGetLastError());
     return DAB_OK;

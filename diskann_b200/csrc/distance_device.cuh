@@ -21,6 +21,10 @@
 #include <cuda_fp16.h>
 #include <stdint.h>
 
+#include <type_traits>
+
+#include "dab_common.cuh"
+
 namespace dab {
 
 enum Kind { KIND_L2 = 0, KIND_IP = 1, KIND_COS = 2 };
@@ -248,6 +252,54 @@ __host__ __device__ inline MetricPlan plan_for(int metric, bool is_int) {
         case DAB_COSINE: return {KIND_COS, POST_ONE_MINUS};
         default: return is_int ? MetricPlan{KIND_COS, POST_ONE_MINUS} : MetricPlan{KIND_IP, POST_ONE_MINUS};
     }
+}
+
+// ---- schema dispatch (host) --------------------------------------------------------------
+// What a row of the index is compared with: a query (float queries are widened to f32,
+// diskann-inmem/src/layers/full.rs:421-423) or another row of the index (data x data).
+enum Operands { OPS_QUERY, OPS_ROW };
+
+// The compile-time values of one distance schema, as the launchers' kernels take them.
+template <typename TQ_, typename TD_, int NA_, int KIND_, int POST_>
+struct Schema {
+    using TQ = TQ_;  // the other operand: float, __half (f16 x f16), int8_t or uint8_t
+    using TD = TD_;  // row elements: float, __half, int8_t or uint8_t
+    static constexpr int NA = NA_, KIND = KIND_, POST = POST_;
+    static constexpr bool IS_INT = std::is_same<TD, int8_t>::value || std::is_same<TD, uint8_t>::value;
+    static constexpr bool SIGNED = std::is_same<TD, int8_t>::value;
+};
+
+// The row type of the kernels that take integer rows as uint8_t plus a SIGNED flag.
+template <typename S>
+using KernelRow = typename std::conditional<S::IS_INT, uint8_t, typename S::TD>::type;
+
+// The reference's schema for TQ x TD under `metric`: (KIND, POST) from plan_for; NA = 2 for cosine over
+// float operands and for f16 x f16 (Strategy2x4, simd.rs:424-483, 989, 1752, 2591), otherwise NA = 4
+// (Strategy4x1 / 4x2; the integer kernels ignore it).  Only these schemas are ever instantiated.
+template <typename TQ, typename TD, typename F>
+int visit_plan(int metric, F&& f) {
+    constexpr bool I = std::is_same<TD, int8_t>::value || std::is_same<TD, uint8_t>::value;
+    constexpr int NA = std::is_same<TQ, __half>::value ? 2 : 4;
+    const MetricPlan plan = plan_for(metric, I);
+    if (plan.kind == KIND_L2) return f(Schema<TQ, TD, NA, KIND_L2, POST_ID>{});
+    if (plan.kind == KIND_COS) return f(Schema<TQ, TD, I ? 4 : 2, KIND_COS, POST_ONE_MINUS>{});
+    if constexpr (!I) {  // float CosineNormalized; for integers it is Cosine
+        if (plan.post == POST_ONE_MINUS) return f(Schema<TQ, TD, NA, KIND_IP, POST_ONE_MINUS>{});
+    }
+    return f(Schema<TQ, TD, NA, KIND_IP, POST_NEG>{});
+}
+
+// Calls f(Schema<...>{}) once, with the schema of rows of `dtype` against operands O under `metric`,
+// and returns what f returns.
+template <Operands O, typename F>
+int visit_schema(int dtype, int metric, F&& f) {
+    switch (dtype) {
+        case DAB_F32: return visit_plan<float, float>(metric, f);
+        case DAB_F16: return visit_plan<typename std::conditional<O == OPS_QUERY, float, __half>::type, __half>(metric, f);
+        case DAB_I8: return visit_plan<int8_t, int8_t>(metric, f);
+        case DAB_U8: return visit_plan<uint8_t, uint8_t>(metric, f);
+    }
+    return fail(DAB_ERR_INVALID_ARGUMENT, "unsupported dtype %d", dtype);
 }
 
 }  // namespace dab

@@ -9,19 +9,6 @@ namespace dab {
 
 constexpr int kWarpsPerBlock = 8;
 
-template <typename T>
-struct IsInt {
-    static constexpr bool value = false;
-};
-template <>
-struct IsInt<int8_t> {
-    static constexpr bool value = true;
-};
-template <>
-struct IsInt<uint8_t> {
-    static constexpr bool value = true;
-};
-
 // ------------------------------------------------------------------ n independent pairs
 // x[i] (dense rows of TX), y[i] (dense rows of TY) -> out[i]
 template <typename TX, typename TY, int NA, int KIND, int POST>
@@ -402,51 +389,24 @@ static int grid_for(uint64_t work_warps, int sm_count) {
     return (int)blocks;
 }
 
-#define DAB_KIND_POST_SWITCH(plan, MACRO)                                                       \
-    do {                                                                                        \
-        if ((plan).kind == KIND_L2) { MACRO(KIND_L2, POST_ID); }                                \
-        else if ((plan).kind == KIND_IP && (plan).post == POST_NEG) { MACRO(KIND_IP, POST_NEG); } \
-        else if ((plan).kind == KIND_IP) { MACRO(KIND_IP, POST_ONE_MINUS); }                    \
-        else { MACRO(KIND_COS, POST_ONE_MINUS); }                                               \
-    } while (0)
-
 int launch_pairs(int dx, int dy, int metric, int dim, const void* x, size_t xs, const void* y, size_t ys, uint64_t n,
                  float* out, int sm_count, cudaStream_t stream) {
-    const bool is_int = dx == DAB_I8 || dx == DAB_U8;
-    const MetricPlan plan = plan_for(metric, is_int);
     const int grid = grid_for(n, sm_count);
     const int block = kWarpsPerBlock * 32;
-    if (dx == DAB_F32 && dy == DAB_F32) {
-#define L(K, P)                                                                                       \
-    if (K == KIND_COS)                                                                                \
-        pair_float_kernel<float, float, 2, K, P><<<grid, block, 0, stream>>>((const float*)x, xs, (const float*)y, ys, n, dim, out); \
-    else                                                                                              \
-        pair_float_kernel<float, float, 4, K, P><<<grid, block, 0, stream>>>((const float*)x, xs, (const float*)y, ys, n, dim, out)
-        DAB_KIND_POST_SWITCH(plan, L);
-#undef L
-    } else if (dx == DAB_F16 && dy == DAB_F16) {
-#define L(K, P) pair_float_kernel<__half, __half, 2, K, P><<<grid, block, 0, stream>>>((const __half*)x, xs, (const __half*)y, ys, n, dim, out)
-        DAB_KIND_POST_SWITCH(plan, L);
-#undef L
-    } else if (dx == DAB_F32 && dy == DAB_F16) {
-#define L(K, P)                                                                                       \
-    if (K == KIND_COS)                                                                                \
-        pair_float_kernel<float, __half, 2, K, P><<<grid, block, 0, stream>>>((const float*)x, xs, (const __half*)y, ys, n, dim, out); \
-    else                                                                                              \
-        pair_float_kernel<float, __half, 4, K, P><<<grid, block, 0, stream>>>((const float*)x, xs, (const __half*)y, ys, n, dim, out)
-        DAB_KIND_POST_SWITCH(plan, L);
-#undef L
-    } else if (dx == DAB_I8 && dy == DAB_I8) {
-#define L(K, P) pair_int_kernel<true, K, P><<<grid, block, 0, stream>>>((const uint8_t*)x, xs, (const uint8_t*)y, ys, n, dim, out)
-        DAB_KIND_POST_SWITCH(plan, L);
-#undef L
-    } else if (dx == DAB_U8 && dy == DAB_U8) {
-#define L(K, P) pair_int_kernel<false, K, P><<<grid, block, 0, stream>>>((const uint8_t*)x, xs, (const uint8_t*)y, ys, n, dim, out)
-        DAB_KIND_POST_SWITCH(plan, L);
-#undef L
-    } else {
-        return fail(DAB_ERR_INVALID_ARGUMENT, "unsupported dtype pair (%d, %d)", dx, dy);
-    }
+    auto launch = [&](auto s) -> int {
+        using S = decltype(s);
+        if constexpr (S::IS_INT)
+            pair_int_kernel<S::SIGNED, S::KIND, S::POST><<<grid, block, 0, stream>>>((const uint8_t*)x, xs, (const uint8_t*)y, ys, n, dim, out);
+        else
+            pair_float_kernel<typename S::TQ, typename S::TD, S::NA, S::KIND, S::POST><<<grid, block, 0, stream>>>(
+                (const typename S::TQ*)x, xs, (const typename S::TD*)y, ys, n, dim, out);
+        return DAB_OK;
+    };
+    int rc;
+    if (dx == dy) rc = visit_schema<OPS_ROW>(dy, metric, launch);
+    else if (dx == DAB_F32 && dy == DAB_F16) rc = visit_schema<OPS_QUERY>(dy, metric, launch);
+    else return fail(DAB_ERR_INVALID_ARGUMENT, "unsupported dtype pair (%d, %d)", dx, dy);
+    if (rc) return rc;
     DAB_LAUNCHED();
     DAB_CUDA(cudaGetLastError());
     return DAB_OK;
@@ -454,145 +414,68 @@ int launch_pairs(int dx, int dy, int metric, int dim, const void* x, size_t xs, 
 
 int launch_frontier(const dab_index* idx, const void* d_queries, uint32_t nq, const uint32_t* d_ids, uint32_t c,
                     float* d_out) {
-    const bool is_int = idx->dtype == DAB_I8 || idx->dtype == DAB_U8;
-    const MetricPlan plan = plan_for(idx->metric, is_int);
     const uint64_t tiles = (uint64_t)nq * ((c + 31) / 32);
     const int grid = grid_for(tiles, idx->sm_count);
     const int block = kWarpsPerBlock * 32;
     const int dim = (int)idx->dim;
-    const size_t smem = (size_t)kWarpsPerBlock * (is_int ? ((dim + 3) & ~3) : dim * 4);
-    if (smem > 200 * 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "dim %d too large for the frontier kernel", dim);
     cudaStream_t st = idx->stream;
-    constexpr int U = 4;
-    // NA = 4 schemas over f32 / f16 rows: the wide-load kernel (16 B per lane)
-    const bool wide = plan.kind != KIND_COS && (idx->dtype == DAB_F32 || idx->dtype == DAB_F16) && idx->row_stride % 16 == 0;
-    if (wide) {
-        const int qstride = (dim + 3) & ~3;
-        const size_t wsmem = (size_t)kWarpsPerBlock * qstride * 4;
-#define LW(TQ, TDD, K, P)                                                                                          \
-    do {                                                                                                          \
-        auto kern = frontier_wide_kernel<TQ, TDD, K, P>;                                                          \
-        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsmem);                      \
-        kern<<<grid, block, wsmem, st>>>((const TQ*)d_queries, nq, d_ids, c, idx->d_vectors, idx->row_stride,      \
-                                         idx->n_total(), dim, qstride, d_out);                                    \
-    } while (0)
-        if (idx->dtype == DAB_F32) {
-            if (plan.kind == KIND_L2) LW(float, float, KIND_L2, POST_ID);
-            else if (plan.post == POST_NEG) LW(float, float, KIND_IP, POST_NEG);
-            else LW(float, float, KIND_IP, POST_ONE_MINUS);
+    const int rc = visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto s) -> int {
+        using S = decltype(s);
+        using TD = typename S::TD;
+        constexpr int K = S::KIND, P = S::POST, U = 4;
+        const size_t smem = (size_t)kWarpsPerBlock * (S::IS_INT ? ((dim + 3) & ~3) : dim * 4);
+        if (smem > 200 * 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "dim %d too large for the frontier kernel", dim);
+        if constexpr (S::IS_INT) {
+            if (dim % 16 == 0 && ((uintptr_t)d_queries & 15) == 0) {
+                const size_t ismem = (size_t)kWarpsPerBlock * dim;
+                auto kern = frontier_int_wide_kernel<S::SIGNED, K, P>;
+                cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ismem);
+                kern<<<grid, block, ismem, st>>>((const uint8_t*)d_queries, nq, d_ids, c, idx->d_vectors, idx->row_stride,
+                                                 idx->n_total(), dim, d_out);
+            } else {
+                auto kern = frontier_int_kernel<S::SIGNED, K, P, U>;
+                cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+                kern<<<grid, block, smem, st>>>((const uint8_t*)d_queries, nq, d_ids, c, idx->d_vectors, idx->row_stride,
+                                                idx->n_total(), dim, d_out);
+            }
+        } else if constexpr (S::NA == 4) {
+            // the wide-load kernel, 16 B per lane: rows are 16-byte aligned, row_stride is a multiple of 32 (dab_create)
+            const int qstride = (dim + 3) & ~3;
+            const size_t wsmem = (size_t)kWarpsPerBlock * qstride * 4;
+            auto kern = frontier_wide_kernel<TD, TD, K, P>;
+            cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsmem);
+            kern<<<grid, block, wsmem, st>>>((const TD*)d_queries, nq, d_ids, c, idx->d_vectors, idx->row_stride, idx->n_total(),
+                                             dim, qstride, d_out);
         } else {
-            if (plan.kind == KIND_L2) LW(__half, __half, KIND_L2, POST_ID);
-            else if (plan.post == POST_NEG) LW(__half, __half, KIND_IP, POST_NEG);
-            else LW(__half, __half, KIND_IP, POST_ONE_MINUS);
+            auto kern = frontier_float_kernel<typename S::TQ, TD, TD, S::NA, K, P, U>;
+            cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            kern<<<grid, block, smem, st>>>((const TD*)d_queries, nq, d_ids, c, idx->d_vectors, idx->row_stride, idx->n_total(),
+                                            dim, d_out);
         }
-#undef LW
-        DAB_LAUNCHED();
-        DAB_CUDA(cudaGetLastError());
         return DAB_OK;
-    }
-#define ARGS nq, d_ids, c, idx->d_vectors, idx->row_stride, idx->n_total(), dim, d_out
-    if (idx->dtype == DAB_F32) {
-#define L(K, P)                                                                                                   \
-    do {                                                                                                          \
-        if (K == KIND_COS) {                                                                                      \
-            auto kern = frontier_float_kernel<float, float, float, 2, K, P, U>;                                    \
-            cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);                   \
-            kern<<<grid, block, smem, st>>>((const float*)d_queries, ARGS);                                       \
-        } else {                                                                                                  \
-            auto kern = frontier_float_kernel<float, float, float, 4, K, P, U>;                                    \
-            cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);                   \
-            kern<<<grid, block, smem, st>>>((const float*)d_queries, ARGS);                                       \
-        }                                                                                                         \
-    } while (0)
-        DAB_KIND_POST_SWITCH(plan, L);
-#undef L
-    } else if (idx->dtype == DAB_F16) {
-#define L(K, P)                                                                                                   \
-    do {                                                                                                          \
-        if (K == KIND_COS) {                                                                                      \
-            auto kern = frontier_float_kernel<float, __half, __half, 2, K, P, U>;                                  \
-            cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);                   \
-            kern<<<grid, block, smem, st>>>((const __half*)d_queries, ARGS);                                      \
-        } else {                                                                                                  \
-            auto kern = frontier_float_kernel<float, __half, __half, 4, K, P, U>;                                  \
-            cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);                   \
-            kern<<<grid, block, smem, st>>>((const __half*)d_queries, ARGS);                                      \
-        }                                                                                                         \
-    } while (0)
-        DAB_KIND_POST_SWITCH(plan, L);
-#undef L
-    } else if (is_int && dim % 16 == 0 && ((uintptr_t)d_queries & 15) == 0) {
-        const size_t ismem = (size_t)kWarpsPerBlock * dim;
-#define L(K, P)                                                                                   \
-    do {                                                                                          \
-        if (idx->dtype == DAB_I8) {                                                               \
-            auto kern = frontier_int_wide_kernel<true, K, P>;                                     \
-            cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ismem);  \
-            kern<<<grid, block, ismem, st>>>((const uint8_t*)d_queries, ARGS);                    \
-        } else {                                                                                  \
-            auto kern = frontier_int_wide_kernel<false, K, P>;                                    \
-            cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ismem);  \
-            kern<<<grid, block, ismem, st>>>((const uint8_t*)d_queries, ARGS);                    \
-        }                                                                                         \
-    } while (0)
-        DAB_KIND_POST_SWITCH(plan, L);
-#undef L
-    } else if (idx->dtype == DAB_I8) {
-#define L(K, P)                                                                                   \
-    do {                                                                                          \
-        auto kern = frontier_int_kernel<true, K, P, U>;                                           \
-        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);       \
-        kern<<<grid, block, smem, st>>>((const uint8_t*)d_queries, ARGS);                         \
-    } while (0)
-        DAB_KIND_POST_SWITCH(plan, L);
-#undef L
-    } else {
-#define L(K, P)                                                                                   \
-    do {                                                                                          \
-        auto kern = frontier_int_kernel<false, K, P, U>;                                          \
-        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);       \
-        kern<<<grid, block, smem, st>>>((const uint8_t*)d_queries, ARGS);                         \
-    } while (0)
-        DAB_KIND_POST_SWITCH(plan, L);
-#undef L
-    }
-#undef ARGS
+    });
+    if (rc) return rc;
     DAB_LAUNCHED();
     DAB_CUDA(cudaGetLastError());
     return DAB_OK;
 }
 
 int launch_rowpairs(const dab_index* idx, const uint32_t* d_a, const uint32_t* d_b, uint64_t n, float* d_out) {
-    const bool is_int = idx->dtype == DAB_I8 || idx->dtype == DAB_U8;
-    const MetricPlan plan = plan_for(idx->metric, is_int);
     const int grid = grid_for(n, idx->sm_count);
     const int block = kWarpsPerBlock * 32;
     const int dim = (int)idx->dim;
     cudaStream_t st = idx->stream;
-#define ARGS d_a, d_b, n, idx->d_vectors, idx->row_stride, idx->n_total(), dim, d_out
-    if (idx->dtype == DAB_F32) {
-#define L(K, P)                                                             \
-    if (K == KIND_COS)                                                      \
-        rowpair_float_kernel<float, 2, K, P><<<grid, block, 0, st>>>(ARGS); \
-    else                                                                    \
-        rowpair_float_kernel<float, 4, K, P><<<grid, block, 0, st>>>(ARGS)
-        DAB_KIND_POST_SWITCH(plan, L);
-#undef L
-    } else if (idx->dtype == DAB_F16) {
-        // data x data for f16 is the f16 x f16 schema (Strategy2x4), simd.rs:989, 1752, 2591
-#define L(K, P) rowpair_float_kernel<__half, 2, K, P><<<grid, block, 0, st>>>(ARGS)
-        DAB_KIND_POST_SWITCH(plan, L);
-#undef L
-    } else if (idx->dtype == DAB_I8) {
-#define L(K, P) rowpair_int_kernel<true, K, P><<<grid, block, 0, st>>>(ARGS)
-        DAB_KIND_POST_SWITCH(plan, L);
-#undef L
-    } else {
-#define L(K, P) rowpair_int_kernel<false, K, P><<<grid, block, 0, st>>>(ARGS)
-        DAB_KIND_POST_SWITCH(plan, L);
-#undef L
-    }
-#undef ARGS
+    const int rc = visit_schema<OPS_ROW>(idx->dtype, idx->metric, [&](auto s) -> int {
+        using S = decltype(s);
+        if constexpr (S::IS_INT)
+            rowpair_int_kernel<S::SIGNED, S::KIND, S::POST><<<grid, block, 0, st>>>(d_a, d_b, n, idx->d_vectors, idx->row_stride,
+                                                                                    idx->n_total(), dim, d_out);
+        else
+            rowpair_float_kernel<typename S::TD, S::NA, S::KIND, S::POST><<<grid, block, 0, st>>>(
+                d_a, d_b, n, idx->d_vectors, idx->row_stride, idx->n_total(), dim, d_out);
+        return DAB_OK;
+    });
+    if (rc) return rc;
     DAB_LAUNCHED();
     DAB_CUDA(cudaGetLastError());
     return DAB_OK;

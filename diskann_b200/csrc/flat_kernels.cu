@@ -252,8 +252,6 @@ int dab_flat_knn(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, u
     if (!queries || !out_ids || !out_dists) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_flat_knn: NULL argument");
     if (k == 0 || k > 2048) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_flat_knn: k must be in [1, 2048]");
     DAB_CUDA(cudaSetDevice(idx->device));
-    const bool is_int = idx->dtype == DAB_I8 || idx->dtype == DAB_U8;
-    const MetricPlan plan = plan_for(idx->metric, is_int);
     const int dim = (int)idx->dim;
     const uint32_t n = (uint32_t)idx->n_points;  // start points are not data
     cudaStream_t st = idx->stream;
@@ -283,66 +281,37 @@ int dab_flat_knn(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, u
     uint32_t* d_top_n = (uint32_t*)(d_top_d + (size_t)nq * k);
     DAB_CUDA(cudaMemsetAsync(d_top_n, 0, (size_t)nq * 4, st));
 
-    const bool fast = !is_int && plan.kind != KIND_COS && (size_t)kFlatWarps * kFQ * dim * 4 <= 200 * 1024;
+    const bool fast_fits = (size_t)kFlatWarps * kFQ * dim * 4 <= 200 * 1024;
     for (uint32_t r0 = 0; r0 < n; r0 += rb) {
         const uint32_t r1 = std::min(n, r0 + rb);
-        if (fast) {
-            const size_t smem = (size_t)kFlatWarps * kFQ * dim * 4;
-            const uint32_t qtiles = (nq + kFlatWarps * kFQ - 1) / (kFlatWarps * kFQ);
-            // enough CTAs along rows to fill the machine ~4x, at least 64 rows per CTA
-            uint32_t rsplit = std::max<uint32_t>(1, std::min<uint32_t>((r1 - r0 + 63) / 64, (idx->sm_count * 8 + qtiles - 1) / qtiles));
-            uint32_t rows_per_cta = ((r1 - r0 + rsplit - 1) / rsplit + kFR - 1) / kFR * kFR;
-            rsplit = (r1 - r0 + rows_per_cta - 1) / rows_per_cta;
-            dim3 grid(rsplit, qtiles);
-#define FLAT(TD, K, P)                                                                                          \
-    do {                                                                                                        \
-        auto kern = flat_float_kernel<TD, K, P>;                                                                \
-        DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));           \
-        kern<<<grid, kFlatWarps * 32, smem, st>>>((const float*)d_q, nq, idx->d_vectors, idx->row_stride, r0, r1, dim, \
-                                                  d_dist, rb, rows_per_cta);                                    \
-    } while (0)
-#define FLAT_T(TD)                                                                         \
-    do {                                                                                   \
-        if (plan.kind == KIND_L2) FLAT(TD, KIND_L2, POST_ID);                              \
-        else if (plan.post == POST_NEG) FLAT(TD, KIND_IP, POST_NEG);                       \
-        else FLAT(TD, KIND_IP, POST_ONE_MINUS);                                            \
-    } while (0)
-            if (idx->dtype == DAB_F32) FLAT_T(float);
-            else FLAT_T(__half);
-#undef FLAT_T
-#undef FLAT
-        } else {
-            const size_t qb = is_int ? round_up(dim, 4) : (size_t)dim * 4;
+        rc = visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto s) -> int {
+            using S = decltype(s);
+            if constexpr (!S::IS_INT && S::KIND != KIND_COS) {
+                if (fast_fits) {
+                    const size_t smem = (size_t)kFlatWarps * kFQ * dim * 4;
+                    const uint32_t qtiles = (nq + kFlatWarps * kFQ - 1) / (kFlatWarps * kFQ);
+                    // enough CTAs along rows to fill the machine ~4x, at least 64 rows per CTA
+                    uint32_t rsplit = std::max<uint32_t>(1, std::min<uint32_t>((r1 - r0 + 63) / 64, (idx->sm_count * 8 + qtiles - 1) / qtiles));
+                    uint32_t rows_per_cta = ((r1 - r0 + rsplit - 1) / rsplit + kFR - 1) / kFR * kFR;
+                    rsplit = (r1 - r0 + rows_per_cta - 1) / rows_per_cta;
+                    dim3 grid(rsplit, qtiles);
+                    auto kern = flat_float_kernel<typename S::TD, S::KIND, S::POST>;
+                    DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                    kern<<<grid, kFlatWarps * 32, smem, st>>>((const float*)d_q, nq, idx->d_vectors, idx->row_stride, r0, r1, dim,
+                                                              d_dist, rb, rows_per_cta);
+                    return DAB_OK;
+                }
+            }
+            const size_t qb = S::IS_INT ? round_up(dim, 4) : (size_t)dim * 4;
             const size_t smem = (size_t)kFlatWarps * round_up(qb, 16);
             const uint64_t tiles = (uint64_t)nq * ((r1 - r0 + 31) / 32);
             int grid = (int)std::min<uint64_t>((tiles + kFlatWarps - 1) / kFlatWarps, (uint64_t)idx->sm_count * 8);
-#define GEN(TD, NA, K, P, II, SG)                                                                               \
-    do {                                                                                                        \
-        auto kern = flat_generic_kernel<TD, NA, K, P, II, SG>;                                                  \
-        DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));           \
-        kern<<<grid, kFlatWarps * 32, smem, st>>>(d_q, nq, idx->d_vectors, idx->row_stride, r0, r1, dim, d_dist, rb); \
-    } while (0)
-            if (idx->dtype == DAB_F32) {
-                if (plan.kind == KIND_COS) GEN(float, 2, KIND_COS, POST_ONE_MINUS, false, false);
-                else if (plan.kind == KIND_L2) GEN(float, 4, KIND_L2, POST_ID, false, false);
-                else if (plan.post == POST_NEG) GEN(float, 4, KIND_IP, POST_NEG, false, false);
-                else GEN(float, 4, KIND_IP, POST_ONE_MINUS, false, false);
-            } else if (idx->dtype == DAB_F16) {
-                if (plan.kind == KIND_COS) GEN(__half, 2, KIND_COS, POST_ONE_MINUS, false, false);
-                else if (plan.kind == KIND_L2) GEN(__half, 4, KIND_L2, POST_ID, false, false);
-                else if (plan.post == POST_NEG) GEN(__half, 4, KIND_IP, POST_NEG, false, false);
-                else GEN(__half, 4, KIND_IP, POST_ONE_MINUS, false, false);
-            } else if (idx->dtype == DAB_I8) {
-                if (plan.kind == KIND_L2) GEN(uint8_t, 4, KIND_L2, POST_ID, true, true);
-                else if (plan.kind == KIND_IP) GEN(uint8_t, 4, KIND_IP, POST_NEG, true, true);
-                else GEN(uint8_t, 4, KIND_COS, POST_ONE_MINUS, true, true);
-            } else {
-                if (plan.kind == KIND_L2) GEN(uint8_t, 4, KIND_L2, POST_ID, true, false);
-                else if (plan.kind == KIND_IP) GEN(uint8_t, 4, KIND_IP, POST_NEG, true, false);
-                else GEN(uint8_t, 4, KIND_COS, POST_ONE_MINUS, true, false);
-            }
-#undef GEN
-        }
+            auto kern = flat_generic_kernel<KernelRow<S>, S::NA, S::KIND, S::POST, S::IS_INT, S::SIGNED>;
+            DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            kern<<<grid, kFlatWarps * 32, smem, st>>>(d_q, nq, idx->d_vectors, idx->row_stride, r0, r1, dim, d_dist, rb);
+            return DAB_OK;
+        });
+        if (rc) return rc;
         DAB_LAUNCHED();
         DAB_CUDA(cudaGetLastError());
         const size_t tsmem = (size_t)kFlatWarps * 2 * k * 4;

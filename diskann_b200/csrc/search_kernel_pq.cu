@@ -447,8 +447,6 @@ __global__ void __launch_bounds__(kRerankWarps * 32) rerank_kernel(const RerankP
 
 static int launch_rerank(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t list_cap, const uint32_t* d_list,
                          const uint32_t* d_list_n, uint32_t* d_ids, float* d_dists, uint32_t* d_counts) {
-    const bool is_int = idx->dtype == DAB_I8 || idx->dtype == DAB_U8;
-    const MetricPlan plan = plan_for(idx->metric, is_int);
     RerankParams p;
     memset(&p, 0, sizeof(p));
     p.vectors = idx->d_vectors;
@@ -464,41 +462,23 @@ static int launch_rerank(dab_index* idx, const void* d_queries, uint32_t nq, uin
     p.out_ids = d_ids;
     p.out_dists = d_dists;
     p.out_counts = d_counts;
-    size_t off = is_int ? round_up((size_t)idx->dim, 16) : round_up((size_t)idx->dim * 4, 16);
-    p.off_ids = (uint32_t)off;
-    off += round_up((size_t)list_cap * 4, 16);
-    p.off_d = (uint32_t)off;
-    off += round_up((size_t)list_cap * 4, 16);
-    p.warp_smem = (uint32_t)off;
-    const size_t smem = off * kRerankWarps;
-    if (smem > 200 * 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "rerank: configuration needs %zu B shared memory per CTA", smem);
     const int grid = (int)std::min<uint64_t>(((uint64_t)nq + kRerankWarps - 1) / kRerankWarps, (uint64_t)idx->sm_count * 8);
-#define DAB_RERANK(TD, K_, P_, ...)                                                                          \
-    do {                                                                                                     \
-        auto kern = rerank_kernel<TD, K_, P_, ##__VA_ARGS__>;                                                \
-        DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));        \
-        kern<<<grid, kRerankWarps * 32, smem, idx->stream>>>(p);                                             \
-    } while (0)
-    if (idx->dtype == DAB_F32) {
-        if (plan.kind == KIND_L2) DAB_RERANK(float, KIND_L2, POST_ID);
-        else if (plan.kind == KIND_COS) DAB_RERANK(float, KIND_COS, POST_ONE_MINUS, 2);
-        else if (plan.post == POST_NEG) DAB_RERANK(float, KIND_IP, POST_NEG);
-        else DAB_RERANK(float, KIND_IP, POST_ONE_MINUS);
-    } else if (idx->dtype == DAB_F16) {
-        if (plan.kind == KIND_L2) DAB_RERANK(__half, KIND_L2, POST_ID, 2);
-        else if (plan.kind == KIND_COS) DAB_RERANK(__half, KIND_COS, POST_ONE_MINUS, 2);
-        else if (plan.post == POST_NEG) DAB_RERANK(__half, KIND_IP, POST_NEG, 2);
-        else DAB_RERANK(__half, KIND_IP, POST_ONE_MINUS, 2);
-    } else if (idx->dtype == DAB_I8) {
-        if (plan.kind == KIND_L2) DAB_RERANK(int8_t, KIND_L2, POST_ID);
-        else if (plan.kind == KIND_IP) DAB_RERANK(int8_t, KIND_IP, POST_NEG);
-        else DAB_RERANK(int8_t, KIND_COS, POST_ONE_MINUS);
-    } else {
-        if (plan.kind == KIND_L2) DAB_RERANK(uint8_t, KIND_L2, POST_ID);
-        else if (plan.kind == KIND_IP) DAB_RERANK(uint8_t, KIND_IP, POST_NEG);
-        else DAB_RERANK(uint8_t, KIND_COS, POST_ONE_MINUS);
-    }
-#undef DAB_RERANK
+    const int rc = visit_schema<OPS_ROW>(idx->dtype, idx->metric, [&](auto s) -> int {
+        using S = decltype(s);
+        size_t off = S::IS_INT ? round_up((size_t)idx->dim, 16) : round_up((size_t)idx->dim * 4, 16);
+        p.off_ids = (uint32_t)off;
+        off += round_up((size_t)list_cap * 4, 16);
+        p.off_d = (uint32_t)off;
+        off += round_up((size_t)list_cap * 4, 16);
+        p.warp_smem = (uint32_t)off;
+        const size_t smem = off * kRerankWarps;
+        if (smem > 200 * 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "rerank: configuration needs %zu B shared memory per CTA", smem);
+        auto kern = rerank_kernel<typename S::TD, S::KIND, S::POST, S::NA>;
+        DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kern<<<grid, kRerankWarps * 32, smem, idx->stream>>>(p);
+        return DAB_OK;
+    });
+    if (rc) return rc;
     DAB_LAUNCHED();
     DAB_CUDA(cudaGetLastError());
     return DAB_OK;

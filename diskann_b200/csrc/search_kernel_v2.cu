@@ -597,9 +597,9 @@ static void (*pick_v2(bool l1, bool reg))(const SearchParamsV2) {
     return l1 ? search_kernel_v2<TD, K, P, Q, true, false> : search_kernel_v2<TD, K, P, Q, false, false>;
 }
 
-int v2_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, bool level1, SearchParamsV2& p, V2Launch& out) {
-    const bool v2_int = idx->dtype == DAB_I8 || idx->dtype == DAB_U8;
-    const MetricPlan plan = plan_for(idx->metric, v2_int);
+// v2_prepare for the index's distance schema S (visit_schema)
+template <typename S>
+static int v2_prepare_schema(const dab_index* idx, uint32_t l_search, uint32_t beam, bool level1, SearchParamsV2& p, V2Launch& out) {
     const uint32_t cap = l_search + idx->n_start;
     const uint32_t row_bytes = (uint32_t)round_up((size_t)idx->dim * elem_size(idx->dtype), 16);
     auto too_big = [&] {
@@ -608,7 +608,7 @@ int v2_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, bool leve
     };
     size_t off = 0;
     p.off_q = (uint32_t)off;
-    off += v2_int ? round_up(round_up((size_t)idx->dim, 4), 16) : round_up((size_t)idx->dim * 4, 16);
+    off += S::IS_INT ? round_up(round_up((size_t)idx->dim, 4), 16) : round_up((size_t)idx->dim * 4, 16);
     const size_t ncand_max = (size_t)beam * idx->max_degree;
     p.off_cid = (uint32_t)off;
     off += round_up(std::max<size_t>(ncand_max, idx->n_start) * 4, 16);
@@ -629,9 +629,9 @@ int v2_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, bool leve
     // rows staged per round: as many as fit ~6 KB per warp, a multiple of the reduce group
     const size_t stage_bytes = 6144;
     const uint32_t stage = std::min<uint32_t>(32, (uint32_t)std::max<size_t>(kGroup, (stage_bytes / row_bytes) / kGroup * kGroup));
-    // QT = 0 where one register tile does not hold the list, for the float cosine schema, and for rows so wide that a
-    // stage of them does not fit: rows read straight from global memory, the global table alone
-    const bool any_len = cap > 256 || (plan.kind == KIND_COS && !v2_int) || round_up(off, 128) + (size_t)stage * row_bytes > 200 * 1024;
+    // QT = 0 where one register tile does not hold the list, for the float cosine schema (NA = 2), and for rows so wide
+    // that a stage of them does not fit: rows read straight from global memory, the global table alone
+    const bool any_len = cap > 256 || S::NA == 2 || round_up(off, 128) + (size_t)stage * row_bytes > 200 * 1024;
     // level-1 visited table: 4 KB of 16-bit tags per warp (2048 slots; the mean visited set of the headline
     // workload is ~1200 ids) when the ids fit 14-bit quotient tags, i.e. n_total <= 16384 * buckets
     size_t t1_bytes = idx->tune.test_visited_log2 ? 512 : 4096;  // tests: a level 1 that fills at once
@@ -675,34 +675,12 @@ int v2_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, bool leve
     out.smem_block = (size_t)p.warp_smem * kV2Warps;
     if (out.smem_block > 200 * 1024) return too_big();
 
-#define PICK2(TD, K, P, Q) out.kern = pick_v2<TD, K, P, Q>(p.t1_buckets != 0, reg)
-#define PICK_Q(TD, K, P)                                                      \
-    do {                                                                      \
-        if (any_len) out.kern = search_kernel_v2<TD, K, P, 0, false, false>; \
-        else if (cap <= 128) PICK2(TD, K, P, 4);                              \
-        else PICK2(TD, K, P, 8);                                              \
-    } while (0)
-#define PICK_T(TD)                                                                                              \
-    do {                                                                                                        \
-        if (plan.kind == KIND_L2) PICK_Q(TD, KIND_L2, POST_ID);                                                  \
-        else if (plan.kind == KIND_COS) out.kern = search_kernel_v2<TD, KIND_COS, POST_ONE_MINUS, 0, false, false>; \
-        else if (plan.post == POST_NEG) PICK_Q(TD, KIND_IP, POST_NEG);                                           \
-        else PICK_Q(TD, KIND_IP, POST_ONE_MINUS);                                                                \
-    } while (0)
-#define PICK_I(TD)                                                       \
-    do {                                                                 \
-        if (plan.kind == KIND_L2) PICK_Q(TD, KIND_L2, POST_ID);           \
-        else if (plan.kind == KIND_IP) PICK_Q(TD, KIND_IP, POST_NEG);     \
-        else PICK_Q(TD, KIND_COS, POST_ONE_MINUS);                        \
-    } while (0)
-    if (idx->dtype == DAB_F32) PICK_T(float);
-    else if (idx->dtype == DAB_F16) PICK_T(__half);
-    else if (idx->dtype == DAB_I8) PICK_I(int8_t);
-    else PICK_I(uint8_t);
-#undef PICK_I
-#undef PICK_T
-#undef PICK_Q
-#undef PICK2
+    using TD = typename S::TD;
+    const bool l1 = p.t1_buckets != 0;
+    // the float cosine schema (NA = 2) always runs with any_len: it has no tiled instantiations
+    if (any_len) out.kern = search_kernel_v2<TD, S::KIND, S::POST, 0, false, false>;
+    else if constexpr (S::NA == 4)
+        out.kern = cap <= 128 ? pick_v2<TD, S::KIND, S::POST, 4>(l1, reg) : pick_v2<TD, S::KIND, S::POST, 8>(l1, reg);
     int per_sm = 0;
     if (cudaFuncSetAttribute(out.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)out.smem_block) != cudaSuccess ||
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, out.kern, kV2Warps * 32, out.smem_block) != cudaSuccess || per_sm < 1) {
@@ -711,6 +689,12 @@ int v2_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, bool leve
     }
     out.grid = per_sm * idx->sm_count;
     return 0;
+}
+
+int v2_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, bool level1, SearchParamsV2& p, V2Launch& out) {
+    return visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto s) {
+        return v2_prepare_schema<decltype(s)>(idx, l_search, beam, level1, p, out);
+    });
 }
 
 }  // namespace dab

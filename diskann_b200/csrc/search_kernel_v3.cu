@@ -296,14 +296,14 @@ __global__ void __launch_bounds__(kV3Warps * 32, kV3MinCtas) search_kernel_v3(co
 }
 
 // ------------------------------------------------------------------ host side
-int v3_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, uint32_t visited_need, SearchParamsV3& p, V3Launch& out) {
+// v3_prepare for the index's distance schema S (visit_schema)
+template <typename S>
+static int v3_prepare_schema(const dab_index* idx, uint32_t l_search, uint32_t beam, uint32_t visited_need, SearchParamsV3& p,
+                             V3Launch& out) {
     // v3 is for short candidate lists (L + start points <= 24), whose visited sets are small.  At the headline L = 100
     // its whole-set tag table (~11.5 KB per warp) leaves 16 warps per SM, while v2's 4 KB level 1 with the global
     // table behind it leaves 28 (f32 rows in registers) or 20 (staged rows), so v2 is faster there
     if (l_search + idx->n_start > 24) return 1;
-    const bool is_int = idx->dtype == DAB_I8 || idx->dtype == DAB_U8;
-    const MetricPlan plan = plan_for(idx->metric, is_int);
-    if (plan.kind == KIND_COS && !is_int) return 1;  // float cosine: NA = 2 schema, search_kernel_v2
     const uint32_t cap = l_search + idx->n_start;
     if (idx->max_degree > 1000) return 1;
     if ((idx->row_stride & 15) != 0) return 1;
@@ -315,7 +315,7 @@ int v3_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, uint32_t 
 
     size_t off = 0;
     p.off_q = (uint32_t)off;
-    off += is_int ? round_up((size_t)idx->dim, 16) : round_up((size_t)idx->dim * 4, 16);
+    off += S::IS_INT ? round_up((size_t)idx->dim, 16) : round_up((size_t)idx->dim * 4, 16);
     const size_t ncand_max = std::max<size_t>((size_t)beam * idx->max_degree, std::min<uint32_t>(32, idx->n_start));
     p.off_cid = (uint32_t)off;
     off += round_up(ncand_max * 4, 16);
@@ -362,36 +362,11 @@ int v3_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, uint32_t 
     p.warp_smem = (uint32_t)round_up(fixed + (size_t)tbytes, 128);
     out.smem_block = (size_t)p.warp_smem * kV3Warps;
 
-#define PICK2(TD, K_, P_, Q_)                                                              \
-    do {                                                                                   \
-        if (std::is_same<TD, float>::value && p.fast_nm) out.kern = search_kernel_v3<float, K_, P_, Q_, true>; \
-        else out.kern = search_kernel_v3<TD, K_, P_, Q_, false>;                            \
-    } while (0)
-#define PICK_Q(TD, K_, P_)                 \
-    do {                                   \
-        if (cap <= 128) PICK2(TD, K_, P_, 4); \
-        else PICK2(TD, K_, P_, 8);         \
-    } while (0)
-#define PICK_T(TD)                                                       \
-    do {                                                                 \
-        if (plan.kind == KIND_L2) PICK_Q(TD, KIND_L2, POST_ID);           \
-        else if (plan.post == POST_NEG) PICK_Q(TD, KIND_IP, POST_NEG);    \
-        else PICK_Q(TD, KIND_IP, POST_ONE_MINUS);                         \
-    } while (0)
-#define PICK_I(TD)                                                       \
-    do {                                                                 \
-        if (plan.kind == KIND_L2) PICK_Q(TD, KIND_L2, POST_ID);           \
-        else if (plan.kind == KIND_IP) PICK_Q(TD, KIND_IP, POST_NEG);     \
-        else PICK_Q(TD, KIND_COS, POST_ONE_MINUS);                        \
-    } while (0)
-    if (idx->dtype == DAB_F32) PICK_T(float);
-    else if (idx->dtype == DAB_F16) PICK_T(__half);
-    else if (idx->dtype == DAB_I8) PICK_I(int8_t);
-    else PICK_I(uint8_t);
-#undef PICK_I
-#undef PICK_T
-#undef PICK_Q
-#undef PICK2
+    using TD = typename S::TD;
+    out.kern = cap <= 128 ? search_kernel_v3<TD, S::KIND, S::POST, 4, false> : search_kernel_v3<TD, S::KIND, S::POST, 8, false>;
+    if constexpr (std::is_same<TD, float>::value) {
+        if (p.fast_nm) out.kern = cap <= 128 ? search_kernel_v3<TD, S::KIND, S::POST, 4, true> : search_kernel_v3<TD, S::KIND, S::POST, 8, true>;
+    }
     if (cudaFuncSetAttribute(out.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)out.smem_block) != cudaSuccess) {
         cudaGetLastError();
         return 1;
@@ -403,6 +378,14 @@ int v3_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, uint32_t 
     }
     out.grid = per_sm * idx->sm_count;
     return 0;
+}
+
+int v3_prepare(const dab_index* idx, uint32_t l_search, uint32_t beam, uint32_t visited_need, SearchParamsV3& p, V3Launch& out) {
+    return visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto s) -> int {
+        using S = decltype(s);
+        if constexpr (S::NA == 2) return 1;  // float cosine: the two-accumulator schema, search_kernel_v2
+        else return v3_prepare_schema<S>(idx, l_search, beam, visited_need, p, out);
+    });
 }
 
 }  // namespace dab
