@@ -60,6 +60,13 @@ SYMBOLS = {
     "dab_minmax_compress": (_i, [_i, _f, _u32, _i, _vp, _u64, _vp, _vp]),
     "dab_minmax_distances": (_i, [_i, _i, _i, _i, _u32, _vp, _vp, _u64, _vp]),
     "dab_minmax_query_distances": (_i, [_i, _i, _i, _u32, _vp, _u32, _vp, _u64, _vp]),
+    "dab_transform_create": (_i, [C.POINTER(_vp), _i, _u32, _u32, _vp, _vp, _vp, _u32]),
+    "dab_transform_destroy": (None, [_vp]),
+    "dab_transform_input_dim": (_u32, [_vp]),
+    "dab_transform_output_dim": (_u32, [_vp]),
+    "dab_transform_apply": (_i, [_vp, _i, _vp, _u64, _vp]),
+    "dab_minmax_compress_transformed": (_i, [_vp, _i, _f, _i, _vp, _u64, _vp, _vp]),
+    "dab_minmax_query_distances_transformed": (_i, [_vp, _i, _i, _i, _vp, _u32, _vp, _u64, _vp]),
     "dab_robust_prune": (_i, [_vp, _vp, _vp, _vp, _vp, _u32, _u32, _u32, _f, _vp, _vp]),
     "dab_build": (_i, [_vp, _u32, _u32, _f, _u32]),
     "dab_flat_knn": (_i, [_vp, _vp, _u32, _u32, _vp, _vp]),

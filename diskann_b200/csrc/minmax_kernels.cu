@@ -10,11 +10,14 @@
 //   * MinMax{IP, L2Squared, Cosine, CosineNormalized} over two Data rows (vectors.rs:206-455): an exact integer inner
 //     product of the codes (bits/distances.rs; dp4a on masked fields, popc for one bit) and a five-term f32 epilogue
 //     in the reference's association.  Eight lanes per pair, 4-byte loads of the dense codes.
+// The quantizer runs on Transform::Null input, or behind a Hadamard transform (transform_kernels.cu writes the
+// transformed rows into device memory and these kernels run on them unchanged, dim = the transform's output dim).
 // Row layout = the reference's canonical-front Data<NBITS> (meta/vector.rs:377-392): MinMaxCompensation {dim u32, b, n, a,
 // norm_squared} (vectors.rs:43-52, 20 bytes) then ceil(dim * NBITS / 8) bytes of codes, value i at bit i * NBITS.
 // HBM-bound byte work: no tensor cores.
 #include "dab_common.cuh"
 #include "quant_device.cuh"
+#include "transform.cuh"
 
 #include <algorithm>
 
@@ -378,6 +381,56 @@ using namespace dab;
 
 static bool mm_bits_ok(int nbits) { return nbits == 1 || nbits == 2 || nbits == 4 || nbits == 8; }
 
+// MinMaxCompressParams for dim-long vectors and the CTA shape of minmax_compress_kernel; false if the staging buffers
+// of one warp do not fit shared memory
+static bool mm_compress_setup(float grid_scale, uint32_t dim, int nbits, uint64_t n, MinMaxCompressParams& p, int& warps, size_t& smem) {
+    memset(&p, 0, sizeof(p));
+    p.grid_scale = grid_scale;
+    p.dim = dim;
+    p.nbits = nbits;
+    p.n = n;
+    p.row_bytes = kMmMeta + (uint32_t)(((uint64_t)dim * nbits + 7) / 8);
+    uint32_t words = (p.row_bytes + 3) / 4;
+    if ((words & 1u) == 0) ++words;
+    p.srow_stride = words * 4;
+    p.warp_smem = 32 * 33 * 4 + 32 * p.srow_stride;
+    warps = 4;
+    while (warps > 1 && (size_t)warps * p.warp_smem > 200 * 1024) warps >>= 1;
+    smem = (size_t)warps * p.warp_smem;
+    return smem <= 200 * 1024;
+}
+
+// p.vectors, p.rows, p.loss and p.first_nan are device pointers
+static cudaError_t mm_compress_launch(const MinMaxCompressParams& p, int warps, size_t smem) {
+    cudaError_t e = cudaFuncSetAttribute(minmax_compress_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess) {
+        const uint64_t groups = (p.n + 31) / 32;
+        const int grid = (int)std::min<uint64_t>((groups + warps - 1) / warps, 132ull * 8);
+        minmax_compress_kernel<<<grid, warps * 32, smem>>>(p);
+        DAB_LAUNCHED();
+        e = cudaGetLastError();
+    }
+    return e;
+}
+
+// the FullQueryMeta kernel, then the distance kernel for p.nbits (p's pointers are device pointers)
+static cudaError_t mm_query_launch(const MinMaxQueryParams& p) {
+    minmax_query_meta_kernel<<<(p.nq + 127) / 128, 128>>>(p);
+    DAB_LAUNCHED();
+    const uint32_t lpp = p.nbits == 8 ? 1 : 8;
+    const uint64_t pairs_per_cta = 256 / lpp;
+    const dim3 grid((unsigned)std::min<uint64_t>((p.n + pairs_per_cta - 1) / pairs_per_cta, 132ull * 8), p.nq);
+    const size_t smem = (size_t)p.dim * 4;
+    switch (p.nbits) {
+        case 8: minmax_query_distance_kernel<8><<<grid, 256, smem>>>(p); break;
+        case 4: minmax_query_distance_kernel<4><<<grid, 256, smem>>>(p); break;
+        case 2: minmax_query_distance_kernel<2><<<grid, 256, smem>>>(p); break;
+        default: minmax_query_distance_kernel<1><<<grid, 256, smem>>>(p); break;
+    }
+    DAB_LAUNCHED();
+    return cudaGetLastError();
+}
+
 extern "C" {
 
 uint32_t dab_minmax_row_bytes(uint32_t dim, int nbits) { return mm_bits_ok(nbits) ? kMmMeta + (uint32_t)(((uint64_t)dim * nbits + 7) / 8) : 0; }
@@ -392,20 +445,10 @@ int dab_minmax_compress(int device, float grid_scale, uint32_t dim, int nbits, c
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(DAB_ERR_NO_DEVICE, "dab_minmax_compress: no CUDA device visible");
     DAB_CUDA(cudaSetDevice(device));
     MinMaxCompressParams p;
-    memset(&p, 0, sizeof(p));
-    p.grid_scale = grid_scale;
-    p.dim = dim;
-    p.nbits = nbits;
-    p.n = n;
-    p.row_bytes = dab_minmax_row_bytes(dim, nbits);
-    uint32_t words = (p.row_bytes + 3) / 4;
-    if ((words & 1u) == 0) ++words;
-    p.srow_stride = words * 4;
-    p.warp_smem = 32 * 33 * 4 + 32 * p.srow_stride;
-    int warps = 4;
-    while (warps > 1 && (size_t)warps * p.warp_smem > 200 * 1024) warps >>= 1;
-    const size_t smem = (size_t)warps * p.warp_smem;
-    if (smem > 200 * 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_minmax_compress: rows of %u bytes do not fit the staging buffers", p.row_bytes);
+    int warps;
+    size_t smem;
+    if (!mm_compress_setup(grid_scale, dim, nbits, n, p, warps, smem))
+        return fail(DAB_ERR_INVALID_ARGUMENT, "dab_minmax_compress: rows of %u bytes do not fit the staging buffers", p.row_bytes);
     float *d_vec = nullptr, *d_loss = nullptr;
     uint8_t* d_rows = nullptr;
     unsigned long long* d_nan = nullptr;
@@ -421,14 +464,7 @@ int dab_minmax_compress(int device, float grid_scale, uint32_t dim, int nbits, c
         p.rows = d_rows;
         p.loss = d_loss;
         p.first_nan = d_nan;
-        e = cudaFuncSetAttribute(minmax_compress_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e == cudaSuccess) {
-            const uint64_t groups = (n + 31) / 32;
-            const int grid = (int)std::min<uint64_t>((groups + warps - 1) / warps, 132ull * 8);
-            minmax_compress_kernel<<<grid, warps * 32, smem>>>(p);
-            DAB_LAUNCHED();
-            e = cudaGetLastError();
-        }
+        e = mm_compress_launch(p, warps, smem);
     }
     if (e == cudaSuccess) e = cudaMemcpy(out_rows, d_rows, n * p.row_bytes, cudaMemcpyDeviceToHost);
     if (e == cudaSuccess && out_loss) e = cudaMemcpy(out_loss, d_loss, n * 4, cudaMemcpyDeviceToHost);
@@ -525,26 +561,126 @@ int dab_minmax_query_distances(int device, int metric, int nbits, uint32_t dim, 
         p.meta = dmeta;
         p.out = dout;
         p.first_nan = d_nan;
-        minmax_query_meta_kernel<<<(nq + 127) / 128, 128>>>(p);
-        DAB_LAUNCHED();
-        const uint32_t lpp = nbits == 8 ? 1 : 8;
-        const uint64_t pairs_per_cta = 256 / lpp;
-        const dim3 grid((unsigned)std::min<uint64_t>((n + pairs_per_cta - 1) / pairs_per_cta, 132ull * 8), nq);
-        const size_t smem = (size_t)dim * 4;
-        switch (nbits) {
-            case 8: minmax_query_distance_kernel<8><<<grid, 256, smem>>>(p); break;
-            case 4: minmax_query_distance_kernel<4><<<grid, 256, smem>>>(p); break;
-            case 2: minmax_query_distance_kernel<2><<<grid, 256, smem>>>(p); break;
-            default: minmax_query_distance_kernel<1><<<grid, 256, smem>>>(p); break;
-        }
-        DAB_LAUNCHED();
-        e = cudaGetLastError();
+        e = mm_query_launch(p);
     }
     if (e == cudaSuccess) e = cudaMemcpy(&first_nan, d_nan, 8, cudaMemcpyDeviceToHost);
     if (e == cudaSuccess && first_nan == ~0ull) e = cudaMemcpy(out, dout, (size_t)nq * n * 4, cudaMemcpyDeviceToHost);
     int rc = DAB_OK;
     if (e != cudaSuccess) rc = fail(e == cudaErrorMemoryAllocation ? DAB_ERR_OUT_OF_MEMORY : DAB_ERR_CUDA, "dab_minmax_query_distances: %s", cudaGetErrorString(e));
     else if (first_nan != ~0ull) rc = fail(DAB_ERR_INVALID_ARGUMENT, "dab_minmax_query_distances: query %llu contains NaN (InputContainsNaN)", first_nan);
+    cudaFree(dq);
+    cudaFree(drows);
+    cudaFree(dmeta);
+    cudaFree(dout);
+    cudaFree(d_nan);
+    return rc;
+}
+
+// ---------------------------------------------------------------- behind a Hadamard transform (transform_kernels.cu)
+
+int dab_minmax_compress_transformed(const dab_transform* t, int device, float grid_scale, int nbits, const float* vectors, uint64_t n,
+                                    uint8_t* out_rows, float* out_loss) {
+    static const char* who = "dab_minmax_compress_transformed";
+    if (!t) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL transform", who);
+    if (!mm_bits_ok(nbits)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: nbits must be 1, 2, 4 or 8", who);
+    if (!(grid_scale > 0.0f)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: grid_scale must be positive (num::Positive)", who);
+    if (n == 0) return DAB_OK;
+    if ((!vectors && t->input_dim) || !out_rows) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", who);
+    const uint32_t dim = t->output_dim;
+    MinMaxCompressParams p;
+    int warps;
+    size_t smem;
+    if (!mm_compress_setup(grid_scale, dim, nbits, n, p, warps, smem))
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: rows of %u bytes do not fit the staging buffers", who, p.row_bytes);
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(DAB_ERR_NO_DEVICE, "%s: no CUDA device visible", who);
+    DAB_CUDA(cudaSetDevice(device));
+    float *d_in = nullptr, *d_vec = nullptr, *d_loss = nullptr;
+    uint8_t* d_rows = nullptr;
+    unsigned long long* d_nan = nullptr;
+    cudaError_t e = cudaMalloc(&d_in, std::max<uint64_t>(1, n * t->input_dim) * 4);
+    if (e == cudaSuccess) e = cudaMalloc(&d_vec, n * dim * 4);
+    if (e == cudaSuccess) e = cudaMalloc(&d_rows, n * p.row_bytes);
+    if (e == cudaSuccess) e = cudaMalloc(&d_loss, n * 4);
+    if (e == cudaSuccess) e = cudaMalloc(&d_nan, 8);
+    if (e == cudaSuccess && t->input_dim) e = cudaMemcpy(d_in, vectors, n * t->input_dim * 4, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemset(d_nan, 0xFF, 8);
+    if (e == cudaSuccess) e = transform_rows(t, d_in, n, d_vec, nullptr);
+    unsigned long long first_nan = ~0ull;
+    if (e == cudaSuccess) {
+        // quantizer.rs:171-228: the quantizer runs on the transformed vector, and so does its NaN check
+        p.vectors = d_vec;
+        p.rows = d_rows;
+        p.loss = d_loss;
+        p.first_nan = d_nan;
+        e = mm_compress_launch(p, warps, smem);
+    }
+    if (e == cudaSuccess) e = cudaMemcpy(out_rows, d_rows, n * p.row_bytes, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && out_loss) e = cudaMemcpy(out_loss, d_loss, n * 4, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess) e = cudaMemcpy(&first_nan, d_nan, 8, cudaMemcpyDeviceToHost);
+    int rc = DAB_OK;
+    if (e != cudaSuccess) rc = fail(e == cudaErrorMemoryAllocation ? DAB_ERR_OUT_OF_MEMORY : DAB_ERR_CUDA, "%s: %s", who, cudaGetErrorString(e));
+    else if (first_nan != ~0ull)
+        rc = fail(DAB_ERR_INVALID_ARGUMENT, "%s: vector %llu contains NaN after the transform (InputContainsNaN); its row was written all the same", who,
+                  first_nan);
+    cudaFree(d_in);
+    cudaFree(d_vec);
+    cudaFree(d_rows);
+    cudaFree(d_loss);
+    cudaFree(d_nan);
+    return rc;
+}
+
+int dab_minmax_query_distances_transformed(const dab_transform* t, int device, int metric, int nbits, const float* queries, uint32_t nq,
+                                           const uint8_t* rows, uint64_t n, float* out) {
+    static const char* who = "dab_minmax_query_distances_transformed";
+    if (!t) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL transform", who);
+    if (!mm_bits_ok(nbits)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: nbits must be 1, 2, 4 or 8", who);
+    if (metric < DAB_COSINE || metric > DAB_COSINE_NORMALIZED) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: unknown metric %d", who, metric);
+    if (nq == 0 || n == 0) return DAB_OK;
+    if ((!queries && t->input_dim) || !rows || !out) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", who);
+    const uint32_t dim = t->output_dim;
+    if ((size_t)dim * 4 > 48 * 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: output dim %u too large", who, dim);
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(DAB_ERR_NO_DEVICE, "%s: no CUDA device visible", who);
+    DAB_CUDA(cudaSetDevice(device));
+    MinMaxQueryParams p;
+    memset(&p, 0, sizeof(p));
+    p.metric = metric;
+    p.nbits = nbits;
+    p.dim = dim;
+    p.nq = nq;
+    p.row_bytes = dab_minmax_row_bytes(dim, nbits);
+    p.n = n;
+    float *dq_in = nullptr, *dq = nullptr, *dmeta = nullptr, *dout = nullptr;
+    uint8_t* drows = nullptr;
+    unsigned long long* d_nan = nullptr;  // [0]: NaN in an untransformed query, [1]: the meta kernel's flag (not read)
+    cudaError_t e = cudaMalloc(&dq_in, std::max<uint64_t>(1, (uint64_t)nq * t->input_dim) * 4);
+    if (e == cudaSuccess) e = cudaMalloc(&dq, (size_t)nq * dim * 4);
+    if (e == cudaSuccess) e = cudaMalloc(&drows, n * p.row_bytes);
+    if (e == cudaSuccess) e = cudaMalloc(&dmeta, (size_t)nq * 8);
+    if (e == cudaSuccess) e = cudaMalloc(&dout, (size_t)nq * n * 4);
+    if (e == cudaSuccess) e = cudaMalloc(&d_nan, 16);
+    if (e == cudaSuccess && t->input_dim) e = cudaMemcpy(dq_in, queries, (size_t)nq * t->input_dim * 4, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(drows, rows, n * p.row_bytes, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemset(d_nan, 0xFF, 16);
+    // quantizer.rs:398-401: the NaN check is on the input; the transformed query may hold NaN (inf - inf) and is used as is
+    if (e == cudaSuccess) e = transform_rows(t, dq_in, nq, dq, d_nan);
+    unsigned long long first_nan = ~0ull;
+    if (e == cudaSuccess) {
+        p.queries = dq;
+        p.rows = drows;
+        p.meta = dmeta;
+        p.out = dout;
+        p.first_nan = d_nan + 1;
+        e = mm_query_launch(p);
+    }
+    if (e == cudaSuccess) e = cudaMemcpy(&first_nan, d_nan, 8, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && first_nan == ~0ull) e = cudaMemcpy(out, dout, (size_t)nq * n * 4, cudaMemcpyDeviceToHost);
+    int rc = DAB_OK;
+    if (e != cudaSuccess) rc = fail(e == cudaErrorMemoryAllocation ? DAB_ERR_OUT_OF_MEMORY : DAB_ERR_CUDA, "%s: %s", who, cudaGetErrorString(e));
+    else if (first_nan != ~0ull) rc = fail(DAB_ERR_INVALID_ARGUMENT, "%s: query %llu contains NaN (InputContainsNaN)", who, first_nan);
+    cudaFree(dq_in);
     cudaFree(dq);
     cudaFree(drows);
     cudaFree(dmeta);

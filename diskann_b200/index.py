@@ -79,17 +79,139 @@ def distance_comparer(metric, dim=None, device=0):
     return call
 
 
-def minmax_compress(vectors, nbits, grid_scale=1.0, device=0):
-    """MinMaxQuantizer (Transform::Null) over the rows of `vectors` [n, dim] f32: (rows u8 [n, 20 + ceil(dim * nbits / 8)]
-    in the reference's canonical-front Data<NBITS> layout, loss f32 [n]).  Raises DabError when a vector contains NaN."""
+def _splitmix64(seed):
+    state = seed & 0xFFFFFFFFFFFFFFFF
+    while True:
+        state = (state + 0x9E3779B97F4A7C15) & 0xFFFFFFFFFFFFFFFF
+        z = state
+        z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & 0xFFFFFFFFFFFFFFFF
+        z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & 0xFFFFFFFFFFFFFFFF
+        yield z ^ (z >> 31)
+
+
+class Transform:
+    """A Hadamard transform in front of the MinMax quantizer: Transform::PaddingHadamard / Transform::DoubleHadamard of
+    diskann-quantization/src/algorithms/transforms, held by the library as a host-side object (dab_transform).
+
+    Build one from the reference's serialized parts (signs as bools, the inner dimension, optional sorted subsample
+    indices) with the constructor, or draw a new one with `padding_hadamard` / `double_hadamard`, which apply the
+    reference's TargetDim rules exactly.  The random draws there come from SplitMix64(seed), not Rust's StdRng: a
+    transform drawn here has the reference's shape but not the signs a reference run with the same seed would draw."""
+
+    PADDING_HADAMARD = 1
+    DOUBLE_HADAMARD = 2
+
+    def __init__(self, kind, signs0, inner_dim, signs1=None, subsample=None):
+        self._h = C.c_void_p()
+        signs0 = np.ascontiguousarray(signs0, np.uint8)
+        signs1 = None if signs1 is None else np.ascontiguousarray(signs1, np.uint8)
+        subsample = None if subsample is None else np.ascontiguousarray(subsample, np.uint32)
+        n_sub = 0 if subsample is None else len(subsample)
+        if subsample is not None and n_sub == 0:
+            subsample = np.zeros(1, np.uint32)  # present but empty: a non-NULL pointer with no entries
+        check(_lib.lib().dab_transform_create(C.byref(self._h), int(kind), len(signs0), int(inner_dim), _ptr(signs0), _ptr(signs1),
+                                              _ptr(subsample), n_sub))
+        self.kind = int(kind)
+        self.signs0, self.signs1, self.inner_dim = signs0, signs1, int(inner_dim)
+        self.subsample = None if subsample is None else subsample[:n_sub]
+
+    @staticmethod
+    def _target(target):
+        """TargetDim: "same", "natural" or an int (Override)."""
+        if target in ("same", "natural"):
+            return target
+        if int(target) < 1:
+            raise DabError(1, f"target dim must be positive, got {target}")
+        return int(target)
+
+    @staticmethod
+    def _subsample(rng, length, amount):
+        """`amount` distinct sorted indices of range(length) (subsample_indices, transforms/utils.rs:60-78), by a partial
+        Fisher-Yates shuffle."""
+        idx = np.arange(length, dtype=np.uint32)
+        for i in range(amount):
+            j = i + next(rng) % (length - i)
+            idx[i], idx[j] = idx[j], idx[i]
+        return np.sort(idx[:amount])
+
+    @classmethod
+    def padding_hadamard(cls, dim, target="same", seed=0):
+        """PaddingHadamard::new (padding_hadamard.rs:94-133): Same -> (padded, output) = (next_pow2(dim), dim), Natural ->
+        (next_pow2(dim), next_pow2(dim)), Override(t) -> (next_pow2(max(t, dim)), t); subsampled when padded > output."""
+        target = cls._target(target)
+        pow2 = lambda v: 1 << (int(v) - 1).bit_length()  # noqa: E731
+        if target == "same":
+            padded, out = pow2(dim), dim
+        elif target == "natural":
+            padded = out = pow2(dim)
+        else:
+            padded, out = pow2(max(target, dim)), target
+        rng = _splitmix64(seed)
+        signs = np.array([next(rng) >> 63 for _ in range(dim)], np.uint8)
+        sub = cls._subsample(rng, padded, out) if padded > out else None
+        return cls(cls.PADDING_HADAMARD, signs, padded, subsample=sub)
+
+    @classmethod
+    def double_hadamard(cls, dim, target="same", seed=0):
+        """DoubleHadamard::new (double_hadamard.rs:98-144): output = dim for Same and Natural, t for Override(t);
+        intermediate = max(dim, output) (len(signs1)); subsampled when dim > output."""
+        target = cls._target(target)
+        out = dim if target in ("same", "natural") else target
+        inter = max(dim, out)
+        rng = _splitmix64(seed)
+        signs0 = np.array([next(rng) >> 63 for _ in range(dim)], np.uint8)
+        signs1 = np.array([next(rng) >> 63 for _ in range(inter)], np.uint8)
+        sub = cls._subsample(rng, dim, out) if dim > out else None
+        return cls(cls.DOUBLE_HADAMARD, signs0, inter, signs1=signs1, subsample=sub)
+
+    @property
+    def input_dim(self):
+        return int(_lib.lib().dab_transform_input_dim(self._h))
+
+    @property
+    def output_dim(self):
+        return int(_lib.lib().dab_transform_output_dim(self._h))
+
+    @property
+    def preserves_norms(self):
+        return self.subsample is None
+
+    def apply(self, vectors, device=0):
+        """transform_into for the rows of `vectors` [n, input_dim] f32 -> [n, output_dim] f32 (on the device)."""
+        vectors = np.ascontiguousarray(vectors, np.float32)
+        if vectors.ndim != 2 or vectors.shape[1] != self.input_dim:
+            raise DabError(1, f"Transform.apply: vectors must be [n, {self.input_dim}] f32, got {vectors.shape}")
+        out = np.empty((vectors.shape[0], self.output_dim), np.float32)
+        check(_lib.lib().dab_transform_apply(self._h, device, _ptr(vectors), vectors.shape[0], _ptr(out)))
+        return out
+
+    def close(self):
+        if getattr(self, "_h", None) is not None and self._h.value:
+            _lib.lib().dab_transform_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        self.close()
+
+
+def minmax_compress(vectors, nbits, grid_scale=1.0, device=0, transform=None):
+    """MinMaxQuantizer over the rows of `vectors` [n, dim] f32: (rows u8 [n, 20 + ceil(out_dim * nbits / 8)] in the
+    reference's canonical-front Data<NBITS> layout, loss f32 [n]).  transform=None is Transform::Null (out_dim = dim);
+    a `Transform` runs first (out_dim = its output_dim).  Raises DabError when a (transformed) vector contains NaN."""
     vectors = np.ascontiguousarray(vectors, np.float32)
     if vectors.ndim != 2:
         raise DabError(1, "minmax_compress: vectors must be [n, dim] f32")
     n, dim = vectors.shape
-    rb = _lib.lib().dab_minmax_row_bytes(dim, nbits)
+    if transform is not None and dim != transform.input_dim:
+        raise DabError(1, f"minmax_compress: vectors have {dim} values, the transform takes {transform.input_dim}")
+    out_dim = dim if transform is None else transform.output_dim
+    rb = _lib.lib().dab_minmax_row_bytes(out_dim, nbits)
     rows = np.zeros((n, rb), np.uint8)
     loss = np.zeros(n, np.float32)
-    check(_lib.lib().dab_minmax_compress(device, grid_scale, dim, nbits, _ptr(vectors), n, _ptr(rows), _ptr(loss)))
+    if transform is None:
+        check(_lib.lib().dab_minmax_compress(device, grid_scale, dim, nbits, _ptr(vectors), n, _ptr(rows), _ptr(loss)))
+    else:
+        check(_lib.lib().dab_minmax_compress_transformed(transform._h, device, grid_scale, nbits, _ptr(vectors), n, _ptr(rows), _ptr(loss)))
     return rows, loss
 
 
@@ -103,14 +225,21 @@ def minmax_distances(metric, nbits_x, nbits_y, dim, x_rows, y_rows, device=0):
     return out
 
 
-def minmax_query_distances(metric, nbits, queries, rows, device=0):
+def minmax_query_distances(metric, nbits, queries, rows, device=0, transform=None):
     """Full-precision queries [nq, dim] f32 against MinMax-compressed rows [n, row_bytes]: out [nq, n]
-    (MinMax{L2Squared, IP, Cosine, CosineNormalized}::evaluate(FullQueryRef, DataRef<NBITS>))."""
+    (MinMax{L2Squared, IP, Cosine, CosineNormalized}::evaluate(FullQueryRef, DataRef<NBITS>)).  With a `Transform` the
+    queries are checked for NaN, then transformed, and the rows must have been compressed behind the same transform."""
     queries = np.ascontiguousarray(queries, np.float32)
     rows = np.ascontiguousarray(rows, np.uint8)
     nq, dim = queries.shape
     out = np.empty((nq, rows.shape[0]), np.float32)
-    check(_lib.lib().dab_minmax_query_distances(device, int(metric), nbits, dim, _ptr(queries), nq, _ptr(rows), rows.shape[0], _ptr(out)))
+    if transform is None:
+        check(_lib.lib().dab_minmax_query_distances(device, int(metric), nbits, dim, _ptr(queries), nq, _ptr(rows), rows.shape[0], _ptr(out)))
+    else:
+        if dim != transform.input_dim:
+            raise DabError(1, f"minmax_query_distances: queries have {dim} values, the transform takes {transform.input_dim}")
+        check(_lib.lib().dab_minmax_query_distances_transformed(transform._h, device, int(metric), nbits, _ptr(queries), nq, _ptr(rows),
+                                                                 rows.shape[0], _ptr(out)))
     return out
 
 

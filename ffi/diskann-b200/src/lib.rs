@@ -233,3 +233,93 @@ pub fn minmax_query_distances(device: i32, metric: Metric, nbits: i32, dim: usiz
     })?;
     Ok(out)
 }
+
+/// `Transform::PaddingHadamard` / `Transform::DoubleHadamard` (diskann-quantization/src/algorithms/transforms) from the
+/// parts the reference serializes (`try_from_parts`); signs are the flatbuffer's bools.  A host-side object: only
+/// `apply` and the MinMax calls below touch the device.
+pub struct Transform {
+    raw: *mut sys::dab_transform,
+}
+
+// immutable after creation: every call takes it by const pointer
+unsafe impl Send for Transform {}
+unsafe impl Sync for Transform {}
+
+impl Transform {
+    fn create(kind: i32, signs0: &[bool], inner_dim: usize, signs1: Option<&[bool]>, subsample: Option<&[u32]>) -> Result<Self> {
+        let s0: Vec<u8> = signs0.iter().map(|&b| b as u8).collect();
+        let s1: Option<Vec<u8>> = signs1.map(|s| s.iter().map(|&b| b as u8).collect());
+        let mut raw = ptr::null_mut();
+        check(unsafe {
+            sys::dab_transform_create(
+                &mut raw,
+                kind,
+                s0.len() as u32,
+                inner_dim as u32,
+                s0.as_ptr(),
+                s1.as_ref().map_or(ptr::null(), |s| s.as_ptr()),
+                // `Some(&[])` must stay distinguishable from `None` (SubsampleEmpty): a dangling non-null pointer
+                subsample.map_or(ptr::null(), |s| s.as_ptr()),
+                subsample.map_or(0, |s| s.len() as u32),
+            )
+        })?;
+        Ok(Self { raw })
+    }
+
+    /// `PaddingHadamard::try_from_parts(signs, padded_dim, subsample)` (padding_hadamard.rs:137-173).
+    pub fn padding_hadamard(signs: &[bool], padded_dim: usize, subsample: Option<&[u32]>) -> Result<Self> {
+        Self::create(sys::DAB_TRANSFORM_PADDING_HADAMARD, signs, padded_dim, None, subsample)
+    }
+
+    /// `DoubleHadamard::try_from_parts(signs0, signs1, subsample)` (double_hadamard.rs:146-206).
+    pub fn double_hadamard(signs0: &[bool], signs1: &[bool], subsample: Option<&[u32]>) -> Result<Self> {
+        Self::create(sys::DAB_TRANSFORM_DOUBLE_HADAMARD, signs0, signs1.len(), Some(signs1), subsample)
+    }
+
+    pub fn input_dim(&self) -> usize {
+        unsafe { sys::dab_transform_input_dim(self.raw) as usize }
+    }
+
+    pub fn output_dim(&self) -> usize {
+        unsafe { sys::dab_transform_output_dim(self.raw) as usize }
+    }
+
+    /// `transform_into` for `src.len() / input_dim` rows, on the device: `[n][output_dim]`.
+    pub fn apply(&self, device: i32, src: &[f32]) -> Result<Vec<f32>> {
+        let n = src.len() / self.input_dim().max(1);
+        let mut out = vec![0f32; n * self.output_dim()];
+        check(unsafe { sys::dab_transform_apply(self.raw, device, src.as_ptr(), n as u64, out.as_mut_ptr()) })?;
+        Ok(out)
+    }
+}
+
+impl Drop for Transform {
+    fn drop(&mut self) {
+        unsafe { sys::dab_transform_destroy(self.raw) }
+    }
+}
+
+/// `MinMaxQuantizer::new(transform, grid_scale)` + `compress_into`: rows of `output_dim` codes, `Err` when a
+/// transformed vector holds NaN (`InputContainsNaN`).
+pub fn minmax_compress_transformed(transform: &Transform, device: i32, grid_scale: f32, nbits: i32, vectors: &[f32]) -> Result<(Vec<u8>, Vec<f32>)> {
+    let n = vectors.len() / transform.input_dim().max(1);
+    let row_bytes = unsafe { sys::dab_minmax_row_bytes(transform.output_dim() as u32, nbits) } as usize;
+    let mut rows = vec![0u8; n * row_bytes];
+    let mut loss = vec![0f32; n];
+    check(unsafe {
+        sys::dab_minmax_compress_transformed(transform.raw, device, grid_scale, nbits, vectors.as_ptr(), n as u64, rows.as_mut_ptr(), loss.as_mut_ptr())
+    })?;
+    Ok((rows, loss))
+}
+
+/// Full-precision queries behind `transform` against rows compressed behind it: `[nq][n]`.  `Err` when an
+/// untransformed query holds NaN.
+pub fn minmax_query_distances_transformed(transform: &Transform, device: i32, metric: Metric, nbits: i32, queries: &[f32], rows: &[u8]) -> Result<Vec<f32>> {
+    let nq = queries.len() / transform.input_dim().max(1);
+    let n = rows.len() / unsafe { sys::dab_minmax_row_bytes(transform.output_dim() as u32, nbits) } as usize;
+    let mut out = vec![0f32; nq * n];
+    check(unsafe {
+        sys::dab_minmax_query_distances_transformed(transform.raw, device, metric as i32, nbits, queries.as_ptr(), nq as u32, rows.as_ptr(), n as u64, out.as_mut_ptr())
+    })?;
+    Ok(out)
+}

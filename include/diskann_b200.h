@@ -314,6 +314,48 @@ int dab_minmax_distances(int device, int metric, int nbits_x, int nbits_y, uint3
 int dab_minmax_query_distances(int device, int metric, int nbits, uint32_t dim, const float* queries, uint32_t nq,
                                const uint8_t* rows, uint64_t n, float* out);
 
+/* ------------------------------------------------------------------ Hadamard transforms in front of MinMax */
+
+/* The Hadamard transforms of diskann-quantization/src/algorithms/transforms, the counterpart of Transform::PaddingHadamard
+ * and Transform::DoubleHadamard (RandomRotation is not offered: its transform_into is a faer sgemm whose summation
+ * order is not restated).  A dab_transform is a host-side object; only the calls that take a device touch one. */
+typedef struct dab_transform dab_transform; /* opaque */
+enum {
+    DAB_TRANSFORM_PADDING_HADAMARD = 1, /* padding_hadamard.rs */
+    DAB_TRANSFORM_DOUBLE_HADAMARD = 2   /* double_hadamard.rs */
+};
+
+/* PaddingHadamard::try_from_parts (padding_hadamard.rs:137-173) / DoubleHadamard::try_from_parts (double_hadamard.rs:
+ * 146-206) from the parts the reference serializes.  Signs are 0 / 1 bytes (the flatbuffer's bool form): signs0 has
+ * input_dim of them; signs1 (DoubleHadamard only, NULL otherwise) has inner_dim.  inner_dim is padded_dim for
+ * PaddingHadamard and len(signs1) for DoubleHadamard.  subsample == NULL: none; otherwise n_subsample sorted indices
+ * into the inner vector.  The output dimension is n_subsample, or inner_dim without a subsample.  Every error of
+ * try_from_parts fails with its own message, in the reference's order; inner_dim > 32768 (one vector has to fit a
+ * warp's shared memory) fails with DAB_ERR_INVALID_ARGUMENT.  No device is touched. */
+int dab_transform_create(dab_transform** out, int kind, uint32_t input_dim, uint32_t inner_dim, const uint8_t* signs0,
+                         const uint8_t* signs1, const uint32_t* subsample, uint32_t n_subsample);
+void dab_transform_destroy(dab_transform* t);
+uint32_t dab_transform_input_dim(const dab_transform* t);   /* 0 for NULL */
+uint32_t dab_transform_output_dim(const dab_transform* t);  /* 0 for NULL */
+
+/* transform_into (padding_hadamard.rs:227-273, double_hadamard.rs:238-287) for n rows: src [n][input_dim] ->
+ * dst [n][output_dim], bit-identical to hadamard_transform's x86-64-v3 order (hadamard.rs:194-371). */
+int dab_transform_apply(const dab_transform* t, int device, const float* src, uint64_t n, float* dst);
+
+/* MinMaxQuantizer::new(transform, grid_scale) + CompressInto<&[f32], DataMutRef<NBITS>> (quantizer.rs:153-228) for n
+ * rows of input_dim values: the rows are transformed, then compressed like dab_minmax_compress with dim = output_dim.
+ * out_rows [n][dab_minmax_row_bytes(output_dim, nbits)], out_loss [n] (may be NULL).  The NaN check runs on the
+ * transformed vectors, as in the reference: the call fails naming the first row whose transformed vector holds a NaN
+ * (an input with two infinities of opposite sign does), after every row has been written. */
+int dab_minmax_compress_transformed(const dab_transform* t, int device, float grid_scale, int nbits, const float* vectors,
+                                    uint64_t n, uint8_t* out_rows, float* out_loss);
+
+/* dab_minmax_query_distances behind a transform: CompressInto<&[f32], FullQueryMut> (quantizer.rs:393-415) checks the
+ * *untransformed* query for NaN, transforms it and takes FullQueryMeta of the transformed vector; then the four MinMax
+ * distances against rows compressed at output_dim.  queries [nq][input_dim], out [nq][n]. */
+int dab_minmax_query_distances_transformed(const dab_transform* t, int device, int metric, int nbits, const float* queries,
+                                           uint32_t nq, const uint8_t* rows, uint64_t n, float* out);
+
 /* ------------------------------------------------------------------ build-side reuse */
 
 /* PruneAccessor::fill + robust_prune (diskann/src/graph/index.rs:2349-2380, 2565-2650;

@@ -16,14 +16,17 @@
 //                                  (diskann-benchmark-core/src/search/graph/knn.rs:208-238) for a
 //                                  whole query batch (the 3' boundary of SURVEY.md §8b)
 //   SearchStats                    diskann/src/graph/index.rs:90 (cmps, hops, result_count)
-//   MinMaxQuantizer                diskann-quantization/src/minmax/quantizer.rs:69-228 (Transform::Null) + the
-//                                  MinMax distance functors over compressed rows (vectors.rs:231-455)
+//   Transform                      Transform::{PaddingHadamard, DoubleHadamard} (diskann-quantization/src/algorithms/
+//                                  transforms): try_from_parts + transform_into
+//   MinMaxQuantizer                diskann-quantization/src/minmax/quantizer.rs:69-228 (Transform::Null or one of the
+//                                  above) + the MinMax distance functors over compressed rows (vectors.rs:231-455)
 //
 // Errors: every non-zero status becomes ANNError (the inmem layer returns Err on length / type
 // mismatch, layers/full.rs:203-213, 306-314; it never panics across the boundary).
 #pragma once
 
 #include <cstdint>
+#include <memory>
 #include <stdexcept>
 #include <string>
 #include <type_traits>
@@ -224,40 +227,93 @@ class GpuKNN {
     Pending pending_[DAB_MAX_SLOTS];
 };
 
-// MinMaxQuantizer (diskann-quantization/src/minmax/quantizer.rs:69-110, Transform::Null) and the MinMax distance
-// functors over compressed rows (vectors.rs:231-455).  Rows are the reference's canonical-front Data<NBITS> bytes.
+// Transform::PaddingHadamard / Transform::DoubleHadamard from the parts the reference serializes (try_from_parts:
+// padding_hadamard.rs:137-173, double_hadamard.rs:146-206); signs are 0 / 1 bytes.  A host-side object; apply() runs
+// transform_into on the device.
+class Transform {
+   public:
+    static Transform padding_hadamard(const std::vector<uint8_t>& signs, uint32_t padded_dim, const std::vector<uint32_t>* subsample = nullptr) {
+        return Transform(DAB_TRANSFORM_PADDING_HADAMARD, signs, padded_dim, nullptr, subsample);
+    }
+    static Transform double_hadamard(const std::vector<uint8_t>& signs0, const std::vector<uint8_t>& signs1,
+                                     const std::vector<uint32_t>* subsample = nullptr) {
+        return Transform(DAB_TRANSFORM_DOUBLE_HADAMARD, signs0, static_cast<uint32_t>(signs1.size()), &signs1, subsample);
+    }
+    Transform(Transform&& o) noexcept : h_(std::exchange(o.h_, nullptr)) {}
+    Transform& operator=(Transform&& o) noexcept {
+        std::swap(h_, o.h_);
+        return *this;
+    }
+    Transform(const Transform&) = delete;
+    Transform& operator=(const Transform&) = delete;
+    ~Transform() { dab_transform_destroy(h_); }
+
+    uint32_t input_dim() const { return dab_transform_input_dim(h_); }
+    uint32_t output_dim() const { return dab_transform_output_dim(h_); }
+    // transform_into for n rows: [n][input_dim] -> [n][output_dim]
+    std::vector<float> apply(const float* src, uint64_t n, int device = 0) const {
+        std::vector<float> out(n * output_dim());
+        check(dab_transform_apply(h_, device, src, n, out.data()));
+        return out;
+    }
+    const dab_transform* handle() const { return h_; }
+
+   private:
+    Transform(int kind, const std::vector<uint8_t>& signs0, uint32_t inner_dim, const std::vector<uint8_t>* signs1,
+              const std::vector<uint32_t>* subsample) {
+        check(dab_transform_create(&h_, kind, static_cast<uint32_t>(signs0.size()), inner_dim, signs0.data(), signs1 ? signs1->data() : nullptr,
+                                   subsample ? subsample->data() : nullptr, subsample ? static_cast<uint32_t>(subsample->size()) : 0u));
+    }
+    dab_transform* h_ = nullptr;
+};
+
+// MinMaxQuantizer (diskann-quantization/src/minmax/quantizer.rs:69-110) with Transform::Null, or behind a Transform, and
+// the MinMax distance functors over compressed rows (vectors.rs:231-455).  Rows are the reference's canonical-front
+// Data<NBITS> bytes at output_dim().
 class MinMaxQuantizer {
    public:
-    MinMaxQuantizer(uint32_t dim, float grid_scale, int device = 0) : dim_(dim), grid_scale_(grid_scale), device_(device) {}
+    MinMaxQuantizer(uint32_t dim, float grid_scale, int device = 0) : dim_(dim), out_dim_(dim), grid_scale_(grid_scale), device_(device) {}
+    MinMaxQuantizer(std::shared_ptr<const Transform> transform, float grid_scale, int device = 0)
+        : dim_(transform->input_dim()), out_dim_(transform->output_dim()), grid_scale_(grid_scale), device_(device), transform_(std::move(transform)) {}
     uint32_t dim() const { return dim_; }
-    uint32_t output_dim() const { return dim_; }
-    // Data::<NBITS>::canonical_bytes(dim)
-    size_t canonical_bytes(int nbits) const { return dab_minmax_row_bytes(dim_, nbits); }
-    // CompressInto<&[f32], DataMutRef<NBITS>> for n vectors; throws ANNError on NaN input (InputContainsNaN)
+    uint32_t output_dim() const { return out_dim_; }
+    // Data::<NBITS>::canonical_bytes(output_dim)
+    size_t canonical_bytes(int nbits) const { return dab_minmax_row_bytes(out_dim_, nbits); }
+    // CompressInto<&[f32], DataMutRef<NBITS>> for n vectors of dim() values; throws ANNError when a (transformed) vector
+    // holds NaN (InputContainsNaN)
     std::vector<uint8_t> compress(const float* vectors, uint64_t n, int nbits, std::vector<float>* loss = nullptr) const {
         std::vector<uint8_t> rows(n * canonical_bytes(nbits));
         if (loss) loss->resize(n);
-        check(dab_minmax_compress(device_, grid_scale_, dim_, nbits, vectors, n, rows.data(), loss ? loss->data() : nullptr));
+        if (transform_)
+            check(dab_minmax_compress_transformed(transform_->handle(), device_, grid_scale_, nbits, vectors, n, rows.data(),
+                                                  loss ? loss->data() : nullptr));
+        else
+            check(dab_minmax_compress(device_, grid_scale_, dim_, nbits, vectors, n, rows.data(), loss ? loss->data() : nullptr));
         return rows;
     }
     // MinMax{L2Squared, IP, Cosine, CosineNormalized}::evaluate(DataRef<N>, DataRef<M>) row by row (N x N, 8 x N)
     std::vector<float> distances(Metric metric, int nbits_x, int nbits_y, const uint8_t* x_rows, const uint8_t* y_rows, uint64_t n) const {
         std::vector<float> out(n);
-        check(dab_minmax_distances(device_, static_cast<int>(metric), nbits_x, nbits_y, dim_, x_rows, y_rows, n, out.data()));
+        check(dab_minmax_distances(device_, static_cast<int>(metric), nbits_x, nbits_y, out_dim_, x_rows, y_rows, n, out.data()));
         return out;
     }
 
     // CompressInto<&[f32], FullQueryMut> + MinMax*::evaluate(FullQueryRef, DataRef<NBITS>) for every (query, row): [nq][n]
     std::vector<float> query_distances(Metric metric, int nbits, const float* queries, uint32_t nq, const uint8_t* rows, uint64_t n) const {
         std::vector<float> out(static_cast<size_t>(nq) * n);
-        check(dab_minmax_query_distances(device_, static_cast<int>(metric), nbits, dim_, queries, nq, rows, n, out.data()));
+        if (transform_)
+            check(dab_minmax_query_distances_transformed(transform_->handle(), device_, static_cast<int>(metric), nbits, queries, nq, rows, n,
+                                                         out.data()));
+        else
+            check(dab_minmax_query_distances(device_, static_cast<int>(metric), nbits, dim_, queries, nq, rows, n, out.data()));
         return out;
     }
 
    private:
-    uint32_t dim_;
+    uint32_t dim_, out_dim_;
     float grid_scale_;
     int device_;
+    std::shared_ptr<const Transform> transform_;
 };
 
 }  // namespace diskann_b200
