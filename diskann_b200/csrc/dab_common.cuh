@@ -65,6 +65,13 @@ struct Tuning {
     void load();
 };
 
+// The largest visited set the searches at (l, beam, mode) have seen; later calls size their visited tables from it
+// (search_kernel.cu).  `mode`: which quantized store the traversal reads (0 for full precision and PQ, 1 for SQ).
+struct VisitedHint {
+    uint32_t l = 0, beam = 0, visited = 0;
+    int mode = 0;
+};
+
 }  // namespace dab
 
 struct dab_index {
@@ -110,8 +117,7 @@ struct dab_index {
     void* slots[DAB_MAX_SLOTS] = {};  // batches in flight (dab_search_batch_async), search_kernel.cu
 
     // search-side state learned across calls
-    uint32_t hint_l = 0, hint_beam = 0, hint_visited = 0;  // largest visited set seen at (L, beam)
-    uint32_t pq_hint_l = 0, pq_hint_beam = 0, pq_hint_visited = 0; int pq_hint_mode = 0;  // the same for the PQ traversal kernel
+    dab::VisitedHint hint, pq_hint;  // full precision; PQ / SQ traversal (visits other nodes: kept apart)
     uint32_t v3_overflow_l = 0, v3_overflow_beam = 0;      // share of queries that outgrew the shared-memory
     float v3_overflow_frac = 0.0f;                         // tables at (L, beam): search_kernel_v3 is skipped when large
 

@@ -1,17 +1,66 @@
-// search_kernel.cu — the host side of batched full-precision search: the dispatcher, the slots of batches in
-// flight and the C entry points (dab_search_batch[_device][_async], dab_wait).
+// search_kernel.cu — the host side of batched graph search: the visited-table policy, the overflow re-runs and the
+// host-buffer calls every search shares (search_host.cuh), the full-precision dispatcher, the slots of batches in flight
+// and the C entry points (dab_search_batch[_device][_async], dab_wait).
 //
 // A batch runs on search_kernel_v3 (visited set in shared memory) where its short lists make that the faster kernel,
 // and on search_kernel_v2 (global visited tables) otherwise; queries whose visited set outgrows its table are re-run
 // on v2 with larger tables, so membership stays exact.  Both kernels restate DiskANNIndex::search_internal
 // (index.rs:1933-2000) bit for bit.
 #include "dab_common.cuh"
+#include "search_host.cuh"
 #include "search_v2.cuh"
 #include "search_v3.cuh"
 
 #include <algorithm>
 
 namespace dab {
+
+int check_search_args(const dab_index* idx, uint32_t k, uint32_t l_search, uint32_t beam, bool need_vectors) {
+    if (!idx->graph_ready || (need_vectors && !idx->vectors_ready))
+        return fail(DAB_ERR_NOT_READY, need_vectors ? "search: vectors and graph must be uploaded first" : "search: graph must be uploaded first");
+    if (k == 0 || l_search == 0 || beam == 0) return fail(DAB_ERR_INVALID_ARGUMENT, "search: k, l_search and beam_width must be > 0");
+    if (beam > 64) return fail(DAB_ERR_INVALID_ARGUMENT, "search: beam_width %u > 64", beam);
+    return DAB_OK;
+}
+
+// ---- visited tables in global memory (search_kernel_v2, search_kernel_pq, search_kernel_pqs) -----------------------
+// Every warp owns a table of `slots` ids in 32-byte buckets of 8.  A query whose visited set passes 7/8 of its table
+// stops and is listed in the pass's overflow list; it is re-run on a larger table, so membership is exact at any size.
+uint64_t table_slots(const dab_index* idx, const VisitedHint& hint, uint32_t l_search, uint32_t beam, int mode) {
+    if (idx->tune.test_visited_log2) return 1ull << idx->tune.test_visited_log2;  // tests force the overflow re-runs
+    // the reference's estimate (scratch.rs:186-192: 1.1 * max_degree * 1.3 * L), never more than the index
+    double est = 1.1 * idx->max_degree * 1.3 * (double)l_search;
+    if (hint.visited > 0 && l_search <= hint.l && beam <= hint.beam && mode == hint.mode) {
+        // the estimate is ~10x what a search touches: 1.15x the largest visited set seen at this (or a larger) L and
+        // beam (visited sets grow monotonically with both) at 87.5 % load
+        const double seen = ((double)hint.visited * 1.15 + idx->max_degree) / 0.875 + 8.0;
+        est = std::min(est, seen);
+    }
+    est = std::min(est, (double)idx->n_total() * 1.34);
+    return std::max<uint64_t>(256, (uint64_t)est + 1);
+}
+
+void learn_visited(VisitedHint& hint, uint32_t l_search, uint32_t beam, int mode, uint32_t visited) {
+    if (l_search != hint.l || beam != hint.beam || mode != hint.mode) hint = VisitedHint{l_search, beam, 0, mode};
+    hint.visited = std::max(hint.visited, visited);
+}
+
+int grow_visited_tables(const dab_index* idx, int& pass, uint64_t& slots) {
+    if (++pass >= 6) return fail(DAB_ERR_VISITED_OVERFLOW, "search: visited set still overflowing after 6 passes");
+    slots *= 4;
+    // a visited set holds at most n_total + max_degree ids: 2 * n_total + 2048 slots take it below the 7/8 limit
+    if (slots > 4 * idx->n_total() + 4096) slots = 2 * idx->n_total() + 2048;
+    return DAB_OK;
+}
+
+int take_overflow_list(cudaStream_t stream, const uint32_t* d_overflow, uint32_t n_over, Scratch& retry) {
+    // the pass that wrote the list is complete, so `retry` (its own work list, or empty) can be overwritten
+    int rc;
+    if ((rc = retry.reserve((size_t)n_over * 4))) return rc;
+    DAB_CUDA(cudaMemcpyAsync(retry.p, d_overflow, (size_t)n_over * 4, cudaMemcpyDeviceToDevice, stream));
+    DAB_CUDA(cudaStreamSynchronize(stream));
+    return DAB_OK;
+}
 
 // ---- one batch of searches as a resumable job ------------------------------------------------
 // A batch is launched (`launch`: kernel + read-back of the four counters into pinned memory, nothing
@@ -80,20 +129,7 @@ int SearchJob::prepare(const void* d_queries, const uint32_t* d_query_rows, uint
     p2.rec_counts = rec_counts;
     p2.rec_cap = rec_cap;
 
-    // visited-table capacity: the reference's estimate (scratch.rs:186-192:
-    // 1.1 * max_degree * 1.3 * L), never more than the index, at least 256 slots
-    double est = 1.1 * idx->max_degree * 1.3 * (double)l_search;
-    const bool hinted = idx->hint_visited > 0 && l_search <= idx->hint_l && beam <= idx->hint_beam;
-    if (hinted) {
-        // later batches: 1.15x the largest visited set seen at this (or a larger) L (visited sets
-        // grow monotonically with L); queries that still overflow are re-run with a larger table
-        const double seen = ((double)idx->hint_visited * 1.15 + idx->max_degree) / 0.875 + 8.0;
-        if (seen < est) est = seen;
-    }
-    if (est > (double)idx->n_total() * 1.34) est = (double)idx->n_total() * 1.34;
-    slots = std::max<uint64_t>(256, (uint64_t)est + 1);
-    if (idx->tune.test_visited_log2) slots = 1ull << idx->tune.test_visited_log2;  // tests force the overflow/retry path
-
+    slots = table_slots(idx, idx->hint, l_search, beam, 0);
     if ((rc = counters->reserve(16 + (size_t)nq * 4))) return rc;
     d_counters = (uint32_t*)counters->p;
     d_overflow = d_counters + 4;
@@ -106,9 +142,7 @@ int SearchJob::prepare(const void* d_queries, const uint32_t* d_query_rows, uint
     // kernel; queries that outgrow their table are re-run on global tables
     stage = 1;
     pass = 0;
-    uint32_t need = 0;
-    if (hinted) need = (uint32_t)std::min<double>((double)idx->hint_visited * 1.15, 4.0e9);
-    if (idx->tune.test_visited_log2) need = (1u << idx->tune.test_visited_log2) / 2;
+    const uint32_t need = idx->tune.test_visited_log2 ? (1u << idx->tune.test_visited_log2) / 2 : 0;  // tests: tables that overflow
     const bool skip = idx->v3_overflow_l == l_search && idx->v3_overflow_beam == beam && idx->v3_overflow_frac > 0.25f;
     memset(&p3, 0, sizeof(p3));
     if (!skip && v3_prepare(idx, l_search, beam, need, p3, v3) == 0) {
@@ -164,56 +198,28 @@ int SearchJob::finish() {
         idx->rec_truncated += h_counters[3];
         const uint32_t n_over = h_counters[1];
         if (!recording) {  // build-time searches run on a growing graph: do not learn from them
-            if (l_search != idx->hint_l || beam != idx->hint_beam) {
-                idx->hint_l = l_search;
-                idx->hint_beam = beam;
-                idx->hint_visited = 0;
-            }
-            idx->hint_visited = std::max(idx->hint_visited, h_counters[2]);
+            learn_visited(idx->hint, l_search, beam, 0, h_counters[2]);
             if (stage == 0) {
                 idx->v3_overflow_l = l_search;
                 idx->v3_overflow_beam = beam;
                 idx->v3_overflow_frac = (float)n_over / (float)nq;
             }
         }
-        if (n_over == 0) {
-            retry_list.release();
-            return DAB_OK;
-        }
+        if (n_over == 0) return DAB_OK;
         // re-run the overflowed queries on (larger) global tables
-        Scratch next;
         int rc;
-        if ((rc = next.reserve((size_t)n_over * 4))) return rc;
-        DAB_CUDA(cudaMemcpyAsync(next.p, d_overflow, (size_t)n_over * 4, cudaMemcpyDeviceToDevice, stream));
-        DAB_CUDA(cudaStreamSynchronize(stream));
-        retry_list.release();
-        retry_list = next;
+        if ((rc = take_overflow_list(stream, d_overflow, n_over, retry_list))) return rc;
         p2.query_list = (const uint32_t*)retry_list.p;
         p2.n_work = n_over;
         if (stage == 0) {
             // the overflowed queries are the largest: size the global tables from the estimate again
             stage = 1;
-            pass = 0;
-            if (!idx->tune.test_visited_log2)
-                slots = std::max<uint64_t>(slots, std::min<uint64_t>((uint64_t)(1.1 * idx->max_degree * 1.3 * (double)l_search) + 1,
-                                                                        (uint64_t)((double)idx->n_total() * 1.34) + 1));
-        } else {
-            if (++pass >= 6) {
-                retry_list.release();
-                return fail(DAB_ERR_VISITED_OVERFLOW, "search: visited set still overflowing after 6 passes");
-            }
-            slots *= 4;
-            if (slots > 4 * idx->n_total() + 4096) slots = 2 * idx->n_total() + 2048;
+            slots = std::max(slots, table_slots(idx, VisitedHint{}, l_search, beam, 0));
+        } else if ((rc = grow_visited_tables(idx, pass, slots))) {
+            return rc;
         }
         if ((rc = launch())) return rc;
     }
-}
-
-static int check_search_args(const dab_index* idx, uint32_t k, uint32_t l_search, uint32_t beam) {
-    if (!idx->vectors_ready || !idx->graph_ready) return fail(DAB_ERR_NOT_READY, "search: vectors and graph must be uploaded first");
-    if (k == 0 || l_search == 0 || beam == 0) return fail(DAB_ERR_INVALID_ARGUMENT, "search: k, l_search and beam_width must be > 0");
-    if (beam > 64) return fail(DAB_ERR_INVALID_ARGUMENT, "search: beam_width %u > 64", beam);
-    return DAB_OK;
 }
 
 // Runs the search over work items on the handle's stream and waits; device pointers only.  `rec_*` optional.
@@ -237,20 +243,59 @@ int run_search(dab_index* idx, const void* d_queries, const uint32_t* d_query_ro
     return job.finish();
 }
 
-// ---- batches in flight (dab_search_batch_async / dab_search_batch_device_async / dab_wait) ----
-struct AsyncHostOut {  // host destinations of a pending host-buffer call
-    uint32_t* ids;
-    float* dists;
-    uint32_t *counts, *cmps, *hops;
+// ---- host-buffer calls -------------------------------------------------------------------------
+// A host-buffer call's results: where the kernels write them and where the caller wants them
+struct HostCopy {
+    SearchOut dev, host;
     uint32_t nq, k;
 };
 
+// reserves the query and result buffers of a host-buffer call (`q`; ids and dists in `out`, counts / cmps / hops in
+// `stats`) and queues the copy of the queries on `stream`
+static int stage_host_call(const dab_index* idx, cudaStream_t stream, Scratch& q, Scratch& out, Scratch& stats, const void* queries,
+                           uint32_t nq, uint32_t k, SearchOut* d) {
+    const size_t qbytes = (size_t)nq * idx->dim * elem_size(idx->dtype);
+    const size_t rbytes = (size_t)nq * k * 4;
+    int rc;
+    if ((rc = q.reserve(qbytes)) || (rc = out.reserve(2 * rbytes)) || (rc = stats.reserve((size_t)nq * 12))) return rc;
+    uint32_t* st = (uint32_t*)stats.p;
+    *d = SearchOut{(uint32_t*)out.p, (float*)((uint8_t*)out.p + rbytes), st, st + nq, st + 2 * (size_t)nq};
+    DAB_CUDA(cudaMemcpyAsync(q.p, queries, qbytes, cudaMemcpyHostToDevice, stream));
+    return DAB_OK;
+}
+
+static int queue_result_copies(cudaStream_t stream, const HostCopy& c) {
+    const size_t rbytes = (size_t)c.nq * c.k * 4, sbytes = (size_t)c.nq * 4;
+    DAB_CUDA(cudaMemcpyAsync(c.host.ids, c.dev.ids, rbytes, cudaMemcpyDeviceToHost, stream));
+    DAB_CUDA(cudaMemcpyAsync(c.host.dists, c.dev.dists, rbytes, cudaMemcpyDeviceToHost, stream));
+    if (c.host.counts) DAB_CUDA(cudaMemcpyAsync(c.host.counts, c.dev.counts, sbytes, cudaMemcpyDeviceToHost, stream));
+    if (c.host.cmps) DAB_CUDA(cudaMemcpyAsync(c.host.cmps, c.dev.cmps, sbytes, cudaMemcpyDeviceToHost, stream));
+    if (c.host.hops) DAB_CUDA(cudaMemcpyAsync(c.host.hops, c.dev.hops, sbytes, cudaMemcpyDeviceToHost, stream));
+    return DAB_OK;
+}
+
+int search_host_buffers(dab_index* idx, const char* api, const void* queries, uint32_t nq, uint32_t k, const SearchOut& out,
+                        const std::function<int(const void* d_queries, const SearchOut& d_out)>& run) {
+    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", api);
+    if (nq == 0) return DAB_OK;
+    if (!queries || !out.ids || !out.dists) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
+    if (k == 0) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: k must be > 0", api);
+    DAB_CUDA(cudaSetDevice(idx->device));
+    HostCopy c{{}, out, nq, k};
+    int rc;
+    if ((rc = stage_host_call(idx, idx->stream, idx->s_queries, idx->s_out, idx->s_stats, queries, nq, k, &c.dev)) ||
+        (rc = run(idx->s_queries.p, c.dev)) || (rc = queue_result_copies(idx->stream, c)))
+        return rc;
+    DAB_CUDA(cudaStreamSynchronize(idx->stream));
+    return DAB_OK;
+}
+
+// ---- batches in flight (dab_search_batch_async / dab_search_batch_device_async / dab_wait) ----
 struct SearchSlot {
     cudaStream_t stream = nullptr;
     Scratch tables, counters, queries, out, stats, h_counters;
     SearchJob* job = nullptr;
-    AsyncHostOut host_out{};
-    bool has_host_out = false;
+    HostCopy host_out{};  // the pending call's result copies (host_out.host.ids null: device buffers)
 };
 
 void search_slots_release(dab_index* idx) {
@@ -283,7 +328,7 @@ static int slot_of(dab_index* idx, uint32_t slot, SearchSlot** out) {
 }
 
 static int slot_launch(dab_index* idx, SearchSlot* s, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam,
-                       uint32_t* d_ids, float* d_dists, uint32_t* d_counts, uint32_t* d_cmps, uint32_t* d_hops) {
+                       const SearchOut& d) {
     int rc;
     if ((rc = s->h_counters.reserve(16))) return rc;
     SearchJob* job = new SearchJob();
@@ -293,7 +338,7 @@ static int slot_launch(dab_index* idx, SearchSlot* s, const void* d_queries, uin
     job->counters = &s->counters;
     job->h_counters = (uint32_t*)s->h_counters.p;
     job->full_grid = true;
-    if ((rc = job->prepare(d_queries, nullptr, nq, k, l_search, beam, d_ids, d_dists, d_counts, d_cmps, d_hops, nullptr, nullptr,
+    if ((rc = job->prepare(d_queries, nullptr, nq, k, l_search, beam, d.ids, d.dists, d.counts, d.cmps, d.hops, nullptr, nullptr,
                            nullptr, 0)) ||
         (rc = job->launch())) {
         delete job;
@@ -322,33 +367,11 @@ int dab_search_batch_device(dab_index* idx, const void* d_queries, uint32_t nq, 
 int dab_search_batch(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
                      uint32_t beam_width, uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
                      uint32_t* out_cmps, uint32_t* out_hops) {
-    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch: idx is NULL");
-    if (nq == 0) return DAB_OK;
-    if (!queries || !out_ids || !out_dists) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch: NULL argument");
-    if (k == 0) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch: k must be > 0");
-    DAB_CUDA(cudaSetDevice(idx->device));
-    const size_t qbytes = (size_t)nq * idx->dim * elem_size(idx->dtype);
-    const size_t rbytes = (size_t)nq * k * 4;
-    int rc;
-    if ((rc = idx->s_queries.reserve(qbytes))) return rc;
-    if ((rc = idx->s_out.reserve(2 * rbytes))) return rc;
-    if ((rc = idx->s_stats.reserve((size_t)nq * 12))) return rc;
-    uint32_t* d_ids = (uint32_t*)idx->s_out.p;
-    float* d_dists = (float*)((uint8_t*)idx->s_out.p + rbytes);
-    uint32_t* d_counts = (uint32_t*)idx->s_stats.p;
-    uint32_t* d_cmps = d_counts + nq;
-    uint32_t* d_hops = d_cmps + nq;
-    DAB_CUDA(cudaMemcpyAsync(idx->s_queries.p, queries, qbytes, cudaMemcpyHostToDevice, idx->stream));
-    if ((rc = run_search(idx, idx->s_queries.p, nullptr, nq, k, l_search, beam_width, d_ids, d_dists, d_counts, d_cmps,
-                         d_hops, nullptr, nullptr, nullptr, 0)))
-        return rc;
-    DAB_CUDA(cudaMemcpyAsync(out_ids, d_ids, rbytes, cudaMemcpyDeviceToHost, idx->stream));
-    DAB_CUDA(cudaMemcpyAsync(out_dists, d_dists, rbytes, cudaMemcpyDeviceToHost, idx->stream));
-    if (out_counts) DAB_CUDA(cudaMemcpyAsync(out_counts, d_counts, (size_t)nq * 4, cudaMemcpyDeviceToHost, idx->stream));
-    if (out_cmps) DAB_CUDA(cudaMemcpyAsync(out_cmps, d_cmps, (size_t)nq * 4, cudaMemcpyDeviceToHost, idx->stream));
-    if (out_hops) DAB_CUDA(cudaMemcpyAsync(out_hops, d_hops, (size_t)nq * 4, cudaMemcpyDeviceToHost, idx->stream));
-    DAB_CUDA(cudaStreamSynchronize(idx->stream));
-    return DAB_OK;
+    return search_host_buffers(idx, "dab_search_batch", queries, nq, k, SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops},
+                               [&](const void* d_queries, const SearchOut& d) {
+                                   return run_search(idx, d_queries, nullptr, nq, k, l_search, beam_width, d.ids, d.dists, d.counts,
+                                                     d.cmps, d.hops, nullptr, nullptr, nullptr, 0);
+                               });
 }
 
 // ---- asynchronous batches: launch on a slot, collect with dab_wait ---------------------------
@@ -357,19 +380,6 @@ int dab_search_batch(dab_index* idx, const void* queries, uint32_t nq, uint32_t 
 // it is queued by this call when no query can overflow its visited table on the way, i.e. nothing waits.
 // dab_wait(slot) blocks until the slot's batch is complete (and, in the rare overflow case, re-runs the
 // affected queries and repeats the result copies).  The buffers must stay valid until dab_wait returns.
-static int queue_result_copies(SearchSlot* s, const AsyncHostOut& o) {
-    const size_t rbytes = (size_t)o.nq * o.k * 4;
-    uint32_t* d_ids = (uint32_t*)s->out.p;
-    float* d_dists = (float*)((uint8_t*)s->out.p + rbytes);
-    uint32_t* d_counts = (uint32_t*)s->stats.p;
-    DAB_CUDA(cudaMemcpyAsync(o.ids, d_ids, rbytes, cudaMemcpyDeviceToHost, s->stream));
-    DAB_CUDA(cudaMemcpyAsync(o.dists, d_dists, rbytes, cudaMemcpyDeviceToHost, s->stream));
-    if (o.counts) DAB_CUDA(cudaMemcpyAsync(o.counts, d_counts, (size_t)o.nq * 4, cudaMemcpyDeviceToHost, s->stream));
-    if (o.cmps) DAB_CUDA(cudaMemcpyAsync(o.cmps, d_counts + o.nq, (size_t)o.nq * 4, cudaMemcpyDeviceToHost, s->stream));
-    if (o.hops) DAB_CUDA(cudaMemcpyAsync(o.hops, d_counts + 2 * (size_t)o.nq, (size_t)o.nq * 4, cudaMemcpyDeviceToHost, s->stream));
-    return DAB_OK;
-}
-
 int dab_search_batch_async(dab_index* idx, uint32_t slot, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
                            uint32_t beam_width, uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps,
                            uint32_t* out_hops) {
@@ -382,21 +392,13 @@ int dab_search_batch_async(dab_index* idx, uint32_t slot, const void* queries, u
     if ((rc = slot_of(idx, slot, &s))) return rc;
     if (s->job) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_async: slot %u still has a batch in flight (call dab_wait)", slot);
     if (nq == 0) return DAB_OK;
-    const size_t qbytes = (size_t)nq * idx->dim * elem_size(idx->dtype);
-    const size_t rbytes = (size_t)nq * k * 4;
-    if ((rc = s->queries.reserve(qbytes))) return rc;
-    if ((rc = s->out.reserve(2 * rbytes))) return rc;
-    if ((rc = s->stats.reserve((size_t)nq * 12))) return rc;
-    uint32_t* d_ids = (uint32_t*)s->out.p;
-    float* d_dists = (float*)((uint8_t*)s->out.p + rbytes);
-    uint32_t* d_counts = (uint32_t*)s->stats.p;
-    DAB_CUDA(cudaMemcpyAsync(s->queries.p, queries, qbytes, cudaMemcpyHostToDevice, s->stream));
-    if ((rc = slot_launch(idx, s, s->queries.p, nq, k, l_search, beam_width, d_ids, d_dists, d_counts, d_counts + nq, d_counts + 2 * (size_t)nq)))
+    HostCopy c{{}, SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, nq, k};
+    if ((rc = stage_host_call(idx, s->stream, s->queries, s->out, s->stats, queries, nq, k, &c.dev)) ||
+        (rc = slot_launch(idx, s, s->queries.p, nq, k, l_search, beam_width, c.dev)))
         return rc;
-    s->host_out = AsyncHostOut{out_ids, out_dists, out_counts, out_cmps, out_hops, nq, k};
-    s->has_host_out = true;
+    s->host_out = c;
     // optimistic copies: valid as they are unless a query overflowed (then dab_wait repeats them)
-    return queue_result_copies(s, s->host_out);
+    return queue_result_copies(s->stream, c);
 }
 
 int dab_search_batch_device_async(dab_index* idx, uint32_t slot, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
@@ -411,8 +413,8 @@ int dab_search_batch_device_async(dab_index* idx, uint32_t slot, const void* d_q
     if ((rc = slot_of(idx, slot, &s))) return rc;
     if (s->job) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_device_async: slot %u still has a batch in flight (call dab_wait)", slot);
     if (nq == 0) return DAB_OK;
-    s->has_host_out = false;
-    return slot_launch(idx, s, d_queries, nq, k, l_search, beam_width, d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops);
+    s->host_out = HostCopy{};
+    return slot_launch(idx, s, d_queries, nq, k, l_search, beam_width, SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops});
 }
 
 int dab_wait(dab_index* idx, uint32_t slot) {
@@ -428,8 +430,8 @@ int dab_wait(dab_index* idx, uint32_t slot) {
     int rc = job->finish();
     delete job;
     if (rc) return rc;
-    if (overflowed && s->has_host_out) {
-        if ((rc = queue_result_copies(s, s->host_out))) return rc;
+    if (overflowed && s->host_out.host.ids) {
+        if ((rc = queue_result_copies(s->stream, s->host_out))) return rc;
         DAB_CUDA(cudaStreamSynchronize(s->stream));
     }
     return DAB_OK;

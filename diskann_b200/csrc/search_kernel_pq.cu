@@ -27,6 +27,7 @@
 #include "dab_common.cuh"
 #include "quant_device.cuh"
 #include "search_common.cuh"
+#include "search_host.cuh"
 #include "search_pq.cuh"
 #include "search_smem.cuh"
 
@@ -487,12 +488,12 @@ static int launch_rerank(dab_index* idx, const void* d_queries, uint32_t nq, uin
 static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam,
                          uint32_t* d_ids, float* d_dists, uint32_t* d_counts, uint32_t* d_cmps, uint32_t* d_hops, bool rerank,
                          int mode = 0) {
-    if (!idx->graph_ready) return fail(DAB_ERR_NOT_READY, "dab_search_batch_pq: graph must be uploaded first");
+    int rc;
+    if ((rc = check_search_args(idx, k, l_search, beam, false))) return rc;
     if (mode == 0 && (!idx->d_pivots || !idx->d_codes || !idx->pq_codes_ready))
         return fail(DAB_ERR_NOT_READY, "dab_search_batch_pq: no PQ codes (dab_upload_pq with codes, or dab_pq_encode_all)");
     if (mode == 1 && (!idx->d_sq_codes || !idx->sq_codes_ready))
         return fail(DAB_ERR_NOT_READY, "dab_search_batch_sq: no scalar-quantized rows (dab_upload_sq with rows, or dab_sq_encode_all)");
-    if (k == 0 || l_search == 0 || beam == 0 || beam > 64) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_pq: bad k / l_search / beam_width");
     // SQStore::distance_computer (providers inmem/scalar.rs:214-226): UnsupportedDistanceMetric
     if (mode == 1 && idx->metric == DAB_COSINE)
         return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_sq: the scalar-quantized store supports L2, InnerProduct and CosineNormalized");
@@ -588,22 +589,10 @@ static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uin
         warps = (uint32_t)grid * kPqWarps;
     }
 
-    // visited-table capacity: the reference's estimate (scratch.rs:186-192) on the first call, then 1.15x the
-    // largest visited set seen at this (or a larger) L at 87.5 % load — the estimate is ~10x what a search
-    // touches, and every query clears its table; queries that still overflow are re-run below
-    uint64_t slots = std::max<uint64_t>(256, (uint64_t)(1.1 * idx->max_degree * 1.3 * (double)l_search) + 1);
-    if (idx->pq_hint_visited > 0 && l_search <= idx->pq_hint_l && beam <= idx->pq_hint_beam && mode == idx->pq_hint_mode &&
-        !idx->tune.test_visited_log2) {
-        const uint64_t seen = (uint64_t)(((double)idx->pq_hint_visited * 1.15 + idx->max_degree) / 0.875) + 8;
-        slots = std::min(slots, std::max<uint64_t>(256, seen));
-    }
-    if (slots > 2 * idx->n_total() + 2048) slots = 2 * idx->n_total() + 2048;
-    if (idx->tune.test_visited_log2) slots = 1ull << idx->tune.test_visited_log2;  // tests force the overflow re-runs
-    int rc;
-    if ((rc = idx->s_counters.reserve(16 + (size_t)nq * 4))) return rc;
-    uint32_t* d_counters = (uint32_t*)idx->s_counters.p;
-    p.counters = d_counters;
-    p.overflow_list = d_counters + 4;
+    if ((rc = idx->s_counters.reserve(16 + (size_t)nq * 4)) || (rc = idx->h_counters.reserve(16))) return rc;
+    p.counters = (uint32_t*)idx->s_counters.p;
+    p.overflow_list = p.counters + 4;
+    uint32_t* h_counters = (uint32_t*)idx->h_counters.p;
     const size_t lut_bytes = mode == 0 && !use_pqs ? (size_t)warps * idx->pq_chunks * idx->pq_centers * 4 : 16;
     if ((rc = idx->s_out2.reserve(lut_bytes))) return rc;
     p.luts = (float*)idx->s_out2.p;
@@ -615,100 +604,62 @@ static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uin
         p.list_counts = p.list_ids + (size_t)nq * cap;
         p.list_cap = cap;
     }
+    // global-table passes: the overflowed queries of one are re-run on larger tables in the next
+    uint64_t slots = table_slots(idx, idx->pq_hint, l_search, beam, mode);
     Scratch retry;
-    for (int pass = 0; pass < 6; ++pass) {
-        p.n_buckets = (uint32_t)((slots + 7) / 8);
-        if ((rc = idx->s_tables.reserve((size_t)warps * p.n_buckets * 32))) {
-            retry.release();
-            return rc;
-        }
-        p.tables = (uint32_t*)idx->s_tables.p;
-        DAB_CUDA(cudaMemsetAsync(d_counters, 0, 16, idx->stream));
-        if (use_pqs) {
-            if ((rc = pqs_launch(idx, p, plan, cap))) {
-                retry.release();
-                return rc;
+    rc = [&]() -> int {
+        for (int pass = 0;;) {
+            int rc2;
+            p.n_buckets = (uint32_t)((slots + 7) / 8);
+            if ((rc2 = idx->s_tables.reserve((size_t)warps * p.n_buckets * 32))) return rc2;
+            p.tables = (uint32_t*)idx->s_tables.p;
+            DAB_CUDA(cudaMemsetAsync(p.counters, 0, 16, idx->stream));
+            if (use_pqs) {
+                if ((rc2 = pqs_launch(idx, p, plan, cap))) return rc2;
+            } else {
+                kern<<<grid, kPqWarps * 32, smem_block, idx->stream>>>(p);
+                DAB_LAUNCHED();
+                DAB_CUDA(cudaGetLastError());
             }
-        } else {
-            kern<<<grid, kPqWarps * 32, smem_block, idx->stream>>>(p);
-            DAB_LAUNCHED();
-            DAB_CUDA(cudaGetLastError());
+            DAB_CUDA(cudaMemcpyAsync(h_counters, p.counters, 16, cudaMemcpyDeviceToHost, idx->stream));
+            DAB_CUDA(cudaStreamSynchronize(idx->stream));
+            learn_visited(idx->pq_hint, l_search, beam, mode, h_counters[2]);
+            const uint32_t n_over = h_counters[1];
+            if (n_over == 0) return DAB_OK;
+            if ((rc2 = take_overflow_list(idx->stream, p.overflow_list, n_over, retry)) || (rc2 = grow_visited_tables(idx, pass, slots)))
+                return rc2;
+            p.query_list = (const uint32_t*)retry.p;
+            p.n_work = n_over;
         }
-        uint32_t h[3] = {0, 0, 0};
-        DAB_CUDA(cudaMemcpyAsync(h, d_counters, 12, cudaMemcpyDeviceToHost, idx->stream));
-        DAB_CUDA(cudaStreamSynchronize(idx->stream));
-        if (l_search != idx->pq_hint_l || beam != idx->pq_hint_beam || mode != idx->pq_hint_mode) {
-            idx->pq_hint_l = l_search;
-            idx->pq_hint_beam = beam;
-            idx->pq_hint_mode = mode;
-            idx->pq_hint_visited = 0;
-        }
-        idx->pq_hint_visited = std::max(idx->pq_hint_visited, h[2]);
-        if (h[1] == 0) {
-            retry.release();
-            if (rerank) return launch_rerank(idx, d_queries, nq, k, cap, p.list_ids, p.list_counts, d_ids, d_dists, d_counts);
-            return DAB_OK;
-        }
-        Scratch next;
-        if ((rc = next.reserve((size_t)h[1] * 4))) {
-            retry.release();
-            return rc;
-        }
-        DAB_CUDA(cudaMemcpy(next.p, d_counters + 4, (size_t)h[1] * 4, cudaMemcpyDeviceToDevice));
-        retry.release();
-        retry = next;
-        p.query_list = (const uint32_t*)retry.p;
-        p.n_work = h[1];
-        slots *= 4;
-    }
+    }();
     retry.release();
-    return fail(DAB_ERR_VISITED_OVERFLOW, "dab_search_batch_pq: visited set still overflowing after 6 passes");
+    if (rc) return rc;
+    return rerank ? launch_rerank(idx, d_queries, nq, k, cap, p.list_ids, p.list_counts, d_ids, d_dists, d_counts) : DAB_OK;
+}
+
+static int search_pq_host(dab_index* idx, const char* api, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                          uint32_t beam_width, const SearchOut& out, bool rerank, int mode) {
+    return search_host_buffers(idx, api, queries, nq, k, out, [&](const void* d_queries, const SearchOut& d) {
+        return run_search_pq(idx, d_queries, nq, k, l_search, beam_width, d.ids, d.dists, d.counts, d.cmps, d.hops, rerank, mode);
+    });
 }
 
 }  // namespace dab
 
 using namespace dab;
 
-static int search_pq_host(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
-                          uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops, bool rerank,
-                          int mode = 0) {
-    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_pq: idx is NULL");
-    if (nq == 0) return DAB_OK;
-    if (!queries || !out_ids || !out_dists) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_pq: NULL argument");
-    if (k == 0) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_pq: k must be > 0");
-    DAB_CUDA(cudaSetDevice(idx->device));
-    const size_t qbytes = (size_t)nq * idx->dim * elem_size(idx->dtype);
-    const size_t rbytes = (size_t)nq * k * 4;
-    int rc;
-    if ((rc = idx->s_queries.reserve(qbytes))) return rc;
-    if ((rc = idx->s_out.reserve(2 * rbytes))) return rc;
-    if ((rc = idx->s_stats.reserve((size_t)nq * 12))) return rc;
-    uint32_t* d_ids = (uint32_t*)idx->s_out.p;
-    float* d_dists = (float*)((uint8_t*)idx->s_out.p + rbytes);
-    uint32_t* d_counts = (uint32_t*)idx->s_stats.p;
-    uint32_t* d_cmps = d_counts + nq;
-    uint32_t* d_hops = d_cmps + nq;
-    DAB_CUDA(cudaMemcpyAsync(idx->s_queries.p, queries, qbytes, cudaMemcpyHostToDevice, idx->stream));
-    if ((rc = run_search_pq(idx, idx->s_queries.p, nq, k, l_search, beam_width, d_ids, d_dists, d_counts, d_cmps, d_hops, rerank, mode))) return rc;
-    DAB_CUDA(cudaMemcpyAsync(out_ids, d_ids, rbytes, cudaMemcpyDeviceToHost, idx->stream));
-    DAB_CUDA(cudaMemcpyAsync(out_dists, d_dists, rbytes, cudaMemcpyDeviceToHost, idx->stream));
-    if (out_counts) DAB_CUDA(cudaMemcpyAsync(out_counts, d_counts, (size_t)nq * 4, cudaMemcpyDeviceToHost, idx->stream));
-    if (out_cmps) DAB_CUDA(cudaMemcpyAsync(out_cmps, d_cmps, (size_t)nq * 4, cudaMemcpyDeviceToHost, idx->stream));
-    if (out_hops) DAB_CUDA(cudaMemcpyAsync(out_hops, d_hops, (size_t)nq * 4, cudaMemcpyDeviceToHost, idx->stream));
-    DAB_CUDA(cudaStreamSynchronize(idx->stream));
-    return DAB_OK;
-}
-
 extern "C" {
 
 int dab_search_batch_pq(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
                         uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops) {
-    return search_pq_host(idx, queries, nq, k, l_search, beam_width, out_ids, out_dists, out_counts, out_cmps, out_hops, false);
+    return search_pq_host(idx, "dab_search_batch_pq", queries, nq, k, l_search, beam_width,
+                          SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, false, 0);
 }
 
 int dab_search_batch_pq_rerank(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
                                uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops) {
-    return search_pq_host(idx, queries, nq, k, l_search, beam_width, out_ids, out_dists, out_counts, out_cmps, out_hops, true);
+    return search_pq_host(idx, "dab_search_batch_pq_rerank", queries, nq, k, l_search, beam_width,
+                          SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, true, 0);
 }
 
 int dab_search_batch_pq_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
@@ -723,7 +674,8 @@ int dab_search_batch_pq_device(dab_index* idx, const void* d_queries, uint32_t n
 
 int dab_search_batch_sq(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
                         int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops) {
-    return search_pq_host(idx, queries, nq, k, l_search, beam_width, out_ids, out_dists, out_counts, out_cmps, out_hops, rerank != 0, 1);
+    return search_pq_host(idx, "dab_search_batch_sq", queries, nq, k, l_search, beam_width,
+                          SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, rerank != 0, 1);
 }
 
 int dab_search_batch_sq_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,

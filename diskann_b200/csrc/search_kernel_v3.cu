@@ -362,10 +362,11 @@ static int v3_prepare_schema(const dab_index* idx, uint32_t l_search, uint32_t b
     p.warp_smem = (uint32_t)round_up(fixed + (size_t)tbytes, 128);
     out.smem_block = (size_t)p.warp_smem * kV3Warps;
 
+    // cap <= 24: the list fits one register tile of the merge (QT = 4, up to 128 entries)
     using TD = typename S::TD;
-    out.kern = cap <= 128 ? search_kernel_v3<TD, S::KIND, S::POST, 4, false> : search_kernel_v3<TD, S::KIND, S::POST, 8, false>;
+    out.kern = search_kernel_v3<TD, S::KIND, S::POST, 4, false>;
     if constexpr (std::is_same<TD, float>::value) {
-        if (p.fast_nm) out.kern = cap <= 128 ? search_kernel_v3<TD, S::KIND, S::POST, 4, true> : search_kernel_v3<TD, S::KIND, S::POST, 8, true>;
+        if (p.fast_nm) out.kern = search_kernel_v3<TD, S::KIND, S::POST, 4, true>;
     }
     if (cudaFuncSetAttribute(out.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)out.smem_block) != cudaSuccess) {
         cudaGetLastError();

@@ -665,7 +665,7 @@ def test_device_batched_build_is_the_reference_multi_insert(dab, dt, metric, d, 
 
 # ---------------------------------------------------------------- PQ traversal (C4 shape) and C3 shape
 
-@pytest.mark.parametrize("path", ["smem_pivots", "global_lut", "smem_pivots_overflow"])
+@pytest.mark.parametrize("path", ["smem_pivots", "global_lut", "smem_pivots_overflow", "global_lut_overflow"])
 @pytest.mark.parametrize("dt,metric,d,chunks", [(np.int8, O.L2, 128, 32), (np.float32, O.L2, 96, 12), (np.float32, O.INNER_PRODUCT, 64, 16),
                                                 (np.uint8, O.COSINE_NORMALIZED, 40, 7), (np.float32, O.INNER_PRODUCT, 100, 25),
                                                 (np.float16, O.L2, 64, 16)])
@@ -674,10 +674,10 @@ def test_pq_traversal_search_identical_to_oracle(dab, monkeypatch, dt, metric, d
     (providers' QuantAccessor, product.rs:311-340) == the oracle's search with pq_codes set.
     Both kernels are covered: search_kernel_pqs (pivots in shared memory, the default where they fit: chunk
     lengths 4 / 8 / mixed, 32 / 25 / 16 / 12 / 7 chunks) and search_kernel_pq (per-warp table in global memory),
-    and the overflow re-run of the former (a 256-slot visited table)."""
-    if path == "global_lut":
+    and the overflow re-runs of both (a 256-slot visited table; the rerank reads the lists the re-runs wrote)."""
+    if path.startswith("global_lut"):
         monkeypatch.setenv("DAB_TEST_PQ_GLOBAL_LUT", "1")
-    if path == "smem_pivots_overflow":
+    if path.endswith("_overflow"):
         monkeypatch.setenv("DAB_TEST_VISITED_LOG2", "8")
     rng = np.random.default_rng(d + chunks)
     n = 4000
@@ -766,13 +766,17 @@ def sq_quantizer(f32, metric):
     return shift, float(scale), float(ssn), float(mean_norm)
 
 
+@pytest.mark.parametrize("tables", ["sized", "overflow"])
 @pytest.mark.parametrize("dt,metric,d,nbits", [(np.float32, O.L2, 128, 8), (np.float32, O.L2, 100, 4), (np.float32, O.INNER_PRODUCT, 64, 8),
                                                (np.float32, O.INNER_PRODUCT, 96, 4), (np.float16, O.COSINE_NORMALIZED, 48, 2),
                                                (np.uint8, O.L2, 128, 1), (np.int8, O.L2, 72, 2), (np.float32, O.L2, 37, 4)])
-def test_sq_traversal_search_identical_to_oracle(dab, dt, metric, d, nbits):
+def test_sq_traversal_search_identical_to_oracle(dab, monkeypatch, dt, metric, d, nbits, tables):
     """dab_search_batch_sq: greedy search through the scalar-quantized accessor (providers inmem/scalar.rs:449-570):
     rows encoded on the device == SQStore::set_vector restated on the CPU (canonical-front layout, dense N-bit codes),
-    and ids / distance bits / cmps / hops == the oracle's search with sq_rows set, with and without Rerank."""
+    and ids / distance bits / cmps / hops == the oracle's search with sq_rows set, with and without Rerank; also with
+    256-slot visited tables, whose overflowed queries are re-run (the rerank reads the lists the re-runs wrote)."""
+    if tables == "overflow":
+        monkeypatch.setenv("DAB_TEST_VISITED_LOG2", "8")
     rng = np.random.default_rng(d * 10 + nbits)
     n = 4000
     vecs, adj, maxdeg = make_index(rng, dt, O.L2 if metric == O.COSINE_NORMALIZED else metric, n, d, 24, 40)

@@ -96,3 +96,10 @@ def test_no_integer_kernel_for_inner_product_one_minus(kernels):
 def test_frontier_float_kernel_only_for_cosine(kernels):
     kinds = [FLOAT_FAMILIES["frontier_float_kernel"](a)[3] for f, a in kernels if f == "frontier_float_kernel"]
     assert kinds and set(kinds) == {KIND_COS}
+
+
+def test_search_kernel_v3_only_for_one_merge_tile(kernels):
+    """v3_prepare takes lists of L + #start <= 24 only: every search_kernel_v3<T, kind, post, QT, FAST> merges its list in
+    one register tile (QT = 4, up to 128 entries); a kernel with a longer tile could never be launched."""
+    tiles = [a[3] for f, a in kernels if f == "search_kernel_v3"]
+    assert tiles and set(tiles) == {4}
