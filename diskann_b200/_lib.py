@@ -67,6 +67,11 @@ SYMBOLS = {
     "dab_transform_apply": (_i, [_vp, _i, _vp, _u64, _vp]),
     "dab_minmax_compress_transformed": (_i, [_vp, _i, _f, _i, _vp, _u64, _vp, _vp]),
     "dab_minmax_query_distances_transformed": (_i, [_vp, _i, _i, _i, _vp, _u32, _vp, _u64, _vp]),
+    "dab_upload_minmax": (_i, [_vp, _i, _f, _vp, _vp]),
+    "dab_minmax_encode_all": (_i, [_vp]),
+    "dab_minmax_download": (_i, [_vp, _vp]),
+    "dab_search_batch_minmax": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _i, _vp, _vp, _vp, _vp, _vp]),
+    "dab_search_batch_minmax_device": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _i, _vp, _vp, _vp, _vp, _vp]),
     "dab_robust_prune": (_i, [_vp, _vp, _vp, _vp, _vp, _u32, _u32, _u32, _f, _vp, _vp]),
     "dab_build": (_i, [_vp, _u32, _u32, _f, _u32]),
     "dab_flat_knn": (_i, [_vp, _vp, _u32, _u32, _vp, _vp]),

@@ -137,6 +137,7 @@ void dab_destroy(dab_index* idx) {
     search_slots_release(idx);
     comm_release(idx);
     tc_release(idx);
+    minmax_release(idx);
     cudaFree(idx->d_vectors);
     cudaFree(idx->d_adj);
     cudaFree(idx->d_pivots);

@@ -26,6 +26,7 @@ extern std::atomic<uint64_t> g_launches;
 void comm_release(struct ::dab_index* idx);  // replicate.cu
 void tc_release(struct ::dab_index* idx);    // flat_tc.cu
 void search_slots_release(struct ::dab_index* idx);  // search_kernel.cu
+void minmax_release(struct ::dab_index* idx);        // minmax_index.cu
 
 #define DAB_CUDA(expr)                                                                        \
     do {                                                                                      \
@@ -66,7 +67,8 @@ struct Tuning {
 };
 
 // The largest visited set the searches at (l, beam, mode) have seen; later calls size their visited tables from it
-// (search_kernel.cu).  `mode`: which quantized store the traversal reads (0 for full precision and PQ, 1 for SQ).
+// (search_kernel.cu).  `mode`: which quantized store the traversal reads (0 for full precision and PQ, 1 for SQ, 2 for
+// MinMax).
 struct VisitedHint {
     uint32_t l = 0, beam = 0, visited = 0;
     int mode = 0;
@@ -109,6 +111,18 @@ struct dab_index {
     float* d_sq_comp = nullptr;    // [n_total]
     uint32_t sq_row_bytes = 0, sq_stride = 0;
     bool sq_codes_ready = false;
+    // MinMax store (minmax_index.cu; providers common/minmax_repr.rs MinMaxElement<NBITS>): the quantizer (width, grid
+    // scale, its own copy of the transform with the tables on the device) and one row per point: dense codes 16 B-aligned
+    // and zero padded, the compensations {b, n, a, norm_squared} apart
+    int mm_nbits = 0;
+    float mm_grid_scale = 0.0f;
+    uint32_t mm_dim = 0, mm_row_bytes = 0, mm_stride = 0;  // transform output dim, canonical row bytes, device row stride
+    dab_transform* mm_transform = nullptr;                 // NULL: Transform::Null
+    uint32_t* d_mm_tables = nullptr;                       // transform_tables(mm_transform)
+    uint8_t* d_mm_codes = nullptr;                         // [n_total][mm_stride]
+    float4* d_mm_meta = nullptr;                           // [n_total]
+    bool mm_ready = false;
+    dab::Scratch s_mm;                                     // staging of the encode and of the searches' compressed queries
 
     // scratch (grow-only)
     dab::Scratch s_queries, s_ids, s_out, s_out2, s_tables, s_counters, s_stats;
@@ -117,7 +131,7 @@ struct dab_index {
     void* slots[DAB_MAX_SLOTS] = {};  // batches in flight (dab_search_batch_async), search_kernel.cu
 
     // search-side state learned across calls
-    dab::VisitedHint hint, pq_hint;  // full precision; PQ / SQ traversal (visits other nodes: kept apart)
+    dab::VisitedHint hint, pq_hint;  // full precision; PQ / SQ / MinMax traversal (visits other nodes: kept apart)
     uint32_t v3_overflow_l = 0, v3_overflow_beam = 0;      // share of queries that outgrew the shared-memory
     float v3_overflow_frac = 0.0f;                         // tables at (L, beam): search_kernel_v3 is skipped when large
 

@@ -16,28 +16,13 @@
 // norm_squared} (vectors.rs:43-52, 20 bytes) then ceil(dim * NBITS / 8) bytes of codes, value i at bit i * NBITS.
 // HBM-bound byte work: no tensor cores.
 #include "dab_common.cuh"
+#include "minmax.cuh"
 #include "quant_device.cuh"
 #include "transform.cuh"
 
 #include <algorithm>
 
 namespace dab {
-
-constexpr int kMmMeta = 20;
-
-struct MinMaxCompressParams {
-    float grid_scale;
-    uint32_t dim;
-    int nbits;
-    const float* vectors;  // [n][dim]
-    uint64_t n;
-    uint8_t* rows;         // [n][row_bytes]
-    uint32_t row_bytes;
-    uint32_t srow_stride;  // bytes between the staged output rows of a warp (an odd number of words: conflict-free)
-    float* loss;           // [n] or NULL
-    unsigned long long* first_nan;
-    uint32_t warp_smem;    // tile + staged rows
-};
 
 // `walk(f)` calls f(i, v_i) for i = 0 .. dim-1 in index order on the lane's own vector, the warp moving 32 x 32 tiles
 // through shared memory (all lanes must call it together).
@@ -206,16 +191,7 @@ __global__ void __launch_bounds__(256) minmax_distance_kernel(const MinMaxDistan
             if (dx != dy || dx != p.dim) {
                 r = __int_as_float(0x7FC00000);  // UnequalLengths
             } else {
-                // vectors.rs:206-228: term0 + term1_x + term1_y + term2, left to right
-                const float term0 = __fmul_rn(__fmul_rn(xa, ya), (float)ip);
-                const float term1_x = __fmul_rn(xn, yb);
-                const float term1_y = __fmul_rn(yn, xb);
-                const float term2 = __fmul_rn(__fmul_rn(xb, yb), (float)dx);
-                const float v = __fadd_rn(__fadd_rn(__fadd_rn(term0, term1_x), term1_y), term2);
-                if (p.metric == DAB_INNER_PRODUCT) r = -v;
-                else if (p.metric == DAB_L2) r = __fadd_rn(__fadd_rn(__fmul_rn(-2.0f, v), xq), yq);
-                else if (p.metric == DAB_COSINE) r = __fsub_rn(1.0f, __fdiv_rn(v, __fmul_rn(__fsqrt_rn(xq), __fsqrt_rn(yq))));
-                else r = __fsub_rn(1.0f, v);
+                r = minmax_finish(p.metric, ip, dx, xb, xn, xa, xq, yb, yn, ya, yq);
             }
             p.out[i] = r;
         }
@@ -381,9 +357,9 @@ using namespace dab;
 
 static bool mm_bits_ok(int nbits) { return nbits == 1 || nbits == 2 || nbits == 4 || nbits == 8; }
 
-// MinMaxCompressParams for dim-long vectors and the CTA shape of minmax_compress_kernel; false if the staging buffers
-// of one warp do not fit shared memory
-static bool mm_compress_setup(float grid_scale, uint32_t dim, int nbits, uint64_t n, MinMaxCompressParams& p, int& warps, size_t& smem) {
+namespace dab {
+
+bool mm_compress_setup(float grid_scale, uint32_t dim, int nbits, uint64_t n, MinMaxCompressParams& p, int& warps, size_t& smem) {
     memset(&p, 0, sizeof(p));
     p.grid_scale = grid_scale;
     p.dim = dim;
@@ -400,18 +376,19 @@ static bool mm_compress_setup(float grid_scale, uint32_t dim, int nbits, uint64_
     return smem <= 200 * 1024;
 }
 
-// p.vectors, p.rows, p.loss and p.first_nan are device pointers
-static cudaError_t mm_compress_launch(const MinMaxCompressParams& p, int warps, size_t smem) {
+cudaError_t mm_compress_launch(const MinMaxCompressParams& p, int warps, size_t smem, cudaStream_t stream) {
     cudaError_t e = cudaFuncSetAttribute(minmax_compress_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e == cudaSuccess) {
         const uint64_t groups = (p.n + 31) / 32;
         const int grid = (int)std::min<uint64_t>((groups + warps - 1) / warps, 132ull * 8);
-        minmax_compress_kernel<<<grid, warps * 32, smem>>>(p);
+        minmax_compress_kernel<<<grid, warps * 32, smem, stream>>>(p);
         DAB_LAUNCHED();
         e = cudaGetLastError();
     }
     return e;
 }
+
+}  // namespace dab
 
 // the FullQueryMeta kernel, then the distance kernel for p.nbits (p's pointers are device pointers)
 static cudaError_t mm_query_launch(const MinMaxQueryParams& p) {

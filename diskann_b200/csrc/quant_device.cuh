@@ -110,6 +110,22 @@ __device__ __forceinline__ void sq_word(uint32_t a, uint32_t b, bool want_ip, ui
     }
 }
 
+// ------------------------------------------------------------------ MinMax epilogue (minmax/vectors.rs:206-228)
+// The distance between two MinMax vectors x and y of `dim` codes from the exact inner product `ip` of their codes and
+// their compensations {b, n, a, norm_squared}: term0 + term1_x + term1_y + term2 left to right, then the metric's finish.
+__device__ __forceinline__ float minmax_finish(int metric, uint32_t ip, uint32_t dim, float xb, float xn, float xa, float xq, float yb,
+                                               float yn, float ya, float yq) {
+    const float term0 = __fmul_rn(__fmul_rn(xa, ya), (float)ip);
+    const float term1_x = __fmul_rn(xn, yb);
+    const float term1_y = __fmul_rn(yn, xb);
+    const float term2 = __fmul_rn(__fmul_rn(xb, yb), (float)dim);
+    const float v = __fadd_rn(__fadd_rn(__fadd_rn(term0, term1_x), term1_y), term2);
+    if (metric == DAB_INNER_PRODUCT) return -v;
+    if (metric == DAB_L2) return __fadd_rn(__fadd_rn(__fmul_rn(-2.0f, v), xq), yq);
+    if (metric == DAB_COSINE) return __fsub_rn(1.0f, __fdiv_rn(v, __fmul_rn(__fsqrt_rn(xq), __fsqrt_rn(yq))));
+    return __fsub_rn(1.0f, v);
+}
+
 // ------------------------------------------------------------------ PQ table entries from shared-memory pivots
 __device__ __forceinline__ void prefetch_l2(const void* ptr) { asm volatile("prefetch.global.L2 [%0];" ::"l"(ptr)); }
 

@@ -24,6 +24,12 @@
 // popc for 1 bit) and the reference's f32 epilogue.  One lane per candidate, 16 B code loads,
 // the query words broadcast from shared memory; traffic is ceil(dim * N / 8) bytes per candidate
 // (+ 4 B compensation for InnerProduct).
+//
+// MODE 2 — the MinMax store (minmax_index.cu; providers common/minmax_repr.rs:167-336, garnet provider.rs:1170-1358):
+// the batch's queries are compressed before the launch by the store's own transform and quantizer into the rows'
+// layout (the query is &[MinMaxElement<N>]); per candidate the same integer core gives the exact inner product of the
+// codes and minmax_finish the MinMax distance of the index metric (vectors.rs:206-228, all four metrics).  Traffic is
+// ceil(dim * N / 8) code bytes + 16 B of compensations per candidate.
 #include "dab_common.cuh"
 #include "quant_device.cuh"
 #include "search_common.cuh"
@@ -106,6 +112,24 @@ __global__ void __launch_bounds__(kPqWarps * 32) search_kernel_pq(const SearchPa
                     }
                     cd[c] = r;
                 }
+            } else if (MODE == 2) {
+                if (c < n) {
+                    const uint32_t id = cid[c];
+                    const uint4* row = reinterpret_cast<const uint4*>(p.mm_codes + (size_t)id * p.mm_stride);
+                    const uint4* q4 = reinterpret_cast<const uint4*>(qc);
+                    const uint32_t vecs = p.mm_stride >> 4;
+                    uint32_t unused = 0, ip = 0;
+                    switch (p.mm_nbits) {
+                        case 8: sq_row<8>(row, q4, vecs, true, unused, ip); break;
+                        case 4: sq_row<4>(row, q4, vecs, true, unused, ip); break;
+                        case 2: sq_row<2>(row, q4, vecs, true, unused, ip); break;
+                        default: sq_row<1>(row, q4, vecs, true, unused, ip); break;
+                    }
+                    // MinMax distance (vectors.rs:206-228) with the query as x, the row as y
+                    const float4 qm = *reinterpret_cast<const float4*>(qc + (p.mm_stride >> 2));
+                    const float4 rm = __ldg(p.mm_meta + id);
+                    cd[c] = minmax_finish(p.mm_metric, ip, p.mm_dim, qm.x, qm.y, qm.z, qm.w, rm.x, rm.y, rm.z, rm.w);
+                }
             } else if (p.direct_cosine) {
                 // DirectCosine (pq/distance/cosine.rs:16-70; direct_distance_impl, fixed_chunk_pq_table.rs:35-59): the
                 // Resumable V3 cosine (Strategy2x4) accumulated chunk by chunk over the pivots the code selects, 1 - cos
@@ -164,7 +188,7 @@ __global__ void __launch_bounds__(kPqWarps * 32) search_kernel_pq(const SearchPa
 
         // ---- query -> f32 (T: Into<f32>), table build, visited clear
         __syncwarp();
-        for (int e = lane; e < dim; e += 32) {
+        for (int e = lane; MODE != 2 && e < dim; e += 32) {
             float v;
             switch (p.dtype) {
                 case DAB_F32: v = reinterpret_cast<const float*>(p.queries)[(size_t)qidx * dim + e]; break;
@@ -217,6 +241,14 @@ __global__ void __launch_bounds__(kPqWarps * 32) search_kernel_pq(const SearchPa
                 }
                 qc[wd] = acc;
             }
+            __syncwarp();
+        }
+        if (MODE == 2) {
+            // the query compressed by minmax_stage_queries: its code words, then {b, n, a, norm_squared}
+            const uint32_t words = p.mm_stride >> 2;
+            const uint32_t* src = reinterpret_cast<const uint32_t*>(p.mm_qcodes + (size_t)qidx * p.mm_stride);
+            for (uint32_t wd = lane; wd < words; wd += 32) qc[wd] = __ldg(src + wd);
+            if (lane == 0) *reinterpret_cast<float4*>(qc + words) = __ldg(p.mm_qmeta + qidx);
             __syncwarp();
         }
         for (uint32_t t = lane; MODE == 0 && !p.direct_cosine && t < entries; t += 32) {
@@ -497,8 +529,10 @@ static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uin
     // SQStore::distance_computer (providers inmem/scalar.rs:214-226): UnsupportedDistanceMetric
     if (mode == 1 && idx->metric == DAB_COSINE)
         return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_sq: the scalar-quantized store supports L2, InnerProduct and CosineNormalized");
+    if (mode == 2 && (!idx->d_mm_codes || !idx->mm_ready))
+        return fail(DAB_ERR_NOT_READY, "dab_search_batch_minmax: no MinMax rows (dab_upload_minmax with rows, or dab_minmax_encode_all)");
     const uint32_t cap = l_search + idx->n_start;
-    if (cap > 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_pq: L + #start must be <= 1024");
+    if (cap > 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: L + #start must be <= 1024", mode == 2 ? "dab_search_batch_minmax" : "dab_search_batch_pq");
     SearchParamsPq p;
     memset(&p, 0, sizeof(p));
     p.adj = idx->d_adj;
@@ -532,6 +566,15 @@ static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uin
         p.sq_mean_norm = idx->sq_mean_norm;
         p.n_chunks = 0;
     }
+    if (mode == 2) {
+        p.mm_codes = idx->d_mm_codes;
+        p.mm_meta = idx->d_mm_meta;
+        p.mm_stride = idx->mm_stride;
+        p.mm_dim = idx->mm_dim;
+        p.mm_nbits = idx->mm_nbits;
+        p.mm_metric = idx->metric;  // MinMaxElement::query_distance: all four metrics (minmax_repr.rs)
+        p.n_chunks = 0;
+    }
     p.out_ids = d_ids;
     p.out_dists = d_dists;
     p.out_counts = d_counts;
@@ -555,6 +598,7 @@ static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uin
     off += round_up((size_t)beam * 4, 16);
     p.off_qc = (uint32_t)off;
     if (mode == 1) off += idx->sq_stride;
+    if (mode == 2) off += idx->mm_stride + 16;  // the query's code row and its four compensations
     off = round_up(off, 16);
     p.off_nrow = (uint32_t)off;  // search_kernel_pqs: the adjacency row copied one hop ahead
     if (mode == 0) off += 96 * 4;
@@ -575,7 +619,8 @@ static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uin
         warps = (uint32_t)plan.grid * (uint32_t)plan.warps;
     } else {
         if (smem_block > 200 * 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_pq: configuration needs %zu B shared memory per CTA", smem_block);
-        if (mode == 1) kern = cap <= 128 ? search_kernel_pq<4, 1> : cap <= 256 ? search_kernel_pq<8, 1> : cap <= 512 ? search_kernel_pq<16, 1> : search_kernel_pq<32, 1>;
+        if (mode == 2) kern = cap <= 128 ? search_kernel_pq<4, 2> : cap <= 256 ? search_kernel_pq<8, 2> : cap <= 512 ? search_kernel_pq<16, 2> : search_kernel_pq<32, 2>;
+        else if (mode == 1) kern = cap <= 128 ? search_kernel_pq<4, 1> : cap <= 256 ? search_kernel_pq<8, 1> : cap <= 512 ? search_kernel_pq<16, 1> : search_kernel_pq<32, 1>;
         else kern = cap <= 128 ? search_kernel_pq<4, 0> : cap <= 256 ? search_kernel_pq<8, 0> : cap <= 512 ? search_kernel_pq<16, 0> : search_kernel_pq<32, 0>;
         DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_block));
         int per_sm = 0;
@@ -604,6 +649,7 @@ static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uin
         p.list_counts = p.list_ids + (size_t)nq * cap;
         p.list_cap = cap;
     }
+    if (mode == 2 && (rc = minmax_stage_queries(idx, d_queries, nq, &p.mm_qcodes, &p.mm_qmeta))) return rc;
     // global-table passes: the overflowed queries of one are re-run on larger tables in the next
     uint64_t slots = table_slots(idx, idx->pq_hint, l_search, beam, mode);
     Scratch retry;
@@ -686,6 +732,22 @@ int dab_search_batch_sq_device(dab_index* idx, const void* d_queries, uint32_t n
     if (!d_queries || !d_out_ids || !d_out_dists) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_sq_device: NULL argument");
     DAB_CUDA(cudaSetDevice(idx->device));
     return run_search_pq(idx, d_queries, nq, k, l_search, beam_width, d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops, rerank != 0, 1);
+}
+
+int dab_search_batch_minmax(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
+                            int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops) {
+    return search_pq_host(idx, "dab_search_batch_minmax", queries, nq, k, l_search, beam_width,
+                          SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, rerank != 0, 2);
+}
+
+int dab_search_batch_minmax_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
+                                   int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts, uint32_t* d_out_cmps,
+                                   uint32_t* d_out_hops) {
+    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_minmax_device: idx is NULL");
+    if (nq == 0) return DAB_OK;
+    if (!d_queries || !d_out_ids || !d_out_dists) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_minmax_device: NULL argument");
+    DAB_CUDA(cudaSetDevice(idx->device));
+    return run_search_pq(idx, d_queries, nq, k, l_search, beam_width, d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops, rerank != 0, 2);
 }
 
 }  // extern "C"

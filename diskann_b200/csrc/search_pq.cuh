@@ -52,6 +52,13 @@ struct SearchParamsPq {
     // search_kernel_pqs: the pivot table of the CTA in shared memory
     uint32_t piv_stride;  // floats between pivot rows (odd multiple of 4: rows of different centres start in different 16-byte bank groups)
     uint32_t piv_bytes;   // n_centers * piv_stride * 4, the per-warp slices follow
+    // MODE 2: the MinMax store and the batch's queries compressed into the same layout (minmax_stage_queries)
+    const uint8_t* mm_codes;   // [n_total][mm_stride], dense N-bit codes, zero padded to 16 B
+    const float4* mm_meta;     // [n_total] {b, n, a, norm_squared}
+    const uint8_t* mm_qcodes;  // [nq][mm_stride]
+    const float4* mm_qmeta;    // [nq]
+    uint32_t mm_stride, mm_dim;
+    int mm_nbits, mm_metric;
 };
 
 // search_kernel_pqs.cu — the shape of one launch of the shared-memory-pivot kernel
@@ -66,6 +73,10 @@ struct PqsPlan {
 bool pqs_plan(const dab_index* idx, uint32_t warp_smem, uint32_t nq, PqsPlan* out);
 int pqs_launch(dab_index* idx, const SearchParamsPq& p, const PqsPlan& plan, uint32_t cap);
 
+// minmax_index.cu — the query side of the MinMax traversal: the nq queries d_queries (index dtype, device memory) go
+// through as_f32, the store's transform and its compressor on the index's stream, into codes [nq][mm_stride] and
+// compensations [nq] in the store's layout.  Fails naming the first query whose transformed vector holds a NaN.
+int minmax_stage_queries(dab_index* idx, const void* d_queries, uint32_t nq, const uint8_t** d_qcodes, const float4** d_qmeta);
 
 
 }  // namespace dab

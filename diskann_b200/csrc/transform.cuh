@@ -27,4 +27,10 @@ constexpr uint32_t kMaxTransformDim = 32768;
 // NaN.  Uploads the sign and subsample tables for the call and frees them before returning.
 cudaError_t transform_rows(const dab_transform* t, const float* d_src, uint64_t n, float* d_dst, unsigned long long* d_first_nan);
 
+// The sign and subsample tables of `t` as the kernel reads them, in one buffer: signs0, signs1, subsample
+std::vector<uint32_t> transform_tables(const dab_transform* t);
+// transform_rows with the tables already resident (d_tables: transform_tables(t) in device memory), queued on `stream`
+cudaError_t transform_launch(const dab_transform* t, const uint32_t* d_tables, const float* d_src, uint64_t n, float* d_dst,
+                             unsigned long long* d_first_nan, cudaStream_t stream);
+
 }  // namespace dab

@@ -135,48 +135,57 @@ __global__ void __launch_bounds__(256) hadamard_transform_kernel(const Transform
     }
 }
 
-cudaError_t transform_rows(const dab_transform* t, const float* d_src, uint64_t n, float* d_dst, unsigned long long* d_first_nan) {
-    if (n == 0) return cudaSuccess;
-    // the tables travel in one buffer: signs0, signs1, subsample
+std::vector<uint32_t> transform_tables(const dab_transform* t) {
     std::vector<uint32_t> tables(t->signs0);
     tables.insert(tables.end(), t->signs1.begin(), t->signs1.end());
     tables.insert(tables.end(), t->subsample.begin(), t->subsample.end());
     tables.push_back(0);  // never empty
+    return tables;
+}
+
+cudaError_t transform_rows(const dab_transform* t, const float* d_src, uint64_t n, float* d_dst, unsigned long long* d_first_nan) {
+    if (n == 0) return cudaSuccess;
+    const std::vector<uint32_t> tables = transform_tables(t);
     uint32_t* d_tables = nullptr;
     cudaError_t e = cudaMalloc(&d_tables, tables.size() * 4);
     if (e == cudaSuccess) e = cudaMemcpy(d_tables, tables.data(), tables.size() * 4, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) {
-        TransformParams p;
-        memset(&p, 0, sizeof(p));
-        p.input_dim = t->input_dim;
-        p.inner_dim = t->inner_dim;
-        p.output_dim = t->output_dim;
-        p.two_stages = t->kind == DAB_TRANSFORM_DOUBLE_HADAMARD;
-        uint32_t split = 1;
-        while (split <= t->inner_dim / 2) split <<= 1;  // the largest power of two <= inner_dim
-        p.split = split;
-        p.scale = 1.0f / sqrtf((float)split);                                                        // hadamard.rs:132
-        p.rescale = t->subsampled ? sqrtf((float)t->inner_dim / (float)t->output_dim) : 1.0f;        // padding_hadamard.rs:262
-        p.signs0 = d_tables;
-        p.signs1 = d_tables + t->signs0.size();
-        p.subsample = t->subsampled ? d_tables + t->signs0.size() + t->signs1.size() : nullptr;
-        p.src = d_src;
-        p.dst = d_dst;
-        p.n = n;
-        p.warp_floats = t->inner_dim + t->inner_dim / 8 + 8;  // sw(inner_dim - 1) < this
-        p.first_nan = d_first_nan;
-        int warps = 8;
-        while (warps > 1 && (size_t)warps * p.warp_floats * 4 > 96 * 1024) warps >>= 1;
-        const size_t smem = (size_t)warps * p.warp_floats * 4;
-        e = cudaFuncSetAttribute(hadamard_transform_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e == cudaSuccess) {
-            const int grid = (int)std::min<uint64_t>((n + warps - 1) / warps, 132ull * 16);
-            hadamard_transform_kernel<<<grid, warps * 32, smem>>>(p);
-            DAB_LAUNCHED();
-            e = cudaGetLastError();
-        }
-    }
+    if (e == cudaSuccess) e = transform_launch(t, d_tables, d_src, n, d_dst, d_first_nan, 0);
     cudaFree(d_tables);  // synchronizes with the kernel
+    return e;
+}
+
+cudaError_t transform_launch(const dab_transform* t, const uint32_t* d_tables, const float* d_src, uint64_t n, float* d_dst,
+                             unsigned long long* d_first_nan, cudaStream_t stream) {
+    if (n == 0) return cudaSuccess;
+    TransformParams p;
+    memset(&p, 0, sizeof(p));
+    p.input_dim = t->input_dim;
+    p.inner_dim = t->inner_dim;
+    p.output_dim = t->output_dim;
+    p.two_stages = t->kind == DAB_TRANSFORM_DOUBLE_HADAMARD;
+    uint32_t split = 1;
+    while (split <= t->inner_dim / 2) split <<= 1;  // the largest power of two <= inner_dim
+    p.split = split;
+    p.scale = 1.0f / sqrtf((float)split);                                                        // hadamard.rs:132
+    p.rescale = t->subsampled ? sqrtf((float)t->inner_dim / (float)t->output_dim) : 1.0f;        // padding_hadamard.rs:262
+    p.signs0 = d_tables;
+    p.signs1 = d_tables + t->signs0.size();
+    p.subsample = t->subsampled ? d_tables + t->signs0.size() + t->signs1.size() : nullptr;
+    p.src = d_src;
+    p.dst = d_dst;
+    p.n = n;
+    p.warp_floats = t->inner_dim + t->inner_dim / 8 + 8;  // sw(inner_dim - 1) < this
+    p.first_nan = d_first_nan;
+    int warps = 8;
+    while (warps > 1 && (size_t)warps * p.warp_floats * 4 > 96 * 1024) warps >>= 1;
+    const size_t smem = (size_t)warps * p.warp_floats * 4;
+    cudaError_t e = cudaFuncSetAttribute(hadamard_transform_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess) {
+        const int grid = (int)std::min<uint64_t>((n + warps - 1) / warps, 132ull * 16);
+        hadamard_transform_kernel<<<grid, warps * 32, smem, stream>>>(p);
+        DAB_LAUNCHED();
+        e = cudaGetLastError();
+    }
     return e;
 }
 

@@ -518,6 +518,48 @@ class GpuIndex:
                                                     C.c_void_p(d_ids), C.c_void_p(d_dists), C.c_void_p(d_counts or None),
                                                     C.c_void_p(d_cmps or None), C.c_void_p(d_hops or None)))
 
+    # -- MinMax store
+    def upload_minmax(self, nbits, grid_scale=1.0, transform=None, rows=None):
+        """MinMaxElement<NBITS> as the index's vector representation: MinMaxQuantizer(transform or Transform::Null,
+        grid_scale) and (optionally) the canonical-front Data<NBITS> rows of every point including the start points.
+        The index keeps its own copy of `transform`."""
+        out_dim = self.dim if transform is None else transform.output_dim
+        row_bytes = _lib.lib().dab_minmax_row_bytes(out_dim, int(nbits))
+        if rows is not None:
+            rows = np.ascontiguousarray(rows, np.uint8)
+            if row_bytes and rows.shape != (self.n_points + self.n_start, row_bytes):
+                raise DabError(1, f"rows must be (n_points + n_start) x {row_bytes} bytes")
+        check(_lib.lib().dab_upload_minmax(self._h, int(nbits), float(grid_scale), transform._h if transform is not None else None,
+                                           _ptr(rows) if rows is not None else None))
+        self.mm_row_bytes = row_bytes
+
+    def minmax_encode_all(self):
+        check(_lib.lib().dab_minmax_encode_all(self._h))
+
+    def download_minmax(self):
+        rows = np.empty((self.n_points + self.n_start, self.mm_row_bytes), np.uint8)
+        check(_lib.lib().dab_minmax_download(self._h, _ptr(rows)))
+        return rows
+
+    def search_batch_minmax(self, queries, k, l_search, beam_width=1, rerank=False):
+        """KNN::search through the MinMax store; rerank=True adds the full-precision Rerank."""
+        queries = self._queries(queries)
+        nq = queries.shape[0]
+        ids = np.empty((nq, k), np.uint32)
+        dists = np.empty((nq, k), np.float32)
+        counts = np.empty(nq, np.uint32)
+        cmps = np.empty(nq, np.uint32)
+        hops = np.empty(nq, np.uint32)
+        check(_lib.lib().dab_search_batch_minmax(self._h, _ptr(queries), nq, k, l_search, beam_width, int(bool(rerank)),
+                                                 _ptr(ids), _ptr(dists), _ptr(counts), _ptr(cmps), _ptr(hops)))
+        return ids, dists, counts, cmps, hops
+
+    def search_batch_minmax_device(self, d_queries, nq, k, l_search, beam_width, d_ids, d_dists, d_counts=0, d_cmps=0, d_hops=0,
+                                   rerank=False):
+        check(_lib.lib().dab_search_batch_minmax_device(self._h, C.c_void_p(d_queries), nq, k, l_search, beam_width, int(bool(rerank)),
+                                                        C.c_void_p(d_ids), C.c_void_p(d_dists), C.c_void_p(d_counts or None),
+                                                        C.c_void_p(d_cmps or None), C.c_void_p(d_hops or None)))
+
     def pq_encode(self, vectors):
         vectors = np.ascontiguousarray(vectors, np.float32)
         out = np.empty((vectors.shape[0], self.pq_chunks), np.uint8)

@@ -151,6 +151,29 @@ impl<T: Element> GpuIndex<T> {
         Ok(b)
     }
 
+    /// The MinMax store (`MinMaxElement<NBITS>` as the vector representation): `MinMaxQuantizer::new(transform, or
+    /// Transform::Null, grid_scale)`, every resident row encoded on the device.  The index keeps its own copy of the
+    /// transform.
+    pub fn set_minmax_quantizer(&mut self, nbits: i32, grid_scale: f32, transform: Option<&Transform>) -> Result<()> {
+        let t = transform.map_or(std::ptr::null(), |t| t.raw as *const sys::dab_transform);
+        check(unsafe { sys::dab_upload_minmax(self.raw, nbits, grid_scale, t, std::ptr::null()) })?;
+        check(unsafe { sys::dab_minmax_encode_all(self.raw) })
+    }
+
+    /// Traversal over the MinMax rows (queries compressed by the store's quantizer); `rerank` adds
+    /// `Pipeline<FilterStartPoints, Rerank>`.
+    pub fn search_batch_minmax(&self, queries: &[T], k: usize, l_search: u32, beam_width: u32, rerank: bool) -> Result<Batch> {
+        assert_eq!(queries.len() % self.dim, 0);
+        let nq = queries.len() / self.dim;
+        let mut b = Batch { k, ids: vec![0; nq * k], dists: vec![0.0; nq * k], counts: vec![0; nq], cmps: vec![0; nq], hops: vec![0; nq] };
+        check(unsafe {
+            sys::dab_search_batch_minmax(self.raw, queries.as_ptr() as *const c_void, nq as u32, k as u32, l_search, beam_width,
+                                         rerank as i32, b.ids.as_mut_ptr(), b.dists.as_mut_ptr(), b.counts.as_mut_ptr(),
+                                         b.cmps.as_mut_ptr(), b.hops.as_mut_ptr())
+        })?;
+        Ok(b)
+    }
+
     /// One process per GPU: join the communicator described by `id` (from `unique_id()` on rank 0) …
     pub fn comm_init(&mut self, id: &[u8; 128], n_ranks: i32, rank: i32) -> Result<()> {
         check(unsafe { sys::dab_comm_init(self.raw, id.as_ptr() as *const _, n_ranks, rank) })

@@ -356,6 +356,39 @@ int dab_minmax_compress_transformed(const dab_transform* t, int device, float gr
 int dab_minmax_query_distances_transformed(const dab_transform* t, int device, int metric, int nbits, const float* queries,
                                            uint32_t nq, const uint8_t* rows, uint64_t n, float* out);
 
+/* ------------------------------------------------------------------ MinMax store of an index */
+
+/* MinMaxElement<NBITS> as the VectorRepr of an index (diskann-providers/src/common/minmax_repr.rs:167-336), the traversal
+ * store diskann-garnet runs (quantization.rs:229-362, MinMax8Bit; provider.rs:1170-1358): MinMaxQuantizer::new(t, or
+ * Transform::Null(dim) when t is NULL, grid_scale) and one row per point (data + start points).  rows are
+ * (n_points + n_start) x dab_minmax_row_bytes(out_dim, nbits) in the canonical-front Data<NBITS> layout, out_dim =
+ * t ? output_dim(t) : dim; NULL when dab_minmax_encode_all follows.  Bits past dim * nbits in a row's last code byte are
+ * ignored, as the reference's BitSlice never reads them.  Fails naming the entry point for nbits not in {1, 2, 4, 8},
+ * grid_scale <= 0, input_dim(t) != dim, and a row whose stored dim is not out_dim (the first such row).  The store keeps
+ * its own copy of t: the caller may destroy t after the call. */
+int dab_upload_minmax(dab_index* idx, int nbits, float grid_scale, const dab_transform* t, const uint8_t* rows);
+/* For every resident row: T::as_f32, the transform, CompressInto<&[f32], DataMutRef<NBITS>> (quantizer.rs:153-228) — what
+ * garnet's backfill stores.  A transformed row holding a NaN fails the call, naming the first such row; the store then
+ * has no rows until the next successful upload or encode. */
+int dab_minmax_encode_all(dab_index* idx);
+/* the rows back in the canonical-front layout, byte for byte what the store holds */
+int dab_minmax_download(dab_index* idx, uint8_t* rows);
+
+/* KNN::search through the MinMax store (garnet DynamicAccessor, provider.rs:1170-1358: as_f32, then
+ * quantizer.query_computer): queries have the index dtype and go through as_f32, the store's transform and its
+ * compressor at the store's NBITS and grid scale (the query is &[MinMaxElement<N>]); every traversal distance, start
+ * points included, is MinMax{Cosine, IP, L2Squared, CosineNormalized} of the index metric between the compressed query
+ * and the row (vectors.rs:206-455; all four metrics).  rerank = 0: the first k non-start entries of the candidate list
+ * with their MinMax distances; rerank = 1: Pipeline<FilterStartPoints, Rerank> over the full-precision rows (garnet
+ * Rerank, provider.rs:1457-1530), as dab_search_batch_sq.  A query whose transformed vector holds a NaN fails the call,
+ * naming the first such query.  L + #start <= 1024.  Outputs as dab_search_batch. */
+int dab_search_batch_minmax(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                            uint32_t beam_width, int rerank, uint32_t* out_ids, float* out_dists,
+                            uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops);
+int dab_search_batch_minmax_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                                   uint32_t beam_width, int rerank, uint32_t* d_out_ids, float* d_out_dists,
+                                   uint32_t* d_out_counts, uint32_t* d_out_cmps, uint32_t* d_out_hops);
+
 /* ------------------------------------------------------------------ build-side reuse */
 
 /* PruneAccessor::fill + robust_prune (diskann/src/graph/index.rs:2349-2380, 2565-2650;
