@@ -239,46 +239,31 @@ flat_topk_kernel(const float* __restrict__ dist, size_t ld, uint32_t nq, uint32_
     if (lane == 0) top_n[q] = n;
 }
 
-}  // namespace dab
-
-using namespace dab;
-
-extern "C" {
-
-int dab_flat_knn(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t* out_ids, float* out_dists) {
-    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_flat_knn: idx is NULL");
-    if (!idx->vectors_ready) return fail(DAB_ERR_NOT_READY, "dab_flat_knn: vectors not uploaded");
-    if (nq == 0) return DAB_OK;
-    if (!queries || !out_ids || !out_dists) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_flat_knn: NULL argument");
-    if (k == 0 || k > 2048) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_flat_knn: k must be in [1, 2048]");
-    DAB_CUDA(cudaSetDevice(idx->device));
+// The exact scan of nq queries already on the device (index dtype, packed rows) into the device top-k lists d_top_ids /
+// d_top_d ([nq][k]).  dab_flat_knn and the queries dab_flat_knn_tc cannot certify both run it.  Its only scratch is
+// s_out2, so a caller may keep its queries and results in the other buffers.
+int flat_knn_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t* d_top_ids, float* d_top_d) {
     const int dim = (int)idx->dim;
     const uint32_t n = (uint32_t)idx->n_points;  // start points are not data
     cudaStream_t st = idx->stream;
 
-    // queries -> device (floats widened to f32 once)
-    const size_t qraw = (size_t)nq * dim * elem_size(idx->dtype);
-    int rc;
-    if ((rc = idx->s_queries.reserve(qraw + (size_t)nq * dim * 4 + 256))) return rc;
-    uint8_t* d_qraw = (uint8_t*)idx->s_queries.p;
-    float* d_qf = (float*)(d_qraw + round_up(qraw, 256));
-    DAB_CUDA(cudaMemcpyAsync(d_qraw, queries, qraw, cudaMemcpyHostToDevice, st));
-    const void* d_q = d_qraw;
-    if (idx->dtype == DAB_F16) {
-        widen_f16_kernel<<<idx->sm_count * 4, 256, 0, st>>>((const __half*)d_qraw, d_qf, (size_t)nq * dim);
-        DAB_LAUNCHED();
-        d_q = d_qf;
-    }
-
     // row block sized so the distance tile stays around 1 GiB
     uint32_t rb = (uint32_t)std::min<uint64_t>(n, std::max<uint64_t>(1024, ((1ull << 30) / 4) / nq));
     rb = (rb + 31) & ~31u;
-    if ((rc = idx->s_out2.reserve((size_t)nq * rb * 4))) return rc;
-    if ((rc = idx->s_out.reserve((size_t)nq * k * 8 + (size_t)nq * 4))) return rc;
-    float* d_dist = (float*)idx->s_out2.p;
-    uint32_t* d_top_ids = (uint32_t*)idx->s_out.p;
-    float* d_top_d = (float*)(d_top_ids + (size_t)nq * k);
-    uint32_t* d_top_n = (uint32_t*)(d_top_d + (size_t)nq * k);
+    // scratch: [f16 queries widened to f32 | per-query list lengths | distance tile]
+    const size_t qf_bytes = idx->dtype == DAB_F16 ? round_up((size_t)nq * dim * 4, 256) : 0;
+    const size_t tn_bytes = round_up((size_t)nq * 4, 256);
+    int rc;
+    if ((rc = idx->s_out2.reserve(qf_bytes + tn_bytes + (size_t)nq * rb * 4))) return rc;
+    float* d_qf = (float*)idx->s_out2.p;
+    uint32_t* d_top_n = (uint32_t*)((uint8_t*)idx->s_out2.p + qf_bytes);
+    float* d_dist = (float*)((uint8_t*)d_top_n + tn_bytes);
+    const void* d_q = d_queries;
+    if (idx->dtype == DAB_F16) {  // floats widened to f32 once
+        widen_f16_kernel<<<idx->sm_count * 4, 256, 0, st>>>((const __half*)d_queries, d_qf, (size_t)nq * dim);
+        DAB_LAUNCHED();
+        d_q = d_qf;
+    }
     DAB_CUDA(cudaMemsetAsync(d_top_n, 0, (size_t)nq * 4, st));
 
     const bool fast_fits = (size_t)kFlatWarps * kFQ * dim * 4 <= 200 * 1024;
@@ -321,6 +306,31 @@ int dab_flat_knn(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, u
         DAB_LAUNCHED();
         DAB_CUDA(cudaGetLastError());
     }
+    return DAB_OK;
+}
+
+}  // namespace dab
+
+using namespace dab;
+
+extern "C" {
+
+int dab_flat_knn(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t* out_ids, float* out_dists) {
+    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_flat_knn: idx is NULL");
+    if (!idx->vectors_ready) return fail(DAB_ERR_NOT_READY, "dab_flat_knn: vectors not uploaded");
+    if (nq == 0) return DAB_OK;
+    if (!queries || !out_ids || !out_dists) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_flat_knn: NULL argument");
+    if (k == 0 || k > 2048) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_flat_knn: k must be in [1, 2048]");
+    DAB_CUDA(cudaSetDevice(idx->device));
+    cudaStream_t st = idx->stream;
+    const size_t qraw = (size_t)nq * idx->dim * elem_size(idx->dtype);
+    int rc;
+    if ((rc = idx->s_queries.reserve(qraw))) return rc;
+    if ((rc = idx->s_out.reserve((size_t)nq * k * 8))) return rc;
+    uint32_t* d_top_ids = (uint32_t*)idx->s_out.p;
+    float* d_top_d = (float*)(d_top_ids + (size_t)nq * k);
+    DAB_CUDA(cudaMemcpyAsync(idx->s_queries.p, queries, qraw, cudaMemcpyHostToDevice, st));
+    if ((rc = flat_knn_device(idx, idx->s_queries.p, nq, k, d_top_ids, d_top_d))) return rc;
     DAB_CUDA(cudaMemcpyAsync(out_ids, d_top_ids, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, st));
     DAB_CUDA(cudaMemcpyAsync(out_dists, d_top_d, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, st));
     DAB_CUDA(cudaStreamSynchronize(st));

@@ -19,9 +19,39 @@
 //     shared memory 32 columns at a time so that each thread owns one query row, which keeps the KP best
 //     columns of the row in a small per-thread set;
 //   * the KP candidates of every (query, base range) are then re-scored with the exact, reference-order
-//     distance kernel (launch_frontier) and the final top-k is taken by (distance, id) — so the
-//     returned distances are bit-identical to the exact scan and the ids are the exact scan's as long
-//     as the approximate scores (error ~1e-5 relative) do not push a true neighbour below KP - k others.
+//     distance kernel (launch_frontier) and the final top-k is taken by (distance, id);
+//   * every query is then certified (certify_kernel): the range's largest kept score W, less a rigorous bound E
+//     on the approximate score's error, must map to a distance strictly above the query's exact k-th distance, so
+//     no row the selection dropped can belong in the top-k.  The queries that fail (ill-conditioned data: a large
+//     common offset, near-duplicates beyond the slack, fp32 sums past 2^24, norms that underflow, NaN / inf rows,
+//     n < k) are re-run through the exact scan (flat_knn_device) and scattered back.  So the ids and the distance
+//     bits always equal dab_flat_knn's.
+//
+// The error bound E (certify_kernel; u = 2^-24 is fp32 round-to-nearest, gamma(n, v) = n v / (1 - n v)).  For a
+// query q and a row b of the range, with B^2 an upper bound of the range's ||b||^2:
+//   * split residuals: x = hi + lo + r with |hi| <= (1 + 2^-8)|x|, |lo| <= 2^-8 (1 + 2^-8)|x|, |r| <= 2^-16 |x|.  The
+//     three products hi.hi + hi.lo + lo.hi miss lo.lo + hi.r + r.hi + (smaller): at most 2^-14 |q_i b_i| per element,
+//     2^-14 ||q|| ||b|| in all (Cauchy-Schwarz).  i8 / u8 rows are exact in bf16: no split error.
+//   * accumulation: the bf16 products are exact in fp32; kp of them (3 dim for floats) are summed in fp32 by the
+//     tensor cores in an unspecified order, assumed no better than truncation: gamma(kp, 2^-23) times the sum of
+//     |products| <= 1.03 ||q|| ||b||.  For i8 / u8 every partial sum is an integer of magnitude <= ||q|| ||b||, so
+//     the dot is exact while ||q|| B < 2^24.  Flushed subnormals cost at most kp 2^-125 (||q|| + ||b|| + 1).
+//     Together: E_dot.
+//   * epilogue: the row's ||b||^2 in `beta` is an fp32 sum (gamma(dim, u) relative), the fma rounds once (u), and
+//     for cosine 1 / ||b|| comes from rsqrtf (2 ulp): rho = 2^-22 + gamma(dim, u) + u relative.
+//   * the exact distance of the row, which is what the k-th distance is compared with, is itself an fp32 sum in
+//     the reference's order: gamma(dim + 2, u) relative for L2, gamma(dim, u) ||q|| ||b|| for the dot, and
+//     2 gamma(dim, u) + 7u absolute for cosine's sqrt / divide / clamp / 1 - x.
+// Every row the selection dropped scored at least W (W = FLT_MAX when the range kept fewer than KP), so with D_k
+// the exact k-th distance a query is certified when, for every range (a 1.01 factor covers the second-order terms):
+//   L2:                        (||q||^2 + W - E)(1 - gamma(dim + 2, u)) > D_k,  E = 2 E_dot + (gamma(dim, u) + 2u)(B^2 + 2 ||q|| B)
+//   IP:                        W - E > D_k,                                      E = E_dot + gamma(dim, u) ||q|| B
+//   float CosineNormalized:    (1 + W - E) - 2u |1 + W - E| > D_k,              E as for IP
+//   Cosine, int CosNormalized: 1 + (W - E) / ||q|| - (2 gamma(dim, u) + 7u) > D_k,  E = ||q|| ((e + 1) rho + e) + kp 2^-70 (||q|| + 1),
+//                              with e the dot's relative term above (0 for exact integer dots)
+// and the query has k finite distances, ||q||^2 + B^2 + 2 ||q|| B < 2^120 (no score can overflow) and, for cosine,
+// ||q||^2 >= 2^-100.  A cosine row whose fp32 ||b||^2 lies in (0, 2^-100) makes its tile uncertifiable: the exact
+// kernel may or may not treat its norm as zero.  A row whose ||b||^2 is 0 scores 0, which is its exact distance 1.
 #include "dab_common.cuh"
 #include "distance_device.cuh"
 
@@ -34,6 +64,7 @@
 namespace dab {
 
 int launch_frontier(const dab_index* idx, const void* d_queries, uint32_t nq, const uint32_t* d_ids, uint32_t c, float* d_out);
+int flat_knn_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t* d_top_ids, float* d_top_d);
 
 namespace {
 
@@ -122,7 +153,7 @@ __device__ __forceinline__ float elem_f32(const T* p, uint32_t i) {
 template <typename T>
 __global__ void prep_bf16_kernel(const uint8_t* __restrict__ rows, size_t row_stride, uint64_t n, uint32_t dim, uint32_t kp, int is_query,
                                  int score_kind /*0 L2, 1 IP, 2 cosine*/, __nv_bfloat16* __restrict__ out, float* __restrict__ alpha,
-                                 float* __restrict__ beta) {
+                                 float* __restrict__ beta, float* __restrict__ tile_nn) {
     constexpr bool kInt = sizeof(T) == 1;
     const int lane = threadIdx.x & 31;
     const uint64_t warp = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5, nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
@@ -158,6 +189,10 @@ __global__ void prep_bf16_kernel(const uint8_t* __restrict__ rows, size_t row_st
                     alpha[r] = nn > 0.0f ? -rsqrtf(nn) : 0.0f;
                     beta[r] = 0.0f;
                 }
+                // the largest fp32 ||b||^2 of the 128-row tile (certify_kernel); +inf marks a tile no query can be
+                // certified against: a non-finite row, or a cosine row whose norm the exact kernel may take for zero
+                const bool bad = !(nn <= 3.402823466e38f) || (score_kind == 2 && nn > 0.0f && nn < 0x1p-100f);
+                atomicMax(reinterpret_cast<unsigned*>(tile_nn) + r / kBN, bad ? 0x7F800000u : __float_as_uint(nn));
             }
         }
     }
@@ -170,6 +205,7 @@ struct TcParams {
     const float* alpha;
     const float* beta;
     uint32_t* cand;            // [nq][n_splits][kKP]
+    float* worst;              // [nq][n_splits]: the largest kept score, +inf when the range kept fewer than KP
 };
 
 template <int KP>
@@ -319,6 +355,7 @@ flat_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         if (q < p.nq) {
             uint32_t* out = p.cand + ((size_t)q * p.n_splits + split) * KP;
             for (uint32_t e = 0; e < (uint32_t)KP; ++e) out[e] = e < cn ? ci[e * 128] : kNoId;
+            p.worst[(size_t)q * p.n_splits + split] = cn == (uint32_t)KP ? worst : __int_as_float(0x7F800000);
         }
     }
 }
@@ -363,6 +400,81 @@ __global__ void __launch_bounds__(128) cand_topk_kernel(const uint32_t* __restri
     }
 }
 
+__device__ __forceinline__ double gamma_n(double n, double v) { return n * v / (1.0 - n * v); }
+
+// One warp per query: is the candidate top-k provably the exact one?  (E: see the header comment.)  Queries that are
+// not certified are appended to redo[1..], redo[0] counting them.  kind: 0 L2, 1 IP, 2 float CosineNormalized,
+// 3 cosine (-q.b / ||b||).
+template <typename T>
+__global__ void __launch_bounds__(128) certify_kernel(const uint8_t* __restrict__ queries, uint32_t nq, uint32_t dim, uint32_t kp, int kind,
+                                                      const float* __restrict__ top_d, uint32_t k, const float* __restrict__ worst,
+                                                      uint32_t n_splits, const float* __restrict__ tile_nn, uint32_t n_tiles,
+                                                      uint32_t tiles_per_split, uint32_t* __restrict__ redo) {
+    constexpr bool kInt = sizeof(T) == 1;
+    const int lane = threadIdx.x & 31;
+    const uint32_t q = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (q >= nq) return;
+    const T* row = reinterpret_cast<const T*>(queries + (size_t)q * dim * sizeof(T));
+    double qq = 0.0;
+    for (uint32_t d = lane; d < dim; d += 32) {
+        const double x = elem_f32(row, d);
+        qq += x * x;
+    }
+#pragma unroll
+    for (int s = 16; s > 0; s >>= 1) qq += __shfl_xor_sync(0xFFFFFFFFu, qq, s);
+    qq *= 1.0 + dim * 0x1p-52;  // the double sum (of exact squares), rounded up
+    const double u = 0x1p-24, g_dim = gamma_n(dim, u), g_ex = gamma_n(dim + 2.0, u), g_kp = gamma_n(kp, 0x1p-23);
+    const double qn = sqrt(qq) * (1.0 + 0x1p-50);
+    const double dk = top_d[(size_t)q * k + k - 1];
+    bool ok = isfinite(qq) && (kind != 3 || qq >= 0x1p-100);
+    for (uint32_t i = lane; i < k; i += 32) ok = ok && isfinite(top_d[(size_t)q * k + i]);
+    for (uint32_t r = lane; r < n_splits && ok; r += 32) {
+        double b2 = 0.0;
+        for (uint32_t t = r * tiles_per_split; t < min(n_tiles, (r + 1) * tiles_per_split); ++t) b2 = fmax(b2, (double)tile_nn[t]);
+        b2 = (b2 + dim * 0x1p-149) / (1.0 - g_dim);  // bounds every exact ||b||^2 of the range
+        const double B = sqrt(b2) * (1.0 + 0x1p-50);
+        const float wf = worst[(size_t)q * n_splits + r];
+        const double w = wf == __int_as_float(0x7F800000) ? 3.402823466e38 : (double)wf;
+        // relative error of the dot per ||q|| ||b||, and its absolute floor
+        const double e = kInt ? (qn * B < 0x1p24 ? 0.0 : 1.03 * g_kp) : 0x1p-14 + 1.03 * g_kp;
+        const double e_abs = kInt ? 0.0 : kp * 0x1p-125 * (qn + B + 1.0);
+        const double e_dot = e * qn * B + e_abs;
+        double lb;
+        if (kind == 0) {
+            lb = (qq + w - 1.01 * (2.0 * e_dot + (g_dim + 2.0 * u) * (b2 + 2.0 * qn * B))) * (1.0 - g_ex);
+        } else if (kind == 1) {
+            lb = w - 1.01 * (e_dot + g_dim * qn * B);
+        } else if (kind == 2) {
+            const double x = 1.0 + w - 1.01 * (e_dot + g_dim * qn * B);
+            lb = x - 2.0 * u * fabs(x);
+        } else {
+            const double rho = 0x1p-22 + g_dim + u;
+            const double ec = qn * ((e + 1.0) * rho + e) + (kInt ? 0.0 : kp * 0x1p-70 * (qn + 1.0));
+            lb = 1.0 + (w - 1.01 * ec) / qn - 1.01 * (2.0 * g_dim + 7.0 * u);
+        }
+        ok = isfinite(b2) && qq + b2 + 2.0 * qn * B < 0x1p120 && lb > dk;
+    }
+    ok = __all_sync(0xFFFFFFFFu, ok);
+    if (lane == 0 && !ok) redo[1 + atomicAdd(redo, 1u)] = q;
+}
+
+// the raw rows of the queries listed in redo[1..], packed in list order (one block per query)
+__global__ void gather_rows_kernel(const uint8_t* __restrict__ src, size_t row_bytes, const uint32_t* __restrict__ redo, uint8_t* __restrict__ dst) {
+    const uint8_t* s = src + (size_t)redo[1 + blockIdx.x] * row_bytes;
+    uint8_t* d = dst + (size_t)blockIdx.x * row_bytes;
+    for (size_t b = threadIdx.x; b < row_bytes; b += blockDim.x) d[b] = s[b];
+}
+
+// their exact top-k lists back into the rows of the whole batch
+__global__ void scatter_topk_kernel(const uint32_t* __restrict__ redo, uint32_t k, const uint32_t* __restrict__ ids, const float* __restrict__ d,
+                                    uint32_t* __restrict__ out_ids, float* __restrict__ out_d) {
+    const size_t q = redo[1 + blockIdx.x];
+    for (uint32_t i = threadIdx.x; i < k; i += blockDim.x) {
+        out_ids[q * k + i] = ids[(size_t)blockIdx.x * k + i];
+        out_d[q * k + i] = d[(size_t)blockIdx.x * k + i];
+    }
+}
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                   const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
@@ -395,6 +507,16 @@ void launch_prep(int dtype, int grid, cudaStream_t st, A... a) {
     }
 }
 
+template <typename... A>
+void launch_certify(int dtype, int grid, cudaStream_t st, A... a) {
+    switch (dtype) {
+        case DAB_F32: certify_kernel<float><<<grid, 128, 0, st>>>(a...); break;
+        case DAB_F16: certify_kernel<__half><<<grid, 128, 0, st>>>(a...); break;
+        case DAB_I8: certify_kernel<int8_t><<<grid, 128, 0, st>>>(a...); break;
+        default: certify_kernel<uint8_t><<<grid, 128, 0, st>>>(a...); break;
+    }
+}
+
 }  // namespace
 
 void tc_release(dab_index* idx) {
@@ -423,41 +545,53 @@ int dab_flat_knn_tc(dab_index* idx, const void* queries, uint32_t nq, uint32_t k
     const uint32_t kp = (uint32_t)round_up((size_t)(is_int ? dim : 3 * dim), kBK);
     const uint64_t n = idx->n_points;  // start points are not data
     const int score_kind = idx->metric == DAB_L2 ? 0 : idx->metric == DAB_COSINE ? 2 : (is_int && idx->metric == DAB_COSINE_NORMALIZED) ? 2 : 1;
+    const int cert_kind = score_kind == 0 ? 0 : score_kind == 2 ? 3 : idx->metric == DAB_INNER_PRODUCT ? 1 : 2;
+    // geometry: queries padded to whole 128-row tiles; base ranges: enough CTAs to fill the machine, whole 128-column
+    // tiles each (at most 48 ranges: the exact re-scoring handles splits x kKP candidates per query)
+    const uint32_t m_tiles = (nq + kBM - 1) / kBM;
+    const uint32_t n_tiles = (uint32_t)((n + kBN - 1) / kBN);
+    uint32_t splits = std::max<uint32_t>(1, std::min<uint32_t>(std::min<uint32_t>(n_tiles, 48), (uint32_t)(idx->sm_count * 2 + m_tiles - 1) / m_tiles));
+    const uint32_t tiles_per_split = (n_tiles + splits - 1) / splits;
+    splits = (n_tiles + tiles_per_split - 1) / tiles_per_split;
+    const uint32_t kp_sel = k <= 10 ? 16u : (uint32_t)kKP;  // per-range candidates: k plus slack for the approximate scores
+    const uint32_t c = splits * kp_sel;
+    const size_t tsmem = (size_t)4 * c * 8;
+    if (tsmem > 200 * 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_flat_knn_tc: %u candidates per query do not fit the selection kernel", c);
     int rc;
-    // base operand (bf16 split rows + score coefficients): built once per uploaded snapshot
+    // base operand (bf16 split rows + score coefficients + per-tile norm bounds): built once per uploaded snapshot
     if (!idx->d_tc_base || idx->tc_version != idx->vectors_version) {
         tc_release(idx);
         DAB_CUDA(cudaMalloc(&idx->d_tc_base, n * (size_t)kp * 2));
-        DAB_CUDA(cudaMalloc(&idx->d_tc_coef, n * 2 * sizeof(float)));
+        DAB_CUDA(cudaMalloc(&idx->d_tc_coef, (n * 2 + n_tiles) * sizeof(float)));
+        DAB_CUDA(cudaMemsetAsync((float*)idx->d_tc_coef + 2 * n, 0, n_tiles * sizeof(float), st));
         launch_prep(idx->dtype, idx->sm_count * 8, st, (const uint8_t*)idx->d_vectors, idx->row_stride, n, dim, kp, 0, score_kind,
-                    (__nv_bfloat16*)idx->d_tc_base, (float*)idx->d_tc_coef, (float*)idx->d_tc_coef + n);
+                    (__nv_bfloat16*)idx->d_tc_base, (float*)idx->d_tc_coef, (float*)idx->d_tc_coef + n, (float*)idx->d_tc_coef + 2 * n);
         DAB_LAUNCHED();
         DAB_CUDA(cudaGetLastError());
         idx->tc_version = idx->vectors_version;
     }
-    // queries: raw copy (exact re-scoring) + bf16 operand, padded to whole 128-row tiles
-    const uint32_t m_tiles = (nq + kBM - 1) / kBM;
-    const size_t qraw = (size_t)nq * dim * elem_size(idx->dtype);
+    // queries: raw copy (exact re-scoring) + bf16 operand
+    const size_t qrow = (size_t)dim * elem_size(idx->dtype);
+    const size_t qraw = (size_t)nq * qrow;
     const size_t qop = (size_t)m_tiles * kBM * kp * 2;
     if ((rc = idx->s_queries.reserve(round_up(qraw, 256) + qop))) return rc;
     uint8_t* d_qraw = (uint8_t*)idx->s_queries.p;
     __nv_bfloat16* d_qop = (__nv_bfloat16*)(d_qraw + round_up(qraw, 256));
     DAB_CUDA(cudaMemcpyAsync(d_qraw, queries, qraw, cudaMemcpyHostToDevice, st));
     DAB_CUDA(cudaMemsetAsync(d_qop, 0, qop, st));
-    launch_prep(idx->dtype, idx->sm_count * 4, st, (const uint8_t*)d_qraw, (size_t)dim * elem_size(idx->dtype), (uint64_t)nq, dim, kp, 1, score_kind,
-                d_qop, (float*)nullptr, (float*)nullptr);
+    launch_prep(idx->dtype, idx->sm_count * 4, st, (const uint8_t*)d_qraw, qrow, (uint64_t)nq, dim, kp, 1, score_kind, d_qop, (float*)nullptr,
+                (float*)nullptr, (float*)nullptr);
     DAB_LAUNCHED();
-    // base ranges: enough CTAs to fill the machine, whole 128-column tiles each
-    const uint32_t n_tiles = (uint32_t)((n + kBN - 1) / kBN);
-    // (at most 48 ranges: the exact re-scoring handles splits x kKP candidates per query)
-    uint32_t splits = std::max<uint32_t>(1, std::min<uint32_t>(std::min<uint32_t>(n_tiles, 48), (uint32_t)(idx->sm_count * 2 + m_tiles - 1) / m_tiles));
-    const uint32_t tiles_per_split = (n_tiles + splits - 1) / splits;
-    splits = (n_tiles + tiles_per_split - 1) / tiles_per_split;
-    const uint32_t kp_sel = k <= 10 ? 16u : (uint32_t)kKP;  // per-range candidates: k plus slack for the approximate scores
-    const uint32_t c = splits * kp_sel;
-    if ((rc = idx->s_ids.reserve((size_t)nq * c * 4))) return rc;
+    // s_ids: [candidates nq x c | W nq x splits | redo: count, query ids | redo queries' rows | their exact top-k]
+    const size_t o_worst = round_up((size_t)nq * c * 4, 256), o_redo = o_worst + round_up((size_t)nq * splits * 4, 256);
+    const size_t o_rows = o_redo + round_up(((size_t)nq + 1) * 4, 256), o_top = o_rows + round_up(qraw, 256);
+    if ((rc = idx->s_ids.reserve(o_top + (size_t)nq * k * 8))) return rc;
     if ((rc = idx->s_out2.reserve((size_t)nq * c * 4))) return rc;
     if ((rc = idx->s_out.reserve((size_t)nq * k * 8))) return rc;
+    uint8_t* ids_base = (uint8_t*)idx->s_ids.p;
+    uint32_t* d_cand = (uint32_t*)ids_base;
+    float* d_worst = (float*)(ids_base + o_worst);
+    uint32_t* d_redo = (uint32_t*)(ids_base + o_redo);
     CUtensorMap map_a, map_b;
     if ((rc = make_map(&map_a, d_qop, (uint64_t)m_tiles * kBM, kp))) return rc;
     if ((rc = make_map(&map_b, idx->d_tc_base, n, kp))) return rc;
@@ -469,7 +603,8 @@ int dab_flat_knn_tc(dab_index* idx, const void* queries, uint32_t nq, uint32_t k
     p.n_splits = splits;
     p.alpha = (const float*)idx->d_tc_coef;
     p.beta = (const float*)idx->d_tc_coef + n;
-    p.cand = (uint32_t*)idx->s_ids.p;
+    p.cand = d_cand;
+    p.worst = d_worst;
     const size_t smem = 1024 + 2 * (size_t)kStages * kTileBytes + 2 * kBN * 4 + 128 * 33 * 4 + 2 * (size_t)kp_sel * 128 * 4 + 2 * (size_t)kStages * 8;
     auto kern = kp_sel == 16 ? flat_tc_kernel<16> : flat_tc_kernel<32>;
     DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -477,15 +612,33 @@ int dab_flat_knn_tc(dab_index* idx, const void* queries, uint32_t nq, uint32_t k
     DAB_LAUNCHED();
     DAB_CUDA(cudaGetLastError());
     // exact distances of the candidates in the reference's SIMD order, then the final top-k
-    if ((rc = launch_frontier(idx, d_qraw, nq, (const uint32_t*)idx->s_ids.p, c, (float*)idx->s_out2.p))) return rc;
+    if ((rc = launch_frontier(idx, d_qraw, nq, d_cand, c, (float*)idx->s_out2.p))) return rc;
     uint32_t* d_top_ids = (uint32_t*)idx->s_out.p;
     float* d_top_d = (float*)(d_top_ids + (size_t)nq * k);
-    const size_t tsmem = (size_t)4 * c * 8;
-    if (tsmem > 200 * 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_flat_knn_tc: %u candidates per query do not fit the selection kernel", c);
     DAB_CUDA(cudaFuncSetAttribute(cand_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tsmem));
-    cand_topk_kernel<<<(nq + 3) / 4, 128, tsmem, st>>>((const uint32_t*)idx->s_ids.p, (const float*)idx->s_out2.p, nq, c, k, d_top_ids, d_top_d);
+    cand_topk_kernel<<<(nq + 3) / 4, 128, tsmem, st>>>(d_cand, (const float*)idx->s_out2.p, nq, c, k, d_top_ids, d_top_d);
     DAB_LAUNCHED();
     DAB_CUDA(cudaGetLastError());
+    // certify every query; the others go through the exact scan
+    DAB_CUDA(cudaMemsetAsync(d_redo, 0, 4, st));
+    launch_certify(idx->dtype, (nq + 3) / 4, st, (const uint8_t*)d_qraw, nq, dim, kp, cert_kind, (const float*)d_top_d, k, (const float*)d_worst,
+                   splits, (const float*)idx->d_tc_coef + 2 * n, n_tiles, tiles_per_split, d_redo);
+    DAB_LAUNCHED();
+    DAB_CUDA(cudaGetLastError());
+    uint32_t n_redo = 0;
+    DAB_CUDA(cudaMemcpyAsync(&n_redo, d_redo, 4, cudaMemcpyDeviceToHost, st));
+    DAB_CUDA(cudaStreamSynchronize(st));
+    if (n_redo) {
+        uint8_t* d_rows = ids_base + o_rows;
+        uint32_t* d_redo_ids = (uint32_t*)(ids_base + o_top);
+        float* d_redo_d = (float*)(d_redo_ids + (size_t)n_redo * k);
+        gather_rows_kernel<<<n_redo, 128, 0, st>>>(d_qraw, qrow, d_redo, d_rows);
+        DAB_LAUNCHED();
+        if ((rc = flat_knn_device(idx, d_rows, n_redo, k, d_redo_ids, d_redo_d))) return rc;
+        scatter_topk_kernel<<<n_redo, 32, 0, st>>>(d_redo, k, d_redo_ids, d_redo_d, d_top_ids, d_top_d);
+        DAB_LAUNCHED();
+        DAB_CUDA(cudaGetLastError());
+    }
     DAB_CUDA(cudaMemcpyAsync(out_ids, d_top_ids, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, st));
     DAB_CUDA(cudaMemcpyAsync(out_dists, d_top_d, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, st));
     DAB_CUDA(cudaStreamSynchronize(st));

@@ -424,9 +424,10 @@ int dab_flat_knn(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, u
  * ||x||^2 + ||y||^2 expansion): bf16 operands (f32 / f16 rows as a 3-product hi/lo split, i8 / u8 exact),
  * fp32 accumulation in registers,
  * fused score expansion and per-row candidate selection in the epilogue; the candidates are then
- * re-scored with the exact reference-order kernel, so out_dists are bit-identical to dab_flat_knn and
- * out_ids equal it unless approximate scores (~1e-5 relative) displace a true neighbour by more than
- * the selection slack.  k <= 24. */
+ * re-scored with the exact reference-order kernel.  Each query is then certified against a rigorous bound
+ * on the approximate scores' error; the queries that cannot be (ill-conditioned data, NaN / inf rows,
+ * n < k) are re-run through the exact scan.  So out_ids and out_dists always equal dab_flat_knn's.
+ * k <= 24. */
 int dab_flat_knn_tc(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t* out_ids,
                     float* out_dists);
 

@@ -870,6 +870,7 @@ void orc_bruteforce_knn(int dtype, int metric, uint32_t dim, const void* base, u
             for (uint64_t i = 0; i < n; ++i) {
                 float d = orc_distance(ORC_FLAVOUR_AVX2, dq, dtype, metric, q,
                                        (const char*)base + i * row_stride, dim, nullptr);
+                if (d != d) continue;  // NaN is never a neighbour (neighbor/queue.rs:131-134)
                 std::pair<float, uint32_t> e(d, (uint32_t)i);
                 if (heap.size() < k) {
                     heap.push_back(e);
