@@ -153,6 +153,7 @@ void dab_destroy(dab_index* idx) {
     idx->s_tables.release();
     idx->s_counters.release();
     idx->s_stats.release();
+    idx->s_stage.release();
     idx->h_stage.release();
     idx->h_counters.release();
     if (idx->own_stream) cudaStreamDestroy(idx->own_stream);

@@ -122,10 +122,10 @@ struct dab_index {
     uint8_t* d_mm_codes = nullptr;                         // [n_total][mm_stride]
     float4* d_mm_meta = nullptr;                           // [n_total]
     bool mm_ready = false;
-    dab::Scratch s_mm;                                     // staging of the encode and of the searches' compressed queries
 
     // scratch (grow-only)
     dab::Scratch s_queries, s_ids, s_out, s_out2, s_tables, s_counters, s_stats;
+    dab::Scratch s_stage;  // MinMax upload / encode / download staging, and the SQ and MinMax searches' compressed queries
     dab::Scratch h_stage;  // pinned host staging
     dab::Scratch h_counters;  // pinned: the four counters a search pass reports
     void* slots[DAB_MAX_SLOTS] = {};  // batches in flight (dab_search_batch_async), search_kernel.cu

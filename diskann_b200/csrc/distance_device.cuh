@@ -34,6 +34,8 @@ constexpr unsigned kFull = 0xFFFFFFFFu;
 
 __device__ __forceinline__ float to_f32(float v) { return v; }
 __device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
+__device__ __forceinline__ float to_f32(int8_t v) { return (float)v; }
+__device__ __forceinline__ float to_f32(uint8_t v) { return (float)v; }
 
 __device__ __forceinline__ float ldg_elem(const float* p) { return __ldg(p); }
 __device__ __forceinline__ float ldg_elem(const __half* p) {

@@ -22,11 +22,6 @@ namespace dab {
 
 namespace {
 
-__device__ __forceinline__ float widen(float v) { return v; }
-__device__ __forceinline__ float widen(__half v) { return __half2float(v); }
-__device__ __forceinline__ float widen(int8_t v) { return (float)v; }
-__device__ __forceinline__ float widen(uint8_t v) { return (float)v; }
-
 // T::as_f32: rows of `dim` elements, src_stride bytes apart -> dense [n][dim] f32
 template <typename T>
 __global__ void __launch_bounds__(256) mm_widen_kernel(const uint8_t* __restrict__ src, size_t src_stride, uint64_t n, uint32_t dim,
@@ -34,7 +29,7 @@ __global__ void __launch_bounds__(256) mm_widen_kernel(const uint8_t* __restrict
     const uint64_t total = n * dim;
     for (uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; t < total; t += (uint64_t)gridDim.x * blockDim.x) {
         const uint64_t r = t / dim;
-        dst[t] = widen(reinterpret_cast<const T*>(src + r * src_stride)[t - r * dim]);
+        dst[t] = to_f32(reinterpret_cast<const T*>(src + r * src_stride)[t - r * dim]);
     }
 }
 
@@ -161,14 +156,13 @@ void minmax_release(dab_index* idx) {
     idx->mm_transform = nullptr;
     idx->mm_nbits = 0;
     idx->mm_ready = false;
-    idx->s_mm.release();
 }
 
 int minmax_stage_queries(dab_index* idx, const void* d_queries, uint32_t nq, const uint8_t** d_qcodes, const float4** d_qmeta) {
     int rc;
     const size_t codes_off = staging_bytes(idx, nq), meta_off = codes_off + round_up((size_t)nq * idx->mm_stride, 256);
-    if ((rc = idx->s_mm.reserve(meta_off + (size_t)nq * 16))) return rc;
-    uint8_t* base = (uint8_t*)idx->s_mm.p;
+    if ((rc = idx->s_stage.reserve(meta_off + (size_t)nq * 16))) return rc;
+    uint8_t* base = (uint8_t*)idx->s_stage.p;
     const Staging s = staging_layout(idx, nq, base);
     uint8_t* qcodes = base + codes_off;
     float4* qmeta = (float4*)(base + meta_off);
@@ -237,8 +231,8 @@ int dab_upload_minmax(dab_index* idx, int nbits, float grid_scale, const dab_tra
     const uint64_t slab = std::max<uint64_t>(1, std::min<uint64_t>(total, (256ull << 20) / in_stride));
     const size_t flag_off = round_up(slab * in_stride, 256);
     int rc;
-    if ((rc = idx->s_mm.reserve(flag_off + 8))) return rc;
-    uint8_t* stage = (uint8_t*)idx->s_mm.p;
+    if ((rc = idx->s_stage.reserve(flag_off + 8))) return rc;
+    uint8_t* stage = (uint8_t*)idx->s_stage.p;
     unsigned long long* d_bad = (unsigned long long*)(stage + flag_off);
     for (uint64_t first = 0; first < total; first += slab) {
         const uint64_t cnt = std::min(slab, total - first);
@@ -273,8 +267,8 @@ int dab_minmax_encode_all(dab_index* idx) {
     const uint64_t total = idx->n_total();
     const uint64_t per_row = (uint64_t)(idx->dim + (idx->mm_transform ? idx->mm_dim : 0)) * 4 + idx->mm_row_bytes;
     const uint64_t slab = std::max<uint64_t>(1, std::min<uint64_t>(total, (256ull << 20) / per_row));
-    if ((rc = idx->s_mm.reserve(staging_bytes(idx, slab)))) return rc;
-    const Staging s = staging_layout(idx, slab, (uint8_t*)idx->s_mm.p);
+    if ((rc = idx->s_stage.reserve(staging_bytes(idx, slab)))) return rc;
+    const Staging s = staging_layout(idx, slab, (uint8_t*)idx->s_stage.p);
     for (uint64_t first = 0; first < total; first += slab) {
         const uint64_t cnt = std::min(slab, total - first);
         DAB_CUDA(cudaMemsetAsync(s.flag, 0xFF, 8, idx->stream));
@@ -305,14 +299,14 @@ int dab_minmax_download(dab_index* idx, uint8_t* rows) {
     const uint64_t total = idx->n_total();
     const uint64_t out_stride = idx->mm_row_bytes;
     const uint64_t slab = std::max<uint64_t>(1, std::min<uint64_t>(total, (256ull << 20) / out_stride));
-    if ((rc = idx->s_mm.reserve(slab * out_stride))) return rc;
+    if ((rc = idx->s_stage.reserve(slab * out_stride))) return rc;
     for (uint64_t first = 0; first < total; first += slab) {
         const uint64_t cnt = std::min(slab, total - first);
         mm_join_kernel<<<grid_for(idx, cnt * out_stride), 256, 0, idx->stream>>>(idx->d_mm_codes + first * idx->mm_stride, idx->d_mm_meta + first, cnt,
-                                                                                 idx->mm_row_bytes, idx->mm_stride, idx->mm_dim, (uint8_t*)idx->s_mm.p);
+                                                                                 idx->mm_row_bytes, idx->mm_stride, idx->mm_dim, (uint8_t*)idx->s_stage.p);
         DAB_LAUNCHED();
         DAB_CUDA(cudaGetLastError());
-        DAB_CUDA(cudaMemcpyAsync(rows + first * out_stride, idx->s_mm.p, cnt * out_stride, cudaMemcpyDeviceToHost, idx->stream));
+        DAB_CUDA(cudaMemcpyAsync(rows + first * out_stride, idx->s_stage.p, cnt * out_stride, cudaMemcpyDeviceToHost, idx->stream));
         DAB_CUDA(cudaStreamSynchronize(idx->stream));
     }
     return DAB_OK;

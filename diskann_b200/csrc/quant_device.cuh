@@ -1,5 +1,6 @@
 // quant_device.cuh — thread-serial emulation of the reference's simd_op for short f32 chunks
-// (PQ LUT entries, encode), shared by quant_kernels.cu and search_kernel_pq.cu.
+// (PQ LUT entries, encode), the packed-code integer cores, the scalar quantizer and the SQ / MinMax
+// epilogues, shared by quant_kernels.cu, sq_index.cu and search_kernel_pq.cu.
 #pragma once
 
 #include "distance_device.cuh"
@@ -108,6 +109,31 @@ __device__ __forceinline__ void sq_word(uint32_t a, uint32_t b, bool want_ip, ui
             l2 = __dp4a(d, d, l2);
         }
     }
+}
+
+// ------------------------------------------------------------------ scalar quantizer (scalar/quantizer.rs:190-239, 407-430)
+// The code of one value: (v - shift) * inverse_scale (= maxv / scale), f32::clamp to [0, maxv] (keeps NaN), rounded half
+// away from zero.  A NaN code packs as 0.
+__device__ __forceinline__ float sq_code(float v, float shift, float inverse_scale, float maxv) {
+    const float t = __fmul_rn(__fsub_rn(v, shift), inverse_scale);
+    return roundf(t != t ? t : (t < 0.0f ? 0.0f : (t > maxv ? maxv : t)));
+}
+
+// The compensation of a vector from `dot`, the sequential FMA chain of its codes with the shift in dimension order
+// (inverse_bit_scale = 1 / maxv).
+__device__ __forceinline__ float sq_compensation(float scale, float inverse_bit_scale, float dot) {
+    return __fmul_rn(__fmul_rn(scale, inverse_bit_scale), dot);
+}
+
+// Compensated{SquaredL2, IP, CosineNormalized} (scalar/vectors.rs:206-237, 310-376, 380-460) of two code vectors x and y
+// from the exact integer cores of their codes; mul = bit_scale * scale^2 (AsFunctor, scalar/quantizer.rs:316-335).  Only
+// InnerProduct reads the compensations.
+__device__ __forceinline__ float sq_finish(int metric, uint32_t l2, uint32_t ip, float mul, float shift_square_norm, float comp_x,
+                                           float comp_y) {
+    if (metric == DAB_INNER_PRODUCT) return -__fadd_rn(__fmaf_rn(mul, (float)ip, shift_square_norm), __fadd_rn(comp_y, comp_x));
+    const float l = __fmul_rn(mul, (float)l2);
+    if (metric == DAB_L2) return l;
+    return __fsub_rn(1.0f, __fsub_rn(1.0f, __fdiv_rn(l, 2.0f)));
 }
 
 // ------------------------------------------------------------------ MinMax epilogue (minmax/vectors.rs:206-228)

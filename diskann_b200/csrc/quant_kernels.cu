@@ -329,14 +329,12 @@ sq_compress_kernel(const float* __restrict__ shift, float scale, uint32_t dim, i
     for (uint64_t v = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; v < n; v += (uint64_t)gridDim.x * blockDim.x) {
         float dot = 0.0f;
         for (uint32_t i = 0; i < dim; ++i) {
-            const float f = vectors[v * dim + i], s = shift[i];
-            float t = __fmul_rn(__fsub_rn(f, s), inverse_scale);
-            float code = t != t ? t : (t < 0.0f ? 0.0f : (t > maxv ? maxv : t));  // f32::clamp keeps NaN
-            code = roundf(code);                                                  // half away from zero
+            const float s = shift[i];
+            const float code = sq_code(vectors[v * dim + i], s, inverse_scale, maxv);
             dot = __fmaf_rn(code, s, dot);
             codes[v * dim + i] = code != code ? (uint8_t)0 : (uint8_t)code;
         }
-        comp[v] = __fmul_rn(__fmul_rn(scale, inverse_bit_scale), dot);
+        comp[v] = sq_compensation(scale, inverse_bit_scale, dot);
     }
 }
 
@@ -362,21 +360,7 @@ sq_distance_kernel(int metric, int nbits, float scale_squared, float shift_squar
         }
         l2 = __reduce_add_sync(kFull, l2);
         ip = __reduce_add_sync(kFull, ip);
-        if (lane == 0) {
-            float r;
-            if (metric == DAB_L2) {
-                r = __fmul_rn(__fmul_rn(bit_scale, scale_squared), (float)l2);
-            } else if (metric == DAB_INNER_PRODUCT) {
-                float m = __fadd_rn(__fmaf_rn(__fmul_rn(bit_scale, scale_squared), (float)ip, shift_square_norm),
-                                    __fadd_rn(comp_y[i], comp_x[i]));
-                r = -m;
-            } else {
-                float l = __fmul_rn(__fmul_rn(bit_scale, scale_squared), (float)l2);
-                float mathematical = __fsub_rn(1.0f, __fdiv_rn(l, 2.0f));
-                r = __fsub_rn(1.0f, mathematical);
-            }
-            out[i] = r;
-        }
+        if (lane == 0) out[i] = sq_finish(metric, l2, ip, __fmul_rn(bit_scale, scale_squared), shift_square_norm, comp_x[i], comp_y[i]);
     }
 }
 

@@ -1,5 +1,5 @@
 // search_kernel_pq.cu — batched greedy search whose traversal distances come from a quantized store:
-// PQ ADC lookups (MODE 0) or scalar-quantized codes (MODE 1, see the SQ notes below).
+// PQ ADC lookups (MODE 0), scalar-quantized codes (MODE 1) or MinMax codes (MODE 2; see the notes below).
 //
 // Restates the providers' quant accessor (diskann-providers/src/model/graph/provider/async_/
 // inmem/product.rs:311-340: expand_beam with `computer.evaluate_similarity(aux_vectors[i])`)
@@ -15,21 +15,18 @@
 //   * visited set, sorted list and post-processing are the shared exact helpers.
 // No tensor cores: LUT gather + byte loads, HBM traffic is n_chunks code bytes per candidate.
 //
-// MODE 1 — the scalar-quantized accessor (providers inmem/scalar.rs:449-570): the query is
-// compressed once per search with the store's own quantizer (SQStore::query_computer, :227-253:
-// as_f32, rescale to the mean norm for InnerProduct, ScalarQuantizer::compress) into the same
-// dense N-bit layout as the rows (bits/slice.rs:261-323), and every candidate distance is
-// Compensated{SquaredL2, IP, CosineNormalized} (scalar/vectors.rs:206-460): an exact integer core
-// over the packed words (bits/distances.rs:397, 979 — here vabsdiffu4 + dp4a on masked fields,
-// popc for 1 bit) and the reference's f32 epilogue.  One lane per candidate, 16 B code loads,
-// the query words broadcast from shared memory; traffic is ceil(dim * N / 8) bytes per candidate
-// (+ 4 B compensation for InnerProduct).
-//
-// MODE 2 — the MinMax store (minmax_index.cu; providers common/minmax_repr.rs:167-336, garnet provider.rs:1170-1358):
-// the batch's queries are compressed before the launch by the store's own transform and quantizer into the rows'
-// layout (the query is &[MinMaxElement<N>]); per candidate the same integer core gives the exact inner product of the
-// codes and minmax_finish the MinMax distance of the index metric (vectors.rs:206-228, all four metrics).  Traffic is
-// ceil(dim * N / 8) code bytes + 16 B of compensations per candidate.
+// MODE 1 and MODE 2 — the two stores of dense N-bit code rows (bits/slice.rs:261-323), 16 B aligned, compensations
+// apart.  Before the launch the batch's queries are compressed by the store's own quantizer into the rows' layout
+// (sq_stage_queries, minmax_stage_queries); the warp copies its query's code words to shared memory.  Per candidate,
+// one lane runs the exact integer core over the packed words (bits/distances.rs:397, 979 — here vabsdiffu4 + dp4a on
+// masked fields, popc for 1 bit) with 16 B code loads, then the store's f32 epilogue:
+//   * MODE 1, the scalar-quantized accessor (providers inmem/scalar.rs:449-570; the query from SQStore::query_computer,
+//     :227-253): sq_finish, Compensated{SquaredL2, IP, CosineNormalized} (scalar/vectors.rs:206-460).  Traffic is
+//     ceil(dim * N / 8) bytes per candidate (+ 4 B compensation for InnerProduct).
+//   * MODE 2, the MinMax store (minmax_index.cu; providers common/minmax_repr.rs:167-336, garnet provider.rs:1170-1358;
+//     the query is &[MinMaxElement<N>] behind the store's transform): minmax_finish, the MinMax distance of the index
+//     metric from the codes' inner product (vectors.rs:206-228, all four metrics).  Traffic is ceil(dim * N / 8) code
+//     bytes + 16 B of compensations per candidate.
 #include "dab_common.cuh"
 #include "quant_device.cuh"
 #include "search_common.cuh"
@@ -66,7 +63,7 @@ __global__ void __launch_bounds__(kPqWarps * 32) search_kernel_pq(const SearchPa
     uint32_t* cid = reinterpret_cast<uint32_t*>(base + p.off_cid);
     float* cd = reinterpret_cast<float*>(base + p.off_cd);
     uint32_t* beam_ids = reinterpret_cast<uint32_t*>(base + p.off_beam);
-    uint32_t* qc = reinterpret_cast<uint32_t*>(base + p.off_qc);  // MODE 1: the query's packed codes
+    uint32_t* qc = reinterpret_cast<uint32_t*>(base + p.off_qc);  // MODE 1 / 2: the query's packed codes
     float q_comp = 0.0f;
 
     const uint32_t warp_slot = blockIdx.x * kPqWarps + wib;
@@ -82,53 +79,30 @@ __global__ void __launch_bounds__(kPqWarps * 32) search_kernel_pq(const SearchPa
     auto adc = [&](uint32_t n) {
         for (uint32_t c0 = 0; c0 < n; c0 += 32) {
             const uint32_t c = c0 + lane;
-            if (MODE == 1) {
+            if (MODE != 0) {
                 if (c < n) {
                     const uint32_t id = cid[c];
-                    const uint4* row = reinterpret_cast<const uint4*>(p.sq_codes + (size_t)id * p.sq_stride);
+                    const uint4* row = reinterpret_cast<const uint4*>(p.row_codes + (size_t)id * p.code_stride);
                     const uint4* q4 = reinterpret_cast<const uint4*>(qc);
-                    const uint32_t vecs = p.sq_stride >> 4;
-                    const bool want_ip = p.sq_metric == DAB_INNER_PRODUCT;
+                    const uint32_t vecs = p.code_stride >> 4;
+                    const bool want_ip = MODE == 2 || p.code_metric == DAB_INNER_PRODUCT;  // MinMax: every metric
                     uint32_t l2 = 0, ip = 0;
-                    switch (p.sq_nbits) {
+                    switch (p.code_nbits) {
                         case 8: sq_row<8>(row, q4, vecs, want_ip, l2, ip); break;
                         case 4: sq_row<4>(row, q4, vecs, want_ip, l2, ip); break;
                         case 2: sq_row<2>(row, q4, vecs, want_ip, l2, ip); break;
                         default: sq_row<1>(row, q4, vecs, want_ip, l2, ip); break;
                     }
-                    // epilogues: scalar/vectors.rs:206-237 (L2), 310-376 (IP), 380-460 (CosineNormalized)
-                    const float ibs = __fdiv_rn(1.0f, (float)((1u << p.sq_nbits) - 1u));
-                    const float bit_scale = __fmul_rn(ibs, ibs);
-                    const float mul = __fmul_rn(bit_scale, p.sq_scale_squared);
-                    float r;
-                    if (want_ip) {
-                        const float m = __fadd_rn(__fmaf_rn(mul, (float)ip, p.sq_shift_square_norm), __fadd_rn(__ldg(p.sq_comp + id), q_comp));
-                        r = -m;
-                    } else if (p.sq_metric == DAB_L2) {
-                        r = __fmul_rn(mul, (float)l2);
+                    // the query as x, the row as y; only InnerProduct loads the row's SQ compensation
+                    if (MODE == 1) {
+                        const float ibs = __fdiv_rn(1.0f, (float)((1u << p.code_nbits) - 1u));
+                        const float mul = __fmul_rn(__fmul_rn(ibs, ibs), p.sq_scale_squared);
+                        cd[c] = sq_finish(p.code_metric, l2, ip, mul, p.sq_shift_square_norm, q_comp, want_ip ? __ldg(p.sq_comp + id) : 0.0f);
                     } else {
-                        const float l = __fmul_rn(mul, (float)l2);
-                        r = __fsub_rn(1.0f, __fsub_rn(1.0f, __fdiv_rn(l, 2.0f)));
+                        const float4 qm = *reinterpret_cast<const float4*>(qc + (p.code_stride >> 2));
+                        const float4 rm = __ldg(p.mm_meta + id);
+                        cd[c] = minmax_finish(p.code_metric, ip, p.mm_dim, qm.x, qm.y, qm.z, qm.w, rm.x, rm.y, rm.z, rm.w);
                     }
-                    cd[c] = r;
-                }
-            } else if (MODE == 2) {
-                if (c < n) {
-                    const uint32_t id = cid[c];
-                    const uint4* row = reinterpret_cast<const uint4*>(p.mm_codes + (size_t)id * p.mm_stride);
-                    const uint4* q4 = reinterpret_cast<const uint4*>(qc);
-                    const uint32_t vecs = p.mm_stride >> 4;
-                    uint32_t unused = 0, ip = 0;
-                    switch (p.mm_nbits) {
-                        case 8: sq_row<8>(row, q4, vecs, true, unused, ip); break;
-                        case 4: sq_row<4>(row, q4, vecs, true, unused, ip); break;
-                        case 2: sq_row<2>(row, q4, vecs, true, unused, ip); break;
-                        default: sq_row<1>(row, q4, vecs, true, unused, ip); break;
-                    }
-                    // MinMax distance (vectors.rs:206-228) with the query as x, the row as y
-                    const float4 qm = *reinterpret_cast<const float4*>(qc + (p.mm_stride >> 2));
-                    const float4 rm = __ldg(p.mm_meta + id);
-                    cd[c] = minmax_finish(p.mm_metric, ip, p.mm_dim, qm.x, qm.y, qm.z, qm.w, rm.x, rm.y, rm.z, rm.w);
                 }
             } else if (p.direct_cosine) {
                 // DirectCosine (pq/distance/cosine.rs:16-70; direct_distance_impl, fixed_chunk_pq_table.rs:35-59): the
@@ -188,7 +162,7 @@ __global__ void __launch_bounds__(kPqWarps * 32) search_kernel_pq(const SearchPa
 
         // ---- query -> f32 (T: Into<f32>), table build, visited clear
         __syncwarp();
-        for (int e = lane; MODE != 2 && e < dim; e += 32) {
+        for (int e = lane; MODE == 0 && e < dim; e += 32) {
             float v;
             switch (p.dtype) {
                 case DAB_F32: v = reinterpret_cast<const float*>(p.queries)[(size_t)qidx * dim + e]; break;
@@ -200,55 +174,14 @@ __global__ void __launch_bounds__(kPqWarps * 32) search_kernel_pq(const SearchPa
         }
         for (uint32_t i = lane; i < nbk; i += 32) store_empty_bucket(table + (size_t)i * 8);
         __syncwarp();
-        if (MODE == 1) {
-            // rescale (scalar/quantizer.rs:300-310): InnerProduct::evaluate(x, x), sqrt, x *= to_norm / norm
-            if (p.sq_metric == DAB_INNER_PRODUCT && p.sq_mean_norm != 0.0f) {
-                float norm = 0.0f;
-                if (lane == 0) norm = __fsqrt_rn(thread_simd_l2ip<KIND_IP>(qf, qf, dim));
-                norm = __shfl_sync(kFull, norm, 0);
-                if (norm != 0.0f) {
-                    const float sc = __fdiv_rn(p.sq_mean_norm, norm);
-                    for (int e = lane; e < dim; e += 32) qf[e] = __fmul_rn(qf[e], sc);
-                }
-                __syncwarp();
-            }
-            // ScalarQuantizer::compress (scalar/quantizer.rs:190-239): codes in parallel ...
-            const float maxv = (float)((1u << p.sq_nbits) - 1u);
-            const float inverse_scale = __fdiv_rn(maxv, p.sq_scale);
-            for (int e = lane; e < dim; e += 32) {
-                const float t = __fmul_rn(__fsub_rn(qf[e], __ldg(p.sq_shift + e)), inverse_scale);
-                const float code = t != t ? t : (t < 0.0f ? 0.0f : (t > maxv ? maxv : t));
-                qf[e] = roundf(code);
-            }
-            __syncwarp();
-            // ... the compensation is one sequential FMA chain over the dimensions (:407-430)
-            if (lane == 0) {
-                float dot = 0.0f;
-                for (int e = 0; e < dim; ++e) dot = __fmaf_rn(qf[e], __ldg(p.sq_shift + e), dot);
-                q_comp = __fmul_rn(__fmul_rn(p.sq_scale, __fdiv_rn(1.0f, maxv)), dot);
-            }
-            q_comp = __shfl_sync(kFull, q_comp, 0);
-            // dense packing, value i at bit i * nbits (bits/slice.rs:261-305); padding words are zero
-            const uint32_t per_word = 32u / (uint32_t)p.sq_nbits;
-            for (uint32_t wd = lane; wd < (p.sq_stride >> 2); wd += 32) {
-                uint32_t acc = 0;
-                for (uint32_t j = 0; j < per_word; ++j) {
-                    const uint32_t e = wd * per_word + j;
-                    if (e < (uint32_t)dim) {
-                        const float c = qf[e];
-                        acc |= (c != c ? 0u : (uint32_t)c) << (j * (uint32_t)p.sq_nbits);
-                    }
-                }
-                qc[wd] = acc;
-            }
-            __syncwarp();
-        }
-        if (MODE == 2) {
-            // the query compressed by minmax_stage_queries: its code words, then {b, n, a, norm_squared}
-            const uint32_t words = p.mm_stride >> 2;
-            const uint32_t* src = reinterpret_cast<const uint32_t*>(p.mm_qcodes + (size_t)qidx * p.mm_stride);
+        if (MODE != 0) {
+            // the query staged before the launch: its code words, then for MinMax its {b, n, a, norm_squared}; the SQ
+            // compensation stays in a register
+            const uint32_t words = p.code_stride >> 2;
+            const uint32_t* src = reinterpret_cast<const uint32_t*>(p.query_codes + (size_t)qidx * p.code_stride);
             for (uint32_t wd = lane; wd < words; wd += 32) qc[wd] = __ldg(src + wd);
-            if (lane == 0) *reinterpret_cast<float4*>(qc + words) = __ldg(p.mm_qmeta + qidx);
+            if (MODE == 1) q_comp = __shfl_sync(kFull, lane == 0 ? __ldg(&p.query_meta[qidx].x) : 0.0f, 0);
+            if (MODE == 2 && lane == 0) *reinterpret_cast<float4*>(qc + words) = __ldg(p.query_meta + qidx);
             __syncwarp();
         }
         for (uint32_t t = lane; MODE == 0 && !p.direct_cosine && t < entries; t += 32) {
@@ -554,25 +487,22 @@ static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uin
     p.ip_table = idx->metric == DAB_INNER_PRODUCT ? 1 : 0;  // L2 and CosineNormalized use TableL2 (dynamic.rs:80-85)
     p.direct_cosine = mode == 0 && idx->metric == DAB_COSINE ? 1 : 0;
     if (mode == 1) {
-        p.sq_codes = idx->d_sq_codes;
+        p.row_codes = idx->d_sq_codes;
+        p.code_stride = idx->sq_stride;
+        p.code_nbits = idx->sq_nbits;
         p.sq_comp = idx->d_sq_comp;
-        p.sq_shift = idx->d_sq_shift;
-        p.sq_stride = idx->sq_stride;
-        p.sq_nbits = idx->sq_nbits;
-        p.sq_metric = idx->metric;
-        p.sq_scale = idx->sq_scale;
         p.sq_scale_squared = idx->sq_scale * idx->sq_scale;  // AsFunctor (scalar/quantizer.rs:316-335)
         p.sq_shift_square_norm = idx->sq_shift_square_norm;
-        p.sq_mean_norm = idx->sq_mean_norm;
-        p.n_chunks = 0;
     }
     if (mode == 2) {
-        p.mm_codes = idx->d_mm_codes;
+        p.row_codes = idx->d_mm_codes;
+        p.code_stride = idx->mm_stride;
+        p.code_nbits = idx->mm_nbits;
         p.mm_meta = idx->d_mm_meta;
-        p.mm_stride = idx->mm_stride;
         p.mm_dim = idx->mm_dim;
-        p.mm_nbits = idx->mm_nbits;
-        p.mm_metric = idx->metric;  // MinMaxElement::query_distance: all four metrics (minmax_repr.rs)
+    }
+    if (mode != 0) {
+        p.code_metric = idx->metric;  // MinMaxElement::query_distance: all four metrics (minmax_repr.rs)
         p.n_chunks = 0;
     }
     p.out_ids = d_ids;
@@ -597,8 +527,8 @@ static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uin
     p.off_beam = (uint32_t)off;
     off += round_up((size_t)beam * 4, 16);
     p.off_qc = (uint32_t)off;
-    if (mode == 1) off += idx->sq_stride;
-    if (mode == 2) off += idx->mm_stride + 16;  // the query's code row and its four compensations
+    if (mode == 1) off += p.code_stride;
+    if (mode == 2) off += p.code_stride + 16;  // the query's code row and its four compensations
     off = round_up(off, 16);
     p.off_nrow = (uint32_t)off;  // search_kernel_pqs: the adjacency row copied one hop ahead
     if (mode == 0) off += 96 * 4;
@@ -649,7 +579,7 @@ static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uin
         p.list_counts = p.list_ids + (size_t)nq * cap;
         p.list_cap = cap;
     }
-    if (mode == 2 && (rc = minmax_stage_queries(idx, d_queries, nq, &p.mm_qcodes, &p.mm_qmeta))) return rc;
+    if (mode != 0 && (rc = (mode == 1 ? sq_stage_queries : minmax_stage_queries)(idx, d_queries, nq, &p.query_codes, &p.query_meta))) return rc;
     // global-table passes: the overflowed queries of one are re-run on larger tables in the next
     uint64_t slots = table_slots(idx, idx->pq_hint, l_search, beam, mode);
     Scratch retry;

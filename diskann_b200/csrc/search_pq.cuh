@@ -1,5 +1,6 @@
 // search_pq.cuh — parameter block shared by the quantized-traversal kernels (search_kernel_pq.cu: per-warp table in
-// global memory, SQ, DirectCosine; search_kernel_pqs.cu: pivots resident in shared memory).
+// global memory, DirectCosine, the SQ and MinMax stores; search_kernel_pqs.cu: pivots resident in shared memory), and
+// the query staging of the two packed-code stores.
 #pragma once
 
 #include "dab_common.cuh"
@@ -9,7 +10,6 @@ namespace dab {
 constexpr int kPqWarps = 4;
 
 struct SearchParamsPq {
-    const uint8_t* vectors;  // only for the f32 view of the query rows in build-free search: unused
     const uint32_t* adj;
     uint32_t adj_stride;
     uint64_t n_points;
@@ -41,24 +41,22 @@ struct SearchParamsPq {
     uint32_t* list_ids;     // [nq][list_cap]
     uint32_t* list_counts;  // [nq]
     uint32_t list_cap;
-    // MODE 1: scalar-quantized store
-    const uint8_t* sq_codes;  // [n_total][sq_stride], dense N-bit codes, zero padded to 16 B
-    const float* sq_comp;     // [n_total]
-    const float* sq_shift;    // [dim]
-    uint32_t sq_stride;
-    int sq_nbits, sq_metric;
-    float sq_scale, sq_scale_squared, sq_shift_square_norm, sq_mean_norm;
     uint32_t warp_smem, off_q, off_qd, off_qi, off_cid, off_cd, off_beam, off_qc, off_nrow;
     // search_kernel_pqs: the pivot table of the CTA in shared memory
     uint32_t piv_stride;  // floats between pivot rows (odd multiple of 4: rows of different centres start in different 16-byte bank groups)
     uint32_t piv_bytes;   // n_centers * piv_stride * 4, the per-warp slices follow
-    // MODE 2: the MinMax store and the batch's queries compressed into the same layout (minmax_stage_queries)
-    const uint8_t* mm_codes;   // [n_total][mm_stride], dense N-bit codes, zero padded to 16 B
-    const float4* mm_meta;     // [n_total] {b, n, a, norm_squared}
-    const uint8_t* mm_qcodes;  // [nq][mm_stride]
-    const float4* mm_qmeta;    // [nq]
-    uint32_t mm_stride, mm_dim;
-    int mm_nbits, mm_metric;
+    // MODE 1: the rows' compensations and the quantizer's constants
+    const float* sq_comp;  // [n_total]
+    float sq_scale_squared, sq_shift_square_norm;
+    // MODE 2: the rows' compensations {b, n, a, norm_squared} and the store's dim
+    const float4* mm_meta;  // [n_total]
+    uint32_t mm_dim;
+    // MODE 1 (SQ) and MODE 2 (MinMax): the store's rows and the batch's queries, staged into the same layout
+    const uint8_t* row_codes;    // [n_total][code_stride], dense N-bit codes, zero padded to 16 B
+    const uint8_t* query_codes;  // [nq][code_stride]
+    const float4* query_meta;    // [nq] SQ: {compensation, -, -, -}; MinMax: {b, n, a, norm_squared}
+    uint32_t code_stride;
+    int code_nbits, code_metric;
 };
 
 // search_kernel_pqs.cu — the shape of one launch of the shared-memory-pivot kernel
@@ -73,9 +71,13 @@ struct PqsPlan {
 bool pqs_plan(const dab_index* idx, uint32_t warp_smem, uint32_t nq, PqsPlan* out);
 int pqs_launch(dab_index* idx, const SearchParamsPq& p, const PqsPlan& plan, uint32_t cap);
 
-// minmax_index.cu — the query side of the MinMax traversal: the nq queries d_queries (index dtype, device memory) go
-// through as_f32, the store's transform and its compressor on the index's stream, into codes [nq][mm_stride] and
-// compensations [nq] in the store's layout.  Fails naming the first query whose transformed vector holds a NaN.
+// The query side of the packed-code traversals: the nq queries d_queries (index dtype, device memory) are compressed by
+// the store's own quantizer on the index's stream into codes [nq][stride] and one float4 per query in the store's
+// layout, in the index's staging scratch.
+// sq_index.cu: as_f32, the InnerProduct rescale, ScalarQuantizer::compress; the compensation in .x.  A NaN packs as 0.
+int sq_stage_queries(dab_index* idx, const void* d_queries, uint32_t nq, const uint8_t** d_qcodes, const float4** d_qmeta);
+// minmax_index.cu: as_f32, the store's transform, its compressor; {b, n, a, norm_squared}.  Fails naming the first
+// query whose transformed vector holds a NaN.
 int minmax_stage_queries(dab_index* idx, const void* d_queries, uint32_t nq, const uint8_t** d_qcodes, const float4** d_qmeta);
 
 

@@ -6,9 +6,11 @@
 // f32 compensation followed by ceil(dim * nbits / 8) bytes of Dense-packed codes (bits/slice.rs:
 // 261-323, value i at bit i * nbits) — what SQStore::set_quant_vector (:193-212) takes and what
 // get_vector returns.  On the device the codes are 16 B-aligned rows (zero padded, so the integer
-// cores can run over whole words) and the compensations a separate array.
+// cores can run over whole words) and the compensations a separate array.  sq_stage_queries
+// compresses a search batch's queries into the same device layout before the traversal starts.
 #include "dab_common.cuh"
-#include "distance_device.cuh"
+#include "quant_device.cuh"
+#include "search_pq.cuh"
 
 #include <algorithm>
 
@@ -43,11 +45,6 @@ __global__ void __launch_bounds__(256) sq_join_kernel(const uint8_t* __restrict_
     }
 }
 
-__device__ __forceinline__ float elem_f32(float v) { return v; }
-__device__ __forceinline__ float elem_f32(__half v) { return __half2float(v); }
-__device__ __forceinline__ float elem_f32(int8_t v) { return (float)v; }
-__device__ __forceinline__ float elem_f32(uint8_t v) { return (float)v; }
-
 // SQStore::set_vector (providers inmem/scalar.rs:150-175): as_f32, then ScalarQuantizer::compress
 // (scalar/quantizer.rs:190-239) with the compensation callback (:407-430).  The compensation is a
 // sequential FMA chain over the dimensions, so one thread owns one row and packs its words as it goes.
@@ -65,10 +62,8 @@ __global__ void __launch_bounds__(128) sq_encode_rows_kernel(const uint8_t* __re
         float dot = 0.0f;
         uint32_t acc = 0, filled = 0, word = 0;
         for (uint32_t i = 0; i < dim; ++i) {
-            const float f = elem_f32(row[i]), s = __ldg(shift + i);
-            const float t = __fmul_rn(__fsub_rn(f, s), inverse_scale);
-            float code = t != t ? t : (t < 0.0f ? 0.0f : (t > maxv ? maxv : t));  // f32::clamp keeps NaN
-            code = roundf(code);                                                  // half away from zero
+            const float s = __ldg(shift + i);
+            const float code = sq_code(to_f32(row[i]), s, inverse_scale, maxv);
             dot = __fmaf_rn(code, s, dot);
             acc |= (code != code ? 0u : (uint32_t)code) << (filled * (uint32_t)nbits);
             if (++filled == per_word) {
@@ -79,7 +74,57 @@ __global__ void __launch_bounds__(128) sq_encode_rows_kernel(const uint8_t* __re
         }
         if (filled) out[word++] = acc;
         for (; word < (stride >> 2); ++word) out[word] = 0;
-        comp[v] = __fmul_rn(__fmul_rn(scale, inverse_bit_scale), dot);
+        comp[v] = sq_compensation(scale, inverse_bit_scale, dot);
+    }
+}
+
+// SQStore::query_computer (:227-253): as_f32, for InnerProduct the rescale to the store's mean norm, then the same
+// compression as the rows.  One warp per query in `work` (its f32 copy): the codes in parallel, the norm and the
+// compensation chain on lane 0; meta.x takes the compensation.
+template <typename T>
+__global__ void __launch_bounds__(128) sq_stage_kernel(const T* __restrict__ queries, uint32_t nq, int dim, const float* __restrict__ shift,
+                                                       float scale, float mean_norm, bool rescale, int nbits, uint32_t stride,
+                                                       float* __restrict__ work, uint32_t* __restrict__ codes, float4* __restrict__ meta) {
+    const int lane = threadIdx.x & 31;
+    const uint32_t q = blockIdx.x * 4u + (threadIdx.x >> 5);
+    if (q >= nq) return;
+    float* qf = work + (size_t)q * dim;
+    for (int e = lane; e < dim; e += 32) qf[e] = to_f32(queries[(size_t)q * dim + e]);
+    __syncwarp();
+    // rescale (scalar/quantizer.rs:300-310): InnerProduct::evaluate(x, x), sqrt, x *= to_norm / norm
+    if (rescale) {
+        float norm = 0.0f;
+        if (lane == 0) norm = __fsqrt_rn(thread_simd_l2ip<KIND_IP>(qf, qf, dim));
+        norm = __shfl_sync(kFull, norm, 0);
+        if (norm != 0.0f) {
+            const float sc = __fdiv_rn(mean_norm, norm);
+            for (int e = lane; e < dim; e += 32) qf[e] = __fmul_rn(qf[e], sc);
+        }
+        __syncwarp();
+    }
+    // ScalarQuantizer::compress: codes in parallel ...
+    const float maxv = (float)((1u << nbits) - 1u);
+    const float inverse_scale = __fdiv_rn(maxv, scale);
+    for (int e = lane; e < dim; e += 32) qf[e] = sq_code(qf[e], __ldg(shift + e), inverse_scale, maxv);
+    __syncwarp();
+    // ... the compensation is one sequential FMA chain over the dimensions
+    if (lane == 0) {
+        float dot = 0.0f;
+        for (int e = 0; e < dim; ++e) dot = __fmaf_rn(qf[e], __ldg(shift + e), dot);
+        meta[q] = make_float4(sq_compensation(scale, __fdiv_rn(1.0f, maxv), dot), 0.0f, 0.0f, 0.0f);
+    }
+    // dense packing, value i at bit i * nbits (bits/slice.rs:261-305); padding words are zero
+    const uint32_t per_word = 32u / (uint32_t)nbits;
+    for (uint32_t wd = lane; wd < (stride >> 2); wd += 32) {
+        uint32_t acc = 0;
+        for (uint32_t j = 0; j < per_word; ++j) {
+            const uint32_t e = wd * per_word + j;
+            if (e < (uint32_t)dim) {
+                const float c = qf[e];
+                acc |= (c != c ? 0u : (uint32_t)c) << (j * (uint32_t)nbits);
+            }
+        }
+        codes[(size_t)q * (stride >> 2) + wd] = acc;
     }
 }
 
@@ -90,6 +135,32 @@ int require_sq(const dab_index* idx, const char* who) {
 }
 
 }  // namespace
+
+int sq_stage_queries(dab_index* idx, const void* d_queries, uint32_t nq, const uint8_t** d_qcodes, const float4** d_qmeta) {
+    int rc;
+    const size_t codes_off = round_up((size_t)nq * idx->dim * 4, 256), meta_off = codes_off + round_up((size_t)nq * idx->sq_stride, 256);
+    if ((rc = idx->s_stage.reserve(meta_off + (size_t)nq * 16))) return rc;
+    uint8_t* base = (uint8_t*)idx->s_stage.p;
+    uint32_t* qcodes = (uint32_t*)(base + codes_off);
+    float4* qmeta = (float4*)(base + meta_off);
+    const bool rescale = idx->metric == DAB_INNER_PRODUCT && idx->sq_mean_norm != 0.0f;
+    const int grid = (int)(((uint64_t)nq + 3) / 4);
+    auto launch = [&](auto* queries) {
+        sq_stage_kernel<<<grid, 128, 0, idx->stream>>>(queries, nq, (int)idx->dim, idx->d_sq_shift, idx->sq_scale, idx->sq_mean_norm, rescale,
+                                                       idx->sq_nbits, idx->sq_stride, (float*)base, qcodes, qmeta);
+    };
+    switch (idx->dtype) {
+        case DAB_F32: launch((const float*)d_queries); break;
+        case DAB_F16: launch((const __half*)d_queries); break;
+        case DAB_I8: launch((const int8_t*)d_queries); break;
+        default: launch((const uint8_t*)d_queries); break;
+    }
+    DAB_LAUNCHED();
+    DAB_CUDA(cudaGetLastError());
+    *d_qcodes = (const uint8_t*)qcodes;
+    *d_qmeta = qmeta;
+    return DAB_OK;
+}
 
 }  // namespace dab
 
