@@ -138,14 +138,14 @@ void dab_destroy(dab_index* idx) {
     comm_release(idx);
     tc_release(idx);
     minmax_release(idx);
+    store_release(idx->sq);
+    store_release(idx->mm);
     cudaFree(idx->d_vectors);
     cudaFree(idx->d_adj);
     cudaFree(idx->d_pivots);
     cudaFree(idx->d_offsets);
     cudaFree(idx->d_codes);
     cudaFree(idx->d_sq_shift);
-    cudaFree(idx->d_sq_codes);
-    cudaFree(idx->d_sq_comp);
     idx->s_queries.release();
     idx->s_ids.release();
     idx->s_out.release();

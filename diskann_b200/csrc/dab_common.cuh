@@ -26,7 +26,7 @@ extern std::atomic<uint64_t> g_launches;
 void comm_release(struct ::dab_index* idx);  // replicate.cu
 void tc_release(struct ::dab_index* idx);    // flat_tc.cu
 void search_slots_release(struct ::dab_index* idx);  // search_kernel.cu
-void minmax_release(struct ::dab_index* idx);        // minmax_index.cu
+void minmax_release(struct ::dab_index* idx);        // minmax_index.cu: the store's transform
 
 #define DAB_CUDA(expr)                                                                        \
     do {                                                                                      \
@@ -74,6 +74,46 @@ struct VisitedHint {
     int mode = 0;
 };
 
+// A store of dense N-bit code rows, one per point (the SQ and MinMax stores of an index).  Host-facing rows use the
+// reference's canonical-front layout (meta/vector.rs): a header — an optional u32 dim word, then meta_words f32 — and
+// ceil(dim * nbits / 8) bytes of dense codes, value i at bit i * nbits (bits/slice.rs:261-323).  On the device the codes
+// are 16 B-aligned rows, zero padded (the integer cores read whole words), and the header's floats a separate
+// [n_total][meta_words] array; the dim word is checked on upload and not stored.  code_store.cu moves rows between the
+// two layouts.
+struct CodeStore {
+    int nbits = 0;                // 0: not set up
+    uint32_t dim = 0;             // codes per row
+    bool dim_word = false;        // the header starts with a u32 dim word
+    uint32_t meta_words = 0;      // f32 per row after it
+    uint32_t row_bytes = 0;       // canonical row: header + codes
+    uint32_t stride = 0;          // device code row
+    uint8_t* d_codes = nullptr;   // [n_total][stride]
+    float* d_meta = nullptr;      // [n_total][meta_words]
+    bool ready = false;           // rows uploaded or encoded
+    __host__ __device__ uint32_t header_bytes() const { return (dim_word ? 4u : 0u) + meta_words * 4u; }
+};
+
+// code_store.cu
+// Releases `s`, then allocates it for n_total rows of `dim` codes of `nbits`, zeroed and not ready.
+int store_alloc(struct ::dab_index* idx, CodeStore& s, int nbits, uint32_t dim, bool dim_word, uint32_t meta_words);
+void store_release(CodeStore& s);
+// "<who>: idx is NULL", or "<who>: <upload> has not been called" while the store is not set up
+int store_require(const struct ::dab_index* idx, CodeStore dab_index::*store, const char* upload, const char* who);
+// n canonical rows (device memory) -> codes [n][s.stride] and meta [n][s.meta_words], queued on the index's stream.  The
+// bits past dim * nbits in a row's last code byte are cleared.  first_bad (device, may be NULL) takes the first row
+// whose dim word is not s.dim.
+int store_split(struct ::dab_index* idx, const CodeStore& s, const uint8_t* rows, uint64_t n, uint8_t* codes, float* meta,
+                unsigned long long* first_bad);
+// every row from host canonical rows, staged in slabs; fails naming the first row whose dim word is not s.dim
+int store_upload(struct ::dab_index* idx, CodeStore& s, const uint8_t* rows, const char* who);
+// every row back to host canonical rows, byte for byte what the store holds
+int store_download(struct ::dab_index* idx, const CodeStore& s, uint8_t* rows);
+// The staging scratch of a packed-code search batch: `work` bytes for the quantizer, then the compressed queries, codes
+// [nq][s.stride] and one float4 per query.
+int stage_query_buffers(struct ::dab_index* idx, const CodeStore& s, uint32_t nq, size_t work, uint8_t** codes, float4** meta);
+// T::as_f32 of n rows of the index dtype, src_stride bytes apart -> dst [n][dim], queued on the index's stream
+int widen_rows(struct ::dab_index* idx, const void* src, size_t src_stride, uint64_t n, float* dst);
+
 }  // namespace dab
 
 struct dab_index {
@@ -102,30 +142,21 @@ struct dab_index {
     uint32_t pq_chunks = 0, pq_centers = 0;
     uint32_t pq_uniform_len = 0;   // every chunk has this many dimensions (0: lengths differ)
     bool pq_codes_ready = false;   // codes uploaded (dab_upload_pq) or produced (dab_pq_encode_all)
-    // scalar-quantized store (providers inmem/scalar.rs SQStore<NBITS>): dense N-bit codes, one 16 B-aligned
-    // row per point, compensations apart (only the inner-product epilogue reads them)
-    int sq_nbits = 0;
+    // packed-code stores: scalar-quantized (sq_index.cu; providers inmem/scalar.rs SQStore<NBITS>), rows of index dim
+    // codes with one f32 compensation (only the inner-product epilogue reads it); MinMax (minmax_index.cu; providers
+    // common/minmax_repr.rs MinMaxElement<NBITS>), rows of the transform's output dim with {b, n, a, norm_squared}
+    dab::CodeStore sq, mm;
+    // the scalar quantizer
     float sq_scale = 0.0f, sq_shift_square_norm = 0.0f, sq_mean_norm = 0.0f;
-    float* d_sq_shift = nullptr;   // [dim]
-    uint8_t* d_sq_codes = nullptr; // [n_total][sq_stride]
-    float* d_sq_comp = nullptr;    // [n_total]
-    uint32_t sq_row_bytes = 0, sq_stride = 0;
-    bool sq_codes_ready = false;
-    // MinMax store (minmax_index.cu; providers common/minmax_repr.rs MinMaxElement<NBITS>): the quantizer (width, grid
-    // scale, its own copy of the transform with the tables on the device) and one row per point: dense codes 16 B-aligned
-    // and zero padded, the compensations {b, n, a, norm_squared} apart
-    int mm_nbits = 0;
+    float* d_sq_shift = nullptr;  // [dim]
+    // the MinMax quantizer: grid scale, its own copy of the transform with the tables on the device
     float mm_grid_scale = 0.0f;
-    uint32_t mm_dim = 0, mm_row_bytes = 0, mm_stride = 0;  // transform output dim, canonical row bytes, device row stride
-    dab_transform* mm_transform = nullptr;                 // NULL: Transform::Null
-    uint32_t* d_mm_tables = nullptr;                       // transform_tables(mm_transform)
-    uint8_t* d_mm_codes = nullptr;                         // [n_total][mm_stride]
-    float4* d_mm_meta = nullptr;                           // [n_total]
-    bool mm_ready = false;
+    dab_transform* mm_transform = nullptr;  // NULL: Transform::Null
+    uint32_t* d_mm_tables = nullptr;        // transform_tables(mm_transform)
 
     // scratch (grow-only)
     dab::Scratch s_queries, s_ids, s_out, s_out2, s_tables, s_counters, s_stats;
-    dab::Scratch s_stage;  // MinMax upload / encode / download staging, and the SQ and MinMax searches' compressed queries
+    dab::Scratch s_stage;  // packed-code store upload / encode / download staging, and the SQ and MinMax searches' compressed queries
     dab::Scratch h_stage;  // pinned host staging
     dab::Scratch h_counters;  // pinned: the four counters a search pass reports
     void* slots[DAB_MAX_SLOTS] = {};  // batches in flight (dab_search_batch_async), search_kernel.cu

@@ -291,21 +291,6 @@ __global__ void __launch_bounds__(256) lloyd_update_kernel(const TrainParams p) 
     }
 }
 
-template <typename T>
-__global__ void rows_to_f32_kernel(const uint8_t* __restrict__ vectors, size_t row_stride, uint64_t first, uint64_t count, uint32_t dim,
-                                   float* __restrict__ out) {
-    const uint64_t total = count * dim;
-    for (uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; t < total; t += (uint64_t)gridDim.x * blockDim.x) {
-        const uint64_t r = t / dim;
-        const uint32_t d = (uint32_t)(t % dim);
-        const T* row = reinterpret_cast<const T*>(vectors + (first + r) * row_stride);
-        float v;
-        if constexpr (sizeof(T) == 2) v = __half2float(row[d]);
-        else v = (float)row[d];
-        out[t] = v;
-    }
-}
-
 struct DevMem {
     void* p = nullptr;
     ~DevMem() { cudaFree(p); }
@@ -439,14 +424,7 @@ int dab_pq_encode_all(dab_index* idx) {
     float* d_f32 = (float*)idx->s_queries.p;
     for (uint64_t first = 0; first < total; first += batch) {
         const uint64_t cnt = std::min(batch, total - first);
-        const int grid = (int)std::min<uint64_t>((cnt * idx->dim + 255) / 256, (uint64_t)idx->sm_count * 16);
-        switch (idx->dtype) {
-            case DAB_F32: rows_to_f32_kernel<float><<<grid, 256, 0, idx->stream>>>(idx->d_vectors, idx->row_stride, first, cnt, idx->dim, d_f32); break;
-            case DAB_F16: rows_to_f32_kernel<__half><<<grid, 256, 0, idx->stream>>>(idx->d_vectors, idx->row_stride, first, cnt, idx->dim, d_f32); break;
-            case DAB_I8: rows_to_f32_kernel<int8_t><<<grid, 256, 0, idx->stream>>>(idx->d_vectors, idx->row_stride, first, cnt, idx->dim, d_f32); break;
-            default: rows_to_f32_kernel<uint8_t><<<grid, 256, 0, idx->stream>>>(idx->d_vectors, idx->row_stride, first, cnt, idx->dim, d_f32); break;
-        }
-        DAB_LAUNCHED();
+        if ((rc = widen_rows(idx, idx->d_vectors + first * idx->row_stride, idx->row_stride, cnt, d_f32))) return rc;
         if ((rc = pq_encode_device(idx, d_f32, cnt, idx->d_codes + first * idx->pq_chunks))) return rc;
     }
     idx->pq_codes_ready = true;

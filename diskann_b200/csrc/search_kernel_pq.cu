@@ -97,11 +97,11 @@ __global__ void __launch_bounds__(kPqWarps * 32) search_kernel_pq(const SearchPa
                     if (MODE == 1) {
                         const float ibs = __fdiv_rn(1.0f, (float)((1u << p.code_nbits) - 1u));
                         const float mul = __fmul_rn(__fmul_rn(ibs, ibs), p.sq_scale_squared);
-                        cd[c] = sq_finish(p.code_metric, l2, ip, mul, p.sq_shift_square_norm, q_comp, want_ip ? __ldg(p.sq_comp + id) : 0.0f);
+                        cd[c] = sq_finish(p.code_metric, l2, ip, mul, p.sq_shift_square_norm, q_comp, want_ip ? __ldg(p.row_meta + id) : 0.0f);
                     } else {
                         const float4 qm = *reinterpret_cast<const float4*>(qc + (p.code_stride >> 2));
-                        const float4 rm = __ldg(p.mm_meta + id);
-                        cd[c] = minmax_finish(p.code_metric, ip, p.mm_dim, qm.x, qm.y, qm.z, qm.w, rm.x, rm.y, rm.z, rm.w);
+                        const float4 rm = __ldg(reinterpret_cast<const float4*>(p.row_meta) + id);
+                        cd[c] = minmax_finish(p.code_metric, ip, p.code_dim, qm.x, qm.y, qm.z, qm.w, rm.x, rm.y, rm.z, rm.w);
                     }
                 }
             } else if (p.direct_cosine) {
@@ -457,13 +457,13 @@ static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uin
     if ((rc = check_search_args(idx, k, l_search, beam, false))) return rc;
     if (mode == 0 && (!idx->d_pivots || !idx->d_codes || !idx->pq_codes_ready))
         return fail(DAB_ERR_NOT_READY, "dab_search_batch_pq: no PQ codes (dab_upload_pq with codes, or dab_pq_encode_all)");
-    if (mode == 1 && (!idx->d_sq_codes || !idx->sq_codes_ready))
-        return fail(DAB_ERR_NOT_READY, "dab_search_batch_sq: no scalar-quantized rows (dab_upload_sq with rows, or dab_sq_encode_all)");
+    const CodeStore& store = mode == 2 ? idx->mm : idx->sq;  // modes 1 and 2
+    if (mode != 0 && (!store.d_codes || !store.ready))
+        return fail(DAB_ERR_NOT_READY, mode == 1 ? "dab_search_batch_sq: no scalar-quantized rows (dab_upload_sq with rows, or dab_sq_encode_all)"
+                                                 : "dab_search_batch_minmax: no MinMax rows (dab_upload_minmax with rows, or dab_minmax_encode_all)");
     // SQStore::distance_computer (providers inmem/scalar.rs:214-226): UnsupportedDistanceMetric
     if (mode == 1 && idx->metric == DAB_COSINE)
         return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_sq: the scalar-quantized store supports L2, InnerProduct and CosineNormalized");
-    if (mode == 2 && (!idx->d_mm_codes || !idx->mm_ready))
-        return fail(DAB_ERR_NOT_READY, "dab_search_batch_minmax: no MinMax rows (dab_upload_minmax with rows, or dab_minmax_encode_all)");
     const uint32_t cap = l_search + idx->n_start;
     if (cap > 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: L + #start must be <= 1024", mode == 2 ? "dab_search_batch_minmax" : "dab_search_batch_pq");
     SearchParamsPq p;
@@ -486,24 +486,18 @@ static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uin
     p.n_centers = idx->pq_centers;
     p.ip_table = idx->metric == DAB_INNER_PRODUCT ? 1 : 0;  // L2 and CosineNormalized use TableL2 (dynamic.rs:80-85)
     p.direct_cosine = mode == 0 && idx->metric == DAB_COSINE ? 1 : 0;
-    if (mode == 1) {
-        p.row_codes = idx->d_sq_codes;
-        p.code_stride = idx->sq_stride;
-        p.code_nbits = idx->sq_nbits;
-        p.sq_comp = idx->d_sq_comp;
-        p.sq_scale_squared = idx->sq_scale * idx->sq_scale;  // AsFunctor (scalar/quantizer.rs:316-335)
-        p.sq_shift_square_norm = idx->sq_shift_square_norm;
-    }
-    if (mode == 2) {
-        p.row_codes = idx->d_mm_codes;
-        p.code_stride = idx->mm_stride;
-        p.code_nbits = idx->mm_nbits;
-        p.mm_meta = idx->d_mm_meta;
-        p.mm_dim = idx->mm_dim;
-    }
     if (mode != 0) {
+        p.row_codes = store.d_codes;
+        p.row_meta = store.d_meta;
+        p.code_stride = store.stride;
+        p.code_dim = store.dim;
+        p.code_nbits = store.nbits;
         p.code_metric = idx->metric;  // MinMaxElement::query_distance: all four metrics (minmax_repr.rs)
         p.n_chunks = 0;
+    }
+    if (mode == 1) {
+        p.sq_scale_squared = idx->sq_scale * idx->sq_scale;  // AsFunctor (scalar/quantizer.rs:316-335)
+        p.sq_shift_square_norm = idx->sq_shift_square_norm;
     }
     p.out_ids = d_ids;
     p.out_dists = d_dists;

@@ -45,13 +45,11 @@ struct SearchParamsPq {
     // search_kernel_pqs: the pivot table of the CTA in shared memory
     uint32_t piv_stride;  // floats between pivot rows (odd multiple of 4: rows of different centres start in different 16-byte bank groups)
     uint32_t piv_bytes;   // n_centers * piv_stride * 4, the per-warp slices follow
-    // MODE 1: the rows' compensations and the quantizer's constants
-    const float* sq_comp;  // [n_total]
-    float sq_scale_squared, sq_shift_square_norm;
-    // MODE 2: the rows' compensations {b, n, a, norm_squared} and the store's dim
-    const float4* mm_meta;  // [n_total]
-    uint32_t mm_dim;
-    // MODE 1 (SQ) and MODE 2 (MinMax): the store's rows and the batch's queries, staged into the same layout
+    // MODE 1 (SQ) and MODE 2 (MinMax): the store's rows and the batch's queries, staged into the same layout.  The order of
+    // these fields steers ptxas's register allocation of search_kernel_pq MODE 1 / 2: check -res-usage when moving them.
+    const float* row_meta;  // SQ: [n_total] compensations; MinMax: [n_total][4] {b, n, a, norm_squared}
+    float sq_scale_squared, sq_shift_square_norm;  // MODE 1: the quantizer's constants
+    uint32_t code_dim;           // codes per row
     const uint8_t* row_codes;    // [n_total][code_stride], dense N-bit codes, zero padded to 16 B
     const uint8_t* query_codes;  // [nq][code_stride]
     const float4* query_meta;    // [nq] SQ: {compensation, -, -, -}; MinMax: {b, n, a, norm_squared}
@@ -73,7 +71,7 @@ int pqs_launch(dab_index* idx, const SearchParamsPq& p, const PqsPlan& plan, uin
 
 // The query side of the packed-code traversals: the nq queries d_queries (index dtype, device memory) are compressed by
 // the store's own quantizer on the index's stream into codes [nq][stride] and one float4 per query in the store's
-// layout, in the index's staging scratch.
+// layout, in the index's staging scratch (stage_query_buffers).
 // sq_index.cu: as_f32, the InnerProduct rescale, ScalarQuantizer::compress; the compensation in .x.  A NaN packs as 0.
 int sq_stage_queries(dab_index* idx, const void* d_queries, uint32_t nq, const uint8_t** d_qcodes, const float4** d_qmeta);
 // minmax_index.cu: as_f32, the store's transform, its compressor; {b, n, a, norm_squared}.  Fails naming the first

@@ -260,12 +260,14 @@ int dab_sq_distances(int device, int metric, int nbits, float scale_squared, flo
  * per point (data + start points) in the reference's canonical-front layout (diskann-quantization/
  * src/meta/vector.rs:478-507): 4 bytes f32 compensation, then ceil(dim * nbits / 8) bytes of
  * Dense-packed codes (bits/slice.rs:261-323) — what set_quant_vector (:193-212) stores.  rows may
- * be NULL when dab_sq_encode_all follows.  nbits in {1, 2, 4, 8}. */
+ * be NULL when dab_sq_encode_all follows.  Bits past dim * nbits in a row's last code byte are
+ * ignored, as the reference's BitSlice never reads them.  nbits in {1, 2, 4, 8}. */
 int dab_upload_sq(dab_index* idx, int nbits, const float* shift, float scale, float shift_square_norm,
                   float mean_norm, const uint8_t* rows);
 /* SQStore::set_vector (scalar.rs:150-175) for every resident row (any dtype, as_f32 first). */
 int dab_sq_encode_all(dab_index* idx);
-/* rows back in the canonical-front layout: (n_points + n_start) x (4 + ceil(dim * nbits / 8)) */
+/* rows back in the canonical-front layout, (n_points + n_start) x (4 + ceil(dim * nbits / 8)): byte
+ * for byte what the store holds, the padding bits of the last code byte cleared */
 int dab_sq_download(dab_index* idx, uint8_t* rows);
 
 /* KNN::search through the scalar-quantized accessor (scalar.rs:449-570): the query is compressed
@@ -371,7 +373,8 @@ int dab_upload_minmax(dab_index* idx, int nbits, float grid_scale, const dab_tra
  * garnet's backfill stores.  A transformed row holding a NaN fails the call, naming the first such row; the store then
  * has no rows until the next successful upload or encode. */
 int dab_minmax_encode_all(dab_index* idx);
-/* the rows back in the canonical-front layout, byte for byte what the store holds */
+/* the rows back in the canonical-front layout, byte for byte what the store holds, the padding bits of the last code
+ * byte cleared */
 int dab_minmax_download(dab_index* idx, uint8_t* rows);
 
 /* KNN::search through the MinMax store (garnet DynamicAccessor, provider.rs:1170-1358: as_f32, then

@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 import oracle_lib as O
+from code_rows import garbage_padding
 
 pytestmark = pytest.mark.gpu
 
@@ -774,7 +775,8 @@ def test_sq_traversal_search_identical_to_oracle(dab, monkeypatch, dt, metric, d
     """dab_search_batch_sq: greedy search through the scalar-quantized accessor (providers inmem/scalar.rs:449-570):
     rows encoded on the device == SQStore::set_vector restated on the CPU (canonical-front layout, dense N-bit codes),
     and ids / distance bits / cmps / hops == the oracle's search with sq_rows set, with and without Rerank; also with
-    256-slot visited tables, whose overflowed queries are re-run (the rerank reads the lists the re-runs wrote)."""
+    256-slot visited tables, whose overflowed queries are re-run (the rerank reads the lists the re-runs wrote).  Host-uploaded
+    rows with garbage padding bits give the same searches and download clean."""
     if tables == "overflow":
         monkeypatch.setenv("DAB_TEST_VISITED_LOG2", "8")
     rng = np.random.default_rng(d * 10 + nbits)
@@ -805,13 +807,14 @@ def test_sq_traversal_search_identical_to_oracle(dab, monkeypatch, dt, metric, d
             want = oidx.search_batch_rerank(queries, k, Ls, beam=beam, threads=4)
             for a, b, name in zip(got, want, ("ids", "dists", "counts", "cmps", "hops")):
                 assert np.array_equal(a.view(np.uint32), b.view(np.uint32)), ("rerank", name, k, Ls, beam)
-        # rows handed over by the host (set_quant_vector) give the same searches
-        g.upload_sq(nbits, shift, scale, ssn, mean_norm, rows=rows)
-        assert np.array_equal(g.download_sq(), rows)
+        # rows handed over by the host (set_quant_vector), with garbage in the padding bits of the last code byte, give
+        # the same searches: the store holds them with the padding cleared
+        g.upload_sq(nbits, shift, scale, ssn, mean_norm, rows=garbage_padding(rows, d, nbits))
         got = g.search_batch_sq(queries, 10, 50, 1)
         want = oidx.search_batch(queries, 10, 50, beam=1, threads=4)
-        for a, b in zip(got, want):
-            assert np.array_equal(a.view(np.uint32), b.view(np.uint32))
+        for a, b, name in zip(got, want, ("ids", "dists", "counts", "cmps", "hops")):
+            assert np.array_equal(a.view(np.uint32), b.view(np.uint32)), ("host rows", name)
+        assert np.array_equal(g.download_sq(), rows)
     with dab.GpuIndex(dab.DType.f32, dab.Metric.Cosine, d, n, 1, maxdeg) as g:
         g.upload_vectors(f32)
         g.upload_graph(adj)

@@ -15,6 +15,7 @@ import pytest
 
 import diskann_b200 as dab
 import oracle_lib as O
+from code_rows import garbage_padding
 from test_minmax_transforms import oracle_apply
 
 T = dab.Transform
@@ -187,15 +188,6 @@ def index_rows(rng, dt, n, d):
     elif dt == np.uint8:
         base = np.clip(np.round(base * 40 + 128), 0, 255).astype(np.uint8)
     return with_medoid(base)
-
-
-def garbage_padding(rows, dim, nbits):
-    """The rows with every bit past dim * nbits in the last code byte set."""
-    tail = (dim * nbits) % 8
-    out = rows.copy()
-    if tail:
-        out[:, -1] |= np.uint8((0xFF << tail) & 0xFF)
-    return out
 
 
 GPU_CASES = [
