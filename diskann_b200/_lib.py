@@ -42,6 +42,12 @@ SYMBOLS = {
     "dab_search_batch_async": (_i, [_vp, _u32, _vp, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
     "dab_search_batch_device_async": (_i, [_vp, _u32, _vp, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
     "dab_wait": (_i, [_vp, _u32]),
+    "dab_search_batch_pq_async": (_i, [_vp, _u32, _vp, _u32, _u32, _u32, _u32, _i, _vp, _vp, _vp, _vp, _vp]),
+    "dab_search_batch_pq_device_async": (_i, [_vp, _u32, _vp, _u32, _u32, _u32, _u32, _i, _vp, _vp, _vp, _vp, _vp]),
+    "dab_search_batch_sq_async": (_i, [_vp, _u32, _vp, _u32, _u32, _u32, _u32, _i, _vp, _vp, _vp, _vp, _vp]),
+    "dab_search_batch_sq_device_async": (_i, [_vp, _u32, _vp, _u32, _u32, _u32, _u32, _i, _vp, _vp, _vp, _vp, _vp]),
+    "dab_search_batch_minmax_async": (_i, [_vp, _u32, _vp, _u32, _u32, _u32, _u32, _i, _vp, _vp, _vp, _vp, _vp]),
+    "dab_search_batch_minmax_device_async": (_i, [_vp, _u32, _vp, _u32, _u32, _u32, _u32, _i, _vp, _vp, _vp, _vp, _vp]),
     "dab_pq_populate_lut": (_i, [_vp, _vp, _u32, _i, _vp]),
     "dab_pq_distances": (_i, [_vp, _vp, _u32, _vp, _u32, _vp]),
     "dab_pq_encode": (_i, [_vp, _vp, _u64, _vp]),

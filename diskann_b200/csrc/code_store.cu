@@ -110,8 +110,9 @@ int store_require(const dab_index* idx, CodeStore dab_index::*store, const char*
     return DAB_OK;
 }
 
-int store_split(dab_index* idx, const CodeStore& s, const uint8_t* rows, uint64_t n, uint8_t* codes, float* meta, unsigned long long* first_bad) {
-    split_kernel<<<grid_for(idx, n * s.stride), 256, 0, idx->stream>>>(s, rows, n, codes, meta, first_bad);
+int store_split(const dab_index* idx, cudaStream_t stream, const CodeStore& s, const uint8_t* rows, uint64_t n, uint8_t* codes, float* meta,
+                unsigned long long* first_bad) {
+    split_kernel<<<grid_for(idx, n * s.stride), 256, 0, stream>>>(s, rows, n, codes, meta, first_bad);
     DAB_LAUNCHED();
     DAB_CUDA(cudaGetLastError());
     return DAB_OK;
@@ -128,7 +129,7 @@ int store_upload(dab_index* idx, CodeStore& s, const uint8_t* rows, const char* 
         const uint64_t cnt = std::min(slab, total - first);
         DAB_CUDA(cudaMemcpyAsync(stage, rows + first * s.row_bytes, cnt * s.row_bytes, cudaMemcpyHostToDevice, idx->stream));
         DAB_CUDA(cudaMemsetAsync(d_bad, 0xFF, 8, idx->stream));
-        if ((rc = store_split(idx, s, stage, cnt, s.d_codes + first * s.stride, s.d_meta + first * s.meta_words, d_bad))) return rc;
+        if ((rc = store_split(idx, idx->stream, s, stage, cnt, s.d_codes + first * s.stride, s.d_meta + first * s.meta_words, d_bad))) return rc;
         unsigned long long bad = ~0ull;
         DAB_CUDA(cudaMemcpyAsync(&bad, d_bad, 8, cudaMemcpyDeviceToHost, idx->stream));
         DAB_CUDA(cudaStreamSynchronize(idx->stream));
@@ -159,24 +160,28 @@ int store_download(dab_index* idx, const CodeStore& s, uint8_t* rows) {
     return DAB_OK;
 }
 
-int stage_query_buffers(dab_index* idx, const CodeStore& s, uint32_t nq, size_t work, uint8_t** codes, float4** meta) {
+size_t stage_query_bytes(const CodeStore& s, uint32_t nq, size_t work) {
+    return round_up(work, 256) + round_up((size_t)nq * s.stride, 256) + (size_t)nq * 16;
+}
+
+int stage_query_buffers(const CodeStore& s, Scratch& stage, uint32_t nq, size_t work, uint8_t** codes, float4** meta) {
     const size_t codes_off = round_up(work, 256), meta_off = codes_off + round_up((size_t)nq * s.stride, 256);
     int rc;
-    if ((rc = idx->s_stage.reserve(meta_off + (size_t)nq * 16))) return rc;
-    uint8_t* base = (uint8_t*)idx->s_stage.p;
+    if ((rc = stage.reserve(stage_query_bytes(s, nq, work)))) return rc;
+    uint8_t* base = (uint8_t*)stage.p;
     *codes = base + codes_off;
     *meta = (float4*)(base + meta_off);
     return DAB_OK;
 }
 
-int widen_rows(dab_index* idx, const void* src, size_t src_stride, uint64_t n, float* dst) {
+int widen_rows(const dab_index* idx, cudaStream_t stream, const void* src, size_t src_stride, uint64_t n, float* dst) {
     const int grid = grid_for(idx, n * idx->dim);
     const uint8_t* s = (const uint8_t*)src;
     switch (idx->dtype) {
-        case DAB_F32: widen_kernel<float><<<grid, 256, 0, idx->stream>>>(s, src_stride, n, idx->dim, dst); break;
-        case DAB_F16: widen_kernel<__half><<<grid, 256, 0, idx->stream>>>(s, src_stride, n, idx->dim, dst); break;
-        case DAB_I8: widen_kernel<int8_t><<<grid, 256, 0, idx->stream>>>(s, src_stride, n, idx->dim, dst); break;
-        default: widen_kernel<uint8_t><<<grid, 256, 0, idx->stream>>>(s, src_stride, n, idx->dim, dst); break;
+        case DAB_F32: widen_kernel<float><<<grid, 256, 0, stream>>>(s, src_stride, n, idx->dim, dst); break;
+        case DAB_F16: widen_kernel<__half><<<grid, 256, 0, stream>>>(s, src_stride, n, idx->dim, dst); break;
+        case DAB_I8: widen_kernel<int8_t><<<grid, 256, 0, stream>>>(s, src_stride, n, idx->dim, dst); break;
+        default: widen_kernel<uint8_t><<<grid, 256, 0, stream>>>(s, src_stride, n, idx->dim, dst); break;
     }
     DAB_LAUNCHED();
     DAB_CUDA(cudaGetLastError());

@@ -283,6 +283,9 @@ int dab_upload_pq(dab_index* idx, const float* pivots, uint32_t n_centers, const
         off32[c] = (uint32_t)offsets[c];
     }
     DAB_CUDA(cudaSetDevice(idx->device));
+    DAB_CUDA(cudaStreamSynchronize(idx->stream));
+    int rc;
+    if ((rc = retire_quantized_stores(idx))) return rc;  // batches in flight read the table and the codes
     cudaFree(idx->d_pivots);
     cudaFree(idx->d_offsets);
     cudaFree(idx->d_codes);

@@ -26,6 +26,10 @@ extern std::atomic<uint64_t> g_launches;
 void comm_release(struct ::dab_index* idx);  // replicate.cu
 void tc_release(struct ::dab_index* idx);    // flat_tc.cu
 void search_slots_release(struct ::dab_index* idx);  // search_kernel.cu
+// search_kernel.cu: called by every call that frees or reallocates a quantized store (PQ table and codes, SQ or MinMax
+// rows), before it frees anything: waits for every slot's stream and bumps dab_index::stores_version, so that a batch in
+// flight whose overflowed queries still need a pass fails in dab_wait instead of launching on the freed buffers
+int retire_quantized_stores(struct ::dab_index* idx);
 void minmax_release(struct ::dab_index* idx);        // minmax_index.cu: the store's transform
 
 #define DAB_CUDA(expr)                                                                        \
@@ -99,20 +103,22 @@ int store_alloc(struct ::dab_index* idx, CodeStore& s, int nbits, uint32_t dim, 
 void store_release(CodeStore& s);
 // "<who>: idx is NULL", or "<who>: <upload> has not been called" while the store is not set up
 int store_require(const struct ::dab_index* idx, CodeStore dab_index::*store, const char* upload, const char* who);
-// n canonical rows (device memory) -> codes [n][s.stride] and meta [n][s.meta_words], queued on the index's stream.  The
-// bits past dim * nbits in a row's last code byte are cleared.  first_bad (device, may be NULL) takes the first row
-// whose dim word is not s.dim.
-int store_split(struct ::dab_index* idx, const CodeStore& s, const uint8_t* rows, uint64_t n, uint8_t* codes, float* meta,
-                unsigned long long* first_bad);
+// n canonical rows (device memory) -> codes [n][s.stride] and meta [n][s.meta_words], queued on `stream`.  The bits
+// past dim * nbits in a row's last code byte are cleared.  first_bad (device, may be NULL) takes the first row whose dim
+// word is not s.dim.
+int store_split(const struct ::dab_index* idx, cudaStream_t stream, const CodeStore& s, const uint8_t* rows, uint64_t n, uint8_t* codes,
+                float* meta, unsigned long long* first_bad);
 // every row from host canonical rows, staged in slabs; fails naming the first row whose dim word is not s.dim
 int store_upload(struct ::dab_index* idx, CodeStore& s, const uint8_t* rows, const char* who);
 // every row back to host canonical rows, byte for byte what the store holds
 int store_download(struct ::dab_index* idx, const CodeStore& s, uint8_t* rows);
-// The staging scratch of a packed-code search batch: `work` bytes for the quantizer, then the compressed queries, codes
-// [nq][s.stride] and one float4 per query.
-int stage_query_buffers(struct ::dab_index* idx, const CodeStore& s, uint32_t nq, size_t work, uint8_t** codes, float4** meta);
-// T::as_f32 of n rows of the index dtype, src_stride bytes apart -> dst [n][dim], queued on the index's stream
-int widen_rows(struct ::dab_index* idx, const void* src, size_t src_stride, uint64_t n, float* dst);
+// The staging scratch `stage` of a packed-code search batch: `work` bytes for the quantizer, then the compressed queries,
+// codes [nq][s.stride] and one float4 per query.
+int stage_query_buffers(const CodeStore& s, Scratch& stage, uint32_t nq, size_t work, uint8_t** codes, float4** meta);
+// the bytes stage_query_buffers reserves
+size_t stage_query_bytes(const CodeStore& s, uint32_t nq, size_t work);
+// T::as_f32 of n rows of the index dtype, src_stride bytes apart -> dst [n][dim], queued on `stream`
+int widen_rows(const struct ::dab_index* idx, cudaStream_t stream, const void* src, size_t src_stride, uint64_t n, float* dst);
 
 }  // namespace dab
 
@@ -166,6 +172,7 @@ struct dab_index {
     uint32_t v3_overflow_l = 0, v3_overflow_beam = 0;      // share of queries that outgrew the shared-memory
     float v3_overflow_frac = 0.0f;                         // tables at (L, beam): search_kernel_v3 is skipped when large
 
+    uint64_t stores_version = 0;  // bumped whenever a quantized store is freed or reallocated (retire_quantized_stores)
     uint64_t rec_truncated = 0;  // build: searches whose expanded-node record was cut at its capacity
     dab::Tuning tune;
 

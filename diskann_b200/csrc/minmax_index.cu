@@ -22,14 +22,15 @@ namespace {
 
 // as_f32 -> transform -> compress_into for n rows (src_stride bytes apart) into canonical rows [n][mm.row_bytes] in
 // `canon`; *first_nan (device) takes the first row whose transformed vector holds a NaN.  `work` holds the f32 rows:
-// n * (dim + out_dim) floats.  Queued on the index's stream.
-int compress_rows(dab_index* idx, const void* src, size_t src_stride, uint64_t n, float* work, uint8_t* canon, unsigned long long* first_nan) {
+// n * (dim + out_dim) floats.  Queued on `stream`.
+int compress_rows(const dab_index* idx, cudaStream_t stream, const void* src, size_t src_stride, uint64_t n, float* work, uint8_t* canon,
+                  unsigned long long* first_nan) {
     int rc;
-    if ((rc = widen_rows(idx, src, src_stride, n, work))) return rc;
+    if ((rc = widen_rows(idx, stream, src, src_stride, n, work))) return rc;
     const float* vec = work;
     if (idx->mm_transform) {
         float* out = work + n * idx->dim;
-        DAB_CUDA(transform_launch(idx->mm_transform, idx->d_mm_tables, work, n, out, nullptr, idx->stream));
+        DAB_CUDA(transform_launch(idx->mm_transform, idx->d_mm_tables, work, n, out, nullptr, stream));
         vec = out;
     }
     MinMaxCompressParams p;
@@ -39,7 +40,7 @@ int compress_rows(dab_index* idx, const void* src, size_t src_stride, uint64_t n
     p.vectors = vec;
     p.rows = canon;
     p.first_nan = first_nan;
-    DAB_CUDA(mm_compress_launch(p, warps, smem, idx->stream));
+    DAB_CUDA(mm_compress_launch(p, warps, smem, stream));
     return DAB_OK;
 }
 
@@ -67,20 +68,19 @@ void minmax_release(dab_index* idx) {
     idx->mm_transform = nullptr;
 }
 
-int minmax_stage_queries(dab_index* idx, const void* d_queries, uint32_t nq, const uint8_t** d_qcodes, const float4** d_qmeta) {
+size_t minmax_stage_bytes(const dab_index* idx, uint32_t nq) { return stage_query_bytes(idx->mm, nq, staging_bytes(idx, nq)); }
+
+int minmax_stage_queries(const dab_index* idx, cudaStream_t stream, Scratch& stage, const void* d_queries, uint32_t nq,
+                         unsigned long long* h_first_nan, const uint8_t** d_qcodes, const float4** d_qmeta) {
     int rc;
     uint8_t* qcodes;
     float4* qmeta;
-    if ((rc = stage_query_buffers(idx, idx->mm, nq, staging_bytes(idx, nq), &qcodes, &qmeta))) return rc;
-    const Staging s = staging_layout(idx, nq, (uint8_t*)idx->s_stage.p);
-    DAB_CUDA(cudaMemsetAsync(s.flag, 0xFF, 8, idx->stream));
-    if ((rc = compress_rows(idx, d_queries, (size_t)idx->dim * elem_size(idx->dtype), nq, s.work, s.canon, s.flag))) return rc;
-    if ((rc = store_split(idx, idx->mm, s.canon, nq, qcodes, (float*)qmeta, nullptr))) return rc;
-    unsigned long long first_nan = ~0ull;
-    DAB_CUDA(cudaMemcpyAsync(&first_nan, s.flag, 8, cudaMemcpyDeviceToHost, idx->stream));
-    DAB_CUDA(cudaStreamSynchronize(idx->stream));
-    if (first_nan != ~0ull)
-        return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_minmax: query %llu contains NaN after the transform (InputContainsNaN)", first_nan);
+    if ((rc = stage_query_buffers(idx->mm, stage, nq, staging_bytes(idx, nq), &qcodes, &qmeta))) return rc;
+    const Staging s = staging_layout(idx, nq, (uint8_t*)stage.p);
+    DAB_CUDA(cudaMemsetAsync(s.flag, 0xFF, 8, stream));
+    if ((rc = compress_rows(idx, stream, d_queries, (size_t)idx->dim * elem_size(idx->dtype), nq, s.work, s.canon, s.flag))) return rc;
+    if ((rc = store_split(idx, stream, idx->mm, s.canon, nq, qcodes, (float*)qmeta, nullptr))) return rc;
+    DAB_CUDA(cudaMemcpyAsync(h_first_nan, s.flag, 8, cudaMemcpyDeviceToHost, stream));
     *d_qcodes = qcodes;
     *d_qmeta = qmeta;
     return DAB_OK;
@@ -109,6 +109,8 @@ int dab_upload_minmax(dab_index* idx, int nbits, float grid_scale, const dab_tra
         return fail(DAB_ERR_INVALID_ARGUMENT, "%s: rows of %u bytes do not fit the compressor's staging buffers", who, probe.row_bytes);
     DAB_CUDA(cudaSetDevice(idx->device));
     DAB_CUDA(cudaStreamSynchronize(idx->stream));
+    int rc;
+    if ((rc = retire_quantized_stores(idx))) return rc;  // batches in flight read the store and its transform
     minmax_release(idx);
     store_release(idx->mm);
     idx->mm_grid_scale = grid_scale;
@@ -119,7 +121,6 @@ int dab_upload_minmax(dab_index* idx, int nbits, float grid_scale, const dab_tra
         DAB_CUDA(cudaMalloc(&idx->d_mm_tables, tables.size() * 4));
         DAB_CUDA(cudaMemcpy(idx->d_mm_tables, tables.data(), tables.size() * 4, cudaMemcpyHostToDevice));
     }
-    int rc;
     if ((rc = store_alloc(idx, idx->mm, nbits, out_dim, true, 4))) return rc;  // the header: dim, then {b, n, a, norm_squared}
     return rows ? store_upload(idx, idx->mm, rows, who) : DAB_OK;
 }
@@ -140,8 +141,8 @@ int dab_minmax_encode_all(dab_index* idx) {
     for (uint64_t first = 0; first < total; first += slab) {
         const uint64_t cnt = std::min(slab, total - first);
         DAB_CUDA(cudaMemsetAsync(s.flag, 0xFF, 8, idx->stream));
-        if ((rc = compress_rows(idx, idx->d_vectors + first * idx->row_stride, idx->row_stride, cnt, s.work, s.canon, s.flag))) return rc;
-        if ((rc = store_split(idx, mm, s.canon, cnt, mm.d_codes + first * mm.stride, mm.d_meta + first * mm.meta_words, nullptr))) return rc;
+        if ((rc = compress_rows(idx, idx->stream, idx->d_vectors + first * idx->row_stride, idx->row_stride, cnt, s.work, s.canon, s.flag))) return rc;
+        if ((rc = store_split(idx, idx->stream, mm, s.canon, cnt, mm.d_codes + first * mm.stride, mm.d_meta + first * mm.meta_words, nullptr))) return rc;
         unsigned long long first_nan = ~0ull;
         DAB_CUDA(cudaMemcpyAsync(&first_nan, s.flag, 8, cudaMemcpyDeviceToHost, idx->stream));
         DAB_CUDA(cudaStreamSynchronize(idx->stream));

@@ -317,6 +317,9 @@ int dab_pq_train(dab_index* idx, const float* train, uint64_t n, uint32_t n_chun
     DAB_CUDA(cudaSetDevice(idx->device));
     cudaStream_t st = idx->stream;
     const uint32_t dim = idx->dim;
+    DAB_CUDA(cudaStreamSynchronize(st));
+    int rc;
+    if ((rc = retire_quantized_stores(idx))) return rc;  // batches in flight read the table and the codes
     // ChunkOffsets::partition (diskann-quantization/src/views.rs:226-243): the first dim % n_chunks chunks get one extra
     std::vector<uint32_t> off(n_chunks + 1, 0);
     uint32_t max_len = 0;
@@ -424,7 +427,7 @@ int dab_pq_encode_all(dab_index* idx) {
     float* d_f32 = (float*)idx->s_queries.p;
     for (uint64_t first = 0; first < total; first += batch) {
         const uint64_t cnt = std::min(batch, total - first);
-        if ((rc = widen_rows(idx, idx->d_vectors + first * idx->row_stride, idx->row_stride, cnt, d_f32))) return rc;
+        if ((rc = widen_rows(idx, idx->stream, idx->d_vectors + first * idx->row_stride, idx->row_stride, cnt, d_f32))) return rc;
         if ((rc = pq_encode_device(idx, d_f32, cnt, idx->d_codes + first * idx->pq_chunks))) return rc;
     }
     idx->pq_codes_ready = true;

@@ -121,6 +121,8 @@ int broadcast_buffers(dab_index* idx, ncclComm_t comm, int root, bool is_root, I
     if (got.pq_chunks) {
         if (!is_root) {
             DAB_CUDA(cudaStreamSynchronize(st));
+            int rc;
+            if ((rc = retire_quantized_stores(idx))) return rc;  // batches in flight read the table and the codes
             cudaFree(idx->d_pivots);
             cudaFree(idx->d_offsets);
             cudaFree(idx->d_codes);

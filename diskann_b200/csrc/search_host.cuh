@@ -34,4 +34,39 @@ struct SearchOut {
 int search_host_buffers(dab_index* idx, const char* api, const void* queries, uint32_t nq, uint32_t k, const SearchOut& out,
                         const std::function<int(const void* d_queries, const SearchOut& d_out)>& run);
 
+// ---- batches in flight ---------------------------------------------------------------------------------------------
+// A batch of any kind (full precision, PQ, SQ, MinMax) as a resumable job.  `launch` queues all of it and waits for
+// nothing; `finish` waits for it, re-runs the queries that outgrew their visited tables and sets `reran` when it did
+// (their results were then written again after the first copies were queued).
+struct SlotJob {
+    bool reran = false;
+    virtual ~SlotJob() = default;
+    virtual int launch() = 0;
+    virtual int finish() = 0;
+};
+
+// A host-buffer call's results: where the kernels write them and where the caller wants them
+struct HostCopy {
+    SearchOut dev, host;
+    uint32_t nq, k;
+};
+
+// A slot of batches in flight: its own stream and grow-only scratch, so that nothing a batch in flight touches is
+// shared with another slot or with the synchronous calls on the handle's stream.
+struct SearchSlot {
+    cudaStream_t stream = nullptr;
+    Scratch tables, counters, queries, out, stats, h_counters;
+    Scratch stage, luts, lists;  // the quantized traversals: staged queries, per-warp LUTs, the rerank's candidate lists
+    SlotJob* job = nullptr;
+    HostCopy host_out{};  // the pending call's result copies (host_out.host.ids null: device buffers)
+};
+
+// The launching half of every *_async call.  Checks the slot (in range, no batch in flight); nq == 0 is then a no-op.
+// A host-buffer call (`host`) gets device buffers in the slot's scratch.  `prepare` builds the job on the slot's stream and
+// scratch with every check the synchronous call makes before it launches, reserves the buffers and queues nothing; then
+// the copy of the queries, the job's launch and the copies of the results are queued, and the call returns without
+// waiting.  (Should a launch fail with a CUDA error half way, what it queued completes before the error is returned.)
+int slot_submit(dab_index* idx, const char* api, uint32_t slot, bool host, const void* queries, uint32_t nq, uint32_t k,
+                const SearchOut& out, const std::function<int(SearchSlot* s, const void* d_queries, const SearchOut& d_out, SlotJob** job)>& prepare);
+
 }  // namespace dab

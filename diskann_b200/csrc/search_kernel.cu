@@ -1,6 +1,7 @@
 // search_kernel.cu — the host side of batched graph search: the visited-table policy, the overflow re-runs and the
 // host-buffer calls every search shares (search_host.cuh), the full-precision dispatcher, the slots of batches in flight
-// and the C entry points (dab_search_batch[_device][_async], dab_wait).
+// (which the quantized *_async calls of search_kernel_pq.cu share) and the C entry points (dab_search_batch[_device][_async],
+// dab_wait).
 //
 // A batch runs on search_kernel_v3 (visited set in shared memory) where its short lists make that the faster kernel,
 // and on search_kernel_v2 (global visited tables) otherwise; queries whose visited set outgrows its table are re-run
@@ -69,7 +70,7 @@ int take_overflow_list(cudaStream_t stream, const uint32_t* d_overflow, uint32_t
 // handle's stream; dab_search_batch_async / dab_wait keep several batches in flight on slot-owned
 // streams so the tail of one batch (workers running out of queries) is filled by the next batch's
 // CTAs and the host<->device copies of neighbouring batches overlap the kernel.
-struct SearchJob {
+struct SearchJob : SlotJob {
     dab_index* idx = nullptr;
     cudaStream_t stream = nullptr;
     Scratch* tables = nullptr;
@@ -92,9 +93,9 @@ struct SearchJob {
     int prepare(const void* d_queries, const uint32_t* d_query_rows, uint32_t nq_, uint32_t k, uint32_t l_search_, uint32_t beam_,
                 uint32_t* d_ids, float* d_dists, uint32_t* d_counts, uint32_t* d_cmps, uint32_t* d_hops, uint32_t* rec_ids,
                 float* rec_dists, uint32_t* rec_counts, uint32_t rec_cap);
-    int launch();
-    int finish();
-    ~SearchJob() { retry_list.release(); }
+    int launch() override;
+    int finish() override;
+    ~SearchJob() override { retry_list.release(); }
 };
 
 int SearchJob::prepare(const void* d_queries, const uint32_t* d_query_rows, uint32_t nq_, uint32_t k, uint32_t l_search_,
@@ -207,6 +208,7 @@ int SearchJob::finish() {
         }
         if (n_over == 0) return DAB_OK;
         // re-run the overflowed queries on (larger) global tables
+        reran = true;
         int rc;
         if ((rc = take_overflow_list(stream, d_overflow, n_over, retry_list))) return rc;
         p2.query_list = (const uint32_t*)retry_list.p;
@@ -244,23 +246,20 @@ int run_search(dab_index* idx, const void* d_queries, const uint32_t* d_query_ro
 }
 
 // ---- host-buffer calls -------------------------------------------------------------------------
-// A host-buffer call's results: where the kernels write them and where the caller wants them
-struct HostCopy {
-    SearchOut dev, host;
-    uint32_t nq, k;
-};
-
 // reserves the query and result buffers of a host-buffer call (`q`; ids and dists in `out`, counts / cmps / hops in
-// `stats`) and queues the copy of the queries on `stream`
-static int stage_host_call(const dab_index* idx, cudaStream_t stream, Scratch& q, Scratch& out, Scratch& stats, const void* queries,
-                           uint32_t nq, uint32_t k, SearchOut* d) {
+// `stats`); nothing is queued
+static int reserve_host_call(const dab_index* idx, Scratch& q, Scratch& out, Scratch& stats, uint32_t nq, uint32_t k, SearchOut* d) {
     const size_t qbytes = (size_t)nq * idx->dim * elem_size(idx->dtype);
     const size_t rbytes = (size_t)nq * k * 4;
     int rc;
     if ((rc = q.reserve(qbytes)) || (rc = out.reserve(2 * rbytes)) || (rc = stats.reserve((size_t)nq * 12))) return rc;
     uint32_t* st = (uint32_t*)stats.p;
     *d = SearchOut{(uint32_t*)out.p, (float*)((uint8_t*)out.p + rbytes), st, st + nq, st + 2 * (size_t)nq};
-    DAB_CUDA(cudaMemcpyAsync(q.p, queries, qbytes, cudaMemcpyHostToDevice, stream));
+    return DAB_OK;
+}
+
+static int queue_query_copy(const dab_index* idx, cudaStream_t stream, void* d_queries, const void* queries, uint32_t nq) {
+    DAB_CUDA(cudaMemcpyAsync(d_queries, queries, (size_t)nq * idx->dim * elem_size(idx->dtype), cudaMemcpyHostToDevice, stream));
     return DAB_OK;
 }
 
@@ -283,21 +282,15 @@ int search_host_buffers(dab_index* idx, const char* api, const void* queries, ui
     DAB_CUDA(cudaSetDevice(idx->device));
     HostCopy c{{}, out, nq, k};
     int rc;
-    if ((rc = stage_host_call(idx, idx->stream, idx->s_queries, idx->s_out, idx->s_stats, queries, nq, k, &c.dev)) ||
-        (rc = run(idx->s_queries.p, c.dev)) || (rc = queue_result_copies(idx->stream, c)))
+    if ((rc = reserve_host_call(idx, idx->s_queries, idx->s_out, idx->s_stats, nq, k, &c.dev)) ||
+        (rc = queue_query_copy(idx, idx->stream, idx->s_queries.p, queries, nq)) || (rc = run(idx->s_queries.p, c.dev)) ||
+        (rc = queue_result_copies(idx->stream, c)))
         return rc;
     DAB_CUDA(cudaStreamSynchronize(idx->stream));
     return DAB_OK;
 }
 
-// ---- batches in flight (dab_search_batch_async / dab_search_batch_device_async / dab_wait) ----
-struct SearchSlot {
-    cudaStream_t stream = nullptr;
-    Scratch tables, counters, queries, out, stats, h_counters;
-    SearchJob* job = nullptr;
-    HostCopy host_out{};  // the pending call's result copies (host_out.host.ids null: device buffers)
-};
-
+// ---- batches in flight (dab_search_batch[_pq|_sq|_minmax][_device]_async / dab_wait) ----
 void search_slots_release(dab_index* idx) {
     for (int i = 0; i < DAB_MAX_SLOTS; ++i) {
         SearchSlot* s = (SearchSlot*)idx->slots[i];
@@ -305,10 +298,20 @@ void search_slots_release(dab_index* idx) {
         if (s->stream) cudaStreamSynchronize(s->stream);
         delete s->job;
         s->tables.release(), s->counters.release(), s->queries.release(), s->out.release(), s->stats.release(), s->h_counters.release();
+        s->stage.release(), s->luts.release(), s->lists.release();
         if (s->stream) cudaStreamDestroy(s->stream);
         delete s;
         idx->slots[i] = nullptr;
     }
+}
+
+int retire_quantized_stores(dab_index* idx) {
+    for (int i = 0; i < DAB_MAX_SLOTS; ++i) {
+        const SearchSlot* s = (const SearchSlot*)idx->slots[i];
+        if (s && s->stream) DAB_CUDA(cudaStreamSynchronize(s->stream));
+    }
+    ++idx->stores_version;
+    return DAB_OK;
 }
 
 static int slot_of(dab_index* idx, uint32_t slot, SearchSlot** out) {
@@ -327,25 +330,52 @@ static int slot_of(dab_index* idx, uint32_t slot, SearchSlot** out) {
     return DAB_OK;
 }
 
-static int slot_launch(dab_index* idx, SearchSlot* s, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam,
-                       const SearchOut& d) {
+int slot_submit(dab_index* idx, const char* api, uint32_t slot, bool host, const void* queries, uint32_t nq, uint32_t k,
+                const SearchOut& out, const std::function<int(SearchSlot* s, const void* d_queries, const SearchOut& d_out, SlotJob** job)>& prepare) {
+    DAB_CUDA(cudaSetDevice(idx->device));
+    SearchSlot* s = nullptr;
+    int rc;
+    if ((rc = slot_of(idx, slot, &s))) return rc;
+    if (s->job) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: slot %u still has a batch in flight (call dab_wait)", api, slot);
+    if (nq == 0) return DAB_OK;
+    HostCopy c{out, SearchOut{}, nq, k};
+    if (host) {
+        c.host = out;
+        if ((rc = reserve_host_call(idx, s->queries, s->out, s->stats, nq, k, &c.dev))) return rc;
+    }
+    const void* d_queries = host ? s->queries.p : queries;
+    SlotJob* job = nullptr;
+    if ((rc = prepare(s, d_queries, c.dev, &job))) {
+        delete job;
+        return rc;
+    }
+    if ((host && (rc = queue_query_copy(idx, s->stream, s->queries.p, queries, nq))) || (rc = job->launch())) {
+        // a launch that failed half way (a CUDA error: every buffer was reserved by prepare) may have queued work that
+        // writes the caller's buffers: it completes before the error is returned, and the slot is idle
+        cudaStreamSynchronize(s->stream);
+        delete job;
+        return rc;
+    }
+    s->job = job;
+    s->host_out = c;
+    // optimistic copies: valid as they are unless a query overflowed (then dab_wait repeats them)
+    return host ? queue_result_copies(s->stream, c) : DAB_OK;
+}
+
+// a full-precision batch on slot `s`: every resident worker is launched (the next batch fills what this one leaves)
+static int prepare_search_job(dab_index* idx, SearchSlot* s, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                              uint32_t beam, const SearchOut& d, SlotJob** out) {
     int rc;
     if ((rc = s->h_counters.reserve(16))) return rc;
     SearchJob* job = new SearchJob();
+    *out = job;
     job->idx = idx;
     job->stream = s->stream;
     job->tables = &s->tables;
     job->counters = &s->counters;
     job->h_counters = (uint32_t*)s->h_counters.p;
     job->full_grid = true;
-    if ((rc = job->prepare(d_queries, nullptr, nq, k, l_search, beam, d.ids, d.dists, d.counts, d.cmps, d.hops, nullptr, nullptr,
-                           nullptr, 0)) ||
-        (rc = job->launch())) {
-        delete job;
-        return rc;
-    }
-    s->job = job;
-    return DAB_OK;
+    return job->prepare(d_queries, nullptr, nq, k, l_search, beam, d.ids, d.dists, d.counts, d.cmps, d.hops, nullptr, nullptr, nullptr, 0);
 }
 
 }  // namespace dab
@@ -387,18 +417,10 @@ int dab_search_batch_async(dab_index* idx, uint32_t slot, const void* queries, u
     if (nq && (!queries || !out_ids || !out_dists)) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_async: NULL argument");
     int rc;
     if ((rc = check_search_args(idx, k, l_search, beam_width))) return rc;
-    DAB_CUDA(cudaSetDevice(idx->device));
-    SearchSlot* s = nullptr;
-    if ((rc = slot_of(idx, slot, &s))) return rc;
-    if (s->job) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_async: slot %u still has a batch in flight (call dab_wait)", slot);
-    if (nq == 0) return DAB_OK;
-    HostCopy c{{}, SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, nq, k};
-    if ((rc = stage_host_call(idx, s->stream, s->queries, s->out, s->stats, queries, nq, k, &c.dev)) ||
-        (rc = slot_launch(idx, s, s->queries.p, nq, k, l_search, beam_width, c.dev)))
-        return rc;
-    s->host_out = c;
-    // optimistic copies: valid as they are unless a query overflowed (then dab_wait repeats them)
-    return queue_result_copies(s->stream, c);
+    return slot_submit(idx, "dab_search_batch_async", slot, true, queries, nq, k, SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops},
+                       [&](SearchSlot* s, const void* d_queries, const SearchOut& d, SlotJob** job) {
+                           return prepare_search_job(idx, s, d_queries, nq, k, l_search, beam_width, d, job);
+                       });
 }
 
 int dab_search_batch_device_async(dab_index* idx, uint32_t slot, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
@@ -408,30 +430,31 @@ int dab_search_batch_device_async(dab_index* idx, uint32_t slot, const void* d_q
     if (nq && (!d_queries || !d_out_ids || !d_out_dists)) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_device_async: NULL argument");
     int rc;
     if ((rc = check_search_args(idx, k, l_search, beam_width))) return rc;
-    DAB_CUDA(cudaSetDevice(idx->device));
-    SearchSlot* s = nullptr;
-    if ((rc = slot_of(idx, slot, &s))) return rc;
-    if (s->job) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_device_async: slot %u still has a batch in flight (call dab_wait)", slot);
-    if (nq == 0) return DAB_OK;
-    s->host_out = HostCopy{};
-    return slot_launch(idx, s, d_queries, nq, k, l_search, beam_width, SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops});
+    return slot_submit(idx, "dab_search_batch_device_async", slot, false, d_queries, nq, k,
+                       SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops},
+                       [&](SearchSlot* s, const void* dq, const SearchOut& d, SlotJob** job) {
+                           return prepare_search_job(idx, s, dq, nq, k, l_search, beam_width, d, job);
+                       });
 }
 
+// Joins a batch of any kind.  In the rare overflow case the job's re-runs (and, for a quantized batch with rerank, the
+// rerank of the whole batch) are queued again by finish: they are waited for here, after the result copies of a
+// host-buffer call are queued once more.
 int dab_wait(dab_index* idx, uint32_t slot) {
     if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_wait: idx is NULL");
     if (slot >= DAB_MAX_SLOTS) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_wait: slot %u out of range (DAB_MAX_SLOTS = %d)", slot, DAB_MAX_SLOTS);
     SearchSlot* s = (SearchSlot*)idx->slots[slot];
     if (!s || !s->job) return DAB_OK;
     DAB_CUDA(cudaSetDevice(idx->device));
-    SearchJob* job = s->job;
+    SlotJob* job = s->job;
     s->job = nullptr;
     DAB_CUDA(cudaStreamSynchronize(s->stream));
-    const bool overflowed = job->h_counters[1] != 0;
     int rc = job->finish();
+    const bool reran = job->reran;
     delete job;
     if (rc) return rc;
-    if (overflowed && s->host_out.host.ids) {
-        if ((rc = queue_result_copies(s->stream, s->host_out))) return rc;
+    if (reran) {
+        if (s->host_out.host.ids && (rc = queue_result_copies(s->stream, s->host_out))) return rc;
         DAB_CUDA(cudaStreamSynchronize(s->stream));
     }
     return DAB_OK;

@@ -411,8 +411,23 @@ __global__ void __launch_bounds__(kRerankWarps * 32) rerank_kernel(const RerankP
     }
 }
 
-static int launch_rerank(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t list_cap, const uint32_t* d_list,
-                         const uint32_t* d_list_n, uint32_t* d_ids, float* d_dists, uint32_t* d_counts) {
+// shared memory of one rerank_kernel warp: the query (i8 / u8 rows: as they are; float rows: f32), the list's ids and
+// distances
+static size_t rerank_warp_smem(bool is_int, uint32_t dim, uint32_t list_cap) {
+    return (is_int ? round_up((size_t)dim, 16) : round_up((size_t)dim * 4, 16)) + 2 * round_up((size_t)list_cap * 4, 16);
+}
+
+// the rerank of lists of list_cap entries fits a CTA of this index's schema
+static int check_rerank(const dab_index* idx, uint32_t list_cap) {
+    return visit_schema<OPS_ROW>(idx->dtype, idx->metric, [&](auto s) -> int {
+        const size_t smem = rerank_warp_smem(decltype(s)::IS_INT, idx->dim, list_cap) * kRerankWarps;
+        if (smem > 200 * 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "rerank: configuration needs %zu B shared memory per CTA", smem);
+        return DAB_OK;
+    });
+}
+
+static int launch_rerank(const dab_index* idx, cudaStream_t stream, const void* d_queries, uint32_t nq, uint32_t k, uint32_t list_cap,
+                         const uint32_t* d_list, const uint32_t* d_list_n, uint32_t* d_ids, float* d_dists, uint32_t* d_counts) {
     RerankParams p;
     memset(&p, 0, sizeof(p));
     p.vectors = idx->d_vectors;
@@ -431,17 +446,15 @@ static int launch_rerank(dab_index* idx, const void* d_queries, uint32_t nq, uin
     const int grid = (int)std::min<uint64_t>(((uint64_t)nq + kRerankWarps - 1) / kRerankWarps, (uint64_t)idx->sm_count * 8);
     const int rc = visit_schema<OPS_ROW>(idx->dtype, idx->metric, [&](auto s) -> int {
         using S = decltype(s);
-        size_t off = S::IS_INT ? round_up((size_t)idx->dim, 16) : round_up((size_t)idx->dim * 4, 16);
+        const size_t off = S::IS_INT ? round_up((size_t)idx->dim, 16) : round_up((size_t)idx->dim * 4, 16);
         p.off_ids = (uint32_t)off;
-        off += round_up((size_t)list_cap * 4, 16);
-        p.off_d = (uint32_t)off;
-        off += round_up((size_t)list_cap * 4, 16);
-        p.warp_smem = (uint32_t)off;
-        const size_t smem = off * kRerankWarps;
+        p.off_d = (uint32_t)(off + round_up((size_t)list_cap * 4, 16));
+        p.warp_smem = (uint32_t)rerank_warp_smem(S::IS_INT, idx->dim, list_cap);
+        const size_t smem = (size_t)p.warp_smem * kRerankWarps;
         if (smem > 200 * 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "rerank: configuration needs %zu B shared memory per CTA", smem);
         auto kern = rerank_kernel<typename S::TD, S::KIND, S::POST, S::NA>;
         DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, kRerankWarps * 32, smem, idx->stream>>>(p);
+        kern<<<grid, kRerankWarps * 32, smem, stream>>>(p);
         return DAB_OK;
     });
     if (rc) return rc;
@@ -450,9 +463,8 @@ static int launch_rerank(dab_index* idx, const void* d_queries, uint32_t nq, uin
     return DAB_OK;
 }
 
-static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam,
-                         uint32_t* d_ids, float* d_dists, uint32_t* d_counts, uint32_t* d_cmps, uint32_t* d_hops, bool rerank,
-                         int mode = 0) {
+// The checks of a quantized search that need no plan: arguments, the store, the metric, the list length
+static int check_pq_args(const dab_index* idx, uint32_t k, uint32_t l_search, uint32_t beam, int mode) {
     int rc;
     if ((rc = check_search_args(idx, k, l_search, beam, false))) return rc;
     if (mode == 0 && (!idx->d_pivots || !idx->d_codes || !idx->pq_codes_ready))
@@ -464,9 +476,65 @@ static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uin
     // SQStore::distance_computer (providers inmem/scalar.rs:214-226): UnsupportedDistanceMetric
     if (mode == 1 && idx->metric == DAB_COSINE)
         return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_sq: the scalar-quantized store supports L2, InnerProduct and CosineNormalized");
-    const uint32_t cap = l_search + idx->n_start;
-    if (cap > 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: L + #start must be <= 1024", mode == 2 ? "dab_search_batch_minmax" : "dab_search_batch_pq");
+    if (l_search + idx->n_start > 1024)
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: L + #start must be <= 1024", mode == 2 ? "dab_search_batch_minmax" : "dab_search_batch_pq");
+    return DAB_OK;
+}
+
+// ---- one quantized batch as a resumable job --------------------------------------------------
+// The quantized counterpart of SearchJob (search_kernel.cu).  `prepare` plans the batch (check_pq_args has passed),
+// makes the checks of the plan and reserves every buffer the first pass needs (nothing is queued); `launch` queues the staging of the queries (SQ, MinMax), the first traversal pass, the
+// read-back of its counters (and the MinMax NaN flag) into pinned memory and, optimistically, the rerank; `finish`
+// waits for the counters, learns the visited-set size, re-runs the queries whose visited set outgrew its table on
+// larger tables and then queues the rerank of the whole batch again.  The synchronous entry points run prepare, launch
+// and finish on the handle's stream and scratch; the *_async calls on a slot's.  A re-run reads the store the batch was
+// planned on: if a quantized store was replaced since (retire_quantized_stores), finish fails instead.
+struct PqSearchJob : SlotJob {
+    dab_index* idx = nullptr;
+    cudaStream_t stream = nullptr;
+    Scratch *tables = nullptr, *counters = nullptr, *stage = nullptr, *luts = nullptr, *lists = nullptr;
+    uint32_t* h_counters = nullptr;  // pinned: the four counters of a pass, then (u64 at word 4) the MinMax NaN flag
+
+    int mode = 0;
+    bool rerank = false;
+    const void* d_queries = nullptr;
+    uint32_t nq = 0, k = 0, l_search = 0, beam = 0, cap = 0;
     SearchParamsPq p;
+    PqsPlan plan;
+    bool use_pqs = false;
+    void (*kern)(const SearchParamsPq) = nullptr;
+    int grid = 0;
+    size_t smem_block = 0;
+    uint64_t slots = 0;
+    int pass = 0;
+    Scratch retry;
+    cudaEvent_t counted = nullptr;  // recorded after the read-back of a pass's counters
+    uint64_t stores_version = 0;    // idx->stores_version when the batch was planned
+
+    int prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint32_t l_search_, uint32_t beam_, const SearchOut& d, bool rerank_, int mode_);
+    int stage_queries();
+    int launch_traversal();
+    int launch() override;
+    int finish() override;
+    int launch_pass();
+    int reserve_tables();
+    unsigned long long first_nan() const { return *(const unsigned long long*)(h_counters + 4); }
+    int nan_error() const {
+        return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_minmax: query %llu contains NaN after the transform (InputContainsNaN)", first_nan());
+    }
+    ~PqSearchJob() override {
+        retry.release();
+        if (counted) cudaEventDestroy(counted);
+    }
+};
+
+int PqSearchJob::prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint32_t l_search_, uint32_t beam_, const SearchOut& d,
+                         bool rerank_, int mode_) {
+    d_queries = d_queries_, nq = nq_, k = k_, l_search = l_search_, beam = beam_, rerank = rerank_, mode = mode_;
+    stores_version = idx->stores_version;
+    int rc;
+    const CodeStore& store = mode == 2 ? idx->mm : idx->sq;  // modes 1 and 2
+    cap = l_search + idx->n_start;
     memset(&p, 0, sizeof(p));
     p.adj = idx->d_adj;
     p.adj_stride = idx->adj_stride;
@@ -499,11 +567,11 @@ static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uin
         p.sq_scale_squared = idx->sq_scale * idx->sq_scale;  // AsFunctor (scalar/quantizer.rs:316-335)
         p.sq_shift_square_norm = idx->sq_shift_square_norm;
     }
-    p.out_ids = d_ids;
-    p.out_dists = d_dists;
-    p.out_counts = d_counts;
-    p.out_cmps = d_cmps;
-    p.out_hops = d_hops;
+    p.out_ids = d.ids;
+    p.out_dists = d.dists;
+    p.out_counts = d.counts;
+    p.out_cmps = d.cmps;
+    p.out_hops = d.hops;
 
     size_t off = 0;
     p.off_q = 0;
@@ -529,12 +597,9 @@ static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uin
     p.warp_smem = (uint32_t)round_up(off, 16);
     // table metrics with a pivot table that fits shared memory: search_kernel_pqs (pivots resident per SM, entries
     // computed on the fly); everything else — SQ, DirectCosine, wide pivots, > 32 chunks — the per-warp kernel below
-    PqsPlan plan;
     memset(&plan, 0, sizeof(plan));
-    const bool use_pqs = mode == 0 && !p.direct_cosine && pqs_plan(idx, p.warp_smem, nq, &plan);
-    const size_t smem_block = (size_t)p.warp_smem * kPqWarps;
-    void (*kern)(const SearchParamsPq) = nullptr;
-    int grid;
+    use_pqs = mode == 0 && !p.direct_cosine && pqs_plan(idx, p.warp_smem, nq, &plan);
+    smem_block = (size_t)p.warp_smem * kPqWarps;
     uint32_t warps;
     if (use_pqs) {
         p.piv_stride = plan.piv_stride;
@@ -558,59 +623,156 @@ static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uin
         warps = (uint32_t)grid * kPqWarps;
     }
 
-    if ((rc = idx->s_counters.reserve(16 + (size_t)nq * 4)) || (rc = idx->h_counters.reserve(16))) return rc;
-    p.counters = (uint32_t*)idx->s_counters.p;
+    if ((rc = counters->reserve(16 + (size_t)nq * 4))) return rc;
+    p.counters = (uint32_t*)counters->p;
     p.overflow_list = p.counters + 4;
-    uint32_t* h_counters = (uint32_t*)idx->h_counters.p;
     const size_t lut_bytes = mode == 0 && !use_pqs ? (size_t)warps * idx->pq_chunks * idx->pq_centers * 4 : 16;
-    if ((rc = idx->s_out2.reserve(lut_bytes))) return rc;
-    p.luts = (float*)idx->s_out2.p;
+    if ((rc = luts->reserve(lut_bytes))) return rc;
+    p.luts = (float*)luts->p;
     p.n_work = nq;
     if (rerank) {
         if (!idx->vectors_ready) return fail(DAB_ERR_NOT_READY, "dab_search_batch_pq: rerank needs the full-precision vectors");
-        if ((rc = idx->s_ids.reserve(((size_t)nq * cap + nq) * 4))) return rc;
-        p.list_ids = (uint32_t*)idx->s_ids.p;
+        if ((rc = check_rerank(idx, cap))) return rc;
+        if ((rc = lists->reserve(((size_t)nq * cap + nq) * 4))) return rc;
+        p.list_ids = (uint32_t*)lists->p;
         p.list_counts = p.list_ids + (size_t)nq * cap;
         p.list_cap = cap;
     }
-    if (mode != 0 && (rc = (mode == 1 ? sq_stage_queries : minmax_stage_queries)(idx, d_queries, nq, &p.query_codes, &p.query_meta))) return rc;
     // global-table passes: the overflowed queries of one are re-run on larger tables in the next
-    uint64_t slots = table_slots(idx, idx->pq_hint, l_search, beam, mode);
-    Scratch retry;
-    rc = [&]() -> int {
-        for (int pass = 0;;) {
-            int rc2;
-            p.n_buckets = (uint32_t)((slots + 7) / 8);
-            if ((rc2 = idx->s_tables.reserve((size_t)warps * p.n_buckets * 32))) return rc2;
-            p.tables = (uint32_t*)idx->s_tables.p;
-            DAB_CUDA(cudaMemsetAsync(p.counters, 0, 16, idx->stream));
-            if (use_pqs) {
-                if ((rc2 = pqs_launch(idx, p, plan, cap))) return rc2;
-            } else {
-                kern<<<grid, kPqWarps * 32, smem_block, idx->stream>>>(p);
-                DAB_LAUNCHED();
-                DAB_CUDA(cudaGetLastError());
-            }
-            DAB_CUDA(cudaMemcpyAsync(h_counters, p.counters, 16, cudaMemcpyDeviceToHost, idx->stream));
-            DAB_CUDA(cudaStreamSynchronize(idx->stream));
-            learn_visited(idx->pq_hint, l_search, beam, mode, h_counters[2]);
-            const uint32_t n_over = h_counters[1];
-            if (n_over == 0) return DAB_OK;
-            if ((rc2 = take_overflow_list(idx->stream, p.overflow_list, n_over, retry)) || (rc2 = grow_visited_tables(idx, pass, slots)))
-                return rc2;
-            p.query_list = (const uint32_t*)retry.p;
-            p.n_work = n_over;
-        }
-    }();
-    retry.release();
-    if (rc) return rc;
-    return rerank ? launch_rerank(idx, d_queries, nq, k, cap, p.list_ids, p.list_counts, d_ids, d_dists, d_counts) : DAB_OK;
+    slots = table_slots(idx, idx->pq_hint, l_search, beam, mode);
+    pass = 0;
+    if ((rc = reserve_tables())) return rc;
+    if ((rc = stage->reserve(mode == 1 ? sq_stage_bytes(idx, nq) : mode == 2 ? minmax_stage_bytes(idx, nq) : 0))) return rc;
+    DAB_CUDA(cudaEventCreateWithFlags(&counted, cudaEventDisableTiming));
+    return DAB_OK;
+}
+
+// SQ and MinMax: the batch's queries compressed by the store's quantizer (MinMax: the NaN flag read back into h_counters)
+int PqSearchJob::stage_queries() {
+    if (mode == 1) return sq_stage_queries(idx, stream, *stage, d_queries, nq, &p.query_codes, &p.query_meta);
+    if (mode == 2) return minmax_stage_queries(idx, stream, *stage, d_queries, nq, (unsigned long long*)(h_counters + 4), &p.query_codes, &p.query_meta);
+    return DAB_OK;
+}
+
+// a visited table of `slots` ids per resident warp
+int PqSearchJob::reserve_tables() {
+    int rc;
+    p.n_buckets = (uint32_t)((slots + 7) / 8);
+    const size_t warps = use_pqs ? (size_t)plan.grid * plan.warps : (size_t)grid * kPqWarps;
+    if ((rc = tables->reserve(warps * p.n_buckets * 32))) return rc;
+    p.tables = (uint32_t*)tables->p;
+    return DAB_OK;
+}
+
+// one traversal pass over p.n_work queries (tables reserved) and the read-back of its counters
+int PqSearchJob::launch_pass() {
+    int rc;
+    DAB_CUDA(cudaMemsetAsync(p.counters, 0, 16, stream));
+    if (use_pqs) {
+        if ((rc = pqs_launch(p, plan, cap, stream))) return rc;
+    } else {
+        kern<<<grid, kPqWarps * 32, smem_block, stream>>>(p);
+        DAB_LAUNCHED();
+        DAB_CUDA(cudaGetLastError());
+    }
+    DAB_CUDA(cudaMemcpyAsync(h_counters, p.counters, 16, cudaMemcpyDeviceToHost, stream));
+    DAB_CUDA(cudaEventRecord(counted, stream));
+    return DAB_OK;
+}
+
+// the first pass and, optimistically, the rerank
+int PqSearchJob::launch_traversal() {
+    int rc;
+    if ((rc = launch_pass())) return rc;
+    return rerank ? launch_rerank(idx, stream, d_queries, nq, k, cap, p.list_ids, p.list_counts, p.out_ids, p.out_dists, p.out_counts) : DAB_OK;
+}
+
+int PqSearchJob::launch() {
+    int rc;
+    if ((rc = stage_queries())) return rc;
+    return launch_traversal();
+}
+
+int PqSearchJob::finish() {
+    DAB_CUDA(cudaEventSynchronize(counted));
+    if (mode == 2 && first_nan() != ~0ull) return nan_error();
+    for (;;) {
+        learn_visited(idx->pq_hint, l_search, beam, mode, h_counters[2]);
+        const uint32_t n_over = h_counters[1];
+        if (n_over == 0) break;
+        // the store the batch was planned on has been freed: its overflowed queries cannot be re-run
+        if (idx->stores_version != stores_version)
+            return fail(DAB_ERR_INVALID_ARGUMENT, "dab_wait: a quantized store was replaced while the batch was in flight; "
+                                                  "%u of its queries could not be re-run", n_over);
+        int rc;
+        if ((rc = take_overflow_list(stream, p.overflow_list, n_over, retry)) || (rc = grow_visited_tables(idx, pass, slots)) ||
+            (rc = reserve_tables()))
+            return rc;
+        p.query_list = (const uint32_t*)retry.p;
+        p.n_work = n_over;
+        reran = true;
+        if ((rc = launch_pass())) return rc;
+        DAB_CUDA(cudaEventSynchronize(counted));
+    }
+    // the rerank queued by launch read lists that the re-runs have since rewritten
+    if (reran && rerank) return launch_rerank(idx, stream, d_queries, nq, k, cap, p.list_ids, p.list_counts, p.out_ids, p.out_dists, p.out_counts);
+    return DAB_OK;
+}
+
+// The synchronous calls: the job on the handle's stream and scratch.  A MinMax batch with a NaN query fails before any
+// traversal is launched.  Device pointers only; returns once the traversal is complete (the rerank may still run).
+static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam,
+                         const SearchOut& d, bool rerank, int mode) {
+    int rc;
+    if ((rc = idx->h_counters.reserve(24))) return rc;
+    PqSearchJob job;
+    job.idx = idx;
+    job.stream = idx->stream;
+    job.tables = &idx->s_tables, job.counters = &idx->s_counters, job.stage = &idx->s_stage, job.luts = &idx->s_out2, job.lists = &idx->s_ids;
+    job.h_counters = (uint32_t*)idx->h_counters.p;
+    if ((rc = check_pq_args(idx, k, l_search, beam, mode)) || (rc = job.prepare(d_queries, nq, k, l_search, beam, d, rerank, mode))) return rc;
+    if ((rc = job.stage_queries())) return rc;
+    if (mode == 2) {
+        DAB_CUDA(cudaStreamSynchronize(idx->stream));
+        if (job.first_nan() != ~0ull) return job.nan_error();
+    }
+    if ((rc = job.launch_traversal())) return rc;
+    return job.finish();
 }
 
 static int search_pq_host(dab_index* idx, const char* api, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
                           uint32_t beam_width, const SearchOut& out, bool rerank, int mode) {
     return search_host_buffers(idx, api, queries, nq, k, out, [&](const void* d_queries, const SearchOut& d) {
-        return run_search_pq(idx, d_queries, nq, k, l_search, beam_width, d.ids, d.dists, d.counts, d.cmps, d.hops, rerank, mode);
+        return run_search_pq(idx, d_queries, nq, k, l_search, beam_width, d, rerank, mode);
+    });
+}
+
+static int search_pq_device(dab_index* idx, const char* api, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                            uint32_t beam_width, const SearchOut& d, bool rerank, int mode) {
+    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", api);
+    if (nq == 0) return DAB_OK;
+    if (!d_queries || !d.ids || !d.dists) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
+    DAB_CUDA(cudaSetDevice(idx->device));
+    return run_search_pq(idx, d_queries, nq, k, l_search, beam_width, d, rerank, mode);
+}
+
+// The *_async calls: the job on the slot's stream and scratch
+static int search_pq_async(dab_index* idx, const char* api, uint32_t slot, bool host, const void* queries, uint32_t nq, uint32_t k,
+                           uint32_t l_search, uint32_t beam_width, const SearchOut& out, bool rerank, int mode) {
+    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", api);
+    if (nq && (!queries || !out.ids || !out.dists)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
+    int rc;
+    if ((rc = check_pq_args(idx, k, l_search, beam_width, mode))) return rc;  // before the slot rules, as the full-precision call
+    return slot_submit(idx, api, slot, host, queries, nq, k, out, [&](SearchSlot* s, const void* d_queries, const SearchOut& d, SlotJob** out_job) {
+        int rc2;
+        if ((rc2 = s->h_counters.reserve(24))) return rc2;
+        PqSearchJob* job = new PqSearchJob();
+        *out_job = job;
+        job->idx = idx;
+        job->stream = s->stream;
+        job->tables = &s->tables, job->counters = &s->counters, job->stage = &s->stage, job->luts = &s->luts, job->lists = &s->lists;
+        job->h_counters = (uint32_t*)s->h_counters.p;
+        return job->prepare(d_queries, nq, k, l_search, beam_width, d, rerank, mode);
     });
 }
 
@@ -635,11 +797,8 @@ int dab_search_batch_pq_rerank(dab_index* idx, const void* queries, uint32_t nq,
 int dab_search_batch_pq_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
                                int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts, uint32_t* d_out_cmps,
                                uint32_t* d_out_hops) {
-    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_pq_device: idx is NULL");
-    if (nq == 0) return DAB_OK;
-    if (!d_queries || !d_out_ids || !d_out_dists) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_pq_device: NULL argument");
-    DAB_CUDA(cudaSetDevice(idx->device));
-    return run_search_pq(idx, d_queries, nq, k, l_search, beam_width, d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops, rerank != 0);
+    return search_pq_device(idx, "dab_search_batch_pq_device", d_queries, nq, k, l_search, beam_width,
+                            SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, 0);
 }
 
 int dab_search_batch_sq(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
@@ -651,11 +810,8 @@ int dab_search_batch_sq(dab_index* idx, const void* queries, uint32_t nq, uint32
 int dab_search_batch_sq_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
                                int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts, uint32_t* d_out_cmps,
                                uint32_t* d_out_hops) {
-    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_sq_device: idx is NULL");
-    if (nq == 0) return DAB_OK;
-    if (!d_queries || !d_out_ids || !d_out_dists) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_sq_device: NULL argument");
-    DAB_CUDA(cudaSetDevice(idx->device));
-    return run_search_pq(idx, d_queries, nq, k, l_search, beam_width, d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops, rerank != 0, 1);
+    return search_pq_device(idx, "dab_search_batch_sq_device", d_queries, nq, k, l_search, beam_width,
+                            SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, 1);
 }
 
 int dab_search_batch_minmax(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
@@ -667,11 +823,51 @@ int dab_search_batch_minmax(dab_index* idx, const void* queries, uint32_t nq, ui
 int dab_search_batch_minmax_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
                                    int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts, uint32_t* d_out_cmps,
                                    uint32_t* d_out_hops) {
-    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_minmax_device: idx is NULL");
-    if (nq == 0) return DAB_OK;
-    if (!d_queries || !d_out_ids || !d_out_dists) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_minmax_device: NULL argument");
-    DAB_CUDA(cudaSetDevice(idx->device));
-    return run_search_pq(idx, d_queries, nq, k, l_search, beam_width, d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops, rerank != 0, 2);
+    return search_pq_device(idx, "dab_search_batch_minmax_device", d_queries, nq, k, l_search, beam_width,
+                            SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, 2);
+}
+
+// ---- asynchronous batches (see dab_search_batch_async): the same jobs on a slot, joined by dab_wait ----
+int dab_search_batch_pq_async(dab_index* idx, uint32_t slot, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                              uint32_t beam_width, int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
+                              uint32_t* out_cmps, uint32_t* out_hops) {
+    return search_pq_async(idx, "dab_search_batch_pq_async", slot, true, queries, nq, k, l_search, beam_width,
+                           SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, rerank != 0, 0);
+}
+
+int dab_search_batch_pq_device_async(dab_index* idx, uint32_t slot, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                                     uint32_t beam_width, int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
+                                     uint32_t* d_out_cmps, uint32_t* d_out_hops) {
+    return search_pq_async(idx, "dab_search_batch_pq_device_async", slot, false, d_queries, nq, k, l_search, beam_width,
+                           SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, 0);
+}
+
+int dab_search_batch_sq_async(dab_index* idx, uint32_t slot, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                              uint32_t beam_width, int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
+                              uint32_t* out_cmps, uint32_t* out_hops) {
+    return search_pq_async(idx, "dab_search_batch_sq_async", slot, true, queries, nq, k, l_search, beam_width,
+                           SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, rerank != 0, 1);
+}
+
+int dab_search_batch_sq_device_async(dab_index* idx, uint32_t slot, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                                     uint32_t beam_width, int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
+                                     uint32_t* d_out_cmps, uint32_t* d_out_hops) {
+    return search_pq_async(idx, "dab_search_batch_sq_device_async", slot, false, d_queries, nq, k, l_search, beam_width,
+                           SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, 1);
+}
+
+int dab_search_batch_minmax_async(dab_index* idx, uint32_t slot, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                                  uint32_t beam_width, int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
+                                  uint32_t* out_cmps, uint32_t* out_hops) {
+    return search_pq_async(idx, "dab_search_batch_minmax_async", slot, true, queries, nq, k, l_search, beam_width,
+                           SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, rerank != 0, 2);
+}
+
+int dab_search_batch_minmax_device_async(dab_index* idx, uint32_t slot, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                                         uint32_t beam_width, int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
+                                         uint32_t* d_out_cmps, uint32_t* d_out_hops) {
+    return search_pq_async(idx, "dab_search_batch_minmax_device_async", slot, false, d_queries, nq, k, l_search, beam_width,
+                           SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, 2);
 }
 
 }  // extern "C"

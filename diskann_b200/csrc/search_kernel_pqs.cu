@@ -378,7 +378,7 @@ bool pqs_plan(const dab_index* idx, uint32_t warp_smem, uint32_t nq, PqsPlan* ou
     return true;
 }
 
-int pqs_launch(dab_index* idx, const SearchParamsPq& p, const PqsPlan& plan, uint32_t cap) {
+int pqs_launch(const SearchParamsPq& p, const PqsPlan& plan, uint32_t cap, cudaStream_t stream) {
     void (*kern)(const SearchParamsPq);
 #define DAB_PQS_PICK(CL_)                                                                                        \
     kern = cap <= 128 ? search_kernel_pqs<4, CL_> : cap <= 256 ? search_kernel_pqs<8, CL_> : cap <= 512 ? search_kernel_pqs<16, CL_> : search_kernel_pqs<32, CL_>
@@ -387,7 +387,7 @@ int pqs_launch(dab_index* idx, const SearchParamsPq& p, const PqsPlan& plan, uin
     else DAB_PQS_PICK(0);
 #undef DAB_PQS_PICK
     DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem));
-    kern<<<plan.grid, plan.warps * 32, plan.smem, idx->stream>>>(p);
+    kern<<<plan.grid, plan.warps * 32, plan.smem, stream>>>(p);
     DAB_LAUNCHED();
     DAB_CUDA(cudaGetLastError());
     return DAB_OK;

@@ -67,16 +67,22 @@ struct PqsPlan {
 };
 // false: this index / call does not fit the kernel (pivot table too large for shared memory, > 32 chunks, ...)
 bool pqs_plan(const dab_index* idx, uint32_t warp_smem, uint32_t nq, PqsPlan* out);
-int pqs_launch(dab_index* idx, const SearchParamsPq& p, const PqsPlan& plan, uint32_t cap);
+int pqs_launch(const SearchParamsPq& p, const PqsPlan& plan, uint32_t cap, cudaStream_t stream);
 
 // The query side of the packed-code traversals: the nq queries d_queries (index dtype, device memory) are compressed by
-// the store's own quantizer on the index's stream into codes [nq][stride] and one float4 per query in the store's
-// layout, in the index's staging scratch (stage_query_buffers).
+// the store's own quantizer on `stream` into codes [nq][stride] and one float4 per query in the store's layout, in the
+// staging scratch `stage` (stage_query_buffers).  Nothing waits.
 // sq_index.cu: as_f32, the InnerProduct rescale, ScalarQuantizer::compress; the compensation in .x.  A NaN packs as 0.
-int sq_stage_queries(dab_index* idx, const void* d_queries, uint32_t nq, const uint8_t** d_qcodes, const float4** d_qmeta);
-// minmax_index.cu: as_f32, the store's transform, its compressor; {b, n, a, norm_squared}.  Fails naming the first
-// query whose transformed vector holds a NaN.
-int minmax_stage_queries(dab_index* idx, const void* d_queries, uint32_t nq, const uint8_t** d_qcodes, const float4** d_qmeta);
+int sq_stage_queries(const dab_index* idx, cudaStream_t stream, Scratch& stage, const void* d_queries, uint32_t nq, const uint8_t** d_qcodes,
+                     const float4** d_qmeta);
+// minmax_index.cu: as_f32, the store's transform, its compressor; {b, n, a, norm_squared}.  The index of the first query
+// whose transformed vector holds a NaN (~0 if none) is copied to *h_first_nan (pinned host memory) on `stream`: it is
+// valid once the stream has passed this point.
+int minmax_stage_queries(const dab_index* idx, cudaStream_t stream, Scratch& stage, const void* d_queries, uint32_t nq,
+                         unsigned long long* h_first_nan, const uint8_t** d_qcodes, const float4** d_qmeta);
+// the staging scratch each of the two needs for nq queries, reserved before anything of a batch is queued
+size_t sq_stage_bytes(const dab_index* idx, uint32_t nq);
+size_t minmax_stage_bytes(const dab_index* idx, uint32_t nq);
 
 
 }  // namespace dab

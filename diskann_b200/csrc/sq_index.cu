@@ -103,16 +103,19 @@ __global__ void __launch_bounds__(128) sq_stage_kernel(const T* __restrict__ que
 
 }  // namespace
 
-int sq_stage_queries(dab_index* idx, const void* d_queries, uint32_t nq, const uint8_t** d_qcodes, const float4** d_qmeta) {
+size_t sq_stage_bytes(const dab_index* idx, uint32_t nq) { return stage_query_bytes(idx->sq, nq, (size_t)nq * idx->dim * 4); }
+
+int sq_stage_queries(const dab_index* idx, cudaStream_t stream, Scratch& stage, const void* d_queries, uint32_t nq, const uint8_t** d_qcodes,
+                     const float4** d_qmeta) {
     int rc;
     uint8_t* qcodes;
     float4* qmeta;
-    if ((rc = stage_query_buffers(idx, idx->sq, nq, (size_t)nq * idx->dim * 4, &qcodes, &qmeta))) return rc;
+    if ((rc = stage_query_buffers(idx->sq, stage, nq, (size_t)nq * idx->dim * 4, &qcodes, &qmeta))) return rc;  // work: the f32 queries
     const bool rescale = idx->metric == DAB_INNER_PRODUCT && idx->sq_mean_norm != 0.0f;
     const int grid = (int)(((uint64_t)nq + 3) / 4);
     auto launch = [&](auto* queries) {
-        sq_stage_kernel<<<grid, 128, 0, idx->stream>>>(queries, nq, (int)idx->dim, idx->d_sq_shift, idx->sq_scale, idx->sq_mean_norm, rescale,
-                                                       idx->sq.nbits, idx->sq.stride, (float*)idx->s_stage.p, (uint32_t*)qcodes, qmeta);
+        sq_stage_kernel<<<grid, 128, 0, stream>>>(queries, nq, (int)idx->dim, idx->d_sq_shift, idx->sq_scale, idx->sq_mean_norm, rescale,
+                                                  idx->sq.nbits, idx->sq.stride, (float*)stage.p, (uint32_t*)qcodes, qmeta);
     };
     switch (idx->dtype) {
         case DAB_F32: launch((const float*)d_queries); break;
@@ -141,6 +144,8 @@ int dab_upload_sq(dab_index* idx, int nbits, const float* shift, float scale, fl
     if (!(scale > 0.0f)) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_upload_sq: scale must be positive");  // ScalarQuantizer::new
     DAB_CUDA(cudaSetDevice(idx->device));
     DAB_CUDA(cudaStreamSynchronize(idx->stream));
+    int rc;
+    if ((rc = retire_quantized_stores(idx))) return rc;  // batches in flight read the store
     store_release(idx->sq);
     cudaFree(idx->d_sq_shift);
     idx->d_sq_shift = nullptr;
@@ -149,7 +154,6 @@ int dab_upload_sq(dab_index* idx, int nbits, const float* shift, float scale, fl
     idx->sq_scale = scale;
     idx->sq_shift_square_norm = shift_square_norm;
     idx->sq_mean_norm = mean_norm;
-    int rc;
     if ((rc = store_alloc(idx, idx->sq, nbits, idx->dim, false, 1))) return rc;  // the header: one f32 compensation
     return rows ? store_upload(idx, idx->sq, rows, "dab_upload_sq") : DAB_OK;
 }

@@ -424,6 +424,53 @@ class GpuIndex:
                                                        C.c_void_p(d_ids), C.c_void_p(d_dists), C.c_void_p(d_counts or None),
                                                        C.c_void_p(d_cmps or None), C.c_void_p(d_hops or None)))
 
+    def _quantized_async(self, fn, slot, queries, k, l_search, beam_width, rerank, out):
+        queries = self._queries(queries)
+        nq = queries.shape[0]
+        if out is None:
+            out = (np.empty((nq, k), np.uint32), np.empty((nq, k), np.float32), np.empty(nq, np.uint32),
+                   np.empty(nq, np.uint32), np.empty(nq, np.uint32))
+        ids, dists, counts, cmps, hops = out
+        check(fn(self._h, slot, _ptr(queries), nq, k, l_search, beam_width, int(bool(rerank)), _ptr(ids), _ptr(dists),
+                 _ptr(counts), _ptr(cmps), _ptr(hops)))
+        self._inflight[slot] = (queries, out)
+        return out
+
+    def _quantized_device_async(self, fn, slot, d_queries, nq, k, l_search, beam_width, d_ids, d_dists, d_counts, d_cmps, d_hops,
+                                rerank):
+        check(fn(self._h, slot, C.c_void_p(d_queries), nq, k, l_search, beam_width, int(bool(rerank)), C.c_void_p(d_ids),
+                 C.c_void_p(d_dists), C.c_void_p(d_counts or None), C.c_void_p(d_cmps or None), C.c_void_p(d_hops or None)))
+
+    def search_batch_pq_async(self, slot, queries, k, l_search, beam_width=1, rerank=False, out=None):
+        """search_batch_pq as a batch in flight on `slot`: returns the output arrays that wait(slot) fills (see
+        search_batch_async)."""
+        return self._quantized_async(_lib.lib().dab_search_batch_pq_async, slot, queries, k, l_search, beam_width, rerank, out)
+
+    def search_batch_pq_device_async(self, slot, d_queries, nq, k, l_search, beam_width, d_ids, d_dists, d_counts=0, d_cmps=0,
+                                     d_hops=0, rerank=True):
+        """Device-pointer flavour of search_batch_pq_async; results stay in HBM."""
+        self._quantized_device_async(_lib.lib().dab_search_batch_pq_device_async, slot, d_queries, nq, k, l_search, beam_width,
+                                     d_ids, d_dists, d_counts, d_cmps, d_hops, rerank)
+
+    def search_batch_sq_async(self, slot, queries, k, l_search, beam_width=1, rerank=False, out=None):
+        """search_batch_sq as a batch in flight on `slot`: returns the output arrays that wait(slot) fills."""
+        return self._quantized_async(_lib.lib().dab_search_batch_sq_async, slot, queries, k, l_search, beam_width, rerank, out)
+
+    def search_batch_sq_device_async(self, slot, d_queries, nq, k, l_search, beam_width, d_ids, d_dists, d_counts=0, d_cmps=0,
+                                     d_hops=0, rerank=True):
+        self._quantized_device_async(_lib.lib().dab_search_batch_sq_device_async, slot, d_queries, nq, k, l_search, beam_width,
+                                     d_ids, d_dists, d_counts, d_cmps, d_hops, rerank)
+
+    def search_batch_minmax_async(self, slot, queries, k, l_search, beam_width=1, rerank=False, out=None):
+        """search_batch_minmax as a batch in flight on `slot`: returns the output arrays that wait(slot) fills.  A query
+        holding a NaN after the transform makes wait(slot) fail."""
+        return self._quantized_async(_lib.lib().dab_search_batch_minmax_async, slot, queries, k, l_search, beam_width, rerank, out)
+
+    def search_batch_minmax_device_async(self, slot, d_queries, nq, k, l_search, beam_width, d_ids, d_dists, d_counts=0, d_cmps=0,
+                                         d_hops=0, rerank=False):
+        self._quantized_device_async(_lib.lib().dab_search_batch_minmax_device_async, slot, d_queries, nq, k, l_search, beam_width,
+                                     d_ids, d_dists, d_counts, d_cmps, d_hops, rerank)
+
     def wait(self, slot):
         """Join the batch in flight on `slot` (no-op when idle)."""
         check(_lib.lib().dab_wait(self._h, slot))

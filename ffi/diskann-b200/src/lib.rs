@@ -174,6 +174,39 @@ impl<T: Element> GpuIndex<T> {
         Ok(b)
     }
 
+    /// `search_batch_pq_rerank` (`rerank`) or the PQ traversal alone, queued on `slot` without waiting: the quantized
+    /// counterpart of `search_batch_async`, with bit-identical results.  Slots are shared by batches of every kind.
+    pub fn search_batch_pq_async<'a>(&'a self, slot: u32, queries: &'a [T], k: usize, l_search: u32, beam_width: u32, rerank: bool)
+        -> Result<InFlight<'a, T>> {
+        self.quantized_async(sys::dab_search_batch_pq_async, slot, queries, k, l_search, beam_width, rerank)
+    }
+
+    /// `search_batch_sq` queued on `slot` without waiting.
+    pub fn search_batch_sq_async<'a>(&'a self, slot: u32, queries: &'a [T], k: usize, l_search: u32, beam_width: u32, rerank: bool)
+        -> Result<InFlight<'a, T>> {
+        self.quantized_async(sys::dab_search_batch_sq_async, slot, queries, k, l_search, beam_width, rerank)
+    }
+
+    /// `search_batch_minmax` queued on `slot` without waiting.  A query holding a NaN after the transform makes
+    /// `InFlight::wait` fail with the synchronous call's error.
+    pub fn search_batch_minmax_async<'a>(&'a self, slot: u32, queries: &'a [T], k: usize, l_search: u32, beam_width: u32, rerank: bool)
+        -> Result<InFlight<'a, T>> {
+        self.quantized_async(sys::dab_search_batch_minmax_async, slot, queries, k, l_search, beam_width, rerank)
+    }
+
+    #[allow(clippy::too_many_arguments)]
+    fn quantized_async<'a>(&'a self, launch: QuantizedAsync, slot: u32, queries: &'a [T], k: usize, l_search: u32, beam_width: u32,
+                           rerank: bool) -> Result<InFlight<'a, T>> {
+        assert_eq!(queries.len() % self.dim, 0);
+        let nq = queries.len() / self.dim;
+        let mut b = Batch { k, ids: vec![0; nq * k], dists: vec![0.0; nq * k], counts: vec![0; nq], cmps: vec![0; nq], hops: vec![0; nq] };
+        check(unsafe {
+            launch(self.raw, slot, queries.as_ptr() as *const c_void, nq as u32, k as u32, l_search, beam_width, rerank as i32,
+                   b.ids.as_mut_ptr(), b.dists.as_mut_ptr(), b.counts.as_mut_ptr(), b.cmps.as_mut_ptr(), b.hops.as_mut_ptr())
+        })?;
+        Ok(InFlight { index: self, slot, batch: Some(b), _queries: queries })
+    }
+
     /// One process per GPU: join the communicator described by `id` (from `unique_id()` on rank 0) …
     pub fn comm_init(&mut self, id: &[u8; 128], n_ranks: i32, rank: i32) -> Result<()> {
         check(unsafe { sys::dab_comm_init(self.raw, id.as_ptr() as *const _, n_ranks, rank) })
@@ -184,6 +217,10 @@ impl<T: Element> GpuIndex<T> {
         check(unsafe { sys::dab_broadcast_index(self.raw, root) })
     }
 }
+
+/// The host-buffer `_async` entry points of the quantized traversals (one signature for PQ, SQ and MinMax).
+type QuantizedAsync = unsafe extern "C" fn(*mut sys::dab_index, u32, *const c_void, u32, u32, u32, u32, std::os::raw::c_int, *mut u32,
+                                           *mut f32, *mut u32, *mut u32, *mut u32) -> std::os::raw::c_int;
 
 /// A batch in flight on one slot of the device.  Dropping it joins the slot (the library writes into the
 /// buffers it owns until then).

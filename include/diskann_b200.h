@@ -190,6 +190,49 @@ int dab_search_batch_device_async(dab_index* idx, uint32_t slot, const void* d_q
                                   uint32_t* d_out_hops);
 int dab_wait(dab_index* idx, uint32_t slot);
 
+/* The PQ, SQ and MinMax traversals (below) as batches in flight: each call takes the arguments
+ * of its synchronous twin plus `slot`, queues the whole batch on the slot's stream (the copy of the queries, their
+ * compression by the store's quantizer for SQ and MinMax, the traversal, the rerank when `rerank` is set, the copies of
+ * the results) and returns without waiting; dab_wait(slot) joins a batch of any kind.
+ *   Results: ids, distance bits, counts, cmps and hops are bit-identical to the synchronous call with the same
+ *     arguments — dab_search_batch_pq (or dab_search_batch_pq_rerank when rerank is set), dab_search_batch_sq,
+ *     dab_search_batch_minmax — including when queries outgrow their visited tables: dab_wait re-runs them, then runs
+ *     the rerank over the whole batch again and repeats the copies of the host-buffer flavour.
+ *   Launch-time errors: every error the synchronous call reports before it launches anything (a store that is not
+ *     ready, Metric::Cosine on the SQ store, L + #start > 1024, NULL buffers, rerank without the full-precision rows)
+ *     is reported by the launching call, and nothing is queued; so are a slot out of range and a slot that still holds
+ *     a batch of any kind (full precision included).
+ *   MinMax NaN query: the launching call does not wait for the query compression.  dab_wait returns
+ *     DAB_ERR_INVALID_ARGUMENT with the synchronous call's message ("query %llu contains NaN after the transform");
+ *     the outputs are then unspecified and the slot is idle.  (The synchronous call still fails before any traversal.)
+ *   The launching calls never wait on the device; the only waits are dab_wait's.
+ *   Buffers: as dab_search_batch_async — the host buffers (pinned memory makes the copies asynchronous) and the device
+ *     buffers of the `_device_` flavour stay valid and untouched until dab_wait(slot) returns, and the graph and the
+ *     stores must not change while a batch is in flight.  dab_upload_pq, dab_pq_train, dab_upload_sq,
+ *     dab_upload_minmax and dab_broadcast_index wait for every slot before they free a store, and a batch launched on
+ *     the replaced store never runs again: if some of its queries still need a re-run, dab_wait returns
+ *     DAB_ERR_INVALID_ARGUMENT instead.  So a caller who breaks that rule gets unspecified results or that error,
+ *     never a freed buffer under a running kernel. */
+int dab_search_batch_pq_async(dab_index* idx, uint32_t slot, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                              uint32_t beam_width, int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
+                              uint32_t* out_cmps, uint32_t* out_hops);
+int dab_search_batch_pq_device_async(dab_index* idx, uint32_t slot, const void* d_queries, uint32_t nq, uint32_t k,
+                                     uint32_t l_search, uint32_t beam_width, int rerank, uint32_t* d_out_ids,
+                                     float* d_out_dists, uint32_t* d_out_counts, uint32_t* d_out_cmps, uint32_t* d_out_hops);
+int dab_search_batch_sq_async(dab_index* idx, uint32_t slot, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                              uint32_t beam_width, int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
+                              uint32_t* out_cmps, uint32_t* out_hops);
+int dab_search_batch_sq_device_async(dab_index* idx, uint32_t slot, const void* d_queries, uint32_t nq, uint32_t k,
+                                     uint32_t l_search, uint32_t beam_width, int rerank, uint32_t* d_out_ids,
+                                     float* d_out_dists, uint32_t* d_out_counts, uint32_t* d_out_cmps, uint32_t* d_out_hops);
+int dab_search_batch_minmax_async(dab_index* idx, uint32_t slot, const void* queries, uint32_t nq, uint32_t k,
+                                  uint32_t l_search, uint32_t beam_width, int rerank, uint32_t* out_ids, float* out_dists,
+                                  uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops);
+int dab_search_batch_minmax_device_async(dab_index* idx, uint32_t slot, const void* d_queries, uint32_t nq, uint32_t k,
+                                         uint32_t l_search, uint32_t beam_width, int rerank, uint32_t* d_out_ids,
+                                         float* d_out_dists, uint32_t* d_out_counts, uint32_t* d_out_cmps,
+                                         uint32_t* d_out_hops);
+
 /* ------------------------------------------------------------------ product quantization */
 
 /* FixedChunkPQTable::populate_chunk_distances / populate_chunk_inner_products

@@ -209,6 +209,18 @@ class GpuKNN {
         check(dab_search_batch_async(p_.raw(), slot, queries, nq, k, l_, beam_, s.r.ids.data(), s.r.distances.data(), s.counts.data(),
                                      s.cmps.data(), s.hops.data()));
     }
+    // The same over the quantized stores (the store must be resident; `rerank`: the full-precision Rerank): PQ, SQ and
+    // MinMax batches share the slots with search_async, and `wait` joins a batch of any kind.  Results equal those of
+    // dab_search_batch_pq[_rerank] / dab_search_batch_sq / dab_search_batch_minmax.
+    void search_pq_async(uint32_t slot, const T* queries, uint32_t nq, uint32_t k, bool rerank) {
+        queue_quantized(dab_search_batch_pq_async, slot, queries, nq, k, rerank);
+    }
+    void search_sq_async(uint32_t slot, const T* queries, uint32_t nq, uint32_t k, bool rerank) {
+        queue_quantized(dab_search_batch_sq_async, slot, queries, nq, k, rerank);
+    }
+    void search_minmax_async(uint32_t slot, const T* queries, uint32_t nq, uint32_t k, bool rerank) {
+        queue_quantized(dab_search_batch_minmax_async, slot, queries, nq, k, rerank);
+    }
     KnnResults wait(uint32_t slot) {
         check(dab_wait(p_.raw(), slot));
         Pending& s = pending_[slot];
@@ -222,6 +234,20 @@ class GpuKNN {
         KnnResults r;
         std::vector<uint32_t> counts, cmps, hops;
     };
+    using QuantizedAsync = int (*)(dab_index*, uint32_t, const void*, uint32_t, uint32_t, uint32_t, uint32_t, int, uint32_t*, float*,
+                                   uint32_t*, uint32_t*, uint32_t*);
+    void queue_quantized(QuantizedAsync fn, uint32_t slot, const T* queries, uint32_t nq, uint32_t k, bool rerank) {
+        if (slot >= DAB_MAX_SLOTS) throw ANNError(DAB_ERR_INVALID_ARGUMENT, "slot out of range");
+        Pending s;  // the slot's buffers are replaced only once the batch is queued
+        s.r.nq = nq;
+        s.r.k = k;
+        s.r.ids.resize((size_t)nq * k);
+        s.r.distances.resize((size_t)nq * k);
+        s.counts.resize(nq), s.cmps.resize(nq), s.hops.resize(nq);
+        check(fn(p_.raw(), slot, queries, nq, k, l_, beam_, rerank ? 1 : 0, s.r.ids.data(), s.r.distances.data(), s.counts.data(),
+                 s.cmps.data(), s.hops.data()));
+        pending_[slot] = std::move(s);  // moving a std::vector keeps its buffer
+    }
     Provider<T>& p_;
     uint32_t l_, beam_;
     Pending pending_[DAB_MAX_SLOTS];
