@@ -477,7 +477,8 @@ __global__ void __launch_bounds__(kV2Warps * 32, REG ? kV2MinCtasReg : QT == 0 ?
                         const uint32_t j = c0 + lane;
                         uint32_t word = c0 == 0 ? wd[0] : (c0 == 32 ? wd[1] : wd[2]);
                         if (c0 >= 96) word = j < p.adj_stride ? __ldg(row + j) : kEmptyV2;
-                        const bool ins = visit_l1(word, j >= 1 && j <= deg);
+                        // ids beyond 2^K cannot be in bounds and would share the tag of id mod 2^K: not tracked
+                        const bool ins = visit_l1(word, j >= 1 && j <= deg && word <= tmap.kmask);
                         const bool isnew = ins && word < n_total;  // is_in_bounds
                         const unsigned mn = __ballot_sync(kFull, isnew);
                         if (isnew) cid[ncand + __popc(mn & ((1u << lane) - 1u))] = word;
