@@ -554,6 +554,7 @@ int dab_build(dab_index* idx, uint32_t pruned_degree, uint32_t l_build, float al
 
     DAB_CUDA(cudaMemsetAsync(idx->d_adj, 0, idx->n_total() * (size_t)idx->adj_stride * 4, st));
     idx->graph_ready = true;
+    ++idx->generation;
 
     DevBuf b_batch, b_rec_ids, b_rec_d, b_rec_n, b_nbr, b_nbr_n, b_keys, b_vals, b_keys2, b_vals2, b_tmp, b_res_ids, b_res_d, b_dropped;
     int rc;

@@ -135,6 +135,7 @@ void dab_destroy(dab_index* idx) {
     cudaSetDevice(idx->device);
     if (idx->own_stream) cudaStreamSynchronize(idx->own_stream);
     search_slots_release(idx);
+    paged_release(idx);
     comm_release(idx);
     tc_release(idx);
     minmax_release(idx);
@@ -185,6 +186,7 @@ static int upload_rows(dab_index* idx, const void* rows, uint64_t first, uint64_
     DAB_CUDA(cudaStreamSynchronize(idx->stream));
     idx->vectors_ready = true;
     ++idx->vectors_version;
+    ++idx->generation;
     return DAB_OK;
 }
 
@@ -241,6 +243,7 @@ static int upload_graph(dab_index* idx, const uint32_t* adj, uint32_t src_stride
                                on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, idx->stream));
     DAB_CUDA(cudaStreamSynchronize(idx->stream));
     idx->graph_ready = true;
+    ++idx->generation;
     return DAB_OK;
 }
 

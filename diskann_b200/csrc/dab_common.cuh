@@ -31,6 +31,7 @@ void search_slots_release(struct ::dab_index* idx);  // search_kernel.cu
 // flight whose overflowed queries still need a pass fails in dab_wait instead of launching on the freed buffers
 int retire_quantized_stores(struct ::dab_index* idx);
 void minmax_release(struct ::dab_index* idx);        // minmax_index.cu: the store's transform
+void paged_release(struct ::dab_index* idx);         // search_paged.cu: every paged search session still open
 
 #define DAB_CUDA(expr)                                                                        \
     do {                                                                                      \
@@ -173,6 +174,10 @@ struct dab_index {
     float v3_overflow_frac = 0.0f;                         // tables at (L, beam): search_kernel_v3 is skipped when large
 
     uint64_t stores_version = 0;  // bumped whenever a quantized store is freed or reallocated (retire_quantized_stores)
+    // bumped by every upload of rows or adjacency, dab_build and the broadcasts: a paged search session that began under
+    // another generation fails its next page (search_paged.cu)
+    uint64_t generation = 0;
+    void* paged = nullptr;  // the open paged search sessions (a list, search_paged.cu)
     uint64_t rec_truncated = 0;  // build: searches whose expanded-node record was cut at its capacity
     dab::Tuning tune;
 

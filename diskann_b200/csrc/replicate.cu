@@ -138,6 +138,7 @@ int broadcast_buffers(dab_index* idx, ncclComm_t comm, int root, bool is_root, I
         DAB_NCCL(n.Broadcast(idx->d_codes, idx->d_codes, total * (size_t)got.pq_chunks, kNcclUint8, root, comm, st));
     }
     DAB_CUDA(cudaStreamSynchronize(st));
+    ++idx->generation;
     idx->vectors_ready = got.vectors_ready != 0;
     if (got.vectors_ready && !is_root) ++idx->vectors_version;
     idx->graph_ready = got.graph_ready != 0;
@@ -269,6 +270,7 @@ int dab_broadcast(dab_index* const* per_gpu, int n_gpus) {
         if (status == DAB_OK && i) {
             per_gpu[i]->vectors_ready = want.vectors_ready != 0;
             ++per_gpu[i]->vectors_version;
+            ++per_gpu[i]->generation;
             per_gpu[i]->graph_ready = want.graph_ready != 0;
             per_gpu[i]->pq_chunks = want.pq_chunks;
             per_gpu[i]->pq_centers = want.pq_centers;

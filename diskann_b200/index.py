@@ -8,13 +8,14 @@ in libdiskann_b200.so on the GPU; numpy is only the host container.
 """
 import ctypes as C
 import enum
+import weakref
 
 import numpy as np
 
 from . import _lib
 from ._lib import DabError, check
 
-__all__ = ["Metric", "DType", "GpuIndex", "distance_comparer", "pair_distances", "DabError", "launch_count"]
+__all__ = ["Metric", "DType", "GpuIndex", "PagedSearch", "distance_comparer", "pair_distances", "DabError", "launch_count"]
 
 
 class Metric(enum.IntEnum):
@@ -249,6 +250,7 @@ class GpuIndex:
     def __init__(self, dtype, metric, dim, n_points, n_start=1, max_degree=83, device=0):
         self._h = C.c_void_p()
         self._inflight = {}  # slot -> (queries, outputs) kept alive while a batch is in flight
+        self._paged = weakref.WeakSet()  # open paged searches: dab_destroy releases them
         self.dtype, self.metric, self.dim = DType(dtype), Metric(metric), int(dim)
         self.n_points, self.n_start, self.max_degree, self.device = int(n_points), int(n_start), int(max_degree), device
         check(_lib.lib().dab_create(C.byref(self._h), int(dtype), int(metric), dim, n_points, n_start, max_degree, device))
@@ -256,6 +258,8 @@ class GpuIndex:
     # -- lifecycle
     def close(self):
         if getattr(self, "_h", None) is not None and self._h.value:
+            for s in list(getattr(self, "_paged", ())):
+                s._h = C.c_void_p()  # released by dab_destroy
             _lib.lib().dab_destroy(self._h)
             self._h = C.c_void_p()
 
@@ -397,6 +401,11 @@ class GpuIndex:
         check(_lib.lib().dab_search_batch(self._h, _ptr(queries), nq, k, l_search, beam_width, _ptr(ids), _ptr(dists),
                                           _ptr(counts), _ptr(cmps), _ptr(hops)))
         return ids, dists, counts, cmps, hops
+
+    def paged_search(self, queries, l_search):
+        """DiskANNIndex::paged_search for the whole batch: a PagedSearch whose next_page(k) returns the next page of
+        every query (each query's list and visited set stay on the device between pages)."""
+        return PagedSearch(self, self._queries(queries), l_search)
 
     def search_batch_device(self, d_queries, nq, k, l_search, beam_width, d_ids, d_dists, d_counts=0, d_cmps=0, d_hops=0):
         """Same with device pointers (integers); results stay in HBM."""
@@ -646,3 +655,44 @@ class GpuIndex:
         dists = np.empty((queries.shape[0], k), np.float32)
         check(_lib.lib().dab_flat_knn_tc(self._h, _ptr(queries), queries.shape[0], k, _ptr(ids), _ptr(dists)))
         return ids, dists
+
+
+class PagedSearch:
+    """PagedSearch (diskann/src/graph/search/paged.rs) over a query batch: successive, non-overlapping pages of one
+    resumable search per query.  Use as a context manager or call close(); closing the index closes it too."""
+
+    def __init__(self, index, queries, l_search):
+        self._h = C.c_void_p()
+        self.index, self.nq, self.l_search = index, queries.shape[0], int(l_search)
+        check(_lib.lib().dab_paged_search_begin(index._h, _ptr(queries), self.nq, self.l_search, C.byref(self._h)))
+        index._paged.add(self)
+
+    def next_page(self, k):
+        """(ids [nq, k], dists [nq, k], counts, cmps, hops): the next page of at most k results per query, padded with
+        UINT32_MAX / +inf; counts[q] == 0 once query q is exhausted; cmps / hops are the session's cumulative counts."""
+        if not self._h.value:
+            raise DabError(1, "next_page: the paged search is closed")
+        ids = np.empty((self.nq, k), np.uint32)
+        dists = np.empty((self.nq, k), np.float32)
+        counts = np.empty(self.nq, np.uint32)
+        cmps = np.empty(self.nq, np.uint32)
+        hops = np.empty(self.nq, np.uint32)
+        check(_lib.lib().dab_paged_search_next(self._h, k, _ptr(ids), _ptr(dists), _ptr(counts), _ptr(cmps), _ptr(hops)))
+        return ids, dists, counts, cmps, hops
+
+    def close(self):
+        if getattr(self, "_h", None) is not None and self._h.value:
+            _lib.lib().dab_paged_search_end(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()

@@ -207,6 +207,16 @@ impl<T: Element> GpuIndex<T> {
         Ok(InFlight { index: self, slot, batch: Some(b), _queries: queries })
     }
 
+    /// `DiskANNIndex::paged_search` for every query of the batch: each `PagedSearch::next_page(k)` resumes the
+    /// queries' searches on the device and returns their next pages (graph/search/paged.rs:53-149).
+    pub fn paged_search(&self, queries: &[T], l_search: u32) -> Result<PagedSearch<'_, T>> {
+        assert_eq!(queries.len() % self.dim, 0);
+        let nq = queries.len() / self.dim;
+        let mut raw = ptr::null_mut();
+        check(unsafe { sys::dab_paged_search_begin(self.raw, queries.as_ptr() as *const c_void, nq as u32, l_search, &mut raw) })?;
+        Ok(PagedSearch { raw, nq, _index: self })
+    }
+
     /// One process per GPU: join the communicator described by `id` (from `unique_id()` on rank 0) …
     pub fn comm_init(&mut self, id: &[u8; 128], n_ranks: i32, rank: i32) -> Result<()> {
         check(unsafe { sys::dab_comm_init(self.raw, id.as_ptr() as *const _, n_ranks, rank) })
@@ -243,6 +253,33 @@ impl<'a, T: Element> Drop for InFlight<'a, T> {
         if self.batch.is_some() {
             unsafe { sys::dab_wait(self.index.raw, self.slot) };
         }
+    }
+}
+
+/// A paged search over a query batch; it borrows the index, so the index outlives it and cannot be changed under it.
+pub struct PagedSearch<'a, T: Element> {
+    raw: *mut sys::dab_paged,
+    nq: usize,
+    _index: &'a GpuIndex<T>,
+}
+
+impl<'a, T: Element> PagedSearch<'a, T> {
+    /// The next page of at most `k` results per query (`0 < k <= l_search`): `counts[q] == 0` once query `q` is
+    /// exhausted; `cmps` / `hops` are the session's cumulative counts.
+    pub fn next_page(&mut self, k: usize) -> Result<Batch> {
+        let nq = self.nq;
+        let mut b = Batch { k, ids: vec![0; nq * k], dists: vec![0.0; nq * k], counts: vec![0; nq], cmps: vec![0; nq], hops: vec![0; nq] };
+        check(unsafe {
+            sys::dab_paged_search_next(self.raw, k as u32, b.ids.as_mut_ptr(), b.dists.as_mut_ptr(), b.counts.as_mut_ptr(),
+                                       b.cmps.as_mut_ptr(), b.hops.as_mut_ptr())
+        })?;
+        Ok(b)
+    }
+}
+
+impl<'a, T: Element> Drop for PagedSearch<'a, T> {
+    fn drop(&mut self) {
+        unsafe { sys::dab_paged_search_end(self.raw) }
     }
 }
 

@@ -169,6 +169,30 @@ int dab_search_batch_device(dab_index* idx, const void* d_queries, uint32_t nq, 
                             float* d_out_dists, uint32_t* d_out_counts, uint32_t* d_out_cmps,
                             uint32_t* d_out_hops);
 
+/* ------------------------------------------------------------------ (3'') paged search */
+
+/* DiskANNIndex::paged_search (diskann/src/graph/index.rs:2075-2155) and PagedSearch::next_page
+ * (graph/search/paged.rs:53-149) for a whole query batch: successive, non-overlapping pages of one
+ * resumable search per query, each query's candidate list and visited set kept on the device
+ * between pages (only the pages cross PCIe).
+ *   begin: queries [nq][dim] of the index dtype (f16 queries are widened as in dab_search_batch);
+ *     l_search + n_start <= 1024.  The start points are expanded once; nothing is counted yet.
+ *   next:  the next page of at most k results per query, 0 < k <= l_search: rows [nq][k] of ids and
+ *     distances, padded with UINT32_MAX / +inf, ordered by non-decreasing distance within a page.
+ *     out_counts[q] == 0 means query q is exhausted (and stays so).  out_cmps / out_hops are the
+ *     session's cumulative comparisons and hops, counted as SearchStats counts them.  The counts,
+ *     cmps and hops pointers may be NULL.  Host buffers only.
+ *   end:   releases the session.
+ * Several sessions may be open on one index.  Any upload of rows or adjacency, dab_build or a
+ * broadcast after a session began makes its next page fail with DAB_ERR_INVALID_ARGUMENT.
+ * dab_destroy releases every session still open; their handles are invalid after it. */
+typedef struct dab_paged dab_paged; /* opaque */
+int dab_paged_search_begin(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search,
+                           dab_paged** out);
+int dab_paged_search_next(dab_paged* s, uint32_t k, uint32_t* out_ids, float* out_dists,
+                          uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops);
+void dab_paged_search_end(dab_paged* s);
+
 /* Batches in flight.  The reference keeps every core busy by handing each query to a task of a
  * thread pool (diskann-benchmark-core/src/search/api.rs:410-419: `search_all` spawns one task per
  * query partition and joins them); the device equivalent is to keep more than one BATCH in flight:

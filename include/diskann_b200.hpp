@@ -253,6 +253,39 @@ class GpuKNN {
     Pending pending_[DAB_MAX_SLOTS];
 };
 
+// DiskANNIndex::paged_search + PagedSearch::next_page (diskann/src/graph/search/paged.rs) for a whole query batch: every
+// next_page(k) returns the next k results of each query's one resumable search, whose list and visited set stay on the
+// device.  Results across pages do not overlap; stats are the session's cumulative cmps / hops.  The provider must
+// outlive the session and stay unchanged (a changed index fails the next page); `queries` are copied at construction.
+template <class T>
+class PagedSearch {
+   public:
+    PagedSearch(Provider<T>& provider, const T* queries, uint32_t nq, uint32_t l_value) : nq_(nq) {
+        check(dab_paged_search_begin(provider.raw(), queries, nq, l_value, &h_));
+    }
+    ~PagedSearch() { dab_paged_search_end(h_); }
+    PagedSearch(const PagedSearch&) = delete;
+    PagedSearch& operator=(const PagedSearch&) = delete;
+
+    // 0 < k <= l_value; stats[q].result_count == 0 once query q is exhausted
+    KnnResults next_page(uint32_t k) {
+        KnnResults r;
+        r.nq = nq_;
+        r.k = k;
+        r.ids.resize((size_t)nq_ * k);
+        r.distances.resize((size_t)nq_ * k);
+        std::vector<uint32_t> counts(nq_), cmps(nq_), hops(nq_);
+        check(dab_paged_search_next(h_, k, r.ids.data(), r.distances.data(), counts.data(), cmps.data(), hops.data()));
+        r.stats.resize(nq_);
+        for (uint32_t i = 0; i < nq_; ++i) r.stats[i] = SearchStats{cmps[i], hops[i], counts[i]};
+        return r;
+    }
+
+   private:
+    dab_paged* h_ = nullptr;
+    uint32_t nq_;
+};
+
 // Transform::PaddingHadamard / Transform::DoubleHadamard from the parts the reference serializes (try_from_parts:
 // padding_hadamard.rs:137-173, double_hadamard.rs:146-206); signs are 0 / 1 bytes.  A host-side object; apply() runs
 // transform_into on the device.
