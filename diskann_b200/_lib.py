@@ -43,6 +43,9 @@ SYMBOLS = {
     "dab_search_batch_device_async": (_i, [_vp, _u32, _vp, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
     "dab_wait": (_i, [_vp, _u32]),
     "dab_paged_search_begin": (_i, [_vp, _vp, _u32, _u32, C.POINTER(_vp)]),
+    "dab_paged_search_begin_pq": (_i, [_vp, _vp, _u32, _u32, C.POINTER(_vp)]),
+    "dab_paged_search_begin_sq": (_i, [_vp, _vp, _u32, _u32, C.POINTER(_vp)]),
+    "dab_paged_search_begin_minmax": (_i, [_vp, _vp, _u32, _u32, C.POINTER(_vp)]),
     "dab_paged_search_next": (_i, [_vp, _u32, _vp, _vp, _vp, _vp, _vp]),
     "dab_paged_search_end": (None, [_vp]),
     "dab_search_batch_pq_async": (_i, [_vp, _u32, _vp, _u32, _u32, _u32, _u32, _i, _vp, _vp, _vp, _vp, _vp]),

@@ -289,6 +289,7 @@ int dab_upload_pq(dab_index* idx, const float* pivots, uint32_t n_centers, const
     DAB_CUDA(cudaStreamSynchronize(idx->stream));
     int rc;
     if ((rc = retire_quantized_stores(idx))) return rc;  // batches in flight read the table and the codes
+    ++idx->store_writes[STORE_PQ];
     cudaFree(idx->d_pivots);
     cudaFree(idx->d_offsets);
     cudaFree(idx->d_codes);

@@ -19,6 +19,9 @@ namespace dab {
 
 constexpr uint32_t kNoId = 0xFFFFFFFFu;
 
+// the quantized stores of an index, numbered as the MODE of the quantized traversals (search_kernel_pq.cu)
+enum QuantStore { STORE_PQ = 0, STORE_SQ = 1, STORE_MINMAX = 2 };
+
 // thread-local error message (dab_last_error)
 char* error_buffer();
 int fail(int code, const char* fmt, ...);
@@ -177,6 +180,9 @@ struct dab_index {
     // bumped by every upload of rows or adjacency, dab_build and the broadcasts: a paged search session that began under
     // another generation fails its next page (search_paged.cu)
     uint64_t generation = 0;
+    // one write counter per quantized store, indexed by dab::QuantStore: bumped by every call that writes the store
+    // (upload, encode-all, PQ training, broadcast).  Only paged search sessions over that store read it.
+    uint64_t store_writes[3] = {};
     void* paged = nullptr;  // the open paged search sessions (a list, search_paged.cu)
     uint64_t rec_truncated = 0;  // build: searches whose expanded-node record was cut at its capacity
     dab::Tuning tune;

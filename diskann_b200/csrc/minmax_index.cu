@@ -111,6 +111,7 @@ int dab_upload_minmax(dab_index* idx, int nbits, float grid_scale, const dab_tra
     DAB_CUDA(cudaStreamSynchronize(idx->stream));
     int rc;
     if ((rc = retire_quantized_stores(idx))) return rc;  // batches in flight read the store and its transform
+    ++idx->store_writes[STORE_MINMAX];
     minmax_release(idx);
     store_release(idx->mm);
     idx->mm_grid_scale = grid_scale;
@@ -132,6 +133,7 @@ int dab_minmax_encode_all(dab_index* idx) {
     if (!idx->vectors_ready) return fail(DAB_ERR_NOT_READY, "%s: vectors not uploaded", who);
     DAB_CUDA(cudaSetDevice(idx->device));
     CodeStore& mm = idx->mm;
+    ++idx->store_writes[STORE_MINMAX];
     mm.ready = false;
     const uint64_t total = idx->n_total();
     const uint64_t per_row = (uint64_t)(idx->dim + (idx->mm_transform ? mm.dim : 0)) * 4 + mm.row_bytes;

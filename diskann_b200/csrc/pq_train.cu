@@ -320,6 +320,7 @@ int dab_pq_train(dab_index* idx, const float* train, uint64_t n, uint32_t n_chun
     DAB_CUDA(cudaStreamSynchronize(st));
     int rc;
     if ((rc = retire_quantized_stores(idx))) return rc;  // batches in flight read the table and the codes
+    ++idx->store_writes[STORE_PQ];
     // ChunkOffsets::partition (diskann-quantization/src/views.rs:226-243): the first dim % n_chunks chunks get one extra
     std::vector<uint32_t> off(n_chunks + 1, 0);
     uint32_t max_len = 0;
@@ -420,6 +421,7 @@ int dab_pq_encode_all(dab_index* idx) {
     if (!idx->d_pivots || !idx->pq_chunks) return fail(DAB_ERR_NOT_READY, "dab_pq_encode_all: no PQ table (dab_upload_pq / dab_pq_train)");
     if (!idx->vectors_ready) return fail(DAB_ERR_NOT_READY, "dab_pq_encode_all: vectors not uploaded");
     DAB_CUDA(cudaSetDevice(idx->device));
+    ++idx->store_writes[STORE_PQ];
     const uint64_t total = idx->n_total();
     const uint64_t batch = std::max<uint64_t>(1, std::min<uint64_t>(total, (256ull << 20) / ((size_t)idx->dim * 4)));
     int rc;

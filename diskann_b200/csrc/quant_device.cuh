@@ -1,6 +1,7 @@
 // quant_device.cuh — thread-serial emulation of the reference's simd_op for short f32 chunks
 // (PQ LUT entries, encode), the packed-code integer cores, the scalar quantizer and the SQ / MinMax
-// epilogues, shared by quant_kernels.cu, sq_index.cu and search_kernel_pq.cu.
+// epilogues, and the per-candidate distances of the quantized traversals, shared by quant_kernels.cu, sq_index.cu,
+// search_kernel_pq.cu and search_paged.cu.
 #pragma once
 
 #include "distance_device.cuh"
@@ -150,6 +151,114 @@ __device__ __forceinline__ float minmax_finish(int metric, uint32_t ip, uint32_t
     if (metric == DAB_L2) return __fadd_rn(__fadd_rn(__fmul_rn(-2.0f, v), xq), yq);
     if (metric == DAB_COSINE) return __fsub_rn(1.0f, __fdiv_rn(v, __fmul_rn(__fsqrt_rn(xq), __fsqrt_rn(yq))));
     return __fsub_rn(1.0f, v);
+}
+
+// ------------------------------------------------------------------ per-candidate distances of the quantized traversals
+// What one lane computes for one candidate in the quantized accessor's expand_beam: search_kernel_pq.cu (one-shot and
+// in-flight batches) and search_paged.cu (paged sessions) share these, so both return the same bits.
+
+// the integer cores of one packed code row against the query's code words, 16 B at a time
+template <int NBITS>
+__device__ __forceinline__ void sq_row(const uint4* __restrict__ row, const uint4* qc, uint32_t vecs, bool want_ip, uint32_t& l2,
+                                       uint32_t& ip) {
+    for (uint32_t v = 0; v < vecs; ++v) {
+        const uint4 a = __ldg(row + v);
+        const uint4 b = qc[v];
+        sq_word<NBITS>(a.x, b.x, want_ip, l2, ip);
+        sq_word<NBITS>(a.y, b.y, want_ip, l2, ip);
+        sq_word<NBITS>(a.z, b.z, want_ip, l2, ip);
+        sq_word<NBITS>(a.w, b.w, want_ip, l2, ip);
+    }
+}
+
+// MODE 1 (SQ) / MODE 2 (MinMax): the distance of packed code row `id` to the query's code words qc (16 B aligned; MinMax:
+// its {b, n, a, norm_squared} follow the words), the query as x and the row as y.  P names the store as SearchParamsPq
+// does (row_codes, row_meta, code_stride, code_nbits, code_metric, code_dim, sq_scale_squared, sq_shift_square_norm).
+// Only SQ InnerProduct loads the row's compensation; MinMax loads the row's four.
+template <int MODE, class P>
+__device__ __forceinline__ float packed_code_distance(const P& p, const uint32_t* qc, float q_comp, uint32_t id) {
+    const uint4* row = reinterpret_cast<const uint4*>(p.row_codes + (size_t)id * p.code_stride);
+    const uint4* q4 = reinterpret_cast<const uint4*>(qc);
+    const uint32_t vecs = p.code_stride >> 4;
+    const bool want_ip = MODE == 2 || p.code_metric == DAB_INNER_PRODUCT;  // MinMax: every metric
+    uint32_t l2 = 0, ip = 0;
+    switch (p.code_nbits) {
+        case 8: sq_row<8>(row, q4, vecs, want_ip, l2, ip); break;
+        case 4: sq_row<4>(row, q4, vecs, want_ip, l2, ip); break;
+        case 2: sq_row<2>(row, q4, vecs, want_ip, l2, ip); break;
+        default: sq_row<1>(row, q4, vecs, want_ip, l2, ip); break;
+    }
+    if (MODE == 1) {
+        const float ibs = __fdiv_rn(1.0f, (float)((1u << p.code_nbits) - 1u));
+        const float mul = __fmul_rn(__fmul_rn(ibs, ibs), p.sq_scale_squared);
+        return sq_finish(p.code_metric, l2, ip, mul, p.sq_shift_square_norm, q_comp, want_ip ? __ldg(p.row_meta + id) : 0.0f);
+    } else {
+        const float4 qm = *reinterpret_cast<const float4*>(qc + (p.code_stride >> 2));
+        const float4 rm = __ldg(reinterpret_cast<const float4*>(p.row_meta) + id);
+        return minmax_finish(p.code_metric, ip, p.code_dim, qm.x, qm.y, qm.z, qm.w, rm.x, rm.y, rm.z, rm.w);
+    }
+}
+
+// PQ: P names the table as SearchParamsPq does (codes, n_chunks, n_centers, offsets, pivots, ip_table).
+// DirectCosine (pq/distance/cosine.rs:16-70; direct_distance_impl, fixed_chunk_pq_table.rs:35-59): the Resumable V3
+// cosine (Strategy2x4) accumulated chunk by chunk over the pivots the code of row `id` selects, 1 - cos.  qf: the f32 query.
+template <class P>
+__device__ __forceinline__ float pq_direct_cosine(const P& p, const float* qf, int dim, uint32_t id) {
+    const uint8_t* code = p.codes + (size_t)id * p.n_chunks;
+    float nx[8], ny[8], xy[8];
+#pragma unroll
+    for (int l = 0; l < 8; ++l) nx[l] = ny[l] = xy[l] = 0.0f;
+    for (uint32_t ch = 0; ch < p.n_chunks; ++ch) {
+        const uint32_t start = p.offsets[ch], stop = p.offsets[ch + 1];
+        const float* xc = qf + start;
+        const float* yc = p.pivots + (size_t)__ldg(code + ch) * dim + start;
+        float a[8], b[8], d[8];
+        thread_simd_combined<2, KIND_IP>(xc, xc, (int)(stop - start), a);
+        thread_simd_combined<2, KIND_IP>(yc, yc, (int)(stop - start), b);
+        thread_simd_combined<2, KIND_IP>(xc, yc, (int)(stop - start), d);
+#pragma unroll
+        for (int l = 0; l < 8; ++l) {
+            nx[l] = __fadd_rn(nx[l], a[l]);
+            ny[l] = __fadd_rn(ny[l], b[l]);
+            xy[l] = __fadd_rn(xy[l], d[l]);
+        }
+    }
+    return __fsub_rn(1.0f, cosine_finish(thread_tree8(nx), thread_tree8(ny), thread_tree8(xy)));
+}
+
+// TableL2 / TableIP: the ADC lookups of row `id` in the query's table (n_chunks x n_centers f32 in global memory, read
+// through L2), summed in chunk order from 0.0 (pq_dist_lookup_single, fixed_chunk_pq_table.rs:82-98)
+template <class P>
+__device__ __forceinline__ float pq_table_distance(const P& p, const float* lut, uint32_t id) {
+    const uint8_t* code = p.codes + (size_t)id * p.n_chunks;
+    float accum = 0.0f;
+    uint32_t ch = 0;
+    if ((p.n_chunks & 15u) == 0) {
+        for (; ch < p.n_chunks; ch += 16) {
+            const uint4 w = __ldg(reinterpret_cast<const uint4*>(code + ch));
+            const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
+            float v[16];
+#pragma unroll
+            for (int k2 = 0; k2 < 16; ++k2) v[k2] = __ldcg(lut + (ch + k2) * p.n_centers + ((ws[k2 >> 2] >> ((k2 & 3) * 8)) & 0xFFu));
+#pragma unroll
+            for (int k2 = 0; k2 < 16; ++k2) accum = __fadd_rn(accum, v[k2]);
+        }
+    } else {
+        for (; ch < p.n_chunks; ++ch) accum = __fadd_rn(accum, __ldcg(lut + ch * p.n_centers + __ldg(code + ch)));
+    }
+    return accum;
+}
+
+// entry t = chunk * n_centers + centre of the query's table (fixed_chunk_pq_table.rs:152-187): TableIP entries are -dot
+template <class P>
+__device__ __forceinline__ float pq_table_entry(const P& p, const float* qf, int dim, uint32_t t) {
+    const uint32_t chunk = t / p.n_centers, center = t % p.n_centers;
+    const uint32_t start = p.offsets[chunk], stop = p.offsets[chunk + 1];
+    const float* piv = p.pivots + (size_t)center * dim + start;
+    float v;
+    if (p.ip_table) v = -thread_simd_l2ip<KIND_IP>(qf + start, piv, (int)(stop - start));
+    else v = thread_simd_l2ip<KIND_L2>(qf + start, piv, (int)(stop - start));
+    return v;
 }
 
 // ------------------------------------------------------------------ PQ table entries from shared-memory pivots

@@ -119,6 +119,7 @@ int broadcast_buffers(dab_index* idx, ncclComm_t comm, int root, bool is_root, I
     if (got.vectors_ready) DAB_NCCL(n.Broadcast(idx->d_vectors, idx->d_vectors, total * idx->row_stride, kNcclUint8, root, comm, st));
     if (got.graph_ready) DAB_NCCL(n.Broadcast(idx->d_adj, idx->d_adj, total * (size_t)idx->adj_stride * 4, kNcclUint8, root, comm, st));
     if (got.pq_chunks) {
+        ++idx->store_writes[STORE_PQ];
         if (!is_root) {
             DAB_CUDA(cudaStreamSynchronize(st));
             int rc;
@@ -231,6 +232,7 @@ int dab_broadcast(dab_index* const* per_gpu, int n_gpus) {
             status = fail(DAB_ERR_INVALID_ARGUMENT, "dab_broadcast: handle %d was created with a different shape than handle 0", i);
         else if (want.pq_chunks) {
             dab_index* r = per_gpu[i];
+            ++r->store_writes[STORE_PQ];
             cudaSetDevice(r->device);
             cudaFree(r->d_pivots);
             cudaFree(r->d_offsets);

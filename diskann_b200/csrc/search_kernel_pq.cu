@@ -12,7 +12,8 @@
 //   * per hop every lane owns one surviving neighbour: coalesced 16 B code loads, one table
 //     gather per chunk, and the sum is accumulated in chunk order from 0.0
 //     (pq_dist_lookup_single, fixed_chunk_pq_table.rs:82-98) -> bit-identical ADC distances;
-//   * visited set, sorted list and post-processing are the shared exact helpers.
+//   * visited set, sorted list and post-processing are the shared exact helpers; the per-candidate distances live in
+//     quant_device.cuh, shared with the paged sessions (search_paged.cu).
 // No tensor cores: LUT gather + byte loads, HBM traffic is n_chunks code bytes per candidate.
 //
 // MODE 1 and MODE 2 — the two stores of dense N-bit code rows (bits/slice.rs:261-323), 16 B aligned, compensations
@@ -38,19 +39,6 @@
 #include <type_traits>
 
 namespace dab {
-
-template <int NBITS>
-__device__ __forceinline__ void sq_row(const uint4* __restrict__ row, const uint4* qc, uint32_t vecs, bool want_ip, uint32_t& l2,
-                                       uint32_t& ip) {
-    for (uint32_t v = 0; v < vecs; ++v) {
-        const uint4 a = __ldg(row + v);
-        const uint4 b = qc[v];
-        sq_word<NBITS>(a.x, b.x, want_ip, l2, ip);
-        sq_word<NBITS>(a.y, b.y, want_ip, l2, ip);
-        sq_word<NBITS>(a.z, b.z, want_ip, l2, ip);
-        sq_word<NBITS>(a.w, b.w, want_ip, l2, ip);
-    }
-}
 
 template <int QT, int MODE>
 __global__ void __launch_bounds__(kPqWarps * 32) search_kernel_pq(const SearchParamsPq p) {
@@ -80,74 +68,11 @@ __global__ void __launch_bounds__(kPqWarps * 32) search_kernel_pq(const SearchPa
         for (uint32_t c0 = 0; c0 < n; c0 += 32) {
             const uint32_t c = c0 + lane;
             if (MODE != 0) {
-                if (c < n) {
-                    const uint32_t id = cid[c];
-                    const uint4* row = reinterpret_cast<const uint4*>(p.row_codes + (size_t)id * p.code_stride);
-                    const uint4* q4 = reinterpret_cast<const uint4*>(qc);
-                    const uint32_t vecs = p.code_stride >> 4;
-                    const bool want_ip = MODE == 2 || p.code_metric == DAB_INNER_PRODUCT;  // MinMax: every metric
-                    uint32_t l2 = 0, ip = 0;
-                    switch (p.code_nbits) {
-                        case 8: sq_row<8>(row, q4, vecs, want_ip, l2, ip); break;
-                        case 4: sq_row<4>(row, q4, vecs, want_ip, l2, ip); break;
-                        case 2: sq_row<2>(row, q4, vecs, want_ip, l2, ip); break;
-                        default: sq_row<1>(row, q4, vecs, want_ip, l2, ip); break;
-                    }
-                    // the query as x, the row as y; only InnerProduct loads the row's SQ compensation
-                    if (MODE == 1) {
-                        const float ibs = __fdiv_rn(1.0f, (float)((1u << p.code_nbits) - 1u));
-                        const float mul = __fmul_rn(__fmul_rn(ibs, ibs), p.sq_scale_squared);
-                        cd[c] = sq_finish(p.code_metric, l2, ip, mul, p.sq_shift_square_norm, q_comp, want_ip ? __ldg(p.row_meta + id) : 0.0f);
-                    } else {
-                        const float4 qm = *reinterpret_cast<const float4*>(qc + (p.code_stride >> 2));
-                        const float4 rm = __ldg(reinterpret_cast<const float4*>(p.row_meta) + id);
-                        cd[c] = minmax_finish(p.code_metric, ip, p.code_dim, qm.x, qm.y, qm.z, qm.w, rm.x, rm.y, rm.z, rm.w);
-                    }
-                }
+                if (c < n) cd[c] = packed_code_distance<MODE>(p, qc, q_comp, cid[c]);
             } else if (p.direct_cosine) {
-                // DirectCosine (pq/distance/cosine.rs:16-70; direct_distance_impl, fixed_chunk_pq_table.rs:35-59): the
-                // Resumable V3 cosine (Strategy2x4) accumulated chunk by chunk over the pivots the code selects, 1 - cos
-                if (c < n) {
-                    const uint8_t* code = p.codes + (size_t)cid[c] * p.n_chunks;
-                    float nx[8], ny[8], xy[8];
-#pragma unroll
-                    for (int l = 0; l < 8; ++l) nx[l] = ny[l] = xy[l] = 0.0f;
-                    for (uint32_t ch = 0; ch < p.n_chunks; ++ch) {
-                        const uint32_t start = p.offsets[ch], stop = p.offsets[ch + 1];
-                        const float* xc = qf + start;
-                        const float* yc = p.pivots + (size_t)__ldg(code + ch) * dim + start;
-                        float a[8], b[8], d[8];
-                        thread_simd_combined<2, KIND_IP>(xc, xc, (int)(stop - start), a);
-                        thread_simd_combined<2, KIND_IP>(yc, yc, (int)(stop - start), b);
-                        thread_simd_combined<2, KIND_IP>(xc, yc, (int)(stop - start), d);
-#pragma unroll
-                        for (int l = 0; l < 8; ++l) {
-                            nx[l] = __fadd_rn(nx[l], a[l]);
-                            ny[l] = __fadd_rn(ny[l], b[l]);
-                            xy[l] = __fadd_rn(xy[l], d[l]);
-                        }
-                    }
-                    cd[c] = __fsub_rn(1.0f, cosine_finish(thread_tree8(nx), thread_tree8(ny), thread_tree8(xy)));
-                }
+                if (c < n) cd[c] = pq_direct_cosine(p, qf, dim, cid[c]);
             } else if (c < n) {
-                const uint8_t* code = p.codes + (size_t)cid[c] * p.n_chunks;
-                float accum = 0.0f;
-                uint32_t ch = 0;
-                if ((p.n_chunks & 15u) == 0) {
-                    for (; ch < p.n_chunks; ch += 16) {
-                        const uint4 w = __ldg(reinterpret_cast<const uint4*>(code + ch));
-                        const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
-                        float v[16];
-#pragma unroll
-                        for (int k2 = 0; k2 < 16; ++k2)
-                            v[k2] = __ldcg(lut + (ch + k2) * p.n_centers + ((ws[k2 >> 2] >> ((k2 & 3) * 8)) & 0xFFu));
-#pragma unroll
-                        for (int k2 = 0; k2 < 16; ++k2) accum = __fadd_rn(accum, v[k2]);
-                    }
-                } else {
-                    for (; ch < p.n_chunks; ++ch) accum = __fadd_rn(accum, __ldcg(lut + ch * p.n_centers + __ldg(code + ch)));
-                }
-                cd[c] = accum;
+                cd[c] = pq_table_distance(p, lut, cid[c]);
             }
         }
         __syncwarp();
@@ -184,15 +109,7 @@ __global__ void __launch_bounds__(kPqWarps * 32) search_kernel_pq(const SearchPa
             if (MODE == 2 && lane == 0) *reinterpret_cast<float4*>(qc + words) = __ldg(p.query_meta + qidx);
             __syncwarp();
         }
-        for (uint32_t t = lane; MODE == 0 && !p.direct_cosine && t < entries; t += 32) {
-            const uint32_t chunk = t / p.n_centers, center = t % p.n_centers;
-            const uint32_t start = p.offsets[chunk], stop = p.offsets[chunk + 1];
-            const float* piv = p.pivots + (size_t)center * dim + start;
-            float v;
-            if (p.ip_table) v = -thread_simd_l2ip<KIND_IP>(qf + start, piv, (int)(stop - start));
-            else v = thread_simd_l2ip<KIND_L2>(qf + start, piv, (int)(stop - start));
-            __stcg(lut + t, v);
-        }
+        for (uint32_t t = lane; MODE == 0 && !p.direct_cosine && t < entries; t += 32) __stcg(lut + t, pq_table_entry(p, qf, dim, t));
         __syncwarp();
 
         uint32_t size = 0, cursor_lo = 0, cmps = 0, hops = 0, nvisited = 0;

@@ -19,9 +19,17 @@
 // search the tail and the log are only appended to, so a query whose table passes 7/8 full simply stops uncommitted:
 // the host gives it a table four times larger, rebuilt from the log up to its committed length (the tail is copied up
 // to its committed length), and runs that query's call again from its committed state.  Membership is exact at any size.
+//
+// The session logic (paged_queries) does not depend on how distances are made.  paged_kernel reads full-precision rows;
+// paged_kernel_quant reads the PQ, SQ or MinMax store with the per-candidate code of the one-shot quantized traversal
+// (quant_device.cuh), so a page carries the same quantized distances (dab_paged_search_begin_{pq,sq,minmax}).  Nothing
+// a session reads between pages lives in the index's shared scratch: the compressed SQ / MinMax queries are session
+// memory, and a PQ query's table is rebuilt at every call in the session's own table scratch.
 #include "dab_common.cuh"
+#include "quant_device.cuh"
 #include "search_common.cuh"
 #include "search_host.cuh"
+#include "search_pq.cuh"
 
 #include <algorithm>
 #include <vector>
@@ -68,6 +76,21 @@ struct PagedParams {
     float* out_dists;
     uint32_t *out_counts, *out_cmps, *out_hops;
     uint32_t warp_smem, off_cid, off_cd, off_wd, off_wi, off_ws;
+    // the quantized sessions (paged_kernel_quant), named as in SearchParamsPq for the per-candidate code
+    int dtype;
+    const float* pivots;  // PQ: the table, [n_centers][dim]
+    const uint32_t* offsets;
+    const uint8_t* codes;  // [n_total][n_chunks]
+    uint32_t n_chunks, n_centers;
+    int ip_table, direct_cosine;
+    float* luts;  // PQ tables: one table per warp of the grid
+    const uint8_t* row_codes;  // SQ / MinMax: the store's rows and the session's staged queries
+    const float* row_meta;
+    uint32_t code_stride, code_dim;
+    int code_nbits, code_metric;
+    float sq_scale_squared, sq_shift_square_norm;
+    const uint8_t* query_codes;  // [nq][code_stride]
+    const float4* query_meta;    // [nq]
 };
 
 // (distance ascending, insertion number descending) as one ascending 64-bit key; -0.0 and +0.0 compare equal
@@ -156,20 +179,18 @@ __device__ __forceinline__ void merge_paged(float* wd, uint32_t* wi, uint32_t* w
     __syncwarp();
 }
 
-template <typename TD, int KIND, int POST, int NA>
-__global__ void __launch_bounds__(kPagedWarps * 32) paged_kernel(const PagedParams p) {
-    constexpr bool INT = std::is_same<TD, int8_t>::value || std::is_same<TD, uint8_t>::value;
-    extern __shared__ __align__(128) uint8_t smem[];
-    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    uint8_t* base = smem + (size_t)wib * p.warp_smem;
-    float* qf = reinterpret_cast<float*>(base);
+// One warp's share of a pass: the session logic of paged search for every query it takes, whatever the distances are.
+// Src is the distance source: load(q) brings query q into the warp's shared memory (before its window is read back),
+// prepare() runs once the window is in place (what the distances need of the loaded query), and distances(cid, cd, n)
+// writes the distances of cid[0..n) into cd[0..n) and ends with the warp converged.
+template <class Src>
+__device__ __forceinline__ void paged_queries(const PagedParams& p, uint8_t* base, int lane, Src& src) {
     uint32_t* cid = reinterpret_cast<uint32_t*>(base + p.off_cid);
     float* cd = reinterpret_cast<float*>(base + p.off_cd);
     float* wd = reinterpret_cast<float*>(base + p.off_wd);
     uint32_t* wi = reinterpret_cast<uint32_t*>(base + p.off_wi);
     uint32_t* ws = reinterpret_cast<uint32_t*>(base + p.off_ws);
     const uint64_t n_total = p.n_points + p.n_start;
-    const int dim = (int)p.dim;
     const uint32_t cap = p.cap;
 
     for (;;) {
@@ -183,16 +204,7 @@ __global__ void __launch_bounds__(kPagedWarps * 32) paged_kernel(const PagedPara
         const uint32_t hlimit = st.n_buckets * 7;  // 87.5 % load
 
         __syncwarp();
-        {
-            const TD* s = reinterpret_cast<const TD*>(p.queries) + (size_t)q * dim;
-            if constexpr (INT) {
-                uint8_t* qb = reinterpret_cast<uint8_t*>(qf);
-                const int qbytes = (dim + 3) & ~3;
-                for (int e = lane; e < qbytes; e += 32) qb[e] = e < dim ? reinterpret_cast<const uint8_t*>(s)[e] : 0;
-            } else {
-                for (int e = lane; e < dim; e += 32) qf[e] = to_f32(s[e]);  // f16 queries are widened (layers/full.rs:421-423)
-            }
-        }
+        src.load(q);
         uint32_t size = 0, cursor = 0, tlen = 0, logn = 0, cmps = 0, hops = 0, seq = 0;
         if (p.begin) {
             for (uint32_t i = lane; i < st.n_buckets; i += 32) store_empty_bucket(st.table + (size_t)i * 8);
@@ -207,10 +219,7 @@ __global__ void __launch_bounds__(kPagedWarps * 32) paged_kernel(const PagedPara
             }
         }
         __syncwarp();
-        int qq = 0;  // Sum x^2 of the query (unused by inner product)
-        if constexpr (INT) {
-            if (KIND != KIND_IP) qq = warp_int_self<std::is_same<TD, int8_t>::value>(reinterpret_cast<const uint8_t*>(qf), dim, lane);
-        }
+        src.prepare();
 
         // HashSet::insert of one id per lane; the new ones are logged in lane order
         auto visit = [&](uint32_t id, bool ok) -> bool {
@@ -245,28 +254,7 @@ __global__ void __launch_bounds__(kPagedWarps * 32) paged_kernel(const PagedPara
             return ncand;
         };
 
-        // distances of cid[0..n) into cd[0..n): rows from global memory, a team per row (distance_device.cuh)
-        auto distances = [&](uint32_t n) {
-            constexpr int S = INT ? 32 : 8 * NA, TEAMS = 32 / S, U = kPagedRows;
-            using Row = typename std::conditional<INT, uint8_t, TD>::type;
-            const int team = lane / S, slot = lane % S;
-            for (uint32_t c0 = 0; c0 < n; c0 += TEAMS * U) {
-                float r[U];
-                uint32_t cc[U];
-                const Row* rows[U];
-#pragma unroll
-                for (int u = 0; u < U; ++u) {
-                    cc[u] = c0 + u * TEAMS + team;
-                    rows[u] = reinterpret_cast<const Row*>(p.vectors + (size_t)cid[min(cc[u], n - 1)] * p.row_stride);
-                }
-                if constexpr (INT) warp_int_multi<std::is_same<TD, int8_t>::value, KIND, U>(reinterpret_cast<const uint8_t*>(qf), rows, dim, lane, qq, r);
-                else team_float_multi<NA, KIND, U>(qf, rows, dim, slot, r);
-#pragma unroll
-                for (int u = 0; u < U; ++u)
-                    if (slot == 0 && cc[u] < n) cd[cc[u]] = post_op<POST>(r[u]);
-            }
-            __syncwarp();
-        };
+        auto distances = [&](uint32_t n) { src.distances(cid, cd, n); };
 
         auto merge = [&](uint32_t n) {
             for (uint32_t c0 = 0; c0 < n; c0 += 32)
@@ -380,6 +368,122 @@ __global__ void __launch_bounds__(kPagedWarps * 32) paged_kernel(const PagedPara
     }
 }
 
+
+// Full precision: rows from global memory with the shared distance schemas (distance_device.cuh)
+template <typename TD, int KIND, int POST, int NA>
+__global__ void __launch_bounds__(kPagedWarps * 32) paged_kernel(const PagedParams p) {
+    constexpr bool INT = std::is_same<TD, int8_t>::value || std::is_same<TD, uint8_t>::value;
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    uint8_t* base = smem + (size_t)wib * p.warp_smem;
+    float* qf = reinterpret_cast<float*>(base);
+    const int dim = (int)p.dim;
+    struct {
+        const PagedParams& p;
+        float* qf;
+        int lane, dim, qq;
+        __device__ __forceinline__ void load(uint32_t q) {
+            const TD* s = reinterpret_cast<const TD*>(p.queries) + (size_t)q * dim;
+            if constexpr (INT) {
+                uint8_t* qb = reinterpret_cast<uint8_t*>(qf);
+                const int qbytes = (dim + 3) & ~3;
+                for (int e = lane; e < qbytes; e += 32) qb[e] = e < dim ? reinterpret_cast<const uint8_t*>(s)[e] : 0;
+            } else {
+                for (int e = lane; e < dim; e += 32) qf[e] = to_f32(s[e]);  // f16 queries are widened (layers/full.rs:421-423)
+            }
+        }
+        __device__ __forceinline__ void prepare() {
+            qq = 0;  // Sum x^2 of the query (unused by inner product)
+            if constexpr (INT) {
+                if (KIND != KIND_IP) qq = warp_int_self<std::is_same<TD, int8_t>::value>(reinterpret_cast<const uint8_t*>(qf), dim, lane);
+            }
+        }
+        // rows from global memory, a team per row
+        __device__ __forceinline__ void distances(const uint32_t* cid, float* cd, uint32_t n) {
+            constexpr int S = INT ? 32 : 8 * NA, TEAMS = 32 / S, U = kPagedRows;
+            using Row = typename std::conditional<INT, uint8_t, TD>::type;
+            const int team = lane / S, slot = lane % S;
+            for (uint32_t c0 = 0; c0 < n; c0 += TEAMS * U) {
+                float r[U];
+                uint32_t cc[U];
+                const Row* rows[U];
+#pragma unroll
+                for (int u = 0; u < U; ++u) {
+                    cc[u] = c0 + u * TEAMS + team;
+                    rows[u] = reinterpret_cast<const Row*>(p.vectors + (size_t)cid[min(cc[u], n - 1)] * p.row_stride);
+                }
+                if constexpr (INT) warp_int_multi<std::is_same<TD, int8_t>::value, KIND, U>(reinterpret_cast<const uint8_t*>(qf), rows, dim, lane, qq, r);
+                else team_float_multi<NA, KIND, U>(qf, rows, dim, slot, r);
+#pragma unroll
+                for (int u = 0; u < U; ++u)
+                    if (slot == 0 && cc[u] < n) cd[cc[u]] = post_op<POST>(r[u]);
+            }
+            __syncwarp();
+        }
+    } src{p, qf, lane, dim, 0};
+    paged_queries(p, base, lane, src);
+}
+
+// The quantized accessors (MODE as search_kernel_pq: 0 PQ, 1 SQ, 2 MinMax), per candidate the code of quant_device.cuh.
+//   PQ: the query (index dtype, T: Into<f32>) in f32 at the front of the warp's shared memory; TableL2 / TableIP build
+//     the query's table into the warp's own slice of the session's table scratch at every call (it is not kept between
+//     calls), DirectCosine reads the pivots directly.
+//   SQ / MinMax: the query's code words (and MinMax its four compensations), staged once at begin into session memory,
+//     copied to the front of the warp's shared memory; the SQ compensation stays in a register.
+template <int MODE>
+__global__ void __launch_bounds__(kPagedWarps * 32) paged_kernel_quant(const PagedParams p) {
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    uint8_t* base = smem + (size_t)wib * p.warp_smem;
+    const uint32_t entries = p.n_chunks * p.n_centers;
+    struct {
+        const PagedParams& p;
+        float* qf;     // PQ: the f32 query
+        uint32_t* qc;  // SQ / MinMax: the query's code words, then (MinMax) {b, n, a, norm_squared}
+        float* lut;    // PQ tables: this warp's table
+        int lane, dim;
+        uint32_t entries;
+        float q_comp;
+        __device__ __forceinline__ void load(uint32_t q) {
+            if (MODE == 0) {
+                for (int e = lane; e < dim; e += 32) {
+                    float v;
+                    switch (p.dtype) {
+                        case DAB_F32: v = reinterpret_cast<const float*>(p.queries)[(size_t)q * dim + e]; break;
+                        case DAB_F16: v = __half2float(reinterpret_cast<const __half*>(p.queries)[(size_t)q * dim + e]); break;
+                        case DAB_I8: v = (float)reinterpret_cast<const int8_t*>(p.queries)[(size_t)q * dim + e]; break;
+                        default: v = (float)reinterpret_cast<const uint8_t*>(p.queries)[(size_t)q * dim + e]; break;
+                    }
+                    qf[e] = v;
+                }
+            } else {
+                const uint32_t words = p.code_stride >> 2;
+                const uint32_t* src = reinterpret_cast<const uint32_t*>(p.query_codes + (size_t)q * p.code_stride);
+                for (uint32_t w = lane; w < words; w += 32) qc[w] = __ldg(src + w);
+                if (MODE == 1) q_comp = __shfl_sync(kFull, lane == 0 ? __ldg(&p.query_meta[q].x) : 0.0f, 0);
+                if (MODE == 2 && lane == 0) *reinterpret_cast<float4*>(qc + words) = __ldg(p.query_meta + q);
+            }
+        }
+        __device__ __forceinline__ void prepare() {
+            if (MODE == 0 && !p.direct_cosine) {
+                for (uint32_t t = lane; t < entries; t += 32) __stcg(lut + t, pq_table_entry(p, qf, dim, t));
+                __syncwarp();
+            }
+        }
+        // one lane per candidate
+        __device__ __forceinline__ void distances(const uint32_t* cid, float* cd, uint32_t n) {
+            for (uint32_t c = lane; c < n; c += 32) {
+                if (MODE != 0) cd[c] = packed_code_distance<MODE>(p, qc, q_comp, cid[c]);
+                else if (p.direct_cosine) cd[c] = pq_direct_cosine(p, qf, dim, cid[c]);
+                else cd[c] = pq_table_distance(p, lut, cid[c]);
+            }
+            __syncwarp();
+        }
+    } src{p, reinterpret_cast<float*>(base), reinterpret_cast<uint32_t*>(base),
+          p.luts + (size_t)(blockIdx.x * kPagedWarps + wib) * entries, lane, (int)p.dim, entries, 0.0f};
+    paged_queries(p, base, lane, src);
+}
+
 // Moves each listed query to the larger storage fresh[i]: the log and the tail up to their committed lengths are copied
 // and the new table is rebuilt from the log.  One warp per query.
 __global__ void __launch_bounds__(kPagedWarps * 32) paged_relocate_kernel(PagedQuery* qs, const uint32_t* ctr, const uint32_t* list,
@@ -425,6 +529,8 @@ struct dab_paged {
     uint64_t generation = 0;
     dab_paged *prev = nullptr, *next = nullptr;  // the index's open sessions
     uint32_t nq = 0, l_search = 0, cap = 0;
+    int store = -1;           // -1: full precision; else the QuantStore the traversal reads
+    uint64_t store_writes = 0;  // idx->store_writes[store] when the session began
     void (*kern)(const PagedParams) = nullptr;
     PagedParams p{};
     size_t smem_block = 0;
@@ -437,6 +543,8 @@ struct dab_paged {
     uint32_t* d_counters = nullptr;  // [0] work taken, [1] overflowed; then the overflow list [nq]
     uint32_t* d_list = nullptr;      // work list of a re-run [nq]
     uint32_t* d_out = nullptr;       // ids [nq][L], dists [nq][L], counts, cmps, hops [nq]
+    uint8_t* d_qcodes = nullptr;     // SQ / MinMax: the compressed queries, codes [nq][stride] then one float4 each
+    float* d_luts = nullptr;         // PQ tables: one table per warp of the grid, rebuilt at every call
     std::vector<uint64_t> slots;     // every query's table size
     std::vector<void*> chunks;       // visited storage (the first for every query, then one per growth)
 };
@@ -477,6 +585,8 @@ void session_free(dab_paged* s) {
     cudaFree(s->d_counters);
     cudaFree(s->d_list);
     cudaFree(s->d_out);
+    cudaFree(s->d_qcodes);
+    cudaFree(s->d_luts);
     for (void* c : s->chunks) cudaFree(c);
     delete s;
 }
@@ -541,11 +651,12 @@ int run_pass(dab_paged* s) {
     }
 }
 
-template <typename S>
-int prepare_kernel(dab_paged* s) {
+// the shared memory of a warp — the query area of `qbytes`, the candidates, the window — and the grid of `kern`;
+// max_per_sm caps the CTAs per SM
+int plan_kernel(dab_paged* s, void (*kern)(const PagedParams), size_t qbytes, int max_per_sm, const char* who) {
     const dab_index* idx = s->idx;
     PagedParams& p = s->p;
-    size_t off = S::IS_INT ? round_up(round_up((size_t)idx->dim, 4), 16) : round_up((size_t)idx->dim * 4, 16);
+    size_t off = qbytes;
     const size_t ncand = round_up(std::max<size_t>(idx->max_degree, 1) * 4, 16), win = round_up((size_t)s->cap * 4, 16);
     p.off_cid = (uint32_t)off, off += ncand;
     p.off_cd = (uint32_t)off, off += ncand;
@@ -554,26 +665,106 @@ int prepare_kernel(dab_paged* s) {
     p.off_ws = (uint32_t)off, off += win;
     p.warp_smem = (uint32_t)round_up(off, 128);
     s->smem_block = (size_t)p.warp_smem * kPagedWarps;
-    s->kern = paged_kernel_of<S>();
+    s->kern = kern;
     int per_sm = 0;
     if (s->smem_block > 200 * 1024 || cudaFuncSetAttribute(s->kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s->smem_block) != cudaSuccess ||
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, s->kern, kPagedWarps * 32, s->smem_block) != cudaSuccess || per_sm < 1) {
         cudaGetLastError();
-        return fail(DAB_ERR_INVALID_ARGUMENT, "dab_paged_search_begin: L=%u, dim=%u need %zu B shared memory per CTA", s->l_search,
-                    idx->dim, s->smem_block);
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: L=%u, dim=%u need %zu B shared memory per CTA", who, s->l_search, idx->dim, s->smem_block);
     }
-    s->grid = per_sm * idx->sm_count;
+    s->grid = std::min(per_sm, max_per_sm) * idx->sm_count;
     return DAB_OK;
 }
 
-int begin_session(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search, dab_paged* s) {
+template <typename S>
+int prepare_kernel(dab_paged* s) {
+    const size_t qbytes = S::IS_INT ? round_up(round_up((size_t)s->idx->dim, 4), 16) : round_up((size_t)s->idx->dim * 4, 16);
+    return plan_kernel(s, paged_kernel_of<S>(), qbytes, INT32_MAX, "dab_paged_search_begin");
+}
+
+const char* begin_name(int store) {
+    return store == STORE_PQ ? "dab_paged_search_begin_pq" : store == STORE_SQ ? "dab_paged_search_begin_sq"
+           : store == STORE_MINMAX ? "dab_paged_search_begin_minmax" : "dab_paged_search_begin";
+}
+
+// The quantized sessions: the store's parameters into the session's PagedParams, the kernel and its plan.  The query
+// area holds the f32 query (PQ) or the query's code row and its four compensations (SQ, MinMax).
+int prepare_quant_kernel(dab_paged* s) {
+    const dab_index* idx = s->idx;
+    PagedParams& p = s->p;
+    p.dtype = idx->dtype;
+    size_t qbytes;
+    int max_per_sm = INT32_MAX;
+    if (s->store == STORE_PQ) {
+        p.pivots = idx->d_pivots;
+        p.offsets = idx->d_offsets;
+        p.codes = idx->d_codes;
+        p.n_chunks = idx->pq_chunks;
+        p.n_centers = idx->pq_centers;
+        p.ip_table = idx->metric == DAB_INNER_PRODUCT ? 1 : 0;  // L2 and CosineNormalized use TableL2 (dynamic.rs:80-85)
+        p.direct_cosine = idx->metric == DAB_COSINE ? 1 : 0;
+        qbytes = round_up((size_t)idx->dim * 4, 16);
+        // every resident warp owns a table (n_chunks x n_centers f32: 32 KB at 32 x 256) that its lookups read through
+        // L2: the cap of search_kernel_pq keeps them L2-resident
+        if (!p.direct_cosine) max_per_sm = 6;
+    } else {
+        const CodeStore& cs = s->store == STORE_SQ ? idx->sq : idx->mm;
+        p.row_codes = cs.d_codes;
+        p.row_meta = cs.d_meta;
+        p.code_stride = cs.stride;
+        p.code_dim = cs.dim;
+        p.code_nbits = cs.nbits;
+        p.code_metric = idx->metric;
+        p.sq_scale_squared = idx->sq_scale * idx->sq_scale;  // AsFunctor (scalar/quantizer.rs:316-335)
+        p.sq_shift_square_norm = idx->sq_shift_square_norm;
+        qbytes = round_up((size_t)cs.stride + 16, 16);
+    }
+    void (*kern)(const PagedParams) = s->store == STORE_PQ ? paged_kernel_quant<0> : s->store == STORE_SQ ? paged_kernel_quant<1> : paged_kernel_quant<2>;
+    return plan_kernel(s, kern, qbytes, max_per_sm, begin_name(s->store));
+}
+
+// SQ and MinMax: the session's queries compressed by the store's quantizer into session memory (staged through the
+// index's staging scratch, which other calls reuse between pages).  A MinMax query holding a NaN after the transform
+// fails, naming the query.
+int stage_session_queries(dab_paged* s) {
+    dab_index* idx = s->idx;
+    cudaStream_t st = idx->stream;
+    const CodeStore& cs = s->store == STORE_SQ ? idx->sq : idx->mm;
+    const uint8_t* qcodes;
+    const float4* qmeta;
+    int rc;
+    unsigned long long* h_nan = nullptr;
+    if (s->store == STORE_SQ) {
+        if ((rc = sq_stage_queries(idx, st, idx->s_stage, s->d_queries, s->nq, &qcodes, &qmeta))) return rc;
+    } else {
+        if ((rc = idx->h_counters.reserve(24))) return rc;
+        h_nan = (unsigned long long*)((uint32_t*)idx->h_counters.p + 4);
+        if ((rc = minmax_stage_queries(idx, st, idx->s_stage, s->d_queries, s->nq, h_nan, &qcodes, &qmeta))) return rc;
+    }
+    const size_t cbytes = (size_t)s->nq * cs.stride;
+    DAB_CUDA(cudaMalloc(&s->d_qcodes, cbytes + (size_t)s->nq * 16));
+    DAB_CUDA(cudaMemcpyAsync(s->d_qcodes, qcodes, cbytes, cudaMemcpyDeviceToDevice, st));
+    DAB_CUDA(cudaMemcpyAsync(s->d_qcodes + cbytes, qmeta, (size_t)s->nq * 16, cudaMemcpyDeviceToDevice, st));
+    DAB_CUDA(cudaStreamSynchronize(st));
+    if (h_nan && *h_nan != ~0ull)
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: query %llu contains NaN after the transform (InputContainsNaN)", begin_name(s->store), *h_nan);
+    s->p.query_codes = s->d_qcodes;
+    s->p.query_meta = (const float4*)(s->d_qcodes + cbytes);
+    return DAB_OK;
+}
+
+int begin_session(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search, int store, dab_paged* s) {
     s->idx = idx;
     s->generation = idx->generation;
+    s->store = store;
+    if (store >= 0) s->store_writes = idx->store_writes[store];
     s->nq = nq;
     s->l_search = l_search;
     s->cap = l_search + idx->n_start;  // PriorityQueueConfiguration::Resizable(L + #start)
     int rc;
-    if ((rc = visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) { return prepare_kernel<decltype(sc)>(s); }))) return rc;
+    if (store >= 0) rc = prepare_quant_kernel(s);
+    else rc = visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) { return prepare_kernel<decltype(sc)>(s); });
+    if (rc) return rc;
     const size_t qbytes = (size_t)nq * idx->dim * elem_size(idx->dtype), wbytes = (size_t)nq * s->cap * 4;
     const size_t n1 = std::max<uint32_t>(nq, 1);
     DAB_CUDA(cudaMalloc(&s->d_queries, std::max<size_t>(qbytes, 16)));
@@ -589,7 +780,7 @@ int begin_session(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_s
     if (nq == 0) return DAB_OK;
     // the reference's estimate of a search's visited set (or DAB_TEST_VISITED_LOG2), at least what the start points
     // and one expansion need; a query that outgrows it gets a larger table
-    const uint64_t slots = std::max<uint64_t>(table_slots(idx, VisitedHint{}, l_search, 1, 0),
+    const uint64_t slots = std::max<uint64_t>(table_slots(idx, VisitedHint{}, l_search, 1, std::max(store, 0)),
                                               idx->tune.test_visited_log2 ? 0 : ((uint64_t)idx->n_start + idx->max_degree) * 8 / 7 + 64);
     s->slots.assign(nq, slots);
     void* chunk = nullptr;
@@ -602,6 +793,15 @@ int begin_session(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_s
     DAB_CUDA(cudaMemcpyAsync(s->d_qs, qs.data(), (size_t)nq * sizeof(PagedQuery), cudaMemcpyHostToDevice, st));
     DAB_CUDA(cudaMemcpyAsync(s->d_queries, queries, qbytes, cudaMemcpyHostToDevice, st));
     DAB_CUDA(cudaMemsetAsync(s->d_ctr, 0, (size_t)nq * C_WORDS * 4, st));
+    if (store == STORE_SQ || store == STORE_MINMAX) {
+        if ((rc = stage_session_queries(s))) return rc;
+        cudaFree(s->d_queries);  // the kernel reads the compressed queries only
+        s->d_queries = nullptr;
+    }
+    if (store == STORE_PQ && !s->p.direct_cosine) {
+        DAB_CUDA(cudaMalloc(&s->d_luts, (size_t)s->grid * kPagedWarps * idx->pq_chunks * idx->pq_centers * 4));
+        s->p.luts = s->d_luts;
+    }
 
     PagedParams& p = s->p;
     p.vectors = idx->d_vectors;
@@ -635,21 +835,40 @@ void paged_release(dab_index* idx) {
     }
 }
 
-}  // namespace dab
+namespace {
 
-extern "C" {
+// The checks of the synchronous calls on the store a quantized session reads (check_pq_args, search_kernel_pq.cu)
+int check_store(const dab_index* idx, int store, const char* who) {
+    int rc;
+    if (store == STORE_PQ) {
+        if (!idx->d_pivots) return fail(DAB_ERR_NOT_READY, "%s: dab_upload_pq has not been called", who);
+        if (!idx->d_codes || !idx->pq_codes_ready)
+            return fail(DAB_ERR_NOT_READY, "%s: no PQ codes (dab_upload_pq with codes, or dab_pq_encode_all)", who);
+    } else if (store == STORE_SQ) {
+        if ((rc = store_require(idx, &dab_index::sq, "dab_upload_sq", who))) return rc;
+        if (!idx->sq.ready) return fail(DAB_ERR_NOT_READY, "%s: no scalar-quantized rows (dab_upload_sq with rows, or dab_sq_encode_all)", who);
+        // SQStore::distance_computer (providers inmem/scalar.rs:214-226): UnsupportedDistanceMetric
+        if (idx->metric == DAB_COSINE)
+            return fail(DAB_ERR_INVALID_ARGUMENT, "%s: the scalar-quantized store supports L2, InnerProduct and CosineNormalized", who);
+    } else if (store == STORE_MINMAX) {
+        if ((rc = store_require(idx, &dab_index::mm, "dab_upload_minmax", who))) return rc;
+        if (!idx->mm.ready) return fail(DAB_ERR_NOT_READY, "%s: no MinMax rows (dab_upload_minmax with rows, or dab_minmax_encode_all)", who);
+    }
+    return DAB_OK;
+}
 
-int dab_paged_search_begin(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search, dab_paged** out) {
-    if (!idx || !out || (nq && !queries)) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_paged_search_begin: NULL argument");
+// dab_paged_search_begin and its quantized forms (store: -1 full precision, else the QuantStore the traversal reads)
+int paged_begin(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search, int store, dab_paged** out) {
+    const char* who = begin_name(store);
+    if (!idx || !out || (nq && !queries)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", who);
     *out = nullptr;
     int rc;
-    if ((rc = check_search_args(idx, 1, l_search, 1))) return rc;
+    if ((rc = check_search_args(idx, 1, l_search, 1, store < 0)) || (rc = check_store(idx, store, who))) return rc;
     if ((uint64_t)l_search + idx->n_start > 1024)
-        return fail(DAB_ERR_INVALID_ARGUMENT, "dab_paged_search_begin: l_search + n_start = %llu > 1024",
-                    (unsigned long long)l_search + idx->n_start);
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: l_search + n_start = %llu > 1024", who, (unsigned long long)l_search + idx->n_start);
     DAB_CUDA(cudaSetDevice(idx->device));
     dab_paged* s = new dab_paged();
-    if ((rc = begin_session(idx, queries, nq, l_search, s))) {
+    if ((rc = begin_session(idx, queries, nq, l_search, store, s))) {
         cudaStreamSynchronize(idx->stream);
         session_free(s);
         return rc;
@@ -659,6 +878,28 @@ int dab_paged_search_begin(dab_index* idx, const void* queries, uint32_t nq, uin
     idx->paged = s;
     *out = s;
     return DAB_OK;
+}
+
+}  // namespace
+
+}  // namespace dab
+
+extern "C" {
+
+int dab_paged_search_begin(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search, dab_paged** out) {
+    return paged_begin(idx, queries, nq, l_search, -1, out);
+}
+
+int dab_paged_search_begin_pq(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search, dab_paged** out) {
+    return paged_begin(idx, queries, nq, l_search, STORE_PQ, out);
+}
+
+int dab_paged_search_begin_sq(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search, dab_paged** out) {
+    return paged_begin(idx, queries, nq, l_search, STORE_SQ, out);
+}
+
+int dab_paged_search_begin_minmax(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search, dab_paged** out) {
+    return paged_begin(idx, queries, nq, l_search, STORE_MINMAX, out);
 }
 
 int dab_paged_search_next(dab_paged* s, uint32_t k, uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps,
@@ -673,6 +914,8 @@ int dab_paged_search_next(dab_paged* s, uint32_t k, uint32_t* out_ids, float* ou
     dab_index* idx = s->idx;
     if (s->generation != idx->generation)
         return fail(DAB_ERR_INVALID_ARGUMENT, "dab_paged_search_next: index changed since the session began");
+    if (s->store >= 0 && s->store_writes != idx->store_writes[s->store])
+        return fail(DAB_ERR_INVALID_ARGUMENT, "dab_paged_search_next: the session's quantized store was written since the session began");
     if (s->nq == 0) return DAB_OK;
     DAB_CUDA(cudaSetDevice(idx->device));
     const size_t nq = s->nq, rk = nq * k;

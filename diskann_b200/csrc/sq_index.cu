@@ -146,6 +146,7 @@ int dab_upload_sq(dab_index* idx, int nbits, const float* shift, float scale, fl
     DAB_CUDA(cudaStreamSynchronize(idx->stream));
     int rc;
     if ((rc = retire_quantized_stores(idx))) return rc;  // batches in flight read the store
+    ++idx->store_writes[STORE_SQ];
     store_release(idx->sq);
     cudaFree(idx->d_sq_shift);
     idx->d_sq_shift = nullptr;
@@ -163,6 +164,7 @@ int dab_sq_encode_all(dab_index* idx) {
     if ((rc = store_require(idx, &dab_index::sq, "dab_upload_sq", "dab_sq_encode_all"))) return rc;
     if (!idx->vectors_ready) return fail(DAB_ERR_NOT_READY, "dab_sq_encode_all: vectors not uploaded");
     DAB_CUDA(cudaSetDevice(idx->device));
+    ++idx->store_writes[STORE_SQ];
     const uint64_t total = idx->n_total();
     const int grid = (int)std::min<uint64_t>((total + 127) / 128, (uint64_t)idx->sm_count * 16);
     const CodeStore& s = idx->sq;

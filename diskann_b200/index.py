@@ -407,6 +407,20 @@ class GpuIndex:
         every query (each query's list and visited set stay on the device between pages)."""
         return PagedSearch(self, self._queries(queries), l_search)
 
+    def paged_search_pq(self, queries, l_search):
+        """paged_search with the PQ traversal distances of search_batch_pq (TableL2 / TableIP, DirectCosine for
+        Metric::Cosine); pages return those distances (paged search has no rerank)."""
+        return PagedSearch(self, self._queries(queries), l_search, _lib.lib().dab_paged_search_begin_pq)
+
+    def paged_search_sq(self, queries, l_search):
+        """paged_search through the scalar-quantized store, as search_batch_sq traverses it; no rerank."""
+        return PagedSearch(self, self._queries(queries), l_search, _lib.lib().dab_paged_search_begin_sq)
+
+    def paged_search_minmax(self, queries, l_search):
+        """paged_search through the MinMax store, as search_batch_minmax traverses it; no rerank.  A query holding a NaN
+        after the store's transform fails the call."""
+        return PagedSearch(self, self._queries(queries), l_search, _lib.lib().dab_paged_search_begin_minmax)
+
     def search_batch_device(self, d_queries, nq, k, l_search, beam_width, d_ids, d_dists, d_counts=0, d_cmps=0, d_hops=0):
         """Same with device pointers (integers); results stay in HBM."""
         check(_lib.lib().dab_search_batch_device(self._h, C.c_void_p(d_queries), nq, k, l_search, beam_width,
@@ -661,10 +675,12 @@ class PagedSearch:
     """PagedSearch (diskann/src/graph/search/paged.rs) over a query batch: successive, non-overlapping pages of one
     resumable search per query.  Use as a context manager or call close(); closing the index closes it too."""
 
-    def __init__(self, index, queries, l_search):
+    def __init__(self, index, queries, l_search, begin=None):
+        """`begin`: the entry point that opens the session (dab_paged_search_begin, or a quantized store's form)"""
         self._h = C.c_void_p()
         self.index, self.nq, self.l_search = index, queries.shape[0], int(l_search)
-        check(_lib.lib().dab_paged_search_begin(index._h, _ptr(queries), self.nq, self.l_search, C.byref(self._h)))
+        begin = begin or _lib.lib().dab_paged_search_begin
+        check(begin(index._h, _ptr(queries), self.nq, self.l_search, C.byref(self._h)))
         index._paged.add(self)
 
     def next_page(self, k):

@@ -217,6 +217,30 @@ impl<T: Element> GpuIndex<T> {
         Ok(PagedSearch { raw, nq, _index: self })
     }
 
+    /// `paged_search` with the PQ traversal distances (TableL2 / TableIP, DirectCosine for `Metric::Cosine`); pages
+    /// return them (the reference's paged search has no post-processing, so no rerank).
+    pub fn paged_search_pq(&self, queries: &[T], l_search: u32) -> Result<PagedSearch<'_, T>> {
+        self.paged_search_with(sys::dab_paged_search_begin_pq, queries, l_search)
+    }
+
+    /// `paged_search` through the scalar-quantized store; no rerank.
+    pub fn paged_search_sq(&self, queries: &[T], l_search: u32) -> Result<PagedSearch<'_, T>> {
+        self.paged_search_with(sys::dab_paged_search_begin_sq, queries, l_search)
+    }
+
+    /// `paged_search` through the MinMax store; no rerank.  A query holding a NaN after the transform is an error.
+    pub fn paged_search_minmax(&self, queries: &[T], l_search: u32) -> Result<PagedSearch<'_, T>> {
+        self.paged_search_with(sys::dab_paged_search_begin_minmax, queries, l_search)
+    }
+
+    fn paged_search_with(&self, begin: PagedBegin, queries: &[T], l_search: u32) -> Result<PagedSearch<'_, T>> {
+        assert_eq!(queries.len() % self.dim, 0);
+        let nq = queries.len() / self.dim;
+        let mut raw = ptr::null_mut();
+        check(unsafe { begin(self.raw, queries.as_ptr() as *const c_void, nq as u32, l_search, &mut raw) })?;
+        Ok(PagedSearch { raw, nq, _index: self })
+    }
+
     /// One process per GPU: join the communicator described by `id` (from `unique_id()` on rank 0) …
     pub fn comm_init(&mut self, id: &[u8; 128], n_ranks: i32, rank: i32) -> Result<()> {
         check(unsafe { sys::dab_comm_init(self.raw, id.as_ptr() as *const _, n_ranks, rank) })
@@ -231,6 +255,9 @@ impl<T: Element> GpuIndex<T> {
 /// The host-buffer `_async` entry points of the quantized traversals (one signature for PQ, SQ and MinMax).
 type QuantizedAsync = unsafe extern "C" fn(*mut sys::dab_index, u32, *const c_void, u32, u32, u32, u32, std::os::raw::c_int, *mut u32,
                                            *mut f32, *mut u32, *mut u32, *mut u32) -> std::os::raw::c_int;
+
+/// The entry points that open a paged search over a quantized store (one signature for PQ, SQ and MinMax).
+type PagedBegin = unsafe extern "C" fn(*mut sys::dab_index, *const c_void, u32, u32, *mut *mut sys::dab_paged) -> std::os::raw::c_int;
 
 /// A batch in flight on one slot of the device.  Dropping it joins the slot (the library writes into the
 /// buffers it owns until then).

@@ -189,6 +189,22 @@ int dab_search_batch_device(dab_index* idx, const void* d_queries, uint32_t nq, 
 typedef struct dab_paged dab_paged; /* opaque */
 int dab_paged_search_begin(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search,
                            dab_paged** out);
+/* The same sessions over the quantized stores: traversal distances from the PQ table and codes (TableL2 / TableIP,
+ * DirectCosine for Metric::Cosine), the scalar-quantized store or the MinMax store, as dab_search_batch_pq /
+ * dab_search_batch_sq / dab_search_batch_minmax compute them (the PQ table of a query is rebuilt at every call; SQ and
+ * MinMax queries are compressed once, at begin).  Pages return those quantized distances: the reference's paged search
+ * applies no post-processing, so there is no rerank.  begin makes the store checks of the synchronous call (a store
+ * never uploaded: "... has not been called"; rows not ready; Metric::Cosine on the SQ store) and fails on a MinMax
+ * query holding a NaN after the transform, naming it; nothing stays allocated after a failed begin.  next and end are
+ * the calls above.  Besides what invalidates every session, any later write to the session's own store (its upload,
+ * encode-all, dab_pq_train or a broadcast) makes its next page fail with DAB_ERR_INVALID_ARGUMENT; writes to another
+ * store do not, and no store write invalidates a full-precision session. */
+int dab_paged_search_begin_pq(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search,
+                              dab_paged** out);
+int dab_paged_search_begin_sq(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search,
+                              dab_paged** out);
+int dab_paged_search_begin_minmax(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search,
+                                  dab_paged** out);
 int dab_paged_search_next(dab_paged* s, uint32_t k, uint32_t* out_ids, float* out_dists,
                           uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops);
 void dab_paged_search_end(dab_paged* s);

@@ -260,8 +260,17 @@ class GpuKNN {
 template <class T>
 class PagedSearch {
    public:
+    // the traversal store of a session: full precision, or one of the quantized stores (no rerank: pages return the
+    // store's distances)
+    enum class Store { FullPrecision, PQ, SQ, MinMax };
+
     PagedSearch(Provider<T>& provider, const T* queries, uint32_t nq, uint32_t l_value) : nq_(nq) {
         check(dab_paged_search_begin(provider.raw(), queries, nq, l_value, &h_));
+    }
+    PagedSearch(Provider<T>& provider, Store store, const T* queries, uint32_t nq, uint32_t l_value) : nq_(nq) {
+        auto begin = store == Store::PQ ? dab_paged_search_begin_pq : store == Store::SQ ? dab_paged_search_begin_sq
+                     : store == Store::MinMax ? dab_paged_search_begin_minmax : dab_paged_search_begin;
+        check(begin(provider.raw(), queries, nq, l_value, &h_));
     }
     ~PagedSearch() { dab_paged_search_end(h_); }
     PagedSearch(const PagedSearch&) = delete;

@@ -6,12 +6,15 @@ process, on the index's stream:
     around the call, which returns only after the device has finished and the page is in host memory;
   * dab_search_batch(k = 10, L = 100), the first page's one-shot twin;
   * dab_search_batch(k = 100, L = 100), one search that returns as many results as ten pages.
+--store picks the traversal store (default fp, full precision): sq (SQ-8), minmax (MinMax-8 behind DoubleHadamard) or
+pq (PQ-32 trained on 100K rows with dab_pq_train); the session is then dab_paged_search_begin_{sq,minmax,pq}, the
+one-shot twins the store's dab_search_batch_{sq,minmax,pq} without rerank, and a comparison reads the store's code row.
 Every timed call runs --reps times after one warm-up (a new session each time for the paged arm); the median is
 reported.  Also reported: the device memory a session holds per query (cudaMemGetInfo before begin, after begin and
 after the last page), and the bytes the traversal reads per query from the cumulative cmps / hops (a 512-byte row per
 comparison, a 4 * (max_degree + 1)-byte adjacency row per hop).  The card's name and power limit are read in the same
 run.
-usage: python tools/bench_paged.py [--n N] [--nq NQ] [--pages P] [--reps R] [--json PATH]"""
+usage: python tools/bench_paged.py [--n N] [--nq NQ] [--pages P] [--reps R] [--store {fp,pq,sq,minmax}] [--json PATH]"""
 import argparse
 import json
 import os
@@ -26,6 +29,7 @@ import numpy as np
 import torch
 
 import bench
+import diskann_b200 as dab
 from bench_minmax_search import build_index, card
 
 K, L = 10, 100
@@ -37,6 +41,7 @@ def main():
     ap.add_argument("--nq", type=int, default=0)
     ap.add_argument("--pages", type=int, default=10)
     ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--store", choices=["fp", "pq", "sq", "minmax"], default="fp")
     ap.add_argument("--json", default="")
     args = ap.parse_args()
     name, power = card()
@@ -44,9 +49,26 @@ def main():
     n, nq = args.n or cfg["n"], args.nq or cfg["nq"]
     stream = torch.cuda.Stream()
     torch.cuda.set_stream(stream)
-    g, _, centers = build_index(cfg, n, stream)
+    g, base, centers = build_index(cfg, n, stream)
     queries = bench.make_data(cfg, bench.SEED_QUERY, nq, centers)
-    row_bytes, adj_bytes = cfg["dim"] * 4, 4 * (g.max_degree + 1)
+    dim = cfg["dim"]
+    row_bytes, adj_bytes = dim * 4, 4 * (g.max_degree + 1)
+    begin, one_shot = g.paged_search, g.search_batch
+    if args.store == "sq":
+        mean, std = base.mean(0).astype(np.float32), float(base.std())
+        shift = (mean - np.float32(2.5 * std)).astype(np.float32)
+        g.upload_sq(8, shift, float(np.float32(5.0 * std)), float(np.dot(shift, shift)), 0.0)
+        g.sq_encode_all()
+        begin, one_shot, row_bytes = g.paged_search_sq, g.search_batch_sq, dim
+    elif args.store == "minmax":
+        g.upload_minmax(8, 1.0, dab.Transform.double_hadamard(dim, "same", seed=7))
+        g.minmax_encode_all()
+        begin, one_shot, row_bytes = g.paged_search_minmax, g.search_batch_minmax, dim + 16
+    elif args.store == "pq":
+        sample = np.sort(np.random.default_rng(bench.SEED_PQ).choice(n, size=min(100_000, n), replace=False))
+        g.pq_train(base[sample].astype(np.float32), 32, 256, 5, bench.SEED_PQ)
+        g.pq_encode_all()
+        begin, one_shot, row_bytes = g.paged_search_pq, g.search_batch_pq, 32
 
     def timed(fn):
         torch.cuda.synchronize()
@@ -56,7 +78,7 @@ def main():
 
     def session():
         free0 = torch.cuda.mem_get_info()[0]
-        t_begin, s = timed(lambda: g.paged_search(queries, L))
+        t_begin, s = timed(lambda: begin(queries, L))
         free1 = torch.cuda.mem_get_info()[0]
         pages = [timed(lambda: s.next_page(K)) for _ in range(args.pages)]
         free2 = torch.cuda.mem_get_info()[0]
@@ -70,8 +92,8 @@ def main():
     cmps, hops = last[-1][1][3].astype(np.float64), last[-1][1][4].astype(np.float64)
     one = {}
     for k in (K, K * args.pages):
-        g.search_batch(queries, k, L)  # warm-up
-        t = [timed(lambda: g.search_batch(queries, k, L)) for _ in range(args.reps)]
+        one_shot(queries, k, L)  # warm-up
+        t = [timed(lambda: one_shot(queries, k, L)) for _ in range(args.reps)]
         r = t[-1][1]
         one[k] = dict(ms=round(statistics.median(x[0] for x in t), 3), mean_cmps=round(float(r[3].mean()), 1),
                       mean_hops=round(float(r[4].mean()), 1),
@@ -89,6 +111,8 @@ def main():
                    algorithmic_mb_per_query=round(float((cmps * row_bytes + hops * adj_bytes).mean()) / 1e6, 4),
                    pages_disjoint=bool(distinct)),
         search_batch_k10=one[K], search_batch_k100=one[K * args.pages])
+    if args.store != "fp":
+        summary["store"] = {"pq": "pq32_dab_pq_train", "sq": "sq8", "minmax": "minmax8_doublehadamard"}[args.store]
     print(json.dumps(summary), flush=True)
     if args.json:
         os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)
