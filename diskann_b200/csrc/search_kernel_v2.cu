@@ -9,7 +9,8 @@
 //
 //   * f32 rows of 32..128 elements with level 1 of the visited set on (REG): every surviving row of a hop
 //     gets one bulk L2 prefetch, then the rows are read straight into registers, 8 lanes per row and
-//     4 rows per pass (wide_distances_f32_fast, the lane mapping of search_kernel_v3);
+//     4 rows per pass (wide_distances_f32_fast, the lane mapping of search_kernel_v3); prefetches and
+//     loads both carry the evict_first policy of the staged copies;
 //   * all other rows are staged in shared memory with cp.async (16 B per lane, eight lanes per row:
 //     one warp instruction moves 128 B of four rows and no lane needs another lane's address; no
 //     registers tied up), a stage of rows in flight at once (a TMA bulk-copy variant was measured
@@ -352,7 +353,7 @@ __global__ void __launch_bounds__(kV2Warps * 32, REG ? kV2MinCtasReg : QT == 0 ?
                         q2[2 * m + 1] = pack2(x.z, x.w);
                     }
                 }
-                wide_distances_f32_fast<KIND, POST>(q2, nm, p.vectors, p.row_stride, cid, n, cd, lane);
+                wide_distances_f32_fast<KIND, POST, true>(q2, nm, p.vectors, p.row_stride, cid, n, cd, lane, row_policy);
                 __syncwarp();
             } else if constexpr (QT == 0) {
                 // a team per row, kRowsInFlight rows per team and pass: the whole warp (integers, NA = 4 float

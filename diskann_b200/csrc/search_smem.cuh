@@ -104,18 +104,37 @@ __device__ __forceinline__ void prefetch_rows(const uint8_t* __restrict__ vector
 // 16 query elements a lane ever multiplies live in registers (packed pairs), and a step covers
 // one pass of 4 rows whose nm 16-byte loads per lane are issued back to back (one pass rather
 // than two per step: 16 fewer registers).
-template <int KIND, int POST>
+// HINT: the prefetches and the loads carry the L2 cache policy `pol` (search_kernel_v2 passes evict_first: a row is
+// read once per query, so rows should leave L2 before the adjacency rows and the rows that many queries share).
+template <int KIND, int POST, bool HINT = false>
 __device__ __forceinline__ void wide_distances_f32_fast(const uint64_t (&q2)[8], int nm, const uint8_t* __restrict__ vectors,
                                                         size_t row_stride, const uint32_t* __restrict__ cid, uint32_t n,
-                                                        float* __restrict__ cd, int lane) {
+                                                        float* __restrict__ cd, int lane, uint64_t pol = 0) {
     const int team = lane >> 3, tl = lane & 7;
-    if (n > 4) prefetch_rows(vectors, row_stride, cid, n, (uint32_t)nm * 128u, lane);
+    if (n > 4) {
+        if constexpr (HINT) {
+            for (uint32_t j = lane; j < n; j += 32)
+                asm volatile("cp.async.bulk.prefetch.L2.global.L2::cache_hint [%0], %1, %2;" ::"l"(vectors + (size_t)cid[j] * row_stride),
+                             "r"((uint32_t)nm * 128u), "l"(pol)
+                             : "memory");
+        } else {
+            prefetch_rows(vectors, row_stride, cid, n, (uint32_t)nm * 128u, lane);
+        }
+    }
     for (uint32_t j0 = 0; j0 < n; j0 += 4) {
         const uint8_t* row0 = vectors + (size_t)cid[min(j0 + team, n - 1)] * row_stride + 16 * tl;
         uint4 v0[4];
 #pragma unroll
-        for (int m = 0; m < 4; ++m)
-            if (m < nm) v0[m] = ldg16(row0 + m * 128);
+        for (int m = 0; m < 4; ++m) {
+            if (m < nm) {
+                if constexpr (HINT)
+                    asm volatile("ld.global.nc.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"
+                                 : "=r"(v0[m].x), "=r"(v0[m].y), "=r"(v0[m].z), "=r"(v0[m].w)
+                                 : "l"(row0 + m * 128), "l"(pol));
+                else
+                    v0[m] = ldg16(row0 + m * 128);
+            }
+        }
         uint64_t a0[2] = {0ull, 0ull};
 #pragma unroll
         for (int m = 0; m < 4; ++m) {
