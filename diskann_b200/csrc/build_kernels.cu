@@ -415,6 +415,186 @@ __global__ void __launch_bounds__(kPruneWarps * 32) backedge_kernel(const Backed
     }
 }
 
+// ------------------------------------------------------------------ consolidation
+// DiskANNIndex::consolidate_vector (index.rs:1819-1931) for every node at once.  Node v's new list depends only on v's
+// list, the lists of its deleted neighbours and the deletion table, and no deleted node's list is ever written, so one
+// pass in any order equals the reference's sequential loop; rows are rewritten in place.  One warp per node:
+//   * a deleted v is left alone; a v with no deleted (or out-of-range) neighbour and at most `degree` distinct live
+//     neighbours is left alone (lists no longer than `degree` skip the distinct count);
+//   * the pool is a set in a canonical order: v's live neighbours in list order, then for each deleted neighbour in
+//     list order its live neighbours in list order, first occurrence kept (the reference's HashSet leaves the order
+//     unspecified).  An id >= n_total is a deleted neighbour with no neighbours.  Membership is a per-warp open-
+//     addressing table in global memory, cleared after each node through the slots the pool recorded;
+//   * v is then dropped; a pool of fewer than `degree` ids is the new list as it is, otherwise robust_prune_list
+//     (index.rs:2397-2454): Distance<T,T>(v, u), sorted by (distance, arrival order) and cut to the 750 smallest —
+//     streamed through the prune's shared-memory pool as in backedge_kernel, since a pool can hold
+//     max_degree * (max_degree + 1) ids — then occlude_list without saturation.
+constexpr uint32_t kConsolidateP = 1024;  // shared-memory pool slots per warp (> kMaxOcclusion)
+
+struct ConsolidateParams {
+    const uint8_t* vectors;
+    size_t row_stride;
+    int dim;
+    uint32_t* adj;
+    uint32_t adj_stride, max_degree;
+    uint64_t n_points, n_total;
+    const uint32_t* deleted;  // NULL: nothing deleted
+    uint32_t degree;
+    float alpha;
+    int prune_kind;
+    uint32_t* hash;  // per warp: 1 << hash_bits ids, kNoId = empty
+    int hash_bits;
+    uint32_t* pool;       // per warp: pool_cap ids
+    uint32_t* pool_slot;  // per warp: the hash slot of each pool id
+    uint32_t pool_cap;
+    uint32_t* counters;  // [0] next node, [1] lists rewritten
+};
+
+// 96 registers: below that ptxas spills the pool-building and prune state of the float schemas
+template <typename TD, int NA, int KIND, int POST, bool IS_INT, bool SIGNED>
+__global__ void __maxnreg__(96) consolidate_kernel(const ConsolidateParams p) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    PruneSmem s = carve(smem + (size_t)wib * prune_smem_bytes(kConsolidateP), kConsolidateP);
+    const uint32_t warp = blockIdx.x * kPruneWarps + wib;
+    const uint32_t hmask = (1u << p.hash_bits) - 1u;
+    uint32_t* hash = p.hash + ((size_t)warp << p.hash_bits);
+    uint32_t* pool = p.pool + (size_t)warp * p.pool_cap;
+    uint32_t* pslot = p.pool_slot + (size_t)warp * p.pool_cap;
+    auto dead = [&](uint32_t id) {  // deleted, or a status lookup that fails
+        return id >= p.n_total || (p.deleted && (__ldg(p.deleted + (id >> 5)) >> (id & 31) & 1u));
+    };
+    uint32_t n = 0;  // pool size
+    // every lane calls; `want`: this lane offers `id`.  New ids are appended in lane order; among lanes offering the
+    // same id the first one inserts it.
+    auto add = [&](uint32_t id, bool want) {
+        const unsigned peers = __match_any_sync(kFull, want ? id : kNoId);
+        uint32_t slot = kNoId;
+        if (want && __ffs(peers) - 1 == lane) {
+            uint32_t h = (id * 0x9E3779B1u) >> (32 - p.hash_bits);
+            for (;;) {
+                const uint32_t old = atomicCAS(hash + h, kNoId, id);
+                if (old == kNoId) {
+                    slot = h;
+                    break;
+                }
+                if (old == id) break;
+                h = (h + 1) & hmask;
+            }
+        }
+        const unsigned mn = __ballot_sync(kFull, slot != kNoId);
+        if (slot != kNoId) {
+            const uint32_t pos = n + __popc(mn & ((1u << lane) - 1u));
+            pool[pos] = id;
+            pslot[pos] = slot;
+        }
+        n += __popc(mn);
+    };
+    for (;;) {
+        uint32_t v = 0;
+        if (lane == 0) v = atomicAdd(p.counters, 1u);
+        v = __shfl_sync(kFull, v, 0);
+        if (v >= p.n_total) break;
+        if (dead(v)) continue;  // ConsolidateKind::Deleted
+        uint32_t* row = p.adj + (size_t)v * p.adj_stride;
+        const uint32_t deg = min(row[0], p.max_degree);
+        bool any_dead = false;
+        for (uint32_t j = lane; j < deg; j += 32) any_dead |= dead(row[1 + j]);
+        any_dead = __any_sync(kFull, any_dead);
+        if (!any_dead && deg <= p.degree) continue;
+        n = 0;
+        for (uint32_t c = 0; c < deg; c += 32) {
+            const uint32_t j = c + lane;
+            const uint32_t id = j < deg ? row[1 + j] : kNoId;
+            add(id, j < deg && !dead(id));
+        }
+        // the early exit counts a self-loop
+        if (any_dead || n > p.degree) {
+            for (uint32_t c = 0; c < deg; c += 32) {
+                const uint32_t j = c + lane;
+                const uint32_t id = j < deg ? row[1 + j] : kNoId;
+                unsigned dm = __ballot_sync(kFull, j < deg && dead(id));
+                while (dm) {
+                    const int src = __ffs(dm) - 1;
+                    dm &= dm - 1;
+                    const uint32_t u = __shfl_sync(kFull, id, src);
+                    if (u >= p.n_total) continue;
+                    const uint32_t* urow = p.adj + (size_t)u * p.adj_stride;
+                    const uint32_t udeg = min(urow[0], p.max_degree);
+                    for (uint32_t c2 = 0; c2 < udeg; c2 += 32) {
+                        const uint32_t j2 = c2 + lane;
+                        const uint32_t w = j2 < udeg ? urow[1 + j2] : kNoId;
+                        add(w, j2 < udeg && !dead(w));
+                    }
+                }
+            }
+            // drop v (a self-loop): its table slot is cleared and the pool after it moves down one place
+            uint32_t pv = kNoId;
+            for (uint32_t c = 0; c < n; c += 32) {
+                const unsigned m = __ballot_sync(kFull, c + lane < n && pool[c + lane] == v);
+                if (m) pv = c + __ffs(m) - 1;
+            }
+            if (pv != kNoId) {
+                if (lane == 0) hash[pslot[pv]] = kNoId;
+                for (uint32_t c = pv; c + 1 < n; c += 32) {
+                    const uint32_t j = c + lane;
+                    uint32_t id = 0, slot = 0;
+                    if (j + 1 < n) id = pool[j + 1], slot = pslot[j + 1];
+                    __syncwarp();
+                    if (j + 1 < n) pool[j] = id, pslot[j] = slot;
+                    __syncwarp();
+                }
+                --n;
+            }
+            if (n < p.degree) {
+                for (uint32_t j = lane; j < n; j += 32) row[1 + j] = pool[j];
+                if (lane == 0) row[0] = n;
+            } else {
+                // Distance<T,T>(v, u) for the pool in arrival order, streamed into the shared pool: whenever its slots
+                // are full it is sorted by (distance, arrival) and cut to 750, which keeps what one sort would keep
+                uint32_t ns = 0;
+                for (uint32_t j0 = 0; j0 < n; j0 += kPairsPerPass) {
+                    const uint32_t cnt = min(n - j0, (uint32_t)kPairsPerPass);
+                    uint32_t rows[kPairsPerPass];
+#pragma unroll
+                    for (int g = 0; g < kPairsPerPass; ++g) rows[g] = pool[j0 + min((uint32_t)g, cnt - 1)];
+                    float dist[kPairsPerPass];
+                    warp_row_distances<TD, NA, KIND, POST, IS_INT, SIGNED>(p.vectors, p.row_stride, p.dim, v, rows, lane, dist);
+#pragma unroll
+                    for (int g = 0; g < kPairsPerPass; ++g) {
+                        if ((uint32_t)g < cnt) {
+                            if (ns == kConsolidateP) {
+                                __syncwarp();
+                                warp_sort_pool(s, ns, kConsolidateP, lane, true);
+                                ns = kMaxOcclusion;
+                            }
+                            if (lane == 0) {
+                                s.ids[ns] = rows[g];
+                                s.d[ns] = dist[g];
+                                s.order[ns] = j0 + g;
+                            }
+                            ++ns;
+                        }
+                    }
+                    __syncwarp();
+                }
+                uint32_t P2 = 2;
+                while (P2 < ns) P2 <<= 1;
+                warp_sort_pool(s, ns, P2, lane, true);
+                ns = min(ns, kMaxOcclusion);
+                const uint32_t found = warp_robust_prune<TD, NA, KIND, POST, IS_INT, SIGNED>(s, ns, v, p.degree, p.alpha, p.prune_kind,
+                                                                                             p.vectors, p.row_stride, p.dim, lane);
+                __syncwarp();
+                for (uint32_t f = lane; f < found; f += 32) row[1 + f] = s.ids[s.nbr[f]];
+                if (lane == 0) row[0] = found;
+            }
+            if (lane == 0) atomicAdd(p.counters + 1, 1u);
+        }
+        for (uint32_t j = lane; j < n; j += 32) hash[pslot[j]] = kNoId;
+        __syncwarp();
+    }
+}
+
 __global__ void iota_kernel(uint32_t* p, uint32_t first, uint32_t n) {
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) p[i] = first + i;
 }
@@ -532,6 +712,68 @@ int dab_robust_prune(dab_index* idx, const uint32_t* pool_ids, const float* pool
     DAB_CUDA(cudaMemcpyAsync(out_ids, b_out.p, np * degree * 4, cudaMemcpyDeviceToHost, idx->stream));
     DAB_CUDA(cudaMemcpyAsync(out_counts, b_cnt.p, np * 4, cudaMemcpyDeviceToHost, idx->stream));
     DAB_CUDA(cudaStreamSynchronize(idx->stream));
+    return DAB_OK;
+}
+
+int dab_consolidate(dab_index* idx, uint32_t pruned_degree, float alpha, uint64_t* out_rewritten) {
+    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_consolidate: idx is NULL");
+    int rc;
+    if ((rc = refuse_in_flight(idx, "dab_consolidate"))) return rc;
+    if (!idx->vectors_ready || !idx->graph_ready) return fail(DAB_ERR_NOT_READY, "dab_consolidate: vectors and graph must be uploaded first");
+    if (pruned_degree == 0 || pruned_degree > idx->max_degree)
+        return fail(DAB_ERR_INVALID_ARGUMENT, "dab_consolidate: pruned_degree must be in [1, max_degree]");
+    if (!(alpha >= 1.0f)) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_consolidate: alpha must be >= 1");
+    DAB_CUDA(cudaSetDevice(idx->device));
+    ConsolidateParams p;
+    memset(&p, 0, sizeof(p));
+    p.vectors = idx->d_vectors;
+    p.row_stride = idx->row_stride;
+    p.dim = (int)idx->dim;
+    p.adj = idx->d_adj;
+    p.adj_stride = idx->adj_stride;
+    p.max_degree = idx->max_degree;
+    p.n_points = idx->n_points;
+    p.n_total = idx->n_total();
+    p.deleted = deleted_filter(idx);
+    p.degree = pruned_degree;
+    p.alpha = alpha;
+    p.prune_kind = idx->metric == DAB_INNER_PRODUCT ? 1 : 0;  // PruneKind::from_metric, config/mod.rs:69-76
+    // a pool holds distinct ids: at most max_degree live neighbours plus max_degree per deleted one, and n_total
+    p.pool_cap = (uint32_t)std::min<uint64_t>(idx->n_total(), (uint64_t)idx->max_degree * (idx->max_degree + 1));
+    p.hash_bits = 5;
+    while ((1ull << p.hash_bits) < 2ull * p.pool_cap) ++p.hash_bits;  // at most half full
+    const size_t warp_bytes = ((1ull << p.hash_bits) + 2ull * p.pool_cap) * 4;
+    const size_t smem = prune_smem_bytes(kConsolidateP) * kPruneWarps;
+    DevBuf b_scratch, b_counters;
+    uint32_t counters[2] = {0, 0};
+    rc = visit_schema<OPS_ROW>(idx->dtype, idx->metric, [&](auto s) -> int {
+        using S = decltype(s);
+        auto kern = consolidate_kernel<KernelRow<S>, S::NA, S::KIND, S::POST, S::IS_INT, S::SIGNED>;
+        DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        int per_sm = 0;
+        DAB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kPruneWarps * 32, smem));
+        // every resident warp, within 2 GB of tables and pools
+        uint64_t blocks = std::max(1, per_sm) * (uint64_t)idx->sm_count;
+        blocks = std::max<uint64_t>(1, std::min<uint64_t>(blocks, (2ull << 30) / (warp_bytes * kPruneWarps)));
+        blocks = std::min<uint64_t>(blocks, (idx->n_total() + kPruneWarps - 1) / kPruneWarps);
+        int rc2;
+        if ((rc2 = b_scratch.alloc(blocks * kPruneWarps * warp_bytes)) || (rc2 = b_counters.alloc(8))) return rc2;
+        p.hash = (uint32_t*)b_scratch.p;
+        p.pool = p.hash + (blocks * kPruneWarps << p.hash_bits);
+        p.pool_slot = p.pool + blocks * kPruneWarps * p.pool_cap;
+        p.counters = (uint32_t*)b_counters.p;
+        DAB_CUDA(cudaMemsetAsync(p.hash, 0xFF, (blocks * kPruneWarps << p.hash_bits) * 4, idx->stream));
+        DAB_CUDA(cudaMemsetAsync(p.counters, 0, 8, idx->stream));
+        kern<<<(int)blocks, kPruneWarps * 32, smem, idx->stream>>>(p);
+        DAB_LAUNCHED();
+        DAB_CUDA(cudaGetLastError());
+        DAB_CUDA(cudaMemcpyAsync(counters, p.counters, 8, cudaMemcpyDeviceToHost, idx->stream));
+        DAB_CUDA(cudaStreamSynchronize(idx->stream));
+        return DAB_OK;
+    });
+    if (rc) return rc;
+    if (counters[1]) ++idx->generation;  // adjacency rows were written: open paged sessions fail their next page
+    if (out_rewritten) *out_rewritten = counters[1];
     return DAB_OK;
 }
 

@@ -139,6 +139,7 @@ void dab_destroy(dab_index* idx) {
     comm_release(idx);
     tc_release(idx);
     minmax_release(idx);
+    deleted_release(idx);
     store_release(idx->sq);
     store_release(idx->mm);
     cudaFree(idx->d_vectors);

@@ -35,6 +35,16 @@ void search_slots_release(struct ::dab_index* idx);  // search_kernel.cu
 int retire_quantized_stores(struct ::dab_index* idx);
 void minmax_release(struct ::dab_index* idx);        // minmax_index.cu: the store's transform
 void paged_release(struct ::dab_index* idx);         // search_paged.cu: every paged search session still open
+// delete_kernels.cu: the deletion table.  deleted_assign replaces it with `words` ((n_total + 31) / 32 of them, bit i of
+// word i / 32 for id i) holding n_deleted set bits; n_deleted == 0 clears it (words may then be NULL).
+int deleted_assign(struct ::dab_index* idx, const uint32_t* words, uint64_t n_deleted);
+int deleted_alloc(struct ::dab_index* idx);  // both copies of the table, every bit clear (nothing when they exist)
+void deleted_release(struct ::dab_index* idx);
+// the device bitmap the searches filter with while some id is deleted, else NULL
+const uint32_t* deleted_filter(const struct ::dab_index* idx);
+// The calls that change the deletion table or consolidate wait for no batch: "<api>: slot i holds a batch in flight"
+// while one does
+int refuse_in_flight(const struct ::dab_index* idx, const char* api);
 
 #define DAB_CUDA(expr)                                                                        \
     do {                                                                                      \
@@ -184,6 +194,11 @@ struct dab_index {
     // (upload, encode-all, PQ training, broadcast).  Only paged search sessions over that store read it.
     uint64_t store_writes[3] = {};
     void* paged = nullptr;  // the open paged search sessions (a list, search_paged.cu)
+    // the deletion table (delete_kernels.cu; providers TableDeleteProviderAsync): one bit per id, kept on the host and
+    // copied to the device after every change.  Both are allocated by the first dab_delete; n_deleted counts set bits.
+    uint32_t* h_deleted = nullptr;  // (n_total + 31) / 32 words
+    uint32_t* d_deleted = nullptr;
+    uint64_t n_deleted = 0;
     uint64_t rec_truncated = 0;  // build: searches whose expanded-node record was cut at its capacity
     dab::Tuning tune;
 
@@ -197,4 +212,5 @@ struct dab_index {
     int nccl_rank = 0, nccl_ranks = 0;
 
     uint64_t n_total() const { return n_points + n_start; }
+    uint64_t deleted_words() const { return (n_total() + 31) / 32; }
 };

@@ -79,6 +79,7 @@ int need_nccl(const char* who) {
 struct IndexMeta {
     uint64_t n_points, row_stride;
     uint32_t dtype, metric, dim, n_start, max_degree, adj_stride, vectors_ready, graph_ready, pq_chunks, pq_centers, pq_codes_ready, pq_uniform_len;
+    uint64_t n_deleted;  // the deletion table travels with the graph: replicas would otherwise return deleted ids
 };
 
 IndexMeta meta_of(const dab_index* idx) {
@@ -98,6 +99,7 @@ IndexMeta meta_of(const dab_index* idx) {
     m.pq_centers = idx->pq_centers;
     m.pq_codes_ready = idx->pq_codes_ready;
     m.pq_uniform_len = idx->pq_uniform_len;
+    m.n_deleted = idx->n_deleted;
     return m;
 }
 
@@ -137,6 +139,18 @@ int broadcast_buffers(dab_index* idx, ncclComm_t comm, int root, bool is_root, I
         DAB_NCCL(n.Broadcast(idx->d_pivots, idx->d_pivots, (size_t)got.pq_centers * idx->dim * 4, kNcclUint8, root, comm, st));
         DAB_NCCL(n.Broadcast(idx->d_offsets, idx->d_offsets, (size_t)(got.pq_chunks + 1) * 4, kNcclUint8, root, comm, st));
         DAB_NCCL(n.Broadcast(idx->d_codes, idx->d_codes, total * (size_t)got.pq_chunks, kNcclUint8, root, comm, st));
+    }
+    int rc;
+    if (got.n_deleted) {
+        // the root's table into every rank's device copy, then into its host copy
+        if ((rc = deleted_alloc(idx))) return rc;
+        DAB_NCCL(n.Broadcast(idx->d_deleted, idx->d_deleted, idx->deleted_words() * 4, kNcclUint8, root, comm, st));
+        std::vector<uint32_t> words(idx->deleted_words());
+        DAB_CUDA(cudaMemcpyAsync(words.data(), idx->d_deleted, idx->deleted_words() * 4, cudaMemcpyDeviceToHost, st));
+        DAB_CUDA(cudaStreamSynchronize(st));
+        if ((rc = deleted_assign(idx, words.data(), got.n_deleted))) return rc;
+    } else if ((rc = deleted_assign(idx, nullptr, 0))) {
+        return rc;
     }
     DAB_CUDA(cudaStreamSynchronize(st));
     ++idx->generation;
@@ -265,6 +279,10 @@ int dab_broadcast(dab_index* const* per_gpu, int n_gpus) {
             bcast((size_t)(want.pq_chunks + 1) * 4, [](dab_index* x) { return x->d_offsets; }) ||
             bcast(total * (size_t)want.pq_chunks, [](dab_index* x) { return x->d_codes; }))
             status = fail(DAB_ERR_CUDA, "dab_broadcast: ncclBroadcast(PQ) failed");
+    }
+    for (int i = 1; i < n_gpus && status == DAB_OK; ++i) {
+        cudaSetDevice(per_gpu[i]->device);
+        status = deleted_assign(per_gpu[i], root->h_deleted, root->n_deleted);
     }
     for (int i = 0; i < n_gpus; ++i) {
         cudaSetDevice(per_gpu[i]->device);

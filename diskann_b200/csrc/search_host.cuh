@@ -29,6 +29,12 @@ struct SearchOut {
     uint32_t *counts, *cmps, *hops;
 };
 
+// RemoveDeletedIdsAndCopy over whole lists (delete_kernels.cu): the traversal wrote each query's non-start entries,
+// list order, into ids / dists [nq][cap] (padded with UINT32_MAX); the first k that `deleted` does not mark go to `out`
+// ([nq][k], padded UINT32_MAX / +inf; counts = how many), queued on `stream`.  cmps and hops are not touched.
+int queue_drop_deleted(const dab_index* idx, cudaStream_t stream, const uint32_t* deleted, const uint32_t* ids, const float* dists,
+                       uint32_t cap, uint32_t nq, uint32_t k, const SearchOut& out);
+
 // The synchronous host-buffer calls: checks the buffers, copies the queries to the handle's scratch, runs `run` on them
 // with device result buffers, copies the results to `out` and waits.  `api` names the entry point in error messages.
 int search_host_buffers(dab_index* idx, const char* api, const void* queries, uint32_t nq, uint32_t k, const SearchOut& out,
@@ -56,7 +62,8 @@ struct HostCopy {
 struct SearchSlot {
     cudaStream_t stream = nullptr;
     Scratch tables, counters, queries, out, stats, h_counters;
-    Scratch stage, luts, lists;  // the quantized traversals: staged queries, per-warp LUTs, the rerank's candidate lists
+    Scratch stage, luts;  // the quantized traversals: staged queries, per-warp LUTs
+    Scratch lists;        // the rerank's candidate lists, or the whole lists a search filters deleted ids from
     SlotJob* job = nullptr;
     HostCopy host_out{};  // the pending call's result copies (host_out.host.ids null: device buffers)
 };

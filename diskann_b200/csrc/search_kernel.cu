@@ -75,11 +75,17 @@ struct SearchJob : SlotJob {
     cudaStream_t stream = nullptr;
     Scratch* tables = nullptr;
     Scratch* counters = nullptr;
+    Scratch* lists = nullptr;        // the whole lists, while deleted ids are filtered
     uint32_t* h_counters = nullptr;  // pinned, 4 words
     bool full_grid = false;          // batches in flight: launch every resident worker (the next batch fills what this one leaves)
 
     uint32_t nq = 0, l_search = 0, beam = 0;
     bool recording = false;
+    // some id is deleted: the traversal writes every non-start entry of a list (k = L + #start) to `lists`, and each
+    // pass is followed by the filter into `filtered`, the caller's buffers
+    const uint32_t* deleted = nullptr;
+    SearchOut filtered{};
+    uint32_t k_out = 0;
     SearchParamsV2 p2;
     SearchParamsV3 p3;
     V2Launch v2;
@@ -104,8 +110,19 @@ int SearchJob::prepare(const void* d_queries, const uint32_t* d_query_rows, uint
     nq = nq_, l_search = l_search_, beam = beam_;
     recording = rec_ids != nullptr;
 
-    memset(&p2, 0, sizeof(p2));
     int rc;
+    // the build's insert searches ignore deletions, as the reference's insert does
+    deleted = recording ? nullptr : deleted_filter(idx);
+    if (deleted) {
+        const size_t cap = (size_t)l_search + idx->n_start;
+        if ((rc = lists->reserve((size_t)nq * cap * 8))) return rc;
+        filtered = SearchOut{d_ids, d_dists, d_counts, d_cmps, d_hops};
+        k_out = k;
+        k = (uint32_t)cap;
+        d_ids = (uint32_t*)lists->p;
+        d_dists = (float*)(d_ids + (size_t)nq * cap);
+    }
+    memset(&p2, 0, sizeof(p2));
     if ((rc = v2_prepare(idx, l_search, beam, full_grid, p2, v2))) return rc;
     p2.vectors = idx->d_vectors;
     p2.row_stride = idx->row_stride;
@@ -189,6 +206,9 @@ int SearchJob::launch() {
     }
     DAB_LAUNCHED();
     DAB_CUDA(cudaGetLastError());
+    // the whole batch: a re-run pass rewrote some of the lists
+    int rc;
+    if (deleted && (rc = queue_drop_deleted(idx, stream, deleted, p2.out_ids, p2.out_dists, p2.cap, nq, k_out, filtered))) return rc;
     DAB_CUDA(cudaMemcpyAsync(h_counters, d_counters, 16, cudaMemcpyDeviceToHost, stream));
     return DAB_OK;
 }
@@ -237,6 +257,7 @@ int run_search(dab_index* idx, const void* d_queries, const uint32_t* d_query_ro
     job.stream = idx->stream;
     job.tables = &idx->s_tables;
     job.counters = &idx->s_counters;
+    job.lists = &idx->s_ids;
     job.h_counters = (uint32_t*)idx->h_counters.p;
     if ((rc = job.prepare(d_queries, d_query_rows, nq, k, l_search, beam, d_ids, d_dists, d_counts, d_cmps, d_hops, rec_ids,
                           rec_dists, rec_counts, rec_cap)))
@@ -373,6 +394,7 @@ static int prepare_search_job(dab_index* idx, SearchSlot* s, const void* d_queri
     job->stream = s->stream;
     job->tables = &s->tables;
     job->counters = &s->counters;
+    job->lists = &s->lists;
     job->h_counters = (uint32_t*)s->h_counters.p;
     job->full_grid = true;
     return job->prepare(d_queries, nullptr, nq, k, l_search, beam, d.ids, d.dists, d.counts, d.cmps, d.hops, nullptr, nullptr, nullptr, 0);

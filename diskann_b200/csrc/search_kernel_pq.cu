@@ -247,6 +247,7 @@ struct RerankParams {
     uint32_t* out_ids;
     float* out_dists;
     uint32_t* out_counts;
+    const uint32_t* deleted;  // the deletion table, or NULL: its ids are dropped with the start points
     uint32_t warp_smem, off_ids, off_d;
 };
 
@@ -274,11 +275,11 @@ __global__ void __launch_bounds__(kRerankWarps * 32) rerank_kernel(const RerankP
             for (int e = lane; e < dim; e += 32) qf[e] = to_f32(s[e]);
         }
         const uint32_t n = min(p.list_counts[q], p.list_cap);
-        uint32_t m = 0;  // candidates that are not start points, traversal order kept
+        uint32_t m = 0;  // candidates that are neither start points nor deleted, traversal order kept
         for (uint32_t b = 0; b < n; b += 32) {
             const uint32_t i = b + lane;
             const uint32_t id = i < n ? p.list_ids[(size_t)q * p.list_cap + i] : kEmptyV2;
-            const bool keep = i < n && id < p.n_points;
+            const bool keep = i < n && id < p.n_points && !(p.deleted && (__ldg(p.deleted + (id >> 5)) >> (id & 31) & 1u));
             const unsigned mk = __ballot_sync(kFull, keep);
             if (keep) cid[m + __popc(mk & ((1u << lane) - 1u))] = id;
             m += __popc(mk);
@@ -344,7 +345,8 @@ static int check_rerank(const dab_index* idx, uint32_t list_cap) {
 }
 
 static int launch_rerank(const dab_index* idx, cudaStream_t stream, const void* d_queries, uint32_t nq, uint32_t k, uint32_t list_cap,
-                         const uint32_t* d_list, const uint32_t* d_list_n, uint32_t* d_ids, float* d_dists, uint32_t* d_counts) {
+                         const uint32_t* d_list, const uint32_t* d_list_n, uint32_t* d_ids, float* d_dists, uint32_t* d_counts,
+                         const uint32_t* deleted) {
     RerankParams p;
     memset(&p, 0, sizeof(p));
     p.vectors = idx->d_vectors;
@@ -360,6 +362,7 @@ static int launch_rerank(const dab_index* idx, cudaStream_t stream, const void* 
     p.out_ids = d_ids;
     p.out_dists = d_dists;
     p.out_counts = d_counts;
+    p.deleted = deleted;
     const int grid = (int)std::min<uint64_t>(((uint64_t)nq + kRerankWarps - 1) / kRerankWarps, (uint64_t)idx->sm_count * 8);
     const int rc = visit_schema<OPS_ROW>(idx->dtype, idx->metric, [&](auto s) -> int {
         using S = decltype(s);
@@ -427,6 +430,10 @@ struct PqSearchJob : SlotJob {
     Scratch retry;
     cudaEvent_t counted = nullptr;  // recorded after the read-back of a pass's counters
     uint64_t stores_version = 0;    // idx->stores_version when the batch was planned
+    // some id is deleted: the rerank drops deleted ids; without rerank the traversal writes every non-start entry of a
+    // list (k = L + #start) to `lists` and the filter takes the first k live ones into `filtered`, the caller's buffers
+    const uint32_t* deleted = nullptr;
+    SearchOut filtered{};
 
     int prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint32_t l_search_, uint32_t beam_, const SearchOut& d, bool rerank_, int mode_);
     int stage_queries();
@@ -434,6 +441,7 @@ struct PqSearchJob : SlotJob {
     int launch() override;
     int finish() override;
     int launch_pass();
+    int launch_post();
     int reserve_tables();
     unsigned long long first_nan() const { return *(const unsigned long long*)(h_counters + 4); }
     int nan_error() const {
@@ -489,6 +497,14 @@ int PqSearchJob::prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint
     p.out_counts = d.counts;
     p.out_cmps = d.cmps;
     p.out_hops = d.hops;
+    deleted = deleted_filter(idx);
+    if (deleted && !rerank) {
+        if ((rc = lists->reserve((size_t)nq * cap * 8))) return rc;
+        filtered = d;
+        p.k = cap;
+        p.out_ids = (uint32_t*)lists->p;
+        p.out_dists = (float*)(p.out_ids + (size_t)nq * cap);
+    }
 
     size_t off = 0;
     p.off_q = 0;
@@ -597,11 +613,18 @@ int PqSearchJob::launch_pass() {
     return DAB_OK;
 }
 
-// the first pass and, optimistically, the rerank
+// the post-processing of the whole batch: the rerank, or the filter of deleted ids
+int PqSearchJob::launch_post() {
+    if (rerank) return launch_rerank(idx, stream, d_queries, nq, k, cap, p.list_ids, p.list_counts, p.out_ids, p.out_dists, p.out_counts, deleted);
+    if (deleted) return queue_drop_deleted(idx, stream, deleted, p.out_ids, p.out_dists, cap, nq, k, filtered);
+    return DAB_OK;
+}
+
+// the first pass and, optimistically, the post-processing
 int PqSearchJob::launch_traversal() {
     int rc;
     if ((rc = launch_pass())) return rc;
-    return rerank ? launch_rerank(idx, stream, d_queries, nq, k, cap, p.list_ids, p.list_counts, p.out_ids, p.out_dists, p.out_counts) : DAB_OK;
+    return launch_post();
 }
 
 int PqSearchJob::launch() {
@@ -631,9 +654,8 @@ int PqSearchJob::finish() {
         if ((rc = launch_pass())) return rc;
         DAB_CUDA(cudaEventSynchronize(counted));
     }
-    // the rerank queued by launch read lists that the re-runs have since rewritten
-    if (reran && rerank) return launch_rerank(idx, stream, d_queries, nq, k, cap, p.list_ids, p.list_counts, p.out_ids, p.out_dists, p.out_counts);
-    return DAB_OK;
+    // the rerank or filter queued by launch read lists that the re-runs have since rewritten
+    return reran ? launch_post() : DAB_OK;
 }
 
 // The synchronous calls: the job on the handle's stream and scratch.  A MinMax batch with a NaN query fails before any

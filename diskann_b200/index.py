@@ -655,6 +655,30 @@ class GpuIndex:
     def build(self, pruned_degree, l_build, alpha=1.2, batch_size=0):
         check(_lib.lib().dab_build(self._h, pruned_degree, l_build, alpha, batch_size))
 
+    # -- deletion (Delete of the providers' TableDeleteProviderAsync; DiskANNIndex::consolidate_vector)
+    def delete(self, ids):
+        """Marks data points deleted: every k-NN search then leaves them out of its results."""
+        ids = np.ascontiguousarray(ids, np.uint32).ravel()
+        check(_lib.lib().dab_delete(self._h, _ptr(ids), ids.shape[0]))
+
+    def release(self, ids):
+        """Clears the deletion mark of deleted points and empties their adjacency rows."""
+        ids = np.ascontiguousarray(ids, np.uint32).ravel()
+        check(_lib.lib().dab_release(self._h, _ptr(ids), ids.shape[0]))
+
+    def delete_status(self, ids):
+        """bool [n]: which of `ids` are deleted."""
+        ids = np.ascontiguousarray(ids, np.uint32).ravel()
+        out = np.zeros(ids.shape[0], np.uint8)
+        check(_lib.lib().dab_delete_status(self._h, _ptr(ids), ids.shape[0], _ptr(out)))
+        return out.astype(bool)
+
+    def consolidate(self, pruned_degree, alpha=1.2):
+        """consolidate_vector for every node: repairs the lists around deleted points; returns the lists rewritten."""
+        n = C.c_uint64()
+        check(_lib.lib().dab_consolidate(self._h, pruned_degree, alpha, C.byref(n)))
+        return int(n.value)
+
     def flat_knn(self, queries, k):
         queries = self._queries(queries)
         ids = np.empty((queries.shape[0], k), np.uint32)

@@ -84,6 +84,30 @@ impl<T: Element> GpuIndex<T> {
         check(unsafe { sys::dab_build(self.raw, pruned_degree, l_build, alpha, 0) })
     }
 
+    /// `Delete::delete`: every k-NN search then leaves these points out of its results.
+    pub fn delete(&mut self, ids: &[u32]) -> Result<()> {
+        check(unsafe { sys::dab_delete(self.raw, ids.as_ptr(), ids.len() as u64) })
+    }
+
+    /// `Delete::release`: clears the deletion mark and empties the adjacency rows of deleted points.
+    pub fn release(&mut self, ids: &[u32]) -> Result<()> {
+        check(unsafe { sys::dab_release(self.raw, ids.as_ptr(), ids.len() as u64) })
+    }
+
+    /// `Delete::status_by_internal_id` for each id: true when deleted.
+    pub fn delete_status(&self, ids: &[u32]) -> Result<Vec<bool>> {
+        let mut out = vec![0u8; ids.len()];
+        check(unsafe { sys::dab_delete_status(self.raw, ids.as_ptr(), ids.len() as u64, out.as_mut_ptr()) })?;
+        Ok(out.into_iter().map(|b| b != 0).collect())
+    }
+
+    /// `consolidate_vector` for every node; returns the number of lists rewritten.
+    pub fn consolidate(&mut self, pruned_degree: u32, alpha: f32) -> Result<u64> {
+        let mut rewritten = 0u64;
+        check(unsafe { sys::dab_consolidate(self.raw, pruned_degree, alpha, &mut rewritten) })?;
+        Ok(rewritten)
+    }
+
     /// `KNN::search` for every query of the batch at once (search_internal + post-processing).
     pub fn search_batch(&self, queries: &[T], k: usize, l_search: u32, beam_width: u32) -> Result<Batch> {
         assert_eq!(queries.len() % self.dim, 0);

@@ -501,6 +501,44 @@ int dab_robust_prune(dab_index* idx, const uint32_t* pool_ids, const float* pool
 int dab_build(dab_index* idx, uint32_t pruned_degree, uint32_t l_build, float alpha,
               uint32_t batch_size);
 
+/* ------------------------------------------------------------------ deletion */
+
+/* Delete::delete / release / status_by_internal_id of the providers' TableDeleteProviderAsync
+ * (diskann-providers/src/model/graph/provider/async_/table_delete_provider.rs; inmem/provider.rs:596-655): one bit per id.
+ *   dab_delete: marks ids deleted; deleting an id twice is a no-op.  An id >= n_points (a start point, which is frozen,
+ *     or an id out of range) fails the call with DAB_ERR_INVALID_ARGUMENT naming the first such id, and nothing changes.
+ *   dab_release: clears the mark and empties the node's adjacency row.  An id that is not deleted fails the call,
+ *     naming the first such id, and nothing changes (the reference would silently clear a live node's list).
+ *   dab_delete_status: out_deleted[i] = 1 when ids[i] is deleted, else 0; ids must be < n_points + n_start.
+ * Every k-NN search (dab_search_batch*, dab_search_batch_pq*, _sq*, _minmax*; host, _device and _async) then applies
+ * the reference's post-processing over the same traversal: without rerank the first k entries of the final candidate
+ * list that are neither start points nor deleted (Pipeline<FilterStartPoints, RemoveDeletedIdsAndCopy>, async_/
+ * postprocess.rs:35-61); with rerank deleted entries are dropped before they are scored.  out_counts is the number of
+ * live results, which can be below k (the rest is padded UINT32_MAX / +inf); cmps and hops are the traversal's, which
+ * still expands deleted nodes.  While nothing is deleted a search launches exactly what it launches without a table.
+ * Paged search applies no post-processing (paged.rs:122), so its pages keep deleted ids; the exhaustive scans
+ * (dab_flat_knn*) stay ground truth over every row, and dab_build ignores the table, as the reference's insert does.
+ * The table travels with dab_broadcast_index and dab_broadcast.  dab_delete, dab_release and dab_consolidate fail with
+ * DAB_ERR_INVALID_ARGUMENT, changing nothing, while any slot holds a batch in flight (join it with dab_wait first).
+ * dab_release, and dab_consolidate when it rewrites a list, make open paged sessions fail their next page; dab_delete
+ * does not. */
+int dab_delete(dab_index* idx, const uint32_t* ids, uint64_t n);
+int dab_release(dab_index* idx, const uint32_t* ids, uint64_t n);
+int dab_delete_status(dab_index* idx, const uint32_t* ids, uint64_t n, uint8_t* out_deleted);
+/* DiskANNIndex::consolidate_vector (diskann/src/graph/index.rs:1819-1931) for every id in [0, n_points + n_start), in
+ * one device pass, which equals the reference's sequential loop in any order: a deleted node is left alone; a node with
+ * no deleted neighbour (an id >= n_points + n_start counts as one, with no neighbours) and at most pruned_degree
+ * distinct live neighbours is left alone; otherwise its pool is the set of its live neighbours and of the live
+ * neighbours of its deleted ones, itself removed, and becomes the new list as it is when it has fewer than
+ * pruned_degree ids, else goes through robust_prune_list (index.rs:2397-2454: Distance<T,T> from the node, sorted, cut to
+ * 750, occlude_list without saturation; the prune kind from the metric, as dab_robust_prune).  Where the reference's
+ * HashSet leaves an order unspecified the pool's order is fixed: the node's live neighbours in list order, then each
+ * deleted neighbour's live neighbours, deleted neighbours in list order, first occurrence kept; exact distance ties
+ * keep that order.  List lengths above max_degree are read as max_degree.  With nothing deleted it still prunes the
+ * lists longer than pruned_degree.  Needs the vectors and the graph; pruned_degree in [1, max_degree]; alpha >= 1.
+ * out_rewritten (may be NULL): the number of lists written. */
+int dab_consolidate(dab_index* idx, uint32_t pruned_degree, float alpha, uint64_t* out_rewritten);
+
 /* exact k-NN by exhaustive scan (diskann/src/flat; ground truth for recall):
  * out_ids [nq][k] ascending distance, ties by lower id. */
 int dab_flat_knn(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t* out_ids,

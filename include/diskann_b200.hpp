@@ -166,6 +166,20 @@ class Provider {
         check(dab_build(h_, pruned_degree, l_build, alpha, batch));
     }
 
+    // deletion: Delete::delete / release / status_by_internal_id, and consolidate_vector for every node
+    void remove(const std::vector<uint32_t>& ids) { check(dab_delete(h_, ids.data(), ids.size())); }
+    void release(const std::vector<uint32_t>& ids) { check(dab_release(h_, ids.data(), ids.size())); }
+    std::vector<uint8_t> delete_status(const std::vector<uint32_t>& ids) {
+        std::vector<uint8_t> out(ids.size());
+        check(dab_delete_status(h_, ids.data(), ids.size(), out.data()));
+        return out;
+    }
+    uint64_t consolidate(uint32_t pruned_degree, float alpha = 1.2f) {
+        uint64_t rewritten = 0;
+        check(dab_consolidate(h_, pruned_degree, alpha, &rewritten));
+        return rewritten;
+    }
+
    private:
     dab_index* h_ = nullptr;
     uint32_t dim_;
