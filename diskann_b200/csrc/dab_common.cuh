@@ -85,11 +85,11 @@ struct Tuning {
 };
 
 // The largest visited set the searches at (l, beam, mode) have seen; later calls size their visited tables from it
-// (search_kernel.cu).  `mode`: which quantized store the traversal reads (0 for full precision and PQ, 1 for SQ, 2 for
-// MinMax).
+// (search_kernel.cu).  `mode`: which quantized store the traversal reads (full precision shares STORE_PQ: the two keep separate
+// hints, dab_index::hint and pq_hint).
 struct VisitedHint {
     uint32_t l = 0, beam = 0, visited = 0;
-    int mode = 0;
+    QuantStore mode = STORE_PQ;
 };
 
 // A store of dense N-bit code rows, one per point (the SQ and MinMax stores of an index).  Host-facing rows use the

@@ -1,8 +1,12 @@
 // search_common.cuh — device helpers shared by the warp-per-query search kernels: the exact
-// bucketed visited set and the batched rank-merge of the sorted candidate list.
+// bucketed visited set, the batched rank-merge of the sorted candidate list, and the per-query
+// steps around a kernel's hop (taking a query, loading it, picking the beam, collecting the new
+// candidates, reporting an overflow, writing the results).
 #pragma once
 
 #include "distance_device.cuh"
+
+#include <type_traits>
 
 namespace dab {
 
@@ -235,6 +239,14 @@ __device__ __forceinline__ bool bucket_insert(uint32_t* table, uint32_t n_bucket
     }
 }
 
+// HashSet::insert of one id into a global table: true when it was newly inserted
+__device__ __forceinline__ bool visit_global(uint32_t* table, uint32_t n_buckets, uint32_t id) {
+    uint32_t bs[8];
+    const uint32_t b = bucket_of(id, n_buckets);
+    load_bucket(table + (size_t)b * 8, bs);
+    return bucket_insert(table, n_buckets, b, bs, id);
+}
+
 // ---- 16-bit quotient tags (the shared-memory visited tables of search_kernel_v3, search_smem.cuh) ----
 // A table of 16-bit entries holds twice the ids per byte without giving up exactness.  Ids < 2^K are hashed with an odd
 // multiplier modulo 2^K (a bijection), h = tag * n_buckets + bucket, so (bucket, tag) identifies
@@ -294,6 +306,156 @@ __device__ __forceinline__ int tag16_probe(uint32_t* table, uint32_t n_buckets, 
         if (++d > 2) return 2;
         b = b + 1 == n_buckets ? 0 : b + 1;
     }
+}
+
+// ---- the steps of a query around its hops ---------------------------------------------------
+// Every traversal kernel runs these once per query or once per hop, outside its own hop body.  They take the few
+// pointers and values they use, so each kernel keeps its own parameter block and shape.
+
+// The warp takes the next work item of the pass from counters[0]: false when the pass is done, else `qidx` is the
+// query to run (`list`: the queries of a re-run pass, NULL: 0 .. n_work-1)
+__device__ __forceinline__ bool next_query(uint32_t* counters, uint32_t n_work, const uint32_t* list, int lane, uint32_t& qidx) {
+    uint32_t w = 0;
+    if (lane == 0) w = atomicAdd(counters, 1u);
+    w = __shfl_sync(kFull, w, 0);
+    if (w >= n_work) return false;
+    qidx = list ? list[w] : w;
+    return true;
+}
+
+// Query q of `queries` (rows of `dim` elements of the index's run-time dtype) as f32 into qf: T: Into<f32>
+__device__ __forceinline__ void widen_query(int dtype, const void* queries, uint32_t q, int dim, float* qf, int lane) {
+    for (int e = lane; e < dim; e += 32) {
+        float v;
+        switch (dtype) {
+            case DAB_F32: v = reinterpret_cast<const float*>(queries)[(size_t)q * dim + e]; break;
+            case DAB_F16: v = __half2float(reinterpret_cast<const __half*>(queries)[(size_t)q * dim + e]); break;
+            case DAB_I8: v = (float)reinterpret_cast<const int8_t*>(queries)[(size_t)q * dim + e]; break;
+            default: v = (float)reinterpret_cast<const uint8_t*>(queries)[(size_t)q * dim + e]; break;
+        }
+        qf[e] = v;
+    }
+}
+
+// The query row `s` into the warp's shared memory for the distance loops of a compile-time row type: i8 / u8 as the
+// bytes they are, zero padded to a multiple of `pad` (what the caller's loops read in whole: 4 or 16); floats as f32
+// (f16 queries are widened, layers/full.rs:421-423)
+template <typename TD>
+__device__ __forceinline__ void load_query(const TD* s, int dim, int pad, float* qf, int lane) {
+    if constexpr (std::is_same<TD, int8_t>::value || std::is_same<TD, uint8_t>::value) {
+        uint8_t* qb = reinterpret_cast<uint8_t*>(qf);
+        const int qbytes = (dim + pad - 1) & ~(pad - 1);
+        for (int e = lane; e < qbytes; e += 32) qb[e] = e < dim ? reinterpret_cast<const uint8_t*>(s)[e] : 0;
+    } else {
+        for (int e = lane; e < dim; e += 32) qf[e] = to_f32(s[e]);
+    }
+}
+
+// MODE 1 (SQ) / MODE 2 (MinMax): a query as staged before the launch — its `words` code words at `codes` into qc, then
+// for MinMax its {b, n, a, norm_squared} (`meta`) behind the words; the SQ compensation (meta->x) stays in a register
+// (q_comp, every lane).  The caller passes the query's own row and float4: handing over the arrays and the query's
+// index instead costs search_kernel_pq<16, 1> seven registers.
+template <int MODE>
+__device__ __forceinline__ void load_query_codes(const uint8_t* codes, const float4* meta, uint32_t words, uint32_t* qc, float& q_comp, int lane) {
+    const uint32_t* src = reinterpret_cast<const uint32_t*>(codes);
+    for (uint32_t wd = lane; wd < words; wd += 32) qc[wd] = __ldg(src + wd);
+    if (MODE == 1) q_comp = __shfl_sync(kFull, lane == 0 ? __ldg(&meta->x) : 0.0f, 0);
+    if (MODE == 2 && lane == 0) *reinterpret_cast<float4*>(qc + words) = __ldg(meta);
+}
+
+// closest_notvisited x beam_width (queue.rs:297-313): the first `beam` unvisited entries of qi[cursor_lo, lim) are
+// flagged visited and their ids written to beam_ids; returns how many.  Lane 0 calls on_pick(b, idx, id) for the b-th
+// of them, list entry idx (the build's record of expanded nodes; the searches leave it empty).
+struct NoPick {
+    __device__ __forceinline__ void operator()(uint32_t, uint32_t, uint32_t) const {}
+};
+template <class OnPick = NoPick>
+__device__ __forceinline__ uint32_t pick_beam(uint32_t* qi, uint32_t lim, uint32_t beam, uint32_t& cursor_lo, uint32_t* beam_ids, int lane,
+                                              OnPick on_pick = OnPick{}) {
+    uint32_t nb = 0;
+    while (nb < beam) {
+        const uint32_t idx = first_unvisited(qi, cursor_lo, lim, lane);
+        if (idx >= lim) break;
+        const uint32_t id = qi[idx];
+        __syncwarp();
+        if (lane == 0) {
+            qi[idx] = id | kFlagV2;
+            beam_ids[nb] = id;
+            on_pick(nb, idx, id);
+        }
+        cursor_lo = idx + 1;
+        ++nb;
+        __syncwarp();
+    }
+    return nb;
+}
+
+// One neighbour per lane after its visited-set insert: those that are new and in bounds (`isnew`) are appended to
+// cid[ncand..) in lane order, i.e. adjacency order
+__device__ __forceinline__ void push_new(bool isnew, uint32_t word, uint32_t* cid, uint32_t& ncand, int lane) {
+    const unsigned mn = __ballot_sync(kFull, isnew);
+    if (isnew) cid[ncand + __popc(mn & ((1u << lane) - 1u))] = word;
+    ncand += __popc(mn);
+}
+// ... and every id that entered the set (`inserted`, in bounds or not) is counted in nvisited
+__device__ __forceinline__ void push_new(bool inserted, bool isnew, uint32_t word, uint32_t* cid, uint32_t& ncand, uint32_t& nvisited, int lane) {
+    const unsigned mi = __ballot_sync(kFull, inserted);
+    push_new(isnew, word, cid, ncand, lane);
+    nvisited += __popc(mi);
+}
+
+// A query whose visited set outgrew its table: counted in counters[1] and listed for the next pass
+__device__ __forceinline__ void report_overflow(uint32_t* counters, uint32_t* overflow_list, uint32_t qidx, int lane) {
+    if (lane == 0) overflow_list[atomicAdd(counters + 1, 1u)] = qidx;
+}
+
+// out_ids / out_dists [q][count, k) <- UINT32_MAX / +inf
+__device__ __forceinline__ void pad_results(uint32_t* out_ids, float* out_dists, uint32_t q, uint32_t k, uint32_t count, int lane) {
+    for (uint32_t i = count + lane; i < k; i += 32) {
+        out_ids[(size_t)q * k + i] = kEmptyV2;
+        out_dists[(size_t)q * k + i] = __int_as_float(0x7F800000);
+    }
+}
+
+// Post-processing (provider.rs:907-950): of the list's first n entries, those that are not start points (id < n_points),
+// the first k, in list order, padded; returns how many were written
+__device__ __forceinline__ uint32_t write_results(const uint32_t* qi, const float* qd, uint32_t n, uint64_t n_points, uint32_t k,
+                                                  uint32_t* out_ids, float* out_dists, uint32_t q, int lane) {
+    uint32_t count = 0;
+    for (uint32_t b = 0; b < n && count < k; b += 32) {
+        const uint32_t i = b + lane;
+        const uint32_t id = i < n ? (qi[i] & ~kFlagV2) : kEmptyV2;
+        const bool keep = i < n && id < n_points;
+        const unsigned m = __ballot_sync(kFull, keep);
+        const uint32_t pos = count + __popc(m & ((1u << lane) - 1u));
+        if (keep && pos < k) {
+            out_ids[(size_t)q * k + pos] = id;
+            out_dists[(size_t)q * k + pos] = qd[i];
+        }
+        count += __popc(m);
+    }
+    count = min(count, k);
+    pad_results(out_ids, out_dists, q, k, count, lane);
+    return count;
+}
+
+// What a completed query reports: its visited-set size into the pass's maximum (counters[2], which sizes later tables),
+// and the optional per-query counts
+__device__ __forceinline__ void write_stats(uint32_t* counters, uint32_t nvisited, uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops,
+                                            uint32_t q, uint32_t count, uint32_t cmps, uint32_t hops, int lane) {
+    if (lane == 0) {
+        atomicMax(counters + 2, nvisited);
+        if (out_counts) out_counts[q] = count;
+        if (out_cmps) out_cmps[q] = cmps;
+        if (out_hops) out_hops[q] = hops;
+    }
+}
+
+// The whole list (best.iter(), start points included) for the rerank stage
+__device__ __forceinline__ void write_list(const uint32_t* qi, uint32_t n, uint32_t* list_ids, uint32_t* list_counts, uint32_t list_cap,
+                                           uint32_t q, int lane) {
+    for (uint32_t i = lane; i < n; i += 32) list_ids[(size_t)q * list_cap + i] = qi[i] & ~kFlagV2;
+    if (lane == 0) list_counts[q] = n;
 }
 
 }  // namespace dab

@@ -5,6 +5,7 @@
 #include "dab_common.cuh"
 
 #include <functional>
+#include <type_traits>
 
 namespace dab {
 
@@ -14,13 +15,64 @@ int check_search_args(const dab_index* idx, uint32_t k, uint32_t l_search, uint3
 
 // Ids a warp's visited table holds in the first global-table pass at (L, beam, mode): the reference's estimate, or less
 // where `hint` has seen the visited sets of this (or a larger) L and beam.  A default VisitedHint is no hint.
-uint64_t table_slots(const dab_index* idx, const VisitedHint& hint, uint32_t l_search, uint32_t beam, int mode);
+uint64_t table_slots(const dab_index* idx, const VisitedHint& hint, uint32_t l_search, uint32_t beam, QuantStore mode);
 // `hint` takes in the largest visited set of a pass at (L, beam, mode)
-void learn_visited(VisitedHint& hint, uint32_t l_search, uint32_t beam, int mode, uint32_t visited);
+void learn_visited(VisitedHint& hint, uint32_t l_search, uint32_t beam, QuantStore mode, uint32_t visited);
 // After a global-table pass `pass` that overflowed: the table of the next one, or DAB_ERR_VISITED_OVERFLOW after six
 int grow_visited_tables(const dab_index* idx, int& pass, uint64_t& slots);
 // The `n_over` query ids a pass reported at `d_overflow` become the work list of the next pass, in `retry`
 int take_overflow_list(cudaStream_t stream, const uint32_t* d_overflow, uint32_t n_over, Scratch& retry);
+
+// The grid of a pass of persistent one-query warps over n_work queries, where resident_ctas CTAs of warps_per_cta warps
+// fit the device: every resident warp runs the same number of queries (10K queries on 3108 resident warps would
+// otherwise pay for 4 full rounds with the last one 22 % full)
+inline int balanced_grid(uint64_t n_work, int resident_ctas, int warps_per_cta) {
+    const uint64_t max_warps = (uint64_t)resident_ctas * warps_per_cta;
+    const uint64_t rounds = (n_work + max_warps - 1) / max_warps;
+    const uint64_t need = (n_work + rounds - 1) / rounds;
+    return (int)((need + warps_per_cta - 1) / warps_per_cta);
+}
+
+// f(std::integral_constant<int, QT>) for the merge tile QT (merge_any, search_common.cuh) of a list of `cap` entries
+template <class F>
+auto visit_list_tile(uint32_t cap, F&& f) {
+    if (cap <= 128) return f(std::integral_constant<int, 4>{});
+    if (cap <= 256) return f(std::integral_constant<int, 8>{});
+    if (cap <= 512) return f(std::integral_constant<int, 16>{});
+    return f(std::integral_constant<int, 32>{});
+}
+
+// A quantized traversal's store is ready: the PQ table and codes, or the SQ / MinMax rows (and the SQ store's metric,
+// SQStore::distance_computer, providers inmem/scalar.rs:214-226).  `who` names the entry point in the message.
+// `upload_first`: a store that was never set up is reported as "<upload call> has not been called" (the paged calls)
+// instead of as missing codes or rows (the batch calls).
+int check_quant_store(const dab_index* idx, QuantStore store, const char* who, bool upload_first);
+
+// The fields a quantized traversal's parameter block (SearchParamsPq, PagedParams) takes from the store it reads
+template <class P>
+void set_store_params(const dab_index* idx, QuantStore store, P& p) {
+    if (store == STORE_PQ) {
+        p.pivots = idx->d_pivots;
+        p.offsets = idx->d_offsets;
+        p.codes = idx->d_codes;
+        p.n_chunks = idx->pq_chunks;
+        p.n_centers = idx->pq_centers;
+        p.ip_table = idx->metric == DAB_INNER_PRODUCT ? 1 : 0;  // L2 and CosineNormalized use TableL2 (dynamic.rs:80-85)
+        p.direct_cosine = idx->metric == DAB_COSINE ? 1 : 0;
+        return;
+    }
+    const CodeStore& cs = store == STORE_SQ ? idx->sq : idx->mm;
+    p.row_codes = cs.d_codes;
+    p.row_meta = cs.d_meta;
+    p.code_stride = cs.stride;
+    p.code_dim = cs.dim;
+    p.code_nbits = cs.nbits;
+    p.code_metric = idx->metric;  // MinMaxElement::query_distance: all four metrics (minmax_repr.rs)
+    if (store == STORE_SQ) {
+        p.sq_scale_squared = idx->sq_scale * idx->sq_scale;  // AsFunctor (scalar/quantizer.rs:316-335)
+        p.sq_shift_square_norm = idx->sq_shift_square_norm;
+    }
+}
 
 // Where a batch's results go: ids and dists [nq][k]; counts, cmps and hops [nq], optional
 struct SearchOut {

@@ -27,7 +27,7 @@ int check_search_args(const dab_index* idx, uint32_t k, uint32_t l_search, uint3
 // ---- visited tables in global memory (search_kernel_v2, search_kernel_pq, search_kernel_pqs) -----------------------
 // Every warp owns a table of `slots` ids in 32-byte buckets of 8.  A query whose visited set passes 7/8 of its table
 // stops and is listed in the pass's overflow list; it is re-run on a larger table, so membership is exact at any size.
-uint64_t table_slots(const dab_index* idx, const VisitedHint& hint, uint32_t l_search, uint32_t beam, int mode) {
+uint64_t table_slots(const dab_index* idx, const VisitedHint& hint, uint32_t l_search, uint32_t beam, QuantStore mode) {
     if (idx->tune.test_visited_log2) return 1ull << idx->tune.test_visited_log2;  // tests force the overflow re-runs
     // the reference's estimate (scratch.rs:186-192: 1.1 * max_degree * 1.3 * L), never more than the index
     double est = 1.1 * idx->max_degree * 1.3 * (double)l_search;
@@ -41,9 +41,29 @@ uint64_t table_slots(const dab_index* idx, const VisitedHint& hint, uint32_t l_s
     return std::max<uint64_t>(256, (uint64_t)est + 1);
 }
 
-void learn_visited(VisitedHint& hint, uint32_t l_search, uint32_t beam, int mode, uint32_t visited) {
+void learn_visited(VisitedHint& hint, uint32_t l_search, uint32_t beam, QuantStore mode, uint32_t visited) {
     if (l_search != hint.l || beam != hint.beam || mode != hint.mode) hint = VisitedHint{l_search, beam, 0, mode};
     hint.visited = std::max(hint.visited, visited);
+}
+
+int check_quant_store(const dab_index* idx, QuantStore store, const char* who, bool upload_first) {
+    if (store == STORE_PQ) {
+        if (upload_first && !idx->d_pivots) return fail(DAB_ERR_NOT_READY, "%s: dab_upload_pq has not been called", who);
+        if (!idx->d_pivots || !idx->d_codes || !idx->pq_codes_ready)
+            return fail(DAB_ERR_NOT_READY, "%s: no PQ codes (dab_upload_pq with codes, or dab_pq_encode_all)", who);
+        return DAB_OK;
+    }
+    const bool sq = store == STORE_SQ;
+    const CodeStore& cs = sq ? idx->sq : idx->mm;
+    int rc;
+    if (upload_first && (rc = store_require(idx, sq ? &dab_index::sq : &dab_index::mm, sq ? "dab_upload_sq" : "dab_upload_minmax", who))) return rc;
+    if (!cs.d_codes || !cs.ready)
+        return fail(DAB_ERR_NOT_READY, sq ? "%s: no scalar-quantized rows (dab_upload_sq with rows, or dab_sq_encode_all)"
+                                          : "%s: no MinMax rows (dab_upload_minmax with rows, or dab_minmax_encode_all)", who);
+    // SQStore::distance_computer (providers inmem/scalar.rs:214-226): UnsupportedDistanceMetric
+    if (sq && idx->metric == DAB_COSINE)
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: the scalar-quantized store supports L2, InnerProduct and CosineNormalized", who);
+    return DAB_OK;
 }
 
 int grow_visited_tables(const dab_index* idx, int& pass, uint64_t& slots) {
@@ -147,7 +167,7 @@ int SearchJob::prepare(const void* d_queries, const uint32_t* d_query_rows, uint
     p2.rec_counts = rec_counts;
     p2.rec_cap = rec_cap;
 
-    slots = table_slots(idx, idx->hint, l_search, beam, 0);
+    slots = table_slots(idx, idx->hint, l_search, beam, STORE_PQ);
     if ((rc = counters->reserve(16 + (size_t)nq * 4))) return rc;
     d_counters = (uint32_t*)counters->p;
     d_overflow = d_counters + 4;
@@ -181,12 +201,7 @@ int SearchJob::prepare(const void* d_queries, const uint32_t* d_query_rows, uint
 int SearchJob::launch() {
     DAB_CUDA(cudaMemsetAsync(d_counters, 0, 16, stream));
     if (stage == 0) {
-        // persistent workers: size the grid so every resident worker runs the same number of queries
-        const uint64_t max_workers = (uint64_t)v3.grid * kV3Warps;
-        const uint64_t rounds = (nq + max_workers - 1) / max_workers;
-        const uint64_t need_warps = (nq + rounds - 1) / rounds;
-        const int launch_grid = (int)((need_warps + kV3Warps - 1) / kV3Warps);
-        v3.kern<<<launch_grid, kV3Warps * 32, v3.smem_block, stream>>>(p3);
+        v3.kern<<<balanced_grid(nq, v3.grid, kV3Warps), kV3Warps * 32, v3.smem_block, stream>>>(p3);
     } else {
         // a visited table per warp: `slots` rounded up to whole 32-byte buckets of 8 ids
         const uint32_t n_buckets = (uint32_t)((slots + 7) / 8);
@@ -194,13 +209,7 @@ int SearchJob::launch() {
         if ((rc = tables->reserve((size_t)v2.grid * kV2Warps * n_buckets * 32))) return rc;
         p2.tables = (uint32_t*)tables->p;
         p2.n_buckets = n_buckets;
-        // one warp per query, persistent: size the grid so every resident warp runs the same
-        // number of queries (10K queries on 3108 slots would otherwise pay for 4 full rounds
-        // with the last one 22 % full)
-        const uint64_t max_warps = (uint64_t)v2.grid * kV2Warps;
-        const uint64_t rounds = (p2.n_work + max_warps - 1) / max_warps;
-        const uint64_t need = (p2.n_work + rounds - 1) / rounds;
-        int launch_grid = (int)((need + kV2Warps - 1) / kV2Warps);
+        int launch_grid = balanced_grid(p2.n_work, v2.grid, kV2Warps);
         if (full_grid) launch_grid = (int)std::min<uint64_t>((uint64_t)v2.grid, ((uint64_t)p2.n_work + kV2Warps - 1) / kV2Warps);
         v2.kern<<<launch_grid, kV2Warps * 32, v2.smem_block, stream>>>(p2);
     }
@@ -219,7 +228,7 @@ int SearchJob::finish() {
         idx->rec_truncated += h_counters[3];
         const uint32_t n_over = h_counters[1];
         if (!recording) {  // build-time searches run on a growing graph: do not learn from them
-            learn_visited(idx->hint, l_search, beam, 0, h_counters[2]);
+            learn_visited(idx->hint, l_search, beam, STORE_PQ, h_counters[2]);
             if (stage == 0) {
                 idx->v3_overflow_l = l_search;
                 idx->v3_overflow_beam = beam;
@@ -236,7 +245,7 @@ int SearchJob::finish() {
         if (stage == 0) {
             // the overflowed queries are the largest: size the global tables from the estimate again
             stage = 1;
-            slots = std::max(slots, table_slots(idx, VisitedHint{}, l_search, beam, 0));
+            slots = std::max(slots, table_slots(idx, VisitedHint{}, l_search, beam, STORE_PQ));
         } else if ((rc = grow_visited_tables(idx, pass, slots))) {
             return rc;
         }

@@ -78,35 +78,14 @@ __global__ void __launch_bounds__(kPqWarps * 32) search_kernel_pq(const SearchPa
         __syncwarp();
     };
 
-    for (;;) {
-        uint32_t w = 0;
-        if (lane == 0) w = atomicAdd(p.counters, 1u);
-        w = __shfl_sync(kFull, w, 0);
-        if (w >= p.n_work) break;
-        const uint32_t qidx = p.query_list ? p.query_list[w] : w;
-
+    for (uint32_t qidx; next_query(p.counters, p.n_work, p.query_list, lane, qidx);) {
         // ---- query -> f32 (T: Into<f32>), table build, visited clear
         __syncwarp();
-        for (int e = lane; MODE == 0 && e < dim; e += 32) {
-            float v;
-            switch (p.dtype) {
-                case DAB_F32: v = reinterpret_cast<const float*>(p.queries)[(size_t)qidx * dim + e]; break;
-                case DAB_F16: v = __half2float(reinterpret_cast<const __half*>(p.queries)[(size_t)qidx * dim + e]); break;
-                case DAB_I8: v = (float)reinterpret_cast<const int8_t*>(p.queries)[(size_t)qidx * dim + e]; break;
-                default: v = (float)reinterpret_cast<const uint8_t*>(p.queries)[(size_t)qidx * dim + e]; break;
-            }
-            qf[e] = v;
-        }
+        if (MODE == 0) widen_query(p.dtype, p.queries, qidx, dim, qf, lane);
         for (uint32_t i = lane; i < nbk; i += 32) store_empty_bucket(table + (size_t)i * 8);
         __syncwarp();
         if (MODE != 0) {
-            // the query staged before the launch: its code words, then for MinMax its {b, n, a, norm_squared}; the SQ
-            // compensation stays in a register
-            const uint32_t words = p.code_stride >> 2;
-            const uint32_t* src = reinterpret_cast<const uint32_t*>(p.query_codes + (size_t)qidx * p.code_stride);
-            for (uint32_t wd = lane; wd < words; wd += 32) qc[wd] = __ldg(src + wd);
-            if (MODE == 1) q_comp = __shfl_sync(kFull, lane == 0 ? __ldg(&p.query_meta[qidx].x) : 0.0f, 0);
-            if (MODE == 2 && lane == 0) *reinterpret_cast<float4*>(qc + words) = __ldg(p.query_meta + qidx);
+            load_query_codes<MODE>(p.query_codes + (size_t)qidx * p.code_stride, p.query_meta + qidx, p.code_stride >> 2, qc, q_comp, lane);
             __syncwarp();
         }
         for (uint32_t t = lane; MODE == 0 && !p.direct_cosine && t < entries; t += 32) __stcg(lut + t, pq_table_entry(p, qf, dim, t));
@@ -121,10 +100,7 @@ __global__ void __launch_bounds__(kPqWarps * 32) search_kernel_pq(const SearchPa
             if ((uint32_t)lane < n) {
                 const uint32_t id = (uint32_t)p.n_points + s0 + lane;
                 cid[lane] = id;
-                const uint32_t b = bucket_of(id, nbk);
-                uint32_t bs[8];
-                load_bucket(table + (size_t)b * 8, bs);
-                bucket_insert(table, nbk, b, bs, id);
+                visit_global(table, nbk, id);
             }
             __syncwarp();
             adc(n);
@@ -136,20 +112,7 @@ __global__ void __launch_bounds__(kPqWarps * 32) search_kernel_pq(const SearchPa
         // ---- greedy loop
         for (;;) {
             const uint32_t lim = min(p.cap, size);
-            uint32_t nb = 0;
-            while (nb < p.beam) {
-                const uint32_t idx = first_unvisited(qi, cursor_lo, lim, lane);
-                if (idx >= lim) break;
-                const uint32_t id = qi[idx];
-                __syncwarp();
-                if (lane == 0) {
-                    qi[idx] = id | kFlagV2;
-                    beam_ids[nb] = id;
-                }
-                cursor_lo = idx + 1;
-                ++nb;
-                __syncwarp();
-            }
+            const uint32_t nb = pick_beam(qi, lim, p.beam, cursor_lo, beam_ids, lane);
             if (nb == 0) break;
             uint32_t ncand = 0;
             for (uint32_t b = 0; b < nb; ++b) {
@@ -159,19 +122,8 @@ __global__ void __launch_bounds__(kPqWarps * 32) search_kernel_pq(const SearchPa
                 for (uint32_t c0 = 0; c0 < deg + 1; c0 += 32) {
                     const uint32_t j = c0 + lane;
                     const uint32_t word = j < p.adj_stride ? __ldg(row + j) : kEmptyV2;
-                    bool inserted = false;
-                    if (j >= 1 && j <= deg) {
-                        const uint32_t b2 = bucket_of(word, nbk);
-                        uint32_t bs[8];
-                        load_bucket(table + (size_t)b2 * 8, bs);
-                        inserted = bucket_insert(table, nbk, b2, bs, word);
-                    }
-                    const bool isnew = inserted && word < n_total;
-                    const unsigned mi = __ballot_sync(kFull, inserted);
-                    const unsigned mn = __ballot_sync(kFull, isnew);
-                    if (isnew) cid[ncand + __popc(mn & ((1u << lane) - 1u))] = word;
-                    ncand += __popc(mn);
-                    nvisited += __popc(mi);
+                    const bool inserted = j >= 1 && j <= deg && visit_global(table, nbk, word);
+                    push_new(inserted, inserted && word < n_total, word, cid, ncand, nvisited, lane);
                 }
                 if (nvisited + p.max_degree > hlimit) {
                     overflow = true;
@@ -188,43 +140,13 @@ __global__ void __launch_bounds__(kPqWarps * 32) search_kernel_pq(const SearchPa
         }
 
         if (overflow) {
-            if (lane == 0) {
-                const uint32_t o = atomicAdd(p.counters + 1, 1u);
-                p.overflow_list[o] = qidx;
-            }
+            report_overflow(p.counters, p.overflow_list, qidx, lane);
             continue;
         }
-        {
-            const uint32_t n = min(p.cap, size);
-            if (p.list_ids) {
-                for (uint32_t i = lane; i < n; i += 32) p.list_ids[(size_t)qidx * p.list_cap + i] = qi[i] & ~kFlagV2;
-                if (lane == 0) p.list_counts[qidx] = n;
-            }
-            uint32_t count = 0;
-            for (uint32_t b = 0; b < n && count < p.k; b += 32) {
-                const uint32_t i = b + lane;
-                const uint32_t id = i < n ? (qi[i] & ~kFlagV2) : kEmptyV2;
-                const bool keep = i < n && id < p.n_points;
-                const unsigned m = __ballot_sync(kFull, keep);
-                const uint32_t pos = count + __popc(m & ((1u << lane) - 1u));
-                if (keep && pos < p.k) {
-                    p.out_ids[(size_t)qidx * p.k + pos] = id;
-                    p.out_dists[(size_t)qidx * p.k + pos] = qd[i];
-                }
-                count += __popc(m);
-            }
-            count = min(count, p.k);
-            for (uint32_t i = count + lane; i < p.k; i += 32) {
-                p.out_ids[(size_t)qidx * p.k + i] = kEmptyV2;
-                p.out_dists[(size_t)qidx * p.k + i] = __int_as_float(0x7F800000);
-            }
-            if (lane == 0) {
-                atomicMax(p.counters + 2, nvisited);
-                if (p.out_counts) p.out_counts[qidx] = count;
-                if (p.out_cmps) p.out_cmps[qidx] = cmps;
-                if (p.out_hops) p.out_hops[qidx] = hops;
-            }
-        }
+        const uint32_t n = min(p.cap, size);
+        if (p.list_ids) write_list(qi, n, p.list_ids, p.list_counts, p.list_cap, qidx, lane);
+        const uint32_t count = write_results(qi, qd, n, p.n_points, p.k, p.out_ids, p.out_dists, qidx, lane);
+        write_stats(p.counters, nvisited, p.out_counts, p.out_cmps, p.out_hops, qidx, count, cmps, hops, lane);
     }
 }
 
@@ -266,14 +188,7 @@ __global__ void __launch_bounds__(kRerankWarps * 32) rerank_kernel(const RerankP
     const int dim = (int)p.dim;
     for (uint32_t q = blockIdx.x * kRerankWarps + wib; q < p.nq; q += gridDim.x * kRerankWarps) {
         __syncwarp();
-        const TD* s = reinterpret_cast<const TD*>(p.queries) + (size_t)q * dim;
-        if constexpr (kInt) {
-            uint8_t* qb = reinterpret_cast<uint8_t*>(qf);
-            const int qbytes = (dim + 15) & ~15;
-            for (int e = lane; e < qbytes; e += 32) qb[e] = e < dim ? reinterpret_cast<const uint8_t*>(s)[e] : 0;
-        } else {
-            for (int e = lane; e < dim; e += 32) qf[e] = to_f32(s[e]);
-        }
+        load_query(reinterpret_cast<const TD*>(p.queries) + (size_t)q * dim, dim, 16, qf, lane);
         const uint32_t n = min(p.list_counts[q], p.list_cap);
         uint32_t m = 0;  // candidates that are neither start points nor deleted, traversal order kept
         for (uint32_t b = 0; b < n; b += 32) {
@@ -321,10 +236,7 @@ __global__ void __launch_bounds__(kRerankWarps * 32) rerank_kernel(const RerankP
             }
         }
         const uint32_t count = min(m, p.k);
-        for (uint32_t i = count + lane; i < p.k; i += 32) {
-            p.out_ids[(size_t)q * p.k + i] = kEmptyV2;
-            p.out_dists[(size_t)q * p.k + i] = __int_as_float(0x7F800000);
-        }
+        pad_results(p.out_ids, p.out_dists, q, p.k, count, lane);
         if (lane == 0 && p.out_counts) p.out_counts[q] = count;
     }
 }
@@ -384,20 +296,13 @@ static int launch_rerank(const dab_index* idx, cudaStream_t stream, const void* 
 }
 
 // The checks of a quantized search that need no plan: arguments, the store, the metric, the list length
-static int check_pq_args(const dab_index* idx, uint32_t k, uint32_t l_search, uint32_t beam, int mode) {
+static int check_pq_args(const dab_index* idx, uint32_t k, uint32_t l_search, uint32_t beam, QuantStore mode) {
     int rc;
-    if ((rc = check_search_args(idx, k, l_search, beam, false))) return rc;
-    if (mode == 0 && (!idx->d_pivots || !idx->d_codes || !idx->pq_codes_ready))
-        return fail(DAB_ERR_NOT_READY, "dab_search_batch_pq: no PQ codes (dab_upload_pq with codes, or dab_pq_encode_all)");
-    const CodeStore& store = mode == 2 ? idx->mm : idx->sq;  // modes 1 and 2
-    if (mode != 0 && (!store.d_codes || !store.ready))
-        return fail(DAB_ERR_NOT_READY, mode == 1 ? "dab_search_batch_sq: no scalar-quantized rows (dab_upload_sq with rows, or dab_sq_encode_all)"
-                                                 : "dab_search_batch_minmax: no MinMax rows (dab_upload_minmax with rows, or dab_minmax_encode_all)");
-    // SQStore::distance_computer (providers inmem/scalar.rs:214-226): UnsupportedDistanceMetric
-    if (mode == 1 && idx->metric == DAB_COSINE)
-        return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_sq: the scalar-quantized store supports L2, InnerProduct and CosineNormalized");
+    // every entry point of a store reports under its synchronous host-buffer call's name
+    const char* who = mode == STORE_PQ ? "dab_search_batch_pq" : mode == STORE_SQ ? "dab_search_batch_sq" : "dab_search_batch_minmax";
+    if ((rc = check_search_args(idx, k, l_search, beam, false)) || (rc = check_quant_store(idx, mode, who, false))) return rc;
     if (l_search + idx->n_start > 1024)
-        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: L + #start must be <= 1024", mode == 2 ? "dab_search_batch_minmax" : "dab_search_batch_pq");
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: L + #start must be <= 1024", mode == STORE_MINMAX ? "dab_search_batch_minmax" : "dab_search_batch_pq");
     return DAB_OK;
 }
 
@@ -415,7 +320,7 @@ struct PqSearchJob : SlotJob {
     Scratch *tables = nullptr, *counters = nullptr, *stage = nullptr, *luts = nullptr, *lists = nullptr;
     uint32_t* h_counters = nullptr;  // pinned: the four counters of a pass, then (u64 at word 4) the MinMax NaN flag
 
-    int mode = 0;
+    QuantStore mode = STORE_PQ;
     bool rerank = false;
     const void* d_queries = nullptr;
     uint32_t nq = 0, k = 0, l_search = 0, beam = 0, cap = 0;
@@ -435,7 +340,7 @@ struct PqSearchJob : SlotJob {
     const uint32_t* deleted = nullptr;
     SearchOut filtered{};
 
-    int prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint32_t l_search_, uint32_t beam_, const SearchOut& d, bool rerank_, int mode_);
+    int prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint32_t l_search_, uint32_t beam_, const SearchOut& d, bool rerank_, QuantStore mode_);
     int stage_queries();
     int launch_traversal();
     int launch() override;
@@ -454,11 +359,10 @@ struct PqSearchJob : SlotJob {
 };
 
 int PqSearchJob::prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint32_t l_search_, uint32_t beam_, const SearchOut& d,
-                         bool rerank_, int mode_) {
+                         bool rerank_, QuantStore mode_) {
     d_queries = d_queries_, nq = nq_, k = k_, l_search = l_search_, beam = beam_, rerank = rerank_, mode = mode_;
     stores_version = idx->stores_version;
     int rc;
-    const CodeStore& store = mode == 2 ? idx->mm : idx->sq;  // modes 1 and 2
     cap = l_search + idx->n_start;
     memset(&p, 0, sizeof(p));
     p.adj = idx->d_adj;
@@ -472,26 +376,7 @@ int PqSearchJob::prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint
     p.k = k;
     p.cap = cap;
     p.beam = beam;
-    p.pivots = idx->d_pivots;
-    p.offsets = idx->d_offsets;
-    p.codes = idx->d_codes;
-    p.n_chunks = idx->pq_chunks;
-    p.n_centers = idx->pq_centers;
-    p.ip_table = idx->metric == DAB_INNER_PRODUCT ? 1 : 0;  // L2 and CosineNormalized use TableL2 (dynamic.rs:80-85)
-    p.direct_cosine = mode == 0 && idx->metric == DAB_COSINE ? 1 : 0;
-    if (mode != 0) {
-        p.row_codes = store.d_codes;
-        p.row_meta = store.d_meta;
-        p.code_stride = store.stride;
-        p.code_dim = store.dim;
-        p.code_nbits = store.nbits;
-        p.code_metric = idx->metric;  // MinMaxElement::query_distance: all four metrics (minmax_repr.rs)
-        p.n_chunks = 0;
-    }
-    if (mode == 1) {
-        p.sq_scale_squared = idx->sq_scale * idx->sq_scale;  // AsFunctor (scalar/quantizer.rs:316-335)
-        p.sq_shift_square_norm = idx->sq_shift_square_norm;
-    }
+    set_store_params(idx, mode, p);
     p.out_ids = d.ids;
     p.out_dists = d.dists;
     p.out_counts = d.counts;
@@ -522,16 +407,16 @@ int PqSearchJob::prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint
     p.off_beam = (uint32_t)off;
     off += round_up((size_t)beam * 4, 16);
     p.off_qc = (uint32_t)off;
-    if (mode == 1) off += p.code_stride;
-    if (mode == 2) off += p.code_stride + 16;  // the query's code row and its four compensations
+    if (mode == STORE_SQ) off += p.code_stride;
+    if (mode == STORE_MINMAX) off += p.code_stride + 16;  // the query's code row and its four compensations
     off = round_up(off, 16);
     p.off_nrow = (uint32_t)off;  // search_kernel_pqs: the adjacency row copied one hop ahead
-    if (mode == 0) off += 96 * 4;
+    if (mode == STORE_PQ) off += 96 * 4;
     p.warp_smem = (uint32_t)round_up(off, 16);
     // table metrics with a pivot table that fits shared memory: search_kernel_pqs (pivots resident per SM, entries
     // computed on the fly); everything else — SQ, DirectCosine, wide pivots, > 32 chunks — the per-warp kernel below
     memset(&plan, 0, sizeof(plan));
-    use_pqs = mode == 0 && !p.direct_cosine && pqs_plan(idx, p.warp_smem, nq, &plan);
+    use_pqs = mode == STORE_PQ && !p.direct_cosine && pqs_plan(idx, p.warp_smem, nq, &plan);
     smem_block = (size_t)p.warp_smem * kPqWarps;
     uint32_t warps;
     if (use_pqs) {
@@ -541,9 +426,10 @@ int PqSearchJob::prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint
         warps = (uint32_t)plan.grid * (uint32_t)plan.warps;
     } else {
         if (smem_block > 200 * 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_pq: configuration needs %zu B shared memory per CTA", smem_block);
-        if (mode == 2) kern = cap <= 128 ? search_kernel_pq<4, 2> : cap <= 256 ? search_kernel_pq<8, 2> : cap <= 512 ? search_kernel_pq<16, 2> : search_kernel_pq<32, 2>;
-        else if (mode == 1) kern = cap <= 128 ? search_kernel_pq<4, 1> : cap <= 256 ? search_kernel_pq<8, 1> : cap <= 512 ? search_kernel_pq<16, 1> : search_kernel_pq<32, 1>;
-        else kern = cap <= 128 ? search_kernel_pq<4, 0> : cap <= 256 ? search_kernel_pq<8, 0> : cap <= 512 ? search_kernel_pq<16, 0> : search_kernel_pq<32, 0>;
+        kern = visit_list_tile(cap, [&](auto qt) {
+            constexpr int QT = decltype(qt)::value;
+            return mode == STORE_MINMAX ? search_kernel_pq<QT, STORE_MINMAX> : mode == STORE_SQ ? search_kernel_pq<QT, STORE_SQ> : search_kernel_pq<QT, STORE_PQ>;
+        });
         DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_block));
         int per_sm = 0;
         DAB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kPqWarps * 32, smem_block));
@@ -551,7 +437,7 @@ int PqSearchJob::prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint
         // every resident warp owns a LUT (n_chunks x n_centers f32: 32 KB at 32 x 256) and a visited table in
         // global memory; ADC terms and probes are L2 hits only while all of them stay L2-resident
         // (the SQ kernel has no LUT: it keeps the occupancy the shared memory allows)
-        if (mode == 0) per_sm = std::min(per_sm, 6);
+        if (mode == STORE_PQ) per_sm = std::min(per_sm, 6);
         grid = (int)std::min<uint64_t>((uint64_t)per_sm * idx->sm_count, ((uint64_t)nq + kPqWarps - 1) / kPqWarps);
         warps = (uint32_t)grid * kPqWarps;
     }
@@ -559,7 +445,7 @@ int PqSearchJob::prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint
     if ((rc = counters->reserve(16 + (size_t)nq * 4))) return rc;
     p.counters = (uint32_t*)counters->p;
     p.overflow_list = p.counters + 4;
-    const size_t lut_bytes = mode == 0 && !use_pqs ? (size_t)warps * idx->pq_chunks * idx->pq_centers * 4 : 16;
+    const size_t lut_bytes = mode == STORE_PQ && !use_pqs ? (size_t)warps * idx->pq_chunks * idx->pq_centers * 4 : 16;
     if ((rc = luts->reserve(lut_bytes))) return rc;
     p.luts = (float*)luts->p;
     p.n_work = nq;
@@ -575,15 +461,15 @@ int PqSearchJob::prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint
     slots = table_slots(idx, idx->pq_hint, l_search, beam, mode);
     pass = 0;
     if ((rc = reserve_tables())) return rc;
-    if ((rc = stage->reserve(mode == 1 ? sq_stage_bytes(idx, nq) : mode == 2 ? minmax_stage_bytes(idx, nq) : 0))) return rc;
+    if ((rc = stage->reserve(mode == STORE_SQ ? sq_stage_bytes(idx, nq) : mode == STORE_MINMAX ? minmax_stage_bytes(idx, nq) : 0))) return rc;
     DAB_CUDA(cudaEventCreateWithFlags(&counted, cudaEventDisableTiming));
     return DAB_OK;
 }
 
 // SQ and MinMax: the batch's queries compressed by the store's quantizer (MinMax: the NaN flag read back into h_counters)
 int PqSearchJob::stage_queries() {
-    if (mode == 1) return sq_stage_queries(idx, stream, *stage, d_queries, nq, &p.query_codes, &p.query_meta);
-    if (mode == 2) return minmax_stage_queries(idx, stream, *stage, d_queries, nq, (unsigned long long*)(h_counters + 4), &p.query_codes, &p.query_meta);
+    if (mode == STORE_SQ) return sq_stage_queries(idx, stream, *stage, d_queries, nq, &p.query_codes, &p.query_meta);
+    if (mode == STORE_MINMAX) return minmax_stage_queries(idx, stream, *stage, d_queries, nq, (unsigned long long*)(h_counters + 4), &p.query_codes, &p.query_meta);
     return DAB_OK;
 }
 
@@ -635,7 +521,7 @@ int PqSearchJob::launch() {
 
 int PqSearchJob::finish() {
     DAB_CUDA(cudaEventSynchronize(counted));
-    if (mode == 2 && first_nan() != ~0ull) return nan_error();
+    if (mode == STORE_MINMAX && first_nan() != ~0ull) return nan_error();
     for (;;) {
         learn_visited(idx->pq_hint, l_search, beam, mode, h_counters[2]);
         const uint32_t n_over = h_counters[1];
@@ -661,7 +547,7 @@ int PqSearchJob::finish() {
 // The synchronous calls: the job on the handle's stream and scratch.  A MinMax batch with a NaN query fails before any
 // traversal is launched.  Device pointers only; returns once the traversal is complete (the rerank may still run).
 static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam,
-                         const SearchOut& d, bool rerank, int mode) {
+                         const SearchOut& d, bool rerank, QuantStore mode) {
     int rc;
     if ((rc = idx->h_counters.reserve(24))) return rc;
     PqSearchJob job;
@@ -671,7 +557,7 @@ static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uin
     job.h_counters = (uint32_t*)idx->h_counters.p;
     if ((rc = check_pq_args(idx, k, l_search, beam, mode)) || (rc = job.prepare(d_queries, nq, k, l_search, beam, d, rerank, mode))) return rc;
     if ((rc = job.stage_queries())) return rc;
-    if (mode == 2) {
+    if (mode == STORE_MINMAX) {
         DAB_CUDA(cudaStreamSynchronize(idx->stream));
         if (job.first_nan() != ~0ull) return job.nan_error();
     }
@@ -680,14 +566,14 @@ static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uin
 }
 
 static int search_pq_host(dab_index* idx, const char* api, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
-                          uint32_t beam_width, const SearchOut& out, bool rerank, int mode) {
+                          uint32_t beam_width, const SearchOut& out, bool rerank, QuantStore mode) {
     return search_host_buffers(idx, api, queries, nq, k, out, [&](const void* d_queries, const SearchOut& d) {
         return run_search_pq(idx, d_queries, nq, k, l_search, beam_width, d, rerank, mode);
     });
 }
 
 static int search_pq_device(dab_index* idx, const char* api, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
-                            uint32_t beam_width, const SearchOut& d, bool rerank, int mode) {
+                            uint32_t beam_width, const SearchOut& d, bool rerank, QuantStore mode) {
     if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", api);
     if (nq == 0) return DAB_OK;
     if (!d_queries || !d.ids || !d.dists) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
@@ -697,7 +583,7 @@ static int search_pq_device(dab_index* idx, const char* api, const void* d_queri
 
 // The *_async calls: the job on the slot's stream and scratch
 static int search_pq_async(dab_index* idx, const char* api, uint32_t slot, bool host, const void* queries, uint32_t nq, uint32_t k,
-                           uint32_t l_search, uint32_t beam_width, const SearchOut& out, bool rerank, int mode) {
+                           uint32_t l_search, uint32_t beam_width, const SearchOut& out, bool rerank, QuantStore mode) {
     if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", api);
     if (nq && (!queries || !out.ids || !out.dists)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
     int rc;
@@ -724,46 +610,46 @@ extern "C" {
 int dab_search_batch_pq(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
                         uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops) {
     return search_pq_host(idx, "dab_search_batch_pq", queries, nq, k, l_search, beam_width,
-                          SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, false, 0);
+                          SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, false, STORE_PQ);
 }
 
 int dab_search_batch_pq_rerank(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
                                uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops) {
     return search_pq_host(idx, "dab_search_batch_pq_rerank", queries, nq, k, l_search, beam_width,
-                          SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, true, 0);
+                          SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, true, STORE_PQ);
 }
 
 int dab_search_batch_pq_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
                                int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts, uint32_t* d_out_cmps,
                                uint32_t* d_out_hops) {
     return search_pq_device(idx, "dab_search_batch_pq_device", d_queries, nq, k, l_search, beam_width,
-                            SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, 0);
+                            SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, STORE_PQ);
 }
 
 int dab_search_batch_sq(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
                         int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops) {
     return search_pq_host(idx, "dab_search_batch_sq", queries, nq, k, l_search, beam_width,
-                          SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, rerank != 0, 1);
+                          SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, rerank != 0, STORE_SQ);
 }
 
 int dab_search_batch_sq_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
                                int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts, uint32_t* d_out_cmps,
                                uint32_t* d_out_hops) {
     return search_pq_device(idx, "dab_search_batch_sq_device", d_queries, nq, k, l_search, beam_width,
-                            SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, 1);
+                            SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, STORE_SQ);
 }
 
 int dab_search_batch_minmax(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
                             int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops) {
     return search_pq_host(idx, "dab_search_batch_minmax", queries, nq, k, l_search, beam_width,
-                          SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, rerank != 0, 2);
+                          SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, rerank != 0, STORE_MINMAX);
 }
 
 int dab_search_batch_minmax_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
                                    int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts, uint32_t* d_out_cmps,
                                    uint32_t* d_out_hops) {
     return search_pq_device(idx, "dab_search_batch_minmax_device", d_queries, nq, k, l_search, beam_width,
-                            SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, 2);
+                            SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, STORE_MINMAX);
 }
 
 // ---- asynchronous batches (see dab_search_batch_async): the same jobs on a slot, joined by dab_wait ----
@@ -771,42 +657,42 @@ int dab_search_batch_pq_async(dab_index* idx, uint32_t slot, const void* queries
                               uint32_t beam_width, int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
                               uint32_t* out_cmps, uint32_t* out_hops) {
     return search_pq_async(idx, "dab_search_batch_pq_async", slot, true, queries, nq, k, l_search, beam_width,
-                           SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, rerank != 0, 0);
+                           SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, rerank != 0, STORE_PQ);
 }
 
 int dab_search_batch_pq_device_async(dab_index* idx, uint32_t slot, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
                                      uint32_t beam_width, int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
                                      uint32_t* d_out_cmps, uint32_t* d_out_hops) {
     return search_pq_async(idx, "dab_search_batch_pq_device_async", slot, false, d_queries, nq, k, l_search, beam_width,
-                           SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, 0);
+                           SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, STORE_PQ);
 }
 
 int dab_search_batch_sq_async(dab_index* idx, uint32_t slot, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
                               uint32_t beam_width, int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
                               uint32_t* out_cmps, uint32_t* out_hops) {
     return search_pq_async(idx, "dab_search_batch_sq_async", slot, true, queries, nq, k, l_search, beam_width,
-                           SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, rerank != 0, 1);
+                           SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, rerank != 0, STORE_SQ);
 }
 
 int dab_search_batch_sq_device_async(dab_index* idx, uint32_t slot, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
                                      uint32_t beam_width, int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
                                      uint32_t* d_out_cmps, uint32_t* d_out_hops) {
     return search_pq_async(idx, "dab_search_batch_sq_device_async", slot, false, d_queries, nq, k, l_search, beam_width,
-                           SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, 1);
+                           SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, STORE_SQ);
 }
 
 int dab_search_batch_minmax_async(dab_index* idx, uint32_t slot, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
                                   uint32_t beam_width, int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
                                   uint32_t* out_cmps, uint32_t* out_hops) {
     return search_pq_async(idx, "dab_search_batch_minmax_async", slot, true, queries, nq, k, l_search, beam_width,
-                           SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, rerank != 0, 2);
+                           SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, rerank != 0, STORE_MINMAX);
 }
 
 int dab_search_batch_minmax_device_async(dab_index* idx, uint32_t slot, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
                                          uint32_t beam_width, int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
                                          uint32_t* d_out_cmps, uint32_t* d_out_hops) {
     return search_pq_async(idx, "dab_search_batch_minmax_device_async", slot, false, d_queries, nq, k, l_search, beam_width,
-                           SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, 2);
+                           SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, STORE_MINMAX);
 }
 
 }  // extern "C"

@@ -26,6 +26,7 @@
 #include "dab_common.cuh"
 #include "quant_device.cuh"
 #include "search_common.cuh"
+#include "search_host.cuh"
 #include "search_pq.cuh"
 
 #include <algorithm>
@@ -120,25 +121,10 @@ __global__ void __launch_bounds__(kPqsMaxWarps * 32, 1) search_kernel_pqs(const 
         __syncwarp();
     };
 
-    for (;;) {
-        uint32_t w = 0;
-        if (lane == 0) w = atomicAdd(p.counters, 1u);
-        w = __shfl_sync(kFull, w, 0);
-        if (w >= p.n_work) break;
-        const uint32_t qidx = p.query_list ? p.query_list[w] : w;
-
+    for (uint32_t qidx; next_query(p.counters, p.n_work, p.query_list, lane, qidx);) {
         // ---- query -> f32 (T: Into<f32>), visited clear
         __syncwarp();
-        for (int e = lane; e < dim; e += 32) {
-            float v;
-            switch (p.dtype) {
-                case DAB_F32: v = reinterpret_cast<const float*>(p.queries)[(size_t)qidx * dim + e]; break;
-                case DAB_F16: v = __half2float(reinterpret_cast<const __half*>(p.queries)[(size_t)qidx * dim + e]); break;
-                case DAB_I8: v = (float)reinterpret_cast<const int8_t*>(p.queries)[(size_t)qidx * dim + e]; break;
-                default: v = (float)reinterpret_cast<const uint8_t*>(p.queries)[(size_t)qidx * dim + e]; break;
-            }
-            qf[e] = v;
-        }
+        widen_query(p.dtype, p.queries, qidx, dim, qf, lane);
         for (uint32_t i = lane; i < nbk; i += 32) store_empty_bucket(table + (size_t)i * 8);
         __syncwarp();
 
@@ -155,29 +141,14 @@ __global__ void __launch_bounds__(kPqsMaxWarps * 32, 1) search_kernel_pqs(const 
                 if ((uint32_t)lane < n) {
                     const uint32_t id = (uint32_t)p.n_points + s0 + lane;
                     cid[lane] = id;
-                    const uint32_t b = bucket_of(id, nbk);
-                    uint32_t bs[8];
-                    load_bucket(table + (size_t)b * 8, bs);
-                    bucket_insert(table, nbk, b, bs, id);
+                    visit_global(table, nbk, id);
                 }
                 s0 += 32;
                 ncand = n;
                 nvisited += n;
             } else {
                 const uint32_t lim = min(p.cap, size);
-                while (nb < p.beam) {
-                    const uint32_t idx = first_unvisited(qi, cursor_lo, lim, lane);
-                    if (idx >= lim) break;
-                    const uint32_t id = qi[idx];
-                    __syncwarp();
-                    if (lane == 0) {
-                        qi[idx] = id | kFlagV2;
-                        beam_ids[nb] = id;
-                    }
-                    cursor_lo = idx + 1;
-                    ++nb;
-                    __syncwarp();
-                }
+                nb = pick_beam(qi, lim, p.beam, cursor_lo, beam_ids, lane);
                 if (nb == 0) break;
                 // the row copied one hop ahead, if the guess was right
                 uint32_t w0[3] = {kEmptyV2, kEmptyV2, kEmptyV2};
@@ -280,12 +251,7 @@ __global__ void __launch_bounds__(kPqsMaxWarps * 32, 1) search_kernel_pqs(const 
                                 load_bucket(table + (size_t)bk[t] * 8, bs[t]);
                                 inserted = bucket_insert(table, nbk, bk[t], bs[t], wd[t]);
                             }
-                            const bool isnew = inserted && wd[t] < n_total;
-                            const unsigned mi = __ballot_sync(kFull, inserted);
-                            const unsigned mn = __ballot_sync(kFull, isnew);
-                            if (isnew) cid[ncand + __popc(mn & ((1u << lane) - 1u))] = wd[t];
-                            ncand += __popc(mn);
-                            nvisited += __popc(mi);
+                            push_new(inserted, inserted && wd[t] < n_total, wd[t], cid, ncand, nvisited, lane);
                         }
                     }
                     if (nvisited + p.max_degree > hlimit) {
@@ -316,43 +282,13 @@ __global__ void __launch_bounds__(kPqsMaxWarps * 32, 1) search_kernel_pqs(const 
         }
 
         if (overflow) {
-            if (lane == 0) {
-                const uint32_t o = atomicAdd(p.counters + 1, 1u);
-                p.overflow_list[o] = qidx;
-            }
+            report_overflow(p.counters, p.overflow_list, qidx, lane);
             continue;
         }
-        {
-            const uint32_t n = min(p.cap, size);
-            if (p.list_ids) {
-                for (uint32_t i = lane; i < n; i += 32) p.list_ids[(size_t)qidx * p.list_cap + i] = qi[i] & ~kFlagV2;
-                if (lane == 0) p.list_counts[qidx] = n;
-            }
-            uint32_t count = 0;
-            for (uint32_t b = 0; b < n && count < p.k; b += 32) {
-                const uint32_t i = b + lane;
-                const uint32_t id = i < n ? (qi[i] & ~kFlagV2) : kEmptyV2;
-                const bool keep = i < n && id < p.n_points;
-                const unsigned m = __ballot_sync(kFull, keep);
-                const uint32_t pos = count + __popc(m & ((1u << lane) - 1u));
-                if (keep && pos < p.k) {
-                    p.out_ids[(size_t)qidx * p.k + pos] = id;
-                    p.out_dists[(size_t)qidx * p.k + pos] = qd[i];
-                }
-                count += __popc(m);
-            }
-            count = min(count, p.k);
-            for (uint32_t i = count + lane; i < p.k; i += 32) {
-                p.out_ids[(size_t)qidx * p.k + i] = kEmptyV2;
-                p.out_dists[(size_t)qidx * p.k + i] = __int_as_float(0x7F800000);
-            }
-            if (lane == 0) {
-                atomicMax(p.counters + 2, nvisited);
-                if (p.out_counts) p.out_counts[qidx] = count;
-                if (p.out_cmps) p.out_cmps[qidx] = cmps;
-                if (p.out_hops) p.out_hops[qidx] = hops;
-            }
-        }
+        const uint32_t n = min(p.cap, size);
+        if (p.list_ids) write_list(qi, n, p.list_ids, p.list_counts, p.list_cap, qidx, lane);
+        const uint32_t count = write_results(qi, qd, n, p.n_points, p.k, p.out_ids, p.out_dists, qidx, lane);
+        write_stats(p.counters, nvisited, p.out_counts, p.out_cmps, p.out_hops, qidx, count, cmps, hops, lane);
     }
 }
 
@@ -379,13 +315,10 @@ bool pqs_plan(const dab_index* idx, uint32_t warp_smem, uint32_t nq, PqsPlan* ou
 }
 
 int pqs_launch(const SearchParamsPq& p, const PqsPlan& plan, uint32_t cap, cudaStream_t stream) {
-    void (*kern)(const SearchParamsPq);
-#define DAB_PQS_PICK(CL_)                                                                                        \
-    kern = cap <= 128 ? search_kernel_pqs<4, CL_> : cap <= 256 ? search_kernel_pqs<8, CL_> : cap <= 512 ? search_kernel_pqs<16, CL_> : search_kernel_pqs<32, CL_>
-    if (plan.chunk_len == 4) DAB_PQS_PICK(4);
-    else if (plan.chunk_len == 8) DAB_PQS_PICK(8);
-    else DAB_PQS_PICK(0);
-#undef DAB_PQS_PICK
+    void (*kern)(const SearchParamsPq) = visit_list_tile(cap, [&](auto qt) {
+        constexpr int QT = decltype(qt)::value;
+        return plan.chunk_len == 4 ? search_kernel_pqs<QT, 4> : plan.chunk_len == 8 ? search_kernel_pqs<QT, 8> : search_kernel_pqs<QT, 0>;
+    });
     DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem));
     kern<<<plan.grid, plan.warps * 32, plan.smem, stream>>>(p);
     DAB_LAUNCHED();

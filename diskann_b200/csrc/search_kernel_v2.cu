@@ -167,19 +167,13 @@ __device__ __forceinline__ void group_distance_int(const uint8_t* __restrict__ q
     }
 }
 
-// Rare paths of the two-level visited set: clearing the warp's global table when its first id arrives, and the
-// atomic insert.  (The kernel is sensitive to its code size — at ~100 KB of SASS every phase ran ~20 % slower than at
+// Rare path of the two-level visited set: clearing the warp's global table when its first id arrives (the atomic
+// insert is visit_global).  (The kernel is sensitive to its code size — at ~100 KB of SASS every phase ran ~20 % slower than at
 // 60 KB — so the hot loop is kept compact: one rolled loop over a row's chunks, no unrolled copies of these.)
 __device__ __forceinline__ void clear_global_table(uint32_t* table, uint32_t nbk, int lane) {
 #pragma unroll 1
     for (uint32_t i = lane; i < nbk; i += 32) store_empty_bucket(table + (size_t)i * 8);
     __syncwarp();
-}
-__device__ __forceinline__ bool global_table_insert(uint32_t* table, uint32_t nbk, uint32_t id) {
-    uint32_t bs[8];
-    const uint32_t b = bucket_of(id, nbk);
-    load_bucket(table + (size_t)b * 8, bs);
-    return bucket_insert(table, nbk, b, bs, id);
 }
 
 // L1 = true: two-level visited set.  Level 1 is a table of 16-bit quotient tags in the warp's own shared memory
@@ -225,24 +219,12 @@ __global__ void __launch_bounds__(kV2Warps * 32, REG ? kV2MinCtasReg : QT == 0 ?
     uint64_t row_policy;
     asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(row_policy));
 
-    for (;;) {
-        uint32_t w = 0;
-        if (lane == 0) w = atomicAdd(p.counters, 1u);
-        w = __shfl_sync(kFull, w, 0);
-        if (w >= p.n_work) break;
-        const uint32_t qidx = p.query_list ? p.query_list[w] : w;
-
+    for (uint32_t qidx; next_query(p.counters, p.n_work, p.query_list, lane, qidx);) {
         __syncwarp();
         {
             const TD* s = p.query_rows ? reinterpret_cast<const TD*>(p.vectors + (size_t)p.query_rows[qidx] * p.row_stride)
                                        : reinterpret_cast<const TD*>(p.queries) + (size_t)qidx * dim;
-            if constexpr (V2Int<TD>::value) {
-                uint8_t* qb = reinterpret_cast<uint8_t*>(qf);
-                const int qbytes = (dim + 3) & ~3;
-                for (int e = lane; e < qbytes; e += 32) qb[e] = e < dim ? reinterpret_cast<const uint8_t*>(s)[e] : 0;
-            } else {
-                for (int e = lane; e < dim; e += 32) qf[e] = to_f32(s[e]);
-            }
+            load_query(s, dim, 4, qf, lane);
             if constexpr (L1) {
                 const uint4 e4 = make_uint4(kEmptyV2, kEmptyV2, kEmptyV2, kEmptyV2);
                 for (uint32_t i = lane; i < nb1 * 2; i += 32) reinterpret_cast<uint4*>(t1)[i] = e4;
@@ -280,7 +262,7 @@ __global__ void __launch_bounds__(kV2Warps * 32, REG ? kV2MinCtasReg : QT == 0 ?
                     l2_used = true;
                 }
                 bool ins2 = false;
-                if (need) ins2 = global_table_insert(table, nbk, id);
+                if (need) ins2 = visit_global(table, nbk, id);
                 nvisited += __popc(__ballot_sync(kFull, ins2));
                 ins |= ins2;
             }
@@ -393,10 +375,7 @@ __global__ void __launch_bounds__(kV2Warps * 32, REG ? kV2MinCtasReg : QT == 0 ?
             } else if ((uint32_t)lane < n) {
                 const uint32_t id = (uint32_t)p.n_points + s0 + lane;
                 cid[lane] = id;
-                uint32_t bs[8];
-                const uint32_t b = bucket_of(id, nbk);
-                load_bucket(table + (size_t)b * 8, bs);
-                bucket_insert(table, nbk, b, bs, id);
+                visit_global(table, nbk, id);
             }
             __syncwarp();
             distances(n);
@@ -408,8 +387,11 @@ __global__ void __launch_bounds__(kV2Warps * 32, REG ? kV2MinCtasReg : QT == 0 ?
         // ---- greedy loop (index.rs:1961-1992)
         for (;;) {
             const uint32_t lim = min(p.cap, size);
+            // closest_notvisited x beam_width (queue.rs:297-313) with the build's record of expanded nodes.  The statements
+            // of pick_beam (search_common.cuh), kept here: through the helper and its callback ptxas spills 4 to 20 bytes
+            // more in most instantiations of this kernel, which is at its register bound
             uint32_t nb = 0;
-            while (nb < p.beam) {  // closest_notvisited x beam_width (queue.rs:297-313)
+            while (nb < p.beam) {
                 const uint32_t idx = first_unvisited(qi, cursor_lo, lim, lane);
                 if (idx >= lim) break;
                 const uint32_t id = qi[idx];
@@ -480,10 +462,7 @@ __global__ void __launch_bounds__(kV2Warps * 32, REG ? kV2MinCtasReg : QT == 0 ?
                         if (c0 >= 96) word = j < p.adj_stride ? __ldg(row + j) : kEmptyV2;
                         // ids beyond 2^K cannot be in bounds and would share the tag of id mod 2^K: not tracked
                         const bool ins = visit_l1(word, j >= 1 && j <= deg && word <= tmap.kmask);
-                        const bool isnew = ins && word < n_total;  // is_in_bounds
-                        const unsigned mn = __ballot_sync(kFull, isnew);
-                        if (isnew) cid[ncand + __popc(mn & ((1u << lane) - 1u))] = word;
-                        ncand += __popc(mn);
+                        push_new(ins && word < n_total, word, cid, ncand, lane);  // is_in_bounds; visit_l1 has counted the insert
                     }
                     if (!closed && n1 + p.max_degree > p.t1_limit) closed = true;
                 } else {
@@ -502,30 +481,14 @@ __global__ void __launch_bounds__(kV2Warps * 32, REG ? kV2MinCtasReg : QT == 0 ?
                     for (int c = 0; c < 3; ++c) {
                         bool inserted = false;
                         if (valid[c]) inserted = bucket_insert(table, nbk, bk[c], bs[c], wd[c]);
-                        const bool isnew = inserted && wd[c] < n_total;  // is_in_bounds
-                        const unsigned mi = __ballot_sync(kFull, inserted);
-                        const unsigned mn = __ballot_sync(kFull, isnew);
-                        if (isnew) cid[ncand + __popc(mn & ((1u << lane) - 1u))] = wd[c];
-                        ncand += __popc(mn);
-                        nvisited += __popc(mi);
+                        push_new(inserted, inserted && wd[c] < n_total, wd[c], cid, ncand, nvisited, lane);  // is_in_bounds
                     }
                     // adjacency rows longer than 95 neighbours: remaining chunks
                     for (uint32_t c0 = 96; c0 < deg + 1; c0 += 32) {
                         const uint32_t j = c0 + lane;
                         const uint32_t word = j < p.adj_stride ? __ldg(row + j) : kEmptyV2;
-                        bool inserted = false;
-                        if (j <= deg) {
-                            const uint32_t b2 = bucket_of(word, nbk);
-                            uint32_t bs2[8];
-                            load_bucket(table + (size_t)b2 * 8, bs2);
-                            inserted = bucket_insert(table, nbk, b2, bs2, word);
-                        }
-                        const bool isnew = inserted && word < n_total;
-                        const unsigned mi = __ballot_sync(kFull, inserted);
-                        const unsigned mn = __ballot_sync(kFull, isnew);
-                        if (isnew) cid[ncand + __popc(mn & ((1u << lane) - 1u))] = word;
-                        ncand += __popc(mn);
-                        nvisited += __popc(mi);
+                        const bool inserted = j <= deg && visit_global(table, nbk, word);
+                        push_new(inserted, inserted && word < n_total, word, cid, ncand, nvisited, lane);
                     }
                 }
                 if (nvisited + p.max_degree > hlimit) {  // the next node could pass the load limit: stop expanding now
@@ -545,43 +508,19 @@ __global__ void __launch_bounds__(kV2Warps * 32, REG ? kV2MinCtasReg : QT == 0 ?
         }
 
         if (overflow) {
-            if (lane == 0) {
-                uint32_t o = atomicAdd(p.counters + 1, 1u);
-                p.overflow_list[o] = qidx;
-            }
+            report_overflow(p.counters, p.overflow_list, qidx, lane);
             continue;
         }
 
         // ---- post-process: drop start points, first k (provider.rs:907-950)
         {
-            const uint32_t n = min(p.cap, size);
-            uint32_t count = 0;
-            for (uint32_t b = 0; b < n && count < p.k; b += 32) {
-                const uint32_t i = b + lane;
-                const uint32_t id = i < n ? (qi[i] & ~kFlagV2) : kEmptyV2;
-                const bool keep = i < n && id < p.n_points;
-                const unsigned m = __ballot_sync(kFull, keep);
-                const uint32_t pos = count + __popc(m & ((1u << lane) - 1u));
-                if (keep && pos < p.k) {
-                    p.out_ids[(size_t)qidx * p.k + pos] = id;
-                    p.out_dists[(size_t)qidx * p.k + pos] = qd[i];
-                }
-                count += __popc(m);
-            }
-            count = min(count, p.k);
-            for (uint32_t i = count + lane; i < p.k; i += 32) {
-                p.out_ids[(size_t)qidx * p.k + i] = kEmptyV2;
-                p.out_dists[(size_t)qidx * p.k + i] = __int_as_float(0x7F800000);
-            }
-            if (lane == 0) {
-                atomicMax(p.counters + 2, n1 + nvisited);
-                if (p.out_counts) p.out_counts[qidx] = count;
-                if (p.out_cmps) p.out_cmps[qidx] = cmps;
-                if (p.out_hops) p.out_hops[qidx] = nrec;
-                if (p.rec_counts) {
-                    p.rec_counts[qidx] = min(nrec, p.rec_cap);
-                    if (nrec > p.rec_cap) atomicAdd(p.counters + 3, 1u);  // expanded nodes beyond the record: reported by dab_build
-                }
+            const uint32_t count = write_results(qi, qd, min(p.cap, size), p.n_points, p.k, p.out_ids, p.out_dists, qidx, lane);
+            // the visited set is level 1's ids plus the global table's (nvisited counts only those when level 1 is on);
+            // every expanded node is a hop, so nrec is the hop count
+            write_stats(p.counters, n1 + nvisited, p.out_counts, p.out_cmps, p.out_hops, qidx, count, cmps, nrec, lane);
+            if (lane == 0 && p.rec_counts) {
+                p.rec_counts[qidx] = min(nrec, p.rec_cap);
+                if (nrec > p.rec_cap) atomicAdd(p.counters + 3, 1u);  // expanded nodes beyond the record: reported by dab_build
             }
         }
     }

@@ -73,24 +73,12 @@ __global__ void __launch_bounds__(kV3Warps * 32, kV3MinCtas) search_kernel_v3(co
     const uint64_t n_total = p.n_points + p.n_start;
     const int dim = (int)p.dim;
 
-    for (;;) {
-        uint32_t w = 0;
-        if (lane == 0) w = atomicAdd(p.counters, 1u);
-        w = __shfl_sync(kFull, w, 0);
-        if (w >= p.n_work) break;
-        const uint32_t qidx = p.query_list ? p.query_list[w] : w;
-
+    for (uint32_t qidx; next_query(p.counters, p.n_work, p.query_list, lane, qidx);) {
         __syncwarp();
         {
             const TD* s = p.query_rows ? reinterpret_cast<const TD*>(p.vectors + (size_t)p.query_rows[qidx] * p.row_stride)
                                        : reinterpret_cast<const TD*>(p.queries) + (size_t)qidx * dim;
-            if constexpr (kInt) {
-                uint8_t* qb = reinterpret_cast<uint8_t*>(qf);
-                const int qbytes = (dim + 15) & ~15;
-                for (int e = lane; e < qbytes; e += 32) qb[e] = e < dim ? reinterpret_cast<const uint8_t*>(s)[e] : 0;
-            } else {
-                for (int e = lane; e < dim; e += 32) qf[e] = to_f32(s[e]);
-            }
+            load_query(s, dim, 16, qf, lane);
             const uint4 e4 = make_uint4(kEmptyV2, kEmptyV2, kEmptyV2, kEmptyV2);
             for (uint32_t i = lane; i < nbk * 2; i += 32) reinterpret_cast<uint4*>(table)[i] = e4;
         }
@@ -154,26 +142,15 @@ __global__ void __launch_bounds__(kV3Warps * 32, kV3MinCtas) search_kernel_v3(co
         // ---- greedy loop (index.rs:1961-1992)
         while (!overflow) {
             const uint32_t lim = min(p.cap, size);
-            uint32_t nb = 0;
-            while (nb < p.beam) {  // closest_notvisited x beam_width (queue.rs:297-313)
-                const uint32_t idx = first_unvisited(qi, cursor_lo, lim, lane);
-                if (idx >= lim) break;
-                const uint32_t id = qi[idx];
-                __syncwarp();
-                if (lane == 0) {
-                    qi[idx] = id | kFlagV2;
-                    beam_ids[nb] = id;
-                    if (p.rec_ids && nrec < p.rec_cap) {
-                        p.rec_ids[(size_t)qidx * p.rec_cap + nrec] = id;
-                        p.rec_dists[(size_t)qidx * p.rec_cap + nrec] = qd[idx];
-                    }
+            // the build records every expanded node and its distance, in expansion order
+            const uint32_t nb = pick_beam(qi, lim, p.beam, cursor_lo, beam_ids, lane, [&](uint32_t b, uint32_t idx, uint32_t id) {
+                if (p.rec_ids && nrec + b < p.rec_cap) {
+                    p.rec_ids[(size_t)qidx * p.rec_cap + nrec + b] = id;
+                    p.rec_dists[(size_t)qidx * p.rec_cap + nrec + b] = qd[idx];
                 }
-                cursor_lo = idx + 1;
-                ++nrec;
-                ++nb;
-                __syncwarp();
-            }
+            });
             if (nb == 0) break;
+            nrec += nb;
 
             uint32_t ncand = 0;
             for (uint32_t b = 0; b < nb; ++b) {
@@ -219,12 +196,7 @@ __global__ void __launch_bounds__(kV3Warps * 32, kV3MinCtas) search_kernel_v3(co
                     bool inserted = false;
                     // ids beyond 2^K cannot be in bounds and never reach the outputs: not tracked
                     if (j >= 1 && j <= deg && word <= tmap.kmask) inserted = visit(word, ovf);
-                    const bool isnew = inserted && word < n_total;  // is_in_bounds
-                    const unsigned mi = __ballot_sync(kFull, inserted);
-                    const unsigned mn = __ballot_sync(kFull, isnew);
-                    if (isnew) cid[ncand + __popc(mn & ((1u << lane) - 1u))] = word;
-                    ncand += __popc(mn);
-                    nvisited += __popc(mi);
+                    push_new(inserted, inserted && word < n_total, word, cid, ncand, nvisited, lane);  // is_in_bounds
                 };
 #pragma unroll
                 for (int c = 0; c < 3; ++c)
@@ -253,43 +225,17 @@ __global__ void __launch_bounds__(kV3Warps * 32, kV3MinCtas) search_kernel_v3(co
 
         if (overflow) {
             if (p.adj_words) asm volatile("cp.async.wait_group 0;" ::: "memory");
-            if (lane == 0) {
-                const uint32_t o = atomicAdd(p.counters + 1, 1u);
-                p.overflow_list[o] = qidx;
-            }
+            report_overflow(p.counters, p.overflow_list, qidx, lane);
             continue;
         }
 
         // ---- post-process: drop start points, first k (provider.rs:907-950)
         {
-            const uint32_t n = min(p.cap, size);
-            uint32_t count = 0;
-            for (uint32_t b = 0; b < n && count < p.k; b += 32) {
-                const uint32_t i = b + lane;
-                const uint32_t id = i < n ? (qi[i] & ~kFlagV2) : kEmptyV2;
-                const bool keep = i < n && id < p.n_points;
-                const unsigned m = __ballot_sync(kFull, keep);
-                const uint32_t pos = count + __popc(m & ((1u << lane) - 1u));
-                if (keep && pos < p.k) {
-                    p.out_ids[(size_t)qidx * p.k + pos] = id;
-                    p.out_dists[(size_t)qidx * p.k + pos] = qd[i];
-                }
-                count += __popc(m);
-            }
-            count = min(count, p.k);
-            for (uint32_t i = count + lane; i < p.k; i += 32) {
-                p.out_ids[(size_t)qidx * p.k + i] = kEmptyV2;
-                p.out_dists[(size_t)qidx * p.k + i] = __int_as_float(0x7F800000);
-            }
-            if (lane == 0) {
-                atomicMax(p.counters + 2, nvisited);
-                if (p.out_counts) p.out_counts[qidx] = count;
-                if (p.out_cmps) p.out_cmps[qidx] = cmps;
-                if (p.out_hops) p.out_hops[qidx] = hops;
-                if (p.rec_counts) {
-                    p.rec_counts[qidx] = min(nrec, p.rec_cap);
-                    if (nrec > p.rec_cap) atomicAdd(p.counters + 3, 1u);  // expanded nodes beyond the record: reported by dab_build
-                }
+            const uint32_t count = write_results(qi, qd, min(p.cap, size), p.n_points, p.k, p.out_ids, p.out_dists, qidx, lane);
+            write_stats(p.counters, nvisited, p.out_counts, p.out_cmps, p.out_hops, qidx, count, cmps, hops, lane);
+            if (lane == 0 && p.rec_counts) {
+                p.rec_counts[qidx] = min(nrec, p.rec_cap);
+                if (nrec > p.rec_cap) atomicAdd(p.counters + 3, 1u);  // expanded nodes beyond the record: reported by dab_build
             }
         }
     }

@@ -193,12 +193,7 @@ __device__ __forceinline__ void paged_queries(const PagedParams& p, uint8_t* bas
     const uint64_t n_total = p.n_points + p.n_start;
     const uint32_t cap = p.cap;
 
-    for (;;) {
-        uint32_t w = 0;
-        if (lane == 0) w = atomicAdd(p.counters, 1u);
-        w = __shfl_sync(kFull, w, 0);
-        if (w >= p.n_work) break;
-        const uint32_t q = p.work ? p.work[w] : w;
+    for (uint32_t q; next_query(p.counters, p.n_work, p.work, lane, q);) {
         const PagedQuery st = p.qs[q];
         uint32_t* ctr = p.ctr + (size_t)q * C_WORDS;
         const uint32_t hlimit = st.n_buckets * 7;  // 87.5 % load
@@ -223,13 +218,7 @@ __device__ __forceinline__ void paged_queries(const PagedParams& p, uint8_t* bas
 
         // HashSet::insert of one id per lane; the new ones are logged in lane order
         auto visit = [&](uint32_t id, bool ok) -> bool {
-            bool ins = false;
-            if (ok) {
-                const uint32_t b = bucket_of(id, st.n_buckets);
-                uint32_t bs[8];
-                load_bucket(st.table + (size_t)b * 8, bs);
-                ins = bucket_insert(st.table, st.n_buckets, b, bs, id);
-            }
+            const bool ins = ok && visit_global(st.table, st.n_buckets, id);
             const unsigned m = __ballot_sync(kFull, ins);
             if (ins) st.log[logn + __popc(m & ((1u << lane) - 1u))] = id;
             logn += __popc(m);
@@ -246,9 +235,7 @@ __device__ __forceinline__ void paged_queries(const PagedParams& p, uint8_t* bas
                 const uint32_t jj = c0 + lane;
                 const uint32_t word = jj < p.adj_stride ? __ldg(row + jj) : kEmptyV2;
                 const bool isnew = visit(word, jj >= 1 && jj <= deg) && word < n_total;  // is_in_bounds after the insert
-                const unsigned mn = __ballot_sync(kFull, isnew);
-                if (isnew) cid[ncand + __popc(mn & ((1u << lane) - 1u))] = word;
-                ncand += __popc(mn);
+                push_new(isnew, word, cid, ncand, lane);
             }
             __syncwarp();
             return ncand;
@@ -301,7 +288,7 @@ __device__ __forceinline__ void paged_queries(const PagedParams& p, uint8_t* bas
         }
 
         if (overflow) {
-            if (lane == 0) p.overflow_list[atomicAdd(p.counters + 1, 1u)] = q;
+            report_overflow(p.counters, p.overflow_list, q, lane);
             continue;
         }
 
@@ -383,14 +370,7 @@ __global__ void __launch_bounds__(kPagedWarps * 32) paged_kernel(const PagedPara
         float* qf;
         int lane, dim, qq;
         __device__ __forceinline__ void load(uint32_t q) {
-            const TD* s = reinterpret_cast<const TD*>(p.queries) + (size_t)q * dim;
-            if constexpr (INT) {
-                uint8_t* qb = reinterpret_cast<uint8_t*>(qf);
-                const int qbytes = (dim + 3) & ~3;
-                for (int e = lane; e < qbytes; e += 32) qb[e] = e < dim ? reinterpret_cast<const uint8_t*>(s)[e] : 0;
-            } else {
-                for (int e = lane; e < dim; e += 32) qf[e] = to_f32(s[e]);  // f16 queries are widened (layers/full.rs:421-423)
-            }
+            load_query(reinterpret_cast<const TD*>(p.queries) + (size_t)q * dim, dim, 4, qf, lane);
         }
         __device__ __forceinline__ void prepare() {
             qq = 0;  // Sum x^2 of the query (unused by inner product)
@@ -445,24 +425,8 @@ __global__ void __launch_bounds__(kPagedWarps * 32) paged_kernel_quant(const Pag
         uint32_t entries;
         float q_comp;
         __device__ __forceinline__ void load(uint32_t q) {
-            if (MODE == 0) {
-                for (int e = lane; e < dim; e += 32) {
-                    float v;
-                    switch (p.dtype) {
-                        case DAB_F32: v = reinterpret_cast<const float*>(p.queries)[(size_t)q * dim + e]; break;
-                        case DAB_F16: v = __half2float(reinterpret_cast<const __half*>(p.queries)[(size_t)q * dim + e]); break;
-                        case DAB_I8: v = (float)reinterpret_cast<const int8_t*>(p.queries)[(size_t)q * dim + e]; break;
-                        default: v = (float)reinterpret_cast<const uint8_t*>(p.queries)[(size_t)q * dim + e]; break;
-                    }
-                    qf[e] = v;
-                }
-            } else {
-                const uint32_t words = p.code_stride >> 2;
-                const uint32_t* src = reinterpret_cast<const uint32_t*>(p.query_codes + (size_t)q * p.code_stride);
-                for (uint32_t w = lane; w < words; w += 32) qc[w] = __ldg(src + w);
-                if (MODE == 1) q_comp = __shfl_sync(kFull, lane == 0 ? __ldg(&p.query_meta[q].x) : 0.0f, 0);
-                if (MODE == 2 && lane == 0) *reinterpret_cast<float4*>(qc + words) = __ldg(p.query_meta + q);
-            }
+            if (MODE == 0) widen_query(p.dtype, p.queries, q, dim, qf, lane);
+            else load_query_codes<MODE>(p.query_codes + (size_t)q * p.code_stride, p.query_meta + q, p.code_stride >> 2, qc, q_comp, lane);
         }
         __device__ __forceinline__ void prepare() {
             if (MODE == 0 && !p.direct_cosine) {
@@ -501,10 +465,7 @@ __global__ void __launch_bounds__(kPagedWarps * 32) paged_relocate_kernel(PagedQ
             if (i < logn) {
                 const uint32_t id = a.log[i];
                 b.log[i] = id;
-                const uint32_t bk = bucket_of(id, b.n_buckets);
-                uint32_t bs[8];
-                load_bucket(b.table + (size_t)bk * 8, bs);
-                bucket_insert(b.table, b.n_buckets, bk, bs, id);
+                visit_global(b.table, b.n_buckets, id);
             }
         }
         __syncwarp();
@@ -611,10 +572,7 @@ int run_pass(dab_paged* s) {
     DAB_CUDA(cudaFuncSetAttribute(s->kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s->smem_block));
     for (int pass = 0;;) {
         DAB_CUDA(cudaMemsetAsync(s->d_counters, 0, 8, st));
-        const uint64_t max_warps = (uint64_t)s->grid * kPagedWarps;
-        const uint64_t rounds = (p.n_work + max_warps - 1) / max_warps;
-        const uint64_t need = (p.n_work + rounds - 1) / rounds;
-        s->kern<<<(int)((need + kPagedWarps - 1) / kPagedWarps), kPagedWarps * 32, s->smem_block, st>>>(p);
+        s->kern<<<balanced_grid(p.n_work, s->grid, kPagedWarps), kPagedWarps * 32, s->smem_block, st>>>(p);
         DAB_LAUNCHED();
         DAB_CUDA(cudaGetLastError());
         uint32_t n_over = 0;
@@ -695,29 +653,14 @@ int prepare_quant_kernel(dab_paged* s) {
     p.dtype = idx->dtype;
     size_t qbytes;
     int max_per_sm = INT32_MAX;
+    set_store_params(idx, (QuantStore)s->store, p);
     if (s->store == STORE_PQ) {
-        p.pivots = idx->d_pivots;
-        p.offsets = idx->d_offsets;
-        p.codes = idx->d_codes;
-        p.n_chunks = idx->pq_chunks;
-        p.n_centers = idx->pq_centers;
-        p.ip_table = idx->metric == DAB_INNER_PRODUCT ? 1 : 0;  // L2 and CosineNormalized use TableL2 (dynamic.rs:80-85)
-        p.direct_cosine = idx->metric == DAB_COSINE ? 1 : 0;
         qbytes = round_up((size_t)idx->dim * 4, 16);
         // every resident warp owns a table (n_chunks x n_centers f32: 32 KB at 32 x 256) that its lookups read through
         // L2: the cap of search_kernel_pq keeps them L2-resident
         if (!p.direct_cosine) max_per_sm = 6;
     } else {
-        const CodeStore& cs = s->store == STORE_SQ ? idx->sq : idx->mm;
-        p.row_codes = cs.d_codes;
-        p.row_meta = cs.d_meta;
-        p.code_stride = cs.stride;
-        p.code_dim = cs.dim;
-        p.code_nbits = cs.nbits;
-        p.code_metric = idx->metric;
-        p.sq_scale_squared = idx->sq_scale * idx->sq_scale;  // AsFunctor (scalar/quantizer.rs:316-335)
-        p.sq_shift_square_norm = idx->sq_shift_square_norm;
-        qbytes = round_up((size_t)cs.stride + 16, 16);
+        qbytes = round_up((size_t)p.code_stride + 16, 16);
     }
     void (*kern)(const PagedParams) = s->store == STORE_PQ ? paged_kernel_quant<0> : s->store == STORE_SQ ? paged_kernel_quant<1> : paged_kernel_quant<2>;
     return plan_kernel(s, kern, qbytes, max_per_sm, begin_name(s->store));
@@ -780,7 +723,8 @@ int begin_session(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_s
     if (nq == 0) return DAB_OK;
     // the reference's estimate of a search's visited set (or DAB_TEST_VISITED_LOG2), at least what the start points
     // and one expansion need; a query that outgrows it gets a larger table
-    const uint64_t slots = std::max<uint64_t>(table_slots(idx, VisitedHint{}, l_search, 1, std::max(store, 0)),
+    // (no hint is consulted, so it does not matter which store's the estimate is asked for)
+    const uint64_t slots = std::max<uint64_t>(table_slots(idx, VisitedHint{}, l_search, 1, STORE_PQ),
                                               idx->tune.test_visited_log2 ? 0 : ((uint64_t)idx->n_start + idx->max_degree) * 8 / 7 + 64);
     s->slots.assign(nq, slots);
     void* chunk = nullptr;
@@ -837,33 +781,13 @@ void paged_release(dab_index* idx) {
 
 namespace {
 
-// The checks of the synchronous calls on the store a quantized session reads (check_pq_args, search_kernel_pq.cu)
-int check_store(const dab_index* idx, int store, const char* who) {
-    int rc;
-    if (store == STORE_PQ) {
-        if (!idx->d_pivots) return fail(DAB_ERR_NOT_READY, "%s: dab_upload_pq has not been called", who);
-        if (!idx->d_codes || !idx->pq_codes_ready)
-            return fail(DAB_ERR_NOT_READY, "%s: no PQ codes (dab_upload_pq with codes, or dab_pq_encode_all)", who);
-    } else if (store == STORE_SQ) {
-        if ((rc = store_require(idx, &dab_index::sq, "dab_upload_sq", who))) return rc;
-        if (!idx->sq.ready) return fail(DAB_ERR_NOT_READY, "%s: no scalar-quantized rows (dab_upload_sq with rows, or dab_sq_encode_all)", who);
-        // SQStore::distance_computer (providers inmem/scalar.rs:214-226): UnsupportedDistanceMetric
-        if (idx->metric == DAB_COSINE)
-            return fail(DAB_ERR_INVALID_ARGUMENT, "%s: the scalar-quantized store supports L2, InnerProduct and CosineNormalized", who);
-    } else if (store == STORE_MINMAX) {
-        if ((rc = store_require(idx, &dab_index::mm, "dab_upload_minmax", who))) return rc;
-        if (!idx->mm.ready) return fail(DAB_ERR_NOT_READY, "%s: no MinMax rows (dab_upload_minmax with rows, or dab_minmax_encode_all)", who);
-    }
-    return DAB_OK;
-}
-
 // dab_paged_search_begin and its quantized forms (store: -1 full precision, else the QuantStore the traversal reads)
 int paged_begin(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search, int store, dab_paged** out) {
     const char* who = begin_name(store);
     if (!idx || !out || (nq && !queries)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", who);
     *out = nullptr;
     int rc;
-    if ((rc = check_search_args(idx, 1, l_search, 1, store < 0)) || (rc = check_store(idx, store, who))) return rc;
+    if ((rc = check_search_args(idx, 1, l_search, 1, store < 0)) || (store >= 0 && (rc = check_quant_store(idx, (QuantStore)store, who, true)))) return rc;
     if ((uint64_t)l_search + idx->n_start > 1024)
         return fail(DAB_ERR_INVALID_ARGUMENT, "%s: l_search + n_start = %llu > 1024", who, (unsigned long long)l_search + idx->n_start);
     DAB_CUDA(cudaSetDevice(idx->device));
