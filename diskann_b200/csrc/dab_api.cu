@@ -105,6 +105,7 @@ int dab_create(dab_index** out, int dtype, int metric, uint32_t dim, uint64_t n_
     idx->max_degree = max_degree;
     idx->device = device;
     cudaDeviceGetAttribute(&idx->sm_count, cudaDevAttrMultiProcessorCount, device);
+    cudaDeviceGetAttribute(&idx->l2_bytes, cudaDevAttrL2CacheSize, device);
     idx->row_stride = round_up((size_t)dim * elem_size(dtype), 32);
     idx->adj_stride = (uint32_t)round_up((size_t)max_degree + 1, 8);
     idx->h_stage.pinned_host = true;

@@ -144,6 +144,7 @@ struct dab_index {
     uint32_t max_degree = 0;
     int device = 0;
     int sm_count = 132;
+    int l2_bytes = 50 << 20;  // the device's L2 cache
 
     cudaStream_t stream = nullptr;      // stream in use
     cudaStream_t own_stream = nullptr;  // library-created

@@ -10,7 +10,7 @@
 //   * f32 rows of 32..128 elements with level 1 of the visited set on (REG): every surviving row of a hop
 //     gets one bulk L2 prefetch, then the rows are read straight into registers, 8 lanes per row and
 //     4 rows per pass (wide_distances_f32_fast, the lane mapping of search_kernel_v3); prefetches and
-//     loads both carry the evict_first policy of the staged copies;
+//     loads both carry the evict_first policy of the staged copies, unless the row store is small enough for L2 to hold;
 //   * all other rows are staged in shared memory with cp.async (16 B per lane, eight lanes per row:
 //     one warp instruction moves 128 B of four rows and no lane needs another lane's address; no
 //     registers tied up), a stage of rows in flight at once (a TMA bulk-copy variant was measured
@@ -215,9 +215,11 @@ __global__ void __launch_bounds__(kV2Warps * 32, REG ? kV2MinCtasReg : QT == 0 ?
     const uint64_t n_total = p.n_points + p.n_start;
     const int dim = (int)p.dim;
     // vector rows stream through L2 (a row is read once per query): evict them first so the
-    // visited tables, which are re-probed every hop, stay resident
+    // visited tables, which are re-probed every hop, stay resident.  REG: a row store that L2 can hold is re-read from L2
+    // by the other queries of the batch, so its rows keep the normal priority
     uint64_t row_policy;
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(row_policy));
+    if (REG && !p.rows_evict_first) asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(row_policy));
+    else asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(row_policy));
 
     for (uint32_t qidx; next_query(p.counters, p.n_work, p.query_list, lane, qidx);) {
         __syncwarp();
@@ -567,6 +569,10 @@ static int v2_prepare_schema(const dab_index* idx, uint32_t l_search, uint32_t b
     p.off_qi = (uint32_t)off;
     off += cap_pad * 4;
     p.row_bytes = row_bytes;
+    // register rows that stream through L2 are evicted first; a store of at most twice the L2 size (100K x 128 f32:
+    // 51 MB on the H100's 50 MB L2) is largely re-read from L2 and keeps the normal priority (staged rows are always
+    // evicted first: at 100K, one batch at a time measured 12 % slower with the normal priority)
+    p.rows_evict_first = idx->n_total() * idx->row_stride > 2 * (uint64_t)idx->l2_bytes;
     // rows staged per round: as many as fit ~6 KB per warp, a multiple of the reduce group
     const size_t stage_bytes = 6144;
     const uint32_t stage = std::min<uint32_t>(32, (uint32_t)std::max<size_t>(kGroup, (stage_bytes / row_bytes) / kGroup * kGroup));

@@ -45,6 +45,7 @@ struct SearchParamsV2 {
     uint32_t row_bytes;   // bytes copied per row (multiple of 16)
     uint32_t row_slot;    // bytes between staged rows (staged rows only, as off_rows)
     uint32_t stage_rows;  // rows staged per round (multiple of kGroup; staged rows only)
+    uint32_t rows_evict_first;  // register rows read with the L2 evict_first policy (else evict_normal; staged rows: always)
 };
 
 struct V2Launch {
