@@ -14,6 +14,7 @@
 //     (index.rs:2264-2341) -> robust_prune_list (index.rs:2397-2454).
 #include "dab_common.cuh"
 #include "distance_device.cuh"
+#include "search_host.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
 
@@ -22,10 +23,6 @@
 #include <vector>
 
 namespace dab {
-
-int run_search(dab_index* idx, const void* d_queries, const uint32_t* d_query_rows, uint32_t nq, uint32_t k,
-               uint32_t l_search, uint32_t beam, uint32_t* d_ids, float* d_dists, uint32_t* d_counts, uint32_t* d_cmps,
-               uint32_t* d_hops, uint32_t* rec_ids, float* rec_dists, uint32_t* rec_counts, uint32_t rec_cap);
 
 constexpr int kPruneWarps = 4;
 constexpr uint32_t kMaxOcclusion = 750;  // graph/config/defaults.rs:13
@@ -749,9 +746,7 @@ int dab_consolidate(dab_index* idx, uint32_t pruned_degree, float alpha, uint64_
     rc = visit_schema<OPS_ROW>(idx->dtype, idx->metric, [&](auto s) -> int {
         using S = decltype(s);
         auto kern = consolidate_kernel<KernelRow<S>, S::NA, S::KIND, S::POST, S::IS_INT, S::SIGNED>;
-        DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int per_sm = 0;
-        DAB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kPruneWarps * 32, smem));
+        const int per_sm = ctas_per_sm(kern, kPruneWarps * 32, smem);
         // every resident warp, within 2 GB of tables and pools
         uint64_t blocks = std::max(1, per_sm) * (uint64_t)idx->sm_count;
         blocks = std::max<uint64_t>(1, std::min<uint64_t>(blocks, (2ull << 30) / (warp_bytes * kPruneWarps)));
@@ -814,6 +809,7 @@ int dab_build(dab_index* idx, uint32_t pruned_degree, uint32_t l_build, float al
                                     (uint32_t*)b_vals2.p, (int)(B * pruned_degree), 0, 32, st);
     if ((rc = b_tmp.alloc(tmp_bytes))) return rc;
 
+    const SearchRecord rec{(const uint32_t*)b_batch.p, (uint32_t*)b_rec_ids.p, (float*)b_rec_d.p, (uint32_t*)b_rec_n.p, rec_cap};
     uint32_t inserted = 0;
     while (inserted < n) {
         // batches grow with the graph so that early points are not all inserted blind
@@ -822,8 +818,8 @@ int dab_build(dab_index* idx, uint32_t pruned_degree, uint32_t l_build, float al
         iota_kernel<<<(b + 255) / 256, 256, 0, st>>>((uint32_t*)b_batch.p, inserted, b);
         DAB_LAUNCHED();
         // 1. search the batch against the current graph, recording expanded nodes
-        if ((rc = run_search(idx, nullptr, (const uint32_t*)b_batch.p, b, 1, l_build, 1, (uint32_t*)b_res_ids.p, (float*)b_res_d.p,
-                             nullptr, nullptr, nullptr, (uint32_t*)b_rec_ids.p, (float*)b_rec_d.p, (uint32_t*)b_rec_n.p, rec_cap)))
+        if ((rc = run_search(idx, nullptr, b, 1, l_build, 1, SearchOut{(uint32_t*)b_res_ids.p, (float*)b_res_d.p, nullptr, nullptr, nullptr},
+                             -1, false, &rec)))
             return rc;
         // 2. robust_prune each point's visited pool -> out-edges
         PruneParams pp;

@@ -67,6 +67,19 @@ inline size_t elem_size(int dtype) {
 }
 inline size_t round_up(size_t x, size_t m) { return (x + m - 1) / m * m; }
 
+// CTAs of `threads` threads with `smem` B of dynamic shared memory (the kernel's attribute is set to it) that one SM holds
+// at once; 0 when the kernel does not fit, with the CUDA error cleared so that the caller reports its own
+template <class P>
+int ctas_per_sm(void (*kern)(P), int threads, size_t smem) {
+    int per_sm = 0;
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem) != cudaSuccess) {
+        cudaGetLastError();
+        return 0;
+    }
+    return per_sm;
+}
+
 // A grow-only device (or pinned host) scratch buffer.
 struct Scratch {
     void* p = nullptr;

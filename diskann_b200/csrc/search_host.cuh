@@ -1,10 +1,10 @@
-// search_host.cuh — the host protocol of full-precision and quantized graph search (defined in search_kernel.cu): argument
-// checks, the size of the per-warp visited tables in global memory, re-runs of the queries that outgrow them, host buffers.
+// search_host.cuh — the host side every graph search shares (defined in search_kernel.cu): argument checks, the size of
+// the per-warp visited tables in global memory, the parameter fields every traversal takes from the index, the one-shot
+// search batch and the slots of batches in flight.
 #pragma once
 
 #include "dab_common.cuh"
 
-#include <functional>
 #include <type_traits>
 
 namespace dab {
@@ -16,12 +16,8 @@ int check_search_args(const dab_index* idx, uint32_t k, uint32_t l_search, uint3
 // Ids a warp's visited table holds in the first global-table pass at (L, beam, mode): the reference's estimate, or less
 // where `hint` has seen the visited sets of this (or a larger) L and beam.  A default VisitedHint is no hint.
 uint64_t table_slots(const dab_index* idx, const VisitedHint& hint, uint32_t l_search, uint32_t beam, QuantStore mode);
-// `hint` takes in the largest visited set of a pass at (L, beam, mode)
-void learn_visited(VisitedHint& hint, uint32_t l_search, uint32_t beam, QuantStore mode, uint32_t visited);
 // After a global-table pass `pass` that overflowed: the table of the next one, or DAB_ERR_VISITED_OVERFLOW after six
 int grow_visited_tables(const dab_index* idx, int& pass, uint64_t& slots);
-// The `n_over` query ids a pass reported at `d_overflow` become the work list of the next pass, in `retry`
-int take_overflow_list(cudaStream_t stream, const uint32_t* d_overflow, uint32_t n_over, Scratch& retry);
 
 // The grid of a pass of persistent one-query warps over n_work queries, where resident_ctas CTAs of warps_per_cta warps
 // fit the device: every resident warp runs the same number of queries (10K queries on 3108 resident warps would
@@ -47,6 +43,39 @@ auto visit_list_tile(uint32_t cap, F&& f) {
 // `upload_first`: a store that was never set up is reported as "<upload call> has not been called" (the paged calls)
 // instead of as missing codes or rows (the batch calls).
 int check_quant_store(const dab_index* idx, QuantStore store, const char* who, bool upload_first);
+
+// The graph fields every traversal's parameter block (SearchParamsV2, SearchParamsV3, SearchParamsPq, PagedParams) takes
+// from the index
+template <class P>
+void set_graph_params(const dab_index* idx, P& p) {
+    p.adj = idx->d_adj;
+    p.adj_stride = idx->adj_stride;
+    p.n_points = idx->n_points;
+    p.n_start = idx->n_start;
+    p.dim = idx->dim;
+    p.max_degree = idx->max_degree;
+}
+
+// The 16-bit quotient tags of a visited table in shared memory (Tag16Map, search_common.cuh) cover ids < 2^K
+inline uint32_t tag_id_bits(uint64_t n_total) {
+    uint32_t K = 8;
+    while (((uint64_t)1 << K) < n_total) ++K;
+    return K;
+}
+// The tag map of a table of `n_buckets` buckets of 16 tags over this index's ids into p.tag_kmask / tag_shift / tag_magic;
+// false (nothing set) when a tag, the id's quotient by n_buckets, needs more than 14 bits or the id and its bucket more
+// than 32
+template <class P>
+bool set_tag_map(const dab_index* idx, uint64_t n_buckets, P& p) {
+    const uint32_t K = tag_id_bits(idx->n_total());
+    uint32_t sbits = 0;
+    while (((uint64_t)1 << sbits) < n_buckets) ++sbits;
+    if (((((uint64_t)1 << K) + 16383) >> 14) > n_buckets || K + sbits > 32) return false;
+    p.tag_kmask = (uint32_t)(((uint64_t)1 << K) - 1);
+    p.tag_shift = K + sbits;
+    p.tag_magic = (uint32_t)((((uint64_t)1 << (K + sbits)) + n_buckets - 1) / n_buckets);
+    return true;
+}
 
 // The fields a quantized traversal's parameter block (SearchParamsPq, PagedParams) takes from the store it reads
 template <class P>
@@ -87,21 +116,25 @@ struct SearchOut {
 int queue_drop_deleted(const dab_index* idx, cudaStream_t stream, const uint32_t* deleted, const uint32_t* ids, const float* dists,
                        uint32_t cap, uint32_t nq, uint32_t k, const SearchOut& out);
 
-// The synchronous host-buffer calls: checks the buffers, copies the queries to the handle's scratch, runs `run` on them
-// with device result buffers, copies the results to `out` and waits.  `api` names the entry point in error messages.
-int search_host_buffers(dab_index* idx, const char* api, const void* queries, uint32_t nq, uint32_t k, const SearchOut& out,
-                        const std::function<int(const void* d_queries, const SearchOut& d_out)>& run);
+// The build's insert searches: the queries are rows of the index, and each records the nodes it expanded
+struct SearchRecord {
+    const uint32_t* query_rows;  // [nq] row ids of the queries
+    uint32_t* ids;               // [nq][cap] expanded nodes, [nq] counts
+    float* dists;
+    uint32_t* counts;
+    uint32_t cap;
+};
+
+// One batch on the handle's stream and scratch, device pointers only.  `store`: -1 full precision, else the QuantStore the
+// traversal reads; `rerank` (quantized) reorders each list by full-precision distances.  Returns once the traversal is
+// complete; a full-precision batch also has its deleted ids filtered, while a quantized batch's rerank or filter may still
+// run.  `rec` (full precision): the build's insert searches, which ignore deletions and teach the visited tables nothing.
+int run_search(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam, const SearchOut& d,
+               int store, bool rerank, const SearchRecord* rec = nullptr);
 
 // ---- batches in flight ---------------------------------------------------------------------------------------------
-// A batch of any kind (full precision, PQ, SQ, MinMax) as a resumable job.  `launch` queues all of it and waits for
-// nothing; `finish` waits for it, re-runs the queries that outgrew their visited tables and sets `reran` when it did
-// (their results were then written again after the first copies were queued).
-struct SlotJob {
-    bool reran = false;
-    virtual ~SlotJob() = default;
-    virtual int launch() = 0;
-    virtual int finish() = 0;
-};
+// A batch of any kind (full precision, PQ, SQ, MinMax) as a resumable job (search_kernel.cu)
+struct SlotJob;
 
 // A host-buffer call's results: where the kernels write them and where the caller wants them
 struct HostCopy {
@@ -119,13 +152,5 @@ struct SearchSlot {
     SlotJob* job = nullptr;
     HostCopy host_out{};  // the pending call's result copies (host_out.host.ids null: device buffers)
 };
-
-// The launching half of every *_async call.  Checks the slot (in range, no batch in flight); nq == 0 is then a no-op.
-// A host-buffer call (`host`) gets device buffers in the slot's scratch.  `prepare` builds the job on the slot's stream and
-// scratch with every check the synchronous call makes before it launches, reserves the buffers and queues nothing; then
-// the copy of the queries, the job's launch and the copies of the results are queued, and the call returns without
-// waiting.  (Should a launch fail with a CUDA error half way, what it queued completes before the error is returned.)
-int slot_submit(dab_index* idx, const char* api, uint32_t slot, bool host, const void* queries, uint32_t nq, uint32_t k,
-                const SearchOut& out, const std::function<int(SearchSlot* s, const void* d_queries, const SearchOut& d_out, SlotJob** job)>& prepare);
 
 }  // namespace dab

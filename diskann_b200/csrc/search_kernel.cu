@@ -1,14 +1,15 @@
-// search_kernel.cu — the host side of batched graph search: the visited-table policy, the overflow re-runs and the
-// host-buffer calls every search shares (search_host.cuh), the full-precision dispatcher, the slots of batches in flight
-// (which the quantized *_async calls of search_kernel_pq.cu share) and the C entry points (dab_search_batch[_device][_async],
-// dab_wait).
+// search_kernel.cu — the host side of batched graph search: the visited-table policy, the one job that runs a batch of
+// any kind with its overflow re-runs and post-processing (full precision; PQ, SQ and MinMax, whose kernels and rerank
+// are in search_kernel_pq.cu and search_kernel_pqs.cu), the slots of batches in flight and the C entry points
+// (dab_search_batch[_pq|_pq_rerank|_sq|_minmax][_device][_async], dab_wait).
 //
-// A batch runs on search_kernel_v3 (visited set in shared memory) where its short lists make that the faster kernel,
-// and on search_kernel_v2 (global visited tables) otherwise; queries whose visited set outgrows its table are re-run
-// on v2 with larger tables, so membership stays exact.  Both kernels restate DiskANNIndex::search_internal
+// A full-precision batch runs on search_kernel_v3 (visited set in shared memory) where its short lists make that the
+// faster kernel, and on search_kernel_v2 (global visited tables) otherwise; queries whose visited set outgrows its table
+// are re-run on v2 with larger tables, so membership stays exact.  Both kernels restate DiskANNIndex::search_internal
 // (index.rs:1933-2000) bit for bit.
 #include "dab_common.cuh"
 #include "search_host.cuh"
+#include "search_pq.cuh"
 #include "search_v2.cuh"
 #include "search_v3.cuh"
 
@@ -41,7 +42,8 @@ uint64_t table_slots(const dab_index* idx, const VisitedHint& hint, uint32_t l_s
     return std::max<uint64_t>(256, (uint64_t)est + 1);
 }
 
-void learn_visited(VisitedHint& hint, uint32_t l_search, uint32_t beam, QuantStore mode, uint32_t visited) {
+// `hint` takes in the largest visited set of a pass at (L, beam, mode)
+static void learn_visited(VisitedHint& hint, uint32_t l_search, uint32_t beam, QuantStore mode, uint32_t visited) {
     if (l_search != hint.l || beam != hint.beam || mode != hint.mode) hint = VisitedHint{l_search, beam, 0, mode};
     hint.visited = std::max(hint.visited, visited);
 }
@@ -74,7 +76,8 @@ int grow_visited_tables(const dab_index* idx, int& pass, uint64_t& slots) {
     return DAB_OK;
 }
 
-int take_overflow_list(cudaStream_t stream, const uint32_t* d_overflow, uint32_t n_over, Scratch& retry) {
+// The `n_over` query ids a pass reported at `d_overflow` become the work list of the next pass, in `retry`
+static int take_overflow_list(cudaStream_t stream, const uint32_t* d_overflow, uint32_t n_over, Scratch& retry) {
     // the pass that wrote the list is complete, so `retry` (its own work list, or empty) can be overwritten
     int rc;
     if ((rc = retry.reserve((size_t)n_over * 4))) return rc;
@@ -83,196 +86,364 @@ int take_overflow_list(cudaStream_t stream, const uint32_t* d_overflow, uint32_t
     return DAB_OK;
 }
 
-// ---- one batch of searches as a resumable job ------------------------------------------------
-// A batch is launched (`launch`: kernel + read-back of the four counters into pinned memory, nothing
-// waits) and later completed (`finish`: waits, learns the visited-set size, re-runs the few queries
-// whose visited set outgrew its table).  The synchronous entry points run launch + finish on the
-// handle's stream; dab_search_batch_async / dab_wait keep several batches in flight on slot-owned
-// streams so the tail of one batch (workers running out of queries) is filled by the next batch's
-// CTAs and the host<->device copies of neighbouring batches overlap the kernel.
-struct SearchJob : SlotJob {
-    dab_index* idx = nullptr;
-    cudaStream_t stream = nullptr;
-    Scratch* tables = nullptr;
-    Scratch* counters = nullptr;
-    Scratch* lists = nullptr;        // the whole lists, while deleted ids are filtered
-    uint32_t* h_counters = nullptr;  // pinned, 4 words
-    bool full_grid = false;          // batches in flight: launch every resident worker (the next batch fills what this one leaves)
 
-    uint32_t nq = 0, l_search = 0, beam = 0;
-    bool recording = false;
-    // some id is deleted: the traversal writes every non-start entry of a list (k = L + #start) to `lists`, and each
-    // pass is followed by the filter into `filtered`, the caller's buffers
+// The checks of a batch that need no plan: the arguments and, for a quantized traversal, the store, its metric and the
+// list length
+static int check_batch_args(const dab_index* idx, uint32_t k, uint32_t l_search, uint32_t beam, int store) {
+    if (store < 0) return check_search_args(idx, k, l_search, beam);
+    const QuantStore mode = (QuantStore)store;
+    // every entry point of a store reports under its synchronous host-buffer call's name
+    const char* who = mode == STORE_PQ ? "dab_search_batch_pq" : mode == STORE_SQ ? "dab_search_batch_sq" : "dab_search_batch_minmax";
+    int rc;
+    if ((rc = check_search_args(idx, k, l_search, beam, false)) || (rc = check_quant_store(idx, mode, who, false))) return rc;
+    if (l_search + idx->n_start > 1024)
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: L + #start must be <= 1024", mode == STORE_MINMAX ? "dab_search_batch_minmax" : "dab_search_batch_pq");
+    return DAB_OK;
+}
+
+// ---- one batch as a resumable job ------------------------------------------------------------------------------------
+// `prepare` plans the batch (check_batch_args has passed), makes the checks of the plan and reserves every buffer the
+// first pass needs; nothing is queued.  `launch` queues all of the batch and waits for nothing: the staging of the
+// queries (SQ, MinMax), the first pass with the read-back of its counters into pinned memory and, optimistically, the
+// post-processing (the rerank, or the filter of deleted ids).  `finish` waits for the counters, learns the visited-set
+// size, re-runs the queries whose visited set outgrew its table on larger tables and then queues the post-processing of
+// the whole batch again; `reran` says it did (the results were written again after the first copies were queued).
+// The synchronous calls run the job on the handle's stream and scratch.  The *_async calls keep several batches in
+// flight on slot-owned streams, so that the tail of one batch (workers running out of queries) is filled by the next
+// batch's CTAs and the host<->device copies of neighbouring batches overlap the kernel.  A re-run of a quantized batch
+// reads the store the batch was planned on: if that store was replaced since (retire_quantized_stores), finish fails.
+struct SlotJob {
+    dab_index* idx;
+    cudaStream_t stream;
+    Scratch *tables, *counters, *stage, *luts, *lists, *pinned;
+    bool full_grid = false;  // full precision, batches in flight: launch every resident worker (the next batch fills what this one leaves)
+
+    int store = -1;  // -1: full precision, else the QuantStore the traversal reads
+    bool rerank = false;
+    const void* d_queries = nullptr;
+    uint32_t nq = 0, k = 0, l_search = 0, beam = 0, cap = 0;
+    SearchRecord rec{};  // the build's insert searches (rec.ids set)
+    // some id is deleted: a rerank drops deleted ids itself; without one (`filter`) the traversal writes every non-start
+    // entry of a list (k = L + #start) to `lists` and the filter takes the first k live ones into `filtered`, the caller's
+    // buffers
     const uint32_t* deleted = nullptr;
-    SearchOut filtered{};
-    uint32_t k_out = 0;
+    bool filter = false;
+    SearchOut out{}, filtered{};  // `out`: where the traversal writes
+    uint32_t *d_counters = nullptr, *d_overflow = nullptr;
+    uint32_t* h_counters = nullptr;  // pinned: the four counters of a pass, then (u64 at word 4) the MinMax NaN flag
+    cudaEvent_t counted = nullptr;   // recorded after the read-back of a pass's counters
+    uint64_t stores_version = 0;     // idx->stores_version when the batch was planned
+    // global-table passes: the n_work queries of `work` (NULL: the whole batch), a visited table of `slots` ids for each
+    // of `warps` resident warps; the overflowed queries of one pass are re-run on larger tables in the next
+    const uint32_t* work = nullptr;
+    uint32_t n_work = 0, warps = 0, n_buckets = 0;
+    uint64_t slots = 0;
+    int pass = 0;
+    Scratch retry;
+    bool reran = false;
+
+    // full precision
     SearchParamsV2 p2;
     SearchParamsV3 p3;
     V2Launch v2;
     V3Launch v3;
-    uint64_t slots = 0;
-    int stage = 1;  // 0: search_kernel_v3 pass in flight, 1: global-table pass in flight
-    int pass = 0;
-    Scratch retry_list;
-    uint32_t *d_counters = nullptr, *d_overflow = nullptr;
+    bool on_v3 = false;  // the first pass runs on search_kernel_v3
+    // quantized
+    SearchParamsPq pq;
+    PqsPlan plan;
+    bool use_pqs = false;
+    PqKernel kern = nullptr;
+    int grid = 0;
+    size_t smem_block = 0;
 
-    int prepare(const void* d_queries, const uint32_t* d_query_rows, uint32_t nq_, uint32_t k, uint32_t l_search_, uint32_t beam_,
-                uint32_t* d_ids, float* d_dists, uint32_t* d_counts, uint32_t* d_cmps, uint32_t* d_hops, uint32_t* rec_ids,
-                float* rec_dists, uint32_t* rec_counts, uint32_t rec_cap);
-    int launch() override;
-    int finish() override;
-    ~SearchJob() override { retry_list.release(); }
+    SlotJob(dab_index* idx_, cudaStream_t stream_, Scratch& tables_, Scratch& counters_, Scratch& stage_, Scratch& luts_,
+            Scratch& lists_, Scratch& pinned_)
+        : idx(idx_), stream(stream_), tables(&tables_), counters(&counters_), stage(&stage_), luts(&luts_), lists(&lists_), pinned(&pinned_) {}
+    ~SlotJob() {
+        retry.release();
+        if (counted) cudaEventDestroy(counted);
+    }
+
+    int prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint32_t l_search_, uint32_t beam_, const SearchOut& d, int store_,
+                bool rerank_, const SearchRecord* rec_);
+    int launch() {
+        int rc;
+        if ((rc = stage_queries()) || (rc = launch_pass())) return rc;
+        return post();
+    }
+    int finish();
+
+    int plan_full();
+    int plan_quant();
+    int reserve_tables();
+    int stage_queries();
+    int launch_pass();
+    int launch_full();
+    int launch_quant();
+    int post();
+
+    // full precision keeps STORE_PQ in a hint of its own
+    VisitedHint& hint() const { return store < 0 ? idx->hint : idx->pq_hint; }
+    QuantStore mode() const { return store < 0 ? STORE_PQ : (QuantStore)store; }
+    unsigned long long first_nan() const { return *(const unsigned long long*)(h_counters + 4); }
+    int nan_error() const {
+        return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_minmax: query %llu contains NaN after the transform (InputContainsNaN)", first_nan());
+    }
+
+    // the fields of a parameter block that every traversal's pass has
+    template <class P>
+    void set_batch_params(P& p) const {
+        set_graph_params(idx, p);
+        p.queries = d_queries;
+        p.n_work = nq;
+        p.k = filter ? cap : k;
+        p.cap = cap;
+        p.beam = beam;
+        p.out_ids = out.ids, p.out_dists = out.dists, p.out_counts = out.counts, p.out_cmps = out.cmps, p.out_hops = out.hops;
+        p.counters = d_counters;
+        p.overflow_list = d_overflow;
+    }
+    // ... and those of search_kernel_v2 and _v3
+    template <class P>
+    void set_full_params(P& p) const {
+        set_batch_params(p);
+        p.vectors = idx->d_vectors;
+        p.row_stride = idx->row_stride;
+        p.query_rows = rec.query_rows;
+        p.rec_ids = rec.ids, p.rec_dists = rec.dists, p.rec_counts = rec.counts, p.rec_cap = rec.cap;
+    }
+    // a global-table pass: its work list and tables
+    template <class P>
+    void set_pass_params(P& p) const {
+        p.query_list = work;
+        p.n_work = n_work;
+        p.tables = (uint32_t*)tables->p;
+        p.n_buckets = n_buckets;
+    }
 };
 
-int SearchJob::prepare(const void* d_queries, const uint32_t* d_query_rows, uint32_t nq_, uint32_t k, uint32_t l_search_,
-                       uint32_t beam_, uint32_t* d_ids, float* d_dists, uint32_t* d_counts, uint32_t* d_cmps, uint32_t* d_hops,
-                       uint32_t* rec_ids, float* rec_dists, uint32_t* rec_counts, uint32_t rec_cap) {
-    nq = nq_, l_search = l_search_, beam = beam_;
-    recording = rec_ids != nullptr;
-
+int SlotJob::prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint32_t l_search_, uint32_t beam_, const SearchOut& d,
+                     int store_, bool rerank_, const SearchRecord* rec_) {
+    d_queries = d_queries_, nq = nq_, k = k_, l_search = l_search_, beam = beam_, store = store_, rerank = rerank_;
+    if (rec_) rec = *rec_;
+    stores_version = idx->stores_version;
+    cap = l_search + idx->n_start;  // scratch.rs:195-208
     int rc;
-    // the build's insert searches ignore deletions, as the reference's insert does
-    deleted = recording ? nullptr : deleted_filter(idx);
-    if (deleted) {
-        const size_t cap = (size_t)l_search + idx->n_start;
-        if ((rc = lists->reserve((size_t)nq * cap * 8))) return rc;
-        filtered = SearchOut{d_ids, d_dists, d_counts, d_cmps, d_hops};
-        k_out = k;
-        k = (uint32_t)cap;
-        d_ids = (uint32_t*)lists->p;
-        d_dists = (float*)(d_ids + (size_t)nq * cap);
-    }
-    memset(&p2, 0, sizeof(p2));
-    if ((rc = v2_prepare(idx, l_search, beam, full_grid, p2, v2))) return rc;
-    p2.vectors = idx->d_vectors;
-    p2.row_stride = idx->row_stride;
-    p2.adj = idx->d_adj;
-    p2.adj_stride = idx->adj_stride;
-    p2.n_points = idx->n_points;
-    p2.n_start = idx->n_start;
-    p2.dim = idx->dim;
-    p2.max_degree = idx->max_degree;
-    p2.queries = d_queries;
-    p2.query_rows = d_query_rows;
-    p2.k = k;
-    p2.cap = l_search + idx->n_start;  // scratch.rs:195-208
-    p2.beam = beam;
-    p2.out_ids = d_ids;
-    p2.out_dists = d_dists;
-    p2.out_counts = d_counts;
-    p2.out_cmps = d_cmps;
-    p2.out_hops = d_hops;
-    p2.rec_ids = rec_ids;
-    p2.rec_dists = rec_dists;
-    p2.rec_counts = rec_counts;
-    p2.rec_cap = rec_cap;
-
-    slots = table_slots(idx, idx->hint, l_search, beam, STORE_PQ);
-    if ((rc = counters->reserve(16 + (size_t)nq * 4))) return rc;
+    if ((rc = pinned->reserve(24)) || (rc = counters->reserve(16 + (size_t)nq * 4))) return rc;
+    h_counters = (uint32_t*)pinned->p;
     d_counters = (uint32_t*)counters->p;
     d_overflow = d_counters + 4;
-    p2.counters = d_counters;
-    p2.overflow_list = d_overflow;
-    p2.n_work = nq;
-    p2.query_list = nullptr;
-
-    // first pass with the visited sets in shared memory (search_kernel_v3) where it is the faster
-    // kernel; queries that outgrow their table are re-run on global tables
-    stage = 1;
-    pass = 0;
-    const uint32_t need = idx->tune.test_visited_log2 ? (1u << idx->tune.test_visited_log2) / 2 : 0;  // tests: tables that overflow
-    const bool skip = idx->v3_overflow_l == l_search && idx->v3_overflow_beam == beam && idx->v3_overflow_frac > 0.25f;
-    memset(&p3, 0, sizeof(p3));
-    if (!skip && v3_prepare(idx, l_search, beam, need, p3, v3) == 0) {
-        stage = 0;
-        p3.vectors = p2.vectors, p3.row_stride = p2.row_stride, p3.adj = p2.adj, p3.adj_stride = p2.adj_stride;
-        p3.n_points = p2.n_points, p3.n_start = p2.n_start, p3.dim = p2.dim, p3.max_degree = p2.max_degree;
-        p3.queries = p2.queries, p3.query_rows = p2.query_rows, p3.query_list = nullptr, p3.n_work = nq;
-        p3.k = p2.k, p3.cap = p2.cap, p3.beam = p2.beam;
-        p3.out_ids = p2.out_ids, p3.out_dists = p2.out_dists, p3.out_counts = p2.out_counts;
-        p3.out_cmps = p2.out_cmps, p3.out_hops = p2.out_hops;
-        p3.rec_ids = p2.rec_ids, p3.rec_dists = p2.rec_dists, p3.rec_counts = p2.rec_counts, p3.rec_cap = p2.rec_cap;
-        p3.counters = d_counters, p3.overflow_list = d_overflow;
+    out = d;
+    // the build's insert searches ignore deletions, as the reference's insert does
+    deleted = rec.ids ? nullptr : deleted_filter(idx);
+    filter = deleted && !rerank;
+    if (filter) {
+        if ((rc = lists->reserve((size_t)nq * cap * 8))) return rc;
+        filtered = d;
+        out.ids = (uint32_t*)lists->p;
+        out.dists = (float*)(out.ids + (size_t)nq * cap);
     }
+    n_work = nq;
+    slots = table_slots(idx, hint(), l_search, beam, mode());
+    if ((rc = store < 0 ? plan_full() : plan_quant())) return rc;
+    if (!on_v3 && (rc = reserve_tables())) return rc;
+    DAB_CUDA(cudaEventCreateWithFlags(&counted, cudaEventDisableTiming));
     return DAB_OK;
 }
 
-// launch the pass of the current stage and queue the read-back of its counters
-int SearchJob::launch() {
+// full precision: search_kernel_v2's plan, and search_kernel_v3's for the first pass where it is the faster kernel
+int SlotJob::plan_full() {
+    int rc;
+    memset(&p2, 0, sizeof(p2));
+    if ((rc = v2_prepare(idx, l_search, beam, full_grid, p2, v2))) return rc;
+    set_full_params(p2);
+    warps = (uint32_t)v2.grid * kV2Warps;
+    // queries that outgrow their table in search_kernel_v3 are re-run on global tables; v3 is skipped where most did so
+    const uint32_t need = idx->tune.test_visited_log2 ? (1u << idx->tune.test_visited_log2) / 2 : 0;  // tests: tables that overflow
+    const bool skip = idx->v3_overflow_l == l_search && idx->v3_overflow_beam == beam && idx->v3_overflow_frac > 0.25f;
+    memset(&p3, 0, sizeof(p3));
+    on_v3 = !skip && v3_prepare(idx, l_search, beam, need, p3, v3) == 0;
+    if (on_v3) set_full_params(p3);
+    return DAB_OK;
+}
+
+// PQ, SQ and MinMax: the shared-memory layout, search_kernel_pqs's plan or search_kernel_pq's grid, and the LUTs, rerank
+// lists and query staging
+int SlotJob::plan_quant() {
+    const QuantStore mode = (QuantStore)store;
+    memset(&pq, 0, sizeof(pq));
+    set_batch_params(pq);
+    pq.dtype = idx->dtype;
+    set_store_params(idx, mode, pq);
+
+    size_t off = 0;
+    pq.off_q = 0;
+    off += round_up((size_t)idx->dim * 4, 16);
+    const size_t cap_pad = round_up(cap, 32) + 32;
+    pq.off_qd = (uint32_t)off;
+    off += cap_pad * 4;
+    pq.off_qi = (uint32_t)off;
+    off += cap_pad * 4;
+    const size_t ncand_max = std::max<size_t>((size_t)beam * idx->max_degree, idx->n_start);
+    pq.off_cid = (uint32_t)off;
+    off += round_up(ncand_max * 4, 16);
+    pq.off_cd = (uint32_t)off;
+    off += round_up(ncand_max * 4, 16);
+    pq.off_beam = (uint32_t)off;
+    off += round_up((size_t)beam * 4, 16);
+    pq.off_qc = (uint32_t)off;
+    if (mode == STORE_SQ) off += pq.code_stride;
+    if (mode == STORE_MINMAX) off += pq.code_stride + 16;  // the query's code row and its four compensations
+    off = round_up(off, 16);
+    pq.off_nrow = (uint32_t)off;  // search_kernel_pqs: the adjacency row copied one hop ahead
+    if (mode == STORE_PQ) off += 96 * 4;
+    pq.warp_smem = (uint32_t)round_up(off, 16);
+    // table metrics with a pivot table that fits shared memory: search_kernel_pqs (pivots resident per SM, entries
+    // computed on the fly); everything else — SQ, MinMax, DirectCosine, wide pivots, > 32 chunks — search_kernel_pq
+    memset(&plan, 0, sizeof(plan));
+    use_pqs = mode == STORE_PQ && !pq.direct_cosine && pqs_plan(idx, pq.warp_smem, nq, &plan);
+    smem_block = (size_t)pq.warp_smem * kPqWarps;
+    if (use_pqs) {
+        pq.piv_stride = plan.piv_stride;
+        pq.piv_bytes = plan.piv_bytes;
+        grid = plan.grid;
+        warps = (uint32_t)plan.grid * (uint32_t)plan.warps;
+    } else {
+        if (smem_block > 200 * 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_pq: configuration needs %zu B shared memory per CTA", smem_block);
+        kern = pq_kernel(cap, mode);
+        int per_sm = ctas_per_sm(kern, kPqWarps * 32, smem_block);
+        if (per_sm < 1) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_pq: kernel does not fit");
+        // every resident warp owns a LUT (n_chunks x n_centers f32: 32 KB at 32 x 256) and a visited table in
+        // global memory; ADC terms and probes are L2 hits only while all of them stay L2-resident
+        // (the SQ kernel has no LUT: it keeps the occupancy the shared memory allows)
+        if (mode == STORE_PQ) per_sm = std::min(per_sm, 6);
+        grid = (int)std::min<uint64_t>((uint64_t)per_sm * idx->sm_count, ((uint64_t)nq + kPqWarps - 1) / kPqWarps);
+        warps = (uint32_t)grid * kPqWarps;
+    }
+
+    int rc;
+    const size_t lut_bytes = mode == STORE_PQ && !use_pqs ? (size_t)warps * idx->pq_chunks * idx->pq_centers * 4 : 16;
+    if ((rc = luts->reserve(lut_bytes))) return rc;
+    pq.luts = (float*)luts->p;
+    if (rerank) {
+        if (!idx->vectors_ready) return fail(DAB_ERR_NOT_READY, "dab_search_batch_pq: rerank needs the full-precision vectors");
+        if ((rc = check_rerank(idx, cap))) return rc;
+        if ((rc = lists->reserve(((size_t)nq * cap + nq) * 4))) return rc;
+        pq.list_ids = (uint32_t*)lists->p;
+        pq.list_counts = pq.list_ids + (size_t)nq * cap;
+        pq.list_cap = cap;
+    }
+    return stage->reserve(mode == STORE_SQ ? sq_stage_bytes(idx, nq) : mode == STORE_MINMAX ? minmax_stage_bytes(idx, nq) : 0);
+}
+
+// a visited table of `slots` ids, in whole 32-byte buckets of 8 ids, for every resident warp
+int SlotJob::reserve_tables() {
+    n_buckets = (uint32_t)((slots + 7) / 8);
+    return tables->reserve((size_t)warps * n_buckets * 32);
+}
+
+// SQ and MinMax: the batch's queries compressed by the store's quantizer (MinMax: the NaN flag read back into h_counters)
+int SlotJob::stage_queries() {
+    if (store == STORE_SQ) return sq_stage_queries(idx, stream, *stage, d_queries, nq, &pq.query_codes, &pq.query_meta);
+    if (store == STORE_MINMAX)
+        return minmax_stage_queries(idx, stream, *stage, d_queries, nq, (unsigned long long*)(h_counters + 4), &pq.query_codes, &pq.query_meta);
+    return DAB_OK;
+}
+
+// one traversal pass over the queries of `work` (tables reserved) and the read-back of its counters
+int SlotJob::launch_pass() {
     DAB_CUDA(cudaMemsetAsync(d_counters, 0, 16, stream));
-    if (stage == 0) {
+    int rc;
+    if ((rc = store < 0 ? launch_full() : launch_quant())) return rc;
+    DAB_CUDA(cudaMemcpyAsync(h_counters, d_counters, 16, cudaMemcpyDeviceToHost, stream));
+    DAB_CUDA(cudaEventRecord(counted, stream));
+    return DAB_OK;
+}
+
+int SlotJob::launch_full() {
+    if (on_v3) {
         v3.kern<<<balanced_grid(nq, v3.grid, kV3Warps), kV3Warps * 32, v3.smem_block, stream>>>(p3);
     } else {
-        // a visited table per warp: `slots` rounded up to whole 32-byte buckets of 8 ids
-        const uint32_t n_buckets = (uint32_t)((slots + 7) / 8);
-        int rc;
-        if ((rc = tables->reserve((size_t)v2.grid * kV2Warps * n_buckets * 32))) return rc;
-        p2.tables = (uint32_t*)tables->p;
-        p2.n_buckets = n_buckets;
-        int launch_grid = balanced_grid(p2.n_work, v2.grid, kV2Warps);
-        if (full_grid) launch_grid = (int)std::min<uint64_t>((uint64_t)v2.grid, ((uint64_t)p2.n_work + kV2Warps - 1) / kV2Warps);
+        set_pass_params(p2);
+        int launch_grid = balanced_grid(n_work, v2.grid, kV2Warps);
+        if (full_grid) launch_grid = (int)std::min<uint64_t>((uint64_t)v2.grid, ((uint64_t)n_work + kV2Warps - 1) / kV2Warps);
         v2.kern<<<launch_grid, kV2Warps * 32, v2.smem_block, stream>>>(p2);
     }
     DAB_LAUNCHED();
     DAB_CUDA(cudaGetLastError());
-    // the whole batch: a re-run pass rewrote some of the lists
-    int rc;
-    if (deleted && (rc = queue_drop_deleted(idx, stream, deleted, p2.out_ids, p2.out_dists, p2.cap, nq, k_out, filtered))) return rc;
-    DAB_CUDA(cudaMemcpyAsync(h_counters, d_counters, 16, cudaMemcpyDeviceToHost, stream));
     return DAB_OK;
 }
 
-int SearchJob::finish() {
+int SlotJob::launch_quant() {
+    set_pass_params(pq);
+    if (use_pqs) return pqs_launch(pq, plan, cap, stream);
+    kern<<<grid, kPqWarps * 32, smem_block, stream>>>(pq);
+    DAB_LAUNCHED();
+    DAB_CUDA(cudaGetLastError());
+    return DAB_OK;
+}
+
+// the post-processing of the whole batch: the rerank, or the filter of deleted ids
+int SlotJob::post() {
+    if (rerank) return launch_rerank(idx, stream, d_queries, nq, k, cap, pq.list_ids, pq.list_counts, out.ids, out.dists, out.counts, deleted);
+    if (filter) return queue_drop_deleted(idx, stream, deleted, out.ids, out.dists, cap, nq, k, filtered);
+    return DAB_OK;
+}
+
+int SlotJob::finish() {
+    DAB_CUDA(cudaEventSynchronize(counted));
+    if (store == STORE_MINMAX && first_nan() != ~0ull) return nan_error();
     for (;;) {
-        DAB_CUDA(cudaStreamSynchronize(stream));
-        idx->rec_truncated += h_counters[3];
         const uint32_t n_over = h_counters[1];
-        if (!recording) {  // build-time searches run on a growing graph: do not learn from them
-            learn_visited(idx->hint, l_search, beam, STORE_PQ, h_counters[2]);
-            if (stage == 0) {
+        if (rec.ids) {
+            idx->rec_truncated += h_counters[3];
+        } else {  // build-time searches run on a growing graph: do not learn from them
+            learn_visited(hint(), l_search, beam, mode(), h_counters[2]);
+            if (on_v3) {
                 idx->v3_overflow_l = l_search;
                 idx->v3_overflow_beam = beam;
                 idx->v3_overflow_frac = (float)n_over / (float)nq;
             }
         }
-        if (n_over == 0) return DAB_OK;
-        // re-run the overflowed queries on (larger) global tables
-        reran = true;
+        if (n_over == 0) break;
+        // the store the batch was planned on has been freed: its overflowed queries cannot be re-run
+        if (store >= 0 && idx->stores_version != stores_version)
+            return fail(DAB_ERR_INVALID_ARGUMENT, "dab_wait: a quantized store was replaced while the batch was in flight; "
+                                                  "%u of its queries could not be re-run", n_over);
         int rc;
-        if ((rc = take_overflow_list(stream, d_overflow, n_over, retry_list))) return rc;
-        p2.query_list = (const uint32_t*)retry_list.p;
-        p2.n_work = n_over;
-        if (stage == 0) {
+        if ((rc = take_overflow_list(stream, d_overflow, n_over, retry))) return rc;
+        if (on_v3) {
             // the overflowed queries are the largest: size the global tables from the estimate again
-            stage = 1;
-            slots = std::max(slots, table_slots(idx, VisitedHint{}, l_search, beam, STORE_PQ));
+            on_v3 = false;
+            slots = std::max(slots, table_slots(idx, VisitedHint{}, l_search, beam, mode()));
         } else if ((rc = grow_visited_tables(idx, pass, slots))) {
             return rc;
         }
-        if ((rc = launch())) return rc;
+        if ((rc = reserve_tables())) return rc;
+        work = (const uint32_t*)retry.p;
+        n_work = n_over;
+        reran = true;
+        if ((rc = launch_pass())) return rc;
+        DAB_CUDA(cudaEventSynchronize(counted));
     }
+    // the post-processing queued by launch read lists that the re-runs have since rewritten
+    return reran ? post() : DAB_OK;
 }
 
-// Runs the search over work items on the handle's stream and waits; device pointers only.  `rec_*` optional.
-int run_search(dab_index* idx, const void* d_queries, const uint32_t* d_query_rows, uint32_t nq, uint32_t k,
-               uint32_t l_search, uint32_t beam, uint32_t* d_ids, float* d_dists, uint32_t* d_counts, uint32_t* d_cmps,
-               uint32_t* d_hops, uint32_t* rec_ids, float* rec_dists, uint32_t* rec_counts, uint32_t rec_cap) {
+int run_search(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam, const SearchOut& d,
+               int store, bool rerank, const SearchRecord* rec) {
     int rc;
-    if ((rc = check_search_args(idx, k, l_search, beam))) return rc;
+    if ((rc = check_batch_args(idx, k, l_search, beam, store))) return rc;
     if (nq == 0) return DAB_OK;
-    if ((rc = idx->h_counters.reserve(16))) return rc;
-    SearchJob job;
-    job.idx = idx;
-    job.stream = idx->stream;
-    job.tables = &idx->s_tables;
-    job.counters = &idx->s_counters;
-    job.lists = &idx->s_ids;
-    job.h_counters = (uint32_t*)idx->h_counters.p;
-    if ((rc = job.prepare(d_queries, d_query_rows, nq, k, l_search, beam, d_ids, d_dists, d_counts, d_cmps, d_hops, rec_ids,
-                          rec_dists, rec_counts, rec_cap)))
-        return rc;
-    if ((rc = job.launch())) return rc;
-    return job.finish();
+    SlotJob job(idx, idx->stream, idx->s_tables, idx->s_counters, idx->s_stage, idx->s_out2, idx->s_ids, idx->h_counters);
+    if ((rc = job.prepare(d_queries, nq, k, l_search, beam, d, store, rerank, rec)) || (rc = job.stage_queries())) return rc;
+    if (store == STORE_MINMAX) {  // a batch with a NaN query fails before any traversal is launched
+        DAB_CUDA(cudaStreamSynchronize(idx->stream));
+        if (job.first_nan() != ~0ull) return job.nan_error();
+    }
+    if ((rc = job.launch_pass()) || (rc = job.post()) || (rc = job.finish())) return rc;
+    if (store < 0 && job.filter) DAB_CUDA(cudaStreamSynchronize(idx->stream));  // the filter follows the counters
+    return DAB_OK;
 }
 
 // ---- host-buffer calls -------------------------------------------------------------------------
@@ -303,8 +474,11 @@ static int queue_result_copies(cudaStream_t stream, const HostCopy& c) {
     return DAB_OK;
 }
 
-int search_host_buffers(dab_index* idx, const char* api, const void* queries, uint32_t nq, uint32_t k, const SearchOut& out,
-                        const std::function<int(const void* d_queries, const SearchOut& d_out)>& run) {
+// ---- the entry points' helpers: `store` -1 (full precision) or a QuantStore; `api` names the call in error messages ----
+// The synchronous host-buffer calls: checks the buffers, copies the queries to the handle's scratch, runs the batch on
+// them with device result buffers, copies the results to `out` and waits.
+static int search_host(dab_index* idx, const char* api, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                       uint32_t beam, const SearchOut& out, int store, bool rerank) {
     if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", api);
     if (nq == 0) return DAB_OK;
     if (!queries || !out.ids || !out.dists) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
@@ -313,14 +487,25 @@ int search_host_buffers(dab_index* idx, const char* api, const void* queries, ui
     HostCopy c{{}, out, nq, k};
     int rc;
     if ((rc = reserve_host_call(idx, idx->s_queries, idx->s_out, idx->s_stats, nq, k, &c.dev)) ||
-        (rc = queue_query_copy(idx, idx->stream, idx->s_queries.p, queries, nq)) || (rc = run(idx->s_queries.p, c.dev)) ||
-        (rc = queue_result_copies(idx->stream, c)))
+        (rc = queue_query_copy(idx, idx->stream, idx->s_queries.p, queries, nq)) ||
+        (rc = run_search(idx, idx->s_queries.p, nq, k, l_search, beam, c.dev, store, rerank)) || (rc = queue_result_copies(idx->stream, c)))
         return rc;
     DAB_CUDA(cudaStreamSynchronize(idx->stream));
     return DAB_OK;
 }
 
-// ---- batches in flight (dab_search_batch[_pq|_sq|_minmax][_device]_async / dab_wait) ----
+// The synchronous device-buffer calls (run_search).  The full-precision call makes its argument checks before it returns
+// for an empty batch; the quantized calls return first.
+static int search_device(dab_index* idx, const char* api, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                         uint32_t beam, const SearchOut& d, int store, bool rerank) {
+    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", api);
+    if (nq == 0 && store >= 0) return DAB_OK;
+    if (nq && (!d_queries || !d.ids || !d.dists)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
+    DAB_CUDA(cudaSetDevice(idx->device));
+    return run_search(idx, d_queries, nq, k, l_search, beam, d, store, rerank);
+}
+
+// ---- batches in flight (dab_search_batch*_async / dab_wait) --------------------------------------------------------
 void search_slots_release(dab_index* idx) {
     for (int i = 0; i < DAB_MAX_SLOTS; ++i) {
         SearchSlot* s = (SearchSlot*)idx->slots[i];
@@ -360,11 +545,18 @@ static int slot_of(dab_index* idx, uint32_t slot, SearchSlot** out) {
     return DAB_OK;
 }
 
-int slot_submit(dab_index* idx, const char* api, uint32_t slot, bool host, const void* queries, uint32_t nq, uint32_t k,
-                const SearchOut& out, const std::function<int(SearchSlot* s, const void* d_queries, const SearchOut& d_out, SlotJob** job)>& prepare) {
+// The *_async calls: the job on the slot's stream and scratch.  After the argument checks, the slot is checked (in range,
+// no batch in flight); nq == 0 is then a no-op.  A host-buffer call (`host`) gets device buffers in the slot's scratch.
+// The job is prepared with every check the synchronous call makes before it launches; then the copy of the queries, the
+// job's launch and the copies of the results are queued, and the call returns without waiting.
+static int search_async(dab_index* idx, const char* api, uint32_t slot, bool host, const void* queries, uint32_t nq, uint32_t k,
+                        uint32_t l_search, uint32_t beam, const SearchOut& out, int store, bool rerank) {
+    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", api);
+    if (nq && (!queries || !out.ids || !out.dists)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
+    int rc;
+    if ((rc = check_batch_args(idx, k, l_search, beam, store))) return rc;
     DAB_CUDA(cudaSetDevice(idx->device));
     SearchSlot* s = nullptr;
-    int rc;
     if ((rc = slot_of(idx, slot, &s))) return rc;
     if (s->job) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: slot %u still has a batch in flight (call dab_wait)", api, slot);
     if (nq == 0) return DAB_OK;
@@ -373,9 +565,9 @@ int slot_submit(dab_index* idx, const char* api, uint32_t slot, bool host, const
         c.host = out;
         if ((rc = reserve_host_call(idx, s->queries, s->out, s->stats, nq, k, &c.dev))) return rc;
     }
-    const void* d_queries = host ? s->queries.p : queries;
-    SlotJob* job = nullptr;
-    if ((rc = prepare(s, d_queries, c.dev, &job))) {
+    SlotJob* job = new SlotJob(idx, s->stream, s->tables, s->counters, s->stage, s->luts, s->lists, s->h_counters);
+    job->full_grid = true;
+    if ((rc = job->prepare(host ? s->queries.p : queries, nq, k, l_search, beam, c.dev, store, rerank, nullptr))) {
         delete job;
         return rc;
     }
@@ -392,47 +584,71 @@ int slot_submit(dab_index* idx, const char* api, uint32_t slot, bool host, const
     return host ? queue_result_copies(s->stream, c) : DAB_OK;
 }
 
-// a full-precision batch on slot `s`: every resident worker is launched (the next batch fills what this one leaves)
-static int prepare_search_job(dab_index* idx, SearchSlot* s, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
-                              uint32_t beam, const SearchOut& d, SlotJob** out) {
-    int rc;
-    if ((rc = s->h_counters.reserve(16))) return rc;
-    SearchJob* job = new SearchJob();
-    *out = job;
-    job->idx = idx;
-    job->stream = s->stream;
-    job->tables = &s->tables;
-    job->counters = &s->counters;
-    job->lists = &s->lists;
-    job->h_counters = (uint32_t*)s->h_counters.p;
-    job->full_grid = true;
-    return job->prepare(d_queries, nullptr, nq, k, l_search, beam, d.ids, d.dists, d.counts, d.cmps, d.hops, nullptr, nullptr, nullptr, 0);
-}
-
 }  // namespace dab
 
 using namespace dab;
 
 extern "C" {
 
-int dab_search_batch_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
-                            uint32_t beam_width, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
-                            uint32_t* d_out_cmps, uint32_t* d_out_hops) {
-    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch: idx is NULL");
-    if (nq && (!d_queries || !d_out_ids || !d_out_dists)) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch: NULL argument");
-    DAB_CUDA(cudaSetDevice(idx->device));
-    return run_search(idx, d_queries, nullptr, nq, k, l_search, beam_width, d_out_ids, d_out_dists, d_out_counts,
-                      d_out_cmps, d_out_hops, nullptr, nullptr, nullptr, 0);
-}
-
 int dab_search_batch(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
                      uint32_t beam_width, uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
                      uint32_t* out_cmps, uint32_t* out_hops) {
-    return search_host_buffers(idx, "dab_search_batch", queries, nq, k, SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops},
-                               [&](const void* d_queries, const SearchOut& d) {
-                                   return run_search(idx, d_queries, nullptr, nq, k, l_search, beam_width, d.ids, d.dists, d.counts,
-                                                     d.cmps, d.hops, nullptr, nullptr, nullptr, 0);
-                               });
+    return search_host(idx, "dab_search_batch", queries, nq, k, l_search, beam_width,
+                       SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, -1, false);
+}
+
+// returns with the outputs complete, the filter of deleted ids included
+int dab_search_batch_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                            uint32_t beam_width, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
+                            uint32_t* d_out_cmps, uint32_t* d_out_hops) {
+    return search_device(idx, "dab_search_batch", d_queries, nq, k, l_search, beam_width,
+                         SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, -1, false);
+}
+
+int dab_search_batch_pq(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
+                        uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops) {
+    return search_host(idx, "dab_search_batch_pq", queries, nq, k, l_search, beam_width,
+                       SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, STORE_PQ, false);
+}
+
+int dab_search_batch_pq_rerank(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
+                               uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops) {
+    return search_host(idx, "dab_search_batch_pq_rerank", queries, nq, k, l_search, beam_width,
+                       SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, STORE_PQ, true);
+}
+
+// The quantized *_device calls return once the traversal is complete; the rerank or the filter may still run
+int dab_search_batch_pq_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
+                               int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts, uint32_t* d_out_cmps,
+                               uint32_t* d_out_hops) {
+    return search_device(idx, "dab_search_batch_pq_device", d_queries, nq, k, l_search, beam_width,
+                         SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, STORE_PQ, rerank != 0);
+}
+
+int dab_search_batch_sq(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
+                        int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops) {
+    return search_host(idx, "dab_search_batch_sq", queries, nq, k, l_search, beam_width,
+                       SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, STORE_SQ, rerank != 0);
+}
+
+int dab_search_batch_sq_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
+                               int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts, uint32_t* d_out_cmps,
+                               uint32_t* d_out_hops) {
+    return search_device(idx, "dab_search_batch_sq_device", d_queries, nq, k, l_search, beam_width,
+                         SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, STORE_SQ, rerank != 0);
+}
+
+int dab_search_batch_minmax(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
+                            int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops) {
+    return search_host(idx, "dab_search_batch_minmax", queries, nq, k, l_search, beam_width,
+                       SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, STORE_MINMAX, rerank != 0);
+}
+
+int dab_search_batch_minmax_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
+                                   int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts, uint32_t* d_out_cmps,
+                                   uint32_t* d_out_hops) {
+    return search_device(idx, "dab_search_batch_minmax_device", d_queries, nq, k, l_search, beam_width,
+                         SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, STORE_MINMAX, rerank != 0);
 }
 
 // ---- asynchronous batches: launch on a slot, collect with dab_wait ---------------------------
@@ -444,33 +660,62 @@ int dab_search_batch(dab_index* idx, const void* queries, uint32_t nq, uint32_t 
 int dab_search_batch_async(dab_index* idx, uint32_t slot, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
                            uint32_t beam_width, uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps,
                            uint32_t* out_hops) {
-    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_async: idx is NULL");
-    if (nq && (!queries || !out_ids || !out_dists)) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_async: NULL argument");
-    int rc;
-    if ((rc = check_search_args(idx, k, l_search, beam_width))) return rc;
-    return slot_submit(idx, "dab_search_batch_async", slot, true, queries, nq, k, SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops},
-                       [&](SearchSlot* s, const void* d_queries, const SearchOut& d, SlotJob** job) {
-                           return prepare_search_job(idx, s, d_queries, nq, k, l_search, beam_width, d, job);
-                       });
+    return search_async(idx, "dab_search_batch_async", slot, true, queries, nq, k, l_search, beam_width,
+                        SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, -1, false);
 }
 
 int dab_search_batch_device_async(dab_index* idx, uint32_t slot, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
                                   uint32_t beam_width, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
                                   uint32_t* d_out_cmps, uint32_t* d_out_hops) {
-    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_device_async: idx is NULL");
-    if (nq && (!d_queries || !d_out_ids || !d_out_dists)) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_device_async: NULL argument");
-    int rc;
-    if ((rc = check_search_args(idx, k, l_search, beam_width))) return rc;
-    return slot_submit(idx, "dab_search_batch_device_async", slot, false, d_queries, nq, k,
-                       SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops},
-                       [&](SearchSlot* s, const void* dq, const SearchOut& d, SlotJob** job) {
-                           return prepare_search_job(idx, s, dq, nq, k, l_search, beam_width, d, job);
-                       });
+    return search_async(idx, "dab_search_batch_device_async", slot, false, d_queries, nq, k, l_search, beam_width,
+                        SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, -1, false);
 }
 
-// Joins a batch of any kind.  In the rare overflow case the job's re-runs (and, for a quantized batch with rerank, the
-// rerank of the whole batch) are queued again by finish: they are waited for here, after the result copies of a
-// host-buffer call are queued once more.
+int dab_search_batch_pq_async(dab_index* idx, uint32_t slot, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                              uint32_t beam_width, int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
+                              uint32_t* out_cmps, uint32_t* out_hops) {
+    return search_async(idx, "dab_search_batch_pq_async", slot, true, queries, nq, k, l_search, beam_width,
+                        SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, STORE_PQ, rerank != 0);
+}
+
+int dab_search_batch_pq_device_async(dab_index* idx, uint32_t slot, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                                     uint32_t beam_width, int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
+                                     uint32_t* d_out_cmps, uint32_t* d_out_hops) {
+    return search_async(idx, "dab_search_batch_pq_device_async", slot, false, d_queries, nq, k, l_search, beam_width,
+                        SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, STORE_PQ, rerank != 0);
+}
+
+int dab_search_batch_sq_async(dab_index* idx, uint32_t slot, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                              uint32_t beam_width, int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
+                              uint32_t* out_cmps, uint32_t* out_hops) {
+    return search_async(idx, "dab_search_batch_sq_async", slot, true, queries, nq, k, l_search, beam_width,
+                        SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, STORE_SQ, rerank != 0);
+}
+
+int dab_search_batch_sq_device_async(dab_index* idx, uint32_t slot, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                                     uint32_t beam_width, int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
+                                     uint32_t* d_out_cmps, uint32_t* d_out_hops) {
+    return search_async(idx, "dab_search_batch_sq_device_async", slot, false, d_queries, nq, k, l_search, beam_width,
+                        SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, STORE_SQ, rerank != 0);
+}
+
+int dab_search_batch_minmax_async(dab_index* idx, uint32_t slot, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                                  uint32_t beam_width, int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
+                                  uint32_t* out_cmps, uint32_t* out_hops) {
+    return search_async(idx, "dab_search_batch_minmax_async", slot, true, queries, nq, k, l_search, beam_width,
+                        SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, STORE_MINMAX, rerank != 0);
+}
+
+int dab_search_batch_minmax_device_async(dab_index* idx, uint32_t slot, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                                         uint32_t beam_width, int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
+                                         uint32_t* d_out_cmps, uint32_t* d_out_hops) {
+    return search_async(idx, "dab_search_batch_minmax_device_async", slot, false, d_queries, nq, k, l_search, beam_width,
+                        SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, STORE_MINMAX, rerank != 0);
+}
+
+// Joins a batch of any kind.  In the rare overflow case the job's re-runs (and then the rerank or the filter of the whole
+// batch) are queued again by finish: they are waited for here, after the result copies of a host-buffer call are queued
+// once more.
 int dab_wait(dab_index* idx, uint32_t slot) {
     if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_wait: idx is NULL");
     if (slot >= DAB_MAX_SLOTS) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_wait: slot %u out of range (DAB_MAX_SLOTS = %d)", slot, DAB_MAX_SLOTS);

@@ -247,8 +247,7 @@ static size_t rerank_warp_smem(bool is_int, uint32_t dim, uint32_t list_cap) {
     return (is_int ? round_up((size_t)dim, 16) : round_up((size_t)dim * 4, 16)) + 2 * round_up((size_t)list_cap * 4, 16);
 }
 
-// the rerank of lists of list_cap entries fits a CTA of this index's schema
-static int check_rerank(const dab_index* idx, uint32_t list_cap) {
+int check_rerank(const dab_index* idx, uint32_t list_cap) {
     return visit_schema<OPS_ROW>(idx->dtype, idx->metric, [&](auto s) -> int {
         const size_t smem = rerank_warp_smem(decltype(s)::IS_INT, idx->dim, list_cap) * kRerankWarps;
         if (smem > 200 * 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "rerank: configuration needs %zu B shared memory per CTA", smem);
@@ -256,9 +255,9 @@ static int check_rerank(const dab_index* idx, uint32_t list_cap) {
     });
 }
 
-static int launch_rerank(const dab_index* idx, cudaStream_t stream, const void* d_queries, uint32_t nq, uint32_t k, uint32_t list_cap,
-                         const uint32_t* d_list, const uint32_t* d_list_n, uint32_t* d_ids, float* d_dists, uint32_t* d_counts,
-                         const uint32_t* deleted) {
+int launch_rerank(const dab_index* idx, cudaStream_t stream, const void* d_queries, uint32_t nq, uint32_t k, uint32_t list_cap,
+                  const uint32_t* d_list, const uint32_t* d_list_n, uint32_t* d_ids, float* d_dists, uint32_t* d_counts,
+                  const uint32_t* deleted) {
     RerankParams p;
     memset(&p, 0, sizeof(p));
     p.vectors = idx->d_vectors;
@@ -295,404 +294,11 @@ static int launch_rerank(const dab_index* idx, cudaStream_t stream, const void* 
     return DAB_OK;
 }
 
-// The checks of a quantized search that need no plan: arguments, the store, the metric, the list length
-static int check_pq_args(const dab_index* idx, uint32_t k, uint32_t l_search, uint32_t beam, QuantStore mode) {
-    int rc;
-    // every entry point of a store reports under its synchronous host-buffer call's name
-    const char* who = mode == STORE_PQ ? "dab_search_batch_pq" : mode == STORE_SQ ? "dab_search_batch_sq" : "dab_search_batch_minmax";
-    if ((rc = check_search_args(idx, k, l_search, beam, false)) || (rc = check_quant_store(idx, mode, who, false))) return rc;
-    if (l_search + idx->n_start > 1024)
-        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: L + #start must be <= 1024", mode == STORE_MINMAX ? "dab_search_batch_minmax" : "dab_search_batch_pq");
-    return DAB_OK;
-}
-
-// ---- one quantized batch as a resumable job --------------------------------------------------
-// The quantized counterpart of SearchJob (search_kernel.cu).  `prepare` plans the batch (check_pq_args has passed),
-// makes the checks of the plan and reserves every buffer the first pass needs (nothing is queued); `launch` queues the staging of the queries (SQ, MinMax), the first traversal pass, the
-// read-back of its counters (and the MinMax NaN flag) into pinned memory and, optimistically, the rerank; `finish`
-// waits for the counters, learns the visited-set size, re-runs the queries whose visited set outgrew its table on
-// larger tables and then queues the rerank of the whole batch again.  The synchronous entry points run prepare, launch
-// and finish on the handle's stream and scratch; the *_async calls on a slot's.  A re-run reads the store the batch was
-// planned on: if a quantized store was replaced since (retire_quantized_stores), finish fails instead.
-struct PqSearchJob : SlotJob {
-    dab_index* idx = nullptr;
-    cudaStream_t stream = nullptr;
-    Scratch *tables = nullptr, *counters = nullptr, *stage = nullptr, *luts = nullptr, *lists = nullptr;
-    uint32_t* h_counters = nullptr;  // pinned: the four counters of a pass, then (u64 at word 4) the MinMax NaN flag
-
-    QuantStore mode = STORE_PQ;
-    bool rerank = false;
-    const void* d_queries = nullptr;
-    uint32_t nq = 0, k = 0, l_search = 0, beam = 0, cap = 0;
-    SearchParamsPq p;
-    PqsPlan plan;
-    bool use_pqs = false;
-    void (*kern)(const SearchParamsPq) = nullptr;
-    int grid = 0;
-    size_t smem_block = 0;
-    uint64_t slots = 0;
-    int pass = 0;
-    Scratch retry;
-    cudaEvent_t counted = nullptr;  // recorded after the read-back of a pass's counters
-    uint64_t stores_version = 0;    // idx->stores_version when the batch was planned
-    // some id is deleted: the rerank drops deleted ids; without rerank the traversal writes every non-start entry of a
-    // list (k = L + #start) to `lists` and the filter takes the first k live ones into `filtered`, the caller's buffers
-    const uint32_t* deleted = nullptr;
-    SearchOut filtered{};
-
-    int prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint32_t l_search_, uint32_t beam_, const SearchOut& d, bool rerank_, QuantStore mode_);
-    int stage_queries();
-    int launch_traversal();
-    int launch() override;
-    int finish() override;
-    int launch_pass();
-    int launch_post();
-    int reserve_tables();
-    unsigned long long first_nan() const { return *(const unsigned long long*)(h_counters + 4); }
-    int nan_error() const {
-        return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_minmax: query %llu contains NaN after the transform (InputContainsNaN)", first_nan());
-    }
-    ~PqSearchJob() override {
-        retry.release();
-        if (counted) cudaEventDestroy(counted);
-    }
-};
-
-int PqSearchJob::prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint32_t l_search_, uint32_t beam_, const SearchOut& d,
-                         bool rerank_, QuantStore mode_) {
-    d_queries = d_queries_, nq = nq_, k = k_, l_search = l_search_, beam = beam_, rerank = rerank_, mode = mode_;
-    stores_version = idx->stores_version;
-    int rc;
-    cap = l_search + idx->n_start;
-    memset(&p, 0, sizeof(p));
-    p.adj = idx->d_adj;
-    p.adj_stride = idx->adj_stride;
-    p.n_points = idx->n_points;
-    p.n_start = idx->n_start;
-    p.dim = idx->dim;
-    p.max_degree = idx->max_degree;
-    p.dtype = idx->dtype;
-    p.queries = d_queries;
-    p.k = k;
-    p.cap = cap;
-    p.beam = beam;
-    set_store_params(idx, mode, p);
-    p.out_ids = d.ids;
-    p.out_dists = d.dists;
-    p.out_counts = d.counts;
-    p.out_cmps = d.cmps;
-    p.out_hops = d.hops;
-    deleted = deleted_filter(idx);
-    if (deleted && !rerank) {
-        if ((rc = lists->reserve((size_t)nq * cap * 8))) return rc;
-        filtered = d;
-        p.k = cap;
-        p.out_ids = (uint32_t*)lists->p;
-        p.out_dists = (float*)(p.out_ids + (size_t)nq * cap);
-    }
-
-    size_t off = 0;
-    p.off_q = 0;
-    off += round_up((size_t)idx->dim * 4, 16);
-    const size_t cap_pad = round_up(cap, 32) + 32;
-    p.off_qd = (uint32_t)off;
-    off += cap_pad * 4;
-    p.off_qi = (uint32_t)off;
-    off += cap_pad * 4;
-    const size_t ncand_max = std::max<size_t>((size_t)beam * idx->max_degree, idx->n_start);
-    p.off_cid = (uint32_t)off;
-    off += round_up(ncand_max * 4, 16);
-    p.off_cd = (uint32_t)off;
-    off += round_up(ncand_max * 4, 16);
-    p.off_beam = (uint32_t)off;
-    off += round_up((size_t)beam * 4, 16);
-    p.off_qc = (uint32_t)off;
-    if (mode == STORE_SQ) off += p.code_stride;
-    if (mode == STORE_MINMAX) off += p.code_stride + 16;  // the query's code row and its four compensations
-    off = round_up(off, 16);
-    p.off_nrow = (uint32_t)off;  // search_kernel_pqs: the adjacency row copied one hop ahead
-    if (mode == STORE_PQ) off += 96 * 4;
-    p.warp_smem = (uint32_t)round_up(off, 16);
-    // table metrics with a pivot table that fits shared memory: search_kernel_pqs (pivots resident per SM, entries
-    // computed on the fly); everything else — SQ, DirectCosine, wide pivots, > 32 chunks — the per-warp kernel below
-    memset(&plan, 0, sizeof(plan));
-    use_pqs = mode == STORE_PQ && !p.direct_cosine && pqs_plan(idx, p.warp_smem, nq, &plan);
-    smem_block = (size_t)p.warp_smem * kPqWarps;
-    uint32_t warps;
-    if (use_pqs) {
-        p.piv_stride = plan.piv_stride;
-        p.piv_bytes = plan.piv_bytes;
-        grid = plan.grid;
-        warps = (uint32_t)plan.grid * (uint32_t)plan.warps;
-    } else {
-        if (smem_block > 200 * 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_pq: configuration needs %zu B shared memory per CTA", smem_block);
-        kern = visit_list_tile(cap, [&](auto qt) {
-            constexpr int QT = decltype(qt)::value;
-            return mode == STORE_MINMAX ? search_kernel_pq<QT, STORE_MINMAX> : mode == STORE_SQ ? search_kernel_pq<QT, STORE_SQ> : search_kernel_pq<QT, STORE_PQ>;
-        });
-        DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_block));
-        int per_sm = 0;
-        DAB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kPqWarps * 32, smem_block));
-        if (per_sm < 1) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_pq: kernel does not fit");
-        // every resident warp owns a LUT (n_chunks x n_centers f32: 32 KB at 32 x 256) and a visited table in
-        // global memory; ADC terms and probes are L2 hits only while all of them stay L2-resident
-        // (the SQ kernel has no LUT: it keeps the occupancy the shared memory allows)
-        if (mode == STORE_PQ) per_sm = std::min(per_sm, 6);
-        grid = (int)std::min<uint64_t>((uint64_t)per_sm * idx->sm_count, ((uint64_t)nq + kPqWarps - 1) / kPqWarps);
-        warps = (uint32_t)grid * kPqWarps;
-    }
-
-    if ((rc = counters->reserve(16 + (size_t)nq * 4))) return rc;
-    p.counters = (uint32_t*)counters->p;
-    p.overflow_list = p.counters + 4;
-    const size_t lut_bytes = mode == STORE_PQ && !use_pqs ? (size_t)warps * idx->pq_chunks * idx->pq_centers * 4 : 16;
-    if ((rc = luts->reserve(lut_bytes))) return rc;
-    p.luts = (float*)luts->p;
-    p.n_work = nq;
-    if (rerank) {
-        if (!idx->vectors_ready) return fail(DAB_ERR_NOT_READY, "dab_search_batch_pq: rerank needs the full-precision vectors");
-        if ((rc = check_rerank(idx, cap))) return rc;
-        if ((rc = lists->reserve(((size_t)nq * cap + nq) * 4))) return rc;
-        p.list_ids = (uint32_t*)lists->p;
-        p.list_counts = p.list_ids + (size_t)nq * cap;
-        p.list_cap = cap;
-    }
-    // global-table passes: the overflowed queries of one are re-run on larger tables in the next
-    slots = table_slots(idx, idx->pq_hint, l_search, beam, mode);
-    pass = 0;
-    if ((rc = reserve_tables())) return rc;
-    if ((rc = stage->reserve(mode == STORE_SQ ? sq_stage_bytes(idx, nq) : mode == STORE_MINMAX ? minmax_stage_bytes(idx, nq) : 0))) return rc;
-    DAB_CUDA(cudaEventCreateWithFlags(&counted, cudaEventDisableTiming));
-    return DAB_OK;
-}
-
-// SQ and MinMax: the batch's queries compressed by the store's quantizer (MinMax: the NaN flag read back into h_counters)
-int PqSearchJob::stage_queries() {
-    if (mode == STORE_SQ) return sq_stage_queries(idx, stream, *stage, d_queries, nq, &p.query_codes, &p.query_meta);
-    if (mode == STORE_MINMAX) return minmax_stage_queries(idx, stream, *stage, d_queries, nq, (unsigned long long*)(h_counters + 4), &p.query_codes, &p.query_meta);
-    return DAB_OK;
-}
-
-// a visited table of `slots` ids per resident warp
-int PqSearchJob::reserve_tables() {
-    int rc;
-    p.n_buckets = (uint32_t)((slots + 7) / 8);
-    const size_t warps = use_pqs ? (size_t)plan.grid * plan.warps : (size_t)grid * kPqWarps;
-    if ((rc = tables->reserve(warps * p.n_buckets * 32))) return rc;
-    p.tables = (uint32_t*)tables->p;
-    return DAB_OK;
-}
-
-// one traversal pass over p.n_work queries (tables reserved) and the read-back of its counters
-int PqSearchJob::launch_pass() {
-    int rc;
-    DAB_CUDA(cudaMemsetAsync(p.counters, 0, 16, stream));
-    if (use_pqs) {
-        if ((rc = pqs_launch(p, plan, cap, stream))) return rc;
-    } else {
-        kern<<<grid, kPqWarps * 32, smem_block, stream>>>(p);
-        DAB_LAUNCHED();
-        DAB_CUDA(cudaGetLastError());
-    }
-    DAB_CUDA(cudaMemcpyAsync(h_counters, p.counters, 16, cudaMemcpyDeviceToHost, stream));
-    DAB_CUDA(cudaEventRecord(counted, stream));
-    return DAB_OK;
-}
-
-// the post-processing of the whole batch: the rerank, or the filter of deleted ids
-int PqSearchJob::launch_post() {
-    if (rerank) return launch_rerank(idx, stream, d_queries, nq, k, cap, p.list_ids, p.list_counts, p.out_ids, p.out_dists, p.out_counts, deleted);
-    if (deleted) return queue_drop_deleted(idx, stream, deleted, p.out_ids, p.out_dists, cap, nq, k, filtered);
-    return DAB_OK;
-}
-
-// the first pass and, optimistically, the post-processing
-int PqSearchJob::launch_traversal() {
-    int rc;
-    if ((rc = launch_pass())) return rc;
-    return launch_post();
-}
-
-int PqSearchJob::launch() {
-    int rc;
-    if ((rc = stage_queries())) return rc;
-    return launch_traversal();
-}
-
-int PqSearchJob::finish() {
-    DAB_CUDA(cudaEventSynchronize(counted));
-    if (mode == STORE_MINMAX && first_nan() != ~0ull) return nan_error();
-    for (;;) {
-        learn_visited(idx->pq_hint, l_search, beam, mode, h_counters[2]);
-        const uint32_t n_over = h_counters[1];
-        if (n_over == 0) break;
-        // the store the batch was planned on has been freed: its overflowed queries cannot be re-run
-        if (idx->stores_version != stores_version)
-            return fail(DAB_ERR_INVALID_ARGUMENT, "dab_wait: a quantized store was replaced while the batch was in flight; "
-                                                  "%u of its queries could not be re-run", n_over);
-        int rc;
-        if ((rc = take_overflow_list(stream, p.overflow_list, n_over, retry)) || (rc = grow_visited_tables(idx, pass, slots)) ||
-            (rc = reserve_tables()))
-            return rc;
-        p.query_list = (const uint32_t*)retry.p;
-        p.n_work = n_over;
-        reran = true;
-        if ((rc = launch_pass())) return rc;
-        DAB_CUDA(cudaEventSynchronize(counted));
-    }
-    // the rerank or filter queued by launch read lists that the re-runs have since rewritten
-    return reran ? launch_post() : DAB_OK;
-}
-
-// The synchronous calls: the job on the handle's stream and scratch.  A MinMax batch with a NaN query fails before any
-// traversal is launched.  Device pointers only; returns once the traversal is complete (the rerank may still run).
-static int run_search_pq(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam,
-                         const SearchOut& d, bool rerank, QuantStore mode) {
-    int rc;
-    if ((rc = idx->h_counters.reserve(24))) return rc;
-    PqSearchJob job;
-    job.idx = idx;
-    job.stream = idx->stream;
-    job.tables = &idx->s_tables, job.counters = &idx->s_counters, job.stage = &idx->s_stage, job.luts = &idx->s_out2, job.lists = &idx->s_ids;
-    job.h_counters = (uint32_t*)idx->h_counters.p;
-    if ((rc = check_pq_args(idx, k, l_search, beam, mode)) || (rc = job.prepare(d_queries, nq, k, l_search, beam, d, rerank, mode))) return rc;
-    if ((rc = job.stage_queries())) return rc;
-    if (mode == STORE_MINMAX) {
-        DAB_CUDA(cudaStreamSynchronize(idx->stream));
-        if (job.first_nan() != ~0ull) return job.nan_error();
-    }
-    if ((rc = job.launch_traversal())) return rc;
-    return job.finish();
-}
-
-static int search_pq_host(dab_index* idx, const char* api, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
-                          uint32_t beam_width, const SearchOut& out, bool rerank, QuantStore mode) {
-    return search_host_buffers(idx, api, queries, nq, k, out, [&](const void* d_queries, const SearchOut& d) {
-        return run_search_pq(idx, d_queries, nq, k, l_search, beam_width, d, rerank, mode);
-    });
-}
-
-static int search_pq_device(dab_index* idx, const char* api, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
-                            uint32_t beam_width, const SearchOut& d, bool rerank, QuantStore mode) {
-    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", api);
-    if (nq == 0) return DAB_OK;
-    if (!d_queries || !d.ids || !d.dists) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
-    DAB_CUDA(cudaSetDevice(idx->device));
-    return run_search_pq(idx, d_queries, nq, k, l_search, beam_width, d, rerank, mode);
-}
-
-// The *_async calls: the job on the slot's stream and scratch
-static int search_pq_async(dab_index* idx, const char* api, uint32_t slot, bool host, const void* queries, uint32_t nq, uint32_t k,
-                           uint32_t l_search, uint32_t beam_width, const SearchOut& out, bool rerank, QuantStore mode) {
-    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", api);
-    if (nq && (!queries || !out.ids || !out.dists)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
-    int rc;
-    if ((rc = check_pq_args(idx, k, l_search, beam_width, mode))) return rc;  // before the slot rules, as the full-precision call
-    return slot_submit(idx, api, slot, host, queries, nq, k, out, [&](SearchSlot* s, const void* d_queries, const SearchOut& d, SlotJob** out_job) {
-        int rc2;
-        if ((rc2 = s->h_counters.reserve(24))) return rc2;
-        PqSearchJob* job = new PqSearchJob();
-        *out_job = job;
-        job->idx = idx;
-        job->stream = s->stream;
-        job->tables = &s->tables, job->counters = &s->counters, job->stage = &s->stage, job->luts = &s->luts, job->lists = &s->lists;
-        job->h_counters = (uint32_t*)s->h_counters.p;
-        return job->prepare(d_queries, nq, k, l_search, beam_width, d, rerank, mode);
+PqKernel pq_kernel(uint32_t cap, QuantStore store) {
+    return visit_list_tile(cap, [&](auto qt) {
+        constexpr int QT = decltype(qt)::value;
+        return store == STORE_MINMAX ? search_kernel_pq<QT, STORE_MINMAX> : store == STORE_SQ ? search_kernel_pq<QT, STORE_SQ> : search_kernel_pq<QT, STORE_PQ>;
     });
 }
 
 }  // namespace dab
-
-using namespace dab;
-
-extern "C" {
-
-int dab_search_batch_pq(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
-                        uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops) {
-    return search_pq_host(idx, "dab_search_batch_pq", queries, nq, k, l_search, beam_width,
-                          SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, false, STORE_PQ);
-}
-
-int dab_search_batch_pq_rerank(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
-                               uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops) {
-    return search_pq_host(idx, "dab_search_batch_pq_rerank", queries, nq, k, l_search, beam_width,
-                          SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, true, STORE_PQ);
-}
-
-int dab_search_batch_pq_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
-                               int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts, uint32_t* d_out_cmps,
-                               uint32_t* d_out_hops) {
-    return search_pq_device(idx, "dab_search_batch_pq_device", d_queries, nq, k, l_search, beam_width,
-                            SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, STORE_PQ);
-}
-
-int dab_search_batch_sq(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
-                        int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops) {
-    return search_pq_host(idx, "dab_search_batch_sq", queries, nq, k, l_search, beam_width,
-                          SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, rerank != 0, STORE_SQ);
-}
-
-int dab_search_batch_sq_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
-                               int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts, uint32_t* d_out_cmps,
-                               uint32_t* d_out_hops) {
-    return search_pq_device(idx, "dab_search_batch_sq_device", d_queries, nq, k, l_search, beam_width,
-                            SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, STORE_SQ);
-}
-
-int dab_search_batch_minmax(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
-                            int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops) {
-    return search_pq_host(idx, "dab_search_batch_minmax", queries, nq, k, l_search, beam_width,
-                          SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, rerank != 0, STORE_MINMAX);
-}
-
-int dab_search_batch_minmax_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
-                                   int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts, uint32_t* d_out_cmps,
-                                   uint32_t* d_out_hops) {
-    return search_pq_device(idx, "dab_search_batch_minmax_device", d_queries, nq, k, l_search, beam_width,
-                            SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, STORE_MINMAX);
-}
-
-// ---- asynchronous batches (see dab_search_batch_async): the same jobs on a slot, joined by dab_wait ----
-int dab_search_batch_pq_async(dab_index* idx, uint32_t slot, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
-                              uint32_t beam_width, int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
-                              uint32_t* out_cmps, uint32_t* out_hops) {
-    return search_pq_async(idx, "dab_search_batch_pq_async", slot, true, queries, nq, k, l_search, beam_width,
-                           SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, rerank != 0, STORE_PQ);
-}
-
-int dab_search_batch_pq_device_async(dab_index* idx, uint32_t slot, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
-                                     uint32_t beam_width, int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
-                                     uint32_t* d_out_cmps, uint32_t* d_out_hops) {
-    return search_pq_async(idx, "dab_search_batch_pq_device_async", slot, false, d_queries, nq, k, l_search, beam_width,
-                           SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, STORE_PQ);
-}
-
-int dab_search_batch_sq_async(dab_index* idx, uint32_t slot, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
-                              uint32_t beam_width, int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
-                              uint32_t* out_cmps, uint32_t* out_hops) {
-    return search_pq_async(idx, "dab_search_batch_sq_async", slot, true, queries, nq, k, l_search, beam_width,
-                           SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, rerank != 0, STORE_SQ);
-}
-
-int dab_search_batch_sq_device_async(dab_index* idx, uint32_t slot, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
-                                     uint32_t beam_width, int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
-                                     uint32_t* d_out_cmps, uint32_t* d_out_hops) {
-    return search_pq_async(idx, "dab_search_batch_sq_device_async", slot, false, d_queries, nq, k, l_search, beam_width,
-                           SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, STORE_SQ);
-}
-
-int dab_search_batch_minmax_async(dab_index* idx, uint32_t slot, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
-                                  uint32_t beam_width, int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
-                                  uint32_t* out_cmps, uint32_t* out_hops) {
-    return search_pq_async(idx, "dab_search_batch_minmax_async", slot, true, queries, nq, k, l_search, beam_width,
-                           SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, rerank != 0, STORE_MINMAX);
-}
-
-int dab_search_batch_minmax_device_async(dab_index* idx, uint32_t slot, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
-                                         uint32_t beam_width, int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
-                                         uint32_t* d_out_cmps, uint32_t* d_out_hops) {
-    return search_pq_async(idx, "dab_search_batch_minmax_device_async", slot, false, d_queries, nq, k, l_search, beam_width,
-                           SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, rerank != 0, STORE_MINMAX);
-}
-
-}  // extern "C"

@@ -31,6 +31,7 @@
 #include "dab_common.cuh"
 #include "distance_device.cuh"
 #include "search_common.cuh"
+#include "search_host.cuh"
 #include "search_smem.cuh"
 #include "search_v2.cuh"
 
@@ -583,17 +584,10 @@ static int v2_prepare_schema(const dab_index* idx, uint32_t l_search, uint32_t b
     // workload is ~1200 ids) when the ids fit 14-bit quotient tags, i.e. n_total <= 16384 * buckets
     size_t t1_bytes = idx->tune.test_visited_log2 ? 512 : 4096;  // tests: a level 1 that fills at once
     p.t1_buckets = 0;
-    uint32_t K = 8;
-    while (((uint64_t)1 << K) < idx->n_total()) ++K;
     const uint64_t nb1 = t1_bytes / 32;
-    uint32_t sbits = 0;
-    while (((uint64_t)1 << sbits) < nb1) ++sbits;
-    if ((((uint64_t)1 << K) + 16383) >> 14 <= nb1 && K + sbits <= 32) {
+    if (set_tag_map(idx, nb1, p)) {
         p.t1_buckets = (uint32_t)nb1;
         p.t1_limit = (uint32_t)(nb1 * 14);
-        p.tag_kmask = (uint32_t)(((uint64_t)1 << K) - 1);
-        p.tag_shift = K + sbits;
-        p.tag_magic = (uint32_t)((((uint64_t)1 << (K + sbits)) + nb1 - 1) / nb1);
     }
     // level 1 pays for itself only while enough warps stay resident: at C2 (24 -> 20 one-warp CTAs per SM) it removes
     // the table traffic (8.8 -> 5.3 GB of DRAM traffic per 10K queries) and is 2 % faster, at C3 (12 -> 10) it is 11 % slower
@@ -628,12 +622,8 @@ static int v2_prepare_schema(const dab_index* idx, uint32_t l_search, uint32_t b
     if (any_len) out.kern = search_kernel_v2<TD, S::KIND, S::POST, 0, false, false>;
     else if constexpr (S::NA == 4)
         out.kern = cap <= 128 ? pick_v2<TD, S::KIND, S::POST, 4>(l1, reg) : pick_v2<TD, S::KIND, S::POST, 8>(l1, reg);
-    int per_sm = 0;
-    if (cudaFuncSetAttribute(out.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)out.smem_block) != cudaSuccess ||
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, out.kern, kV2Warps * 32, out.smem_block) != cudaSuccess || per_sm < 1) {
-        cudaGetLastError();
-        return too_big();
-    }
+    const int per_sm = ctas_per_sm(out.kern, kV2Warps * 32, out.smem_block);
+    if (per_sm < 1) return too_big();
     out.grid = per_sm * idx->sm_count;
     return 0;
 }

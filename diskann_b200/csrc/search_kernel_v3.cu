@@ -24,6 +24,7 @@
 #include "dab_common.cuh"
 #include "distance_device.cuh"
 #include "search_common.cuh"
+#include "search_host.cuh"
 #include "search_smem.cuh"
 #include "search_v3.cuh"
 
@@ -254,8 +255,7 @@ static int v3_prepare_schema(const dab_index* idx, uint32_t l_search, uint32_t b
     if (idx->max_degree > 1000) return 1;
     if ((idx->row_stride & 15) != 0) return 1;
     // quotient tags: ids < 2^K, tag = h / n_buckets must fit 14 bits
-    uint32_t K = 8;
-    while (((uint64_t)1 << K) < idx->n_total()) ++K;
+    const uint32_t K = tag_id_bits(idx->n_total());
     if (K > 30) return 1;
     const uint64_t min_buckets = std::max<uint64_t>(16, (((uint64_t)1 << K) + 16383) >> 14);
 
@@ -293,14 +293,9 @@ static int v3_prepare_schema(const dab_index* idx, uint32_t l_search, uint32_t b
         tbytes = (long long)round_up((size_t)((visited_need + idx->max_degree) / 0.875) * 2 + 32, 32);
     if (tbytes < (long long)min_buckets * 32) tbytes = (long long)min_buckets * 32;
     if (tbytes > table_bytes_at(1)) return 1;
-    uint64_t nbk = (uint64_t)tbytes / 32;
-    uint32_t sbits = 0;
-    while (((uint64_t)1 << sbits) < nbk) ++sbits;
-    if (K + sbits > 32) return 1;
+    const uint64_t nbk = (uint64_t)tbytes / 32;
+    if (!set_tag_map(idx, nbk, p)) return 1;
     p.n_buckets = (uint32_t)nbk;
-    p.tag_kmask = (uint32_t)(((uint64_t)1 << K) - 1);
-    p.tag_shift = K + sbits;
-    p.tag_magic = (uint32_t)((((uint64_t)1 << (K + sbits)) + nbk - 1) / nbk);
     p.visited_limit = (uint32_t)(nbk * 14);  // 87.5 % of 16 tags per bucket
     p.fast_nm = (idx->dtype == DAB_F32 && idx->dim % 32 == 0 && idx->dim <= 128) ? idx->dim / 32 : 0;
     out.capacity = p.visited_limit > idx->max_degree ? p.visited_limit - idx->max_degree : 0;
@@ -314,15 +309,8 @@ static int v3_prepare_schema(const dab_index* idx, uint32_t l_search, uint32_t b
     if constexpr (std::is_same<TD, float>::value) {
         if (p.fast_nm) out.kern = search_kernel_v3<TD, S::KIND, S::POST, 4, true>;
     }
-    if (cudaFuncSetAttribute(out.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)out.smem_block) != cudaSuccess) {
-        cudaGetLastError();
-        return 1;
-    }
-    int per_sm = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, out.kern, kV3Warps * 32, out.smem_block) != cudaSuccess || per_sm < 1) {
-        cudaGetLastError();
-        return 1;
-    }
+    const int per_sm = ctas_per_sm(out.kern, kV3Warps * 32, out.smem_block);
+    if (per_sm < 1) return 1;
     out.grid = per_sm * idx->sm_count;
     return 0;
 }

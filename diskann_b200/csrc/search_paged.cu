@@ -624,12 +624,9 @@ int plan_kernel(dab_paged* s, void (*kern)(const PagedParams), size_t qbytes, in
     p.warp_smem = (uint32_t)round_up(off, 128);
     s->smem_block = (size_t)p.warp_smem * kPagedWarps;
     s->kern = kern;
-    int per_sm = 0;
-    if (s->smem_block > 200 * 1024 || cudaFuncSetAttribute(s->kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s->smem_block) != cudaSuccess ||
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, s->kern, kPagedWarps * 32, s->smem_block) != cudaSuccess || per_sm < 1) {
-        cudaGetLastError();
+    const int per_sm = s->smem_block > 200 * 1024 ? 0 : ctas_per_sm(s->kern, kPagedWarps * 32, s->smem_block);
+    if (per_sm < 1)
         return fail(DAB_ERR_INVALID_ARGUMENT, "%s: L=%u, dim=%u need %zu B shared memory per CTA", who, s->l_search, idx->dim, s->smem_block);
-    }
     s->grid = std::min(per_sm, max_per_sm) * idx->sm_count;
     return DAB_OK;
 }
@@ -750,12 +747,7 @@ int begin_session(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_s
     PagedParams& p = s->p;
     p.vectors = idx->d_vectors;
     p.row_stride = idx->row_stride;
-    p.adj = idx->d_adj;
-    p.adj_stride = idx->adj_stride;
-    p.n_points = idx->n_points;
-    p.n_start = idx->n_start;
-    p.dim = idx->dim;
-    p.max_degree = idx->max_degree;
+    set_graph_params(idx, p);
     p.queries = s->d_queries;
     p.counters = s->d_counters;
     p.overflow_list = s->d_counters + 2;

@@ -57,6 +57,18 @@ struct SearchParamsPq {
     int code_nbits, code_metric;
 };
 
+// search_kernel_pq.cu
+using PqKernel = void (*)(const SearchParamsPq);
+// search_kernel_pq's instantiation for lists of `cap` entries over `store`
+PqKernel pq_kernel(uint32_t cap, QuantStore store);
+// The rerank of lists of list_cap entries fits a CTA of this index's schema
+int check_rerank(const dab_index* idx, uint32_t list_cap);
+// Reranks each query's list (d_list [nq][list_cap], d_list_n [nq]) by full-precision distance, the start points and the ids
+// `deleted` marks (may be NULL) dropped: the first k into d_ids / d_dists [nq][k] and d_counts, queued on `stream`
+int launch_rerank(const dab_index* idx, cudaStream_t stream, const void* d_queries, uint32_t nq, uint32_t k, uint32_t list_cap,
+                  const uint32_t* d_list, const uint32_t* d_list_n, uint32_t* d_ids, float* d_dists, uint32_t* d_counts,
+                  const uint32_t* deleted);
+
 // search_kernel_pqs.cu — the shape of one launch of the shared-memory-pivot kernel
 struct PqsPlan {
     int warps;         // warps (= queries in flight) per CTA, one CTA per SM

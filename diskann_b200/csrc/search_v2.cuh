@@ -1,5 +1,5 @@
 // search_v2.cuh — launch parameters of search_kernel_v2, shared by the kernel
-// (search_kernel_v2.cu) and the host dispatcher (run_search, search_kernel.cu).
+// (search_kernel_v2.cu) and the host dispatcher (SlotJob, search_kernel.cu).
 #pragma once
 
 #include "dab_common.cuh"

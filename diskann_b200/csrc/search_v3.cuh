@@ -1,5 +1,5 @@
 // search_v3.cuh — launch parameters of search_kernel_v3 (visited set in shared memory), shared by
-// the kernel (search_kernel_v3.cu) and the host dispatcher (run_search, search_kernel.cu).
+// the kernel (search_kernel_v3.cu) and the host dispatcher (SlotJob, search_kernel.cu).
 #pragma once
 
 #include "dab_common.cuh"
