@@ -86,6 +86,7 @@ SYMBOLS = {
     "dab_search_batch_minmax_device": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _i, _vp, _vp, _vp, _vp, _vp]),
     "dab_robust_prune": (_i, [_vp, _vp, _vp, _vp, _vp, _u32, _u32, _u32, _f, _vp, _vp]),
     "dab_build": (_i, [_vp, _u32, _u32, _f, _u32]),
+    "dab_insert": (_i, [_vp, _vp, _vp, _u64, _u32, _u32, _f, _u32]),
     "dab_delete": (_i, [_vp, _vp, _u64]),
     "dab_release": (_i, [_vp, _vp, _u64]),
     "dab_delete_status": (_i, [_vp, _vp, _u64, _vp]),

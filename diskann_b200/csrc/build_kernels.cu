@@ -664,6 +664,102 @@ struct DevBuf {
     }
 };
 
+// One multi_insert (index.rs:815-1030, intra_batch_candidates = None, no bootstrap) over the ids in `batch`, on the graph
+// the previous step left; dab_build and dab_insert run their batches through it.
+//   1. every member is searched against the graph as it was before the step (beam 1, l_build), recording the nodes it
+//      expanded (VisitedSearchRecord, index.rs:276-282; the record is sized generously and a search that still outgrows
+//      it is counted in rec_truncated);
+//   2. each member's record is pruned to pruned_degree (index.rs:2349-2380) and its out-list written;
+//   3. the back-edges are grouped by target (aggregate_backedges, index.rs:123-143; stable radix sort) and each target
+//      gets one add_edge_and_prune (index.rs:2264-2341) with max_backedges = pruned_degree.
+// backedge_kernel takes a target's sources in the order the pairs arrive, and add_edge_and_prune takes them sorted
+// (index.rs:986-992): the ids in `batch` must be ascending.  Steps 1 and 2 do not depend on the members' order.
+struct LinkStep {
+    DevBuf batch, rec_ids, rec_d, rec_n, nbr, nbr_n, keys, vals, keys2, vals2, tmp, res_ids, res_d, dropped;
+    size_t tmp_bytes = 0;
+    uint32_t rec_cap = 0, pruned_degree = 0, l_build = 0;
+    float alpha = 0.0f;
+
+    // buffers for steps of up to `cap` ids
+    int alloc(dab_index* idx, uint32_t cap, uint32_t pruned_degree_, uint32_t l_build_, float alpha_) {
+        pruned_degree = pruned_degree_, l_build = l_build_, alpha = alpha_;
+        rec_cap = std::min<uint32_t>(2048, 4 * l_build + 64);
+        idx->rec_truncated = 0;
+        int rc;
+        const size_t B = cap;
+        if ((rc = batch.alloc(B * 4)) || (rc = rec_ids.alloc(B * rec_cap * 4)) || (rc = rec_d.alloc(B * rec_cap * 4)) ||
+            (rc = rec_n.alloc(B * 4)) || (rc = nbr.alloc(B * pruned_degree * 4)) || (rc = nbr_n.alloc(B * 4)) ||
+            (rc = keys.alloc(B * pruned_degree * 4)) || (rc = vals.alloc(B * pruned_degree * 4)) ||
+            (rc = keys2.alloc(B * pruned_degree * 4)) || (rc = vals2.alloc(B * pruned_degree * 4)) || (rc = res_ids.alloc(B * 4)) ||
+            (rc = res_d.alloc(B * 4)))
+            return rc;
+        if ((rc = dropped.alloc(4))) return rc;
+        DAB_CUDA(cudaMemsetAsync(dropped.p, 0, 4, idx->stream));
+        cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, (const uint32_t*)keys.p, (uint32_t*)keys2.p, (const uint32_t*)vals.p,
+                                        (uint32_t*)vals2.p, (int)(B * pruned_degree), 0, 32, idx->stream);
+        return tmp.alloc(tmp_bytes);
+    }
+
+    // one step over batch[0, b)
+    int run(dab_index* idx, uint32_t b) {
+        cudaStream_t st = idx->stream;
+        int rc;
+        const SearchRecord rec{(const uint32_t*)batch.p, (uint32_t*)rec_ids.p, (float*)rec_d.p, (uint32_t*)rec_n.p, rec_cap};
+        // 1. search the batch against the current graph, recording expanded nodes
+        if ((rc = run_search(idx, nullptr, b, 1, l_build, 1, SearchOut{(uint32_t*)res_ids.p, (float*)res_d.p, nullptr, nullptr, nullptr},
+                             -1, false, &rec)))
+            return rc;
+        // 2. robust_prune each point's visited pool -> out-edges
+        PruneParams pp;
+        memset(&pp, 0, sizeof(pp));
+        pp.pool_ids = (const uint32_t*)rec_ids.p;
+        pp.pool_d = (const float*)rec_d.p;
+        pp.pool_len = (const uint32_t*)rec_n.p;
+        pp.pool_cap = rec_cap;
+        pp.locations = (const uint32_t*)batch.p;
+        pp.n_pools = b;
+        pp.degree = pruned_degree;
+        pp.alpha = alpha;
+        pp.out_ids = (uint32_t*)nbr.p;
+        pp.out_counts = (uint32_t*)nbr_n.p;
+        pp.adj = idx->d_adj;
+        pp.adj_stride = idx->adj_stride;
+        if ((rc = launch_prune(idx, pp))) return rc;
+        // 3. back-edges grouped by destination
+        const uint32_t n_pairs = b * pruned_degree;
+        make_pairs_kernel<<<(n_pairs + 255) / 256, 256, 0, st>>>((const uint32_t*)batch.p, (const uint32_t*)nbr.p, (const uint32_t*)nbr_n.p, b,
+                                                                 pruned_degree, pruned_degree, (uint32_t*)keys.p, (uint32_t*)vals.p);
+        DAB_LAUNCHED();
+        cudaError_t e = cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, (const uint32_t*)keys.p, (uint32_t*)keys2.p, (const uint32_t*)vals.p,
+                                                        (uint32_t*)vals2.p, (int)n_pairs, 0, 32, st);
+        if (e != cudaSuccess) return fail(DAB_ERR_CUDA, "build: radix sort failed: %s", cudaGetErrorString(e));
+        DAB_LAUNCHED();
+        BackedgeParams bp;
+        memset(&bp, 0, sizeof(bp));
+        bp.keys = (const uint32_t*)keys2.p;
+        bp.vals = (const uint32_t*)vals2.p;
+        bp.n_pairs = n_pairs;
+        bp.degree = pruned_degree;
+        bp.alpha = alpha;
+        bp.dropped = (uint32_t*)dropped.p;
+        return launch_backedges(idx, bp);
+    }
+
+    // after the last step: dropped back-edges and truncated records, reported under `who`
+    int report(dab_index* idx, const char* who) {
+        uint32_t n_dropped = 0;
+        DAB_CUDA(cudaMemcpyAsync(&n_dropped, dropped.p, 4, cudaMemcpyDeviceToHost, idx->stream));
+        DAB_CUDA(cudaStreamSynchronize(idx->stream));
+        if (n_dropped)
+            return fail(DAB_ERR_INVALID_ARGUMENT, "%s: %u back-edges exceeded the per-destination list of a batch and were dropped "
+                        "(the graph is usable but not the reference's; use a smaller batch_size)", who, n_dropped);
+        if (idx->rec_truncated)
+            return fail(DAB_ERR_INVALID_ARGUMENT, "%s: %llu insert searches expanded more than %u nodes; their prune pools were cut "
+                        "(the graph is usable but not the reference's)", who, (unsigned long long)idx->rec_truncated, rec_cap);
+        return DAB_OK;
+    }
+};
+
 }  // namespace dab
 
 using namespace dab;
@@ -783,91 +879,66 @@ int dab_build(dab_index* idx, uint32_t pruned_degree, uint32_t l_build, float al
     DAB_CUDA(cudaSetDevice(idx->device));
     const uint32_t n = (uint32_t)idx->n_points;
     if (batch_size == 0) batch_size = std::max<uint32_t>(1024, std::min<uint32_t>(65536, n / 16));
-    // VisitedSearchRecord keeps every expanded node (index.rs:276-282; SortedNeighbors truncates to the 750
-    // closest afterwards): the record is sized generously and a search that still outgrows it is reported
-    const uint32_t rec_cap = std::min<uint32_t>(2048, 4 * l_build + 64);
-    idx->rec_truncated = 0;
     cudaStream_t st = idx->stream;
 
     DAB_CUDA(cudaMemsetAsync(idx->d_adj, 0, idx->n_total() * (size_t)idx->adj_stride * 4, st));
     idx->graph_ready = true;
     ++idx->generation;
 
-    DevBuf b_batch, b_rec_ids, b_rec_d, b_rec_n, b_nbr, b_nbr_n, b_keys, b_vals, b_keys2, b_vals2, b_tmp, b_res_ids, b_res_d, b_dropped;
+    LinkStep step;
     int rc;
-    const size_t B = batch_size;
-    if ((rc = b_batch.alloc(B * 4)) || (rc = b_rec_ids.alloc(B * rec_cap * 4)) || (rc = b_rec_d.alloc(B * rec_cap * 4)) ||
-        (rc = b_rec_n.alloc(B * 4)) || (rc = b_nbr.alloc(B * pruned_degree * 4)) || (rc = b_nbr_n.alloc(B * 4)) ||
-        (rc = b_keys.alloc(B * pruned_degree * 4)) || (rc = b_vals.alloc(B * pruned_degree * 4)) ||
-        (rc = b_keys2.alloc(B * pruned_degree * 4)) || (rc = b_vals2.alloc(B * pruned_degree * 4)) || (rc = b_res_ids.alloc(B * 4)) ||
-        (rc = b_res_d.alloc(B * 4)))
-        return rc;
-    if ((rc = b_dropped.alloc(4))) return rc;
-    DAB_CUDA(cudaMemsetAsync(b_dropped.p, 0, 4, st));
-    size_t tmp_bytes = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, (const uint32_t*)b_keys.p, (uint32_t*)b_keys2.p, (const uint32_t*)b_vals.p,
-                                    (uint32_t*)b_vals2.p, (int)(B * pruned_degree), 0, 32, st);
-    if ((rc = b_tmp.alloc(tmp_bytes))) return rc;
-
-    const SearchRecord rec{(const uint32_t*)b_batch.p, (uint32_t*)b_rec_ids.p, (float*)b_rec_d.p, (uint32_t*)b_rec_n.p, rec_cap};
+    if ((rc = step.alloc(idx, batch_size, pruned_degree, l_build, alpha))) return rc;
     uint32_t inserted = 0;
     while (inserted < n) {
         // batches grow with the graph so that early points are not all inserted blind
         uint32_t b = std::min<uint32_t>(batch_size, std::max<uint32_t>(1, inserted / 8));
         b = std::min(b, n - inserted);
-        iota_kernel<<<(b + 255) / 256, 256, 0, st>>>((uint32_t*)b_batch.p, inserted, b);
+        iota_kernel<<<(b + 255) / 256, 256, 0, st>>>((uint32_t*)step.batch.p, inserted, b);
         DAB_LAUNCHED();
-        // 1. search the batch against the current graph, recording expanded nodes
-        if ((rc = run_search(idx, nullptr, b, 1, l_build, 1, SearchOut{(uint32_t*)b_res_ids.p, (float*)b_res_d.p, nullptr, nullptr, nullptr},
-                             -1, false, &rec)))
-            return rc;
-        // 2. robust_prune each point's visited pool -> out-edges
-        PruneParams pp;
-        memset(&pp, 0, sizeof(pp));
-        pp.pool_ids = (const uint32_t*)b_rec_ids.p;
-        pp.pool_d = (const float*)b_rec_d.p;
-        pp.pool_len = (const uint32_t*)b_rec_n.p;
-        pp.pool_cap = rec_cap;
-        pp.locations = (const uint32_t*)b_batch.p;
-        pp.n_pools = b;
-        pp.degree = pruned_degree;
-        pp.alpha = alpha;
-        pp.out_ids = (uint32_t*)b_nbr.p;
-        pp.out_counts = (uint32_t*)b_nbr_n.p;
-        pp.adj = idx->d_adj;
-        pp.adj_stride = idx->adj_stride;
-        if ((rc = launch_prune(idx, pp))) return rc;
-        // 3. back-edges grouped by destination
-        const uint32_t n_pairs = b * pruned_degree;
-        make_pairs_kernel<<<(n_pairs + 255) / 256, 256, 0, st>>>((const uint32_t*)b_batch.p, (const uint32_t*)b_nbr.p,
-                                                                 (const uint32_t*)b_nbr_n.p, b, pruned_degree, pruned_degree,
-                                                                 (uint32_t*)b_keys.p, (uint32_t*)b_vals.p);
-        DAB_LAUNCHED();
-        cudaError_t e = cub::DeviceRadixSort::SortPairs(b_tmp.p, tmp_bytes, (const uint32_t*)b_keys.p, (uint32_t*)b_keys2.p,
-                                                        (const uint32_t*)b_vals.p, (uint32_t*)b_vals2.p, (int)n_pairs, 0, 32, st);
-        if (e != cudaSuccess) return fail(DAB_ERR_CUDA, "build: radix sort failed: %s", cudaGetErrorString(e));
-        DAB_LAUNCHED();
-        BackedgeParams bp;
-        memset(&bp, 0, sizeof(bp));
-        bp.keys = (const uint32_t*)b_keys2.p;
-        bp.vals = (const uint32_t*)b_vals2.p;
-        bp.n_pairs = n_pairs;
-        bp.degree = pruned_degree;
-        bp.alpha = alpha;
-        bp.dropped = (uint32_t*)b_dropped.p;
-        if ((rc = launch_backedges(idx, bp))) return rc;
+        if ((rc = step.run(idx, b))) return rc;
         inserted += b;
     }
-    uint32_t dropped = 0;
-    DAB_CUDA(cudaMemcpyAsync(&dropped, b_dropped.p, 4, cudaMemcpyDeviceToHost, st));
-    DAB_CUDA(cudaStreamSynchronize(st));
-    if (dropped)
-        return fail(DAB_ERR_INVALID_ARGUMENT, "dab_build: %u back-edges exceeded the per-destination list of a batch and were dropped "
-                    "(the graph is usable but not the reference's; use a smaller batch_size)", dropped);
-    if (idx->rec_truncated)
-        return fail(DAB_ERR_INVALID_ARGUMENT, "dab_build: %llu insert searches expanded more than %u nodes; their prune pools were cut "
-                    "(the graph is usable but not the reference's)", (unsigned long long)idx->rec_truncated, rec_cap);
-    return DAB_OK;
+    return step.report(idx, "dab_build");
+}
+
+int dab_insert(dab_index* idx, const uint32_t* ids, const void* rows, uint64_t n, uint32_t pruned_degree, uint32_t l_build, float alpha,
+               uint32_t batch_size) {
+    static const char* who = "dab_insert";
+    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", who);
+    if (n && (!ids || !rows)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", who);
+    if (pruned_degree == 0 || pruned_degree > idx->max_degree)
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: pruned_degree must be in [1, max_degree]", who);
+    if (l_build == 0) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: l_build must be > 0", who);
+    if (!(alpha >= 1.0f)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: alpha must be >= 1", who);
+    int rc;
+    if ((rc = refuse_in_flight(idx, who))) return rc;
+    if ((rc = insert_check_ids(idx, ids, n, who))) return rc;
+    if (!idx->vectors_ready) return fail(DAB_ERR_NOT_READY, "%s: vectors (including start rows) must be uploaded first", who);
+    if (idx->n_start == 0) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: the index needs at least one start point", who);
+    if (n == 0) return DAB_OK;
+    DAB_CUDA(cudaSetDevice(idx->device));
+    // set_element: the rows and every store that holds rows; nothing is written when an encoder's check fails
+    if ((rc = insert_rows(idx, ids, rows, n, who))) return rc;
+    cudaStream_t st = idx->stream;
+    if (!idx->graph_ready) {  // never uploaded or built: start from empty adjacency, as dab_build does
+        DAB_CUDA(cudaMemsetAsync(idx->d_adj, 0, idx->n_total() * (size_t)idx->adj_stride * 4, st));
+        idx->graph_ready = true;
+    }
+    ++idx->generation;
+    if (batch_size == 0) batch_size = 65536;  // the cap of dab_build's default batch size
+    const uint32_t cap = (uint32_t)std::min<uint64_t>(batch_size, n);
+    LinkStep step;
+    if ((rc = step.alloc(idx, cap, pruned_degree, l_build, alpha))) return rc;
+    // consecutive chunks in the caller's order, each one multi_insert; a chunk goes to the step sorted ascending
+    std::vector<uint32_t> chunk;
+    for (uint64_t first = 0; first < n; first += cap) {
+        const uint32_t b = (uint32_t)std::min<uint64_t>(cap, n - first);
+        chunk.assign(ids + first, ids + first + b);
+        std::sort(chunk.begin(), chunk.end());
+        DAB_CUDA(cudaMemcpyAsync(step.batch.p, chunk.data(), (size_t)b * 4, cudaMemcpyHostToDevice, st));
+        if ((rc = step.run(idx, b))) return rc;
+    }
+    return step.report(idx, who);
 }
 
 }  // extern "C"

@@ -147,6 +147,26 @@ size_t stage_query_bytes(const CodeStore& s, uint32_t nq, size_t work);
 // T::as_f32 of n rows of the index dtype, src_stride bytes apart -> dst [n][dim], queued on `stream`
 int widen_rows(const struct ::dab_index* idx, cudaStream_t stream, const void* src, size_t src_stride, uint64_t n, float* dst);
 
+// The store encoders over n rows of the index dtype, src_stride bytes apart, into any codes / meta arrays ([n] rows at
+// the store's device layout), queued on `stream`.
+// quant_kernels.cu: BasicTable::compress_into of n f32 rows on the idx stream (synchronizes); fails naming the first row
+// infinitely far from every centre, numbered from first_row
+int pq_encode_device(struct ::dab_index* idx, const float* d_vectors, uint64_t n, uint8_t* d_codes_out, uint64_t first_row);
+// sq_index.cu: SQStore::set_vector
+int sq_encode_rows(const struct ::dab_index* idx, cudaStream_t stream, const uint8_t* src, size_t src_stride, uint64_t n, uint8_t* codes,
+                   float* comp);
+// minmax_index.cu: as_f32 -> transform -> compress, in `work` (minmax_encode_bytes(idx, n) bytes); *h_first_nan (host,
+// valid once the stream is synchronized) takes the first row whose transformed vector holds a NaN, else ~0
+size_t minmax_encode_bytes(const struct ::dab_index* idx, uint64_t n);
+int minmax_encode_rows(const struct ::dab_index* idx, cudaStream_t stream, uint8_t* work, const void* src, size_t src_stride, uint64_t n,
+                       uint8_t* codes, float* meta, unsigned long long* h_first_nan);
+
+// insert_rows.cu, for dab_insert: "<who>: ..." naming the first id that is not a data point, repeats or is deleted
+int insert_check_ids(const struct ::dab_index* idx, const uint32_t* ids, uint64_t n, const char* who);
+// rows[i] -> row ids[i] of the index and of every quantized store that holds rows, encoded as the encode-all calls
+// encode; every encoder check runs before anything is written
+int insert_rows(struct ::dab_index* idx, const uint32_t* ids, const void* rows, uint64_t n, const char* who);
+
 }  // namespace dab
 
 struct dab_index {

@@ -61,6 +61,19 @@ Staging staging_layout(const dab_index* idx, uint64_t n, uint8_t* base) {
 
 }  // namespace
 
+size_t minmax_encode_bytes(const dab_index* idx, uint64_t n) { return staging_bytes(idx, n); }
+
+int minmax_encode_rows(const dab_index* idx, cudaStream_t stream, uint8_t* work, const void* src, size_t src_stride, uint64_t n, uint8_t* codes,
+                       float* meta, unsigned long long* h_first_nan) {
+    const Staging s = staging_layout(idx, n, work);
+    int rc;
+    DAB_CUDA(cudaMemsetAsync(s.flag, 0xFF, 8, stream));
+    if ((rc = compress_rows(idx, stream, src, src_stride, n, s.work, s.canon, s.flag))) return rc;
+    if ((rc = store_split(idx, stream, idx->mm, s.canon, n, codes, meta, nullptr))) return rc;
+    DAB_CUDA(cudaMemcpyAsync(h_first_nan, s.flag, 8, cudaMemcpyDeviceToHost, stream));
+    return DAB_OK;
+}
+
 void minmax_release(dab_index* idx) {
     cudaFree(idx->d_mm_tables);
     delete idx->mm_transform;
@@ -139,14 +152,12 @@ int dab_minmax_encode_all(dab_index* idx) {
     const uint64_t per_row = (uint64_t)(idx->dim + (idx->mm_transform ? mm.dim : 0)) * 4 + mm.row_bytes;
     const uint64_t slab = std::max<uint64_t>(1, std::min<uint64_t>(total, (256ull << 20) / per_row));
     if ((rc = idx->s_stage.reserve(staging_bytes(idx, slab)))) return rc;
-    const Staging s = staging_layout(idx, slab, (uint8_t*)idx->s_stage.p);
     for (uint64_t first = 0; first < total; first += slab) {
         const uint64_t cnt = std::min(slab, total - first);
-        DAB_CUDA(cudaMemsetAsync(s.flag, 0xFF, 8, idx->stream));
-        if ((rc = compress_rows(idx, idx->stream, idx->d_vectors + first * idx->row_stride, idx->row_stride, cnt, s.work, s.canon, s.flag))) return rc;
-        if ((rc = store_split(idx, idx->stream, mm, s.canon, cnt, mm.d_codes + first * mm.stride, mm.d_meta + first * mm.meta_words, nullptr))) return rc;
         unsigned long long first_nan = ~0ull;
-        DAB_CUDA(cudaMemcpyAsync(&first_nan, s.flag, 8, cudaMemcpyDeviceToHost, idx->stream));
+        if ((rc = minmax_encode_rows(idx, idx->stream, (uint8_t*)idx->s_stage.p, idx->d_vectors + first * idx->row_stride, idx->row_stride, cnt,
+                                     mm.d_codes + first * mm.stride, mm.d_meta + first * mm.meta_words, &first_nan)))
+            return rc;
         DAB_CUDA(cudaStreamSynchronize(idx->stream));
         if (first_nan != ~0ull)
             return fail(DAB_ERR_INVALID_ARGUMENT, "%s: row %llu contains NaN after the transform (InputContainsNaN)", who,

@@ -299,9 +299,6 @@ struct DevMem {
 
 }  // namespace
 
-// defined in quant_kernels.cu
-int pq_encode_device(dab_index* idx, const float* d_vectors, uint64_t n, uint8_t* d_codes_out);
-
 }  // namespace dab
 
 using namespace dab;
@@ -430,7 +427,7 @@ int dab_pq_encode_all(dab_index* idx) {
     for (uint64_t first = 0; first < total; first += batch) {
         const uint64_t cnt = std::min(batch, total - first);
         if ((rc = widen_rows(idx, idx->stream, idx->d_vectors + first * idx->row_stride, idx->row_stride, cnt, d_f32))) return rc;
-        if ((rc = pq_encode_device(idx, d_f32, cnt, idx->d_codes + first * idx->pq_chunks))) return rc;
+        if ((rc = pq_encode_device(idx, d_f32, cnt, idx->d_codes + first * idx->pq_chunks, 0))) return rc;
     }
     idx->pq_codes_ready = true;
     return DAB_OK;

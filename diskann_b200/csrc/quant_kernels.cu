@@ -446,7 +446,7 @@ namespace dab {
 // pq_encode_kernel over n f32 vectors already on the device; codes written to d_codes_out (device).
 // Used by dab_pq_encode_all (pq_train.cu).  Rows that are infinitely far from every centre
 // (inf / NaN input) are reported like BasicTable::compress_into does.
-int pq_encode_device(dab_index* idx, const float* d_vectors, uint64_t n, uint8_t* d_codes_out) {
+int pq_encode_device(dab_index* idx, const float* d_vectors, uint64_t n, uint8_t* d_codes_out, uint64_t first_row) {
     int rc;
     if ((rc = idx->s_counters.reserve(16))) return rc;
     unsigned long long* d_bad = (unsigned long long*)idx->s_counters.p;
@@ -462,7 +462,7 @@ int pq_encode_device(dab_index* idx, const float* d_vectors, uint64_t n, uint8_t
     DAB_CUDA(cudaStreamSynchronize(idx->stream));
     if (bad != ~0ull)
         return fail(DAB_ERR_INVALID_ARGUMENT, "pq encode: vector %llu chunk %llu is infinitely far from every center (inf/NaN input)",
-                    bad / idx->pq_chunks, bad % idx->pq_chunks);
+                    first_row + bad / idx->pq_chunks, bad % idx->pq_chunks);
     return DAB_OK;
 }
 }  // namespace dab

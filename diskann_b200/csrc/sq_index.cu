@@ -103,6 +103,23 @@ __global__ void __launch_bounds__(128) sq_stage_kernel(const T* __restrict__ que
 
 }  // namespace
 
+int sq_encode_rows(const dab_index* idx, cudaStream_t stream, const uint8_t* src, size_t src_stride, uint64_t n, uint8_t* codes, float* comp) {
+    const int grid = (int)std::min<uint64_t>((n + 127) / 128, (uint64_t)idx->sm_count * 16);
+    const CodeStore& s = idx->sq;
+#define DAB_SQ_ENCODE(T) \
+    sq_encode_rows_kernel<T><<<grid, 128, 0, stream>>>(src, src_stride, n, idx->dim, idx->d_sq_shift, idx->sq_scale, s.nbits, s.stride, codes, comp)
+    switch (idx->dtype) {
+        case DAB_F32: DAB_SQ_ENCODE(float); break;
+        case DAB_F16: DAB_SQ_ENCODE(__half); break;
+        case DAB_I8: DAB_SQ_ENCODE(int8_t); break;
+        default: DAB_SQ_ENCODE(uint8_t); break;
+    }
+#undef DAB_SQ_ENCODE
+    DAB_LAUNCHED();
+    DAB_CUDA(cudaGetLastError());
+    return DAB_OK;
+}
+
 size_t sq_stage_bytes(const dab_index* idx, uint32_t nq) { return stage_query_bytes(idx->sq, nq, (size_t)nq * idx->dim * 4); }
 
 int sq_stage_queries(const dab_index* idx, cudaStream_t stream, Scratch& stage, const void* d_queries, uint32_t nq, const uint8_t** d_qcodes,
@@ -165,21 +182,7 @@ int dab_sq_encode_all(dab_index* idx) {
     if (!idx->vectors_ready) return fail(DAB_ERR_NOT_READY, "dab_sq_encode_all: vectors not uploaded");
     DAB_CUDA(cudaSetDevice(idx->device));
     ++idx->store_writes[STORE_SQ];
-    const uint64_t total = idx->n_total();
-    const int grid = (int)std::min<uint64_t>((total + 127) / 128, (uint64_t)idx->sm_count * 16);
-    const CodeStore& s = idx->sq;
-#define DAB_SQ_ENCODE(T)                                                                                                       \
-    sq_encode_rows_kernel<T><<<grid, 128, 0, idx->stream>>>(idx->d_vectors, idx->row_stride, total, idx->dim, idx->d_sq_shift, \
-                                                            idx->sq_scale, s.nbits, s.stride, s.d_codes, s.d_meta)
-    switch (idx->dtype) {
-        case DAB_F32: DAB_SQ_ENCODE(float); break;
-        case DAB_F16: DAB_SQ_ENCODE(__half); break;
-        case DAB_I8: DAB_SQ_ENCODE(int8_t); break;
-        default: DAB_SQ_ENCODE(uint8_t); break;
-    }
-#undef DAB_SQ_ENCODE
-    DAB_LAUNCHED();
-    DAB_CUDA(cudaGetLastError());
+    if ((rc = sq_encode_rows(idx, idx->stream, idx->d_vectors, idx->row_stride, idx->n_total(), idx->sq.d_codes, idx->sq.d_meta))) return rc;
     DAB_CUDA(cudaStreamSynchronize(idx->stream));
     idx->sq.ready = true;
     return DAB_OK;

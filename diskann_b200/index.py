@@ -655,6 +655,15 @@ class GpuIndex:
     def build(self, pruned_degree, l_build, alpha=1.2, batch_size=0):
         check(_lib.lib().dab_build(self._h, pruned_degree, l_build, alpha, batch_size))
 
+    def insert(self, ids, rows, pruned_degree, l_build, alpha=1.2, batch_size=0):
+        """DiskANNIndex::insert / multi_insert into the graph as it stands: rows[i] becomes point ids[i] (in the index and
+        in every quantized store that holds rows) and is linked in consecutive chunks of batch_size (0: 65536)."""
+        ids = np.ascontiguousarray(ids, np.uint32).ravel()
+        rows = self._rows(rows)
+        if rows.shape[0] != ids.shape[0]:
+            raise DabError(1, f"insert: {ids.shape[0]} ids for {rows.shape[0]} rows")
+        check(_lib.lib().dab_insert(self._h, _ptr(ids), _ptr(rows), ids.shape[0], pruned_degree, l_build, alpha, batch_size))
+
     # -- deletion (Delete of the providers' TableDeleteProviderAsync; DiskANNIndex::consolidate_vector)
     def delete(self, ids):
         """Marks data points deleted: every k-NN search then leaves them out of its results."""

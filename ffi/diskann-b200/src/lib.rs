@@ -84,6 +84,16 @@ impl<T: Element> GpuIndex<T> {
         check(unsafe { sys::dab_build(self.raw, pruned_degree, l_build, alpha, 0) })
     }
 
+    /// `DiskANNIndex::insert` / `multi_insert` into the graph as it stands: dense rows `[ids.len()][dim]` become the
+    /// points `ids`, linked in consecutive chunks of `batch_size` (0: 65536).
+    pub fn insert(&mut self, ids: &[u32], rows: &[T], pruned_degree: u32, l_build: u32, alpha: f32, batch_size: u32) -> Result<()> {
+        assert_eq!(rows.len(), ids.len() * self.dim, "one row per id");
+        check(unsafe {
+            sys::dab_insert(self.raw, ids.as_ptr(), rows.as_ptr() as *const c_void, ids.len() as u64, pruned_degree, l_build, alpha,
+                            batch_size)
+        })
+    }
+
     /// `Delete::delete`: every k-NN search then leaves these points out of its results.
     pub fn delete(&mut self, ids: &[u32]) -> Result<()> {
         check(unsafe { sys::dab_delete(self.raw, ids.as_ptr(), ids.len() as u64) })

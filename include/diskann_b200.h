@@ -501,6 +501,34 @@ int dab_robust_prune(dab_index* idx, const uint32_t* pool_ids, const float* pool
 int dab_build(dab_index* idx, uint32_t pruned_degree, uint32_t l_build, float alpha,
               uint32_t batch_size);
 
+/* Inserts points into the index as it stands: DiskANNIndex::insert (diskann/src/graph/index.rs:226-341) and multi_insert
+ * (:815-1030).  rows holds [n][dim] values of the index dtype, dense, on the host (as dab_upload_vectors); ids[i] takes
+ * rows[i].
+ *   set_element: every row is written into the index and into each quantized store that holds rows (the PQ codes when
+ *     codes were uploaded or encoded, the SQ and MinMax stores when they hold rows), the aux stores before the base
+ *     store as the inmem providers do (diskann-providers/.../async_/inmem/provider.rs:695-725).  The codes are
+ *     byte-identical to what dab_pq_encode_all, dab_sq_encode_all and dab_minmax_encode_all write for those rows; a store
+ *     without rows stays without rows.  The encoders' checks (a PQ row infinitely far from every centre, a MinMax row
+ *     with a NaN after the transform) run before anything is written and fail naming the caller's row index, leaving the
+ *     rows, every store and the adjacency as they were.
+ *   linking: the ids are cut into consecutive chunks of batch_size in the caller's order (0: 65536, the cap of
+ *     dab_build's default batch size), and each chunk is one multi_insert on the graph the previous chunk left, with
+ *     dab_build's semantics: every member searched against the graph as it was before the chunk (beam 1, l_build, a
+ *     visited record, the deletion table ignored), pruned to pruned_degree and its out-list written, then one
+ *     add_edge_and_prune per back-edge target with its sources sorted; max_backedges = pruned_degree,
+ *     intra_batch_candidates = None, no bootstrap.  batch_size = 1 is DiskANNIndex::insert point by point.  A graph that
+ *     was never uploaded or built starts empty, so an index can be grown from its start points by inserts alone.
+ * Any id in [0, n_points) that is not deleted may be inserted: a row no list reaches, a released slot, or a live point,
+ * whose vector and out-list are then replaced.  DAB_ERR_INVALID_ARGUMENT, changing nothing and naming the first
+ * offending id: an id >= n_points (start points are frozen), a repeated id, a deleted id (dab_release it first); also
+ * NULL pointers with n > 0, pruned_degree outside [1, max_degree], l_build == 0, alpha < 1, or any slot holding a batch
+ * in flight.  DAB_ERR_NOT_READY when no vectors were uploaded.  n == 0 returns DAB_OK after these checks.  Back-edges
+ * dropped and visited records cut are reported as dab_build reports them (the graph is then usable but not the
+ * reference's).  Open paged sessions fail their next page; the tensor-core scan rebuilds its operand on its next use;
+ * dab_flat_knn* still scan every row. */
+int dab_insert(dab_index* idx, const uint32_t* ids, const void* rows, uint64_t n, uint32_t pruned_degree, uint32_t l_build,
+               float alpha, uint32_t batch_size);
+
 /* ------------------------------------------------------------------ deletion */
 
 /* Delete::delete / release / status_by_internal_id of the providers' TableDeleteProviderAsync

@@ -165,6 +165,11 @@ class Provider {
     void build(uint32_t pruned_degree, uint32_t l_build, float alpha = 1.2f, uint32_t batch = 0) {
         check(dab_build(h_, pruned_degree, l_build, alpha, batch));
     }
+    // DiskANNIndex::insert / multi_insert into the graph as it stands: rows [ids.size()][dim] become points ids
+    void insert(const std::vector<uint32_t>& ids, const T* rows, uint32_t pruned_degree, uint32_t l_build, float alpha = 1.2f,
+                uint32_t batch = 0) {
+        check(dab_insert(h_, ids.data(), rows, ids.size(), pruned_degree, l_build, alpha, batch));
+    }
 
     // deletion: Delete::delete / release / status_by_internal_id, and consolidate_vector for every node
     void remove(const std::vector<uint32_t>& ids) { check(dab_delete(h_, ids.data(), ids.size())); }
