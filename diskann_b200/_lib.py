@@ -91,6 +91,8 @@ SYMBOLS = {
     "dab_release": (_i, [_vp, _vp, _u64]),
     "dab_delete_status": (_i, [_vp, _vp, _u64, _vp]),
     "dab_consolidate": (_i, [_vp, _u32, _f, C.POINTER(_u64)]),
+    "dab_inplace_delete": (_i, [_vp, _vp, _u64, _i, _u32, _u32, _u32, _u32, _f, _u32]),
+    "dab_drop_deleted_neighbors": (_i, [_vp, _u32, _i, C.POINTER(_u64)]),
     "dab_flat_knn": (_i, [_vp, _vp, _u32, _u32, _vp, _vp]),
     "dab_flat_knn_tc": (_i, [_vp, _vp, _u32, _u32, _vp, _vp]),
 }

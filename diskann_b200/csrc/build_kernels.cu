@@ -260,6 +260,26 @@ __global__ void __launch_bounds__(kPruneWarps * 32) prune_pools_kernel(const Pru
 }
 
 // ------------------------------------------------------------------ back-edges
+// this lane's share of: src is kNoId (no target) or appears in vals[start, e)
+__device__ __forceinline__ bool segment_repeats(const uint32_t* vals, uint32_t start, uint32_t e, uint32_t src, int lane) {
+    bool hit = src == kNoId;
+    for (uint32_t f = start + lane; f < e; f += 32) hit |= vals[f] == src;
+    return hit;
+}
+
+// id in the ascending a[0, n)
+__device__ __forceinline__ bool sorted_contains(const uint32_t* a, uint32_t n, uint32_t id) {
+    uint32_t lo = 0, hi = n;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (__ldg(a + mid) < id)
+            lo = mid + 1;
+        else
+            hi = mid;
+    }
+    return lo < n && __ldg(a + lo) == id;
+}
+
 struct BackedgeParams {
     const uint8_t* vectors;
     size_t row_stride;
@@ -274,6 +294,10 @@ struct BackedgeParams {
     uint32_t* adj;
     uint32_t adj_stride;
     uint32_t* dropped;      // in-edges that did not fit the per-destination list of a batch
+    // in-place deletes (inplace_backedge_kernel): the ids every visited list loses, ascending
+    const uint32_t* remove;
+    uint32_t n_remove;
+    uint64_t n_total;  // ids at or above it have no row: left out of a prune pool
 };
 
 __global__ void make_pairs_kernel(const uint32_t* __restrict__ batch_ids, const uint32_t* __restrict__ nbr_ids,
@@ -290,8 +314,13 @@ __global__ void make_pairs_kernel(const uint32_t* __restrict__ batch_ids, const 
 
 // One warp per destination segment: add_edge_and_prune (index.rs:2264-2341) with all the incoming
 // edges of the batch at once; on overflow robust_prune_list (index.rs:2397-2454).
-template <typename TD, int NA, int KIND, int POST, bool IS_INT, bool SIGNED>
-__global__ void __launch_bounds__(kPruneWarps * 32) backedge_kernel(const BackedgeParams p) {
+// REMOVE (in-place deletes): the segment's key is add_edge_and_prune's `source` and its values are the targets, in the
+// order they are appended; the ids of p.remove are first taken out of the list (to_remove), a list that lost one is
+// written even when nothing is added, a target already appended earlier in the segment is not appended again
+// (extend_from_slice), a value kNoId only makes the source visited, and a stray id (>= n_total) in an overflowing list
+// is left out of the prune pool.
+template <typename TD, int NA, int KIND, int POST, bool IS_INT, bool SIGNED, bool REMOVE>
+__device__ __forceinline__ void backedge_segments(const BackedgeParams p) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     uint8_t* base = smem + (size_t)wib * (prune_smem_bytes(p.P) + 4 * (size_t)p.P);
@@ -314,6 +343,21 @@ __global__ void __launch_bounds__(kPruneWarps * 32) backedge_kernel(const Backed
             __syncwarp();
             for (uint32_t t = lane; t < deg; t += 32) list[t] = row[1 + t];
             __syncwarp();
+            bool did_remove = false;
+            if constexpr (REMOVE) {
+                uint32_t kept = 0;
+                for (uint32_t c0 = 0; c0 < deg; c0 += 32) {
+                    const uint32_t id = c0 + lane < deg ? list[c0 + lane] : kNoId;
+                    const bool keep = c0 + lane < deg && !sorted_contains(p.remove, p.n_remove, id);
+                    const unsigned m = __ballot_sync(kFull, keep);
+                    __syncwarp();
+                    if (keep) list[kept + __popc(m & ((1u << lane) - 1u))] = id;
+                    __syncwarp();
+                    kept += __popc(m);
+                }
+                did_remove = kept != deg;
+                deg = kept;
+            }
             // add_edge_and_prune(sorted sources, q) (index.rs:2264-2341, called once per target by
             // multi_insert, index.rs:986-1003): extend_from_slice appends every source that is not yet
             // in the list (sources arrive in ascending id order: the radix sort is stable and the
@@ -330,9 +374,10 @@ __global__ void __launch_bounds__(kPruneWarps * 32) backedge_kernel(const Backed
                 if (src == q) continue;
                 bool present = false;
                 for (uint32_t t = lane; t < deg0; t += 32) present |= list[t] == src;
+                if constexpr (REMOVE) present |= segment_repeats(p.vals, start, e, src, lane);
                 if (!__any_sync(kFull, present)) ++n_new;
             }
-            if (n_new == 0) continue;
+            if (n_new == 0 && !did_remove) continue;
             bool changed = true;
             if (deg0 + n_new <= p.max_degree) {
                 for (uint32_t e = start; e < p.n_pairs && p.keys[e] == q; ++e) {
@@ -340,6 +385,7 @@ __global__ void __launch_bounds__(kPruneWarps * 32) backedge_kernel(const Backed
                     if (src == q) continue;
                     bool present = false;
                     for (uint32_t t = lane; t < deg0; t += 32) present |= list[t] == src;
+                    if constexpr (REMOVE) present |= segment_repeats(p.vals, start, e, src, lane);
                     if (__any_sync(kFull, present)) continue;
                     if (lane == 0) list[deg] = src;
                     ++deg;
@@ -379,6 +425,8 @@ __global__ void __launch_bounds__(kPruneWarps * 32) backedge_kernel(const Backed
                 for (uint32_t t = 0; t < deg0; ++t) {
                     const uint32_t id = list[t];
                     if (id == q) continue;
+                    if constexpr (REMOVE)
+                        if (id >= p.n_total) continue;  // a stray id: robust_prune_list's fill finds no row for it
                     pend[npend++] = id;
                     if (npend == kPairsPerPass) flush();
                 }
@@ -387,6 +435,7 @@ __global__ void __launch_bounds__(kPruneWarps * 32) backedge_kernel(const Backed
                     if (src == q) continue;
                     bool present = false;
                     for (uint32_t t = lane; t < deg0; t += 32) present |= list[t] == src;
+                    if constexpr (REMOVE) present |= segment_repeats(p.vals, start, e, src, lane);
                     if (__any_sync(kFull, present)) continue;
                     pend[npend++] = src;
                     if (npend == kPairsPerPass) flush();
@@ -410,6 +459,16 @@ __global__ void __launch_bounds__(kPruneWarps * 32) backedge_kernel(const Backed
             __syncwarp();
         }
     }
+}
+
+template <typename TD, int NA, int KIND, int POST, bool IS_INT, bool SIGNED>
+__global__ void __launch_bounds__(kPruneWarps * 32) backedge_kernel(const BackedgeParams p) {
+    backedge_segments<TD, NA, KIND, POST, IS_INT, SIGNED, false>(p);
+}
+
+template <typename TD, int NA, int KIND, int POST, bool IS_INT, bool SIGNED>
+__global__ void __launch_bounds__(kPruneWarps * 32) inplace_backedge_kernel(const BackedgeParams p) {
+    backedge_segments<TD, NA, KIND, POST, IS_INT, SIGNED, true>(p);
 }
 
 // ------------------------------------------------------------------ consolidation
@@ -592,6 +651,183 @@ __global__ void __maxnreg__(96) consolidate_kernel(const ConsolidateParams p) {
     }
 }
 
+// ------------------------------------------------------------------ in-place deletes
+// inplace_delete_inner (index.rs:1585-1749) for every member of a chunk, one warp per member, on the graph as it was
+// before the chunk, every member already deleted.  The member's replace candidates and in-neighbours (the three
+// candidate routines, index.rs:1139-1336), then its scored edges as (source, target) pairs, member-major: each
+// in-neighbour c's pairs (c, r) for the num_to_replace candidates r nearest to c, or one (c, kNoId) when there are none,
+// then for each live neighbour a in list order the pairs (r, a) for the candidates r nearest to a.  Candidates are
+// ordered by (Distance<T,T>, position in the replace candidates): warp_sort_pool with the positions as arrival order.
+// An in-neighbour listed twice yields the same pairs twice, which add_edge_and_prune's extend_from_slice makes a
+// no-op, as the reference's HashMap::insert replacing the entry with an equal one.  The count pass (keys NULL) writes
+// each member's pair count without computing a distance; the write pass writes the pairs from offsets[w].
+struct WorklistParams {
+    const uint8_t* vectors;
+    size_t row_stride;
+    int dim;
+    const uint32_t* adj;
+    uint32_t adj_stride, max_degree;
+    uint64_t n_total;
+    const uint32_t* deleted;  // the table, the chunk's members marked
+    const uint32_t* members;
+    uint32_t n_members;
+    int method;
+    uint32_t num_to_replace, k_value;
+    const uint32_t* topk;    // VisitedAndTopK: each member's filtered search list [n_members][topk_cap], topk_n long
+    const uint32_t* topk_n;
+    uint32_t topk_cap;
+    uint32_t P;  // shared-memory pool slots per warp: a power of two >= the longest replace-candidate list
+    // per warp: the member's live neighbours [max_degree], in-neighbours [inn_cap]; TwoHopAndOneHop: the two-hop set
+    // [cand_cap] with the table slot of each id, and an open-addressing table of 1 << hash_bits ids (kNoId = empty)
+    uint32_t *onehop, *inn, *cand, *cand_slot, *hash;
+    uint32_t inn_cap, cand_cap;
+    int hash_bits;
+    uint32_t* counts;          // count pass: [n_members] pairs
+    const uint32_t* offsets;   // write pass: [n_members] first pair
+    uint32_t *keys, *vals;     // write pass: sources, targets
+};
+
+template <typename TD, int NA, int KIND, int POST, bool IS_INT, bool SIGNED>
+__global__ void __launch_bounds__(kPruneWarps * 32) inplace_worklist_kernel(const WorklistParams p) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    PruneSmem s = carve(smem + (size_t)wib * prune_smem_bytes(p.P), p.P);
+    const uint32_t warp = blockIdx.x * kPruneWarps + wib, nwarps = gridDim.x * kPruneWarps;
+    uint32_t* onehop = p.onehop + (size_t)warp * p.max_degree;
+    uint32_t* inn = p.inn + (size_t)warp * p.inn_cap;
+    uint32_t* cand = p.cand + (size_t)warp * p.cand_cap;
+    uint32_t* cslot = p.cand_slot + (size_t)warp * p.cand_cap;
+    uint32_t* hash = p.hash + ((size_t)warp << p.hash_bits);
+    const uint32_t hmask = (1u << p.hash_bits) - 1u;
+    const bool write = p.keys != nullptr;
+    auto dead = [&](uint32_t id) { return id >= p.n_total || (__ldg(p.deleted + (id >> 5)) >> (id & 31) & 1u); };
+    // every lane calls: the ids of the lanes with `want` go to out[n..] in lane order
+    auto append = [&](uint32_t* out, uint32_t& n, uint32_t id, bool want) {
+        const unsigned m = __ballot_sync(kFull, want);
+        if (want) out[n + __popc(m & ((1u << lane) - 1u))] = id;
+        n += __popc(m);
+    };
+    for (uint32_t w = warp; w < p.n_members; w += nwarps) {
+        const uint32_t m = p.members[w];
+        const uint32_t* mrow = p.adj + (size_t)m * p.adj_stride;
+        const uint32_t mdeg = min(mrow[0], p.max_degree);
+        uint32_t n1 = 0;  // live neighbours, list order (get_undeleted_neighbors)
+        for (uint32_t c0 = 0; c0 < mdeg; c0 += 32) {
+            const uint32_t id = c0 + lane < mdeg ? mrow[1 + c0 + lane] : kNoId;
+            append(onehop, n1, id, c0 + lane < mdeg && !dead(id));
+        }
+        __syncwarp();
+        const uint32_t *rc = onehop, *cands = onehop;  // replace candidates; the ids whose lists may hold m
+        uint32_t nrc = n1, ncand = n1;
+        if (p.method == DAB_INPLACE_VISITED_AND_TOPK) {
+            cands = rc = p.topk + (size_t)w * p.topk_cap;
+            ncand = p.topk_n[w];
+            nrc = min(ncand, p.k_value);
+        } else if (p.method == DAB_INPLACE_TWO_HOP_AND_ONE_HOP) {
+            // the live ids of {one-hop} and their neighbours, first occurrence kept
+            ncand = 0;
+            auto add = [&](uint32_t id, bool want) {
+                const unsigned peers = __match_any_sync(kFull, want ? id : kNoId);
+                uint32_t slot = kNoId;
+                if (want && __ffs(peers) - 1 == lane) {
+                    uint32_t h = (id * 0x9E3779B1u) >> (32 - p.hash_bits);
+                    for (;;) {
+                        const uint32_t old = atomicCAS(hash + h, kNoId, id);
+                        if (old == kNoId) {
+                            slot = h;
+                            break;
+                        }
+                        if (old == id) break;
+                        h = (h + 1) & hmask;
+                    }
+                }
+                const unsigned mn = __ballot_sync(kFull, slot != kNoId);
+                if (slot != kNoId) {
+                    const uint32_t pos = ncand + __popc(mn & ((1u << lane) - 1u));
+                    cand[pos] = id;
+                    cslot[pos] = slot;
+                }
+                ncand += __popc(mn);
+            };
+            for (uint32_t c0 = 0; c0 < n1; c0 += 32) add(c0 + lane < n1 ? onehop[c0 + lane] : kNoId, c0 + lane < n1);
+            for (uint32_t i = 0; i < n1; ++i) {
+                const uint32_t* r = p.adj + (size_t)onehop[i] * p.adj_stride;
+                const uint32_t deg = min(r[0], p.max_degree);
+                for (uint32_t c0 = 0; c0 < deg; c0 += 32) {
+                    const uint32_t id = c0 + lane < deg ? r[1 + c0 + lane] : kNoId;
+                    add(id, c0 + lane < deg && !dead(id));
+                }
+            }
+            __syncwarp();
+            cands = cand;
+        }
+        // in-neighbours: the candidates whose list holds m (return_refs_to_deleted_vertex)
+        uint32_t nin = 0;
+        for (uint32_t i = 0; i < ncand; ++i) {
+            const uint32_t c = cands[i];
+            const uint32_t* r = p.adj + (size_t)c * p.adj_stride;
+            const uint32_t deg = min(r[0], p.max_degree);
+            bool hit = false;
+            for (uint32_t j = lane; j < deg; j += 32) hit |= r[1 + j] == m;
+            if (__any_sync(kFull, hit)) {
+                if (lane == 0) inn[nin] = c;
+                ++nin;
+            }
+        }
+        if (p.method == DAB_INPLACE_TWO_HOP_AND_ONE_HOP)
+            for (uint32_t j = lane; j < ncand; j += 32) hash[cslot[j]] = kNoId;
+        __syncwarp();
+        // the scored edges of every in-neighbour, then of every live neighbour
+        uint32_t npairs = 0;
+        uint32_t* keys = write ? p.keys + p.offsets[w] : nullptr;
+        uint32_t* vals = write ? p.vals + p.offsets[w] : nullptr;
+        for (uint32_t j = 0; j < nin + n1; ++j) {
+            const bool in = j < nin;
+            const uint32_t x = in ? inn[j] : onehop[j - nin];
+            uint32_t self = 0;
+            for (uint32_t c0 = 0; c0 < nrc; c0 += 32) self += __popc(__ballot_sync(kFull, c0 + lane < nrc && rc[c0 + lane] == x));
+            const uint32_t take = min(p.num_to_replace, nrc - self);
+            if (write && take > 0) {
+                uint32_t n = 0;
+                for (uint32_t i0 = 0; i0 < nrc; i0 += kPairsPerPass) {
+                    const uint32_t cnt = min(nrc - i0, (uint32_t)kPairsPerPass);
+                    uint32_t rows[kPairsPerPass];
+#pragma unroll
+                    for (int g = 0; g < kPairsPerPass; ++g) rows[g] = rc[i0 + min((uint32_t)g, cnt - 1)];
+                    float dist[kPairsPerPass];
+                    warp_row_distances<TD, NA, KIND, POST, IS_INT, SIGNED>(p.vectors, p.row_stride, p.dim, x, rows, lane, dist);
+#pragma unroll
+                    for (int g = 0; g < kPairsPerPass; ++g) {
+                        if ((uint32_t)g < cnt && rows[g] != x) {
+                            if (lane == 0) {
+                                s.ids[n] = rows[g];
+                                s.d[n] = dist[g];
+                                s.order[n] = i0 + g;
+                            }
+                            ++n;
+                        }
+                    }
+                }
+                __syncwarp();
+                uint32_t P2 = 2;
+                while (P2 < n) P2 <<= 1;
+                warp_sort_pool(s, n, P2, lane, true);
+                for (uint32_t t = lane; t < take; t += 32) {
+                    keys[npairs + t] = in ? x : s.ids[t];
+                    vals[npairs + t] = in ? s.ids[t] : x;
+                }
+                __syncwarp();
+            }
+            if (in && take == 0 && write && lane == 0) {  // edges[c] is set, empty
+                keys[npairs] = x;
+                vals[npairs] = kNoId;
+            }
+            npairs += in ? max(take, 1u) : take;
+        }
+        if (!write && lane == 0) p.counts[w] = npairs;
+    }
+}
+
 __global__ void iota_kernel(uint32_t* p, uint32_t first, uint32_t n) {
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) p[i] = first + i;
 }
@@ -625,7 +861,8 @@ static int launch_prune(const dab_index* idx, PruneParams& p) {
     return DAB_OK;
 }
 
-static int launch_backedges(const dab_index* idx, BackedgeParams& p) {
+// `remove`: inplace_backedge_kernel, with p.remove set
+static int launch_backedges(const dab_index* idx, BackedgeParams& p, bool remove = false) {
     p.vectors = idx->d_vectors;
     p.row_stride = idx->row_stride;
     p.dim = (int)idx->dim;
@@ -641,7 +878,8 @@ static int launch_backedges(const dab_index* idx, BackedgeParams& p) {
     const int grid = (int)std::min<uint64_t>(((uint64_t)chunks + kPruneWarps - 1) / kPruneWarps, (uint64_t)idx->sm_count * 8);
     const int rc = visit_schema<OPS_ROW>(idx->dtype, idx->metric, [&](auto s) -> int {
         using S = decltype(s);
-        auto kern = backedge_kernel<KernelRow<S>, S::NA, S::KIND, S::POST, S::IS_INT, S::SIGNED>;
+        auto kern = remove ? inplace_backedge_kernel<KernelRow<S>, S::NA, S::KIND, S::POST, S::IS_INT, S::SIGNED>
+                           : backedge_kernel<KernelRow<S>, S::NA, S::KIND, S::POST, S::IS_INT, S::SIGNED>;
         DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, kPruneWarps * 32, smem, idx->stream>>>(p);
         return DAB_OK;
@@ -760,6 +998,175 @@ struct LinkStep {
     }
 };
 
+// The work-list kernel's shared-memory pool slots per warp: a power of two >= the longest replace-candidate list
+static uint32_t inplace_pool_slots(const dab_index* idx, int method, uint32_t k_value, uint32_t l_value) {
+    uint32_t longest = idx->max_degree;
+    if (method == DAB_INPLACE_VISITED_AND_TOPK) longest = std::max(longest, std::min(k_value, l_value));
+    return pow2_at_least(std::max<uint32_t>(longest, 2));
+}
+
+// Whether the work-list and apply kernels' shared memory fits one CTA (checked before anything is changed)
+static bool inplace_fits(const dab_index* idx, int method, uint32_t k_value, uint32_t l_value) {
+    const uint32_t pb = std::max<uint32_t>(1024, pow2_at_least(idx->max_degree + 2));  // launch_backedges' pool
+    return prune_smem_bytes(inplace_pool_slots(idx, method, k_value, l_value)) * kPruneWarps <= 200 * 1024 &&
+           (prune_smem_bytes(pb) + 4 * (size_t)pb) * kPruneWarps <= 200 * 1024;
+}
+
+// Grows `b` to at least `bytes` (contents not kept)
+static int grow(DevBuf& b, size_t& have, size_t bytes) {
+    if (bytes <= have) return DAB_OK;
+    have = bytes;
+    return b.alloc(bytes);
+}
+
+// One chunk of multi_inplace_delete; `chunk` holds its ids in the caller's order, already marked deleted
+struct InplaceDelete {
+    int method;
+    uint32_t num_to_replace, k_value, l_value, pruned_degree;
+    float alpha;
+    DevBuf members, sorted, lists, topk, topk_n, scratch, counts, offsets, keys, vals, keys2, vals2, tmp;
+    size_t cap_members = 0, cap_sorted = 0, cap_lists = 0, cap_topk = 0, cap_topk_n = 0, cap_scratch = 0, cap_counts = 0,
+           cap_offsets = 0, cap_keys = 0, cap_vals = 0, cap_keys2 = 0, cap_vals2 = 0, cap_tmp = 0;
+
+    int run(dab_index* idx, const uint32_t* chunk, uint32_t b) {
+        cudaStream_t st = idx->stream;
+        int rc;
+        if ((rc = grow(members, cap_members, (size_t)b * 4)) || (rc = grow(sorted, cap_sorted, (size_t)b * 4)) ||
+            (rc = grow(counts, cap_counts, (size_t)b * 4)) || (rc = grow(offsets, cap_offsets, (size_t)b * 4)))
+            return rc;
+        std::vector<uint32_t> ascending(chunk, chunk + b);
+        std::sort(ascending.begin(), ascending.end());
+        DAB_CUDA(cudaMemcpyAsync(members.p, chunk, (size_t)b * 4, cudaMemcpyHostToDevice, st));
+        DAB_CUDA(cudaMemcpyAsync(sorted.p, ascending.data(), (size_t)b * 4, cudaMemcpyHostToDevice, st));
+        WorklistParams p;
+        memset(&p, 0, sizeof(p));
+        p.vectors = idx->d_vectors;
+        p.row_stride = idx->row_stride;
+        p.dim = (int)idx->dim;
+        p.adj = idx->d_adj;
+        p.adj_stride = idx->adj_stride;
+        p.max_degree = idx->max_degree;
+        p.n_total = idx->n_total();
+        p.deleted = idx->d_deleted;
+        p.members = (const uint32_t*)members.p;
+        p.n_members = b;
+        p.method = method;
+        p.num_to_replace = num_to_replace;
+        p.k_value = k_value;
+        p.P = inplace_pool_slots(idx, method, k_value, l_value);
+        p.inn_cap = idx->max_degree;
+        if (method == DAB_INPLACE_VISITED_AND_TOPK) {
+            // search_internal from each member's row, beam 1, L = l_value, start points kept; then the first l_value
+            // entries that are not deleted (RemoveDeletedIdsAndCopy, which keeps start points)
+            const uint32_t cap = l_value + idx->n_start;
+            if ((rc = grow(lists, cap_lists, (size_t)b * cap * 8)) || (rc = grow(topk, cap_topk, (size_t)b * l_value * 8)) ||
+                (rc = grow(topk_n, cap_topk_n, (size_t)b * 4)))
+                return rc;
+            uint32_t* l_ids = (uint32_t*)lists.p;
+            float* l_d = (float*)(l_ids + (size_t)b * cap);
+            SearchRecord rec{};
+            rec.query_rows = (const uint32_t*)members.p;
+            rec.keep_starts = true;
+            if ((rc = run_search(idx, nullptr, b, cap, l_value, 1, SearchOut{l_ids, l_d, nullptr, nullptr, nullptr}, -1, false, &rec)))
+                return rc;
+            uint32_t* t_ids = (uint32_t*)topk.p;
+            if ((rc = queue_drop_deleted(idx, st, idx->d_deleted, l_ids, l_d, cap, b, l_value,
+                                         SearchOut{t_ids, (float*)(t_ids + (size_t)b * l_value), (uint32_t*)topk_n.p, nullptr, nullptr},
+                                         idx->n_total())))
+                return rc;
+            p.topk = t_ids;
+            p.topk_n = (const uint32_t*)topk_n.p;
+            p.topk_cap = l_value;
+            p.inn_cap = std::max(p.inn_cap, l_value);
+        }
+        if (method == DAB_INPLACE_TWO_HOP_AND_ONE_HOP) {
+            // distinct ids: the live neighbours and theirs, never more than the index holds
+            p.cand_cap = (uint32_t)std::min<uint64_t>(idx->n_total(), (uint64_t)idx->max_degree * (idx->max_degree + 1));
+            p.hash_bits = 5;
+            while ((1ull << p.hash_bits) < 2ull * p.cand_cap) ++p.hash_bits;  // at most half full
+            p.inn_cap = std::max(p.inn_cap, p.cand_cap);
+        }
+        const size_t smem = prune_smem_bytes(p.P) * kPruneWarps;
+        const size_t warp_words = (size_t)idx->max_degree + p.inn_cap + 2ull * p.cand_cap + (p.cand_cap ? 1ull << p.hash_bits : 0);
+        rc = visit_schema<OPS_ROW>(idx->dtype, idx->metric, [&](auto sch) -> int {
+            using S = decltype(sch);
+            auto kern = inplace_worklist_kernel<KernelRow<S>, S::NA, S::KIND, S::POST, S::IS_INT, S::SIGNED>;
+            const int per_sm = ctas_per_sm(kern, kPruneWarps * 32, smem);
+            if (per_sm < 1) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_inplace_delete: the work-list kernel does not fit");
+            // every resident warp, within 2 GB of per-warp lists and tables
+            uint64_t blocks = (uint64_t)per_sm * idx->sm_count;
+            blocks = std::max<uint64_t>(1, std::min<uint64_t>(blocks, (2ull << 30) / (warp_words * 4 * kPruneWarps)));
+            blocks = std::min<uint64_t>(blocks, ((uint64_t)b + kPruneWarps - 1) / kPruneWarps);
+            const size_t warps = blocks * kPruneWarps;
+            int rc2;
+            if ((rc2 = grow(scratch, cap_scratch, warps * warp_words * 4))) return rc2;
+            p.onehop = (uint32_t*)scratch.p;
+            p.inn = p.onehop + warps * idx->max_degree;
+            p.cand = p.inn + warps * p.inn_cap;
+            p.cand_slot = p.cand + warps * p.cand_cap;
+            p.hash = p.cand_slot + warps * p.cand_cap;
+            if (p.cand_cap) DAB_CUDA(cudaMemsetAsync(p.hash, 0xFF, (warps << p.hash_bits) * 4, st));
+            // count pass, offsets, write pass
+            p.counts = (uint32_t*)counts.p;
+            kern<<<(int)blocks, kPruneWarps * 32, smem, st>>>(p);
+            DAB_LAUNCHED();
+            DAB_CUDA(cudaGetLastError());
+            std::vector<uint32_t> n_of(b), first(b);
+            DAB_CUDA(cudaMemcpyAsync(n_of.data(), counts.p, (size_t)b * 4, cudaMemcpyDeviceToHost, st));
+            DAB_CUDA(cudaStreamSynchronize(st));
+            uint64_t total = 0;
+            for (uint32_t i = 0; i < b; ++i) {
+                first[i] = (uint32_t)total;
+                total += n_of[i];
+            }
+            if (total >= 0x7FFFFFFFull) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_inplace_delete: %llu edges in one chunk (use a smaller batch_size)",
+                                                    (unsigned long long)total);
+            n_pairs = (uint32_t)total;
+            if (n_pairs == 0) return DAB_OK;
+            if ((rc2 = grow(keys, cap_keys, total * 4)) || (rc2 = grow(vals, cap_vals, total * 4)) ||
+                (rc2 = grow(keys2, cap_keys2, total * 4)) || (rc2 = grow(vals2, cap_vals2, total * 4)))
+                return rc2;
+            DAB_CUDA(cudaMemcpyAsync(offsets.p, first.data(), (size_t)b * 4, cudaMemcpyHostToDevice, st));
+            p.counts = nullptr;
+            p.offsets = (const uint32_t*)offsets.p;
+            p.keys = (uint32_t*)keys.p;
+            p.vals = (uint32_t*)vals.p;
+            kern<<<(int)blocks, kPruneWarps * 32, smem, st>>>(p);
+            DAB_LAUNCHED();
+            DAB_CUDA(cudaGetLastError());
+            return DAB_OK;
+        });
+        if (rc) return rc;
+        if (n_pairs) {
+            // the targets of each source in the members' order (a stable sort), then one add_edge_and_prune per source
+            size_t need = 0;
+            cub::DeviceRadixSort::SortPairs(nullptr, need, (const uint32_t*)keys.p, (uint32_t*)keys2.p, (const uint32_t*)vals.p,
+                                            (uint32_t*)vals2.p, (int)n_pairs, 0, 32, st);
+            if ((rc = grow(tmp, cap_tmp, need))) return rc;
+            cudaError_t e = cub::DeviceRadixSort::SortPairs(tmp.p, need, (const uint32_t*)keys.p, (uint32_t*)keys2.p, (const uint32_t*)vals.p,
+                                                            (uint32_t*)vals2.p, (int)n_pairs, 0, 32, st);
+            if (e != cudaSuccess) return fail(DAB_ERR_CUDA, "dab_inplace_delete: radix sort failed: %s", cudaGetErrorString(e));
+            DAB_LAUNCHED();
+            BackedgeParams bp;
+            memset(&bp, 0, sizeof(bp));
+            bp.keys = (const uint32_t*)keys2.p;
+            bp.vals = (const uint32_t*)vals2.p;
+            bp.n_pairs = n_pairs;
+            bp.degree = pruned_degree;
+            bp.alpha = alpha;
+            bp.remove = (const uint32_t*)sorted.p;
+            bp.n_remove = b;
+            bp.n_total = idx->n_total();
+            if ((rc = launch_backedges(idx, bp, true))) return rc;
+        }
+        // drop_adj_list of every member
+        if ((rc = clear_rows(idx, (const uint32_t*)members.p, b))) return rc;
+        DAB_CUDA(cudaStreamSynchronize(st));
+        return DAB_OK;
+    }
+    uint32_t n_pairs = 0;
+};
+
 }  // namespace dab
 
 using namespace dab;
@@ -865,6 +1272,51 @@ int dab_consolidate(dab_index* idx, uint32_t pruned_degree, float alpha, uint64_
     if (rc) return rc;
     if (counters[1]) ++idx->generation;  // adjacency rows were written: open paged sessions fail their next page
     if (out_rewritten) *out_rewritten = counters[1];
+    return DAB_OK;
+}
+
+int dab_inplace_delete(dab_index* idx, const uint32_t* ids, uint64_t n, int method, uint32_t num_to_replace, uint32_t k_value,
+                       uint32_t l_value, uint32_t pruned_degree, float alpha, uint32_t batch_size) {
+    static const char* who = "dab_inplace_delete";
+    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", who);
+    if (n && !ids) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", who);
+    if (method != DAB_INPLACE_VISITED_AND_TOPK && method != DAB_INPLACE_TWO_HOP_AND_ONE_HOP && method != DAB_INPLACE_ONE_HOP)
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: unknown method %d", who, method);
+    if (pruned_degree == 0 || pruned_degree > idx->max_degree)
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: pruned_degree must be in [1, max_degree]", who);
+    if (!(alpha >= 1.0f)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: alpha must be >= 1", who);
+    if (method == DAB_INPLACE_VISITED_AND_TOPK && (l_value == 0 || (uint64_t)l_value + idx->n_start > 1024))
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: l_value must be > 0 and l_value + #start <= 1024", who);
+    int rc;
+    if ((rc = refuse_in_flight(idx, who))) return rc;
+    std::vector<uint32_t> seen((idx->n_points + 31) / 32, 0u);
+    for (uint64_t i = 0; i < n; ++i) {
+        const uint32_t id = ids[i];
+        if (id >= idx->n_points)
+            return fail(DAB_ERR_INVALID_ARGUMENT, "%s: id %u is not a data point (n_points %llu; start points cannot be deleted)", who, id,
+                        (unsigned long long)idx->n_points);
+        if (seen[id >> 5] >> (id & 31) & 1u) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: id %u is repeated", who, id);
+        seen[id >> 5] |= 1u << (id & 31);
+    }
+    if (!idx->vectors_ready || !idx->graph_ready) return fail(DAB_ERR_NOT_READY, "%s: vectors and graph must be uploaded first", who);
+    if (!inplace_fits(idx, method, k_value, l_value))
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: max_degree %u (or k_value) too large for the kernels' shared memory", who, idx->max_degree);
+    if (n == 0) return DAB_OK;
+    DAB_CUDA(cudaSetDevice(idx->device));
+    const uint32_t cap = (uint32_t)std::min<uint64_t>(batch_size ? batch_size : n, n);
+    InplaceDelete del;
+    del.method = method;
+    del.num_to_replace = num_to_replace;
+    del.k_value = k_value;
+    del.l_value = l_value;
+    del.pruned_degree = pruned_degree;
+    del.alpha = alpha;
+    ++idx->generation;  // every chunk empties its members' lists: open paged sessions fail their next page
+    for (uint64_t first = 0; first < n; first += cap) {
+        const uint32_t b = (uint32_t)std::min<uint64_t>(cap, n - first);
+        // every member is deleted before any list is read
+        if ((rc = deleted_mark(idx, ids + first, b)) || (rc = del.run(idx, ids + first, b))) return rc;
+    }
     return DAB_OK;
 }
 

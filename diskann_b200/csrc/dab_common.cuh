@@ -42,6 +42,10 @@ int deleted_alloc(struct ::dab_index* idx);  // both copies of the table, every 
 void deleted_release(struct ::dab_index* idx);
 // the device bitmap the searches filter with while some id is deleted, else NULL
 const uint32_t* deleted_filter(const struct ::dab_index* idx);
+// marks the n ids (data points) deleted in both copies of the table (dab_delete without its checks)
+int deleted_mark(struct ::dab_index* idx, const uint32_t* ids, uint64_t n);
+// adj[ids[i]] <- the empty list, for the n device ids, queued on the index stream
+int clear_rows(const struct ::dab_index* idx, const uint32_t* d_ids, uint64_t n);
 // The calls that change the deletion table or consolidate wait for no batch: "<api>: slot i holds a batch in flight"
 // while one does
 int refuse_in_flight(const struct ::dab_index* idx, const char* api);

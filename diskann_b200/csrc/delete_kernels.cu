@@ -50,10 +50,10 @@ __global__ void __launch_bounds__(128) drop_deleted_kernel(const uint32_t* __res
 }
 
 int queue_drop_deleted(const dab_index* idx, cudaStream_t stream, const uint32_t* deleted, const uint32_t* ids, const float* dists,
-                       uint32_t cap, uint32_t nq, uint32_t k, const SearchOut& out) {
+                       uint32_t cap, uint32_t nq, uint32_t k, const SearchOut& out, uint64_t bound) {
     if (nq == 0) return DAB_OK;
     const int grid = (int)std::min<uint64_t>(((uint64_t)nq + 3) / 4, (uint64_t)idx->sm_count * 16);
-    drop_deleted_kernel<<<grid, 128, 0, stream>>>(ids, dists, cap, nq, k, deleted, idx->n_points, out.ids, out.dists, out.counts);
+    drop_deleted_kernel<<<grid, 128, 0, stream>>>(ids, dists, cap, nq, k, deleted, bound, out.ids, out.dists, out.counts);
     DAB_LAUNCHED();
     DAB_CUDA(cudaGetLastError());
     return DAB_OK;
@@ -85,6 +85,21 @@ static int deleted_push(dab_index* idx) {
     return DAB_OK;
 }
 
+static bool is_deleted(const dab_index* idx, uint64_t id);
+
+int deleted_mark(dab_index* idx, const uint32_t* ids, uint64_t n) {
+    int rc;
+    if ((rc = deleted_alloc(idx))) return rc;
+    for (uint64_t i = 0; i < n; ++i) {
+        const uint32_t id = ids[i];
+        if (!is_deleted(idx, id)) {
+            idx->h_deleted[id >> 5] |= 1u << (id & 31);
+            ++idx->n_deleted;
+        }
+    }
+    return deleted_push(idx);
+}
+
 int deleted_assign(dab_index* idx, const uint32_t* words, uint64_t n_deleted) {
     if (n_deleted == 0 && !idx->h_deleted) return DAB_OK;
     int rc;
@@ -112,6 +127,58 @@ int refuse_in_flight(const dab_index* idx, const char* api) {
 __global__ void clear_rows_kernel(uint32_t* __restrict__ adj, uint32_t adj_stride, const uint32_t* __restrict__ ids, uint64_t n) {
     for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
         adj[(size_t)ids[i] * adj_stride] = 0;
+}
+
+int clear_rows(const dab_index* idx, const uint32_t* d_ids, uint64_t n) {
+    const int grid = (int)std::min<uint64_t>((n + 255) / 256, (uint64_t)idx->sm_count * 8);
+    clear_rows_kernel<<<grid, 256, 0, idx->stream>>>(idx->d_adj, idx->adj_stride, d_ids, n);
+    DAB_LAUNCHED();
+    DAB_CUDA(cudaGetLastError());
+    return DAB_OK;
+}
+
+// DiskANNIndex::drop_deleted_neighbors (index.rs:1756-1816) for every node, one warp per node.  A node's new list depends
+// only on its own list, the table and, with only_orphans, the lengths of its deleted neighbours' lists, and no deleted
+// node's list is written: one pass in any order equals the sequential loop.  `list`: per warp, max_degree words of
+// shared memory holding the list as read.
+__global__ void __launch_bounds__(128) drop_deleted_neighbors_kernel(uint32_t* __restrict__ adj, uint32_t adj_stride, uint32_t max_degree,
+                                                                     uint64_t n_total, const uint32_t* __restrict__ deleted,
+                                                                     uint32_t degree, int only_orphans, uint32_t* __restrict__ rewritten) {
+    extern __shared__ uint32_t drop_smem[];
+    const int lane = threadIdx.x & 31;
+    uint32_t* list = drop_smem + (threadIdx.x >> 5) * max_degree;
+    auto dead = [&](uint32_t id) { return id >= n_total || (deleted && (__ldg(deleted + (id >> 5)) >> (id & 31) & 1u)); };
+    for (uint64_t v = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5; v < n_total; v += ((uint64_t)gridDim.x * blockDim.x) >> 5) {
+        if (dead((uint32_t)v)) continue;  // ConsolidateKind::Deleted
+        uint32_t* row = adj + v * adj_stride;
+        const uint32_t deg = min(row[0], max_degree);
+        bool any_dead = false;
+        for (uint32_t j = lane; j < deg; j += 32) {
+            list[j] = row[1 + j];
+            any_dead |= dead(list[j]);
+        }
+        any_dead = __any_sync(0xFFFFFFFFu, any_dead);
+        if (!any_dead && deg <= degree) continue;  // nothing deleted, and no prune needed
+        __syncwarp();
+        // the pool: live neighbours in list order, then (only_orphans) the deleted ones whose list is not empty
+        uint32_t n = 0;
+        for (int pass = 0; pass < (only_orphans ? 2 : 1); ++pass) {
+            for (uint32_t c0 = 0; c0 < deg; c0 += 32) {
+                const uint32_t j = c0 + lane;
+                const uint32_t id = j < deg ? list[j] : kNoId;
+                bool keep = j < deg && !dead(id);
+                if (pass == 1) keep = j < deg && dead(id) && id < n_total && adj[(size_t)id * adj_stride] != 0;
+                const unsigned m = __ballot_sync(0xFFFFFFFFu, keep);
+                if (keep) row[1 + n + __popc(m & ((1u << lane) - 1u))] = id;
+                n += __popc(m);
+            }
+        }
+        __syncwarp();
+        if (lane == 0) {
+            row[0] = n;
+            atomicAdd(rewritten, 1u);
+        }
+    }
 }
 
 }  // namespace dab
@@ -166,6 +233,33 @@ int dab_release(dab_index* idx, const uint32_t* ids, uint64_t n) {
     }
     ++idx->generation;  // adjacency rows were written
     return deleted_push(idx);
+}
+
+int dab_drop_deleted_neighbors(dab_index* idx, uint32_t pruned_degree, int only_orphans, uint64_t* out_rewritten) {
+    static const char* who = "dab_drop_deleted_neighbors";
+    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", who);
+    int rc;
+    if ((rc = refuse_in_flight(idx, who))) return rc;
+    if (!idx->graph_ready) return fail(DAB_ERR_NOT_READY, "%s: the graph must be uploaded first", who);
+    if (pruned_degree == 0 || pruned_degree > idx->max_degree)
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: pruned_degree must be in [1, max_degree]", who);
+    DAB_CUDA(cudaSetDevice(idx->device));
+    if ((rc = idx->s_counters.reserve(4))) return rc;
+    uint32_t* d_rewritten = (uint32_t*)idx->s_counters.p;
+    DAB_CUDA(cudaMemsetAsync(d_rewritten, 0, 4, idx->stream));
+    const size_t smem = (size_t)4 * idx->max_degree * 4;
+    const int grid = (int)std::min<uint64_t>((idx->n_total() + 3) / 4, (uint64_t)idx->sm_count * 16);
+    DAB_CUDA(cudaFuncSetAttribute(drop_deleted_neighbors_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    drop_deleted_neighbors_kernel<<<grid, 128, smem, idx->stream>>>(idx->d_adj, idx->adj_stride, idx->max_degree, idx->n_total(),
+                                                                   deleted_filter(idx), pruned_degree, only_orphans ? 1 : 0, d_rewritten);
+    DAB_LAUNCHED();
+    DAB_CUDA(cudaGetLastError());
+    uint32_t rewritten = 0;
+    DAB_CUDA(cudaMemcpyAsync(&rewritten, d_rewritten, 4, cudaMemcpyDeviceToHost, idx->stream));
+    DAB_CUDA(cudaStreamSynchronize(idx->stream));
+    if (rewritten) ++idx->generation;  // adjacency rows were written: open paged sessions fail their next page
+    if (out_rewritten) *out_rewritten = rewritten;
+    return DAB_OK;
 }
 
 int dab_delete_status(dab_index* idx, const uint32_t* ids, uint64_t n, uint8_t* out_deleted) {

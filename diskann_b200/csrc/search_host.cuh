@@ -110,25 +110,30 @@ struct SearchOut {
     uint32_t *counts, *cmps, *hops;
 };
 
-// RemoveDeletedIdsAndCopy over whole lists (delete_kernels.cu): the traversal wrote each query's non-start entries,
-// list order, into ids / dists [nq][cap] (padded with UINT32_MAX); the first k that `deleted` does not mark go to `out`
-// ([nq][k], padded UINT32_MAX / +inf; counts = how many), queued on `stream`.  cmps and hops are not touched.
+// RemoveDeletedIdsAndCopy over whole lists (delete_kernels.cu): the traversal wrote each query's entries below `bound`
+// (n_points: no start points; n_total: all), list order, into ids / dists [nq][cap] (padded with UINT32_MAX); the first
+// k below `bound` that `deleted` does not mark go to `out` ([nq][k], padded UINT32_MAX / +inf; counts = how many), queued
+// on `stream`.  cmps and hops are not touched.
 int queue_drop_deleted(const dab_index* idx, cudaStream_t stream, const uint32_t* deleted, const uint32_t* ids, const float* dists,
-                       uint32_t cap, uint32_t nq, uint32_t k, const SearchOut& out);
+                       uint32_t cap, uint32_t nq, uint32_t k, const SearchOut& out, uint64_t bound);
 
-// The build's insert searches: the queries are rows of the index, and each records the nodes it expanded
+// Searches whose queries are rows of the index (the build's insert searches, in-place deletes): they ignore deletions
+// and teach the visited tables nothing.  With `ids` each records the nodes it expanded; with `keep_starts` its results
+// are the list's entries with start points kept (the caller filters them).
 struct SearchRecord {
     const uint32_t* query_rows;  // [nq] row ids of the queries
-    uint32_t* ids;               // [nq][cap] expanded nodes, [nq] counts
+    uint32_t* ids;               // [nq][cap] expanded nodes, [nq] counts (NULL: no record)
     float* dists;
     uint32_t* counts;
     uint32_t cap;
+    bool keep_starts;
 };
 
 // One batch on the handle's stream and scratch, device pointers only.  `store`: -1 full precision, else the QuantStore the
 // traversal reads; `rerank` (quantized) reorders each list by full-precision distances.  Returns once the traversal is
 // complete; a full-precision batch also has its deleted ids filtered, while a quantized batch's rerank or filter may still
-// run.  `rec` (full precision): the build's insert searches, which ignore deletions and teach the visited tables nothing.
+// run.  `rec` (full precision): searches over rows of the index, which ignore deletions and teach the visited tables
+// nothing.
 int run_search(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam, const SearchOut& d,
                int store, bool rerank, const SearchRecord* rec = nullptr);
 

@@ -122,7 +122,7 @@ struct SlotJob {
     bool rerank = false;
     const void* d_queries = nullptr;
     uint32_t nq = 0, k = 0, l_search = 0, beam = 0, cap = 0;
-    SearchRecord rec{};  // the build's insert searches (rec.ids set)
+    SearchRecord rec{};  // searches over rows of the index (rec.query_rows set)
     // some id is deleted: a rerank drops deleted ids itself; without one (`filter`) the traversal writes every non-start
     // entry of a list (k = L + #start) to `lists` and the filter takes the first k live ones into `filtered`, the caller's
     // buffers
@@ -211,6 +211,7 @@ struct SlotJob {
         p.row_stride = idx->row_stride;
         p.query_rows = rec.query_rows;
         p.rec_ids = rec.ids, p.rec_dists = rec.dists, p.rec_counts = rec.counts, p.rec_cap = rec.cap;
+        p.result_bound = rec.keep_starts ? idx->n_total() : idx->n_points;
     }
     // a global-table pass: its work list and tables
     template <class P>
@@ -234,8 +235,8 @@ int SlotJob::prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint32_t
     d_counters = (uint32_t*)counters->p;
     d_overflow = d_counters + 4;
     out = d;
-    // the build's insert searches ignore deletions, as the reference's insert does
-    deleted = rec.ids ? nullptr : deleted_filter(idx);
+    // searches over rows of the index ignore deletions, as the reference's insert and in-place delete do
+    deleted = rec.query_rows ? nullptr : deleted_filter(idx);
     filter = deleted && !rerank;
     if (filter) {
         if ((rc = lists->reserve((size_t)nq * cap * 8))) return rc;
@@ -386,7 +387,7 @@ int SlotJob::launch_quant() {
 // the post-processing of the whole batch: the rerank, or the filter of deleted ids
 int SlotJob::post() {
     if (rerank) return launch_rerank(idx, stream, d_queries, nq, k, cap, pq.list_ids, pq.list_counts, out.ids, out.dists, out.counts, deleted);
-    if (filter) return queue_drop_deleted(idx, stream, deleted, out.ids, out.dists, cap, nq, k, filtered);
+    if (filter) return queue_drop_deleted(idx, stream, deleted, out.ids, out.dists, cap, nq, k, filtered, idx->n_points);
     return DAB_OK;
 }
 
@@ -395,9 +396,9 @@ int SlotJob::finish() {
     if (store == STORE_MINMAX && first_nan() != ~0ull) return nan_error();
     for (;;) {
         const uint32_t n_over = h_counters[1];
-        if (rec.ids) {
+        if (rec.query_rows) {
             idx->rec_truncated += h_counters[3];
-        } else {  // build-time searches run on a growing graph: do not learn from them
+        } else {  // searches over rows run on a graph being changed: do not learn from them
             learn_visited(hint(), l_search, beam, mode(), h_counters[2]);
             if (on_v3) {
                 idx->v3_overflow_l = l_search;

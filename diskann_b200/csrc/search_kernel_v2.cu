@@ -517,7 +517,7 @@ __global__ void __launch_bounds__(kV2Warps * 32, REG ? kV2MinCtasReg : QT == 0 ?
 
         // ---- post-process: drop start points, first k (provider.rs:907-950)
         {
-            const uint32_t count = write_results(qi, qd, min(p.cap, size), p.n_points, p.k, p.out_ids, p.out_dists, qidx, lane);
+            const uint32_t count = write_results(qi, qd, min(p.cap, size), p.result_bound, p.k, p.out_ids, p.out_dists, qidx, lane);
             // the visited set is level 1's ids plus the global table's (nvisited counts only those when level 1 is on);
             // every expanded node is a hop, so nrec is the hop count
             write_stats(p.counters, n1 + nvisited, p.out_counts, p.out_cmps, p.out_hops, qidx, count, cmps, nrec, lane);

@@ -232,7 +232,7 @@ __global__ void __launch_bounds__(kV3Warps * 32, kV3MinCtas) search_kernel_v3(co
 
         // ---- post-process: drop start points, first k (provider.rs:907-950)
         {
-            const uint32_t count = write_results(qi, qd, min(p.cap, size), p.n_points, p.k, p.out_ids, p.out_dists, qidx, lane);
+            const uint32_t count = write_results(qi, qd, min(p.cap, size), p.result_bound, p.k, p.out_ids, p.out_dists, qidx, lane);
             write_stats(p.counters, nvisited, p.out_counts, p.out_cmps, p.out_hops, qidx, count, cmps, hops, lane);
             if (lane == 0 && p.rec_counts) {
                 p.rec_counts[qidx] = min(nrec, p.rec_cap);

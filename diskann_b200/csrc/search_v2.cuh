@@ -46,6 +46,7 @@ struct SearchParamsV2 {
     uint32_t row_slot;    // bytes between staged rows (staged rows only, as off_rows)
     uint32_t stage_rows;  // rows staged per round (multiple of kGroup; staged rows only)
     uint32_t rows_evict_first;  // register rows read with the L2 evict_first policy (else evict_normal; staged rows: always)
+    uint64_t result_bound;  // ids below it are results: n_points (start points dropped), or n_total (kept)
 };
 
 struct V2Launch {

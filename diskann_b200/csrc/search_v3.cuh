@@ -39,6 +39,7 @@ struct SearchParamsV3 {
     // per-warp shared memory layout (bytes)
     uint32_t warp_smem, off_q, off_qd, off_qi, off_cid, off_cd, off_beam, off_adj, off_table;
     uint32_t adj_words;  // words of an adjacency row prefetched into shared memory (0: off)
+    uint64_t result_bound;  // ids below it are results: n_points (start points dropped), or n_total (kept)
 };
 
 struct V3Launch {

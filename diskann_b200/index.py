@@ -688,6 +688,23 @@ class GpuIndex:
         check(_lib.lib().dab_consolidate(self._h, pruned_degree, alpha, C.byref(n)))
         return int(n.value)
 
+    INPLACE_METHODS = {"visited_and_topk": 0, "two_hop_and_one_hop": 1, "one_hop": 2}
+
+    def inplace_delete(self, ids, num_to_replace, method, pruned_degree, alpha=1.2, k_value=20, l_value=50, batch_size=1):
+        """multi_inplace_delete: deletes `ids` and repairs only the lists around them, in consecutive chunks of batch_size
+        (1: inplace_delete id by id; 0: one chunk).  `method`: "visited_and_topk" (k_value, l_value),
+        "two_hop_and_one_hop" or "one_hop", or the DAB_INPLACE_* number."""
+        ids = np.ascontiguousarray(ids, np.uint32).ravel()
+        m = self.INPLACE_METHODS[method] if isinstance(method, str) else int(method)
+        check(_lib.lib().dab_inplace_delete(self._h, _ptr(ids), ids.shape[0], m, num_to_replace, k_value, l_value, pruned_degree, alpha,
+                                            batch_size))
+
+    def drop_deleted_neighbors(self, pruned_degree, only_orphans=False):
+        """drop_deleted_neighbors for every node: removes the edges to deleted points; returns the lists rewritten."""
+        n = C.c_uint64()
+        check(_lib.lib().dab_drop_deleted_neighbors(self._h, pruned_degree, 1 if only_orphans else 0, C.byref(n)))
+        return int(n.value)
+
     def flat_knn(self, queries, k):
         queries = self._queries(queries)
         ids = np.empty((queries.shape[0], k), np.uint32)

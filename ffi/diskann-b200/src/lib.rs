@@ -118,6 +118,24 @@ impl<T: Element> GpuIndex<T> {
         Ok(rewritten)
     }
 
+    /// `multi_inplace_delete` in chunks of `batch_size` (1: `inplace_delete` id by id, 0: one chunk); `method` is one
+    /// of the DAB_INPLACE_* values of diskann_b200.h: 0 VisitedAndTopK (with `k_value`, `l_value`), 1 TwoHopAndOneHop, 2 OneHop.
+    #[allow(clippy::too_many_arguments)]
+    pub fn inplace_delete(&mut self, ids: &[u32], num_to_replace: u32, method: i32, pruned_degree: u32, alpha: f32, k_value: u32,
+                          l_value: u32, batch_size: u32) -> Result<()> {
+        check(unsafe {
+            sys::dab_inplace_delete(self.raw, ids.as_ptr(), ids.len() as u64, method, num_to_replace, k_value, l_value, pruned_degree, alpha,
+                                    batch_size)
+        })
+    }
+
+    /// `drop_deleted_neighbors` for every node; returns the number of lists rewritten.
+    pub fn drop_deleted_neighbors(&mut self, pruned_degree: u32, only_orphans: bool) -> Result<u64> {
+        let mut rewritten = 0u64;
+        check(unsafe { sys::dab_drop_deleted_neighbors(self.raw, pruned_degree, only_orphans as i32, &mut rewritten) })?;
+        Ok(rewritten)
+    }
+
     /// `KNN::search` for every query of the batch at once (search_internal + post-processing).
     pub fn search_batch(&self, queries: &[T], k: usize, l_search: u32, beam_width: u32) -> Result<Batch> {
         assert_eq!(queries.len() % self.dim, 0);

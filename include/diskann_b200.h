@@ -567,6 +567,61 @@ int dab_delete_status(dab_index* idx, const uint32_t* ids, uint64_t n, uint8_t* 
  * out_rewritten (may be NULL): the number of lists written. */
 int dab_consolidate(dab_index* idx, uint32_t pruned_degree, float alpha, uint64_t* out_rewritten);
 
+/* The three ways DiskANNIndex::inplace_delete finds the lists to repair (diskann/src/graph/misc.rs:28) */
+enum { DAB_INPLACE_VISITED_AND_TOPK = 0, DAB_INPLACE_TWO_HOP_AND_ONE_HOP = 1, DAB_INPLACE_ONE_HOP = 2 };
+
+/* DiskANNIndex::multi_inplace_delete (diskann/src/graph/index.rs:1338-1520): deletes ids and repairs only the lists
+ * around each of them, so the cost follows n, not the size of the index.  The ids are cut into consecutive chunks of
+ * batch_size (max_minibatch_par) in the caller's order, members kept in that order; batch_size = 1 is inplace_delete
+ * called id by id (the reference's default), 0 is one chunk of all n.  Each chunk, on the graph the previous one left:
+ *   1. work lists (inplace_delete_inner, index.rs:1585-1749).  Every member of the chunk is marked deleted before any
+ *      list is read: of the schedules the reference's parallel tasks allow (each marks its member, then reads the graph),
+ *      the device takes this one, which is also the only one in which step 2 never adds an edge to a chunk-mate.  Then,
+ *      per member m, with live meaning neither deleted nor an id >= n_points + n_start:
+ *        OneHop: replace candidates = m's live neighbours in list order; in-neighbours = those of them whose list holds m.
+ *        TwoHopAndOneHop: the same replace candidates; in-neighbours = the live ids of {m's live neighbours and their
+ *          neighbours} whose list holds m.
+ *        VisitedAndTopK{k_value, l_value}: search_internal with m's own row as the query (beam 1, L = l_value, the
+ *          deletion table ignored during the traversal); deleted ids are dropped from the whole best list, start points
+ *          kept (RemoveDeletedIdsAndCopy), and the first l_value taken; in-neighbours = those whose list holds m,
+ *          replace candidates = the first k_value (k_value may exceed l_value).
+ *      With Distance<T,T>, each in-neighbour c gets edges[c] = the num_to_replace replace candidates nearest to c,
+ *      c excluded (a later entry for the same c replaces an earlier one, and an empty one still counts); then each
+ *      live neighbour a of m is appended to edges[r] for each of the num_to_replace replace candidates r nearest to a,
+ *      a excluded.  Exact distance ties, and the cut at num_to_replace, are ordered by position in the replace
+ *      candidates (the reference's sort_unstable_by leaves them unspecified).
+ *   2. apply: every source with an entry in any member's edges gets one add_edge_and_prune (index.rs:2264-2341): the
+ *      chunk's ids are removed from its list, then the members' edges[source], concatenated in chunk order, are
+ *      appended, skipping ids already present; a list with nothing added and nothing removed stays as it is, a list
+ *      that fits max_degree is written, and a longer one goes through robust_prune_list (index.rs:2397-2454) at
+ *      pruned_degree and alpha, without saturation (the prune kind from the metric, as dab_consolidate).  An id
+ *      >= n_points + n_start kept in such a list is left out of the prune pool: it has no row, so robust_prune_list's
+ *      fill finds nothing for it (the ids of a list that fits are kept as they are).
+ *   3. drop: every member's list is emptied.
+ * An id >= n_points + n_start met in a list counts as deleted with no neighbours, as in dab_consolidate (the
+ * reference's status or neighbour lookup would fail there); list lengths above max_degree are read as max_degree.
+ * Any data id may be given, one that is already deleted included (the reference's delete is idempotent, and repairing
+ * a soft-deleted point in place is legitimate).  Afterwards the ids are in the deletion table (as after dab_delete),
+ * the rows and every quantized store are untouched, dab_release -> dab_insert reuses the ids, and open paged sessions
+ * fail their next page.  num_to_replace = 0 is valid: the edges to the ids are still removed.
+ * DAB_ERR_INVALID_ARGUMENT, changing nothing and naming the first offending id: an id >= n_points (start points are
+ * frozen), a repeated id; also NULL ids with n > 0, an unknown method, pruned_degree outside [1, max_degree], alpha < 1,
+ * for VisitedAndTopK l_value == 0 or l_value + n_start > 1024, a max_degree (or VisitedAndTopK's min(k_value,
+ * l_value)) too large for the kernels' shared memory, or any slot holding a batch in flight.  DAB_ERR_NOT_READY when
+ * the vectors and graph are missing.  n == 0 returns DAB_OK after these checks.  A failure after them (out of memory,
+ * a chunk with 2^31 or more edges, a CUDA error) leaves the chunks before the failing one applied and the failing
+ * chunk's ids marked deleted but not repaired: searches leave them out, and dab_consolidate repairs the graph. */
+int dab_inplace_delete(dab_index* idx, const uint32_t* ids, uint64_t n, int method, uint32_t num_to_replace, uint32_t k_value,
+                       uint32_t l_value, uint32_t pruned_degree, float alpha, uint32_t batch_size);
+/* DiskANNIndex::drop_deleted_neighbors (index.rs:1756-1816) for every id in [0, n_points + n_start), in one device pass,
+ * which equals the sequential loop in any order since a deleted node's list is never written: a deleted node is left
+ * alone; otherwise the pool is its live neighbours in list order, not deduplicated, followed with only_orphans by its
+ * deleted neighbours whose own list is not empty, in list order (an id >= n_points + n_start counts as deleted with no
+ * neighbours); the pool becomes the list unless the node had no deleted neighbour and the pool holds at most
+ * pruned_degree ids.  pruned_degree in [1, max_degree]; refused while any slot holds a batch in flight; open paged
+ * sessions fail their next page when a list was written.  out_rewritten (may be NULL): the number of lists written. */
+int dab_drop_deleted_neighbors(dab_index* idx, uint32_t pruned_degree, int only_orphans, uint64_t* out_rewritten);
+
 /* exact k-NN by exhaustive scan (diskann/src/flat; ground truth for recall):
  * out_ids [nq][k] ascending distance, ties by lower id. */
 int dab_flat_knn(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t* out_ids,

@@ -184,6 +184,18 @@ class Provider {
         check(dab_consolidate(h_, pruned_degree, alpha, &rewritten));
         return rewritten;
     }
+    // DiskANNIndex::multi_inplace_delete in chunks of batch_size (1: inplace_delete id by id, 0: one chunk);
+    // method: DAB_INPLACE_VISITED_AND_TOPK (k_value, l_value), DAB_INPLACE_TWO_HOP_AND_ONE_HOP or DAB_INPLACE_ONE_HOP
+    void inplace_delete(const std::vector<uint32_t>& ids, uint32_t num_to_replace, int method, uint32_t pruned_degree, float alpha = 1.2f,
+                        uint32_t k_value = 20, uint32_t l_value = 50, uint32_t batch_size = 1) {
+        check(dab_inplace_delete(h_, ids.data(), ids.size(), method, num_to_replace, k_value, l_value, pruned_degree, alpha, batch_size));
+    }
+    // drop_deleted_neighbors for every node; returns the lists rewritten
+    uint64_t drop_deleted_neighbors(uint32_t pruned_degree, bool only_orphans = false) {
+        uint64_t rewritten = 0;
+        check(dab_drop_deleted_neighbors(h_, pruned_degree, only_orphans ? 1 : 0, &rewritten));
+        return rewritten;
+    }
 
    private:
     dab_index* h_ = nullptr;
