@@ -93,6 +93,9 @@ SYMBOLS = {
     "dab_consolidate": (_i, [_vp, _u32, _f, C.POINTER(_u64)]),
     "dab_inplace_delete": (_i, [_vp, _vp, _u64, _i, _u32, _u32, _u32, _u32, _f, _u32]),
     "dab_drop_deleted_neighbors": (_i, [_vp, _u32, _i, C.POINTER(_u64)]),
+    "dab_count_reachable": (_i, [_vp, _vp, _u32, C.POINTER(_u64)]),
+    "dab_degree_stats": (_i, [_vp, _vp, _u64, C.POINTER(_u32), C.POINTER(_f), C.POINTER(_u32), C.POINTER(_u64)]),
+    "dab_prune_range": (_i, [_vp, _vp, _u64, _u32, _f, C.POINTER(_u64)]),
     "dab_flat_knn": (_i, [_vp, _vp, _u32, _u32, _vp, _vp]),
     "dab_flat_knn_tc": (_i, [_vp, _vp, _u32, _u32, _vp, _vp]),
 }

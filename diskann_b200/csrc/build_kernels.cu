@@ -485,6 +485,12 @@ __global__ void __launch_bounds__(kPruneWarps * 32) inplace_backedge_kernel(cons
 //     (index.rs:2397-2454): Distance<T,T>(v, u), sorted by (distance, arrival order) and cut to the 750 smallest —
 //     streamed through the prune's shared-memory pool as in backedge_kernel, since a pool can hold
 //     max_degree * (max_degree + 1) ids — then occlude_list without saturation.
+// RANGE (prune_range_kernel): DiskANNIndex::prune_range (index.rs:2656-2700) over the nodes of p.ids (every id when
+// NULL), each listed once.  The deletion table is not read (the full-precision PruneAccessor::fill finds a row for every
+// id, deleted or not): a deleted node is pruned like any other and its deleted neighbours stay in its pool.  A node whose
+// list holds at most `degree` ids is left alone; any other list goes through robust_prune_list with the pool of its
+// distinct ids, itself and the ids >= n_total (no row: view.get finds nothing) left out, however short that pool is.
+// Each prune reads only its own list and rows, so one pass equals the reference's loop.
 constexpr uint32_t kConsolidateP = 1024;  // shared-memory pool slots per warp (> kMaxOcclusion)
 
 struct ConsolidateParams {
@@ -506,9 +512,13 @@ struct ConsolidateParams {
     uint32_t* counters;  // [0] next node, [1] lists rewritten
 };
 
-// 96 registers: below that ptxas spills the pool-building and prune state of the float schemas
-template <typename TD, int NA, int KIND, int POST, bool IS_INT, bool SIGNED>
-__global__ void __maxnreg__(96) consolidate_kernel(const ConsolidateParams p) {
+struct PruneRangeParams : ConsolidateParams {
+    const uint32_t* ids;  // the nodes to prune, n_ids of them (NULL: ids [0, n_ids))
+    uint32_t n_ids;
+};
+
+template <typename TD, int NA, int KIND, int POST, bool IS_INT, bool SIGNED, bool RANGE, class Params>
+__device__ __forceinline__ void consolidate_nodes(const Params p) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     PruneSmem s = carve(smem + (size_t)wib * prune_smem_bytes(kConsolidateP), kConsolidateP);
@@ -517,8 +527,8 @@ __global__ void __maxnreg__(96) consolidate_kernel(const ConsolidateParams p) {
     uint32_t* hash = p.hash + ((size_t)warp << p.hash_bits);
     uint32_t* pool = p.pool + (size_t)warp * p.pool_cap;
     uint32_t* pslot = p.pool_slot + (size_t)warp * p.pool_cap;
-    auto dead = [&](uint32_t id) {  // deleted, or a status lookup that fails
-        return id >= p.n_total || (p.deleted && (__ldg(p.deleted + (id >> 5)) >> (id & 31) & 1u));
+    auto dead = [&](uint32_t id) {  // deleted, or a status lookup that fails; RANGE: no row
+        return id >= p.n_total || (!RANGE && p.deleted && (__ldg(p.deleted + (id >> 5)) >> (id & 31) & 1u));
     };
     uint32_t n = 0;  // pool size
     // every lane calls; `want`: this lane offers `id`.  New ids are appended in lane order; among lanes offering the
@@ -550,13 +560,20 @@ __global__ void __maxnreg__(96) consolidate_kernel(const ConsolidateParams p) {
         uint32_t v = 0;
         if (lane == 0) v = atomicAdd(p.counters, 1u);
         v = __shfl_sync(kFull, v, 0);
-        if (v >= p.n_total) break;
-        if (dead(v)) continue;  // ConsolidateKind::Deleted
+        if constexpr (RANGE) {
+            if (v >= p.n_ids) break;
+            if (p.ids) v = p.ids[v];
+        } else {
+            if (v >= p.n_total) break;
+            if (dead(v)) continue;  // ConsolidateKind::Deleted
+        }
         uint32_t* row = p.adj + (size_t)v * p.adj_stride;
         const uint32_t deg = min(row[0], p.max_degree);
         bool any_dead = false;
-        for (uint32_t j = lane; j < deg; j += 32) any_dead |= dead(row[1 + j]);
-        any_dead = __any_sync(kFull, any_dead);
+        if constexpr (!RANGE) {
+            for (uint32_t j = lane; j < deg; j += 32) any_dead |= dead(row[1 + j]);
+            any_dead = __any_sync(kFull, any_dead);
+        }
         if (!any_dead && deg <= p.degree) continue;
         n = 0;
         for (uint32_t c = 0; c < deg; c += 32) {
@@ -565,22 +582,24 @@ __global__ void __maxnreg__(96) consolidate_kernel(const ConsolidateParams p) {
             add(id, j < deg && !dead(id));
         }
         // the early exit counts a self-loop
-        if (any_dead || n > p.degree) {
-            for (uint32_t c = 0; c < deg; c += 32) {
-                const uint32_t j = c + lane;
-                const uint32_t id = j < deg ? row[1 + j] : kNoId;
-                unsigned dm = __ballot_sync(kFull, j < deg && dead(id));
-                while (dm) {
-                    const int src = __ffs(dm) - 1;
-                    dm &= dm - 1;
-                    const uint32_t u = __shfl_sync(kFull, id, src);
-                    if (u >= p.n_total) continue;
-                    const uint32_t* urow = p.adj + (size_t)u * p.adj_stride;
-                    const uint32_t udeg = min(urow[0], p.max_degree);
-                    for (uint32_t c2 = 0; c2 < udeg; c2 += 32) {
-                        const uint32_t j2 = c2 + lane;
-                        const uint32_t w = j2 < udeg ? urow[1 + j2] : kNoId;
-                        add(w, j2 < udeg && !dead(w));
+        if (RANGE || any_dead || n > p.degree) {
+            if constexpr (!RANGE) {  // the deleted neighbours' lists join the pool
+                for (uint32_t c = 0; c < deg; c += 32) {
+                    const uint32_t j = c + lane;
+                    const uint32_t id = j < deg ? row[1 + j] : kNoId;
+                    unsigned dm = __ballot_sync(kFull, j < deg && dead(id));
+                    while (dm) {
+                        const int src = __ffs(dm) - 1;
+                        dm &= dm - 1;
+                        const uint32_t u = __shfl_sync(kFull, id, src);
+                        if (u >= p.n_total) continue;
+                        const uint32_t* urow = p.adj + (size_t)u * p.adj_stride;
+                        const uint32_t udeg = min(urow[0], p.max_degree);
+                        for (uint32_t c2 = 0; c2 < udeg; c2 += 32) {
+                            const uint32_t j2 = c2 + lane;
+                            const uint32_t w = j2 < udeg ? urow[1 + j2] : kNoId;
+                            add(w, j2 < udeg && !dead(w));
+                        }
                     }
                 }
             }
@@ -602,7 +621,7 @@ __global__ void __maxnreg__(96) consolidate_kernel(const ConsolidateParams p) {
                 }
                 --n;
             }
-            if (n < p.degree) {
+            if (!RANGE && n < p.degree) {
                 for (uint32_t j = lane; j < n; j += 32) row[1 + j] = pool[j];
                 if (lane == 0) row[0] = n;
             } else {
@@ -649,6 +668,17 @@ __global__ void __maxnreg__(96) consolidate_kernel(const ConsolidateParams p) {
         for (uint32_t j = lane; j < n; j += 32) hash[pslot[j]] = kNoId;
         __syncwarp();
     }
+}
+
+// 96 registers: below that ptxas spills the pool-building and prune state of the float schemas
+template <typename TD, int NA, int KIND, int POST, bool IS_INT, bool SIGNED>
+__global__ void __maxnreg__(96) consolidate_kernel(const ConsolidateParams p) {
+    consolidate_nodes<TD, NA, KIND, POST, IS_INT, SIGNED, false>(p);
+}
+
+template <typename TD, int NA, int KIND, int POST, bool IS_INT, bool SIGNED>
+__global__ void __maxnreg__(96) prune_range_kernel(const PruneRangeParams p) {
+    consolidate_nodes<TD, NA, KIND, POST, IS_INT, SIGNED, true>(p);
 }
 
 // ------------------------------------------------------------------ in-place deletes
@@ -889,18 +919,6 @@ static int launch_backedges(const dab_index* idx, BackedgeParams& p, bool remove
     DAB_CUDA(cudaGetLastError());
     return DAB_OK;
 }
-
-struct DevBuf {
-    void* p = nullptr;
-    ~DevBuf() { cudaFree(p); }
-    int alloc(size_t n) {
-        cudaFree(p);
-        p = nullptr;
-        cudaError_t e = cudaMalloc(&p, n ? n : 1);
-        if (e != cudaSuccess) return fail(DAB_ERR_OUT_OF_MEMORY, "build: cudaMalloc(%zu) failed: %s", n, cudaGetErrorString(e));
-        return DAB_OK;
-    }
-};
 
 // One multi_insert (index.rs:815-1030, intra_batch_candidates = None, no bootstrap) over the ids in `batch`, on the graph
 // the previous step left; dab_build and dab_insert run their batches through it.
@@ -1254,6 +1272,87 @@ int dab_consolidate(dab_index* idx, uint32_t pruned_degree, float alpha, uint64_
         uint64_t blocks = std::max(1, per_sm) * (uint64_t)idx->sm_count;
         blocks = std::max<uint64_t>(1, std::min<uint64_t>(blocks, (2ull << 30) / (warp_bytes * kPruneWarps)));
         blocks = std::min<uint64_t>(blocks, (idx->n_total() + kPruneWarps - 1) / kPruneWarps);
+        int rc2;
+        if ((rc2 = b_scratch.alloc(blocks * kPruneWarps * warp_bytes)) || (rc2 = b_counters.alloc(8))) return rc2;
+        p.hash = (uint32_t*)b_scratch.p;
+        p.pool = p.hash + (blocks * kPruneWarps << p.hash_bits);
+        p.pool_slot = p.pool + blocks * kPruneWarps * p.pool_cap;
+        p.counters = (uint32_t*)b_counters.p;
+        DAB_CUDA(cudaMemsetAsync(p.hash, 0xFF, (blocks * kPruneWarps << p.hash_bits) * 4, idx->stream));
+        DAB_CUDA(cudaMemsetAsync(p.counters, 0, 8, idx->stream));
+        kern<<<(int)blocks, kPruneWarps * 32, smem, idx->stream>>>(p);
+        DAB_LAUNCHED();
+        DAB_CUDA(cudaGetLastError());
+        DAB_CUDA(cudaMemcpyAsync(counters, p.counters, 8, cudaMemcpyDeviceToHost, idx->stream));
+        DAB_CUDA(cudaStreamSynchronize(idx->stream));
+        return DAB_OK;
+    });
+    if (rc) return rc;
+    if (counters[1]) ++idx->generation;  // adjacency rows were written: open paged sessions fail their next page
+    if (out_rewritten) *out_rewritten = counters[1];
+    return DAB_OK;
+}
+
+int dab_prune_range(dab_index* idx, const uint32_t* ids, uint64_t n, uint32_t pruned_degree, float alpha, uint64_t* out_rewritten) {
+    static const char* who = "dab_prune_range";
+    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", who);
+    if (!ids && n) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: ids is NULL with n > 0", who);
+    int rc;
+    if ((rc = refuse_in_flight(idx, who))) return rc;
+    if (!idx->vectors_ready || !idx->graph_ready) return fail(DAB_ERR_NOT_READY, "%s: vectors and graph must be uploaded first", who);
+    if (pruned_degree == 0 || pruned_degree > idx->max_degree)
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: pruned_degree must be in [1, max_degree]", who);
+    if (!(alpha >= 1.0f)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: alpha must be >= 1", who);
+    // each id once, in first-occurrence order: a repeat is a no-op in the reference, and two warps must not share a row
+    std::vector<uint32_t> distinct;
+    if (ids) {
+        std::vector<uint32_t> seen(idx->deleted_words(), 0u);
+        for (uint64_t i = 0; i < n; ++i) {
+            const uint32_t id = ids[i];
+            if (id >= idx->n_total())
+                return fail(DAB_ERR_INVALID_ARGUMENT, "%s: id %u out of range (%llu ids)", who, id, (unsigned long long)idx->n_total());
+            if (seen[id >> 5] >> (id & 31) & 1u) continue;
+            seen[id >> 5] |= 1u << (id & 31);
+            distinct.push_back(id);
+        }
+    }
+    const uint64_t n_ids = ids ? distinct.size() : idx->n_total();
+    if (out_rewritten) *out_rewritten = 0;
+    if (n_ids == 0) return DAB_OK;
+    DAB_CUDA(cudaSetDevice(idx->device));
+    PruneRangeParams p;
+    memset(&p, 0, sizeof(p));
+    p.vectors = idx->d_vectors;
+    p.row_stride = idx->row_stride;
+    p.dim = (int)idx->dim;
+    p.adj = idx->d_adj;
+    p.adj_stride = idx->adj_stride;
+    p.max_degree = idx->max_degree;
+    p.n_points = idx->n_points;
+    p.n_total = idx->n_total();
+    p.degree = pruned_degree;
+    p.alpha = alpha;
+    p.prune_kind = idx->metric == DAB_INNER_PRODUCT ? 1 : 0;  // PruneKind::from_metric, config/mod.rs:69-76
+    p.pool_cap = (uint32_t)std::min<uint64_t>(idx->n_total(), idx->max_degree);  // the distinct ids of one list
+    p.hash_bits = 5;
+    while ((1ull << p.hash_bits) < 2ull * p.pool_cap) ++p.hash_bits;  // at most half full
+    p.n_ids = (uint32_t)n_ids;
+    const size_t warp_bytes = ((1ull << p.hash_bits) + 2ull * p.pool_cap) * 4;
+    const size_t smem = prune_smem_bytes(kConsolidateP) * kPruneWarps;
+    DevBuf b_ids, b_scratch, b_counters;
+    if (ids) {
+        if ((rc = b_ids.alloc(n_ids * 4))) return rc;
+        DAB_CUDA(cudaMemcpyAsync(b_ids.p, distinct.data(), n_ids * 4, cudaMemcpyHostToDevice, idx->stream));
+        p.ids = (const uint32_t*)b_ids.p;
+    }
+    uint32_t counters[2] = {0, 0};
+    rc = visit_schema<OPS_ROW>(idx->dtype, idx->metric, [&](auto s) -> int {
+        using S = decltype(s);
+        auto kern = prune_range_kernel<KernelRow<S>, S::NA, S::KIND, S::POST, S::IS_INT, S::SIGNED>;
+        const int per_sm = ctas_per_sm(kern, kPruneWarps * 32, smem);
+        if (per_sm < 1) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: the prune kernel does not fit", who);
+        uint64_t blocks = (uint64_t)per_sm * idx->sm_count;
+        blocks = std::min<uint64_t>(blocks, (n_ids + kPruneWarps - 1) / kPruneWarps);
         int rc2;
         if ((rc2 = b_scratch.alloc(blocks * kPruneWarps * warp_bytes)) || (rc2 = b_counters.alloc(8))) return rc2;
         p.hash = (uint32_t*)b_scratch.p;

@@ -71,14 +71,14 @@ __global__ void __launch_bounds__(256) join_kernel(const CodeStore s, const uint
     }
 }
 
-int grid_for(const dab_index* idx, uint64_t work) { return (int)std::max<uint64_t>(1, std::min<uint64_t>((work + 255) / 256, (uint64_t)idx->sm_count * 16)); }
-
 // rows per slab of the host copies: a 100M-point store does not need a second full copy on the device
 uint64_t slab_rows(const dab_index* idx, uint64_t row_bytes) {
     return std::max<uint64_t>(1, std::min<uint64_t>(idx->n_total(), (256ull << 20) / row_bytes));
 }
 
 }  // namespace
+
+int grid_for(const dab_index* idx, uint64_t work) { return (int)std::max<uint64_t>(1, std::min<uint64_t>((work + 255) / 256, (uint64_t)idx->sm_count * 16)); }
 
 void store_release(CodeStore& s) {
     cudaFree(s.d_codes);

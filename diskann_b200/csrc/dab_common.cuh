@@ -84,6 +84,23 @@ int ctas_per_sm(void (*kern)(P), int threads, size_t smem) {
     return per_sm;
 }
 
+// A device buffer owned by one call, freed when it goes out of scope (cudaFree waits for the whole device).  alloc()
+// frees what it held and allocates n bytes; on failure "<who>: cudaMalloc(n) failed".
+struct DevBuf {
+    void* p = nullptr;
+    ~DevBuf() { cudaFree(p); }
+    int alloc(size_t n, const char* who = "build") {
+        cudaFree(p);
+        p = nullptr;
+        cudaError_t e = cudaMalloc(&p, n ? n : 1);
+        if (e != cudaSuccess) return fail(DAB_ERR_OUT_OF_MEMORY, "%s: cudaMalloc(%zu) failed: %s", who, n, cudaGetErrorString(e));
+        return DAB_OK;
+    }
+};
+
+// code_store.cu: blocks of 256 threads for `work` threads, at most 16 per SM (grid-stride kernels)
+int grid_for(const struct ::dab_index* idx, uint64_t work);
+
 // A grow-only device (or pinned host) scratch buffer.
 struct Scratch {
     void* p = nullptr;

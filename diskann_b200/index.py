@@ -705,6 +705,39 @@ class GpuIndex:
         check(_lib.lib().dab_drop_deleted_neighbors(self._h, pruned_degree, 1 if only_orphans else 0, C.byref(n)))
         return int(n.value)
 
+    # -- graph checks (DiskANNIndex::count_reachable_nodes / get_degree_stats) and the final prune (prune_range)
+    @staticmethod
+    def _id_list(ids):
+        """(pointer, n) of an explicit id list; an empty list still passes a valid pointer (None means "the default")"""
+        ids = np.ascontiguousarray(ids, np.uint32).ravel()
+        return _ptr(ids if ids.size else np.zeros(1, np.uint32)), ids.shape[0], ids
+
+    def count_reachable(self, start_ids=None):
+        """count_reachable_nodes: the ids a breadth-first walk reaches from start_ids (None: the start points)."""
+        n = C.c_uint64()
+        if start_ids is None:
+            check(_lib.lib().dab_count_reachable(self._h, None, 0, C.byref(n)))
+        else:
+            p, k, _keep = self._id_list(start_ids)
+            check(_lib.lib().dab_count_reachable(self._h, p, k, C.byref(n)))
+        return int(n.value)
+
+    def degree_stats(self, ids=None):
+        """get_degree_stats over ids (None: every id) -> (max_degree, avg_degree as np.float32, min_degree,
+        cnt_less_than_two)."""
+        mx, avg, mn, lt2 = C.c_uint32(), C.c_float(), C.c_uint32(), C.c_uint64()
+        p, k, _keep = (None, 0, None) if ids is None else self._id_list(ids)
+        check(_lib.lib().dab_degree_stats(self._h, p, k, C.byref(mx), C.byref(avg), C.byref(mn), C.byref(lt2)))
+        return int(mx.value), np.float32(avg.value), int(mn.value), int(lt2.value)
+
+    def prune_range(self, ids, pruned_degree, alpha=1.2):
+        """prune_range over ids (None: every id): robust_prune_list of every list longer than pruned_degree; returns the
+        lists rewritten.  Arguments in the C ABI's order, as the C++ and Rust bindings take them."""
+        n = C.c_uint64()
+        p, k, _keep = (None, 0, None) if ids is None else self._id_list(ids)
+        check(_lib.lib().dab_prune_range(self._h, p, k, pruned_degree, alpha, C.byref(n)))
+        return int(n.value)
+
     def flat_knn(self, queries, k):
         queries = self._queries(queries)
         ids = np.empty((queries.shape[0], k), np.uint32)

@@ -136,6 +136,42 @@ impl<T: Element> GpuIndex<T> {
         Ok(rewritten)
     }
 
+    /// `count_reachable_nodes` from `start_ids` (`None`: the index's start points).
+    pub fn count_reachable(&self, start_ids: Option<&[u32]>) -> Result<u64> {
+        let mut count = 0u64;
+        let none = [0u32; 1]; // an empty list still passes a pointer: NULL means the start points
+        let (ptr, n) = match start_ids {
+            None => (std::ptr::null(), 0),
+            Some(ids) => (if ids.is_empty() { none.as_ptr() } else { ids.as_ptr() }, ids.len() as u32),
+        };
+        check(unsafe { sys::dab_count_reachable(self.raw, ptr, n, &mut count) })?;
+        Ok(count)
+    }
+
+    /// `get_degree_stats` over `ids` (`None`: every id): (max_degree, avg_degree, min_degree, cnt_less_than_two).
+    pub fn degree_stats(&self, ids: Option<&[u32]>) -> Result<(u32, f32, u32, u64)> {
+        let (mut mx, mut avg, mut mn, mut lt2) = (0u32, 0f32, 0u32, 0u64);
+        let none = [0u32; 1];
+        let (ptr, n) = match ids {
+            None => (std::ptr::null(), 0),
+            Some(ids) => (if ids.is_empty() { none.as_ptr() } else { ids.as_ptr() }, ids.len() as u64),
+        };
+        check(unsafe { sys::dab_degree_stats(self.raw, ptr, n, &mut mx, &mut avg, &mut mn, &mut lt2) })?;
+        Ok((mx, avg, mn, lt2))
+    }
+
+    /// `prune_range` over `ids` (`None`: every id); returns the number of lists rewritten.
+    pub fn prune_range(&mut self, ids: Option<&[u32]>, pruned_degree: u32, alpha: f32) -> Result<u64> {
+        let mut rewritten = 0u64;
+        let none = [0u32; 1];
+        let (ptr, n) = match ids {
+            None => (std::ptr::null(), 0),
+            Some(ids) => (if ids.is_empty() { none.as_ptr() } else { ids.as_ptr() }, ids.len() as u64),
+        };
+        check(unsafe { sys::dab_prune_range(self.raw, ptr, n, pruned_degree, alpha, &mut rewritten) })?;
+        Ok(rewritten)
+    }
+
     /// `KNN::search` for every query of the batch at once (search_internal + post-processing).
     pub fn search_batch(&self, queries: &[T], k: usize, l_search: u32, beam_width: u32) -> Result<Batch> {
         assert_eq!(queries.len() % self.dim, 0);

@@ -622,6 +622,49 @@ int dab_inplace_delete(dab_index* idx, const uint32_t* ids, uint64_t n, int meth
  * sessions fail their next page when a list was written.  out_rewritten (may be NULL): the number of lists written. */
 int dab_drop_deleted_neighbors(dab_index* idx, uint32_t pruned_degree, int only_orphans, uint64_t* out_rewritten);
 
+/* Graph checks and the final prune.
+ *
+ * DiskANNIndex::count_reachable_nodes (diskann/src/graph/index.rs:2161-2189), the reference's health check after a
+ * build, a delete or an insert: *out_count = the number of distinct ids its breadth-first walk expands from the n
+ * start_ids, the start ids included, each counted once, whatever their order or repeats.  start_ids NULL (n must be 0)
+ * walks from the index's start points [n_points, n_points + n_start), what provider().starting_points() returns
+ * (diskann-providers/src/model/graph/provider/async_/inmem/provider.rs:326-328); an explicit list of n = 0 reaches
+ * nothing.  Deleted ids are walked like any other (get_neighbors does not read the deletion table); list lengths above
+ * max_degree are read as max_degree, as the searches read them.  An id >= n_points + n_start in the list of an
+ * expanded node makes the reference's get_neighbors fail (SimpleNeighborProviderAsync::get_neighbors_sync has no list
+ * for it): the call then returns DAB_ERR_INVALID_ARGUMENT naming the smallest such id the walk reached; one in a list the
+ * walk never expands is ignored.  DAB_ERR_INVALID_ARGUMENT, before anything runs, for a start id >= n_points + n_start
+ * or NULL start_ids with n > 0; DAB_ERR_NOT_READY without a graph.  Read-only (no paged session is disturbed), so it
+ * is allowed while batches are in flight; it runs on the handle's stream and returns with the count.  Its scratch (the
+ * visited bitmap and one queue of n_points + n_start ids) is allocated and freed per call, and freeing device memory
+ * waits for the whole device: a call made while batches are in flight returns after they have finished. */
+int dab_count_reachable(dab_index* idx, const uint32_t* start_ids, uint32_t n, uint64_t* out_count);
+/* DiskANNIndex::get_degree_stats (index.rs:2191-2240; DegreeStats, index.rs:69-74) over the list lengths of the n ids,
+ * each occurrence counted (a repeated id counts once per occurrence, as the reference's loop).  ids NULL (n must be 0)
+ * is provider().iter(): every id in [0, n_points + n_start), start points and deleted ids included (inmem/provider.rs:
+ * 330-333); an explicit list of n = 0 gives all zeros, the reference's guard.  out_avg = (float)total / (float)count
+ * with total summed exactly and each conversion rounded to nearest, like Rust's `as f32`: bit-exact.  out_less_than_two
+ * counts the lists shorter than 2.  List lengths above max_degree are read as max_degree.  DAB_ERR_INVALID_ARGUMENT for
+ * an id >= n_points + n_start, NULL ids with n > 0 or a NULL output; DAB_ERR_NOT_READY without a graph.  Read-only,
+ * allowed while batches are in flight, on the handle's stream; like dab_count_reachable it frees per-call scratch, so
+ * it returns after the batches in flight have finished. */
+int dab_degree_stats(dab_index* idx, const uint32_t* ids, uint64_t n, uint32_t* out_max, float* out_avg, uint32_t* out_min,
+                     uint64_t* out_less_than_two);
+/* DiskANNIndex::prune_range (index.rs:2656-2700), "the final step of graph construction", over the n ids (ids NULL with
+ * n = 0: every id in [0, n_points + n_start)): a list of at most pruned_degree entries is left alone; any other becomes
+ * robust_prune_list(id, list) (index.rs:2397-2454): the pool is the list's distinct ids (first occurrence kept) without
+ * id itself and without the ids >= n_points + n_start, which have no row (view.get finds nothing), however short that
+ * leaves it; Distance<T,T> from id's row, sorted by (distance, position), cut to 750, then occlude_list at pruned_degree
+ * and alpha without saturation, the prune kind from the metric — the prune dab_consolidate runs.  The full-precision
+ * PruneAccessor::fill (inmem/full_precision.rs:145-150) finds a row for every id and reads no deletion table, so a
+ * deleted id's list is pruned like any other and deleted neighbours stay in the pools.  Each prune reads only its own
+ * list and rows, so all ids run at once and equal the reference's loop; a repeated id equals one occurrence (the
+ * second prune is a no-op).  *out_rewritten (may be NULL): the lists written.  The rows and every quantized store are
+ * untouched; when a list was written open paged sessions fail their next page.  DAB_ERR_INVALID_ARGUMENT, changing
+ * nothing: an id >= n_points + n_start (naming the first), NULL ids with n > 0, pruned_degree outside [1, max_degree],
+ * alpha < 1, or any slot holding a batch in flight; DAB_ERR_NOT_READY without the vectors and graph. */
+int dab_prune_range(dab_index* idx, const uint32_t* ids, uint64_t n, uint32_t pruned_degree, float alpha, uint64_t* out_rewritten);
+
 /* exact k-NN by exhaustive scan (diskann/src/flat; ground truth for recall):
  * out_ids [nq][k] ascending distance, ties by lower id. */
 int dab_flat_knn(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t* out_ids,

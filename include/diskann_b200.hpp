@@ -197,7 +197,50 @@ class Provider {
         return rewritten;
     }
 
+    // DiskANNIndex::count_reachable_nodes from the start points, or from explicit start ids
+    uint64_t count_reachable() {
+        uint64_t count = 0;
+        check(dab_count_reachable(h_, nullptr, 0, &count));
+        return count;
+    }
+    uint64_t count_reachable(const std::vector<uint32_t>& start_ids) {
+        uint64_t count = 0;
+        const uint32_t none = 0;  // an empty list still passes a pointer: NULL would mean the start points
+        check(dab_count_reachable(h_, start_ids.empty() ? &none : start_ids.data(), (uint32_t)start_ids.size(), &count));
+        return count;
+    }
+    // DiskANNIndex::get_degree_stats over every id, or over explicit ids (an empty list gives all zeros)
+    struct DegreeStats {
+        uint32_t max_degree = 0;
+        float avg_degree = 0.0f;
+        uint32_t min_degree = 0;
+        uint64_t cnt_less_than_two = 0;
+    };
+    DegreeStats degree_stats() { return degree_stats_of(nullptr, 0); }
+    DegreeStats degree_stats(const std::vector<uint32_t>& ids) {
+        const uint32_t none = 0;
+        return degree_stats_of(ids.empty() ? &none : ids.data(), ids.size());
+    }
+    // DiskANNIndex::prune_range over every id, or over explicit ids; returns the lists rewritten
+    uint64_t prune_range(uint32_t pruned_degree, float alpha = 1.2f) {
+        uint64_t rewritten = 0;
+        check(dab_prune_range(h_, nullptr, 0, pruned_degree, alpha, &rewritten));
+        return rewritten;
+    }
+    uint64_t prune_range(const std::vector<uint32_t>& ids, uint32_t pruned_degree, float alpha = 1.2f) {
+        uint64_t rewritten = 0;
+        const uint32_t none = 0;
+        check(dab_prune_range(h_, ids.empty() ? &none : ids.data(), ids.size(), pruned_degree, alpha, &rewritten));
+        return rewritten;
+    }
+
    private:
+    DegreeStats degree_stats_of(const uint32_t* ids, uint64_t n) {
+        DegreeStats s;
+        check(dab_degree_stats(h_, ids, n, &s.max_degree, &s.avg_degree, &s.min_degree, &s.cnt_less_than_two));
+        return s;
+    }
+
     dab_index* h_ = nullptr;
     uint32_t dim_;
     uint64_t n_points_;
