@@ -39,6 +39,9 @@ SYMBOLS = {
     "dab_pairwise": (_i, [_vp, _vp, _u32, _vp]),
     "dab_search_batch": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
     "dab_search_batch_device": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
+    "dab_upload_attributes": (_i, [_vp, _vp, _vp, _u64, _u64]),
+    "dab_search_batch_diverse": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
+    "dab_search_batch_diverse_device": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
     "dab_search_batch_async": (_i, [_vp, _u32, _vp, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
     "dab_search_batch_device_async": (_i, [_vp, _u32, _vp, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
     "dab_wait": (_i, [_vp, _u32]),

@@ -68,6 +68,9 @@ void Tuning::load() {
     const long v = t ? atol(t) : 0;
     test_visited_log2 = v >= 8 && v <= 30 ? (int)v : 0;
     test_pq_global_lut = getenv("DAB_TEST_PQ_GLOBAL_LUT") != nullptr;
+    const char* dp = getenv("DAB_TEST_DIVERSE_POOL");
+    const long pv = dp ? atol(dp) : 0;
+    test_diverse_pool = pv >= 1 && pv <= (1 << 20) ? (uint32_t)pv : 0;
 }
 
 }  // namespace dab
@@ -141,6 +144,7 @@ void dab_destroy(dab_index* idx) {
     tc_release(idx);
     minmax_release(idx);
     deleted_release(idx);
+    attributes_release(idx);
     store_release(idx->sq);
     store_release(idx->mm);
     cudaFree(idx->d_vectors);

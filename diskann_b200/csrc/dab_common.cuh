@@ -35,6 +35,7 @@ void search_slots_release(struct ::dab_index* idx);  // search_kernel.cu
 int retire_quantized_stores(struct ::dab_index* idx);
 void minmax_release(struct ::dab_index* idx);        // minmax_index.cu: the store's transform
 void paged_release(struct ::dab_index* idx);         // search_paged.cu: every paged search session still open
+void attributes_release(struct ::dab_index* idx);    // search_diverse.cu: the attribute table
 // delete_kernels.cu: the deletion table.  deleted_assign replaces it with `words` ((n_total + 31) / 32 of them, bit i of
 // word i / 32 for id i) holding n_deleted set bits; n_deleted == 0 clears it (words may then be NULL).
 int deleted_assign(struct ::dab_index* idx, const uint32_t* words, uint64_t n_deleted);
@@ -115,6 +116,7 @@ struct Scratch {
 struct Tuning {
     int test_visited_log2 = 0;        // DAB_TEST_VISITED_LOG2: tests force the overflow / retry path
     bool test_pq_global_lut = false;  // DAB_TEST_PQ_GLOBAL_LUT: PQ kernels with the per-warp table in global memory also where the pivots fit shared memory
+    uint32_t test_diverse_pool = 0;   // DAB_TEST_DIVERSE_POOL: local-queue entries of a diverse search's first pass (tests force its re-runs)
     void load();
 };
 
@@ -255,6 +257,11 @@ struct dab_index {
     uint32_t* d_deleted = nullptr;
     uint64_t n_deleted = 0;
     uint64_t rec_truncated = 0;  // build: searches whose expanded-node record was cut at its capacity
+    // the attribute table of diverse search (search_diverse.cu): one value and one presence bit per id, allocated by the
+    // first dab_upload_attributes (nothing present).  Independent of the graph: inserts, deletes and releases leave it.
+    uint32_t* d_attr_values = nullptr;   // [n_total]
+    uint32_t* d_attr_present = nullptr;  // (n_total + 31) / 32 words
+    uint32_t* h_attr_present = nullptr;  // the host copy of the presence bits
     dab::Tuning tune;
 
     // tensor-core exhaustive scan (flat_tc.cu): bf16 operand copy of the rows + score coefficients

@@ -1,13 +1,15 @@
 // search_kernel.cu — the host side of batched graph search: the visited-table policy, the one job that runs a batch of
 // any kind with its overflow re-runs and post-processing (full precision; PQ, SQ and MinMax, whose kernels and rerank
 // are in search_kernel_pq.cu and search_kernel_pqs.cu), the slots of batches in flight and the C entry points
-// (dab_search_batch[_pq|_pq_rerank|_sq|_minmax][_device][_async], dab_wait).
+// (dab_search_batch[_pq|_pq_rerank|_sq|_minmax][_device][_async], dab_search_batch_diverse[_device], dab_wait).  The
+// diverse search (search_diverse.cu) is one more kind of the job.
 //
 // A full-precision batch runs on search_kernel_v3 (visited set in shared memory) where its short lists make that the
 // faster kernel, and on search_kernel_v2 (global visited tables) otherwise; queries whose visited set outgrows its table
 // are re-run on v2 with larger tables, so membership stays exact.  Both kernels restate DiskANNIndex::search_internal
 // (index.rs:1933-2000) bit for bit.
 #include "dab_common.cuh"
+#include "search_diverse.cuh"
 #include "search_host.cuh"
 #include "search_pq.cuh"
 #include "search_v2.cuh"
@@ -120,6 +122,10 @@ struct SlotJob {
 
     int store = -1;  // -1: full precision, else the QuantStore the traversal reads
     bool rerank = false;
+    // > 0: a diverse search (full precision) with at most diverse_k results per attribute value; its local queues are
+    // `pool` entries for every warp a pass launches, in `luts` (which only the quantized kinds use otherwise)
+    uint32_t diverse_k = 0;
+    uint64_t pool = 0;
     const void* d_queries = nullptr;
     uint32_t nq = 0, k = 0, l_search = 0, beam = 0, cap = 0;
     SearchRecord rec{};  // searches over rows of the index (rec.query_rows set)
@@ -155,6 +161,9 @@ struct SlotJob {
     PqKernel kern = nullptr;
     int grid = 0;
     size_t smem_block = 0;
+    // diverse
+    SearchParamsDiverse pd;
+    DiversePlan dplan;
 
     SlotJob(dab_index* idx_, cudaStream_t stream_, Scratch& tables_, Scratch& counters_, Scratch& stage_, Scratch& luts_,
             Scratch& lists_, Scratch& pinned_)
@@ -175,11 +184,14 @@ struct SlotJob {
 
     int plan_full();
     int plan_quant();
+    int plan_diverse();
     int reserve_tables();
+    int reserve_pools();
     int stage_queries();
     int launch_pass();
     int launch_full();
     int launch_quant();
+    int launch_diverse();
     int post();
 
     // full precision keeps STORE_PQ in a hint of its own
@@ -228,7 +240,8 @@ int SlotJob::prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint32_t
     d_queries = d_queries_, nq = nq_, k = k_, l_search = l_search_, beam = beam_, store = store_, rerank = rerank_;
     if (rec_) rec = *rec_;
     stores_version = idx->stores_version;
-    cap = l_search + idx->n_start;  // scratch.rs:195-208
+    // scratch.rs:195-208; a diverse search's list holds L (Diverse::create_scratch, diverse_search.rs:149-177)
+    cap = diverse_k ? l_search : l_search + idx->n_start;
     int rc;
     if ((rc = pinned->reserve(24)) || (rc = counters->reserve(16 + (size_t)nq * 4))) return rc;
     h_counters = (uint32_t*)pinned->p;
@@ -245,8 +258,9 @@ int SlotJob::prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint32_t
         out.dists = (float*)(out.ids + (size_t)nq * cap);
     }
     n_work = nq;
-    slots = table_slots(idx, hint(), l_search, beam, mode());
-    if ((rc = store < 0 ? plan_full() : plan_quant())) return rc;
+    // a diverse search visits other nodes than a k-NN search: it neither reads nor teaches the hints
+    slots = table_slots(idx, diverse_k ? VisitedHint{} : hint(), l_search, beam, mode());
+    if ((rc = diverse_k ? plan_diverse() : store < 0 ? plan_full() : plan_quant())) return rc;
     if (!on_v3 && (rc = reserve_tables())) return rc;
     DAB_CUDA(cudaEventCreateWithFlags(&counted, cudaEventDisableTiming));
     return DAB_OK;
@@ -337,6 +351,35 @@ int SlotJob::plan_quant() {
     return stage->reserve(mode == STORE_SQ ? sq_stage_bytes(idx, nq) : mode == STORE_MINMAX ? minmax_stage_bytes(idx, nq) : 0);
 }
 
+// diverse: the kernel's plan, the attribute table and the local queues of the first pass
+int SlotJob::plan_diverse() {
+    memset(&pd, 0, sizeof(pd));
+    int rc;
+    if ((rc = diverse_plan(idx, l_search, beam, pd, dplan))) return rc;
+    set_batch_params(pd);
+    pd.vectors = idx->d_vectors;
+    pd.row_stride = idx->row_stride;
+    pd.attr_values = idx->d_attr_values;
+    pd.attr_present = idx->d_attr_present;
+    pd.diverse_k = diverse_k;
+    // diverse_priority_queue.rs:96 in 64 bits; a local queue holds distinct ids, so a capacity of n_total never fills
+    // and every larger one behaves the same
+    pd.local_cap = (uint32_t)std::min<uint64_t>((uint64_t)diverse_k * l_search / k, idx->n_total());
+    warps = (uint32_t)dplan.grid * kDivWarps;
+    pool = diverse_pool_first(idx, l_search);
+    return reserve_pools();
+}
+
+// the local queues of the warps the next pass over n_work queries launches (diverse_launch's grid)
+int SlotJob::reserve_pools() {
+    int rc;
+    const uint64_t pass_warps = (uint64_t)balanced_grid(n_work, dplan.grid, kDivWarps) * kDivWarps;
+    if ((rc = luts->reserve((size_t)pass_warps * pool * 16))) return rc;
+    pd.pools = (uint32_t*)luts->p;
+    pd.pool_cap = (uint32_t)pool;
+    return DAB_OK;
+}
+
 // a visited table of `slots` ids, in whole 32-byte buckets of 8 ids, for every resident warp
 int SlotJob::reserve_tables() {
     n_buckets = (uint32_t)((slots + 7) / 8);
@@ -355,7 +398,7 @@ int SlotJob::stage_queries() {
 int SlotJob::launch_pass() {
     DAB_CUDA(cudaMemsetAsync(d_counters, 0, 16, stream));
     int rc;
-    if ((rc = store < 0 ? launch_full() : launch_quant())) return rc;
+    if ((rc = diverse_k ? launch_diverse() : store < 0 ? launch_full() : launch_quant())) return rc;
     DAB_CUDA(cudaMemcpyAsync(h_counters, d_counters, 16, cudaMemcpyDeviceToHost, stream));
     DAB_CUDA(cudaEventRecord(counted, stream));
     return DAB_OK;
@@ -384,6 +427,11 @@ int SlotJob::launch_quant() {
     return DAB_OK;
 }
 
+int SlotJob::launch_diverse() {
+    set_pass_params(pd);
+    return diverse_launch(pd, dplan, stream);
+}
+
 // the post-processing of the whole batch: the rerank, or the filter of deleted ids
 int SlotJob::post() {
     if (rerank) return launch_rerank(idx, stream, d_queries, nq, k, cap, pq.list_ids, pq.list_counts, out.ids, out.dists, out.counts, deleted);
@@ -398,7 +446,7 @@ int SlotJob::finish() {
         const uint32_t n_over = h_counters[1];
         if (rec.query_rows) {
             idx->rec_truncated += h_counters[3];
-        } else {  // searches over rows run on a graph being changed: do not learn from them
+        } else if (!diverse_k) {  // searches over rows run on a graph being changed: do not learn from them
             learn_visited(hint(), l_search, beam, mode(), h_counters[2]);
             if (on_v3) {
                 idx->v3_overflow_l = l_search;
@@ -417,12 +465,24 @@ int SlotJob::finish() {
             // the overflowed queries are the largest: size the global tables from the estimate again
             on_v3 = false;
             slots = std::max(slots, table_slots(idx, VisitedHint{}, l_search, beam, mode()));
-        } else if ((rc = grow_visited_tables(idx, pass, slots))) {
+        } else if ((!diverse_k || n_over > h_counters[3]) && (rc = grow_visited_tables(idx, pass, slots))) {
+            // (a diverse pass counts in counters[3] the queries that stopped on their local queues instead)
             return rc;
         }
         if ((rc = reserve_tables())) return rc;
         work = (const uint32_t*)retry.p;
         n_work = n_over;
+        if (diverse_k) {
+            if (h_counters[3]) {
+                const uint64_t grown = diverse_pool_grow(idx, pool);
+                // a pool of n_total entries takes every id: it cannot overflow
+                if (grown == pool)
+                    return fail(DAB_ERR_VISITED_OVERFLOW, "dab_search_batch_diverse: local queues outgrew %llu entries",
+                                (unsigned long long)pool);
+                pool = grown;
+            }
+            if ((rc = reserve_pools())) return rc;
+        }
         reran = true;
         if ((rc = launch_pass())) return rc;
         DAB_CUDA(cudaEventSynchronize(counted));
@@ -431,12 +491,28 @@ int SlotJob::finish() {
     return reran ? post() : DAB_OK;
 }
 
-int run_search(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam, const SearchOut& d,
-               int store, bool rerank, const SearchRecord* rec) {
+// The checks of a diverse search (DiverseSearchParams::new, diverse_search.rs:80-97; Diverse::new, :119-134), all made
+// before any device work.  diverse_k > k is accepted: the reference declares DiverseKGreaterThanTotalK and never returns it.
+static int check_diverse_args(const dab_index* idx, const char* api, uint32_t k, uint32_t l_search, uint32_t beam, uint32_t diverse_k) {
+    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", api);
     int rc;
-    if ((rc = check_batch_args(idx, k, l_search, beam, store))) return rc;
+    if ((rc = check_search_args(idx, k, l_search, beam))) return rc;
+    if (diverse_k == 0) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: diverse k_value cannot be zero", api);
+    if (l_search < k) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: l_value (%u) must be greater than or equal to total_k_value (%u)", api, l_search, k);
+    if (l_search > kDiverseMaxL) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: l_value %u > %u", api, l_search, kDiverseMaxL);
+    if ((rc = diverse_check_smem(idx, api, l_search, beam))) return rc;
+    if (!idx->d_attr_values) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: no attribute table (dab_upload_attributes has not been called)", api);
+    return DAB_OK;
+}
+
+// `diverse_k` > 0: a diverse search, whose arguments check_diverse_args has passed
+static int run_job(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam, const SearchOut& d,
+                   int store, bool rerank, const SearchRecord* rec, uint32_t diverse_k) {
+    int rc;
+    if (!diverse_k && (rc = check_batch_args(idx, k, l_search, beam, store))) return rc;
     if (nq == 0) return DAB_OK;
     SlotJob job(idx, idx->stream, idx->s_tables, idx->s_counters, idx->s_stage, idx->s_out2, idx->s_ids, idx->h_counters);
+    job.diverse_k = diverse_k;
     if ((rc = job.prepare(d_queries, nq, k, l_search, beam, d, store, rerank, rec)) || (rc = job.stage_queries())) return rc;
     if (store == STORE_MINMAX) {  // a batch with a NaN query fails before any traversal is launched
         DAB_CUDA(cudaStreamSynchronize(idx->stream));
@@ -445,6 +521,11 @@ int run_search(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, u
     if ((rc = job.launch_pass()) || (rc = job.post()) || (rc = job.finish())) return rc;
     if (store < 0 && job.filter) DAB_CUDA(cudaStreamSynchronize(idx->stream));  // the filter follows the counters
     return DAB_OK;
+}
+
+int run_search(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam, const SearchOut& d,
+               int store, bool rerank, const SearchRecord* rec) {
+    return run_job(idx, d_queries, nq, k, l_search, beam, d, store, rerank, rec, 0);
 }
 
 // ---- host-buffer calls -------------------------------------------------------------------------
@@ -479,7 +560,7 @@ static int queue_result_copies(cudaStream_t stream, const HostCopy& c) {
 // The synchronous host-buffer calls: checks the buffers, copies the queries to the handle's scratch, runs the batch on
 // them with device result buffers, copies the results to `out` and waits.
 static int search_host(dab_index* idx, const char* api, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
-                       uint32_t beam, const SearchOut& out, int store, bool rerank) {
+                       uint32_t beam, const SearchOut& out, int store, bool rerank, uint32_t diverse_k = 0) {
     if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", api);
     if (nq == 0) return DAB_OK;
     if (!queries || !out.ids || !out.dists) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
@@ -489,7 +570,8 @@ static int search_host(dab_index* idx, const char* api, const void* queries, uin
     int rc;
     if ((rc = reserve_host_call(idx, idx->s_queries, idx->s_out, idx->s_stats, nq, k, &c.dev)) ||
         (rc = queue_query_copy(idx, idx->stream, idx->s_queries.p, queries, nq)) ||
-        (rc = run_search(idx, idx->s_queries.p, nq, k, l_search, beam, c.dev, store, rerank)) || (rc = queue_result_copies(idx->stream, c)))
+        (rc = run_job(idx, idx->s_queries.p, nq, k, l_search, beam, c.dev, store, rerank, nullptr, diverse_k)) ||
+        (rc = queue_result_copies(idx->stream, c)))
         return rc;
     DAB_CUDA(cudaStreamSynchronize(idx->stream));
     return DAB_OK;
@@ -498,12 +580,12 @@ static int search_host(dab_index* idx, const char* api, const void* queries, uin
 // The synchronous device-buffer calls (run_search).  The full-precision call makes its argument checks before it returns
 // for an empty batch; the quantized calls return first.
 static int search_device(dab_index* idx, const char* api, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
-                         uint32_t beam, const SearchOut& d, int store, bool rerank) {
+                         uint32_t beam, const SearchOut& d, int store, bool rerank, uint32_t diverse_k = 0) {
     if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", api);
     if (nq == 0 && store >= 0) return DAB_OK;
     if (nq && (!d_queries || !d.ids || !d.dists)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
     DAB_CUDA(cudaSetDevice(idx->device));
-    return run_search(idx, d_queries, nq, k, l_search, beam, d, store, rerank);
+    return run_job(idx, d_queries, nq, k, l_search, beam, d, store, rerank, nullptr, diverse_k);
 }
 
 // ---- batches in flight (dab_search_batch*_async / dab_wait) --------------------------------------------------------
@@ -650,6 +732,26 @@ int dab_search_batch_minmax_device(dab_index* idx, const void* d_queries, uint32
                                    uint32_t* d_out_hops) {
     return search_device(idx, "dab_search_batch_minmax_device", d_queries, nq, k, l_search, beam_width,
                          SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, STORE_MINMAX, rerank != 0);
+}
+
+// Diverse::search (diverse_search.rs:189-234): every argument is checked before the queries are copied
+int dab_search_batch_diverse(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
+                             uint32_t diverse_k, uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps,
+                             uint32_t* out_hops) {
+    int rc;
+    if ((rc = check_diverse_args(idx, "dab_search_batch_diverse", k, l_search, beam_width, diverse_k))) return rc;
+    return search_host(idx, "dab_search_batch_diverse", queries, nq, k, l_search, beam_width,
+                       SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, -1, false, diverse_k);
+}
+
+// returns with the outputs complete, the filter of deleted ids included
+int dab_search_batch_diverse_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
+                                    uint32_t diverse_k, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
+                                    uint32_t* d_out_cmps, uint32_t* d_out_hops) {
+    int rc;
+    if ((rc = check_diverse_args(idx, "dab_search_batch_diverse_device", k, l_search, beam_width, diverse_k))) return rc;
+    return search_device(idx, "dab_search_batch_diverse_device", d_queries, nq, k, l_search, beam_width,
+                         SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, -1, false, diverse_k);
 }
 
 // ---- asynchronous batches: launch on a slot, collect with dab_wait ---------------------------

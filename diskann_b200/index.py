@@ -427,6 +427,34 @@ class GpuIndex:
                                                  C.c_void_p(d_ids), C.c_void_p(d_dists), C.c_void_p(d_counts or None),
                                                  C.c_void_p(d_cmps or None), C.c_void_p(d_hops or None)))
 
+    def upload_attributes(self, values, present=None, first=0):
+        """The attribute of ids first .. first + len(values) - 1 for search_batch_diverse: `values` u32, `present` bool
+        (None: every id of the range has its value; False: the id has no attribute, so diverse search skips it)."""
+        values = np.ascontiguousarray(values, np.uint32).ravel()
+        pres = None if present is None else np.ascontiguousarray(present, np.uint8).ravel()
+        if pres is not None and pres.shape != values.shape:
+            raise ValueError("upload_attributes: present must have one entry per value")
+        check(_lib.lib().dab_upload_attributes(self._h, _ptr(values), None if pres is None else _ptr(pres), first, values.shape[0]))
+
+    def search_batch_diverse(self, queries, k, l_search, diverse_k, beam_width=1):
+        """Diverse::search for the whole batch: at most diverse_k results per attribute value (upload_attributes);
+        (ids [nq,k], dists [nq,k], counts, cmps, hops)."""
+        queries = self._queries(queries)
+        nq = queries.shape[0]
+        ids = np.empty((nq, k), np.uint32)
+        dists = np.empty((nq, k), np.float32)
+        counts, cmps, hops = (np.empty(nq, np.uint32) for _ in range(3))
+        check(_lib.lib().dab_search_batch_diverse(self._h, _ptr(queries), nq, k, l_search, beam_width, diverse_k, _ptr(ids), _ptr(dists),
+                                                  _ptr(counts), _ptr(cmps), _ptr(hops)))
+        return ids, dists, counts, cmps, hops
+
+    def search_batch_diverse_device(self, d_queries, nq, k, l_search, diverse_k, beam_width, d_ids, d_dists, d_counts=0, d_cmps=0,
+                                    d_hops=0):
+        """search_batch_diverse with device pointers (integers); results stay in HBM."""
+        check(_lib.lib().dab_search_batch_diverse_device(self._h, C.c_void_p(d_queries), nq, k, l_search, beam_width, diverse_k,
+                                                         C.c_void_p(d_ids), C.c_void_p(d_dists), C.c_void_p(d_counts or None),
+                                                         C.c_void_p(d_cmps or None), C.c_void_p(d_hops or None)))
+
     def search_batch_async(self, slot, queries, k, l_search, beam_width=1, out=None):
         """Queue a batch on `slot` (host buffers) and return its output arrays without waiting; they are
         valid after wait(slot).  `queries` is used as passed (it must stay alive and unchanged until then);

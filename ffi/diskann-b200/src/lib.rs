@@ -184,6 +184,32 @@ impl<T: Element> GpuIndex<T> {
         Ok(b)
     }
 
+    /// The attribute of ids `first ..` for `search_batch_diverse` (the reference's `AttributeValueProvider`); `present`
+    /// `None`: every id of the range has its value, else `false` marks an id without an attribute.
+    pub fn upload_attributes(&mut self, values: &[u32], present: Option<&[bool]>, first: u64) -> Result<()> {
+        let flags: Option<Vec<u8>> = present.map(|p| {
+            assert_eq!(p.len(), values.len());
+            p.iter().map(|&b| b as u8).collect()
+        });
+        check(unsafe {
+            sys::dab_upload_attributes(self.raw, values.as_ptr(), flags.as_ref().map_or(std::ptr::null(), |f| f.as_ptr()), first,
+                                       values.len() as u64)
+        })
+    }
+
+    /// `Diverse::search` (diverse_search.rs:189-234): at most `diverse_k` results per attribute value.
+    pub fn search_batch_diverse(&self, queries: &[T], k: usize, l_search: u32, diverse_k: u32, beam_width: u32) -> Result<Batch> {
+        assert_eq!(queries.len() % self.dim, 0);
+        let nq = queries.len() / self.dim;
+        let mut b = Batch { k, ids: vec![0; nq * k], dists: vec![0.0; nq * k], counts: vec![0; nq], cmps: vec![0; nq], hops: vec![0; nq] };
+        check(unsafe {
+            sys::dab_search_batch_diverse(self.raw, queries.as_ptr() as *const c_void, nq as u32, k as u32, l_search, beam_width, diverse_k,
+                                          b.ids.as_mut_ptr(), b.dists.as_mut_ptr(), b.counts.as_mut_ptr(), b.cmps.as_mut_ptr(),
+                                          b.hops.as_mut_ptr())
+        })?;
+        Ok(b)
+    }
+
     /// Queue a batch on `slot` without waiting (`search_all`'s one task per partition, api.rs:410-419, mapped to
     /// device slots).  The returned guard borrows the queries and owns the result buffers; `InFlight::wait` joins it.
     pub fn search_batch_async<'a>(&'a self, slot: u32, queries: &'a [T], k: usize, l_search: u32, beam_width: u32) -> Result<InFlight<'a, T>> {

@@ -169,6 +169,42 @@ int dab_search_batch_device(dab_index* idx, const void* d_queries, uint32_t nq, 
                             float* d_out_dists, uint32_t* d_out_counts, uint32_t* d_out_cmps,
                             uint32_t* d_out_hops);
 
+/* ------------------------------------------------------------------ (3''') diverse search */
+
+/* The attribute table of diverse search: AttributeValueProvider::get
+ * (diskann/src/neighbor/diverse_priority_queue.rs:265-279) as one u32 value and one presence
+ * bit per id, over every id of the index (start points included).  Ids [first, first + count)
+ * take values[i]; present[i] != 0 marks id first + i as having an attribute (present NULL: all
+ * of them), present[i] == 0 as having none.  first + count <= n_points + n_start.  The first
+ * call allocates the table with no id present.  The table is independent of the graph: inserts,
+ * deletes and releases neither read nor clear it (an inserted point has what was uploaded for
+ * its id). */
+int dab_upload_attributes(dab_index* idx, const uint32_t* values, const uint8_t* present,
+                          uint64_t first, uint64_t count);
+
+/* Diverse::search (diskann/src/graph/search/diverse_search.rs:189-234) for a whole query batch:
+ * search_internal with a DiverseNeighborQueue (neighbor/diverse_priority_queue.rs:90-220) of L
+ * entries and one local queue of diverse_k * L / k entries per attribute value, then its
+ * post_process (at most diverse_k entries per attribute value stay in the list) and the k-NN
+ * post-processing of the first L entries (start points and deleted ids dropped, the first k kept).
+ * Ids without an attribute never enter the list; they are still visited and counted in cmps.
+ * Full-precision rows of every dtype and metric; k >= 1, diverse_k >= 1 (diverse_k > k is
+ * accepted, as in the reference), k <= l_search <= 1024, 1 <= beam_width <= 64, a CTA's shared
+ * memory fits 200 KB: 4 x (query row (f32 for float rows, the bytes for i8 / u8) + 12 * l_search
+ * + 8 * beam_width * max_degree + 4 * beam_width bytes, each part rounded up to 16, the whole to
+ * 128), and an attribute table must have been uploaded: each is checked before any device work
+ * and fails with DAB_ERR_INVALID_ARGUMENT and a message.  Outputs as dab_search_batch. */
+int dab_search_batch_diverse(dab_index* idx, const void* queries, uint32_t nq, uint32_t k,
+                             uint32_t l_search, uint32_t beam_width, uint32_t diverse_k,
+                             uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
+                             uint32_t* out_cmps, uint32_t* out_hops);
+/* the same with device buffers; returns with the outputs complete */
+int dab_search_batch_diverse_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k,
+                                    uint32_t l_search, uint32_t beam_width, uint32_t diverse_k,
+                                    uint32_t* d_out_ids, float* d_out_dists,
+                                    uint32_t* d_out_counts, uint32_t* d_out_cmps,
+                                    uint32_t* d_out_hops);
+
 /* ------------------------------------------------------------------ (3'') paged search */
 
 /* DiskANNIndex::paged_search (diskann/src/graph/index.rs:2075-2155) and PagedSearch::next_page

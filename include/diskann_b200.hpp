@@ -161,6 +161,12 @@ class Provider {
         return out;
     }
 
+    // AttributeValueProvider for diverse search: ids [first, first + count) take values[i]; present[i] == 0 (present
+    // NULL: none) marks an id without an attribute
+    void set_attributes(const uint32_t* values, const uint8_t* present, uint64_t first, uint64_t count) {
+        check(dab_upload_attributes(h_, values, present, first, count));
+    }
+
     // index construction on the device (multi_insert semantics)
     void build(uint32_t pruned_degree, uint32_t l_build, float alpha = 1.2f, uint32_t batch = 0) {
         check(dab_build(h_, pruned_degree, l_build, alpha, batch));
@@ -245,6 +251,32 @@ class Provider {
     uint32_t dim_;
     uint64_t n_points_;
     uint32_t n_start_, max_degree_;
+};
+
+// Diverse::search for a whole batch (diverse_search.rs:114-234): Diverse::new(Knn::new(l_value, beam_width),
+// DiverseSearchParams::new(_, diverse_k, k, provider's attributes)); at most diverse_k results per attribute value.
+template <class T>
+class GpuDiverse {
+   public:
+    GpuDiverse(Provider<T>& provider, uint32_t l_value, uint32_t diverse_k, uint32_t beam_width = 1)
+        : p_(provider), l_(l_value), diverse_k_(diverse_k), beam_(beam_width) {}
+    KnnResults search(const T* queries, uint32_t nq, uint32_t k) {
+        KnnResults r;
+        r.nq = nq;
+        r.k = k;
+        r.ids.resize((size_t)nq * k);
+        r.distances.resize((size_t)nq * k);
+        std::vector<uint32_t> counts(nq), cmps(nq), hops(nq);
+        check(dab_search_batch_diverse(p_.raw(), queries, nq, k, l_, beam_, diverse_k_, r.ids.data(), r.distances.data(), counts.data(),
+                                       cmps.data(), hops.data()));
+        r.stats.resize(nq);
+        for (uint32_t i = 0; i < nq; ++i) r.stats[i] = SearchStats{cmps[i], hops[i], counts[i]};
+        return r;
+    }
+
+   private:
+    Provider<T>& p_;
+    uint32_t l_, diverse_k_, beam_;
 };
 
 // KNN::search for a whole batch: Knn::new(l_value, beam_width) + k results per query.

@@ -66,6 +66,9 @@ for dt, ddt, metric, d in ((np.float32, dab.DType.f32, dab.Metric.L2, 100), (np.
         block = g.pairwise(ids[3, :17])
         got = g.search_batch(base[:64], 5, 64, 1)                # search_kernel_v2
         got4 = g.search_batch(base[:64], 5, 40, 4)
+        g.upload_attributes(rng.integers(0, 7, n + 1), rng.random(n + 1) < 0.9)
+        div = g.search_batch_diverse(base[:64], 5, 40, 2, 1)     # diverse_kernel
+        div4 = g.search_batch_diverse(base[:64], 5, 300, 1, 4)
         knn = g.flat_knn(base[:16], 5)
         knn_tc = g.flat_knn_tc(base[:16], 5)                     # wgmma + TMA path
         assert np.array_equal(knn[0], knn_tc[0])
@@ -74,6 +77,6 @@ for dt, ddt, metric, d in ((np.float32, dab.DType.f32, dab.Metric.L2, 100), (np.
             g.pq_encode_all()
             pq = g.search_batch_pq(base[:32], 5, 40, 1, rerank=True)  # PQ traversal + rerank kernel
             g.pq_self_distances(ids[4, :20], ids[5, :20])
-        print(dt.__name__, "deg max", int(adj[:, 0].max()), "search ok", int(got[2].min()), int(got4[2].min()),
+        print(dt.__name__, "deg max", int(adj[:, 0].max()), "search ok", int(got[2].min()), int(got4[2].min()), int(div[2].min()), int(div4[2].min()),
               "finite", bool(np.isfinite(out[1:]).all() and np.isfinite(pairs).all() and np.isfinite(block).all()), knn[0].shape)
 print("sanitize_check done")
