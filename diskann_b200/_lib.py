@@ -42,6 +42,12 @@ SYMBOLS = {
     "dab_upload_attributes": (_i, [_vp, _vp, _vp, _u64, _u64]),
     "dab_search_batch_diverse": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
     "dab_search_batch_diverse_device": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
+    "dab_search_batch_diverse_pq": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _u32, _i, _vp, _vp, _vp, _vp, _vp]),
+    "dab_search_batch_diverse_pq_device": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _u32, _i, _vp, _vp, _vp, _vp, _vp]),
+    "dab_search_batch_diverse_sq": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _u32, _i, _vp, _vp, _vp, _vp, _vp]),
+    "dab_search_batch_diverse_sq_device": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _u32, _i, _vp, _vp, _vp, _vp, _vp]),
+    "dab_search_batch_diverse_minmax": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _u32, _i, _vp, _vp, _vp, _vp, _vp]),
+    "dab_search_batch_diverse_minmax_device": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _u32, _i, _vp, _vp, _vp, _vp, _vp]),
     "dab_search_batch_async": (_i, [_vp, _u32, _vp, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
     "dab_search_batch_device_async": (_i, [_vp, _u32, _vp, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
     "dab_wait": (_i, [_vp, _u32]),

@@ -161,6 +161,7 @@ void dab_destroy(dab_index* idx) {
     idx->s_counters.release();
     idx->s_stats.release();
     idx->s_stage.release();
+    idx->s_pools.release();
     idx->h_stage.release();
     idx->h_counters.release();
     if (idx->own_stream) cudaStreamDestroy(idx->own_stream);

@@ -234,6 +234,7 @@ struct dab_index {
     // scratch (grow-only)
     dab::Scratch s_queries, s_ids, s_out, s_out2, s_tables, s_counters, s_stats;
     dab::Scratch s_stage;  // packed-code store upload / encode / download staging, and the SQ and MinMax searches' compressed queries
+    dab::Scratch s_pools;  // the local queues of diverse search (search_diverse.cu)
     dab::Scratch h_stage;  // pinned host staging
     dab::Scratch h_counters;  // pinned: the four counters a search pass reports
     void* slots[DAB_MAX_SLOTS] = {};  // batches in flight (dab_search_batch_async), search_kernel.cu

@@ -3,8 +3,9 @@
 // DiverseNeighborQueue (diskann/src/neighbor/diverse_priority_queue.rs:90-220), then its post_process and the default
 // post-processing of the first L entries; and the attribute table it reads (dab_upload_attributes).
 //
-// One warp per query on global visited tables, full-precision rows of every type and metric of the k-NN path.  The
-// warp keeps, per query:
+// One warp per query on global visited tables, over full-precision rows of every type and metric of the k-NN path
+// (diverse_kernel) or the PQ, SQ and MinMax stores with the distances of their k-NN traversal and an optional
+// full-precision rerank of the post-processed list (diverse_kernel_quant).  The warp keeps, per query:
 //   the global list   L entries sorted as a NeighborPriorityQueue sorts them (distance ascending, a later insertion
 //                     first among equal distances), each with its id | visited flag and its attribute, in shared memory;
 //                     the cursor is the reference's plain index (after a removal at the cursor it may point at a visited
@@ -19,6 +20,7 @@
 // counters[3] and is re-run by the job on a pool four times larger (at most n_total entries, which never overflow), so
 // no query is ever answered from a truncated pool.  A query that outgrew its visited table instead gets a larger table.
 #include "dab_common.cuh"
+#include "quant_device.cuh"
 #include "search_common.cuh"
 #include "search_diverse.cuh"
 #include "search_host.cuh"
@@ -258,17 +260,17 @@ __device__ __forceinline__ void diverse_post_process(const SearchParamsDiverse& 
     q.size = w;
 }
 
-template <typename TD, int KIND, int POST, int NA>
-__global__ void __launch_bounds__(kDivWarps * 32) diverse_kernel(const SearchParamsDiverse p) {
-    constexpr bool INT = std::is_same<TD, int8_t>::value || std::is_same<TD, uint8_t>::value;
-    extern __shared__ __align__(128) uint8_t smem[];
-    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    uint8_t* base = smem + (size_t)wib * p.warp_smem;
-    float* qf = reinterpret_cast<float*>(base);
+// One warp's share of a pass: the diverse search of every query it takes, whatever the distances are.  Src is the
+// distance source: load(q) brings query q into the front of the warp's shared memory, prepare() runs once the visited
+// table is cleared (what the distances need of the loaded query), and distances(cid, cd, n) writes the distances of
+// cid[0..n) into cd[0..n) and ends with the warp converged.  LIST: with p.list_ids, the post-processed list of each
+// query is written for the rerank.
+template <bool LIST, class Src>
+__device__ __forceinline__ void diverse_queries(const SearchParamsDiverse& p, uint8_t* base, int lane, Src& src) {
+    const int wib = threadIdx.x >> 5;
     uint32_t* cid = reinterpret_cast<uint32_t*>(base + p.off_cid);
     float* cd = reinterpret_cast<float*>(base + p.off_cd);
     uint32_t* beam_ids = reinterpret_cast<uint32_t*>(base + p.off_beam);
-    const int dim = (int)p.dim;
     const uint32_t warp_slot = blockIdx.x * kDivWarps + wib;
     const uint32_t nbk = p.n_buckets;
     uint32_t* table = p.tables + (size_t)warp_slot * nbk * 8;
@@ -276,39 +278,14 @@ __global__ void __launch_bounds__(kDivWarps * 32) diverse_kernel(const SearchPar
     const uint64_t n_total = p.n_points + p.n_start;
     uint32_t* pool = p.pools + (size_t)warp_slot * p.pool_cap * 4;
 
-    // distances of cid[0..n) into cd[0..n): a team of lanes per row, rows from global memory
-    int qq = 0;  // integer rows: Sum x^2 of the query (unused by inner product)
-    auto distances = [&](uint32_t n) {
-        constexpr int S = INT ? 32 : 8 * NA, TEAMS = 32 / S, U = kDivRows;
-        using Row = typename std::conditional<INT, uint8_t, TD>::type;
-        const int team = lane / S, slot = lane % S;
-        for (uint32_t c0 = 0; c0 < n; c0 += TEAMS * U) {
-            float r[U];
-            uint32_t cc[U];
-            const Row* rows[U];
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                cc[u] = c0 + u * TEAMS + team;
-                rows[u] = reinterpret_cast<const Row*>(p.vectors + (size_t)cid[min(cc[u], n - 1)] * p.row_stride);
-            }
-            if constexpr (INT) warp_int_multi<std::is_same<TD, int8_t>::value, KIND, U>(reinterpret_cast<const uint8_t*>(qf), rows, dim, lane, qq, r);
-            else team_float_multi<NA, KIND, U>(qf, rows, dim, slot, r);
-#pragma unroll
-            for (int u = 0; u < U; ++u)
-                if (slot == 0 && cc[u] < n) cd[cc[u]] = post_op<POST>(r[u]);
-        }
-        __syncwarp();
-    };
+    auto distances = [&](uint32_t n) { src.distances(cid, cd, n); };
 
     for (uint32_t qidx; next_query(p.counters, p.n_work, p.query_list, lane, qidx);) {
         __syncwarp();
-        load_query(reinterpret_cast<const TD*>(p.queries) + (size_t)qidx * dim, dim, 4, qf, lane);
+        src.load(qidx);
         for (uint32_t i = lane; i < nbk; i += 32) store_empty_bucket(table + (size_t)i * 8);
         __syncwarp();
-        if constexpr (INT) {
-            if (KIND != KIND_IP) qq = warp_int_self<std::is_same<TD, int8_t>::value>(reinterpret_cast<const uint8_t*>(qf), dim, lane);
-        }
-
+        src.prepare();
         DivQuery q;
         q.gd = reinterpret_cast<float*>(base + p.off_gd);
         q.gi = reinterpret_cast<uint32_t*>(base + p.off_gi);
@@ -384,9 +361,98 @@ __global__ void __launch_bounds__(kDivWarps * 32) diverse_kernel(const SearchPar
             continue;
         }
         diverse_post_process(p, q, lane);
+        if constexpr (LIST) {
+            if (p.list_ids) write_list(q.gi, q.size, p.list_ids, p.list_counts, p.list_cap, qidx, lane);
+        }
         const uint32_t count = write_results(q.gi, q.gd, q.size, p.n_points, p.k, p.out_ids, p.out_dists, qidx, lane);
         write_stats(p.counters, nvisited, p.out_counts, p.out_cmps, p.out_hops, qidx, count, cmps, hops, lane);
     }
+}
+
+// Full precision: rows from global memory with the shared distance schemas (distance_device.cuh), a team of lanes per row
+template <typename TD, int KIND, int POST, int NA>
+__global__ void __launch_bounds__(kDivWarps * 32) diverse_kernel(const SearchParamsDiverse p) {
+    constexpr bool INT = std::is_same<TD, int8_t>::value || std::is_same<TD, uint8_t>::value;
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    uint8_t* base = smem + (size_t)wib * p.warp_smem;
+    struct {
+        const SearchParamsDiverse& p;
+        float* qf;
+        int lane, dim, qq;  // qq, integer rows: Sum x^2 of the query (unused by inner product)
+        __device__ __forceinline__ void load(uint32_t q) { load_query(reinterpret_cast<const TD*>(p.queries) + (size_t)q * dim, dim, 4, qf, lane); }
+        __device__ __forceinline__ void prepare() {
+            if constexpr (INT) {
+                if (KIND != KIND_IP) qq = warp_int_self<std::is_same<TD, int8_t>::value>(reinterpret_cast<const uint8_t*>(qf), dim, lane);
+            }
+        }
+        __device__ __forceinline__ void distances(const uint32_t* cid, float* cd, uint32_t n) {
+            constexpr int S = INT ? 32 : 8 * NA, TEAMS = 32 / S, U = kDivRows;
+            using Row = typename std::conditional<INT, uint8_t, TD>::type;
+            const int team = lane / S, slot = lane % S;
+            for (uint32_t c0 = 0; c0 < n; c0 += TEAMS * U) {
+                float r[U];
+                uint32_t cc[U];
+                const Row* rows[U];
+#pragma unroll
+                for (int u = 0; u < U; ++u) {
+                    cc[u] = c0 + u * TEAMS + team;
+                    rows[u] = reinterpret_cast<const Row*>(p.vectors + (size_t)cid[min(cc[u], n - 1)] * p.row_stride);
+                }
+                if constexpr (INT) warp_int_multi<std::is_same<TD, int8_t>::value, KIND, U>(reinterpret_cast<const uint8_t*>(qf), rows, dim, lane, qq, r);
+                else team_float_multi<NA, KIND, U>(qf, rows, dim, slot, r);
+#pragma unroll
+                for (int u = 0; u < U; ++u)
+                    if (slot == 0 && cc[u] < n) cd[cc[u]] = post_op<POST>(r[u]);
+            }
+            __syncwarp();
+        }
+    } src{p, reinterpret_cast<float*>(base), lane, (int)p.dim, 0};
+    diverse_queries<false>(p, base, lane, src);
+}
+
+// The quantized accessors (MODE as search_kernel_pq: 0 PQ, 1 SQ, 2 MinMax), per candidate the code of quant_device.cuh,
+// one lane per candidate: the traversal distances of dab_search_batch_{pq,sq,minmax}.
+//   PQ: the query (index dtype, T: Into<f32>) in f32 at the front of the warp's shared memory; TableL2 / TableIP build
+//     the query's table once per query into the warp's own slice of p.luts (global memory, read through L2: the table
+//     does not fit next to the list in shared memory), DirectCosine reads the pivots directly.
+//   SQ / MinMax: the query's code words (and MinMax its four compensations), staged before the launch, copied to the
+//     front of the warp's shared memory; the SQ compensation stays in a register.
+template <int MODE>
+__global__ void __launch_bounds__(kDivWarps * 32) diverse_kernel_quant(const SearchParamsDiverse p) {
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    uint8_t* base = smem + (size_t)wib * p.warp_smem;
+    const uint32_t entries = p.n_chunks * p.n_centers;
+    struct {
+        const SearchParamsDiverse& p;
+        float* qf;     // PQ: the f32 query
+        uint32_t* qc;  // SQ / MinMax: the query's code words, then (MinMax) {b, n, a, norm_squared}
+        float* lut;    // PQ tables: this warp's table
+        int lane, dim;
+        uint32_t entries;
+        float q_comp;
+        __device__ __forceinline__ void load(uint32_t q) {
+            if (MODE == 0) widen_query(p.dtype, p.queries, q, dim, qf, lane);
+            else load_query_codes<MODE>(p.query_codes + (size_t)q * p.code_stride, p.query_meta + q, p.code_stride >> 2, qc, q_comp, lane);
+        }
+        __device__ __forceinline__ void prepare() {
+            if (MODE == 0 && !p.direct_cosine) {
+                for (uint32_t t = lane; t < entries; t += 32) __stcg(lut + t, pq_table_entry(p, qf, dim, t));
+                __syncwarp();
+            }
+        }
+        __device__ __forceinline__ void distances(const uint32_t* cid, float* cd, uint32_t n) {
+            for (uint32_t c = lane; c < n; c += 32) {
+                if (MODE != 0) cd[c] = packed_code_distance<MODE>(p, qc, q_comp, cid[c]);
+                else if (p.direct_cosine) cd[c] = pq_direct_cosine(p, qf, dim, cid[c]);
+                else cd[c] = pq_table_distance(p, lut, cid[c]);
+            }
+            __syncwarp();
+        }
+    } src{p, reinterpret_cast<float*>(base), reinterpret_cast<uint32_t*>(base),
+          p.luts + (size_t)(blockIdx.x * kDivWarps + wib) * entries, lane, (int)p.dim, entries, 0.0f};
+    diverse_queries<true>(p, base, lane, src);
 }
 
 template <typename S>
@@ -396,11 +462,14 @@ void (*diverse_kernel_of())(const SearchParamsDiverse) {
 
 }  // namespace
 
-// A warp's shared memory: the query (integer rows: its bytes; float rows: f32), the list's distances, ids and attributes,
-// a hop's candidate ids and distances, the beam; `p` (may be NULL) takes the offsets
-static size_t diverse_warp_smem(const dab_index* idx, uint32_t l_search, uint32_t beam, SearchParamsDiverse* p) {
+// A warp's shared memory: the query area (kDiverseMaxSmem's comment), the list's distances, ids and attributes, a hop's
+// candidate ids and distances, the beam; `p` (may be NULL) takes the offsets.  `store`: -1 full precision, else a
+// QuantStore.
+static size_t diverse_warp_smem(const dab_index* idx, uint32_t l_search, uint32_t beam, int store, SearchParamsDiverse* p) {
     const bool is_int = idx->dtype == DAB_I8 || idx->dtype == DAB_U8;
-    size_t off = is_int ? round_up(round_up((size_t)idx->dim, 4), 16) : round_up((size_t)idx->dim * 4, 16);
+    size_t off;
+    if (store == STORE_SQ || store == STORE_MINMAX) off = round_up((size_t)(store == STORE_SQ ? idx->sq : idx->mm).stride + 16, 16);
+    else off = is_int && store < 0 ? round_up(round_up((size_t)idx->dim, 4), 16) : round_up((size_t)idx->dim * 4, 16);
     const size_t list = round_up((size_t)l_search * 4, 16);
     const size_t ncand = round_up(std::max<size_t>((size_t)beam * idx->max_degree, 32) * 4, 16);
     SearchParamsDiverse scratch;
@@ -414,26 +483,37 @@ static size_t diverse_warp_smem(const dab_index* idx, uint32_t l_search, uint32_
     return round_up(off, 128);
 }
 
-int diverse_check_smem(const dab_index* idx, const char* api, uint32_t l_search, uint32_t beam) {
-    const size_t smem = diverse_warp_smem(idx, l_search, beam, nullptr) * kDivWarps;
+int diverse_check_smem(const dab_index* idx, const char* api, uint32_t l_search, uint32_t beam, int store) {
+    const size_t smem = diverse_warp_smem(idx, l_search, beam, store, nullptr) * kDivWarps;
     if (smem > kDiverseMaxSmem)
         return fail(DAB_ERR_INVALID_ARGUMENT, "%s: L=%u, beam_width=%u, dim=%u, max_degree=%u need %zu B shared memory per CTA (> %zu)", api,
                     l_search, beam, idx->dim, idx->max_degree, smem, kDiverseMaxSmem);
     return DAB_OK;
 }
 
-int diverse_plan(const dab_index* idx, uint32_t l_search, uint32_t beam, SearchParamsDiverse& p, DiversePlan& plan) {
+// the grid of `kern` at `smem_block` bytes per CTA, at most max_per_sm CTAs per SM
+static int diverse_grid(const dab_index* idx, uint32_t l_search, uint32_t beam, int max_per_sm, DiversePlan& plan) {
+    const int per_sm = plan.smem_block > kDiverseMaxSmem ? 0 : ctas_per_sm(plan.kern, kDivWarps * 32, plan.smem_block);
+    if (per_sm < 1)
+        return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_diverse: L=%u, beam_width=%u, dim=%u need %zu B shared memory per CTA",
+                    l_search, beam, idx->dim, plan.smem_block);
+    plan.grid = std::min(per_sm, max_per_sm) * idx->sm_count;
+    return DAB_OK;
+}
+
+int diverse_plan(const dab_index* idx, uint32_t l_search, uint32_t beam, int store, SearchParamsDiverse& p, DiversePlan& plan) {
+    p.warp_smem = (uint32_t)diverse_warp_smem(idx, l_search, beam, store, &p);
+    plan.smem_block = (size_t)p.warp_smem * kDivWarps;
+    if (store >= 0) {
+        plan.kern = store == STORE_PQ ? diverse_kernel_quant<0> : store == STORE_SQ ? diverse_kernel_quant<1> : diverse_kernel_quant<2>;
+        // every resident warp owns a PQ table (n_chunks x n_centers f32: 32 KB at 32 x 256) that its lookups read
+        // through L2: the cap of search_kernel_pq keeps them L2-resident
+        const bool tables = store == STORE_PQ && idx->metric != DAB_COSINE;
+        return diverse_grid(idx, l_search, beam, tables ? 6 : INT32_MAX, plan);
+    }
     return visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) -> int {
-        using S = decltype(sc);
-        p.warp_smem = (uint32_t)diverse_warp_smem(idx, l_search, beam, &p);
-        plan.smem_block = (size_t)p.warp_smem * kDivWarps;
-        plan.kern = diverse_kernel_of<S>();
-        const int per_sm = plan.smem_block > kDiverseMaxSmem ? 0 : ctas_per_sm(plan.kern, kDivWarps * 32, plan.smem_block);
-        if (per_sm < 1)
-            return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_diverse: L=%u, beam_width=%u, dim=%u need %zu B shared memory per CTA",
-                        l_search, beam, idx->dim, plan.smem_block);
-        plan.grid = per_sm * idx->sm_count;
-        return DAB_OK;
+        plan.kern = diverse_kernel_of<decltype(sc)>();
+        return diverse_grid(idx, l_search, beam, INT32_MAX, plan);
     });
 }
 

@@ -1,8 +1,9 @@
 // search_kernel.cu — the host side of batched graph search: the visited-table policy, the one job that runs a batch of
 // any kind with its overflow re-runs and post-processing (full precision; PQ, SQ and MinMax, whose kernels and rerank
 // are in search_kernel_pq.cu and search_kernel_pqs.cu), the slots of batches in flight and the C entry points
-// (dab_search_batch[_pq|_pq_rerank|_sq|_minmax][_device][_async], dab_search_batch_diverse[_device], dab_wait).  The
-// diverse search (search_diverse.cu) is one more kind of the job.
+// (dab_search_batch[_pq|_pq_rerank|_sq|_minmax][_device][_async], dab_search_batch_diverse[_pq|_sq|_minmax][_device],
+// dab_wait).  The diverse search (search_diverse.cu), over full-precision rows or a quantized store, is one more kind of
+// the job.
 //
 // A full-precision batch runs on search_kernel_v3 (visited set in shared memory) where its short lists make that the
 // faster kernel, and on search_kernel_v2 (global visited tables) otherwise; queries whose visited set outgrows its table
@@ -122,10 +123,12 @@ struct SlotJob {
 
     int store = -1;  // -1: full precision, else the QuantStore the traversal reads
     bool rerank = false;
-    // > 0: a diverse search (full precision) with at most diverse_k results per attribute value; its local queues are
-    // `pool` entries for every warp a pass launches, in `luts` (which only the quantized kinds use otherwise)
+    // > 0: a diverse search with at most diverse_k results per attribute value, over full-precision rows or `store`; its
+    // local queues are `pool` entries for every warp a pass launches, in `pools` (the synchronous calls' own region: a
+    // PQ traversal's tables stay in `luts`, as in every quantized kind)
     uint32_t diverse_k = 0;
     uint64_t pool = 0;
+    Scratch* pools = nullptr;
     const void* d_queries = nullptr;
     uint32_t nq = 0, k = 0, l_search = 0, beam = 0, cap = 0;
     SearchRecord rec{};  // searches over rows of the index (rec.query_rows set)
@@ -355,7 +358,7 @@ int SlotJob::plan_quant() {
 int SlotJob::plan_diverse() {
     memset(&pd, 0, sizeof(pd));
     int rc;
-    if ((rc = diverse_plan(idx, l_search, beam, pd, dplan))) return rc;
+    if ((rc = diverse_plan(idx, l_search, beam, store, pd, dplan))) return rc;
     set_batch_params(pd);
     pd.vectors = idx->d_vectors;
     pd.row_stride = idx->row_stride;
@@ -366,6 +369,23 @@ int SlotJob::plan_diverse() {
     // and every larger one behaves the same
     pd.local_cap = (uint32_t)std::min<uint64_t>((uint64_t)diverse_k * l_search / k, idx->n_total());
     warps = (uint32_t)dplan.grid * kDivWarps;
+    if (store >= 0) {
+        // the quantized traversal: the store, a PQ table for every warp of the grid, the lists of the rerank (the
+        // post-processed list, at most L ids: list_cap = cap = L) and the staging of the queries
+        const QuantStore mode = (QuantStore)store;
+        pd.dtype = idx->dtype;
+        set_store_params(idx, mode, pd);
+        const size_t lut_bytes = mode == STORE_PQ && !pd.direct_cosine ? (size_t)warps * idx->pq_chunks * idx->pq_centers * 4 : 16;
+        if ((rc = luts->reserve(lut_bytes))) return rc;
+        pd.luts = (float*)luts->p;
+        if (rerank) {
+            if ((rc = lists->reserve(((size_t)nq * cap + nq) * 4))) return rc;
+            pd.list_ids = (uint32_t*)lists->p;
+            pd.list_counts = pd.list_ids + (size_t)nq * cap;
+            pd.list_cap = cap;
+        }
+        if ((rc = stage->reserve(mode == STORE_SQ ? sq_stage_bytes(idx, nq) : mode == STORE_MINMAX ? minmax_stage_bytes(idx, nq) : 0))) return rc;
+    }
     pool = diverse_pool_first(idx, l_search);
     return reserve_pools();
 }
@@ -374,8 +394,8 @@ int SlotJob::plan_diverse() {
 int SlotJob::reserve_pools() {
     int rc;
     const uint64_t pass_warps = (uint64_t)balanced_grid(n_work, dplan.grid, kDivWarps) * kDivWarps;
-    if ((rc = luts->reserve((size_t)pass_warps * pool * 16))) return rc;
-    pd.pools = (uint32_t*)luts->p;
+    if ((rc = pools->reserve((size_t)pass_warps * pool * 16))) return rc;
+    pd.pools = (uint32_t*)pools->p;
     pd.pool_cap = (uint32_t)pool;
     return DAB_OK;
 }
@@ -388,9 +408,11 @@ int SlotJob::reserve_tables() {
 
 // SQ and MinMax: the batch's queries compressed by the store's quantizer (MinMax: the NaN flag read back into h_counters)
 int SlotJob::stage_queries() {
-    if (store == STORE_SQ) return sq_stage_queries(idx, stream, *stage, d_queries, nq, &pq.query_codes, &pq.query_meta);
+    const uint8_t** codes = diverse_k ? &pd.query_codes : &pq.query_codes;
+    const float4** meta = diverse_k ? &pd.query_meta : &pq.query_meta;
+    if (store == STORE_SQ) return sq_stage_queries(idx, stream, *stage, d_queries, nq, codes, meta);
     if (store == STORE_MINMAX)
-        return minmax_stage_queries(idx, stream, *stage, d_queries, nq, (unsigned long long*)(h_counters + 4), &pq.query_codes, &pq.query_meta);
+        return minmax_stage_queries(idx, stream, *stage, d_queries, nq, (unsigned long long*)(h_counters + 4), codes, meta);
     return DAB_OK;
 }
 
@@ -434,7 +456,11 @@ int SlotJob::launch_diverse() {
 
 // the post-processing of the whole batch: the rerank, or the filter of deleted ids
 int SlotJob::post() {
-    if (rerank) return launch_rerank(idx, stream, d_queries, nq, k, cap, pq.list_ids, pq.list_counts, out.ids, out.dists, out.counts, deleted);
+    if (rerank) {
+        const uint32_t* list_ids = diverse_k ? pd.list_ids : pq.list_ids;
+        const uint32_t* list_counts = diverse_k ? pd.list_counts : pq.list_counts;
+        return launch_rerank(idx, stream, d_queries, nq, k, cap, list_ids, list_counts, out.ids, out.dists, out.counts, deleted);
+    }
     if (filter) return queue_drop_deleted(idx, stream, deleted, out.ids, out.dists, cap, nq, k, filtered, idx->n_points);
     return DAB_OK;
 }
@@ -493,15 +519,23 @@ int SlotJob::finish() {
 
 // The checks of a diverse search (DiverseSearchParams::new, diverse_search.rs:80-97; Diverse::new, :119-134), all made
 // before any device work.  diverse_k > k is accepted: the reference declares DiverseKGreaterThanTotalK and never returns it.
-static int check_diverse_args(const dab_index* idx, const char* api, uint32_t k, uint32_t l_search, uint32_t beam, uint32_t diverse_k) {
+// Over a quantized store (`store` >= 0) the store checks of the synchronous quantized call follow, reported under `api`.
+static int check_diverse_args(const dab_index* idx, const char* api, uint32_t k, uint32_t l_search, uint32_t beam, uint32_t diverse_k,
+                              int store = -1, bool rerank = false) {
     if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", api);
     int rc;
-    if ((rc = check_search_args(idx, k, l_search, beam))) return rc;
+    if ((rc = check_search_args(idx, k, l_search, beam, store < 0))) return rc;
     if (diverse_k == 0) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: diverse k_value cannot be zero", api);
     if (l_search < k) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: l_value (%u) must be greater than or equal to total_k_value (%u)", api, l_search, k);
     if (l_search > kDiverseMaxL) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: l_value %u > %u", api, l_search, kDiverseMaxL);
-    if ((rc = diverse_check_smem(idx, api, l_search, beam))) return rc;
+    if ((rc = diverse_check_smem(idx, api, l_search, beam, store))) return rc;
     if (!idx->d_attr_values) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: no attribute table (dab_upload_attributes has not been called)", api);
+    if (store < 0) return DAB_OK;
+    if ((rc = check_quant_store(idx, (QuantStore)store, api, false))) return rc;
+    if (rerank) {
+        if (!idx->vectors_ready) return fail(DAB_ERR_NOT_READY, "%s: rerank needs the full-precision vectors", api);
+        if ((rc = check_rerank(idx, l_search))) return rc;
+    }
     return DAB_OK;
 }
 
@@ -513,6 +547,7 @@ static int run_job(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t 
     if (nq == 0) return DAB_OK;
     SlotJob job(idx, idx->stream, idx->s_tables, idx->s_counters, idx->s_stage, idx->s_out2, idx->s_ids, idx->h_counters);
     job.diverse_k = diverse_k;
+    job.pools = &idx->s_pools;
     if ((rc = job.prepare(d_queries, nq, k, l_search, beam, d, store, rerank, rec)) || (rc = job.stage_queries())) return rc;
     if (store == STORE_MINMAX) {  // a batch with a NaN query fails before any traversal is launched
         DAB_CUDA(cudaStreamSynchronize(idx->stream));
@@ -586,6 +621,18 @@ static int search_device(dab_index* idx, const char* api, const void* d_queries,
     if (nq && (!d_queries || !d.ids || !d.dists)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
     DAB_CUDA(cudaSetDevice(idx->device));
     return run_job(idx, d_queries, nq, k, l_search, beam, d, store, rerank, nullptr, diverse_k);
+}
+
+// The diverse search over a quantized store: every argument and store check before the queries are copied; the device
+// form waits for the rerank or the filter of deleted ids, so that it returns with its outputs complete
+static int search_diverse_quant(dab_index* idx, const char* api, bool host, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                                uint32_t beam, uint32_t diverse_k, int rerank, const SearchOut& out, QuantStore store) {
+    int rc;
+    if ((rc = check_diverse_args(idx, api, k, l_search, beam, diverse_k, store, rerank != 0))) return rc;
+    if (host) return search_host(idx, api, queries, nq, k, l_search, beam, out, store, rerank != 0, diverse_k);
+    if ((rc = search_device(idx, api, queries, nq, k, l_search, beam, out, store, rerank != 0, diverse_k))) return rc;
+    DAB_CUDA(cudaStreamSynchronize(idx->stream));
+    return DAB_OK;
 }
 
 // ---- batches in flight (dab_search_batch*_async / dab_wait) --------------------------------------------------------
@@ -752,6 +799,48 @@ int dab_search_batch_diverse_device(dab_index* idx, const void* d_queries, uint3
     if ((rc = check_diverse_args(idx, "dab_search_batch_diverse_device", k, l_search, beam_width, diverse_k))) return rc;
     return search_device(idx, "dab_search_batch_diverse_device", d_queries, nq, k, l_search, beam_width,
                          SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, -1, false, diverse_k);
+}
+
+int dab_search_batch_diverse_pq(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
+                                uint32_t diverse_k, int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps,
+                                uint32_t* out_hops) {
+    return search_diverse_quant(idx, "dab_search_batch_diverse_pq", true, queries, nq, k, l_search, beam_width, diverse_k, rerank,
+                                SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, STORE_PQ);
+}
+
+int dab_search_batch_diverse_pq_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                                       uint32_t beam_width, uint32_t diverse_k, int rerank, uint32_t* d_out_ids, float* d_out_dists,
+                                       uint32_t* d_out_counts, uint32_t* d_out_cmps, uint32_t* d_out_hops) {
+    return search_diverse_quant(idx, "dab_search_batch_diverse_pq_device", false, d_queries, nq, k, l_search, beam_width, diverse_k, rerank,
+                                SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, STORE_PQ);
+}
+
+int dab_search_batch_diverse_sq(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
+                                uint32_t diverse_k, int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps,
+                                uint32_t* out_hops) {
+    return search_diverse_quant(idx, "dab_search_batch_diverse_sq", true, queries, nq, k, l_search, beam_width, diverse_k, rerank,
+                                SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, STORE_SQ);
+}
+
+int dab_search_batch_diverse_sq_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                                       uint32_t beam_width, uint32_t diverse_k, int rerank, uint32_t* d_out_ids, float* d_out_dists,
+                                       uint32_t* d_out_counts, uint32_t* d_out_cmps, uint32_t* d_out_hops) {
+    return search_diverse_quant(idx, "dab_search_batch_diverse_sq_device", false, d_queries, nq, k, l_search, beam_width, diverse_k, rerank,
+                                SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, STORE_SQ);
+}
+
+int dab_search_batch_diverse_minmax(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
+                                    uint32_t diverse_k, int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
+                                    uint32_t* out_cmps, uint32_t* out_hops) {
+    return search_diverse_quant(idx, "dab_search_batch_diverse_minmax", true, queries, nq, k, l_search, beam_width, diverse_k, rerank,
+                                SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, STORE_MINMAX);
+}
+
+int dab_search_batch_diverse_minmax_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                                           uint32_t beam_width, uint32_t diverse_k, int rerank, uint32_t* d_out_ids, float* d_out_dists,
+                                           uint32_t* d_out_counts, uint32_t* d_out_cmps, uint32_t* d_out_hops) {
+    return search_diverse_quant(idx, "dab_search_batch_diverse_minmax_device", false, d_queries, nq, k, l_search, beam_width, diverse_k,
+                                rerank, SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, STORE_MINMAX);
 }
 
 // ---- asynchronous batches: launch on a slot, collect with dab_wait ---------------------------

@@ -455,6 +455,52 @@ class GpuIndex:
                                                          C.c_void_p(d_ids), C.c_void_p(d_dists), C.c_void_p(d_counts or None),
                                                          C.c_void_p(d_cmps or None), C.c_void_p(d_hops or None)))
 
+    def _diverse_quant(self, store, queries, k, l_search, diverse_k, beam_width, rerank):
+        queries = self._queries(queries)
+        nq = queries.shape[0]
+        ids = np.empty((nq, k), np.uint32)
+        dists = np.empty((nq, k), np.float32)
+        counts, cmps, hops = (np.empty(nq, np.uint32) for _ in range(3))
+        fn = getattr(_lib.lib(), f"dab_search_batch_diverse_{store}")
+        check(fn(self._h, _ptr(queries), nq, k, l_search, beam_width, diverse_k, int(bool(rerank)), _ptr(ids), _ptr(dists), _ptr(counts),
+                 _ptr(cmps), _ptr(hops)))
+        return ids, dists, counts, cmps, hops
+
+    def _diverse_quant_device(self, store, d_queries, nq, k, l_search, diverse_k, beam_width, rerank, d_ids, d_dists, d_counts, d_cmps,
+                              d_hops):
+        fn = getattr(_lib.lib(), f"dab_search_batch_diverse_{store}_device")
+        check(fn(self._h, C.c_void_p(d_queries), nq, k, l_search, beam_width, diverse_k, int(bool(rerank)), C.c_void_p(d_ids),
+                 C.c_void_p(d_dists), C.c_void_p(d_counts or None), C.c_void_p(d_cmps or None), C.c_void_p(d_hops or None)))
+
+    def search_batch_diverse_pq(self, queries, k, l_search, diverse_k, beam_width=1, rerank=False):
+        """search_batch_diverse with the traversal distances of search_batch_pq (PQ store); rerank=True reranks the
+        post-processed list by full-precision distance."""
+        return self._diverse_quant("pq", queries, k, l_search, diverse_k, beam_width, rerank)
+
+    def search_batch_diverse_sq(self, queries, k, l_search, diverse_k, beam_width=1, rerank=False):
+        """search_batch_diverse with the traversal distances of search_batch_sq (scalar-quantized store)."""
+        return self._diverse_quant("sq", queries, k, l_search, diverse_k, beam_width, rerank)
+
+    def search_batch_diverse_minmax(self, queries, k, l_search, diverse_k, beam_width=1, rerank=False):
+        """search_batch_diverse with the traversal distances of search_batch_minmax (MinMax store)."""
+        return self._diverse_quant("minmax", queries, k, l_search, diverse_k, beam_width, rerank)
+
+    def search_batch_diverse_pq_device(self, d_queries, nq, k, l_search, diverse_k, beam_width, d_ids, d_dists, d_counts=0, d_cmps=0,
+                                       d_hops=0, rerank=False):
+        """search_batch_diverse_pq with device pointers (integers); results stay in HBM, complete on return."""
+        self._diverse_quant_device("pq", d_queries, nq, k, l_search, diverse_k, beam_width, rerank, d_ids, d_dists, d_counts, d_cmps, d_hops)
+
+    def search_batch_diverse_sq_device(self, d_queries, nq, k, l_search, diverse_k, beam_width, d_ids, d_dists, d_counts=0, d_cmps=0,
+                                       d_hops=0, rerank=False):
+        """search_batch_diverse_sq with device pointers (integers); results stay in HBM, complete on return."""
+        self._diverse_quant_device("sq", d_queries, nq, k, l_search, diverse_k, beam_width, rerank, d_ids, d_dists, d_counts, d_cmps, d_hops)
+
+    def search_batch_diverse_minmax_device(self, d_queries, nq, k, l_search, diverse_k, beam_width, d_ids, d_dists, d_counts=0, d_cmps=0,
+                                           d_hops=0, rerank=False):
+        """search_batch_diverse_minmax with device pointers (integers); results stay in HBM, complete on return."""
+        self._diverse_quant_device("minmax", d_queries, nq, k, l_search, diverse_k, beam_width, rerank, d_ids, d_dists, d_counts, d_cmps,
+                                   d_hops)
+
     def search_batch_async(self, slot, queries, k, l_search, beam_width=1, out=None):
         """Queue a batch on `slot` (host buffers) and return its output arrays without waiting; they are
         valid after wait(slot).  `queries` is used as passed (it must stay alive and unchanged until then);

@@ -210,6 +210,36 @@ impl<T: Element> GpuIndex<T> {
         Ok(b)
     }
 
+    /// `search_batch_diverse` with the traversal distances of `search_batch_pq` (the PQ store); `rerank`: the
+    /// full-precision `Rerank` of the post-processed list.
+    pub fn search_batch_diverse_pq(&self, queries: &[T], k: usize, l_search: u32, diverse_k: u32, beam_width: u32, rerank: bool) -> Result<Batch> {
+        self.diverse_quantized(sys::dab_search_batch_diverse_pq, queries, k, l_search, diverse_k, beam_width, rerank)
+    }
+
+    /// `search_batch_diverse` with the traversal distances of `search_batch_sq` (the scalar-quantized store).
+    pub fn search_batch_diverse_sq(&self, queries: &[T], k: usize, l_search: u32, diverse_k: u32, beam_width: u32, rerank: bool) -> Result<Batch> {
+        self.diverse_quantized(sys::dab_search_batch_diverse_sq, queries, k, l_search, diverse_k, beam_width, rerank)
+    }
+
+    /// `search_batch_diverse` with the traversal distances of `search_batch_minmax` (the MinMax store).
+    pub fn search_batch_diverse_minmax(&self, queries: &[T], k: usize, l_search: u32, diverse_k: u32, beam_width: u32, rerank: bool)
+        -> Result<Batch> {
+        self.diverse_quantized(sys::dab_search_batch_diverse_minmax, queries, k, l_search, diverse_k, beam_width, rerank)
+    }
+
+    #[allow(clippy::too_many_arguments)]
+    fn diverse_quantized(&self, f: DiverseQuantized, queries: &[T], k: usize, l_search: u32, diverse_k: u32, beam_width: u32, rerank: bool)
+        -> Result<Batch> {
+        assert_eq!(queries.len() % self.dim, 0);
+        let nq = queries.len() / self.dim;
+        let mut b = Batch { k, ids: vec![0; nq * k], dists: vec![0.0; nq * k], counts: vec![0; nq], cmps: vec![0; nq], hops: vec![0; nq] };
+        check(unsafe {
+            f(self.raw, queries.as_ptr() as *const c_void, nq as u32, k as u32, l_search, beam_width, diverse_k, rerank as i32,
+              b.ids.as_mut_ptr(), b.dists.as_mut_ptr(), b.counts.as_mut_ptr(), b.cmps.as_mut_ptr(), b.hops.as_mut_ptr())
+        })?;
+        Ok(b)
+    }
+
     /// Queue a batch on `slot` without waiting (`search_all`'s one task per partition, api.rs:410-419, mapped to
     /// device slots).  The returned guard borrows the queries and owns the result buffers; `InFlight::wait` joins it.
     pub fn search_batch_async<'a>(&'a self, slot: u32, queries: &'a [T], k: usize, l_search: u32, beam_width: u32) -> Result<InFlight<'a, T>> {
@@ -371,6 +401,8 @@ type QuantizedAsync = unsafe extern "C" fn(*mut sys::dab_index, u32, *const c_vo
                                            *mut f32, *mut u32, *mut u32, *mut u32) -> std::os::raw::c_int;
 
 /// The entry points that open a paged search over a quantized store (one signature for PQ, SQ and MinMax).
+type DiverseQuantized = unsafe extern "C" fn(*mut sys::dab_index, *const c_void, u32, u32, u32, u32, u32, std::os::raw::c_int,
+                                             *mut u32, *mut f32, *mut u32, *mut u32, *mut u32) -> std::os::raw::c_int;
 type PagedBegin = unsafe extern "C" fn(*mut sys::dab_index, *const c_void, u32, u32, *mut *mut sys::dab_paged) -> std::os::raw::c_int;
 
 /// A batch in flight on one slot of the device.  Dropping it joins the slot (the library writes into the

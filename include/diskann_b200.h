@@ -205,6 +205,52 @@ int dab_search_batch_diverse_device(dab_index* idx, const void* d_queries, uint3
                                     uint32_t* d_out_counts, uint32_t* d_out_cmps,
                                     uint32_t* d_out_hops);
 
+/* Diverse::search over a quantized store (diverse_search.rs:189-234 with the quantized strategy):
+ * the traversal distances are those of dab_search_batch_pq / _sq / _minmax on the same store (PQ:
+ * TableL2 / TableIP, DirectCosine for Metric::Cosine; SQ and MinMax: the queries compressed by the
+ * store's quantizer), the list and the local queues run as in dab_search_batch_diverse, and
+ * best.post_process() keeps at most diverse_k entries per attribute value.
+ *   rerank == 0: the default post-processing of the first L entries (start points and deleted ids
+ *     dropped, the first k kept) with their quantized distances;
+ *   rerank != 0: Pipeline<FilterStartPoints, Rerank> over the post-processed list (providers
+ *     inmem/product.rs:391-400, full_precision.rs:356-399): each remaining entry that is not
+ *     deleted gets its full-precision distance, the list is sorted by it (ties keep list order)
+ *     and the first k are kept.  The diverse limit holds: the rerank reorders a subset of the list.
+ * cmps / hops follow SearchStats as in dab_search_batch_diverse.  Checked before any device work:
+ * the arguments of dab_search_batch_diverse (the shared memory with the query area the f32 query
+ * for PQ, the store's code row + 16 bytes for SQ and MinMax), then the store checks of the
+ * synchronous quantized call (store uploaded with rows, no Metric::Cosine on the SQ store, rerank
+ * only with the full-precision vectors uploaded); a MinMax query that holds a NaN after the
+ * transform fails the call.  Outputs as dab_search_batch; the _device forms return with the
+ * outputs complete. */
+int dab_search_batch_diverse_pq(dab_index* idx, const void* queries, uint32_t nq, uint32_t k,
+                                uint32_t l_search, uint32_t beam_width, uint32_t diverse_k,
+                                int rerank, uint32_t* out_ids, float* out_dists,
+                                uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops);
+int dab_search_batch_diverse_sq(dab_index* idx, const void* queries, uint32_t nq, uint32_t k,
+                                uint32_t l_search, uint32_t beam_width, uint32_t diverse_k,
+                                int rerank, uint32_t* out_ids, float* out_dists,
+                                uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops);
+int dab_search_batch_diverse_minmax(dab_index* idx, const void* queries, uint32_t nq, uint32_t k,
+                                    uint32_t l_search, uint32_t beam_width, uint32_t diverse_k,
+                                    int rerank, uint32_t* out_ids, float* out_dists,
+                                    uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops);
+int dab_search_batch_diverse_pq_device(dab_index* idx, const void* d_queries, uint32_t nq,
+                                       uint32_t k, uint32_t l_search, uint32_t beam_width,
+                                       uint32_t diverse_k, int rerank, uint32_t* d_out_ids,
+                                       float* d_out_dists, uint32_t* d_out_counts,
+                                       uint32_t* d_out_cmps, uint32_t* d_out_hops);
+int dab_search_batch_diverse_sq_device(dab_index* idx, const void* d_queries, uint32_t nq,
+                                       uint32_t k, uint32_t l_search, uint32_t beam_width,
+                                       uint32_t diverse_k, int rerank, uint32_t* d_out_ids,
+                                       float* d_out_dists, uint32_t* d_out_counts,
+                                       uint32_t* d_out_cmps, uint32_t* d_out_hops);
+int dab_search_batch_diverse_minmax_device(dab_index* idx, const void* d_queries, uint32_t nq,
+                                           uint32_t k, uint32_t l_search, uint32_t beam_width,
+                                           uint32_t diverse_k, int rerank, uint32_t* d_out_ids,
+                                           float* d_out_dists, uint32_t* d_out_counts,
+                                           uint32_t* d_out_cmps, uint32_t* d_out_hops);
+
 /* ------------------------------------------------------------------ (3'') paged search */
 
 /* DiskANNIndex::paged_search (diskann/src/graph/index.rs:2075-2155) and PagedSearch::next_page

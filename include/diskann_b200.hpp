@@ -273,8 +273,35 @@ class GpuDiverse {
         for (uint32_t i = 0; i < nq; ++i) r.stats[i] = SearchStats{cmps[i], hops[i], counts[i]};
         return r;
     }
+    // The same over the quantized stores (the store must be resident): the traversal distances of
+    // dab_search_batch_pq / _sq / _minmax; `rerank`: Pipeline<FilterStartPoints, Rerank> over the post-processed list
+    KnnResults search_pq(const T* queries, uint32_t nq, uint32_t k, bool rerank) {
+        return search_quantized(dab_search_batch_diverse_pq, queries, nq, k, rerank);
+    }
+    KnnResults search_sq(const T* queries, uint32_t nq, uint32_t k, bool rerank) {
+        return search_quantized(dab_search_batch_diverse_sq, queries, nq, k, rerank);
+    }
+    KnnResults search_minmax(const T* queries, uint32_t nq, uint32_t k, bool rerank) {
+        return search_quantized(dab_search_batch_diverse_minmax, queries, nq, k, rerank);
+    }
 
    private:
+    using Quantized = int (*)(dab_index*, const void*, uint32_t, uint32_t, uint32_t, uint32_t, uint32_t, int, uint32_t*, float*, uint32_t*,
+                              uint32_t*, uint32_t*);
+    KnnResults search_quantized(Quantized fn, const T* queries, uint32_t nq, uint32_t k, bool rerank) {
+        KnnResults r;
+        r.nq = nq;
+        r.k = k;
+        r.ids.resize((size_t)nq * k);
+        r.distances.resize((size_t)nq * k);
+        std::vector<uint32_t> counts(nq), cmps(nq), hops(nq);
+        check(fn(p_.raw(), queries, nq, k, l_, beam_, diverse_k_, rerank ? 1 : 0, r.ids.data(), r.distances.data(), counts.data(), cmps.data(),
+                 hops.data()));
+        r.stats.resize(nq);
+        for (uint32_t i = 0; i < nq; ++i) r.stats[i] = SearchStats{cmps[i], hops[i], counts[i]};
+        return r;
+    }
+
     Provider<T>& p_;
     uint32_t l_, diverse_k_, beam_;
 };

@@ -11,9 +11,17 @@ share of its ground truth (10, or fewer when the cardinality allows fewer) the s
 checked on every result row: the largest number of results that share an attribute value, and the queries where it
 exceeds diverse_k (the reference's tie drift may allow that; it is reported as measured).  Those queries are searched
 again by the CPU oracle (orc_search_batch_diverse over the downloaded graph): whether it returns the same ids, distance
-bits, counts, cmps and hops, and how many of its queue removals failed on an exact distance tie.  The card's name and
-power limit are read in the same run.
-usage: python tools/bench_diverse.py [--n N] [--nq NQ] [--reps R] [--json PATH]"""
+bits, counts, cmps and hops, and how many of its queue removals failed on an exact distance tie; over the PQ and MinMax
+stores the first 16 of them, by orc_search_batch_diverse_table fed the store's distances to every id (the SQ store is not
+checked: its restatement holds every row's codes unpacked, too large at C2).  The k-NN batch's recall@10 against the
+nearest 10 is reported with it.  The card's name and power limit are read in the same run.
+--store picks the traversal store (default fp, full precision): sq (SQ-8), minmax (MinMax-8 behind DoubleHadamard) or
+pq (PQ-32 trained on 100K rows with dab_pq_train), as tools/bench_paged.py sets them up; the calls are then
+dab_search_batch_diverse_{sq,minmax,pq}_device and dab_search_batch_{sq,minmax,pq}_device, with --rerank the
+full-precision rerank of both.  Each diverse row also reports its re-run passes: the kernel launches of one call beyond
+those of a call that re-runs nothing (the fewest launches of four one-query calls), and an upper bound on the queries
+whose visited table can have overflowed (final visited set = cmps, plus max_degree, past 7/8 of the first pass's table).
+usage: python tools/bench_diverse.py [--n N] [--nq NQ] [--reps R] [--store {fp,pq,sq,minmax}] [--rerank] [--json PATH]"""
 import argparse
 import json
 import os
@@ -27,13 +35,16 @@ import numpy as np
 import torch
 
 import bench
+import diskann_b200 as dab
 from bench_minmax_search import build_index, card
 
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import diverse_oracle  # noqa: E402  the CPU checker of the queries over diverse_k
+import diverse_table_oracle  # noqa: E402  ... and over a quantized store's distances
 import oracle_lib  # noqa: E402
 
 K, L, TOP = 10, 100, 4096
+OVER_SAMPLE = 16  # quantized stores: the queries over diverse_k the oracle checks
 
 
 def nearest(base_t, queries, top):
@@ -69,6 +80,8 @@ def main():
     ap.add_argument("--n", type=int, default=0)
     ap.add_argument("--nq", type=int, default=0)
     ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--store", choices=["fp", "pq", "sq", "minmax"], default="fp")
+    ap.add_argument("--rerank", action="store_true")
     ap.add_argument("--json", default="")
     args = ap.parse_args()
     name, power = card()
@@ -84,6 +97,58 @@ def main():
     outs = (torch.empty((nq, K), dtype=torch.int32, device="cuda"), torch.empty((nq, K), dtype=torch.float32, device="cuda"),
             *(torch.empty(nq, dtype=torch.int32, device="cuda") for _ in range(3)))
     ptrs = [o.data_ptr() for o in outs]
+    dim = cfg["dim"]
+    if args.store == "sq":
+        mean, std = base.mean(0).astype(np.float32), float(base.std())
+        shift = (mean - np.float32(2.5 * std)).astype(np.float32)
+        g.upload_sq(8, shift, float(np.float32(5.0 * std)), float(np.dot(shift, shift)), 0.0)
+        g.sq_encode_all()
+    elif args.store == "minmax":
+        g.upload_minmax(8, 1.0, dab.Transform.double_hadamard(dim, "same", seed=7))
+        g.minmax_encode_all()
+    elif args.store == "pq":
+        sample = np.sort(np.random.default_rng(bench.SEED_PQ).choice(n, size=min(100_000, n), replace=False))
+        g.pq_train(base[sample].astype(np.float32), 32, 256, 5, bench.SEED_PQ)
+        g.pq_encode_all()
+    rr = dict(rerank=args.rerank)
+
+    stores = {}
+
+    def store_distances(q):
+        """the store's traversal distance of query q to every id (the quantizer restated on the CPU, as the tests do)"""
+        from test_paged_search_quantized import PQStore
+        if args.store == "minmax":
+            from test_minmax_search import compress
+            if "rows" not in stores:
+                stores["rows"] = g.download_minmax()
+            rows = stores["rows"]
+            qr = compress(q[None], dab.Transform.double_hadamard(dim, "same", seed=7), 8)[0]
+            return oracle_lib.minmax_distances(oracle_lib.L2, 8, 8, np.broadcast_to(qr, rows.shape), rows)
+        if "st" not in stores:
+            stores["st"] = PQStore(*g.download_pq(), oracle_lib.L2)
+        return stores["st"].distances(q)
+
+    def knn_call():
+        if args.store == "fp":
+            g.search_batch_device(d_q.data_ptr(), nq, K, L, 1, *ptrs)
+        else:
+            getattr(g, f"search_batch_{args.store}_device")(d_q.data_ptr(), nq, K, L, 1, *ptrs, **rr)
+
+    def diverse_call(dk, q_ptr=None, m=None):
+        q_ptr, m = q_ptr or d_q.data_ptr(), m or nq
+        if args.store == "fp":
+            g.search_batch_diverse_device(q_ptr, m, K, L, dk, 1, *ptrs)
+        else:
+            getattr(g, f"search_batch_diverse_{args.store}_device")(q_ptr, m, K, L, dk, 1, *ptrs, **rr)
+
+    def launches(call):
+        before = dab.launch_count()
+        call()
+        stream.synchronize()
+        return dab.launch_count() - before
+
+    # the first pass's visited table (table_slots without a hint: 1.1 * max_degree * 1.3 * L) and its 7/8 limit
+    hlimit = (max(256, int(1.1 * g.max_degree * 1.3 * L) + 1) + 7) // 8 * 7
 
     def timed(call):
         call()
@@ -101,7 +166,9 @@ def main():
         return dict(ms_per_batch=round(t, 3), qps=round(nq / t * 1e3, 1), mean_cmps=round(float(res[3].mean()), 1),
                     mean_hops=round(float(res[4].mean()), 1)), res
 
-    knn, _ = timed(lambda: g.search_batch_device(d_q.data_ptr(), nq, K, L, 1, *ptrs))
+    knn, kres = timed(knn_call)
+    kids = kres[0].view(np.uint32)
+    knn["recall_at_10"] = round(float(np.mean([len(np.intersect1d(order[qi, :K], kids[qi, :kres[2][qi]])) / K for qi in range(nq)])), 4)
     rows = []
     oracle = None
     rng = np.random.default_rng(0xD1CE)
@@ -109,7 +176,10 @@ def main():
         attrs = rng.integers(0, card_n, n + 1).astype(np.uint32)
         g.upload_attributes(attrs)
         for dk in (1, 3):
-            r, res = timed(lambda: g.search_batch_diverse_device(d_q.data_ptr(), nq, K, L, dk, 1, *ptrs))
+            r, res = timed(lambda: diverse_call(dk))
+            base_launches = min(launches(lambda: diverse_call(dk, d_q[i:i + 1].data_ptr(), 1)) for i in range(4))
+            r.update(rerun_passes=launches(lambda: diverse_call(dk)) - base_launches,
+                     queries_near_visited_limit=int((res[3].astype(np.int64) + g.max_degree > hlimit).sum()))
             ids, counts = res[0].view(np.uint32), res[2]
             want = min(K, card_n * dk)
             truth = diverse_truth(order, attrs, dk, want)
@@ -126,18 +196,25 @@ def main():
                      truth_size=want, truth_full_sorts=full_sorts, mean_count=round(float(counts.mean()), 2),
                      max_results_per_value=max(worst), queries_over_diverse_k=int(sum(w > dk for w in worst)))
             over = np.array([qi for qi in range(nq) if worst[qi] > dk], np.int64)
-            if over.size:
+            if over.size and args.store != "sq":
                 if oracle is None:
                     vecs = np.concatenate([base, bench.find_medoid(base)[None, :]])
                     oracle = oracle_lib.Index(vecs, g.download_graph(), n, 1, oracle_lib.L2)
-                want_o = diverse_oracle.search_batch(oracle, queries[over], K, L, dk, attrs)
+                if args.store == "fp":
+                    want_o = diverse_oracle.search_batch(oracle, queries[over], K, L, dk, attrs)
+                else:
+                    over = over[:OVER_SAMPLE]  # the store's distances to every id, one query at a time
+                    tables = np.stack([store_distances(q) for q in queries[over]])
+                    want_o = diverse_table_oracle.search_batch_table(oracle, tables, queries[over], K, L, dk, attrs, rerank=args.rerank)
+                    r.update(over_diverse_k_checked=int(over.size))
                 same = all(np.array_equal(np.asarray(a)[over].view(np.uint32), np.asarray(b).view(np.uint32))
                            for a, b in zip(res, want_o[:5]))
                 r.update(over_diverse_k_equal_to_oracle=bool(same), over_diverse_k_failed_removals=int(want_o[5].sum()))
             print(json.dumps(r), flush=True)
             rows.append(r)
     summary = dict(gpu=name, power_limit_max_sm_clock=power, workload="c2_1Mx128_f32_l2", n=n, nq=nq, L=L, k=K, reps=args.reps,
-                   search_batch=knn, diverse=rows)
+                   store={"fp": "full_precision", "pq": "pq32_dab_pq_train", "sq": "sq8", "minmax": "minmax8_doublehadamard"}[args.store],
+                   rerank=args.rerank, search_batch=knn, diverse=rows)
     print(json.dumps(summary), flush=True)
     if args.json:
         os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)

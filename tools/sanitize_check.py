@@ -77,6 +77,18 @@ for dt, ddt, metric, d in ((np.float32, dab.DType.f32, dab.Metric.L2, 100), (np.
             g.pq_encode_all()
             pq = g.search_batch_pq(base[:32], 5, 40, 1, rerank=True)  # PQ traversal + rerank kernel
             g.pq_self_distances(ids[4, :20], ids[5, :20])
+            for rr in (False, True):                                 # diverse_kernel_quant<0>, then rerank
+                g.search_batch_diverse_pq(base[:32], 5, 40, 2, 1, rerank=rr)
+        f32 = base.astype(np.float32)
+        std = float(f32.std())
+        shift = (f32.mean(0) - np.float32(2.5 * std)).astype(np.float32)
+        g.upload_sq(8, shift, 5.0 * std, -float((shift * shift).sum()))
+        g.sq_encode_all()
+        g.upload_minmax(4, 1.0, None)
+        g.minmax_encode_all()
+        for rr in (False, True):                                     # diverse_kernel_quant<1> and <2>
+            g.search_batch_diverse_sq(base[:32], 5, 40, 2, 2, rerank=rr)
+            g.search_batch_diverse_minmax(base[:32], 5, 40, 2, 1, rerank=rr)
         print(dt.__name__, "deg max", int(adj[:, 0].max()), "search ok", int(got[2].min()), int(got4[2].min()), int(div[2].min()), int(div4[2].min()),
               "finite", bool(np.isfinite(out[1:]).all() and np.isfinite(pairs).all() and np.isfinite(block).all()), knn[0].shape)
 print("sanitize_check done")
