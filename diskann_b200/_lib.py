@@ -51,6 +51,12 @@ SYMBOLS = {
     "dab_search_batch_async": (_i, [_vp, _u32, _vp, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
     "dab_search_batch_device_async": (_i, [_vp, _u32, _vp, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
     "dab_wait": (_i, [_vp, _u32]),
+    "dab_range_search": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, C.POINTER(_vp)]),
+    "dab_range_search_device": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, C.POINTER(_vp)]),
+    "dab_range_offsets": (_i, [_vp, _vp, _vp, _vp, _vp]),
+    "dab_range_results": (_i, [_vp, _vp, _vp]),
+    "dab_range_results_device": (_i, [_vp, _vp, _vp]),
+    "dab_range_free": (None, [_vp]),
     "dab_paged_search_begin": (_i, [_vp, _vp, _u32, _u32, C.POINTER(_vp)]),
     "dab_paged_search_begin_pq": (_i, [_vp, _vp, _u32, _u32, C.POINTER(_vp)]),
     "dab_paged_search_begin_sq": (_i, [_vp, _vp, _u32, _u32, C.POINTER(_vp)]),

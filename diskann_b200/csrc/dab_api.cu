@@ -71,6 +71,15 @@ void Tuning::load() {
     const char* dp = getenv("DAB_TEST_DIVERSE_POOL");
     const long pv = dp ? atol(dp) : 0;
     test_diverse_pool = pv >= 1 && pv <= (1 << 20) ? (uint32_t)pv : 0;
+    const char* rl = getenv("DAB_TEST_RANGE_LIST");
+    const long lv = rl ? atol(rl) : 0;
+    test_range_list = lv >= 1 && lv <= (1 << 20) ? (uint32_t)lv : 0;
+    const char* ra = getenv("DAB_TEST_RANGE_ARENA");
+    const long long av = ra ? atoll(ra) : 0;
+    test_range_arena = av >= 1 ? (uint64_t)av : 0;
+    const char* rm = getenv("DAB_TEST_RANGE_LIMIT");
+    const long long mv = rm ? atoll(rm) : 0;
+    test_range_limit = mv >= 1 ? (uint64_t)mv : 0;
 }
 
 }  // namespace dab
@@ -140,6 +149,7 @@ void dab_destroy(dab_index* idx) {
     if (idx->own_stream) cudaStreamSynchronize(idx->own_stream);
     search_slots_release(idx);
     paged_release(idx);
+    range_release(idx);
     comm_release(idx);
     tc_release(idx);
     minmax_release(idx);

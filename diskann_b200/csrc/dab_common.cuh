@@ -36,6 +36,7 @@ int retire_quantized_stores(struct ::dab_index* idx);
 void minmax_release(struct ::dab_index* idx);        // minmax_index.cu: the store's transform
 void paged_release(struct ::dab_index* idx);         // search_paged.cu: every paged search session still open
 void attributes_release(struct ::dab_index* idx);    // search_diverse.cu: the attribute table
+void range_release(struct ::dab_index* idx);         // search_range.cu: every range search result set still open
 // delete_kernels.cu: the deletion table.  deleted_assign replaces it with `words` ((n_total + 31) / 32 of them, bit i of
 // word i / 32 for id i) holding n_deleted set bits; n_deleted == 0 clears it (words may then be NULL).
 int deleted_assign(struct ::dab_index* idx, const uint32_t* words, uint64_t n_deleted);
@@ -117,6 +118,9 @@ struct Tuning {
     int test_visited_log2 = 0;        // DAB_TEST_VISITED_LOG2: tests force the overflow / retry path
     bool test_pq_global_lut = false;  // DAB_TEST_PQ_GLOBAL_LUT: PQ kernels with the per-warp table in global memory also where the pivots fit shared memory
     uint32_t test_diverse_pool = 0;   // DAB_TEST_DIVERSE_POOL: local-queue entries of a diverse search's first pass (tests force its re-runs)
+    uint32_t test_range_list = 0;     // DAB_TEST_RANGE_LIST: in_range entries per warp in a range search's first pass (tests force its re-runs)
+    uint64_t test_range_arena = 0;    // DAB_TEST_RANGE_ARENA: entries of a range search's first result arena (tests force its extension)
+    uint64_t test_range_limit = 0;    // DAB_TEST_RANGE_LIMIT: most entries a range search may hold (tests reach its out-of-memory failure)
     void load();
 };
 
@@ -252,6 +256,7 @@ struct dab_index {
     // (upload, encode-all, PQ training, broadcast).  Only paged search sessions over that store read it.
     uint64_t store_writes[3] = {};
     void* paged = nullptr;  // the open paged search sessions (a list, search_paged.cu)
+    dab_range* ranges = nullptr;  // the open range search result sets (a list, search_range.cu)
     // the deletion table (delete_kernels.cu; providers TableDeleteProviderAsync): one bit per id, kept on the host and
     // copied to the device after every change.  Both are allocated by the first dab_delete; n_deleted counts set bits.
     uint32_t* h_deleted = nullptr;  // (n_total + 31) / 32 words

@@ -119,7 +119,8 @@ int queue_drop_deleted(const dab_index* idx, cudaStream_t stream, const uint32_t
 
 // Searches whose queries are rows of the index (the build's insert searches, in-place deletes): they ignore deletions
 // and teach the visited tables nothing.  With `ids` each records the nodes it expanded; with `keep_starts` its results
-// are the list's entries with start points kept (the caller filters them).
+// are the list's entries with start points kept (the caller filters them).  `keep_deleted`, for queries that are not
+// rows (the first phase of range search): the results keep deleted ids too, and the caller filters them.
 struct SearchRecord {
     const uint32_t* query_rows;  // [nq] row ids of the queries
     uint32_t* ids;               // [nq][cap] expanded nodes, [nq] counts (NULL: no record)
@@ -127,6 +128,7 @@ struct SearchRecord {
     uint32_t* counts;
     uint32_t cap;
     bool keep_starts;
+    bool keep_deleted;
 };
 
 // One batch on the handle's stream and scratch, device pointers only.  `store`: -1 full precision, else the QuantStore the

@@ -3,7 +3,8 @@
 // are in search_kernel_pq.cu and search_kernel_pqs.cu), the slots of batches in flight and the C entry points
 // (dab_search_batch[_pq|_pq_rerank|_sq|_minmax][_device][_async], dab_search_batch_diverse[_pq|_sq|_minmax][_device],
 // dab_wait).  The diverse search (search_diverse.cu), over full-precision rows or a quantized store, is one more kind of
-// the job.
+// the job; so is the first phase of range search (search_range.cu), a full-precision batch that keeps start points and
+// deleted ids.
 //
 // A full-precision batch runs on search_kernel_v3 (visited set in shared memory) where its short lists make that the
 // faster kernel, and on search_kernel_v2 (global visited tables) otherwise; queries whose visited set outgrows its table
@@ -252,7 +253,7 @@ int SlotJob::prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint32_t
     d_overflow = d_counters + 4;
     out = d;
     // searches over rows of the index ignore deletions, as the reference's insert and in-place delete do
-    deleted = rec.query_rows ? nullptr : deleted_filter(idx);
+    deleted = rec.query_rows || rec.keep_deleted ? nullptr : deleted_filter(idx);
     filter = deleted && !rerank;
     if (filter) {
         if ((rc = lists->reserve((size_t)nq * cap * 8))) return rc;

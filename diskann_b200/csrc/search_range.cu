@@ -1,0 +1,649 @@
+// search_range.cu — batched range search on the device: Range::search and range_search_internal
+// (diskann/src/graph/search/range_search.rs:255-469) over full-precision rows, and the result sets it returns
+// (dab_range_search[_device], dab_range_offsets, dab_range_results[_device], dab_range_free).
+//
+// Phase 1 is the k-NN traversal at L (search_kernel_v3 / _v2 through run_search, unchanged): with k = L and start
+// points and deleted ids kept, it writes each query's first L list entries, its cmps and its hops.  Phase 2 is
+// range_kernel, one warp per query on global visited tables:
+//   in_range  the phase-1 entries with distance <= radius, in list order, in the warp's region of global memory;
+//   round 2   iff |in_range| >= (f32(L) * initial_slack) as usize and |in_range| < max_returned: the visited table is
+//             cleared and re-seeded with the in_range ids, and the frontier, the unconsumed suffix of in_range, is
+//             expanded beam_width ids at a time in expand_beam order; each new neighbour with d <= radius * range_slack
+//             is appended while |in_range| < max_returned (the cap may cut a hop short);
+//   output    in_range in insertion order without start points, deleted ids, ids with d <= inner_radius (when given)
+//             and ids with d > radius.
+// The hops of a query that took the second round are phase1 + (phase1 + phase2), as the reference adds its cumulative
+// scratch.hops to phase 1's; cmps are phase 1's.  A hop's nodes are expanded, scored and appended one node at a time:
+// the visited inserts and the appends come in the reference's order, and nothing after the cap is observable.
+//
+// No query is answered from truncated storage.  A query whose visited set outgrows its table, or whose in_range
+// outgrows its region, stops and is re-run: on tables from grow_visited_tables, or on regions four times larger (at
+// most min(max_returned, n_total) entries, which in_range, of distinct ids, cannot outgrow).  A completed query claims
+// space for its filtered results in the batch's arena; one that finds no room reports its count and is re-run once the
+// arena has been extended by exactly what those queries need.  A scan and a compaction then lay the results out in
+// query order in the result set, which owns its memory: later writes to the index do not change it.
+#include "dab_common.cuh"
+#include "search_common.cuh"
+#include "search_host.cuh"
+
+#include <algorithm>
+
+struct dab_range {
+    dab_index* idx = nullptr;
+    dab_range *prev = nullptr, *next = nullptr;  // the index's open result sets
+    uint32_t nq = 0;
+    uint64_t total = 0;
+    void* d_stats = nullptr;  // offsets [nq + 1] u64, cmps [nq], hops [nq] u32, second_round [nq] u8
+    void* d_results = nullptr;  // ids [total] u32, dists [total] f32
+    uint64_t* offsets() const { return (uint64_t*)d_stats; }
+    uint32_t* cmps() const { return (uint32_t*)(offsets() + nq + 1); }
+    uint32_t* hops() const { return cmps() + nq; }
+    uint8_t* second() const { return (uint8_t*)(hops() + nq); }
+};
+
+namespace dab {
+
+namespace {
+
+constexpr int kRangeWarps = 4;
+constexpr int kRangeRows = 4;                  // rows in flight per team in the distance loop
+constexpr size_t kRangeMaxSmem = 200 * 1024;   // a CTA's shared memory
+constexpr uint64_t kRegionBudget = 1ull << 31;  // bytes of in_range regions one pass may take
+
+struct RangeParams {
+    const uint32_t* adj;
+    uint32_t adj_stride;
+    uint64_t n_points;
+    uint32_t n_start;
+    uint32_t dim;
+    uint32_t max_degree;
+    const uint8_t* vectors;
+    size_t row_stride;
+    const void* queries;
+    const uint32_t* query_list;  // the queries of a re-run pass (NULL: 0 .. n_work-1)
+    uint32_t n_work;
+    uint32_t l_search, beam;
+    // phase 1: the first L list entries of every query [nq][L], their number and the hops [nq]
+    const uint32_t* list_ids;
+    const float* list_dists;
+    const uint32_t* list_counts;
+    const uint32_t* list_hops;
+    float radius, bound, inner_radius;  // bound: radius * range_slack
+    int has_inner;
+    uint64_t min_in_range;  // (f32(L) * initial_slack) as usize
+    uint64_t max_returned;  // UINT64_MAX: None
+    const uint32_t* deleted;  // NULL: nothing deleted
+    uint32_t* tables;
+    uint32_t n_buckets;
+    uint32_t* regions;  // region_cap ids then region_cap dists for every warp of the pass
+    uint32_t region_cap;
+    // counters[0] work cursor, [1] stopped queries (listed in overflow_list), [2] largest visited set, [3] the stopped
+    // queries whose region was full, [4] queries without room in the arena (listed in arena_fail)
+    uint32_t* counters;
+    uint32_t* overflow_list;
+    uint32_t* arena_fail;
+    // the arena: positions [arena_first, arena_end) are arena_ids / arena_dists [0, arena_end - arena_first);
+    // arena_ctr: the next position, the entries written, the entries of the queries that found no room
+    uint32_t* arena_ids;
+    float* arena_dists;
+    uint64_t arena_first, arena_end;
+    unsigned long long* arena_ctr;
+    uint64_t* q_pos;
+    uint32_t *q_count, *out_hops;
+    uint8_t* out_second;
+    uint32_t warp_smem, off_cid, off_cd;
+};
+
+// One warp per query of the pass's work list
+template <typename TD, int KIND, int POST, int NA>
+__global__ void __launch_bounds__(kRangeWarps * 32) range_kernel(const RangeParams p) {
+    constexpr bool INT = std::is_same<TD, int8_t>::value || std::is_same<TD, uint8_t>::value;
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    uint8_t* base = smem + (size_t)wib * p.warp_smem;
+    float* qf = reinterpret_cast<float*>(base);
+    uint32_t* cid = reinterpret_cast<uint32_t*>(base + p.off_cid);
+    float* cd = reinterpret_cast<float*>(base + p.off_cd);
+    const uint32_t warp_slot = blockIdx.x * kRangeWarps + wib;
+    const uint32_t nbk = p.n_buckets;
+    uint32_t* table = p.tables + (size_t)warp_slot * nbk * 8;
+    const uint32_t hlimit = nbk * 7;  // 87.5 % load
+    const uint64_t n_total = p.n_points + p.n_start;
+    uint32_t* rid = p.regions + (size_t)warp_slot * p.region_cap * 2;
+    float* rd = reinterpret_cast<float*>(rid + p.region_cap);
+    const int dim = (int)p.dim;
+    const unsigned below = (1u << lane) - 1u;
+
+    for (uint32_t qidx; next_query(p.counters, p.n_work, p.query_list, lane, qidx);) {
+        // ---- in_range: the phase-1 prefix within the radius, in list order
+        const uint32_t* li = p.list_ids + (size_t)qidx * p.l_search;
+        const float* ld = p.list_dists + (size_t)qidx * p.l_search;
+        const uint32_t n1 = p.list_counts[qidx];
+        uint64_t size = 0;
+        for (uint32_t b = 0; b < n1; b += 32) {
+            const uint32_t i = b + lane;
+            const float d = i < n1 ? ld[i] : 0.0f;
+            const bool in = i < n1 && d <= p.radius;
+            const unsigned m = __ballot_sync(kFull, in);
+            const uint64_t at = size + __popc(m & below);
+            if (in && at < p.region_cap) rid[at] = li[i], rd[at] = d;
+            size += __popc(m);
+        }
+        bool region_full = size > p.region_cap, overflow = region_full;
+        const bool second = size >= p.min_in_range && size < p.max_returned;
+        uint32_t hops = p.list_hops[qidx], nvisited = 0;
+        __syncwarp();
+
+        if (second && !overflow) {
+            // ---- range_search_internal: the visited set is the in_range ids, the frontier the suffix not yet expanded
+            load_query(reinterpret_cast<const TD*>(p.queries) + (size_t)qidx * dim, dim, 4, qf, lane);
+            for (uint32_t i = lane; i < nbk; i += 32) store_empty_bucket(table + (size_t)i * 8);
+            __syncwarp();
+            int qq = 0;  // integer rows: Sum x^2 of the query (unused by inner product)
+            if constexpr (INT) {
+                if (KIND != KIND_IP) qq = warp_int_self<std::is_same<TD, int8_t>::value>(reinterpret_cast<const uint8_t*>(qf), dim, lane);
+            }
+            for (uint32_t i = lane; i < size; i += 32) visit_global(table, nbk, rid[i]);
+            __syncwarp();  // every seed is in the table before any lane probes it for a neighbour
+            nvisited = (uint32_t)size;
+            overflow = nvisited + p.max_degree > hlimit;
+            uint64_t front = 0;
+            uint32_t hops2 = 0;
+            while (!overflow && front < size && size < p.max_returned) {
+                const uint32_t nb = (uint32_t)min((unsigned long long)p.beam, (unsigned long long)(size - front));
+                const uint64_t f0 = front;
+                front += nb;
+                hops2 += nb;
+                for (uint32_t b = 0; b < nb && size < p.max_returned; ++b) {
+                    // expand_beam of one node: its unvisited, in-bounds neighbours in adjacency order
+                    const uint32_t node = rid[f0 + b];
+                    const uint32_t* row = p.adj + (size_t)node * p.adj_stride;
+                    const uint32_t deg = min(__ldg(row), p.max_degree);
+                    uint32_t ncand = 0;
+                    for (uint32_t c0 = 0; c0 < deg + 1; c0 += 32) {
+                        const uint32_t j = c0 + lane;
+                        const uint32_t word = j < p.adj_stride ? __ldg(row + j) : kEmptyV2;
+                        const bool inserted = j >= 1 && j <= deg && visit_global(table, nbk, word);
+                        push_new(inserted, inserted && word < n_total, word, cid, ncand, nvisited, lane);
+                    }
+                    if (nvisited + p.max_degree > hlimit) {
+                        overflow = true;
+                        break;
+                    }
+                    __syncwarp();
+                    // the distances of the shared schemas (distance_device.cuh), a team of lanes per row
+                    {
+                        constexpr int S = INT ? 32 : 8 * NA, TEAMS = 32 / S, U = kRangeRows;
+                        using Row = typename std::conditional<INT, uint8_t, TD>::type;
+                        const int team = lane / S, slot = lane % S;
+                        for (uint32_t c0 = 0; c0 < ncand; c0 += TEAMS * U) {
+                            float r[U];
+                            uint32_t cc[U];
+                            const Row* rows[U];
+#pragma unroll
+                            for (int u = 0; u < U; ++u) {
+                                cc[u] = c0 + u * TEAMS + team;
+                                rows[u] = reinterpret_cast<const Row*>(p.vectors + (size_t)cid[min(cc[u], ncand - 1)] * p.row_stride);
+                            }
+                            if constexpr (INT) warp_int_multi<std::is_same<TD, int8_t>::value, KIND, U>(reinterpret_cast<const uint8_t*>(qf), rows, dim, lane, qq, r);
+                            else team_float_multi<NA, KIND, U>(qf, rows, dim, slot, r);
+#pragma unroll
+                            for (int u = 0; u < U; ++u)
+                                if (slot == 0 && cc[u] < ncand) cd[cc[u]] = post_op<POST>(r[u]);
+                        }
+                        __syncwarp();
+                    }
+                    // the appends, in order, while in_range is below max_returned
+                    for (uint32_t c0 = 0; c0 < ncand && size < p.max_returned; c0 += 32) {
+                        const uint32_t c = c0 + lane;
+                        const float d = c < ncand ? cd[c] : 0.0f;
+                        const bool ok = c < ncand && d <= p.bound;
+                        const unsigned m = __ballot_sync(kFull, ok);
+                        const uint32_t take = (uint32_t)min((unsigned long long)__popc(m), (unsigned long long)(p.max_returned - size));
+                        if (size + take > p.region_cap) {
+                            region_full = overflow = true;
+                            break;
+                        }
+                        const uint32_t rank = __popc(m & below);
+                        if (ok && rank < take) rid[size + rank] = cid[c], rd[size + rank] = d;
+                        size += take;
+                    }
+                    __syncwarp();
+                    if (overflow) break;
+                }
+            }
+            hops = hops + (hops + hops2);
+        }
+
+        if (overflow) {
+            report_overflow(p.counters, p.overflow_list, qidx, lane);
+            if (region_full && lane == 0) atomicAdd(p.counters + 3, 1u);
+            continue;
+        }
+
+        // ---- the output: start points, deleted ids, the inner radius and the radius filtered out
+        auto keep = [&](uint64_t i) {
+            if (i >= size) return false;
+            const uint32_t id = rid[i];
+            const float d = rd[i];
+            if (id >= p.n_points) return false;
+            if (p.deleted && (__ldg(p.deleted + (id >> 5)) >> (id & 31) & 1u)) return false;
+            if (p.has_inner && d <= p.inner_radius) return false;
+            return d <= p.radius;
+        };
+        uint32_t count = 0;
+        for (uint64_t b = 0; b < size; b += 32) count += __popc(__ballot_sync(kFull, keep(b + lane)));
+        unsigned long long pos = 0;
+        int fits = 1;
+        if (lane == 0 && count) {
+            pos = atomicAdd(p.arena_ctr, (unsigned long long)count);
+            fits = pos + count <= p.arena_end;
+            if (fits) {
+                atomicAdd(p.arena_ctr + 1, (unsigned long long)count);
+            } else {
+                p.arena_fail[atomicAdd(p.counters + 4, 1u)] = qidx;
+                atomicAdd(p.arena_ctr + 2, (unsigned long long)count);
+            }
+        }
+        pos = __shfl_sync(kFull, pos, 0);
+        fits = __shfl_sync(kFull, fits, 0);
+        if (fits && count) {
+            uint32_t w = 0;
+            for (uint64_t b = 0; b < size; b += 32) {
+                const uint64_t i = b + lane;
+                const bool k = keep(i);
+                const unsigned m = __ballot_sync(kFull, k);
+                if (k) {
+                    const uint64_t at = pos - p.arena_first + w + __popc(m & below);
+                    p.arena_ids[at] = rid[i];
+                    p.arena_dists[at] = rd[i];
+                }
+                w += __popc(m);
+            }
+        }
+        if (lane == 0) {
+            atomicMax(p.counters + 2, nvisited);
+            p.q_count[qidx] = count;
+            p.q_pos[qidx] = pos;
+            p.out_hops[qidx] = hops;
+            p.out_second[qidx] = second ? 1 : 0;
+        }
+    }
+}
+
+// offsets [nq + 1] <- the exclusive prefix sums of counts, by one block of 1024 threads
+__global__ void __launch_bounds__(1024) range_scan(const uint32_t* counts, uint32_t nq, uint64_t* offsets) {
+    __shared__ unsigned long long part[1024];
+    const uint32_t t = threadIdx.x, per = (nq + 1023) / 1024;
+    const uint64_t lo = (uint64_t)t * per, hi = lo + per < nq ? lo + per : (uint64_t)nq;
+    unsigned long long s = 0;
+    for (uint64_t i = lo; i < hi; ++i) s += counts[i];
+    part[t] = s;
+    __syncthreads();
+    for (uint32_t o = 1; o < 1024; o <<= 1) {
+        const unsigned long long v = t >= o ? part[t - o] : 0;
+        __syncthreads();
+        part[t] += v;
+        __syncthreads();
+    }
+    unsigned long long run = part[t] - s;
+    for (uint64_t i = lo; i < hi; ++i) {
+        offsets[i] = run;
+        run += counts[i];
+    }
+    if (t == 1023) offsets[nq] = part[1023];
+}
+
+// The results of query q from the arena (positions below `split` in the first part, the rest in the second) to
+// out [offsets[q], offsets[q + 1]), a warp per query
+__global__ void range_compact(const uint64_t* q_pos, const uint32_t* q_count, const uint64_t* offsets, uint32_t nq, const uint32_t* a1_ids,
+                              const float* a1_dists, const uint32_t* a2_ids, const float* a2_dists, uint64_t split, uint32_t* out_ids,
+                              float* out_dists) {
+    const int lane = threadIdx.x & 31;
+    const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x >> 5);
+    for (uint64_t q = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5; q < nq; q += warps) {
+        const uint64_t pos = q_pos[q], dst = offsets[q];
+        const uint32_t n = q_count[q];
+        const uint32_t* si = pos < split ? a1_ids + pos : a2_ids + (pos - split);
+        const float* sd = pos < split ? a1_dists + pos : a2_dists + (pos - split);
+        for (uint32_t i = lane; i < n; i += 32) {
+            out_ids[dst + i] = si[i];
+            out_dists[dst + i] = sd[i];
+        }
+    }
+}
+
+template <typename S>
+void (*range_kernel_of())(const RangeParams) {
+    return range_kernel<typename S::TD, S::KIND, S::POST, S::NA>;
+}
+
+// A warp's shared memory: the query (i8 / u8: its bytes rounded up to 16; floats: dim f32), then one node's candidate
+// ids and distances
+size_t range_warp_smem(const dab_index* idx, RangeParams* p) {
+    const bool is_int = idx->dtype == DAB_I8 || idx->dtype == DAB_U8;
+    size_t off = is_int ? round_up(round_up((size_t)idx->dim, 4), 16) : round_up((size_t)idx->dim * 4, 16);
+    const size_t ncand = round_up(std::max<size_t>(idx->max_degree, 32) * 4, 16);
+    RangeParams scratch;
+    RangeParams& q = p ? *p : scratch;
+    q.off_cid = (uint32_t)off, off += ncand;
+    q.off_cd = (uint32_t)off, off += ncand;
+    return round_up(off, 128);
+}
+
+// The range search's own checks, after Range::validate_and_create's (range_search.rs:91-131) in its order
+int check_range_args(const dab_index* idx, const char* api, uint32_t l_search, uint32_t beam, float radius, int has_inner, float inner_radius,
+                     float initial_slack, float range_slack, uint64_t max_returned) {
+    if (!idx->graph_ready || !idx->vectors_ready) return fail(DAB_ERR_NOT_READY, "%s: vectors and graph must be uploaded first", api);
+    if (beam == 0) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: beam_width must be > 0 (BeamWidthZero)", api);
+    if (l_search == 0) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: l_search must be > 0 (LZero)", api);
+    if (max_returned != 0 && max_returned < l_search)
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: max_returned (%llu) must be >= l_search (%u) (MaxReturnedLessThanInitialL)", api,
+                    (unsigned long long)max_returned, l_search);
+    if (!(initial_slack >= 0.0f && initial_slack <= 1.0f))
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: initial_slack %g must be in [0, 1] (StartingListSlackValueError)", api, (double)initial_slack);
+    if (range_slack < 1.0f) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: range_slack %g must be >= 1 (RangeSearchSlackValueError)", api, (double)range_slack);
+    if (has_inner && inner_radius > radius)
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: inner_radius %g must be <= radius %g (InnerRadiusValueError)", api, (double)inner_radius, (double)radius);
+    if (beam > 64) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: beam_width %u > 64", api, beam);
+    const size_t smem = range_warp_smem(idx, nullptr) * kRangeWarps;
+    if (smem > kRangeMaxSmem)
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: dim=%u, max_degree=%u need %zu B shared memory per CTA (> %zu)", api, idx->dim, idx->max_degree,
+                    smem, kRangeMaxSmem);
+    return DAB_OK;
+}
+
+// n entries (ids and dists) of result storage, or DAB_ERR_OUT_OF_MEMORY naming what the batch needs
+int alloc_entries(const dab_index* idx, const char* api, DevBuf& buf, uint64_t n, uint64_t need) {
+    const uint64_t limit = idx->tune.test_range_limit ? idx->tune.test_range_limit : UINT64_MAX;
+    if (n > limit || buf.alloc(n * 8, api))
+        return fail(DAB_ERR_OUT_OF_MEMORY, "%s: the batch's results need %llu entries (%llu bytes), more than device memory holds", api,
+                    (unsigned long long)need, (unsigned long long)need * 8);
+    return DAB_OK;
+}
+
+void range_unlink(dab_range* r) {
+    if (r->prev) r->prev->next = r->next;
+    else r->idx->ranges = r->next;
+    if (r->next) r->next->prev = r->prev;
+}
+
+void range_free(dab_range* r) {
+    cudaFree(r->d_stats);
+    cudaFree(r->d_results);
+    delete r;
+}
+
+// Both phases for nq >= 1 queries (checks passed) into a new result set
+int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t nq, uint32_t l_search, uint32_t beam, float radius, int has_inner,
+              float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, dab_range* r) {
+    cudaStream_t st = idx->stream;
+    int rc;
+    // ---- the result set's statistics, then phase 1: the first L entries of every list with start points and
+    // deleted ids kept, its cmps (the result set's) and hops
+    const size_t stat_bytes = ((size_t)nq + 1) * 8 + (size_t)nq * 9;
+    DAB_CUDA(cudaMalloc(&r->d_stats, stat_bytes));
+    DevBuf p1;
+    const size_t lq = (size_t)nq * l_search;
+    if ((rc = p1.alloc(lq * 8 + (size_t)nq * 8, api))) return rc;
+    uint32_t* list_ids = (uint32_t*)p1.p;
+    float* list_dists = (float*)(list_ids + lq);
+    uint32_t* list_counts = (uint32_t*)(list_dists + lq);
+    uint32_t* list_hops = list_counts + nq;
+    SearchRecord rec{};
+    rec.keep_starts = true;
+    rec.keep_deleted = true;
+    if ((rc = run_search(idx, d_queries, nq, l_search, l_search, beam, SearchOut{list_ids, list_dists, list_counts, r->cmps(), list_hops}, -1,
+                         false, &rec)))
+        return rc;
+
+    // ---- phase 2
+    RangeParams p;
+    memset(&p, 0, sizeof(p));
+    p.warp_smem = (uint32_t)range_warp_smem(idx, &p);
+    const size_t smem_block = (size_t)p.warp_smem * kRangeWarps;
+    void (*kern)(const RangeParams) = nullptr;
+    visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) -> int {
+        kern = range_kernel_of<decltype(sc)>();
+        return DAB_OK;
+    });
+    const int per_sm = ctas_per_sm(kern, kRangeWarps * 32, smem_block);
+    if (per_sm < 1) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: dim=%u needs %zu B shared memory per CTA", api, idx->dim, smem_block);
+    const int resident = per_sm * idx->sm_count;
+    set_graph_params(idx, p);
+    p.vectors = idx->d_vectors;
+    p.row_stride = idx->row_stride;
+    p.queries = d_queries;
+    p.l_search = l_search;
+    p.beam = beam;
+    p.list_ids = list_ids, p.list_dists = list_dists, p.list_counts = list_counts, p.list_hops = list_hops;
+    p.radius = radius;
+    p.bound = radius * range_slack;  // an f32 product, as the reference's
+    p.has_inner = has_inner ? 1 : 0;
+    p.inner_radius = inner_radius;
+    p.min_in_range = (uint64_t)((float)l_search * initial_slack);
+    p.max_returned = max_returned ? max_returned : UINT64_MAX;
+    p.deleted = deleted_filter(idx);
+    p.out_hops = r->hops();
+    p.out_second = r->second();
+
+    DevBuf ctr, per_query, tables, regions, arena1, arena2;
+    if ((rc = ctr.alloc(64 + (size_t)nq * 8, api)) || (rc = per_query.alloc((size_t)nq * 12, api))) return rc;
+    p.arena_ctr = (unsigned long long*)ctr.p;
+    p.counters = (uint32_t*)((uint8_t*)ctr.p + 32);
+    p.overflow_list = (uint32_t*)((uint8_t*)ctr.p + 64);
+    p.arena_fail = p.overflow_list + nq;
+    p.q_pos = (uint64_t*)per_query.p;
+    p.q_count = (uint32_t*)(p.q_pos + nq);
+    DAB_CUDA(cudaMemsetAsync(ctr.p, 0, 64, st));
+    uint32_t* h = (uint32_t*)idx->h_counters.p;  // pinned: the five counters, then the three arena counters
+
+    // the in_range regions and the arena of the first pass
+    const uint64_t region_max = std::min<uint64_t>(p.max_returned, idx->n_total());
+    uint64_t region = idx->tune.test_range_list ? idx->tune.test_range_list : round_up(std::max<uint64_t>(4ull * l_search, 1024), 32);
+    region = std::min(region, region_max);
+    uint64_t slots = table_slots(idx, VisitedHint{}, l_search, beam, STORE_PQ);
+    const uint64_t limit = idx->tune.test_range_limit ? idx->tune.test_range_limit : UINT64_MAX;
+    const uint64_t arena_first = std::min<uint64_t>(idx->tune.test_range_arena ? idx->tune.test_range_arena : (uint64_t)nq * l_search, limit);
+    if ((rc = alloc_entries(idx, api, arena1, arena_first, arena_first))) return rc;
+    p.arena_ids = (uint32_t*)arena1.p;
+    p.arena_dists = (float*)(p.arena_ids + arena_first);
+    p.arena_first = 0;
+    p.arena_end = arena_first;
+
+    DevBuf retry;
+    if ((rc = retry.alloc((size_t)nq * 4, api))) return rc;
+    p.n_work = nq;
+    int pass = 0;
+    bool grown = false;
+    uint64_t used = 0;
+    for (;;) {
+        // the grid of this pass: one warp per query at most, and regions within kRegionBudget
+        int grid = balanced_grid(p.n_work, resident, kRangeWarps);
+        const uint64_t region_grid = std::max<uint64_t>(1, kRegionBudget / (region * 8 * kRangeWarps));
+        grid = (int)std::min<uint64_t>(grid, region_grid);
+        const uint64_t warps = (uint64_t)grid * kRangeWarps;
+        p.n_buckets = (uint32_t)((slots + 7) / 8);
+        p.region_cap = (uint32_t)region;
+        if ((rc = tables.alloc(warps * p.n_buckets * 32, api)) || (rc = regions.alloc(warps * region * 8, api))) return rc;
+        p.tables = (uint32_t*)tables.p;
+        p.regions = (uint32_t*)regions.p;
+        DAB_CUDA(cudaMemsetAsync(p.counters, 0, 16, st));
+        DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_block));
+        kern<<<grid, kRangeWarps * 32, smem_block, st>>>(p);
+        DAB_LAUNCHED();
+        DAB_CUDA(cudaGetLastError());
+        DAB_CUDA(cudaMemcpyAsync(h, ctr.p, 64, cudaMemcpyDeviceToHost, st));
+        DAB_CUDA(cudaStreamSynchronize(st));
+        const unsigned long long* actr = (const unsigned long long*)h;
+        const uint32_t* c = h + 8;
+        const uint32_t n_over = c[1], n_region = c[3], n_fail = c[4];
+        if (n_over) {
+            // the stopped queries are the next pass's work: on larger tables, larger regions, or both
+            if (n_over > n_region && (rc = grow_visited_tables(idx, pass, slots))) return rc;
+            if (n_region) region = std::min(region * 4, region_max);
+            DAB_CUDA(cudaMemcpyAsync(retry.p, p.overflow_list, (size_t)n_over * 4, cudaMemcpyDeviceToDevice, st));
+            p.query_list = (const uint32_t*)retry.p;
+            p.n_work = n_over;
+            continue;
+        }
+        if (n_fail) {
+            // every query has completed; those that found no room re-run into an arena of exactly what they need
+            if (grown) return fail(DAB_ERR_CUDA, "%s: queries re-run into the extended arena found no room", api);
+            used = actr[1];
+            const uint64_t need = actr[2];
+            if ((rc = alloc_entries(idx, api, arena2, need, used + need))) return rc;
+            grown = true;
+            p.arena_ids = (uint32_t*)arena2.p;
+            p.arena_dists = (float*)(p.arena_ids + need);
+            p.arena_first = used;
+            p.arena_end = used + need;
+            const unsigned long long reset[3] = {used, used, 0};
+            DAB_CUDA(cudaMemcpyAsync(ctr.p, reset, sizeof(reset), cudaMemcpyHostToDevice, st));
+            DAB_CUDA(cudaMemsetAsync(p.counters + 4, 0, 4, st));
+            DAB_CUDA(cudaMemcpyAsync(retry.p, p.arena_fail, (size_t)n_fail * 4, cudaMemcpyDeviceToDevice, st));
+            DAB_CUDA(cudaStreamSynchronize(st));  // `reset` is read from pageable host memory
+            p.query_list = (const uint32_t*)retry.p;
+            p.n_work = n_fail;
+            continue;
+        }
+        break;
+    }
+    cudaFree(tables.p), cudaFree(regions.p);
+    tables.p = regions.p = nullptr;
+
+    // ---- the result set: offsets, then the results in query order
+    range_scan<<<1, 1024, 0, st>>>(p.q_count, nq, r->offsets());
+    DAB_LAUNCHED();
+    DAB_CUDA(cudaGetLastError());
+    DAB_CUDA(cudaMemcpyAsync(&r->total, r->offsets() + nq, 8, cudaMemcpyDeviceToHost, st));
+    DAB_CUDA(cudaStreamSynchronize(st));
+    DevBuf out;
+    if ((rc = alloc_entries(idx, api, out, r->total, r->total))) return rc;
+    const uint64_t split = grown ? used : UINT64_MAX;
+    const uint32_t* a2_ids = grown ? (const uint32_t*)arena2.p : nullptr;
+    const float* a2_dists = grown ? (const float*)(a2_ids + (p.arena_end - used)) : nullptr;
+    range_compact<<<grid_for(idx, (uint64_t)nq * 32), 256, 0, st>>>(p.q_pos, p.q_count, r->offsets(), nq, (const uint32_t*)arena1.p,
+                                                                    (const float*)((const uint32_t*)arena1.p + arena_first), a2_ids, a2_dists,
+                                                                    split, (uint32_t*)out.p, (float*)((uint32_t*)out.p + r->total));
+    DAB_LAUNCHED();
+    DAB_CUDA(cudaGetLastError());
+    DAB_CUDA(cudaStreamSynchronize(st));
+    r->d_results = out.p;
+    out.p = nullptr;
+    return DAB_OK;
+}
+
+// a batch of no queries: offsets {0}
+int range_empty(dab_index* idx, dab_range* r) {
+    DAB_CUDA(cudaMalloc(&r->d_stats, 8));
+    DAB_CUDA(cudaMemsetAsync(r->d_stats, 0, 8, idx->stream));
+    DAB_CUDA(cudaStreamSynchronize(idx->stream));
+    return DAB_OK;
+}
+
+// nq >= 1 queries, from the host (`host`, copied to the handle's scratch) or the device
+int range_queries(dab_index* idx, const char* api, bool host, const void* queries, uint32_t nq, uint32_t l_search, uint32_t beam, float radius,
+                  int has_inner, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, dab_range* r) {
+    const void* d_queries = queries;
+    if (host) {
+        const size_t qbytes = (size_t)nq * idx->dim * elem_size(idx->dtype);
+        int rc;
+        if ((rc = idx->s_queries.reserve(qbytes))) return rc;
+        d_queries = idx->s_queries.p;
+        DAB_CUDA(cudaMemcpyAsync(idx->s_queries.p, queries, qbytes, cudaMemcpyHostToDevice, idx->stream));
+    }
+    return range_run(idx, api, d_queries, nq, l_search, beam, radius, has_inner, inner_radius, initial_slack, range_slack, max_returned, r);
+}
+
+int range_search(dab_index* idx, const char* api, bool host, const void* queries, uint32_t nq, uint32_t l_search, uint32_t beam, float radius,
+                 int has_inner, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, dab_range** out) {
+    if (!idx || !out || (nq && !queries)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
+    *out = nullptr;
+    int rc;
+    if ((rc = check_range_args(idx, api, l_search, beam, radius, has_inner, inner_radius, initial_slack, range_slack, max_returned))) return rc;
+    DAB_CUDA(cudaSetDevice(idx->device));
+    if ((rc = idx->h_counters.reserve(64))) return rc;
+    dab_range* r = new dab_range();
+    r->idx = idx;
+    r->nq = nq;
+    if ((rc = nq ? range_queries(idx, api, host, queries, nq, l_search, beam, radius, has_inner, inner_radius, initial_slack, range_slack,
+                                 max_returned, r)
+                 : range_empty(idx, r))) {
+        cudaStreamSynchronize(idx->stream);
+        range_free(r);
+        return rc;
+    }
+    r->next = idx->ranges;
+    if (r->next) r->next->prev = r;
+    idx->ranges = r;
+    *out = r;
+    return DAB_OK;
+}
+
+}  // namespace
+
+void range_release(dab_index* idx) {
+    while (idx->ranges) {
+        dab_range* r = idx->ranges;
+        range_unlink(r);
+        range_free(r);
+    }
+}
+
+}  // namespace dab
+
+using namespace dab;
+
+extern "C" {
+
+int dab_range_search(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search, uint32_t beam_width, float radius, int has_inner_radius,
+                     float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, dab_range** out) {
+    return range_search(idx, "dab_range_search", true, queries, nq, l_search, beam_width, radius, has_inner_radius, inner_radius, initial_slack,
+                        range_slack, max_returned, out);
+}
+
+int dab_range_search_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t l_search, uint32_t beam_width, float radius,
+                            int has_inner_radius, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned,
+                            dab_range** out) {
+    return range_search(idx, "dab_range_search_device", false, d_queries, nq, l_search, beam_width, radius, has_inner_radius, inner_radius,
+                        initial_slack, range_slack, max_returned, out);
+}
+
+int dab_range_offsets(const dab_range* r, uint64_t* offsets, uint32_t* cmps, uint32_t* hops, uint8_t* second_round) {
+    if (!r || !offsets) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_range_offsets: NULL argument");
+    DAB_CUDA(cudaSetDevice(r->idx->device));
+    const size_t nq = r->nq;
+    DAB_CUDA(cudaMemcpy(offsets, r->offsets(), (nq + 1) * 8, cudaMemcpyDeviceToHost));
+    if (nq && cmps) DAB_CUDA(cudaMemcpy(cmps, r->cmps(), nq * 4, cudaMemcpyDeviceToHost));
+    if (nq && hops) DAB_CUDA(cudaMemcpy(hops, r->hops(), nq * 4, cudaMemcpyDeviceToHost));
+    if (nq && second_round) DAB_CUDA(cudaMemcpy(second_round, r->second(), nq, cudaMemcpyDeviceToHost));
+    return DAB_OK;
+}
+
+static int range_results(const dab_range* r, const char* api, uint32_t* ids, float* dists, cudaMemcpyKind kind) {
+    if (!r || (r->total && (!ids || !dists))) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
+    if (!r->total) return DAB_OK;
+    DAB_CUDA(cudaSetDevice(r->idx->device));
+    DAB_CUDA(cudaMemcpy(ids, r->d_results, r->total * 4, kind));
+    DAB_CUDA(cudaMemcpy(dists, (const uint32_t*)r->d_results + r->total, r->total * 4, kind));
+    return DAB_OK;
+}
+
+int dab_range_results(const dab_range* r, uint32_t* ids, float* dists) {
+    return range_results(r, "dab_range_results", ids, dists, cudaMemcpyDeviceToHost);
+}
+
+int dab_range_results_device(const dab_range* r, uint32_t* d_ids, float* d_dists) {
+    return range_results(r, "dab_range_results_device", d_ids, d_dists, cudaMemcpyDeviceToDevice);
+}
+
+void dab_range_free(dab_range* r) {
+    if (!r) return;
+    cudaSetDevice(r->idx->device);
+    cudaStreamSynchronize(r->idx->stream);
+    range_unlink(r);
+    range_free(r);
+}
+
+}  // extern "C"

@@ -251,6 +251,7 @@ class GpuIndex:
         self._h = C.c_void_p()
         self._inflight = {}  # slot -> (queries, outputs) kept alive while a batch is in flight
         self._paged = weakref.WeakSet()  # open paged searches: dab_destroy releases them
+        self._ranges = weakref.WeakSet()  # open range search result sets: dab_destroy releases them too
         self.dtype, self.metric, self.dim = DType(dtype), Metric(metric), int(dim)
         self.n_points, self.n_start, self.max_degree, self.device = int(n_points), int(n_start), int(max_degree), device
         check(_lib.lib().dab_create(C.byref(self._h), int(dtype), int(metric), dim, n_points, n_start, max_degree, device))
@@ -258,7 +259,7 @@ class GpuIndex:
     # -- lifecycle
     def close(self):
         if getattr(self, "_h", None) is not None and self._h.value:
-            for s in list(getattr(self, "_paged", ())):
+            for s in list(getattr(self, "_paged", ())) + list(getattr(self, "_ranges", ())):
                 s._h = C.c_void_p()  # released by dab_destroy
             _lib.lib().dab_destroy(self._h)
             self._h = C.c_void_p()
@@ -420,6 +421,28 @@ class GpuIndex:
         """paged_search through the MinMax store, as search_batch_minmax traverses it; no rerank.  A query holding a NaN
         after the store's transform fails the call."""
         return PagedSearch(self, self._queries(queries), l_search, _lib.lib().dab_paged_search_begin_minmax)
+
+    def range_search(self, queries, l_search, radius, *, beam_width=1, inner_radius=None, initial_slack=1.0, range_slack=1.0,
+                     max_returned=None):
+        """Range::search for the whole batch: every point within `radius` of each query, in the reference's order.
+        Returns (offsets [nq + 1] u64, ids, dists, cmps, hops, second_round): query q's results are
+        ids[offsets[q]:offsets[q + 1]].  max_returned=None: no limit."""
+        with self.range_search_set(queries, l_search, radius, beam_width=beam_width, inner_radius=inner_radius,
+                                   initial_slack=initial_slack, range_slack=range_slack, max_returned=max_returned) as r:
+            offsets, cmps, hops, second = r.offsets()
+            ids, dists = r.results()
+        return offsets, ids, dists, cmps, hops, second
+
+    def range_search_set(self, queries, l_search, radius, **kw):
+        """range_search, keeping the result set on the device: a RangeResults"""
+        return RangeResults(self, _lib.lib().dab_range_search, _ptr(self._queries(queries)), len(queries), l_search, radius, **kw)
+
+    def range_search_device(self, d_queries, nq, l_search, radius, *, beam_width=1, inner_radius=None, initial_slack=1.0,
+                            range_slack=1.0, max_returned=None):
+        """range_search of `nq` queries at the device pointer `d_queries` (an integer): a RangeResults, whose
+        results_device copies the results to device buffers"""
+        return RangeResults(self, _lib.lib().dab_range_search_device, C.c_void_p(d_queries), nq, l_search, radius, beam_width=beam_width,
+                            inner_radius=inner_radius, initial_slack=initial_slack, range_slack=range_slack, max_returned=max_returned)
 
     def search_batch_device(self, d_queries, nq, k, l_search, beam_width, d_ids, d_dists, d_counts=0, d_cmps=0, d_hops=0):
         """Same with device pointers (integers); results stay in HBM."""
@@ -856,6 +879,65 @@ class PagedSearch:
     def close(self):
         if getattr(self, "_h", None) is not None and self._h.value:
             _lib.lib().dab_paged_search_end(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+
+class RangeResults:
+    """One range search batch's results, resident on the device (dab_range): a snapshot that later writes to the index
+    do not change.  Use as a context manager or call close(); closing the index closes it too."""
+
+    def __init__(self, index, search, queries, nq, l_search, radius, beam_width=1, inner_radius=None, initial_slack=1.0,
+                 range_slack=1.0, max_returned=None):
+        self._h = C.c_void_p()
+        self.nq = int(nq)
+        check(search(index._h, queries, self.nq, l_search, beam_width, radius, int(inner_radius is not None),
+                     0.0 if inner_radius is None else inner_radius, initial_slack, range_slack, max_returned or 0, C.byref(self._h)))
+        index._ranges.add(self)
+
+    def _live(self):
+        if not self._h.value:
+            raise DabError(1, "the range search results are closed")
+        return self._h
+
+    def offsets(self):
+        """(offsets [nq + 1] u64, cmps, hops, second_round [nq] bool)"""
+        offsets = np.empty(self.nq + 1, np.uint64)
+        cmps, hops = np.empty(self.nq, np.uint32), np.empty(self.nq, np.uint32)
+        second = np.empty(self.nq, np.uint8)
+        check(_lib.lib().dab_range_offsets(self._live(), _ptr(offsets), _ptr(cmps), _ptr(hops), _ptr(second)))
+        return offsets, cmps, hops, second.astype(bool)
+
+    def total(self):
+        offsets = np.empty(self.nq + 1, np.uint64)
+        check(_lib.lib().dab_range_offsets(self._live(), _ptr(offsets), None, None, None))
+        return int(offsets[-1])
+
+    def results(self):
+        """(ids, dists) of every query, in query order"""
+        n = self.total()
+        ids, dists = np.empty(n, np.uint32), np.empty(n, np.float32)
+        check(_lib.lib().dab_range_results(self._live(), _ptr(ids), _ptr(dists)))
+        return ids, dists
+
+    def results_device(self, d_ids, d_dists):
+        """the results into device buffers (integers) of total() entries each"""
+        check(_lib.lib().dab_range_results_device(self._live(), C.c_void_p(d_ids), C.c_void_p(d_dists)))
+
+    def close(self):
+        if getattr(self, "_h", None) is not None and self._h.value:
+            _lib.lib().dab_range_free(self._h)
             self._h = C.c_void_p()
 
     def __del__(self):

@@ -51,6 +51,33 @@ pub struct Batch {
     pub hops: Vec<u32>,
 }
 
+/// `Range`'s parameters besides `starting_l` and `radius`, with the reference's defaults
+#[derive(Clone, Copy, Debug)]
+pub struct RangeArgs {
+    pub beam_width: u32,
+    pub inner_radius: Option<f32>,
+    pub initial_slack: f32,
+    pub range_slack: f32,
+    pub max_returned: Option<u64>,
+}
+
+impl Default for RangeArgs {
+    fn default() -> Self {
+        RangeArgs { beam_width: 1, inner_radius: None, initial_slack: 1.0, range_slack: 1.0, max_returned: None }
+    }
+}
+
+/// A range search batch: query q's results are `ids[offsets[q]..offsets[q + 1]]` with their distances
+#[derive(Debug, Default)]
+pub struct RangeBatch {
+    pub offsets: Vec<u64>,
+    pub ids: Vec<u32>,
+    pub dists: Vec<f32>,
+    pub cmps: Vec<u32>,
+    pub hops: Vec<u32>,
+    pub second_round: Vec<u8>,
+}
+
 pub struct GpuIndex<T: Element> {
     raw: *mut sys::dab_index,
     dim: usize,
@@ -208,6 +235,33 @@ impl<T: Element> GpuIndex<T> {
                                           b.hops.as_mut_ptr())
         })?;
         Ok(b)
+    }
+
+    /// `Range::search` (range_search.rs:255-469) for the batch: every point within `radius` of each query, query q's
+    /// results at `offsets[q] .. offsets[q + 1]` in the reference's output order.
+    pub fn range_search(&self, queries: &[T], l_search: u32, radius: f32, args: RangeArgs) -> Result<RangeBatch> {
+        assert_eq!(queries.len() % self.dim, 0);
+        let nq = queries.len() / self.dim;
+        let mut set: *mut sys::dab_range = std::ptr::null_mut();
+        check(unsafe {
+            sys::dab_range_search(self.raw, queries.as_ptr() as *const c_void, nq as u32, l_search, args.beam_width, radius,
+                                  args.inner_radius.is_some() as i32, args.inner_radius.unwrap_or(0.0), args.initial_slack,
+                                  args.range_slack, args.max_returned.unwrap_or(0), &mut set)
+        })?;
+        let mut r = RangeBatch { offsets: vec![0; nq + 1], ids: Vec::new(), dists: Vec::new(), cmps: vec![0; nq], hops: vec![0; nq],
+                                 second_round: vec![0; nq] };
+        let rc = unsafe {
+            sys::dab_range_offsets(set, r.offsets.as_mut_ptr(), r.cmps.as_mut_ptr(), r.hops.as_mut_ptr(), r.second_round.as_mut_ptr())
+        };
+        if rc == 0 {
+            let total = r.offsets[nq] as usize;
+            r.ids = vec![0; total];
+            r.dists = vec![0.0; total];
+        }
+        let rc = if rc == 0 { unsafe { sys::dab_range_results(set, r.ids.as_mut_ptr(), r.dists.as_mut_ptr()) } } else { rc };
+        unsafe { sys::dab_range_free(set) };
+        check(rc)?;
+        Ok(r)
     }
 
     /// `search_batch_diverse` with the traversal distances of `search_batch_pq` (the PQ store); `rerank`: the

@@ -251,6 +251,51 @@ int dab_search_batch_diverse_minmax_device(dab_index* idx, const void* d_queries
                                            float* d_out_dists, uint32_t* d_out_counts,
                                            uint32_t* d_out_cmps, uint32_t* d_out_hops);
 
+/* ------------------------------------------------------------------ (3'''') range search */
+
+/* Range::search (diskann/src/graph/search/range_search.rs:255-469) for a whole query batch over
+ * full-precision rows of every dtype and metric: every point within `radius` of each query.
+ *   phase 1: the k-NN traversal of dab_search_batch with a list of l_search + n_start entries;
+ *     in_range is its first l_search entries with distance <= radius, in list order.
+ *   second round iff |in_range| >= (size_t)((float)l_search * initial_slack) and
+ *     |in_range| < max_returned: the visited set is re-seeded with the in_range ids and the
+ *     graph is walked breadth-first from them, beam_width ids at a time; each new neighbour with
+ *     distance <= radius * range_slack (an f32 product) is appended while |in_range| < max_returned.
+ *   results: in_range in insertion order (not sorted) without start points, deleted ids, ids
+ *     with distance <= inner_radius (when has_inner_radius) and ids with distance > radius.
+ * Deleted ids and start points are walked and count toward max_returned; they are never returned.
+ * Per query: cmps are phase 1's comparisons; hops are phase 1's, or phase1 + (phase1 + phase2)
+ * when the second round ran (the reference adds its cumulative hop count to phase 1's);
+ * second_round says whether it ran.  max_returned == 0 means no limit (the reference rejects
+ * every limit below l_search).  Queries [nq][dim] have the index dtype (f16 queries are widened).
+ * Checked before any device work, each failing with DAB_ERR_INVALID_ARGUMENT and a message, in
+ * the reference's order: beam_width == 0, l_search == 0, max_returned < l_search,
+ * initial_slack outside [0, 1] (NaN included), range_slack < 1, inner_radius > radius; then
+ * beam_width > 64 and a CTA's shared memory above 200 KB (4 x (the query row + 8 * max(max_degree,
+ * 32) bytes)).  DAB_ERR_NOT_READY without vectors and graph.  A batch whose results cannot be held
+ * in device memory fails with DAB_ERR_OUT_OF_MEMORY naming the entries it needs; nothing stays
+ * allocated and the index stays usable.
+ * On success *out is a result set resident on the device: a snapshot that later uploads, inserts
+ * and deletes do not change.  dab_destroy releases every result set still open; their handles
+ * are invalid after it. */
+typedef struct dab_range dab_range; /* opaque: one batch's results, resident on the device */
+int dab_range_search(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search,
+                     uint32_t beam_width, float radius, int has_inner_radius, float inner_radius,
+                     float initial_slack, float range_slack, uint64_t max_returned, dab_range** out);
+/* the same with the queries in device memory */
+int dab_range_search_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t l_search,
+                            uint32_t beam_width, float radius, int has_inner_radius,
+                            float inner_radius, float initial_slack, float range_slack,
+                            uint64_t max_returned, dab_range** out);
+/* offsets [nq + 1]: query q's results are entries offsets[q] .. offsets[q + 1] - 1; cmps, hops
+ * [nq] u32 and second_round [nq] (0 / 1) may be NULL.  Host buffers. */
+int dab_range_offsets(const dab_range* r, uint64_t* offsets, uint32_t* cmps, uint32_t* hops,
+                      uint8_t* second_round);
+/* the offsets[nq] results: ids and distances, host buffers / device buffers */
+int dab_range_results(const dab_range* r, uint32_t* ids, float* dists);
+int dab_range_results_device(const dab_range* r, uint32_t* d_ids, float* d_dists);
+void dab_range_free(dab_range* r);
+
 /* ------------------------------------------------------------------ (3'') paged search */
 
 /* DiskANNIndex::paged_search (diskann/src/graph/index.rs:2075-2155) and PagedSearch::next_page

@@ -253,6 +253,52 @@ class Provider {
     uint32_t n_start_, max_degree_;
 };
 
+// Range::search for a whole batch (range_search.rs:255-469): query q's results are ids / distances
+// [offsets[q], offsets[q + 1]) in the reference's output order
+struct RangeResults {
+    uint32_t nq = 0;
+    std::vector<uint64_t> offsets;  // [nq + 1]
+    std::vector<uint32_t> ids;
+    std::vector<float> distances;
+    std::vector<uint32_t> cmps, hops;
+    std::vector<uint8_t> second_round;  // range_search_second_round
+};
+
+// Range::builder(starting_l, radius) with its optional fields; max_returned 0: None
+template <class T>
+class GpuRange {
+   public:
+    GpuRange(Provider<T>& provider, uint32_t starting_l, float radius, uint32_t beam_width = 1, bool has_inner_radius = false,
+             float inner_radius = 0.0f, float initial_slack = 1.0f, float range_slack = 1.0f, uint64_t max_returned = 0)
+        : p_(provider), l_(starting_l), beam_(beam_width), radius_(radius), has_inner_(has_inner_radius), inner_(inner_radius),
+          initial_slack_(initial_slack), range_slack_(range_slack), max_returned_(max_returned) {}
+    RangeResults search(const T* queries, uint32_t nq) {
+        dab_range* set = nullptr;
+        check(dab_range_search(p_.raw(), queries, nq, l_, beam_, radius_, has_inner_ ? 1 : 0, inner_, initial_slack_, range_slack_,
+                               max_returned_, &set));
+        std::unique_ptr<dab_range, void (*)(dab_range*)> owned(set, dab_range_free);
+        RangeResults r;
+        r.nq = nq;
+        r.offsets.resize((size_t)nq + 1);
+        r.cmps.resize(nq);
+        r.hops.resize(nq);
+        r.second_round.resize(nq);
+        check(dab_range_offsets(set, r.offsets.data(), r.cmps.data(), r.hops.data(), r.second_round.data()));
+        r.ids.resize(r.offsets[nq]);
+        r.distances.resize(r.offsets[nq]);
+        check(dab_range_results(set, r.ids.data(), r.distances.data()));
+        return r;
+    }
+
+   private:
+    Provider<T>& p_;
+    uint32_t l_, beam_;
+    float radius_;
+    bool has_inner_;
+    float inner_, initial_slack_, range_slack_;
+    uint64_t max_returned_;
+};
+
 // Diverse::search for a whole batch (diverse_search.rs:114-234): Diverse::new(Knn::new(l_value, beam_width),
 // DiverseSearchParams::new(_, diverse_k, k, provider's attributes)); at most diverse_k results per attribute value.
 template <class T>

@@ -1,0 +1,123 @@
+"""Range search on the C2 workload of bench.py, against the k-NN search at the same L.
+
+C2: 1M x 128 f32 rows, L2, a Vamana graph built on the device (R = 64, L_build = 100), 10K queries, L = 100.  The radii
+are those at which the exact mean in-range count is about 10, 100 and 1000: bisection on the radius over the exact
+distances of every query to every row (f64, on the GPU with torch).  For each radius dab_range_search_device runs --reps
+times after two warm-up calls, timed with CUDA events around each call (which returns with the result set complete);
+the median is reported.  Phase 1 is the k-NN traversal with k = L, which dab_search_batch_device runs on its own at the
+same L and beam: it is timed the same way and reported as the phase-1 time, and the rest of the range call as phase 2
+(its in_range pass, second rounds, re-runs, scan and compaction).  Per radius: the mean and largest result counts, the
+share of queries that took a second round, mean hops, and the reference's average_precision (benchmark-core/src/
+recall.rs: the share of all exact in-range ids, over all queries, that the search returned).  The card's name and power
+limit are read in the same run.
+usage: python tools/bench_range.py [--n N] [--nq NQ] [--reps R] [--beam B] [--json PATH]"""
+import argparse
+import json
+import os
+import statistics
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+import numpy as np
+import torch
+
+import bench
+from bench_minmax_search import build_index, card
+
+L, TARGETS, CHUNK = 100, (10, 100, 1000), 128
+
+
+def in_range_sets(base_t, bn, queries, radius, want_ids):
+    """exact in-range counts of every query (and, with want_ids, their ids) at `radius`, f64"""
+    counts, ids = [], []
+    for q0 in range(0, queries.shape[0], CHUNK):
+        q = torch.from_numpy(queries[q0:q0 + CHUNK]).cuda().double()
+        d = bn[None, :] - 2.0 * (q @ base_t.T) + (q * q).sum(1, keepdim=True)
+        m = d <= radius
+        counts.append(m.sum(1).cpu().numpy())
+        if want_ids:
+            nz = torch.nonzero(m).cpu().numpy()
+            ids.extend(np.split(nz[:, 1], np.cumsum(np.bincount(nz[:, 0], minlength=m.shape[0]))[:-1]))
+    return np.concatenate(counts), ids
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--n", type=int, default=0)
+    ap.add_argument("--nq", type=int, default=0)
+    ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--beam", type=int, default=1)
+    ap.add_argument("--json", default="")
+    args = ap.parse_args()
+    name, power = card()
+    cfg = dict(bench.WORKLOADS["c2_1Mx128_f32_l2"])
+    n, nq = args.n or cfg["n"], args.nq or cfg["nq"]
+    stream = torch.cuda.Stream()
+    torch.cuda.set_stream(stream)
+    g, base, centers = build_index(cfg, n, stream)
+    queries = bench.make_data(cfg, bench.SEED_QUERY, nq, centers)
+    base_t = torch.from_numpy(base).cuda().double()
+    bn = (base_t * base_t).sum(1)
+    d_q = torch.from_numpy(queries).cuda()
+
+    def timed(call):
+        call()
+        call()
+        ms = []
+        for _ in range(args.reps):
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record(stream)
+            call()
+            b.record(stream)
+            b.synchronize()
+            ms.append(a.elapsed_time(b))
+        return statistics.median(ms)
+
+    outs = (torch.empty((nq, L), dtype=torch.int32, device="cuda"), torch.empty((nq, L), dtype=torch.float32, device="cuda"),
+            *(torch.empty(nq, dtype=torch.int32, device="cuda") for _ in range(3)))
+    knn_ms = timed(lambda: g.search_batch_device(d_q.data_ptr(), nq, L, L, args.beam, *(o.data_ptr() for o in outs)))
+    knn_d = outs[1].cpu().numpy()
+
+    sample = queries[:: max(1, nq // 1000)]
+    rows = []
+    for target in TARGETS:
+        lo, hi = 0.0, float(np.median(knn_d[:, -1])) * 16
+        for _ in range(30):  # bisection on the mean exact count over a sample of the queries
+            mid = (lo + hi) / 2
+            if in_range_sets(base_t, bn, sample, mid, False)[0].mean() < target:
+                lo = mid
+            else:
+                hi = mid
+        radius = float(np.float32(hi))
+        exact, truth = in_range_sets(base_t, bn, queries, radius, True)
+
+        def call():
+            with g.range_search_device(d_q.data_ptr(), nq, L, radius, beam_width=args.beam):
+                pass
+        ms = timed(call)
+        with g.range_search_device(d_q.data_ptr(), nq, L, radius, beam_width=args.beam) as r:
+            offsets, cmps, hops, second = r.offsets()
+            ids, _ = r.results()
+        counts = np.diff(offsets.astype(np.int64))
+        found = sum(len(np.intersect1d(truth[q], ids[offsets[q]:offsets[q + 1]])) for q in range(nq))
+        row = dict(target_mean_count=target, radius=radius, exact_mean_count=round(float(exact.mean()), 2), exact_max_count=int(exact.max()),
+                   ms_per_batch=round(ms, 3), phase1_ms=round(knn_ms, 3), phase2_ms=round(ms - knn_ms, 3), qps=round(nq / ms * 1e3, 1),
+                   mean_count=round(float(counts.mean()), 2), max_count=int(counts.max()),
+                   second_round_share=round(float(second.mean()), 4), mean_hops=round(float(hops.mean()), 1),
+                   mean_cmps=round(float(cmps.mean()), 1), average_precision=round(found / max(1, int(exact.sum())), 4))
+        print(json.dumps(row), flush=True)
+        rows.append(row)
+    summary = dict(gpu=name, power_limit_max_sm_clock=power, workload="c2_1Mx128_f32_l2", n=n, nq=nq, L=L, beam=args.beam,
+                   reps=args.reps, knn_batch_ms=round(knn_ms, 3), range=rows)
+    print(json.dumps(summary), flush=True)
+    if args.json:
+        os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)
+        with open(args.json, "w") as f:
+            json.dump(summary, f, indent=1)
+    g.close()
+
+
+if __name__ == "__main__":
+    main()

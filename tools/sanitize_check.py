@@ -69,6 +69,9 @@ for dt, ddt, metric, d in ((np.float32, dab.DType.f32, dab.Metric.L2, 100), (np.
         g.upload_attributes(rng.integers(0, 7, n + 1), rng.random(n + 1) < 0.9)
         div = g.search_batch_diverse(base[:64], 5, 40, 2, 1)     # diverse_kernel
         div4 = g.search_batch_diverse(base[:64], 5, 300, 1, 4)
+        rad = float(np.median(got[1][:, 4]))                     # range_kernel, range_scan, range_compact
+        rng1 = g.range_search(base[:64], 20, rad, initial_slack=0.2)
+        rng4 = g.range_search(base[:64], 10, rad * 2, beam_width=4, max_returned=70)
         knn = g.flat_knn(base[:16], 5)
         knn_tc = g.flat_knn_tc(base[:16], 5)                     # wgmma + TMA path
         assert np.array_equal(knn[0], knn_tc[0])
