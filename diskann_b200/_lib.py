@@ -53,6 +53,12 @@ SYMBOLS = {
     "dab_wait": (_i, [_vp, _u32]),
     "dab_range_search": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, C.POINTER(_vp)]),
     "dab_range_search_device": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, C.POINTER(_vp)]),
+    "dab_range_search_pq": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, _i, C.POINTER(_vp)]),
+    "dab_range_search_pq_device": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, _i, C.POINTER(_vp)]),
+    "dab_range_search_sq": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, _i, C.POINTER(_vp)]),
+    "dab_range_search_sq_device": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, _i, C.POINTER(_vp)]),
+    "dab_range_search_minmax": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, _i, C.POINTER(_vp)]),
+    "dab_range_search_minmax_device": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, _i, C.POINTER(_vp)]),
     "dab_range_offsets": (_i, [_vp, _vp, _vp, _vp, _vp]),
     "dab_range_results": (_i, [_vp, _vp, _vp]),
     "dab_range_results_device": (_i, [_vp, _vp, _vp]),

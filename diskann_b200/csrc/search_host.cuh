@@ -117,10 +117,18 @@ struct SearchOut {
 int queue_drop_deleted(const dab_index* idx, cudaStream_t stream, const uint32_t* deleted, const uint32_t* ids, const float* dists,
                        uint32_t cap, uint32_t nq, uint32_t k, const SearchOut& out, uint64_t bound);
 
+// SQ and MinMax: a batch's queries as the store's quantizer compressed them (search_pq.cuh), in the handle's staging
+// scratch until the next call that stages
+struct StagedQueries {
+    const uint8_t* codes;
+    const float4* meta;
+};
+
 // Searches whose queries are rows of the index (the build's insert searches, in-place deletes): they ignore deletions
 // and teach the visited tables nothing.  With `ids` each records the nodes it expanded; with `keep_starts` its results
 // are the list's entries with start points kept (the caller filters them).  `keep_deleted`, for queries that are not
-// rows (the first phase of range search): the results keep deleted ids too, and the caller filters them.
+// rows (the first phase of range search): the results keep deleted ids too, and the caller filters them.  `staged`
+// (NULL: not wanted) receives an SQ or MinMax batch's compressed queries, for a caller that reads them after the search.
 struct SearchRecord {
     const uint32_t* query_rows;  // [nq] row ids of the queries
     uint32_t* ids;               // [nq][cap] expanded nodes, [nq] counts (NULL: no record)
@@ -129,6 +137,7 @@ struct SearchRecord {
     uint32_t cap;
     bool keep_starts;
     bool keep_deleted;
+    StagedQueries* staged;
 };
 
 // One batch on the handle's stream and scratch, device pointers only.  `store`: -1 full precision, else the QuantStore the

@@ -3,8 +3,8 @@
 // are in search_kernel_pq.cu and search_kernel_pqs.cu), the slots of batches in flight and the C entry points
 // (dab_search_batch[_pq|_pq_rerank|_sq|_minmax][_device][_async], dab_search_batch_diverse[_pq|_sq|_minmax][_device],
 // dab_wait).  The diverse search (search_diverse.cu), over full-precision rows or a quantized store, is one more kind of
-// the job; so is the first phase of range search (search_range.cu), a full-precision batch that keeps start points and
-// deleted ids.
+// the job; so is the first phase of range search (search_range.cu), a batch over full-precision rows or a quantized
+// store that keeps start points and deleted ids.
 //
 // A full-precision batch runs on search_kernel_v3 (visited set in shared memory) where its short lists make that the
 // faster kernel, and on search_kernel_v2 (global visited tables) otherwise; queries whose visited set outgrows its table
@@ -320,7 +320,8 @@ int SlotJob::plan_quant() {
     // table metrics with a pivot table that fits shared memory: search_kernel_pqs (pivots resident per SM, entries
     // computed on the fly); everything else — SQ, MinMax, DirectCosine, wide pivots, > 32 chunks — search_kernel_pq
     memset(&plan, 0, sizeof(plan));
-    use_pqs = mode == STORE_PQ && !pq.direct_cosine && pqs_plan(idx, pq.warp_smem, nq, &plan);
+    // (a list that keeps its start points, range search's first phase, runs on search_kernel_pq_starts)
+    use_pqs = mode == STORE_PQ && !pq.direct_cosine && !rec.keep_starts && pqs_plan(idx, pq.warp_smem, nq, &plan);
     smem_block = (size_t)pq.warp_smem * kPqWarps;
     if (use_pqs) {
         pq.piv_stride = plan.piv_stride;
@@ -329,7 +330,7 @@ int SlotJob::plan_quant() {
         warps = (uint32_t)plan.grid * (uint32_t)plan.warps;
     } else {
         if (smem_block > 200 * 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_pq: configuration needs %zu B shared memory per CTA", smem_block);
-        kern = pq_kernel(cap, mode);
+        kern = pq_kernel(cap, mode, rec.keep_starts);
         int per_sm = ctas_per_sm(kern, kPqWarps * 32, smem_block);
         if (per_sm < 1) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_pq: kernel does not fit");
         // every resident warp owns a LUT (n_chunks x n_centers f32: 32 KB at 32 x 256) and a visited table in
@@ -550,6 +551,7 @@ static int run_job(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t 
     job.diverse_k = diverse_k;
     job.pools = &idx->s_pools;
     if ((rc = job.prepare(d_queries, nq, k, l_search, beam, d, store, rerank, rec)) || (rc = job.stage_queries())) return rc;
+    if (rec && rec->staged && store >= 0) *rec->staged = StagedQueries{job.pq.query_codes, job.pq.query_meta};
     if (store == STORE_MINMAX) {  // a batch with a NaN query fails before any traversal is launched
         DAB_CUDA(cudaStreamSynchronize(idx->stream));
         if (job.first_nan() != ~0ull) return job.nan_error();

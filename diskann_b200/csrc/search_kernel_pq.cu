@@ -40,8 +40,10 @@
 
 namespace dab {
 
-template <int QT, int MODE>
-__global__ void __launch_bounds__(kPqWarps * 32) search_kernel_pq(const SearchParamsPq p) {
+// One warp's share of a pass.  KEEP_STARTS: the results are the list's first k entries with start points kept (the
+// first phase of range search, which filters them itself).
+template <int QT, int MODE, bool KEEP_STARTS>
+__device__ __forceinline__ void pq_queries(const SearchParamsPq& p) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     uint8_t* base = smem + (size_t)wib * p.warp_smem;
@@ -145,9 +147,19 @@ __global__ void __launch_bounds__(kPqWarps * 32) search_kernel_pq(const SearchPa
         }
         const uint32_t n = min(p.cap, size);
         if (p.list_ids) write_list(qi, n, p.list_ids, p.list_counts, p.list_cap, qidx, lane);
-        const uint32_t count = write_results(qi, qd, n, p.n_points, p.k, p.out_ids, p.out_dists, qidx, lane);
+        const uint32_t count = write_results(qi, qd, n, KEEP_STARTS ? n_total : p.n_points, p.k, p.out_ids, p.out_dists, qidx, lane);
         write_stats(p.counters, nvisited, p.out_counts, p.out_cmps, p.out_hops, qidx, count, cmps, hops, lane);
     }
+}
+
+template <int QT, int MODE>
+__global__ void __launch_bounds__(kPqWarps * 32) search_kernel_pq(const SearchParamsPq p) {
+    pq_queries<QT, MODE, false>(p);
+}
+
+template <int QT, int MODE>
+__global__ void __launch_bounds__(kPqWarps * 32) search_kernel_pq_starts(const SearchParamsPq p) {
+    pq_queries<QT, MODE, true>(p);
 }
 
 // ---- Rerank (diskann-providers/.../inmem/full_precision.rs:356-399 behind FilterStartPoints,
@@ -179,7 +191,6 @@ struct RerankParams {
 template <typename TD, int KIND, int POST, int NA = 4>
 __global__ void __launch_bounds__(kRerankWarps * 32) rerank_kernel(const RerankParams p) {
     extern __shared__ __align__(16) uint8_t smem[];
-    constexpr bool kInt = std::is_same<TD, int8_t>::value || std::is_same<TD, uint8_t>::value;
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     uint8_t* base = smem + (size_t)wib * p.warp_smem;
     float* qf = reinterpret_cast<float*>(base);
@@ -200,28 +211,7 @@ __global__ void __launch_bounds__(kRerankWarps * 32) rerank_kernel(const RerankP
             m += __popc(mk);
         }
         __syncwarp();
-        if constexpr (kInt) {
-            int qq = 0;
-            if (KIND != KIND_IP) qq = warp_int_self<std::is_same<TD, int8_t>::value>(reinterpret_cast<const uint8_t*>(qf), dim, lane);
-            wide_distances_int<std::is_same<TD, int8_t>::value, KIND, POST, 4>(reinterpret_cast<const uint8_t*>(qf), qq, p.vectors, p.row_stride,
-                                                                             cid, m, cd, dim, lane);
-        } else if constexpr (NA == 2) {
-            constexpr int S = 16, U = 2;
-            const int team = lane / S, slot = lane % S;
-            for (uint32_t c0 = 0; c0 < m; c0 += 2 * U) {  // every lane takes part in the team shuffles: uniform trip count
-                const TD* rows[U];
-#pragma unroll
-                for (int u = 0; u < U; ++u)
-                    rows[u] = reinterpret_cast<const TD*>(p.vectors + (size_t)cid[min(c0 + team * U + u, m - 1)] * p.row_stride);
-                float r[U];
-                team_float_multi<2, KIND, U>(qf, rows, dim, slot, r);
-#pragma unroll
-                for (int u = 0; u < U; ++u)
-                    if (slot == 0 && c0 + team * U + u < m) cd[c0 + team * U + u] = post_op<POST>(r[u]);
-            }
-        } else {
-            wide_distances<TD, KIND, POST, 2, 4>(qf, p.vectors, p.row_stride, cid, m, cd, dim, lane);
-        }
+        rerank_distances<TD, KIND, POST, NA>(qf, p.vectors, p.row_stride, cid, m, cd, dim, lane);
         __syncwarp();
         for (uint32_t i = lane; i < m; i += 32) {
             const float di = cd[i];
@@ -294,9 +284,13 @@ int launch_rerank(const dab_index* idx, cudaStream_t stream, const void* d_queri
     return DAB_OK;
 }
 
-PqKernel pq_kernel(uint32_t cap, QuantStore store) {
-    return visit_list_tile(cap, [&](auto qt) {
+PqKernel pq_kernel(uint32_t cap, QuantStore store, bool keep_starts) {
+    return visit_list_tile(cap, [&](auto qt) -> PqKernel {
         constexpr int QT = decltype(qt)::value;
+        if (keep_starts)
+            return store == STORE_MINMAX ? search_kernel_pq_starts<QT, STORE_MINMAX>
+                   : store == STORE_SQ  ? search_kernel_pq_starts<QT, STORE_SQ>
+                                        : search_kernel_pq_starts<QT, STORE_PQ>;
         return store == STORE_MINMAX ? search_kernel_pq<QT, STORE_MINMAX> : store == STORE_SQ ? search_kernel_pq<QT, STORE_SQ> : search_kernel_pq<QT, STORE_PQ>;
     });
 }

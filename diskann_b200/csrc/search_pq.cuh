@@ -59,8 +59,9 @@ struct SearchParamsPq {
 
 // search_kernel_pq.cu
 using PqKernel = void (*)(const SearchParamsPq);
-// search_kernel_pq's instantiation for lists of `cap` entries over `store`
-PqKernel pq_kernel(uint32_t cap, QuantStore store);
+// search_kernel_pq's instantiation for lists of `cap` entries over `store`; `keep_starts`: the one whose results keep
+// start points (search_kernel_pq_starts)
+PqKernel pq_kernel(uint32_t cap, QuantStore store, bool keep_starts = false);
 // The rerank of lists of list_cap entries fits a CTA of this index's schema
 int check_rerank(const dab_index* idx, uint32_t list_cap);
 // Reranks each query's list (d_list [nq][list_cap], d_list_n [nq]) by full-precision distance, the start points and the ids

@@ -1,10 +1,12 @@
 // search_range.cu — batched range search on the device: Range::search and range_search_internal
-// (diskann/src/graph/search/range_search.rs:255-469) over full-precision rows, and the result sets it returns
-// (dab_range_search[_device], dab_range_offsets, dab_range_results[_device], dab_range_free).
+// (diskann/src/graph/search/range_search.rs:255-469) over full-precision rows or the PQ, SQ and MinMax stores, and the
+// result sets it returns (dab_range_search[_pq|_sq|_minmax][_device], dab_range_offsets, dab_range_results[_device],
+// dab_range_free).
 //
-// Phase 1 is the k-NN traversal at L (search_kernel_v3 / _v2 through run_search, unchanged): with k = L and start
-// points and deleted ids kept, it writes each query's first L list entries, its cmps and its hops.  Phase 2 is
-// range_kernel, one warp per query on global visited tables:
+// Phase 1 is the k-NN traversal at L through run_search (search_kernel_v3 / _v2 over full-precision rows,
+// search_kernel_pq_starts over a store): with k = L and start points and deleted ids kept, it writes each query's first
+// L list entries, its cmps and its hops.  Phase 2 is range_kernel (full precision) or range_kernel_quant (the store's
+// distances, those of its k-NN traversal), one warp per query on global visited tables:
 //   in_range  the phase-1 entries with distance <= radius, in list order, in the warp's region of global memory;
 //   round 2   iff |in_range| >= (f32(L) * initial_slack) as usize and |in_range| < max_returned: the visited table is
 //             cleared and re-seeded with the in_range ids, and the frontier, the unconsumed suffix of in_range, is
@@ -12,6 +14,12 @@
 //             is appended while |in_range| < max_returned (the cap may cut a hop short);
 //   output    in_range in insertion order without start points, deleted ids, ids with d <= inner_radius (when given)
 //             and ids with d > radius.
+// Every distance of both phases is the store's, so over a store the output compares the store's distances.  With
+// rerank, the quantized strategies' Pipeline<FilterStartPoints, Rerank> (providers inmem/product.rs:391-401,
+// full_precision.rs:356-399) runs instead over each query's in_range: start points and deleted ids dropped, every other
+// id's full-precision Distance<T, T> to the query (range_rerank_kernel, the rerank_kernel schemas), the entries outside
+// (inner_radius, radius] of that distance dropped, and the rest sorted by it, stably (ties in in_range order, -0.0 equal
+// to +0.0; the reference's sort_unstable_by leaves ties unspecified, and NaN has been filtered out before the sort).
 // The hops of a query that took the second round are phase1 + (phase1 + phase2), as the reference adds its cumulative
 // scratch.hops to phase 1's; cmps are phase 1's.  A hop's nodes are expanded, scored and appended one node at a time:
 // the visited inserts and the appends come in the reference's order, and nothing after the cap is observable.
@@ -23,8 +31,13 @@
 // arena has been extended by exactly what those queries need.  A scan and a compaction then lay the results out in
 // query order in the result set, which owns its memory: later writes to the index do not change it.
 #include "dab_common.cuh"
+#include "quant_device.cuh"
 #include "search_common.cuh"
 #include "search_host.cuh"
+#include "search_pq.cuh"
+#include "search_smem.cuh"
+
+#include <cub/device/device_segmented_sort.cuh>
 
 #include <algorithm>
 
@@ -92,16 +105,33 @@ struct RangeParams {
     uint32_t *q_count, *out_hops;
     uint8_t* out_second;
     uint32_t warp_smem, off_cid, off_cd;
+    // the quantized stores (range_kernel_quant), named as in SearchParamsPq for the per-candidate code
+    // (quant_device.cuh).  Fields of the full-precision kernel come first, so that its parameter offsets stay as they were.
+    int dtype;
+    const float* pivots;  // PQ: the table, [n_centers][dim]
+    const uint32_t* offsets;
+    const uint8_t* codes;  // [n_total][n_chunks]
+    uint32_t n_chunks, n_centers;
+    int ip_table, direct_cosine;
+    float* luts;  // PQ tables (TableL2 / TableIP): n_chunks x n_centers f32 for every resident warp
+    const uint8_t* row_codes;  // SQ / MinMax: the store's rows and the batch's staged queries
+    const float* row_meta;
+    uint32_t code_stride, code_dim;
+    int code_nbits, code_metric;
+    float sq_scale_squared, sq_shift_square_norm;
+    const uint8_t* query_codes;  // [nq][code_stride]
+    const float4* query_meta;    // [nq]
+    int rerank;  // the output keeps every in_range id but start points and deleted ids, for range_rerank
 };
 
-// One warp per query of the pass's work list
-template <typename TD, int KIND, int POST, int NA>
-__global__ void __launch_bounds__(kRangeWarps * 32) range_kernel(const RangeParams p) {
-    constexpr bool INT = std::is_same<TD, int8_t>::value || std::is_same<TD, uint8_t>::value;
-    extern __shared__ __align__(128) uint8_t smem[];
-    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    uint8_t* base = smem + (size_t)wib * p.warp_smem;
-    float* qf = reinterpret_cast<float*>(base);
+// One warp's share of a pass: the queries of the work list it takes, whatever the distances are.  Src is the distance
+// source: load(q) brings query q into the front of the warp's shared memory, prepare() runs once the visited table is
+// cleared (what the distances need of the loaded query), and distances(cid, cd, n) writes the distances of cid[0..n)
+// into cd[0..n) and ends with the warp converged.  radius_filter: the output drops the ids outside (inner_radius,
+// radius]; without it only start points and deleted ids are dropped (the rerank filters on its own distances).
+template <class Src>
+__device__ __forceinline__ void range_queries(const RangeParams& p, uint8_t* base, int lane, Src& src, bool radius_filter) {
+    const int wib = threadIdx.x >> 5;
     uint32_t* cid = reinterpret_cast<uint32_t*>(base + p.off_cid);
     float* cd = reinterpret_cast<float*>(base + p.off_cd);
     const uint32_t warp_slot = blockIdx.x * kRangeWarps + wib;
@@ -111,7 +141,6 @@ __global__ void __launch_bounds__(kRangeWarps * 32) range_kernel(const RangePara
     const uint64_t n_total = p.n_points + p.n_start;
     uint32_t* rid = p.regions + (size_t)warp_slot * p.region_cap * 2;
     float* rd = reinterpret_cast<float*>(rid + p.region_cap);
-    const int dim = (int)p.dim;
     const unsigned below = (1u << lane) - 1u;
 
     for (uint32_t qidx; next_query(p.counters, p.n_work, p.query_list, lane, qidx);) {
@@ -136,13 +165,10 @@ __global__ void __launch_bounds__(kRangeWarps * 32) range_kernel(const RangePara
 
         if (second && !overflow) {
             // ---- range_search_internal: the visited set is the in_range ids, the frontier the suffix not yet expanded
-            load_query(reinterpret_cast<const TD*>(p.queries) + (size_t)qidx * dim, dim, 4, qf, lane);
+            src.load(qidx);
             for (uint32_t i = lane; i < nbk; i += 32) store_empty_bucket(table + (size_t)i * 8);
             __syncwarp();
-            int qq = 0;  // integer rows: Sum x^2 of the query (unused by inner product)
-            if constexpr (INT) {
-                if (KIND != KIND_IP) qq = warp_int_self<std::is_same<TD, int8_t>::value>(reinterpret_cast<const uint8_t*>(qf), dim, lane);
-            }
+            src.prepare();
             for (uint32_t i = lane; i < size; i += 32) visit_global(table, nbk, rid[i]);
             __syncwarp();  // every seed is in the table before any lane probes it for a neighbour
             nvisited = (uint32_t)size;
@@ -171,28 +197,7 @@ __global__ void __launch_bounds__(kRangeWarps * 32) range_kernel(const RangePara
                         break;
                     }
                     __syncwarp();
-                    // the distances of the shared schemas (distance_device.cuh), a team of lanes per row
-                    {
-                        constexpr int S = INT ? 32 : 8 * NA, TEAMS = 32 / S, U = kRangeRows;
-                        using Row = typename std::conditional<INT, uint8_t, TD>::type;
-                        const int team = lane / S, slot = lane % S;
-                        for (uint32_t c0 = 0; c0 < ncand; c0 += TEAMS * U) {
-                            float r[U];
-                            uint32_t cc[U];
-                            const Row* rows[U];
-#pragma unroll
-                            for (int u = 0; u < U; ++u) {
-                                cc[u] = c0 + u * TEAMS + team;
-                                rows[u] = reinterpret_cast<const Row*>(p.vectors + (size_t)cid[min(cc[u], ncand - 1)] * p.row_stride);
-                            }
-                            if constexpr (INT) warp_int_multi<std::is_same<TD, int8_t>::value, KIND, U>(reinterpret_cast<const uint8_t*>(qf), rows, dim, lane, qq, r);
-                            else team_float_multi<NA, KIND, U>(qf, rows, dim, slot, r);
-#pragma unroll
-                            for (int u = 0; u < U; ++u)
-                                if (slot == 0 && cc[u] < ncand) cd[cc[u]] = post_op<POST>(r[u]);
-                        }
-                        __syncwarp();
-                    }
+                    src.distances(cid, cd, ncand);
                     // the appends, in order, while in_range is below max_returned
                     for (uint32_t c0 = 0; c0 < ncand && size < p.max_returned; c0 += 32) {
                         const uint32_t c = c0 + lane;
@@ -228,6 +233,7 @@ __global__ void __launch_bounds__(kRangeWarps * 32) range_kernel(const RangePara
             const float d = rd[i];
             if (id >= p.n_points) return false;
             if (p.deleted && (__ldg(p.deleted + (id >> 5)) >> (id & 31) & 1u)) return false;
+            if (!radius_filter) return true;
             if (p.has_inner && d <= p.inner_radius) return false;
             return d <= p.radius;
         };
@@ -269,6 +275,92 @@ __global__ void __launch_bounds__(kRangeWarps * 32) range_kernel(const RangePara
             p.out_second[qidx] = second ? 1 : 0;
         }
     }
+}
+
+// Full precision: rows from global memory with the shared distance schemas (distance_device.cuh), a team of lanes per row
+template <typename TD, int KIND, int POST, int NA>
+__global__ void __launch_bounds__(kRangeWarps * 32) range_kernel(const RangeParams p) {
+    constexpr bool INT = std::is_same<TD, int8_t>::value || std::is_same<TD, uint8_t>::value;
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    uint8_t* base = smem + (size_t)wib * p.warp_smem;
+    struct {
+        const RangeParams& p;
+        float* qf;
+        int lane, dim, qq;  // qq, integer rows: Sum x^2 of the query (unused by inner product)
+        __device__ __forceinline__ void load(uint32_t q) { load_query(reinterpret_cast<const TD*>(p.queries) + (size_t)q * dim, dim, 4, qf, lane); }
+        __device__ __forceinline__ void prepare() {
+            if constexpr (INT) {
+                if (KIND != KIND_IP) qq = warp_int_self<std::is_same<TD, int8_t>::value>(reinterpret_cast<const uint8_t*>(qf), dim, lane);
+            }
+        }
+        __device__ __forceinline__ void distances(const uint32_t* cid, float* cd, uint32_t n) {
+            constexpr int S = INT ? 32 : 8 * NA, TEAMS = 32 / S, U = kRangeRows;
+            using Row = typename std::conditional<INT, uint8_t, TD>::type;
+            const int team = lane / S, slot = lane % S;
+            for (uint32_t c0 = 0; c0 < n; c0 += TEAMS * U) {
+                float r[U];
+                uint32_t cc[U];
+                const Row* rows[U];
+#pragma unroll
+                for (int u = 0; u < U; ++u) {
+                    cc[u] = c0 + u * TEAMS + team;
+                    rows[u] = reinterpret_cast<const Row*>(p.vectors + (size_t)cid[min(cc[u], n - 1)] * p.row_stride);
+                }
+                if constexpr (INT) warp_int_multi<std::is_same<TD, int8_t>::value, KIND, U>(reinterpret_cast<const uint8_t*>(qf), rows, dim, lane, qq, r);
+                else team_float_multi<NA, KIND, U>(qf, rows, dim, slot, r);
+#pragma unroll
+                for (int u = 0; u < U; ++u)
+                    if (slot == 0 && cc[u] < n) cd[cc[u]] = post_op<POST>(r[u]);
+            }
+            __syncwarp();
+        }
+    } src{p, reinterpret_cast<float*>(base), lane, (int)p.dim, 0};
+    range_queries(p, base, lane, src, true);
+}
+
+// The quantized accessors (MODE as search_kernel_pq: 0 PQ, 1 SQ, 2 MinMax), per candidate the code of quant_device.cuh,
+// one lane per candidate: the traversal distances of dab_search_batch_{pq,sq,minmax}.
+//   PQ: the query (index dtype, T: Into<f32>) in f32 at the front of the warp's shared memory; TableL2 / TableIP build
+//     the query's table once per query into the warp's own slice of p.luts (global memory, read through L2),
+//     DirectCosine reads the pivots directly.
+//   SQ / MinMax: the query's code words (and MinMax its four compensations), staged before phase 1, copied to the front
+//     of the warp's shared memory; the SQ compensation stays in a register.
+template <int MODE>
+__global__ void __launch_bounds__(kRangeWarps * 32) range_kernel_quant(const RangeParams p) {
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    uint8_t* base = smem + (size_t)wib * p.warp_smem;
+    const uint32_t entries = p.n_chunks * p.n_centers;
+    struct {
+        const RangeParams& p;
+        float* qf;     // PQ: the f32 query
+        uint32_t* qc;  // SQ / MinMax: the query's code words, then (MinMax) {b, n, a, norm_squared}
+        float* lut;    // PQ tables: this warp's table
+        int lane, dim;
+        uint32_t entries;
+        float q_comp;
+        __device__ __forceinline__ void load(uint32_t q) {
+            if (MODE == 0) widen_query(p.dtype, p.queries, q, dim, qf, lane);
+            else load_query_codes<MODE>(p.query_codes + (size_t)q * p.code_stride, p.query_meta + q, p.code_stride >> 2, qc, q_comp, lane);
+        }
+        __device__ __forceinline__ void prepare() {
+            if (MODE == 0 && !p.direct_cosine) {
+                for (uint32_t t = lane; t < entries; t += 32) __stcg(lut + t, pq_table_entry(p, qf, dim, t));
+                __syncwarp();
+            }
+        }
+        __device__ __forceinline__ void distances(const uint32_t* cid, float* cd, uint32_t n) {
+            for (uint32_t c = lane; c < n; c += 32) {
+                if (MODE != 0) cd[c] = packed_code_distance<MODE>(p, qc, q_comp, cid[c]);
+                else if (p.direct_cosine) cd[c] = pq_direct_cosine(p, qf, dim, cid[c]);
+                else cd[c] = pq_table_distance(p, lut, cid[c]);
+            }
+            __syncwarp();
+        }
+    } src{p, reinterpret_cast<float*>(base), reinterpret_cast<uint32_t*>(base),
+          p.luts + (size_t)(blockIdx.x * kRangeWarps + wib) * entries, lane, (int)p.dim, entries, 0.0f};
+    range_queries(p, base, lane, src, !p.rerank);
 }
 
 // offsets [nq + 1] <- the exclusive prefix sums of counts, by one block of 1024 threads
@@ -313,16 +405,106 @@ __global__ void range_compact(const uint64_t* q_pos, const uint32_t* q_count, co
     }
 }
 
+// ---- the rerank: full-precision distances in place, the radius filter, a stable sort per query --------------------
+constexpr int kRangeRerankWarps = 4;
+
+struct RangeRerankParams {
+    const uint8_t* vectors;
+    size_t row_stride;
+    uint32_t dim, nq;
+    const void* queries;  // index dtype
+    const uint64_t* offsets;  // [nq + 1]: query q's results are ids / dists [offsets[q], offsets[q + 1])
+    const uint32_t* ids;
+    float* dists;
+    float radius, inner_radius;
+    int has_inner;
+    uint32_t* counts;  // [nq] results within (inner_radius, radius]
+    uint32_t warp_smem;
+};
+
+__device__ __forceinline__ bool in_band(float d, float radius, int has_inner, float inner_radius) {
+    return !(has_inner && d <= inner_radius) && d <= radius;
+}
+
+// One warp per query: every result's Distance<T, T> to the query written over its quantized distance, and how many lie
+// within (inner_radius, radius]
+template <typename TD, int KIND, int POST, int NA>
+__global__ void __launch_bounds__(kRangeRerankWarps * 32) range_rerank_kernel(const RangeRerankParams p) {
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    float* qf = reinterpret_cast<float*>(smem + (size_t)wib * p.warp_smem);
+    for (uint32_t q = blockIdx.x * kRangeRerankWarps + wib; q < p.nq; q += gridDim.x * kRangeRerankWarps) {
+        const uint64_t b = p.offsets[q];
+        const uint32_t m = (uint32_t)(p.offsets[q + 1] - b);
+        uint32_t count = 0;
+        if (m) {
+            __syncwarp();
+            load_query(reinterpret_cast<const TD*>(p.queries) + (size_t)q * p.dim, (int)p.dim, 16, qf, lane);
+            __syncwarp();
+            rerank_distances<TD, KIND, POST, NA>(qf, p.vectors, p.row_stride, p.ids + b, m, p.dists + b, (int)p.dim, lane);
+            __syncwarp();
+            for (uint32_t i = lane; i < m; i += 32) count += in_band(p.dists[b + i], p.radius, p.has_inner, p.inner_radius) ? 1u : 0u;
+            count = __reduce_add_sync(kFull, count);
+        }
+        if (lane == 0) p.counts[q] = count;
+    }
+}
+
+// An f32 distance as a u32 key of the same order, -0.0 and +0.0 one key (no NaN reaches the sort)
+__device__ __forceinline__ uint32_t sort_key(float d) {
+    const uint32_t b = __float_as_uint(d == 0.0f ? 0.0f : d);
+    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+
+// One warp per query: the results within (inner_radius, radius], in order, from [from[q], from[q + 1]) to
+// [to[q], to[q + 1]) of ids / dists, with their sort keys and their positions
+__global__ void range_rerank_filter(const uint64_t* from, const uint64_t* to, uint32_t nq, const uint32_t* ids, const float* dists, float radius,
+                                    int has_inner, float inner_radius, uint32_t* out_ids, float* out_dists, uint32_t* keys, uint32_t* pos) {
+    const int lane = threadIdx.x & 31;
+    const unsigned below = (1u << lane) - 1u;
+    const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x >> 5);
+    for (uint64_t q = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5; q < nq; q += warps) {
+        const uint64_t b = from[q], e = from[q + 1];
+        uint64_t w = to[q];
+        for (uint64_t i0 = b; i0 < e; i0 += 32) {
+            const uint64_t i = i0 + lane;
+            const float d = i < e ? dists[i] : 0.0f;
+            const bool k = i < e && in_band(d, radius, has_inner, inner_radius);
+            const unsigned m = __ballot_sync(kFull, k);
+            if (k) {
+                const uint64_t at = w + __popc(m & below);
+                out_ids[at] = ids[i];
+                out_dists[at] = d;
+                keys[at] = sort_key(d);
+                pos[at] = (uint32_t)at;
+            }
+            w += __popc(m);
+        }
+    }
+}
+
+// out[i] <- in[pos[i]], ids and dists
+__global__ void range_rerank_gather(const uint32_t* pos, uint64_t n, const uint32_t* in_ids, const float* in_dists, uint32_t* out_ids,
+                                    float* out_dists) {
+    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        out_ids[i] = in_ids[pos[i]];
+        out_dists[i] = in_dists[pos[i]];
+    }
+}
+
 template <typename S>
 void (*range_kernel_of())(const RangeParams) {
     return range_kernel<typename S::TD, S::KIND, S::POST, S::NA>;
 }
 
-// A warp's shared memory: the query (i8 / u8: its bytes rounded up to 16; floats: dim f32), then one node's candidate
-// ids and distances
-size_t range_warp_smem(const dab_index* idx, RangeParams* p) {
+// A warp's shared memory: the query area, then one node's candidate ids and distances.  The query area is the query
+// itself over full-precision rows (i8 / u8: its bytes rounded up to 16; floats: dim f32), the f32 query for PQ, and the
+// query's code row plus 16 bytes of compensations for SQ and MinMax.  `store`: -1 full precision, else a QuantStore.
+size_t range_warp_smem(const dab_index* idx, int store, RangeParams* p) {
     const bool is_int = idx->dtype == DAB_I8 || idx->dtype == DAB_U8;
-    size_t off = is_int ? round_up(round_up((size_t)idx->dim, 4), 16) : round_up((size_t)idx->dim * 4, 16);
+    size_t off;
+    if (store == STORE_SQ || store == STORE_MINMAX) off = round_up((size_t)(store == STORE_SQ ? idx->sq : idx->mm).stride + 16, 16);
+    else off = is_int && store < 0 ? round_up(round_up((size_t)idx->dim, 4), 16) : round_up((size_t)idx->dim * 4, 16);
     const size_t ncand = round_up(std::max<size_t>(idx->max_degree, 32) * 4, 16);
     RangeParams scratch;
     RangeParams& q = p ? *p : scratch;
@@ -331,10 +513,19 @@ size_t range_warp_smem(const dab_index* idx, RangeParams* p) {
     return round_up(off, 128);
 }
 
-// The range search's own checks, after Range::validate_and_create's (range_search.rs:91-131) in its order
-int check_range_args(const dab_index* idx, const char* api, uint32_t l_search, uint32_t beam, float radius, int has_inner, float inner_radius,
-                     float initial_slack, float range_slack, uint64_t max_returned) {
-    if (!idx->graph_ready || !idx->vectors_ready) return fail(DAB_ERR_NOT_READY, "%s: vectors and graph must be uploaded first", api);
+// range_rerank_kernel's shared memory per warp: the query (i8 / u8 rows: as they are; float rows: f32)
+size_t range_rerank_smem(const dab_index* idx) {
+    const bool is_int = idx->dtype == DAB_I8 || idx->dtype == DAB_U8;
+    return is_int ? round_up((size_t)idx->dim, 16) : round_up((size_t)idx->dim * 4, 16);
+}
+
+// The range search's own checks, after Range::validate_and_create's (range_search.rs:91-131) in its order.  Over a
+// quantized store (`store` >= 0) the traversal reads the graph and the store only; the store checks of its k-NN call
+// follow, then those of the rerank.
+int check_range_args(const dab_index* idx, const char* api, int store, bool rerank, uint32_t l_search, uint32_t beam, float radius,
+                     int has_inner, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned) {
+    if (store < 0 && (!idx->graph_ready || !idx->vectors_ready)) return fail(DAB_ERR_NOT_READY, "%s: vectors and graph must be uploaded first", api);
+    if (store >= 0 && !idx->graph_ready) return fail(DAB_ERR_NOT_READY, "%s: graph must be uploaded first", api);
     if (beam == 0) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: beam_width must be > 0 (BeamWidthZero)", api);
     if (l_search == 0) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: l_search must be > 0 (LZero)", api);
     if (max_returned != 0 && max_returned < l_search)
@@ -346,10 +537,20 @@ int check_range_args(const dab_index* idx, const char* api, uint32_t l_search, u
     if (has_inner && inner_radius > radius)
         return fail(DAB_ERR_INVALID_ARGUMENT, "%s: inner_radius %g must be <= radius %g (InnerRadiusValueError)", api, (double)inner_radius, (double)radius);
     if (beam > 64) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: beam_width %u > 64", api, beam);
-    const size_t smem = range_warp_smem(idx, nullptr) * kRangeWarps;
+    const size_t smem = range_warp_smem(idx, store, nullptr) * kRangeWarps;
     if (smem > kRangeMaxSmem)
         return fail(DAB_ERR_INVALID_ARGUMENT, "%s: dim=%u, max_degree=%u need %zu B shared memory per CTA (> %zu)", api, idx->dim, idx->max_degree,
                     smem, kRangeMaxSmem);
+    if (store < 0) return DAB_OK;
+    int rc;
+    if ((rc = check_quant_store(idx, (QuantStore)store, api, false))) return rc;
+    if (l_search + idx->n_start > 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: L + #start must be <= 1024", api);
+    if (rerank) {
+        if (!idx->vectors_ready) return fail(DAB_ERR_NOT_READY, "%s: rerank needs the full-precision vectors", api);
+        const size_t rsmem = range_rerank_smem(idx) * kRangeRerankWarps;
+        if (rsmem > kRangeMaxSmem) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: dim=%u needs %zu B shared memory per CTA in the rerank (> %zu)", api,
+                                                idx->dim, rsmem, kRangeMaxSmem);
+    }
     return DAB_OK;
 }
 
@@ -374,9 +575,91 @@ void range_free(dab_range* r) {
     delete r;
 }
 
-// Both phases for nq >= 1 queries (checks passed) into a new result set
+// The rerank of a result set whose results are every in_range id but start points and deleted ids: their full-precision
+// distances, then those within (inner_radius, radius] sorted per query by that distance, stably
+int range_rerank(dab_index* idx, const char* api, const void* d_queries, uint32_t nq, float radius, int has_inner, float inner_radius,
+                 dab_range* r) {
+    cudaStream_t st = idx->stream;
+    int rc;
+    DevBuf counts, offsets;
+    if ((rc = counts.alloc((size_t)nq * 4, api)) || (rc = offsets.alloc(((size_t)nq + 1) * 8, api))) return rc;
+    RangeRerankParams p;
+    memset(&p, 0, sizeof(p));
+    p.vectors = idx->d_vectors;
+    p.row_stride = idx->row_stride;
+    p.dim = idx->dim;
+    p.nq = nq;
+    p.queries = d_queries;
+    p.offsets = r->offsets();
+    p.ids = (const uint32_t*)r->d_results;
+    p.dists = (float*)((uint32_t*)r->d_results + r->total);
+    p.radius = radius;
+    p.inner_radius = inner_radius;
+    p.has_inner = has_inner ? 1 : 0;
+    p.counts = (uint32_t*)counts.p;
+    p.warp_smem = (uint32_t)range_rerank_smem(idx);
+    const size_t smem = (size_t)p.warp_smem * kRangeRerankWarps;
+    const int grid = (int)std::min<uint64_t>(((uint64_t)nq + kRangeRerankWarps - 1) / kRangeRerankWarps, (uint64_t)idx->sm_count * 8);
+    if ((rc = visit_schema<OPS_ROW>(idx->dtype, idx->metric, [&](auto sc) -> int {
+             using S = decltype(sc);
+             auto kern = range_rerank_kernel<typename S::TD, S::KIND, S::POST, S::NA>;
+             DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+             kern<<<grid, kRangeRerankWarps * 32, smem, st>>>(p);
+             return DAB_OK;
+         })))
+        return rc;
+    DAB_LAUNCHED();
+    DAB_CUDA(cudaGetLastError());
+    range_scan<<<1, 1024, 0, st>>>(p.counts, nq, (uint64_t*)offsets.p);
+    DAB_LAUNCHED();
+    DAB_CUDA(cudaGetLastError());
+    uint64_t total = 0;
+    DAB_CUDA(cudaMemcpyAsync(&total, (uint64_t*)offsets.p + nq, 8, cudaMemcpyDeviceToHost, st));
+    DAB_CUDA(cudaStreamSynchronize(st));
+
+    // the filtered results with their keys and positions, then the sort (CUB counts its items in int)
+    DevBuf kept, keys, out;
+    if (total > (uint64_t)INT32_MAX)
+        return fail(DAB_ERR_OUT_OF_MEMORY, "%s: the rerank sorts %llu entries, more than %d", api, (unsigned long long)total, INT32_MAX);
+    if ((rc = alloc_entries(idx, api, kept, total, total)) || (rc = alloc_entries(idx, api, keys, 2 * total, total)) ||
+        (rc = alloc_entries(idx, api, out, total, total)))
+        return rc;
+    uint32_t* kept_ids = (uint32_t*)kept.p;
+    float* kept_dists = (float*)(kept_ids + total);
+    uint32_t* k_in = (uint32_t*)keys.p;
+    uint32_t* v_in = k_in + total;
+    uint32_t* k_out = v_in + total;
+    uint32_t* v_out = k_out + total;
+    range_rerank_filter<<<grid_for(idx, (uint64_t)nq * 32), 256, 0, st>>>(r->offsets(), (const uint64_t*)offsets.p, nq, p.ids, p.dists, radius,
+                                                                          p.has_inner, inner_radius, kept_ids, kept_dists, k_in, v_in);
+    DAB_LAUNCHED();
+    DAB_CUDA(cudaGetLastError());
+    if (total) {
+        const uint64_t* seg = (const uint64_t*)offsets.p;
+        size_t tmp_bytes = 0;
+        DAB_CUDA(cub::DeviceSegmentedSort::StableSortPairs(nullptr, tmp_bytes, k_in, k_out, v_in, v_out, (int)total, (int)nq, seg, seg + 1, st));
+        DevBuf tmp;
+        if ((rc = tmp.alloc(tmp_bytes, api))) return rc;
+        DAB_CUDA(cub::DeviceSegmentedSort::StableSortPairs(tmp.p, tmp_bytes, k_in, k_out, v_in, v_out, (int)total, (int)nq, seg, seg + 1, st));
+        DAB_LAUNCHED();
+        range_rerank_gather<<<grid_for(idx, total), 256, 0, st>>>(v_out, total, kept_ids, kept_dists, (uint32_t*)out.p,
+                                                                  (float*)((uint32_t*)out.p + total));
+        DAB_LAUNCHED();
+        DAB_CUDA(cudaGetLastError());
+    }
+    DAB_CUDA(cudaMemcpyAsync(r->offsets(), offsets.p, ((size_t)nq + 1) * 8, cudaMemcpyDeviceToDevice, st));
+    DAB_CUDA(cudaStreamSynchronize(st));
+    cudaFree(r->d_results);
+    r->d_results = out.p;
+    out.p = nullptr;
+    r->total = total;
+    return DAB_OK;
+}
+
+// Both phases for nq >= 1 queries (checks passed) into a new result set: over full-precision rows (`store` -1) or a
+// QuantStore, whose results `rerank` reorders by full-precision distance
 int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t nq, uint32_t l_search, uint32_t beam, float radius, int has_inner,
-              float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, dab_range* r) {
+              float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, int store, bool rerank, dab_range* r) {
     cudaStream_t st = idx->stream;
     int rc;
     // ---- the result set's statistics, then phase 1: the first L entries of every list with start points and
@@ -393,23 +676,43 @@ int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t n
     SearchRecord rec{};
     rec.keep_starts = true;
     rec.keep_deleted = true;
-    if ((rc = run_search(idx, d_queries, nq, l_search, l_search, beam, SearchOut{list_ids, list_dists, list_counts, r->cmps(), list_hops}, -1,
+    StagedQueries staged{};  // SQ / MinMax: the queries phase 1 compressed, which phase 2 reads too
+    rec.staged = &staged;
+    if ((rc = run_search(idx, d_queries, nq, l_search, l_search, beam, SearchOut{list_ids, list_dists, list_counts, r->cmps(), list_hops}, store,
                          false, &rec)))
         return rc;
 
     // ---- phase 2
     RangeParams p;
     memset(&p, 0, sizeof(p));
-    p.warp_smem = (uint32_t)range_warp_smem(idx, &p);
+    p.warp_smem = (uint32_t)range_warp_smem(idx, store, &p);
     const size_t smem_block = (size_t)p.warp_smem * kRangeWarps;
     void (*kern)(const RangeParams) = nullptr;
-    visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) -> int {
-        kern = range_kernel_of<decltype(sc)>();
-        return DAB_OK;
-    });
-    const int per_sm = ctas_per_sm(kern, kRangeWarps * 32, smem_block);
+    if (store >= 0) {
+        kern = store == STORE_PQ ? range_kernel_quant<0> : store == STORE_SQ ? range_kernel_quant<1> : range_kernel_quant<2>;
+    } else {
+        visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) -> int {
+            kern = range_kernel_of<decltype(sc)>();
+            return DAB_OK;
+        });
+    }
+    int per_sm = ctas_per_sm(kern, kRangeWarps * 32, smem_block);
     if (per_sm < 1) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: dim=%u needs %zu B shared memory per CTA", api, idx->dim, smem_block);
+    // every resident warp owns a PQ table (n_chunks x n_centers f32: 32 KB at 32 x 256) that its lookups read through
+    // L2: the cap of search_kernel_pq keeps them L2-resident
+    const bool pq_tables = store == STORE_PQ && idx->metric != DAB_COSINE;
+    if (pq_tables) per_sm = std::min(per_sm, 6);
     const int resident = per_sm * idx->sm_count;
+    DevBuf luts;
+    if (store >= 0) {
+        p.dtype = idx->dtype;
+        set_store_params(idx, (QuantStore)store, p);
+        p.query_codes = staged.codes;
+        p.query_meta = staged.meta;
+        p.rerank = rerank ? 1 : 0;
+        if ((rc = luts.alloc(pq_tables ? (size_t)resident * kRangeWarps * idx->pq_chunks * idx->pq_centers * 4 : 16, api))) return rc;
+        p.luts = (float*)luts.p;
+    }
     set_graph_params(idx, p);
     p.vectors = idx->d_vectors;
     p.row_stride = idx->row_stride;
@@ -531,6 +834,11 @@ int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t n
     DAB_CUDA(cudaStreamSynchronize(st));
     r->d_results = out.p;
     out.p = nullptr;
+    if (rerank) {
+        cudaFree(luts.p), cudaFree(p1.p), cudaFree(arena1.p), cudaFree(arena2.p);
+        luts.p = p1.p = arena1.p = arena2.p = nullptr;
+        return range_rerank(idx, api, d_queries, nq, radius, has_inner, inner_radius, r);
+    }
     return DAB_OK;
 }
 
@@ -543,8 +851,9 @@ int range_empty(dab_index* idx, dab_range* r) {
 }
 
 // nq >= 1 queries, from the host (`host`, copied to the handle's scratch) or the device
-int range_queries(dab_index* idx, const char* api, bool host, const void* queries, uint32_t nq, uint32_t l_search, uint32_t beam, float radius,
-                  int has_inner, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, dab_range* r) {
+int range_batch(dab_index* idx, const char* api, bool host, const void* queries, uint32_t nq, uint32_t l_search, uint32_t beam, float radius,
+                int has_inner, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, int store, bool rerank,
+                dab_range* r) {
     const void* d_queries = queries;
     if (host) {
         const size_t qbytes = (size_t)nq * idx->dim * elem_size(idx->dtype);
@@ -553,22 +862,28 @@ int range_queries(dab_index* idx, const char* api, bool host, const void* querie
         d_queries = idx->s_queries.p;
         DAB_CUDA(cudaMemcpyAsync(idx->s_queries.p, queries, qbytes, cudaMemcpyHostToDevice, idx->stream));
     }
-    return range_run(idx, api, d_queries, nq, l_search, beam, radius, has_inner, inner_radius, initial_slack, range_slack, max_returned, r);
+    return range_run(idx, api, d_queries, nq, l_search, beam, radius, has_inner, inner_radius, initial_slack, range_slack, max_returned, store,
+                     rerank, r);
 }
 
+// `store`: -1 full precision, else the QuantStore both phases read; `rerank` (a store) reorders the results by
+// full-precision distance
 int range_search(dab_index* idx, const char* api, bool host, const void* queries, uint32_t nq, uint32_t l_search, uint32_t beam, float radius,
-                 int has_inner, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, dab_range** out) {
+                 int has_inner, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, dab_range** out,
+                 int store = -1, bool rerank = false) {
     if (!idx || !out || (nq && !queries)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
     *out = nullptr;
     int rc;
-    if ((rc = check_range_args(idx, api, l_search, beam, radius, has_inner, inner_radius, initial_slack, range_slack, max_returned))) return rc;
+    if ((rc = check_range_args(idx, api, store, rerank, l_search, beam, radius, has_inner, inner_radius, initial_slack, range_slack,
+                               max_returned)))
+        return rc;
     DAB_CUDA(cudaSetDevice(idx->device));
     if ((rc = idx->h_counters.reserve(64))) return rc;
     dab_range* r = new dab_range();
     r->idx = idx;
     r->nq = nq;
-    if ((rc = nq ? range_queries(idx, api, host, queries, nq, l_search, beam, radius, has_inner, inner_radius, initial_slack, range_slack,
-                                 max_returned, r)
+    if ((rc = nq ? range_batch(idx, api, host, queries, nq, l_search, beam, radius, has_inner, inner_radius, initial_slack, range_slack,
+                               max_returned, store, rerank, r)
                  : range_empty(idx, r))) {
         cudaStreamSynchronize(idx->stream);
         range_free(r);
@@ -608,6 +923,48 @@ int dab_range_search_device(dab_index* idx, const void* d_queries, uint32_t nq, 
                             dab_range** out) {
     return range_search(idx, "dab_range_search_device", false, d_queries, nq, l_search, beam_width, radius, has_inner_radius, inner_radius,
                         initial_slack, range_slack, max_returned, out);
+}
+
+int dab_range_search_pq(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search, uint32_t beam_width, float radius,
+                        int has_inner_radius, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, int rerank,
+                        dab_range** out) {
+    return range_search(idx, "dab_range_search_pq", true, queries, nq, l_search, beam_width, radius, has_inner_radius, inner_radius, initial_slack,
+                        range_slack, max_returned, out, STORE_PQ, rerank != 0);
+}
+
+int dab_range_search_pq_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t l_search, uint32_t beam_width, float radius,
+                               int has_inner_radius, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, int rerank,
+                               dab_range** out) {
+    return range_search(idx, "dab_range_search_pq_device", false, d_queries, nq, l_search, beam_width, radius, has_inner_radius, inner_radius,
+                        initial_slack, range_slack, max_returned, out, STORE_PQ, rerank != 0);
+}
+
+int dab_range_search_sq(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search, uint32_t beam_width, float radius,
+                        int has_inner_radius, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, int rerank,
+                        dab_range** out) {
+    return range_search(idx, "dab_range_search_sq", true, queries, nq, l_search, beam_width, radius, has_inner_radius, inner_radius, initial_slack,
+                        range_slack, max_returned, out, STORE_SQ, rerank != 0);
+}
+
+int dab_range_search_sq_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t l_search, uint32_t beam_width, float radius,
+                               int has_inner_radius, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, int rerank,
+                               dab_range** out) {
+    return range_search(idx, "dab_range_search_sq_device", false, d_queries, nq, l_search, beam_width, radius, has_inner_radius, inner_radius,
+                        initial_slack, range_slack, max_returned, out, STORE_SQ, rerank != 0);
+}
+
+int dab_range_search_minmax(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search, uint32_t beam_width, float radius,
+                            int has_inner_radius, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, int rerank,
+                            dab_range** out) {
+    return range_search(idx, "dab_range_search_minmax", true, queries, nq, l_search, beam_width, radius, has_inner_radius, inner_radius,
+                        initial_slack, range_slack, max_returned, out, STORE_MINMAX, rerank != 0);
+}
+
+int dab_range_search_minmax_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t l_search, uint32_t beam_width, float radius,
+                                   int has_inner_radius, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned,
+                                   int rerank, dab_range** out) {
+    return range_search(idx, "dab_range_search_minmax_device", false, d_queries, nq, l_search, beam_width, radius, has_inner_radius,
+                        inner_radius, initial_slack, range_slack, max_returned, out, STORE_MINMAX, rerank != 0);
 }
 
 int dab_range_offsets(const dab_range* r, uint64_t* offsets, uint32_t* cmps, uint32_t* hops, uint8_t* second_round) {

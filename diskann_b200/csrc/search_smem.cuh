@@ -357,5 +357,37 @@ __device__ __forceinline__ void wide_distances_int(const uint8_t* __restrict__ q
     }
 }
 
+// ---- the full-precision distances of a rerank --------------------------------------------------
+// Distance<T, T> of rows cid[0..m) to the query at qf (load_query with a pad of 16) into cd[0..m), as the rerank kernels
+// compute them (rerank_kernel, search_kernel_pq.cu; range_rerank_kernel, search_range.cu): the wide-load loops for f32
+// rows and integers; NA = 2 — f16 x f16 (Strategy2x4, both sides widened to f32 lanes, so the f32 copy of the query is
+// the same operand) and Metric::Cosine over float rows — one team of 16 lanes per row.  cid and cd may be in shared or
+// global memory.
+template <typename TD, int KIND, int POST, int NA>
+__device__ __forceinline__ void rerank_distances(const float* qf, const uint8_t* vectors, size_t row_stride, const uint32_t* cid, uint32_t m,
+                                                 float* cd, int dim, int lane) {
+    if constexpr (std::is_same<TD, int8_t>::value || std::is_same<TD, uint8_t>::value) {
+        int qq = 0;
+        if (KIND != KIND_IP) qq = warp_int_self<std::is_same<TD, int8_t>::value>(reinterpret_cast<const uint8_t*>(qf), dim, lane);
+        wide_distances_int<std::is_same<TD, int8_t>::value, KIND, POST, 4>(reinterpret_cast<const uint8_t*>(qf), qq, vectors, row_stride, cid, m,
+                                                                         cd, dim, lane);
+    } else if constexpr (NA == 2) {
+        constexpr int S = 16, U = 2;
+        const int team = lane / S, slot = lane % S;
+        for (uint32_t c0 = 0; c0 < m; c0 += 2 * U) {  // every lane takes part in the team shuffles: uniform trip count
+            const TD* rows[U];
+#pragma unroll
+            for (int u = 0; u < U; ++u) rows[u] = reinterpret_cast<const TD*>(vectors + (size_t)cid[min(c0 + team * U + u, m - 1)] * row_stride);
+            float r[U];
+            team_float_multi<2, KIND, U>(qf, rows, dim, slot, r);
+#pragma unroll
+            for (int u = 0; u < U; ++u)
+                if (slot == 0 && c0 + team * U + u < m) cd[c0 + team * U + u] = post_op<POST>(r[u]);
+        }
+    } else {
+        wide_distances<TD, KIND, POST, 2, 4>(qf, vectors, row_stride, cid, m, cd, dim, lane);
+    }
+}
+
 }  // namespace
 }  // namespace dab

@@ -444,6 +444,55 @@ class GpuIndex:
         return RangeResults(self, _lib.lib().dab_range_search_device, C.c_void_p(d_queries), nq, l_search, radius, beam_width=beam_width,
                             inner_radius=inner_radius, initial_slack=initial_slack, range_slack=range_slack, max_returned=max_returned)
 
+    def _range_quant(self, store, queries, l_search, radius, rerank=False, **kw):
+        with RangeResults(self, getattr(_lib.lib(), f"dab_range_search_{store}"), _ptr(self._queries(queries)), len(queries), l_search, radius,
+                          rerank=bool(rerank), **kw) as r:
+            offsets, cmps, hops, second = r.offsets()
+            ids, dists = r.results()
+        return offsets, ids, dists, cmps, hops, second
+
+    def range_search_pq(self, queries, l_search, radius, *, beam_width=1, inner_radius=None, initial_slack=1.0, range_slack=1.0,
+                        max_returned=None, rerank=False):
+        """range_search with every distance of both phases the PQ store's (those of search_batch_pq).  rerank=True: the
+        in_range ids by full-precision distance, those within (inner_radius, radius] of it, sorted by it, with it."""
+        return self._range_quant("pq", queries, l_search, radius, beam_width=beam_width, inner_radius=inner_radius, initial_slack=initial_slack,
+                                 range_slack=range_slack, max_returned=max_returned, rerank=rerank)
+
+    def range_search_sq(self, queries, l_search, radius, *, beam_width=1, inner_radius=None, initial_slack=1.0, range_slack=1.0,
+                        max_returned=None, rerank=False):
+        """range_search_pq over the scalar-quantized store (the distances of search_batch_sq)"""
+        return self._range_quant("sq", queries, l_search, radius, beam_width=beam_width, inner_radius=inner_radius, initial_slack=initial_slack,
+                                 range_slack=range_slack, max_returned=max_returned, rerank=rerank)
+
+    def range_search_minmax(self, queries, l_search, radius, *, beam_width=1, inner_radius=None, initial_slack=1.0, range_slack=1.0,
+                            max_returned=None, rerank=False):
+        """range_search_pq over the MinMax store (the distances of search_batch_minmax).  A query holding a NaN after the
+        store's transform fails the call."""
+        return self._range_quant("minmax", queries, l_search, radius, beam_width=beam_width, inner_radius=inner_radius,
+                                 initial_slack=initial_slack, range_slack=range_slack, max_returned=max_returned, rerank=rerank)
+
+    def _range_quant_device(self, store, d_queries, nq, l_search, radius, rerank=False, **kw):
+        return RangeResults(self, getattr(_lib.lib(), f"dab_range_search_{store}_device"), C.c_void_p(d_queries), nq, l_search, radius,
+                            rerank=bool(rerank), **kw)
+
+    def range_search_pq_device(self, d_queries, nq, l_search, radius, *, beam_width=1, inner_radius=None, initial_slack=1.0, range_slack=1.0,
+                               max_returned=None, rerank=False):
+        """range_search_pq of `nq` queries at the device pointer `d_queries` (an integer): a RangeResults"""
+        return self._range_quant_device("pq", d_queries, nq, l_search, radius, beam_width=beam_width, inner_radius=inner_radius,
+                                        initial_slack=initial_slack, range_slack=range_slack, max_returned=max_returned, rerank=rerank)
+
+    def range_search_sq_device(self, d_queries, nq, l_search, radius, *, beam_width=1, inner_radius=None, initial_slack=1.0, range_slack=1.0,
+                               max_returned=None, rerank=False):
+        """range_search_sq of `nq` queries at the device pointer `d_queries` (an integer): a RangeResults"""
+        return self._range_quant_device("sq", d_queries, nq, l_search, radius, beam_width=beam_width, inner_radius=inner_radius,
+                                        initial_slack=initial_slack, range_slack=range_slack, max_returned=max_returned, rerank=rerank)
+
+    def range_search_minmax_device(self, d_queries, nq, l_search, radius, *, beam_width=1, inner_radius=None, initial_slack=1.0,
+                                   range_slack=1.0, max_returned=None, rerank=False):
+        """range_search_minmax of `nq` queries at the device pointer `d_queries` (an integer): a RangeResults"""
+        return self._range_quant_device("minmax", d_queries, nq, l_search, radius, beam_width=beam_width, inner_radius=inner_radius,
+                                        initial_slack=initial_slack, range_slack=range_slack, max_returned=max_returned, rerank=rerank)
+
     def search_batch_device(self, d_queries, nq, k, l_search, beam_width, d_ids, d_dists, d_counts=0, d_cmps=0, d_hops=0):
         """Same with device pointers (integers); results stay in HBM."""
         check(_lib.lib().dab_search_batch_device(self._h, C.c_void_p(d_queries), nq, k, l_search, beam_width,
@@ -899,11 +948,16 @@ class RangeResults:
     do not change.  Use as a context manager or call close(); closing the index closes it too."""
 
     def __init__(self, index, search, queries, nq, l_search, radius, beam_width=1, inner_radius=None, initial_slack=1.0,
-                 range_slack=1.0, max_returned=None):
+                 range_slack=1.0, max_returned=None, rerank=None):
+        """`rerank`: None for the full-precision call, else the rerank flag of a quantized store's call"""
         self._h = C.c_void_p()
         self.nq = int(nq)
+        store_args = () if rerank is None else (int(bool(rerank)),)
         check(search(index._h, queries, self.nq, l_search, beam_width, radius, int(inner_radius is not None),
-                     0.0 if inner_radius is None else inner_radius, initial_slack, range_slack, max_returned or 0, C.byref(self._h)))
+                     0.0 if inner_radius is None else inner_radius, initial_slack, range_slack, max_returned or 0, *store_args,
+                     C.byref(self._h)))
+        # the index outlives the set: when both are collected together, close() sees whether dab_destroy already freed it
+        self._index = index
         index._ranges.add(self)
 
     def _live(self):
@@ -937,7 +991,8 @@ class RangeResults:
 
     def close(self):
         if getattr(self, "_h", None) is not None and self._h.value:
-            _lib.lib().dab_range_free(self._h)
+            if self._index._h.value:  # else released by dab_destroy
+                _lib.lib().dab_range_free(self._h)
             self._h = C.c_void_p()
 
     def __del__(self):

@@ -248,20 +248,35 @@ impl<T: Element> GpuIndex<T> {
                                   args.inner_radius.is_some() as i32, args.inner_radius.unwrap_or(0.0), args.initial_slack,
                                   args.range_slack, args.max_returned.unwrap_or(0), &mut set)
         })?;
-        let mut r = RangeBatch { offsets: vec![0; nq + 1], ids: Vec::new(), dists: Vec::new(), cmps: vec![0; nq], hops: vec![0; nq],
-                                 second_round: vec![0; nq] };
-        let rc = unsafe {
-            sys::dab_range_offsets(set, r.offsets.as_mut_ptr(), r.cmps.as_mut_ptr(), r.hops.as_mut_ptr(), r.second_round.as_mut_ptr())
-        };
-        if rc == 0 {
-            let total = r.offsets[nq] as usize;
-            r.ids = vec![0; total];
-            r.dists = vec![0.0; total];
-        }
-        let rc = if rc == 0 { unsafe { sys::dab_range_results(set, r.ids.as_mut_ptr(), r.dists.as_mut_ptr()) } } else { rc };
-        unsafe { sys::dab_range_free(set) };
-        check(rc)?;
-        Ok(r)
+        take_range(set, nq)
+    }
+
+    /// `range_search` with every distance of both phases the PQ store's (those of `search_batch_pq`); `rerank`: the
+    /// in_range ids by full-precision distance, those within (inner_radius, radius] of it, sorted by it, with it.
+    pub fn range_search_pq(&self, queries: &[T], l_search: u32, radius: f32, args: RangeArgs, rerank: bool) -> Result<RangeBatch> {
+        self.range_quantized(sys::dab_range_search_pq, queries, l_search, radius, args, rerank)
+    }
+
+    /// `range_search_pq` over the scalar-quantized store (the distances of `search_batch_sq`).
+    pub fn range_search_sq(&self, queries: &[T], l_search: u32, radius: f32, args: RangeArgs, rerank: bool) -> Result<RangeBatch> {
+        self.range_quantized(sys::dab_range_search_sq, queries, l_search, radius, args, rerank)
+    }
+
+    /// `range_search_pq` over the MinMax store (the distances of `search_batch_minmax`).
+    pub fn range_search_minmax(&self, queries: &[T], l_search: u32, radius: f32, args: RangeArgs, rerank: bool) -> Result<RangeBatch> {
+        self.range_quantized(sys::dab_range_search_minmax, queries, l_search, radius, args, rerank)
+    }
+
+    fn range_quantized(&self, f: RangeQuantized, queries: &[T], l_search: u32, radius: f32, args: RangeArgs, rerank: bool)
+        -> Result<RangeBatch> {
+        assert_eq!(queries.len() % self.dim, 0);
+        let nq = queries.len() / self.dim;
+        let mut set: *mut sys::dab_range = std::ptr::null_mut();
+        check(unsafe {
+            f(self.raw, queries.as_ptr() as *const c_void, nq as u32, l_search, args.beam_width, radius, args.inner_radius.is_some() as i32,
+              args.inner_radius.unwrap_or(0.0), args.initial_slack, args.range_slack, args.max_returned.unwrap_or(0), rerank as i32, &mut set)
+        })?;
+        take_range(set, nq)
     }
 
     /// `search_batch_diverse` with the traversal distances of `search_batch_pq` (the PQ store); `rerank`: the
@@ -457,6 +472,25 @@ type QuantizedAsync = unsafe extern "C" fn(*mut sys::dab_index, u32, *const c_vo
 /// The entry points that open a paged search over a quantized store (one signature for PQ, SQ and MinMax).
 type DiverseQuantized = unsafe extern "C" fn(*mut sys::dab_index, *const c_void, u32, u32, u32, u32, u32, std::os::raw::c_int,
                                              *mut u32, *mut f32, *mut u32, *mut u32, *mut u32) -> std::os::raw::c_int;
+type RangeQuantized = unsafe extern "C" fn(*mut sys::dab_index, *const c_void, u32, u32, u32, f32, std::os::raw::c_int, f32, f32, f32, u64,
+                                           std::os::raw::c_int, *mut *mut sys::dab_range) -> std::os::raw::c_int;
+
+/// The offsets, stats and results of a range search's result set, which is freed
+fn take_range(set: *mut sys::dab_range, nq: usize) -> Result<RangeBatch> {
+    let mut r = RangeBatch { offsets: vec![0; nq + 1], ids: Vec::new(), dists: Vec::new(), cmps: vec![0; nq], hops: vec![0; nq],
+                             second_round: vec![0; nq] };
+    let rc = unsafe { sys::dab_range_offsets(set, r.offsets.as_mut_ptr(), r.cmps.as_mut_ptr(), r.hops.as_mut_ptr(), r.second_round.as_mut_ptr()) };
+    if rc == 0 {
+        let total = r.offsets[nq] as usize;
+        r.ids = vec![0; total];
+        r.dists = vec![0.0; total];
+    }
+    let rc = if rc == 0 { unsafe { sys::dab_range_results(set, r.ids.as_mut_ptr(), r.dists.as_mut_ptr()) } } else { rc };
+    unsafe { sys::dab_range_free(set) };
+    check(rc)?;
+    Ok(r)
+}
+
 type PagedBegin = unsafe extern "C" fn(*mut sys::dab_index, *const c_void, u32, u32, *mut *mut sys::dab_paged) -> std::os::raw::c_int;
 
 /// A batch in flight on one slot of the device.  Dropping it joins the slot (the library writes into the

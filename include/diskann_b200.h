@@ -287,6 +287,51 @@ int dab_range_search_device(dab_index* idx, const void* d_queries, uint32_t nq, 
                             uint32_t beam_width, float radius, int has_inner_radius,
                             float inner_radius, float initial_slack, float range_slack,
                             uint64_t max_returned, dab_range** out);
+/* Range::search over the PQ, SQ or MinMax store: the arguments and result set of dab_range_search,
+ * plus `rerank`.  Every distance of both phases is the store's, those of
+ * dab_search_batch_{pq,sq,minmax} on the same index: PQ TableL2 for L2 and CosineNormalized,
+ * TableIP for InnerProduct, DirectCosine for Cosine; SQ compensated distances (Cosine refused);
+ * MinMax every metric behind the store's transform (a query holding a NaN after the transform fails
+ * the call, naming it).  SQ and MinMax compress the queries once, before the launch.
+ *   rerank == 0: the results of dab_range_search with the store's distances (in insertion order,
+ *     the radius and inner radius compared with the store's distances).
+ *   rerank != 0: in_range (decided on the store's distances) without start points and deleted ids;
+ *     each id's full-precision distance to the query; the ids with inner_radius < d <= radius of
+ *     that distance, sorted by it (stable: ties in in_range order, -0.0 equal to +0.0).  The result
+ *     set holds the full-precision distances.
+ * cmps, hops and second_round are those of the traversal, with or without rerank.  Checked before
+ * any device work: every check of dab_range_search (the shared-memory bound with the query area of
+ * the store: the f32 query for PQ, the code row + 16 B for SQ and MinMax; the graph must be
+ * uploaded), then the store's (its rows uploaded, SQ not under Cosine, l_search + n_start <= 1024)
+ * and, with rerank, the full-precision vectors (DAB_ERR_NOT_READY), which are not needed without
+ * it.  DAB_ERR_OUT_OF_MEMORY as dab_range_search, the rerank's sort included. */
+int dab_range_search_pq(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search,
+                        uint32_t beam_width, float radius, int has_inner_radius, float inner_radius,
+                        float initial_slack, float range_slack, uint64_t max_returned, int rerank,
+                        dab_range** out);
+int dab_range_search_pq_device(dab_index* idx, const void* d_queries, uint32_t nq,
+                               uint32_t l_search, uint32_t beam_width, float radius,
+                               int has_inner_radius, float inner_radius, float initial_slack,
+                               float range_slack, uint64_t max_returned, int rerank,
+                               dab_range** out);
+int dab_range_search_sq(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search,
+                        uint32_t beam_width, float radius, int has_inner_radius, float inner_radius,
+                        float initial_slack, float range_slack, uint64_t max_returned, int rerank,
+                        dab_range** out);
+int dab_range_search_sq_device(dab_index* idx, const void* d_queries, uint32_t nq,
+                               uint32_t l_search, uint32_t beam_width, float radius,
+                               int has_inner_radius, float inner_radius, float initial_slack,
+                               float range_slack, uint64_t max_returned, int rerank,
+                               dab_range** out);
+int dab_range_search_minmax(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search,
+                            uint32_t beam_width, float radius, int has_inner_radius,
+                            float inner_radius, float initial_slack, float range_slack,
+                            uint64_t max_returned, int rerank, dab_range** out);
+int dab_range_search_minmax_device(dab_index* idx, const void* d_queries, uint32_t nq,
+                                   uint32_t l_search, uint32_t beam_width, float radius,
+                                   int has_inner_radius, float inner_radius, float initial_slack,
+                                   float range_slack, uint64_t max_returned, int rerank,
+                                   dab_range** out);
 /* offsets [nq + 1]: query q's results are entries offsets[q] .. offsets[q + 1] - 1; cmps, hops
  * [nq] u32 and second_round [nq] (0 / 1) may be NULL.  Host buffers. */
 int dab_range_offsets(const dab_range* r, uint64_t* offsets, uint32_t* cmps, uint32_t* hops,

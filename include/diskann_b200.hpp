@@ -276,6 +276,26 @@ class GpuRange {
         dab_range* set = nullptr;
         check(dab_range_search(p_.raw(), queries, nq, l_, beam_, radius_, has_inner_ ? 1 : 0, inner_, initial_slack_, range_slack_,
                                max_returned_, &set));
+        return take(set, nq);
+    }
+    // Range::search over the provider's PQ, SQ or MinMax store: every distance of both phases the store's; `rerank`: the
+    // in_range ids by full-precision distance, those within (inner_radius, radius] of it, sorted by it, with it
+    RangeResults search_pq(const T* queries, uint32_t nq, bool rerank = false) { return search_store(dab_range_search_pq, queries, nq, rerank); }
+    RangeResults search_sq(const T* queries, uint32_t nq, bool rerank = false) { return search_store(dab_range_search_sq, queries, nq, rerank); }
+    RangeResults search_minmax(const T* queries, uint32_t nq, bool rerank = false) {
+        return search_store(dab_range_search_minmax, queries, nq, rerank);
+    }
+
+   private:
+    using StoreSearch = int (*)(dab_index*, const void*, uint32_t, uint32_t, uint32_t, float, int, float, float, float, uint64_t, int, dab_range**);
+    RangeResults search_store(StoreSearch f, const T* queries, uint32_t nq, bool rerank) {
+        dab_range* set = nullptr;
+        check(f(p_.raw(), queries, nq, l_, beam_, radius_, has_inner_ ? 1 : 0, inner_, initial_slack_, range_slack_, max_returned_, rerank ? 1 : 0,
+                &set));
+        return take(set, nq);
+    }
+    // the offsets, stats and results of a result set, which is freed
+    static RangeResults take(dab_range* set, uint32_t nq) {
         std::unique_ptr<dab_range, void (*)(dab_range*)> owned(set, dab_range_free);
         RangeResults r;
         r.nq = nq;
@@ -290,7 +310,6 @@ class GpuRange {
         return r;
     }
 
-   private:
     Provider<T>& p_;
     uint32_t l_, beam_;
     float radius_;

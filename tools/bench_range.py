@@ -10,7 +10,12 @@ same L and beam: it is timed the same way and reported as the phase-1 time, and 
 share of queries that took a second round, mean hops, and the reference's average_precision (benchmark-core/src/
 recall.rs: the share of all exact in-range ids, over all queries, that the search returned).  The card's name and power
 limit are read in the same run.
-usage: python tools/bench_range.py [--n N] [--nq NQ] [--reps R] [--beam B] [--json PATH]"""
+--store runs the search over a compressed store as well (the stores of bench_diverse.py: pq, PQ-32 trained on the device;
+sq, SQ-8; minmax, MinMax-8 behind DoubleHadamard) with dab_range_search_{pq,sq,minmax}_device, and --rerank its
+full-precision rerank.  Each radius then has a row for the store next to the full-precision row, timed the same way
+(phase 1 of the store is dab_search_batch_{pq,sq,minmax}_device at L), with its average_precision against the same exact
+full-precision in-range sets.
+usage: python tools/bench_range.py [--n N] [--nq NQ] [--reps R] [--beam B] [--store {fp,pq,sq,minmax}] [--rerank] [--json PATH]"""
 import argparse
 import json
 import os
@@ -24,6 +29,7 @@ import numpy as np
 import torch
 
 import bench
+import diskann_b200 as dab
 from bench_minmax_search import build_index, card
 
 L, TARGETS, CHUNK = 100, (10, 100, 1000), 128
@@ -49,6 +55,8 @@ def main():
     ap.add_argument("--nq", type=int, default=0)
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--beam", type=int, default=1)
+    ap.add_argument("--store", choices=["fp", "pq", "sq", "minmax"], default="fp")
+    ap.add_argument("--rerank", action="store_true")
     ap.add_argument("--json", default="")
     args = ap.parse_args()
     name, power = card()
@@ -61,6 +69,19 @@ def main():
     base_t = torch.from_numpy(base).cuda().double()
     bn = (base_t * base_t).sum(1)
     d_q = torch.from_numpy(queries).cuda()
+    if args.store == "sq":
+        mean, std = base.mean(0).astype(np.float32), float(base.std())
+        shift = (mean - np.float32(2.5 * std)).astype(np.float32)
+        g.upload_sq(8, shift, float(np.float32(5.0 * std)), float(np.dot(shift, shift)), 0.0)
+        g.sq_encode_all()
+    elif args.store == "minmax":
+        g.upload_minmax(8, 1.0, dab.Transform.double_hadamard(cfg["dim"], "same", seed=7))
+        g.minmax_encode_all()
+    elif args.store == "pq":
+        pick = np.sort(np.random.default_rng(bench.SEED_PQ).choice(n, size=min(100_000, n), replace=False))
+        g.pq_train(base[pick].astype(np.float32), 32, 256, 5, bench.SEED_PQ)
+        g.pq_encode_all()
+    stores = ["fp"] if args.store == "fp" else ["fp", args.store]
 
     def timed(call):
         call()
@@ -79,6 +100,15 @@ def main():
             *(torch.empty(nq, dtype=torch.int32, device="cuda") for _ in range(3)))
     knn_ms = timed(lambda: g.search_batch_device(d_q.data_ptr(), nq, L, L, args.beam, *(o.data_ptr() for o in outs)))
     knn_d = outs[1].cpu().numpy()
+    phase1 = {"fp": knn_ms}
+    if args.store != "fp":
+        phase1[args.store] = timed(lambda: getattr(g, f"search_batch_{args.store}_device")(d_q.data_ptr(), nq, L, L, args.beam,
+                                                                                           *(o.data_ptr() for o in outs)))
+
+    def range_set(store, radius):
+        if store == "fp":
+            return g.range_search_device(d_q.data_ptr(), nq, L, radius, beam_width=args.beam)
+        return getattr(g, f"range_search_{store}_device")(d_q.data_ptr(), nq, L, radius, beam_width=args.beam, rerank=args.rerank)
 
     sample = queries[:: max(1, nq // 1000)]
     rows = []
@@ -93,24 +123,27 @@ def main():
         radius = float(np.float32(hi))
         exact, truth = in_range_sets(base_t, bn, queries, radius, True)
 
-        def call():
-            with g.range_search_device(d_q.data_ptr(), nq, L, radius, beam_width=args.beam):
-                pass
-        ms = timed(call)
-        with g.range_search_device(d_q.data_ptr(), nq, L, radius, beam_width=args.beam) as r:
-            offsets, cmps, hops, second = r.offsets()
-            ids, _ = r.results()
-        counts = np.diff(offsets.astype(np.int64))
-        found = sum(len(np.intersect1d(truth[q], ids[offsets[q]:offsets[q + 1]])) for q in range(nq))
-        row = dict(target_mean_count=target, radius=radius, exact_mean_count=round(float(exact.mean()), 2), exact_max_count=int(exact.max()),
-                   ms_per_batch=round(ms, 3), phase1_ms=round(knn_ms, 3), phase2_ms=round(ms - knn_ms, 3), qps=round(nq / ms * 1e3, 1),
-                   mean_count=round(float(counts.mean()), 2), max_count=int(counts.max()),
-                   second_round_share=round(float(second.mean()), 4), mean_hops=round(float(hops.mean()), 1),
-                   mean_cmps=round(float(cmps.mean()), 1), average_precision=round(found / max(1, int(exact.sum())), 4))
-        print(json.dumps(row), flush=True)
-        rows.append(row)
+        for store in stores:
+            def call():
+                with range_set(store, radius):
+                    pass
+            ms = timed(call)
+            with range_set(store, radius) as r:
+                offsets, cmps, hops, second = r.offsets()
+                ids, _ = r.results()
+            counts = np.diff(offsets.astype(np.int64))
+            found = sum(len(np.intersect1d(truth[q], ids[offsets[q]:offsets[q + 1]])) for q in range(nq))
+            row = dict(store=store, rerank=args.rerank and store != "fp", target_mean_count=target, radius=radius,
+                       exact_mean_count=round(float(exact.mean()), 2), exact_max_count=int(exact.max()), ms_per_batch=round(ms, 3),
+                       phase1_ms=round(phase1[store], 3), phase2_ms=round(ms - phase1[store], 3), qps=round(nq / ms * 1e3, 1),
+                       mean_count=round(float(counts.mean()), 2), max_count=int(counts.max()),
+                       second_round_share=round(float(second.mean()), 4), mean_hops=round(float(hops.mean()), 1),
+                       mean_cmps=round(float(cmps.mean()), 1), average_precision=round(found / max(1, int(exact.sum())), 4))
+            print(json.dumps(row), flush=True)
+            rows.append(row)
     summary = dict(gpu=name, power_limit_max_sm_clock=power, workload="c2_1Mx128_f32_l2", n=n, nq=nq, L=L, beam=args.beam,
-                   reps=args.reps, knn_batch_ms=round(knn_ms, 3), range=rows)
+                   store={"fp": "full_precision", "pq": "pq32_dab_pq_train", "sq": "sq8", "minmax": "minmax8_doublehadamard"}[args.store],
+                   rerank=args.rerank, reps=args.reps, knn_batch_ms=round(knn_ms, 3), range=rows)
     print(json.dumps(summary), flush=True)
     if args.json:
         os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)
