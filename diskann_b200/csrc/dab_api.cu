@@ -155,6 +155,7 @@ void dab_destroy(dab_index* idx) {
     minmax_release(idx);
     deleted_release(idx);
     attributes_release(idx);
+    labels_release(idx);
     store_release(idx->sq);
     store_release(idx->mm);
     cudaFree(idx->d_vectors);

@@ -36,6 +36,7 @@ int retire_quantized_stores(struct ::dab_index* idx);
 void minmax_release(struct ::dab_index* idx);        // minmax_index.cu: the store's transform
 void paged_release(struct ::dab_index* idx);         // search_paged.cu: every paged search session still open
 void attributes_release(struct ::dab_index* idx);    // search_diverse.cu: the attribute table
+void labels_release(struct ::dab_index* idx);        // search_filtered.cu: the label table
 void range_release(struct ::dab_index* idx);         // search_range.cu: every range search result set still open
 // delete_kernels.cu: the deletion table.  deleted_assign replaces it with `words` ((n_total + 31) / 32 of them, bit i of
 // word i / 32 for id i) holding n_deleted set bits; n_deleted == 0 clears it (words may then be NULL).
@@ -238,7 +239,7 @@ struct dab_index {
     // scratch (grow-only)
     dab::Scratch s_queries, s_ids, s_out, s_out2, s_tables, s_counters, s_stats;
     dab::Scratch s_stage;  // packed-code store upload / encode / download staging, and the SQ and MinMax searches' compressed queries
-    dab::Scratch s_pools;  // the local queues of diverse search (search_diverse.cu)
+    dab::Scratch s_pools;  // the local queues of diverse search (search_diverse.cu), or a filtered search's masks and adaptive-L table
     dab::Scratch h_stage;  // pinned host staging
     dab::Scratch h_counters;  // pinned: the four counters a search pass reports
     void* slots[DAB_MAX_SLOTS] = {};  // batches in flight (dab_search_batch_async), search_kernel.cu
@@ -268,6 +269,9 @@ struct dab_index {
     uint32_t* d_attr_values = nullptr;   // [n_total]
     uint32_t* d_attr_present = nullptr;  // (n_total + 31) / 32 words
     uint32_t* h_attr_present = nullptr;  // the host copy of the presence bits
+    // the label table of filtered search (search_filtered.cu): one 64-bit label set per id, allocated by the first
+    // dab_upload_labels (every set empty).  Independent of the graph, as the attribute table is.
+    uint64_t* d_labels = nullptr;  // [n_total]
     dab::Tuning tune;
 
     // tensor-core exhaustive scan (flat_tc.cu): bf16 operand copy of the rows + score coefficients

@@ -1,0 +1,359 @@
+// search_filtered.cu — label-filtered batched search on the device: InlineFilterSearch::search (diskann/src/graph/search/
+// inline_filter_search.rs:89-160), i.e. inline_filter_search_internal (:166-282) with its optional AdaptiveL, then the
+// default post-processing of the first L matches; and the label table it reads (dab_upload_labels).
+//
+// One warp per query on global visited tables, over full-precision rows of every type and metric of the k-NN path.  The
+// traversal is search_internal's: every evaluated neighbour enters the list, accepted or not.  Next to it the warp keeps,
+// in shared memory:
+//   the matched list  the accepted start points and neighbours, at most L of them, ordered by distance with a later
+//                     match after an earlier one at an equal distance (-0.0 equal to +0.0, NaN after every number).
+//                     That is a stable sort of all matches followed by take(L): the reference sorts with
+//                     sort_unstable_by(fast_distance), which leaves the order of exactly equal distances (and of NaN)
+//                     open, and this is the one place where the device fixes an order the reference leaves open.
+// A candidate's label set is read (8 B) next to its visited probe, when it is collected.  Adaptive L: after the hop in
+// which the evaluated neighbours reach `samples`, the list's capacity becomes the new L of the host's table (computed
+// with the reference's f64 expression, never in device math) if that is above L; NeighborPriorityQueue::reconfigure
+// (queue.rs:339-353) cuts a longer list, so a "grown" L below L + #start shortens it.  A query whose visited set outgrows
+// its table is re-run from its start points by the job, and so takes the same decision again.
+#include "dab_common.cuh"
+#include "search_common.cuh"
+#include "search_filtered.cuh"
+#include "search_host.cuh"
+
+#include <algorithm>
+#include <cmath>
+
+namespace dab {
+
+namespace {
+
+constexpr int kFiltRows = 4;  // rows in flight per team in the distance loop
+
+__device__ __forceinline__ bool label_accepts(uint64_t labels, uint64_t mask, uint32_t match_all) {
+    const uint64_t x = labels & mask;
+    return match_all ? x == mask : x != 0;
+}
+
+// fast_distance's order as an unsigned key: -0.0 and +0.0 equal, every NaN after every number
+__device__ __forceinline__ uint32_t order_key(float d) {
+    if (d != d) return 0xFFFFFFFFu;
+    const uint32_t u = __float_as_uint(d == 0.0f ? 0.0f : d);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+// The accepted ones among candidates c0 .. c0+m-1 (m <= 32; lane j owns candidate j) into the matched list of at most
+// `cap` entries: a new entry goes after every entry of an equal key, old or new, and an entry pushed past cap is dropped.
+// Old entries move right by #new(key < theirs); the list is walked in tiles of 32 from the top, as merge_round_chunked
+// does, so no tile overwrites an entry a lower tile still has to read.
+__device__ __forceinline__ void matched_merge(float* md, uint32_t* mi, uint32_t cap, uint32_t& size, const uint32_t* cid, const float* cd,
+                                              const uint32_t* ca, uint32_t c0, uint32_t m, int lane) {
+    const uint32_t j = (uint32_t)lane;
+    const bool acc = j < m && ca[c0 + j];
+    const float dj = acc ? cd[c0 + j] : 0.0f;
+    const uint32_t kj = order_key(dj);
+    const bool valid = acc && !(size == cap && kj >= order_key(md[cap - 1]));
+    const unsigned vm = __ballot_sync(kFull, valid);
+    if (!vm) return;
+    uint32_t lo = 0, hi = size;  // upper bound among the old entries
+    while (__any_sync(kFull, lo < hi)) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (lo < hi) {
+            if (order_key(md[mid]) <= kj) lo = mid + 1;
+            else hi = mid;
+        }
+    }
+    uint32_t rn = 0;
+    for (unsigned it = vm; it;) {
+        const int i = __ffs(it) - 1;
+        it &= it - 1;
+        const uint32_t ki = __shfl_sync(kFull, kj, i);
+        rn += (ki < kj || (ki == kj && (uint32_t)i < j)) ? 1u : 0u;
+    }
+    const uint32_t pos = lo + rn;
+    const bool keep_new = valid && pos < cap;
+    const uint32_t idj = valid ? cid[c0 + j] : 0;
+    __syncwarp();
+#pragma unroll 1
+    for (uint32_t t = (size + 31) / 32; t-- > 0;) {
+        const uint32_t e = t * 32 + lane;
+        const float od = e < size ? md[e] : 0.0f;
+        const uint32_t oi = e < size ? mi[e] : 0, ke = order_key(od);
+        uint32_t sh = 0;
+        for (unsigned it = vm; it;) {
+            const int i = __ffs(it) - 1;
+            it &= it - 1;
+            sh += __shfl_sync(kFull, kj, i) < ke ? 1u : 0u;
+        }
+        __syncwarp();
+        if (e < size && sh != 0 && e + sh < cap) md[e + sh] = od, mi[e + sh] = oi;
+        __syncwarp();
+    }
+    if (keep_new) md[pos] = dj, mi[pos] = idj;
+    size = min(cap, size + (uint32_t)__popc(vm));
+    __syncwarp();
+}
+
+// One warp's share of a pass.  Src is the distance source of diverse search: load(q), prepare(), distances(cid, cd, n).
+template <class Src>
+__device__ __forceinline__ void filtered_queries(const SearchParamsFiltered& p, uint8_t* base, int lane, Src& src) {
+    const int wib = threadIdx.x >> 5;
+    float* bd = reinterpret_cast<float*>(base + p.off_bd);
+    uint32_t* bi = reinterpret_cast<uint32_t*>(base + p.off_bi);
+    float* md = reinterpret_cast<float*>(base + p.off_md);
+    uint32_t* mi = reinterpret_cast<uint32_t*>(base + p.off_mi);
+    uint32_t* cid = reinterpret_cast<uint32_t*>(base + p.off_cid);
+    float* cd = reinterpret_cast<float*>(base + p.off_cd);
+    uint32_t* ca = reinterpret_cast<uint32_t*>(base + p.off_ca);
+    uint32_t* beam_ids = reinterpret_cast<uint32_t*>(base + p.off_beam);
+    const uint32_t nbk = p.n_buckets;
+    uint32_t* table = p.tables + (size_t)(blockIdx.x * kFiltWarps + wib) * nbk * 8;
+    const uint32_t hlimit = nbk * 7;  // 87.5 % load
+    const uint64_t n_total = p.n_points + p.n_start;
+
+    for (uint32_t qidx; next_query(p.counters, p.n_work, p.query_list, lane, qidx);) {
+        __syncwarp();
+        src.load(qidx);
+        for (uint32_t i = lane; i < nbk; i += 32) store_empty_bucket(table + (size_t)i * 8);
+        __syncwarp();
+        src.prepare();
+        const uint64_t mask = __ldg(p.masks + qidx);
+        uint32_t cap = p.best_cap, size = 0, cursor = 0, msize = 0;
+        uint32_t cmps = 0, hops = 0, nvisited = 0, sample_visited = 0, sample_matched = 0;
+        bool adjusted = p.samples == 0, overflow = false;
+
+        // the candidates cid[0..n) (with their decisions in ca) into the list and the matched list, in order
+        auto insert_all = [&](uint32_t n) {
+            for (uint32_t c0 = 0; c0 < n; c0 += 32) {
+                const uint32_t m = min(32u, n - c0);
+                merge_round_chunked<8>(bd, bi, cap, size, cursor, cid, cd, c0, m, lane);
+                matched_merge(md, mi, p.cap, msize, cid, cd, ca, c0, m, lane);
+            }
+        };
+
+        // ---- start points (start_point_distances, provider.rs:406-433), in id order; they count in neither cmps nor
+        // the sample
+        for (uint32_t s0 = 0; s0 < p.n_start; s0 += 32) {
+            const uint32_t n = min(32u, p.n_start - s0);
+            if ((uint32_t)lane < n) {
+                const uint32_t id = (uint32_t)p.n_points + s0 + lane;
+                cid[lane] = id;
+                ca[lane] = label_accepts(__ldg(p.labels + id), mask, p.match_all);
+                visit_global(table, nbk, id);
+            }
+            __syncwarp();
+            src.distances(cid, cd, n);
+            insert_all(n);
+            nvisited += n;
+        }
+
+        // ---- closest_notvisited x beam, expand_beam_filtered, every neighbour into the list and the accepted ones into
+        // the matched list; then the adaptive-L decision of the hop
+        for (;;) {
+            const uint32_t nb = pick_beam(bi, size, p.beam, cursor, beam_ids, lane);
+            if (nb == 0) break;
+            uint32_t ncand = 0;
+            for (uint32_t b = 0; b < nb; ++b) {
+                const uint32_t* row = p.adj + (size_t)beam_ids[b] * p.adj_stride;
+                const uint32_t deg = min(__ldg(row), p.max_degree);
+                for (uint32_t c0 = 0; c0 < deg + 1; c0 += 32) {
+                    const uint32_t j = c0 + lane;
+                    const uint32_t word = j < p.adj_stride ? __ldg(row + j) : kEmptyV2;
+                    const bool inserted = j >= 1 && j <= deg && visit_global(table, nbk, word);
+                    const bool isnew = inserted && word < n_total;
+                    const bool acc = isnew && label_accepts(__ldg(p.labels + word), mask, p.match_all);
+                    const unsigned mn = __ballot_sync(kFull, isnew);
+                    if (isnew) ca[ncand + __popc(mn & ((1u << lane) - 1u))] = acc;
+                    push_new(inserted, isnew, word, cid, ncand, nvisited, lane);
+                }
+                if (nvisited + p.max_degree > hlimit) {
+                    overflow = true;
+                    break;
+                }
+            }
+            if (overflow) break;
+            __syncwarp();
+            src.distances(cid, cd, ncand);
+            insert_all(ncand);
+            uint32_t matched = 0;
+            for (uint32_t c = lane; c < ncand; c += 32) matched += ca[c];
+            sample_matched += __reduce_add_sync(kFull, matched);
+            sample_visited += ncand;
+            cmps += ncand;
+            hops += nb;
+            if (!adjusted && sample_visited >= p.samples) {
+                adjusted = true;
+                const uint32_t new_l = p.adapt[(size_t)(sample_visited - p.samples) * (p.samples + p.span) + sample_matched];
+                if (new_l > p.cap) {
+                    // reconfigure(new_l): the capacity is new_l, a longer list is cut
+                    cap = new_l;
+                    size = min(size, new_l);
+                    cursor = min(cursor, new_l);
+                }
+            }
+        }
+
+        if (overflow) {
+            report_overflow(p.counters, p.overflow_list, qidx, lane);
+            continue;
+        }
+        // post-processing of matched_results.take(L): start points dropped, the first k kept
+        const uint32_t count = write_results(mi, md, msize, p.n_points, p.k, p.out_ids, p.out_dists, qidx, lane);
+        write_stats(p.counters, nvisited, p.out_counts, p.out_cmps, p.out_hops, qidx, count, cmps, hops, lane);
+    }
+}
+
+// Full precision: rows from global memory with the shared distance schemas (distance_device.cuh), a team of lanes per row
+template <typename TD, int KIND, int POST, int NA>
+__global__ void __launch_bounds__(kFiltWarps * 32) filtered_kernel(const SearchParamsFiltered p) {
+    constexpr bool INT = std::is_same<TD, int8_t>::value || std::is_same<TD, uint8_t>::value;
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    uint8_t* base = smem + (size_t)wib * p.warp_smem;
+    struct {
+        const SearchParamsFiltered& p;
+        float* qf;
+        int lane, dim, qq;  // qq, integer rows: Sum x^2 of the query (unused by inner product)
+        __device__ __forceinline__ void load(uint32_t q) { load_query(reinterpret_cast<const TD*>(p.queries) + (size_t)q * dim, dim, 4, qf, lane); }
+        __device__ __forceinline__ void prepare() {
+            if constexpr (INT) {
+                if (KIND != KIND_IP) qq = warp_int_self<std::is_same<TD, int8_t>::value>(reinterpret_cast<const uint8_t*>(qf), dim, lane);
+            }
+        }
+        __device__ __forceinline__ void distances(const uint32_t* cid, float* cd, uint32_t n) {
+            constexpr int S = INT ? 32 : 8 * NA, TEAMS = 32 / S, U = kFiltRows;
+            using Row = typename std::conditional<INT, uint8_t, TD>::type;
+            const int team = lane / S, slot = lane % S;
+            for (uint32_t c0 = 0; c0 < n; c0 += TEAMS * U) {
+                float r[U];
+                uint32_t cc[U];
+                const Row* rows[U];
+#pragma unroll
+                for (int u = 0; u < U; ++u) {
+                    cc[u] = c0 + u * TEAMS + team;
+                    rows[u] = reinterpret_cast<const Row*>(p.vectors + (size_t)cid[min(cc[u], n - 1)] * p.row_stride);
+                }
+                if constexpr (INT) warp_int_multi<std::is_same<TD, int8_t>::value, KIND, U>(reinterpret_cast<const uint8_t*>(qf), rows, dim, lane, qq, r);
+                else team_float_multi<NA, KIND, U>(qf, rows, dim, slot, r);
+#pragma unroll
+                for (int u = 0; u < U; ++u)
+                    if (slot == 0 && cc[u] < n) cd[cc[u]] = post_op<POST>(r[u]);
+            }
+            __syncwarp();
+        }
+    } src{p, reinterpret_cast<float*>(base), lane, (int)p.dim, 0};
+    filtered_queries(p, base, lane, src);
+}
+
+template <typename S>
+void (*filtered_kernel_of())(const SearchParamsFiltered) {
+    return filtered_kernel<typename S::TD, S::KIND, S::POST, S::NA>;
+}
+
+}  // namespace
+
+uint32_t adaptive_l(uint32_t base_l, uint64_t visited, uint64_t matched, double scale) {
+    if (matched == 0 || visited == 0) return (uint32_t)((double)base_l * scale);
+    const double specificity = (double)matched / (double)visited;
+    double multiplier;
+    if (specificity >= 0.5) multiplier = 1.0;
+    else if (specificity >= 0.1) multiplier = 2.0;
+    else multiplier = std::pow(2.0, -std::log10(specificity));
+    multiplier = std::min(std::max(multiplier, 1.0), scale);  // f64::clamp(1.0, scale)
+    return (uint32_t)((double)base_l * multiplier);
+}
+
+std::vector<uint16_t> adaptive_table(uint32_t l_search, uint32_t samples, uint32_t span, double scale) {
+    const size_t width = (size_t)samples + span;
+    std::vector<uint16_t> t((size_t)span * width, 0);
+    for (uint32_t r = 0; r < span; ++r) {
+        const uint64_t visited = (uint64_t)samples + r;
+        for (uint64_t m = 0; m <= visited; ++m) t[r * width + m] = (uint16_t)adaptive_l(l_search, visited, m, scale);
+    }
+    return t;
+}
+
+// A warp's shared memory: the query area (floats: dim f32; i8 / u8: the bytes rounded up to 16), the list's distances
+// and ids (best_max entries), the matched list's (L), a hop's candidate ids, distances and decisions, the beam
+static size_t filtered_warp_smem(const dab_index* idx, uint32_t l_search, uint32_t best_max, uint32_t beam, SearchParamsFiltered* p) {
+    const bool is_int = idx->dtype == DAB_I8 || idx->dtype == DAB_U8;
+    size_t off = is_int ? round_up(round_up((size_t)idx->dim, 4), 16) : round_up((size_t)idx->dim * 4, 16);
+    const size_t best = round_up((size_t)best_max * 4, 16), matched = round_up((size_t)l_search * 4, 16);
+    const size_t ncand = round_up(std::max<size_t>((size_t)beam * idx->max_degree, 32) * 4, 16);
+    SearchParamsFiltered scratch;
+    SearchParamsFiltered& q = p ? *p : scratch;
+    q.off_bd = (uint32_t)off, off += best;
+    q.off_bi = (uint32_t)off, off += best;
+    q.off_md = (uint32_t)off, off += matched;
+    q.off_mi = (uint32_t)off, off += matched;
+    q.off_cid = (uint32_t)off, off += ncand;
+    q.off_cd = (uint32_t)off, off += ncand;
+    q.off_ca = (uint32_t)off, off += ncand;
+    q.off_beam = (uint32_t)off, off += round_up((size_t)beam * 4, 16);
+    return round_up(off, 128);
+}
+
+int filtered_check_smem(const dab_index* idx, const char* api, uint32_t l_search, uint32_t best_max, uint32_t beam) {
+    const size_t smem = filtered_warp_smem(idx, l_search, best_max, beam, nullptr) * kFiltWarps;
+    if (smem > kFilteredMaxSmem)
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: L=%u, longest list %u, beam_width=%u, dim=%u, max_degree=%u need %zu B shared memory per CTA (> %zu)",
+                    api, l_search, best_max, beam, idx->dim, idx->max_degree, smem, kFilteredMaxSmem);
+    return DAB_OK;
+}
+
+int filtered_plan(const dab_index* idx, uint32_t l_search, uint32_t best_max, uint32_t beam, SearchParamsFiltered& p, FilteredPlan& plan) {
+    p.warp_smem = (uint32_t)filtered_warp_smem(idx, l_search, best_max, beam, &p);
+    plan.smem_block = (size_t)p.warp_smem * kFiltWarps;
+    return visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) -> int {
+        plan.kern = filtered_kernel_of<decltype(sc)>();
+        const int per_sm = plan.smem_block > kFilteredMaxSmem ? 0 : ctas_per_sm(plan.kern, kFiltWarps * 32, plan.smem_block);
+        if (per_sm < 1)
+            return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_filtered: L=%u, beam_width=%u, dim=%u need %zu B shared memory per CTA",
+                        l_search, beam, idx->dim, plan.smem_block);
+        plan.grid = per_sm * idx->sm_count;
+        return DAB_OK;
+    });
+}
+
+int filtered_launch(const SearchParamsFiltered& p, const FilteredPlan& plan, cudaStream_t stream) {
+    DAB_CUDA(cudaFuncSetAttribute(plan.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem_block));
+    plan.kern<<<balanced_grid(p.n_work, plan.grid, kFiltWarps), kFiltWarps * 32, plan.smem_block, stream>>>(p);
+    DAB_LAUNCHED();
+    DAB_CUDA(cudaGetLastError());
+    return DAB_OK;
+}
+
+// ---- the label table ---------------------------------------------------------------------------------------------
+void labels_release(dab_index* idx) {
+    cudaFree(idx->d_labels);
+    idx->d_labels = nullptr;
+}
+
+}  // namespace dab
+
+using namespace dab;
+
+extern "C" {
+
+int dab_upload_labels(dab_index* idx, const uint64_t* labels, uint64_t first, uint64_t count) {
+    if (!idx || (count && !labels)) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_upload_labels: NULL argument");
+    if (first > idx->n_total() || count > idx->n_total() - first)
+        return fail(DAB_ERR_INVALID_ARGUMENT, "dab_upload_labels: ids [%llu, %llu) out of range (%llu ids)", (unsigned long long)first,
+                    (unsigned long long)(first + count), (unsigned long long)idx->n_total());
+    DAB_CUDA(cudaSetDevice(idx->device));
+    if (!idx->d_labels) {
+        // the table is published only once it exists and is cleared
+        DevBuf table;
+        int rc;
+        if ((rc = table.alloc(idx->n_total() * 8, "dab_upload_labels"))) return rc;
+        DAB_CUDA(cudaMemsetAsync(table.p, 0, idx->n_total() * 8, idx->stream));
+        DAB_CUDA(cudaStreamSynchronize(idx->stream));
+        idx->d_labels = (uint64_t*)table.p;
+        table.p = nullptr;
+    }
+    if (count == 0) return DAB_OK;
+    DAB_CUDA(cudaMemcpyAsync(idx->d_labels + first, labels, count * 8, cudaMemcpyHostToDevice, idx->stream));
+    DAB_CUDA(cudaStreamSynchronize(idx->stream));
+    return DAB_OK;
+}
+
+}  // extern "C"

@@ -2,9 +2,10 @@
 // any kind with its overflow re-runs and post-processing (full precision; PQ, SQ and MinMax, whose kernels and rerank
 // are in search_kernel_pq.cu and search_kernel_pqs.cu), the slots of batches in flight and the C entry points
 // (dab_search_batch[_pq|_pq_rerank|_sq|_minmax][_device][_async], dab_search_batch_diverse[_pq|_sq|_minmax][_device],
-// dab_wait).  The diverse search (search_diverse.cu), over full-precision rows or a quantized store, is one more kind of
-// the job; so is the first phase of range search (search_range.cu), a batch over full-precision rows or a quantized
-// store that keeps start points and deleted ids.
+// dab_search_batch_filtered[_device], dab_wait).  The diverse search (search_diverse.cu), over full-precision rows or a
+// quantized store, is one more kind of the job; so are the filtered search (search_filtered.cu) and the first phase of
+// range search (search_range.cu), a batch over full-precision rows or a quantized store that keeps start points and
+// deleted ids.
 //
 // A full-precision batch runs on search_kernel_v3 (visited set in shared memory) where its short lists make that the
 // faster kernel, and on search_kernel_v2 (global visited tables) otherwise; queries whose visited set outgrows its table
@@ -12,12 +13,14 @@
 // (index.rs:1933-2000) bit for bit.
 #include "dab_common.cuh"
 #include "search_diverse.cuh"
+#include "search_filtered.cuh"
 #include "search_host.cuh"
 #include "search_pq.cuh"
 #include "search_v2.cuh"
 #include "search_v3.cuh"
 
 #include <algorithm>
+#include <cmath>
 
 namespace dab {
 
@@ -130,6 +133,8 @@ struct SlotJob {
     uint32_t diverse_k = 0;
     uint64_t pool = 0;
     Scratch* pools = nullptr;
+    // set: a filtered search over full-precision rows (FilterSpec, search_filtered.cuh)
+    const FilterSpec* filt = nullptr;
     const void* d_queries = nullptr;
     uint32_t nq = 0, k = 0, l_search = 0, beam = 0, cap = 0;
     SearchRecord rec{};  // searches over rows of the index (rec.query_rows set)
@@ -168,6 +173,9 @@ struct SlotJob {
     // diverse
     SearchParamsDiverse pd;
     DiversePlan dplan;
+    // filtered
+    SearchParamsFiltered pf;
+    FilteredPlan fplan;
 
     SlotJob(dab_index* idx_, cudaStream_t stream_, Scratch& tables_, Scratch& counters_, Scratch& stage_, Scratch& luts_,
             Scratch& lists_, Scratch& pinned_)
@@ -189,6 +197,7 @@ struct SlotJob {
     int plan_full();
     int plan_quant();
     int plan_diverse();
+    int plan_filtered();
     int reserve_tables();
     int reserve_pools();
     int stage_queries();
@@ -196,6 +205,7 @@ struct SlotJob {
     int launch_full();
     int launch_quant();
     int launch_diverse();
+    int launch_filtered();
     int post();
 
     // full precision keeps STORE_PQ in a hint of its own
@@ -244,8 +254,9 @@ int SlotJob::prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint32_t
     d_queries = d_queries_, nq = nq_, k = k_, l_search = l_search_, beam = beam_, store = store_, rerank = rerank_;
     if (rec_) rec = *rec_;
     stores_version = idx->stores_version;
-    // scratch.rs:195-208; a diverse search's list holds L (Diverse::create_scratch, diverse_search.rs:149-177)
-    cap = diverse_k ? l_search : l_search + idx->n_start;
+    // scratch.rs:195-208; a diverse search's list holds L (Diverse::create_scratch, diverse_search.rs:149-177), and a
+    // filtered search's results are the first L matches
+    cap = diverse_k || filt ? l_search : l_search + idx->n_start;
     int rc;
     if ((rc = pinned->reserve(24)) || (rc = counters->reserve(16 + (size_t)nq * 4))) return rc;
     h_counters = (uint32_t*)pinned->p;
@@ -262,9 +273,11 @@ int SlotJob::prepare(const void* d_queries_, uint32_t nq_, uint32_t k_, uint32_t
         out.dists = (float*)(out.ids + (size_t)nq * cap);
     }
     n_work = nq;
-    // a diverse search visits other nodes than a k-NN search: it neither reads nor teaches the hints
-    slots = table_slots(idx, diverse_k ? VisitedHint{} : hint(), l_search, beam, mode());
-    if ((rc = diverse_k ? plan_diverse() : store < 0 ? plan_full() : plan_quant())) return rc;
+    // a diverse search visits other nodes than a k-NN search, and a filtered one's list may grow: they neither read nor
+    // teach the hints; a filtered search's tables are sized for its longest list
+    if (filt) slots = table_slots(idx, VisitedHint{}, std::max(l_search, filt->best_max), beam, mode());
+    else slots = table_slots(idx, diverse_k ? VisitedHint{} : hint(), l_search, beam, mode());
+    if ((rc = filt ? plan_filtered() : diverse_k ? plan_diverse() : store < 0 ? plan_full() : plan_quant())) return rc;
     if (!on_v3 && (rc = reserve_tables())) return rc;
     DAB_CUDA(cudaEventCreateWithFlags(&counted, cudaEventDisableTiming));
     return DAB_OK;
@@ -392,6 +405,25 @@ int SlotJob::plan_diverse() {
     return reserve_pools();
 }
 
+// filtered: the kernel's plan, the label table, the masks and adaptive L's table
+int SlotJob::plan_filtered() {
+    memset(&pf, 0, sizeof(pf));
+    int rc;
+    if ((rc = filtered_plan(idx, l_search, filt->best_max, beam, pf, fplan))) return rc;
+    set_batch_params(pf);
+    pf.vectors = idx->d_vectors;
+    pf.row_stride = idx->row_stride;
+    pf.labels = idx->d_labels;
+    pf.masks = filt->masks;
+    pf.match_all = filt->match_all;
+    pf.best_cap = l_search + idx->n_start;
+    pf.samples = filt->adapt ? filt->samples : 0;
+    pf.span = beam * idx->max_degree;
+    pf.adapt = filt->adapt;
+    warps = (uint32_t)fplan.grid * kFiltWarps;
+    return DAB_OK;
+}
+
 // the local queues of the warps the next pass over n_work queries launches (diverse_launch's grid)
 int SlotJob::reserve_pools() {
     int rc;
@@ -422,7 +454,7 @@ int SlotJob::stage_queries() {
 int SlotJob::launch_pass() {
     DAB_CUDA(cudaMemsetAsync(d_counters, 0, 16, stream));
     int rc;
-    if ((rc = diverse_k ? launch_diverse() : store < 0 ? launch_full() : launch_quant())) return rc;
+    if ((rc = filt ? launch_filtered() : diverse_k ? launch_diverse() : store < 0 ? launch_full() : launch_quant())) return rc;
     DAB_CUDA(cudaMemcpyAsync(h_counters, d_counters, 16, cudaMemcpyDeviceToHost, stream));
     DAB_CUDA(cudaEventRecord(counted, stream));
     return DAB_OK;
@@ -456,6 +488,11 @@ int SlotJob::launch_diverse() {
     return diverse_launch(pd, dplan, stream);
 }
 
+int SlotJob::launch_filtered() {
+    set_pass_params(pf);
+    return filtered_launch(pf, fplan, stream);
+}
+
 // the post-processing of the whole batch: the rerank, or the filter of deleted ids
 int SlotJob::post() {
     if (rerank) {
@@ -474,7 +511,7 @@ int SlotJob::finish() {
         const uint32_t n_over = h_counters[1];
         if (rec.query_rows) {
             idx->rec_truncated += h_counters[3];
-        } else if (!diverse_k) {  // searches over rows run on a graph being changed: do not learn from them
+        } else if (!diverse_k && !filt) {  // searches over rows run on a graph being changed: do not learn from them
             learn_visited(hint(), l_search, beam, mode(), h_counters[2]);
             if (on_v3) {
                 idx->v3_overflow_l = l_search;
@@ -541,14 +578,16 @@ static int check_diverse_args(const dab_index* idx, const char* api, uint32_t k,
     return DAB_OK;
 }
 
-// `diverse_k` > 0: a diverse search, whose arguments check_diverse_args has passed
+// `diverse_k` > 0: a diverse search, whose arguments check_diverse_args has passed; `filt`: a filtered search, whose
+// arguments check_filtered_args has passed
 static int run_job(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam, const SearchOut& d,
-                   int store, bool rerank, const SearchRecord* rec, uint32_t diverse_k) {
+                   int store, bool rerank, const SearchRecord* rec, uint32_t diverse_k, const FilterSpec* filt = nullptr) {
     int rc;
-    if (!diverse_k && (rc = check_batch_args(idx, k, l_search, beam, store))) return rc;
+    if (!diverse_k && !filt && (rc = check_batch_args(idx, k, l_search, beam, store))) return rc;
     if (nq == 0) return DAB_OK;
     SlotJob job(idx, idx->stream, idx->s_tables, idx->s_counters, idx->s_stage, idx->s_out2, idx->s_ids, idx->h_counters);
     job.diverse_k = diverse_k;
+    job.filt = filt;
     job.pools = &idx->s_pools;
     if ((rc = job.prepare(d_queries, nq, k, l_search, beam, d, store, rerank, rec)) || (rc = job.stage_queries())) return rc;
     if (rec && rec->staged && store >= 0) *rec->staged = StagedQueries{job.pq.query_codes, job.pq.query_meta};
@@ -598,7 +637,7 @@ static int queue_result_copies(cudaStream_t stream, const HostCopy& c) {
 // The synchronous host-buffer calls: checks the buffers, copies the queries to the handle's scratch, runs the batch on
 // them with device result buffers, copies the results to `out` and waits.
 static int search_host(dab_index* idx, const char* api, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
-                       uint32_t beam, const SearchOut& out, int store, bool rerank, uint32_t diverse_k = 0) {
+                       uint32_t beam, const SearchOut& out, int store, bool rerank, uint32_t diverse_k = 0, const FilterSpec* filt = nullptr) {
     if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", api);
     if (nq == 0) return DAB_OK;
     if (!queries || !out.ids || !out.dists) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
@@ -608,7 +647,7 @@ static int search_host(dab_index* idx, const char* api, const void* queries, uin
     int rc;
     if ((rc = reserve_host_call(idx, idx->s_queries, idx->s_out, idx->s_stats, nq, k, &c.dev)) ||
         (rc = queue_query_copy(idx, idx->stream, idx->s_queries.p, queries, nq)) ||
-        (rc = run_job(idx, idx->s_queries.p, nq, k, l_search, beam, c.dev, store, rerank, nullptr, diverse_k)) ||
+        (rc = run_job(idx, idx->s_queries.p, nq, k, l_search, beam, c.dev, store, rerank, nullptr, diverse_k, filt)) ||
         (rc = queue_result_copies(idx->stream, c)))
         return rc;
     DAB_CUDA(cudaStreamSynchronize(idx->stream));
@@ -618,12 +657,12 @@ static int search_host(dab_index* idx, const char* api, const void* queries, uin
 // The synchronous device-buffer calls (run_search).  The full-precision call makes its argument checks before it returns
 // for an empty batch; the quantized calls return first.
 static int search_device(dab_index* idx, const char* api, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
-                         uint32_t beam, const SearchOut& d, int store, bool rerank, uint32_t diverse_k = 0) {
+                         uint32_t beam, const SearchOut& d, int store, bool rerank, uint32_t diverse_k = 0, const FilterSpec* filt = nullptr) {
     if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", api);
     if (nq == 0 && store >= 0) return DAB_OK;
     if (nq && (!d_queries || !d.ids || !d.dists)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
     DAB_CUDA(cudaSetDevice(idx->device));
-    return run_job(idx, d_queries, nq, k, l_search, beam, d, store, rerank, nullptr, diverse_k);
+    return run_job(idx, d_queries, nq, k, l_search, beam, d, store, rerank, nullptr, diverse_k, filt);
 }
 
 // The diverse search over a quantized store: every argument and store check before the queries are copied; the device
@@ -634,6 +673,62 @@ static int search_diverse_quant(dab_index* idx, const char* api, bool host, cons
     if ((rc = check_diverse_args(idx, api, k, l_search, beam, diverse_k, store, rerank != 0))) return rc;
     if (host) return search_host(idx, api, queries, nq, k, l_search, beam, out, store, rerank != 0, diverse_k);
     if ((rc = search_device(idx, api, queries, nq, k, l_search, beam, out, store, rerank != 0, diverse_k))) return rc;
+    DAB_CUDA(cudaStreamSynchronize(idx->stream));
+    return DAB_OK;
+}
+
+// The checks of a filtered search, all made before any device work: InlineFilterSearch's (k >= 1 and L >= k from Knn::new,
+// scale >= 1.0 from AdaptiveL::new, which a NaN scale does not pass either), the label table, and what the kernel holds:
+// L + #start and floor(L * scale) at most kFilteredMaxL, and its shared memory.  *best_max: the longest list.
+static int check_filtered_args(const dab_index* idx, const char* api, uint32_t k, uint32_t l_search, uint32_t beam,
+                               uint32_t adaptive_samples, double adaptive_scale, uint32_t* best_max) {
+    if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", api);
+    int rc;
+    if ((rc = check_search_args(idx, k, l_search, beam))) return rc;
+    if (l_search < k) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: l_value (%u) must be greater than or equal to k_value (%u)", api, l_search, k);
+    if (adaptive_samples && !(adaptive_scale >= 1.0)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: adaptive L scale factor must be >= 1.0", api);
+    if (!idx->d_labels) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: no label table (dab_upload_labels has not been called)", api);
+    if ((uint64_t)l_search + idx->n_start > kFilteredMaxL)
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: L + #start = %llu > %u", api, (unsigned long long)l_search + idx->n_start, kFilteredMaxL);
+    *best_max = l_search + idx->n_start;
+    if (adaptive_samples) {
+        const double grown = std::floor((double)l_search * adaptive_scale);
+        if (grown > kFilteredMaxL)
+            return fail(DAB_ERR_INVALID_ARGUMENT, "%s: floor(L * scale) = %.17g > %u", api, grown, kFilteredMaxL);
+        *best_max = std::max(*best_max, (uint32_t)grown);
+    }
+    return filtered_check_smem(idx, api, l_search, *best_max, beam);
+}
+
+// InlineFilterSearch::search over a batch: the checks, then the masks (host call: copied to the handle's scratch) and
+// adaptive L's table on the device, then the job.  The device form returns with its outputs complete.
+static int search_filtered(dab_index* idx, const char* api, bool host, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                           uint32_t beam, const uint64_t* masks, uint32_t match_all, uint32_t adaptive_samples, double adaptive_scale,
+                           const SearchOut& out) {
+    uint32_t best_max = 0;
+    int rc;
+    if ((rc = check_filtered_args(idx, api, k, l_search, beam, adaptive_samples, adaptive_scale, &best_max))) return rc;
+    if (nq == 0) return DAB_OK;
+    if (!masks) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
+    DAB_CUDA(cudaSetDevice(idx->device));
+    // the sample counts distinct evaluated neighbours, data points only: past n_points it is never reached
+    const bool adaptive = adaptive_samples && adaptive_samples <= idx->n_points;
+    const uint32_t span = beam * idx->max_degree;
+    std::vector<uint16_t> table;
+    if (adaptive) table = adaptive_table(l_search, adaptive_samples, span, adaptive_scale);
+    const size_t mask_bytes = host ? round_up((size_t)nq * 8, 16) : 0;
+    if ((rc = idx->s_pools.reserve(mask_bytes + table.size() * 2 + 16))) return rc;
+    FilterSpec spec{masks, match_all, adaptive_samples, nullptr, best_max};
+    if (host) {
+        DAB_CUDA(cudaMemcpyAsync(idx->s_pools.p, masks, (size_t)nq * 8, cudaMemcpyHostToDevice, idx->stream));
+        spec.masks = (const uint64_t*)idx->s_pools.p;
+    }
+    if (adaptive) {
+        spec.adapt = (const uint16_t*)((uint8_t*)idx->s_pools.p + mask_bytes);
+        DAB_CUDA(cudaMemcpyAsync((void*)spec.adapt, table.data(), table.size() * 2, cudaMemcpyHostToDevice, idx->stream));
+    }
+    if (host) return search_host(idx, api, queries, nq, k, l_search, beam, out, -1, false, 0, &spec);
+    if ((rc = search_device(idx, api, queries, nq, k, l_search, beam, out, -1, false, 0, &spec))) return rc;
     DAB_CUDA(cudaStreamSynchronize(idx->stream));
     return DAB_OK;
 }
@@ -844,6 +939,25 @@ int dab_search_batch_diverse_minmax_device(dab_index* idx, const void* d_queries
                                            uint32_t* d_out_counts, uint32_t* d_out_cmps, uint32_t* d_out_hops) {
     return search_diverse_quant(idx, "dab_search_batch_diverse_minmax_device", false, d_queries, nq, k, l_search, beam_width, diverse_k,
                                 rerank, SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, STORE_MINMAX);
+}
+
+// InlineFilterSearch::search (inline_filter_search.rs:89-160): every argument is checked before the masks and the queries
+// are copied
+int dab_search_batch_filtered(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
+                              const uint64_t* query_masks, uint32_t match_all, uint32_t adaptive_samples, double adaptive_scale,
+                              uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps, uint32_t* out_hops) {
+    return search_filtered(idx, "dab_search_batch_filtered", true, queries, nq, k, l_search, beam_width, query_masks, match_all,
+                           adaptive_samples, adaptive_scale, SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops});
+}
+
+// query_masks is a device pointer; returns with the outputs complete, the filter of deleted ids included
+int dab_search_batch_filtered_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                                     uint32_t beam_width, const uint64_t* d_query_masks, uint32_t match_all, uint32_t adaptive_samples,
+                                     double adaptive_scale, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
+                                     uint32_t* d_out_cmps, uint32_t* d_out_hops) {
+    return search_filtered(idx, "dab_search_batch_filtered_device", false, d_queries, nq, k, l_search, beam_width, d_query_masks,
+                           match_all, adaptive_samples, adaptive_scale,
+                           SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops});
 }
 
 // ---- asynchronous batches: launch on a slot, collect with dab_wait ---------------------------

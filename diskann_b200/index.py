@@ -527,6 +527,45 @@ class GpuIndex:
                                                          C.c_void_p(d_ids), C.c_void_p(d_dists), C.c_void_p(d_counts or None),
                                                          C.c_void_p(d_cmps or None), C.c_void_p(d_hops or None)))
 
+    def upload_labels(self, labels, first=0):
+        """The 64-bit label sets of ids first .. first + len(labels) - 1 for search_batch_filtered (u64 each)."""
+        labels = np.ascontiguousarray(labels, np.uint64).ravel()
+        check(_lib.lib().dab_upload_labels(self._h, _ptr(labels), first, labels.shape[0]))
+
+    @staticmethod
+    def _adaptive(adaptive_l):
+        if adaptive_l is None:
+            return 0, 1.0
+        samples, scale = adaptive_l
+        if samples == 0:
+            raise ValueError("adaptive_l: sample count cannot be zero")
+        return int(samples), float(scale)
+
+    def search_batch_filtered(self, queries, masks, k, l_search, beam_width=1, match_all=False, adaptive_l=None):
+        """InlineFilterSearch::search for the whole batch over the label table (upload_labels): query q accepts id i when
+        labels[i] & masks[q] != 0 (match_all=False) or == masks[q] (match_all=True); `masks` u64 per query (or one for
+        all); adaptive_l: None or (samples, scale).  (ids [nq,k], dists [nq,k], counts, cmps, hops)."""
+        queries = self._queries(queries)
+        nq = queries.shape[0]
+        masks = np.ascontiguousarray(np.broadcast_to(np.asarray(masks, np.uint64), (nq,)))
+        samples, scale = self._adaptive(adaptive_l)
+        ids = np.empty((nq, k), np.uint32)
+        dists = np.empty((nq, k), np.float32)
+        counts, cmps, hops = (np.empty(nq, np.uint32) for _ in range(3))
+        check(_lib.lib().dab_search_batch_filtered(self._h, _ptr(queries), nq, k, l_search, beam_width, _ptr(masks), int(bool(match_all)),
+                                                   samples, scale, _ptr(ids), _ptr(dists), _ptr(counts), _ptr(cmps), _ptr(hops)))
+        return ids, dists, counts, cmps, hops
+
+    def search_batch_filtered_device(self, d_queries, nq, k, l_search, beam_width, d_masks, d_ids, d_dists, d_counts=0, d_cmps=0,
+                                     d_hops=0, match_all=False, adaptive_l=None):
+        """search_batch_filtered with device pointers (integers), the masks included; results stay in HBM, complete on
+        return."""
+        samples, scale = self._adaptive(adaptive_l)
+        check(_lib.lib().dab_search_batch_filtered_device(self._h, C.c_void_p(d_queries), nq, k, l_search, beam_width, C.c_void_p(d_masks),
+                                                          int(bool(match_all)), samples, scale, C.c_void_p(d_ids), C.c_void_p(d_dists),
+                                                          C.c_void_p(d_counts or None), C.c_void_p(d_cmps or None),
+                                                          C.c_void_p(d_hops or None)))
+
     def _diverse_quant(self, store, queries, k, l_search, diverse_k, beam_width, rerank):
         queries = self._queries(queries)
         nq = queries.shape[0]

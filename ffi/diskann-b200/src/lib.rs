@@ -237,6 +237,30 @@ impl<T: Element> GpuIndex<T> {
         Ok(b)
     }
 
+    /// The 64-bit label sets of ids `first ..` for `search_batch_filtered`.
+    pub fn upload_labels(&mut self, labels: &[u64], first: u64) -> Result<()> {
+        check(unsafe { sys::dab_upload_labels(self.raw, labels.as_ptr(), first, labels.len() as u64) })
+    }
+
+    /// `InlineFilterSearch::search` (inline_filter_search.rs:89-160): query q accepts id i when `labels[i] & masks[q]` is
+    /// non-zero (`match_all` false) or equals `masks[q]` (`match_all` true); `adaptive_l`: `None` or `(samples, scale)`,
+    /// the reference's `AdaptiveL` (samples >= 1).
+    pub fn search_batch_filtered(&self, queries: &[T], masks: &[u64], k: usize, l_search: u32, beam_width: u32, match_all: bool,
+                                 adaptive_l: Option<(u32, f64)>) -> Result<Batch> {
+        assert_eq!(queries.len() % self.dim, 0);
+        let nq = queries.len() / self.dim;
+        assert_eq!(masks.len(), nq);
+        let (samples, scale) = adaptive_l.unwrap_or((0, 1.0));
+        assert!(adaptive_l.is_none() || samples > 0, "AdaptiveL: sample count cannot be zero");
+        let mut b = Batch { k, ids: vec![0; nq * k], dists: vec![0.0; nq * k], counts: vec![0; nq], cmps: vec![0; nq], hops: vec![0; nq] };
+        check(unsafe {
+            sys::dab_search_batch_filtered(self.raw, queries.as_ptr() as *const c_void, nq as u32, k as u32, l_search, beam_width,
+                                           masks.as_ptr(), match_all as u32, samples, scale, b.ids.as_mut_ptr(), b.dists.as_mut_ptr(),
+                                           b.counts.as_mut_ptr(), b.cmps.as_mut_ptr(), b.hops.as_mut_ptr())
+        })?;
+        Ok(b)
+    }
+
     /// `Range::search` (range_search.rs:255-469) for the batch: every point within `radius` of each query, query q's
     /// results at `offsets[q] .. offsets[q + 1]` in the reference's output order.
     pub fn range_search(&self, queries: &[T], l_search: u32, radius: f32, args: RangeArgs) -> Result<RangeBatch> {

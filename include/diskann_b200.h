@@ -251,6 +251,53 @@ int dab_search_batch_diverse_minmax_device(dab_index* idx, const void* d_queries
                                            float* d_out_dists, uint32_t* d_out_counts,
                                            uint32_t* d_out_cmps, uint32_t* d_out_hops);
 
+/* ------------------------------------------------------------------ (3''''') filtered search */
+
+/* The label table of filtered search: one 64-bit label set per id, over every id of the index
+ * (start points included).  Ids [first, first + count) take labels[i];
+ * first + count <= n_points + n_start.  The first call allocates the table with every set empty
+ * (8 bytes per id).  The table is independent of the graph: inserts, deletes and releases neither
+ * read nor clear it. */
+int dab_upload_labels(dab_index* idx, const uint64_t* labels, uint64_t first, uint64_t count);
+
+/* InlineFilterSearch::search (diskann/src/graph/search/inline_filter_search.rs:89-160) for a whole
+ * query batch over full-precision rows of every dtype and metric.  Query q accepts id i when
+ *   match_all == 0 (ANY): labels[i] & query_masks[q] != 0;
+ *   match_all != 0 (ALL): labels[i] & query_masks[q] == query_masks[q] (an empty mask accepts all).
+ * The traversal is the k-NN traversal of dab_search_batch (inline_filter_search_internal,
+ * :166-282): every evaluated neighbour enters the list of L + n_start entries, accepted or not;
+ * the accepted start points and neighbours are also kept as matches.  Results: the first L
+ * matches by distance, start points and deleted ids dropped, the first k kept; a query can
+ * return fewer than k.  Among matches at exactly equal distances an earlier match comes first
+ * (the reference's sort_unstable leaves that order open), and NaN distances come last.  cmps
+ * counts the evaluated neighbours (start points are not counted, as in the reference), hops the
+ * expanded nodes.
+ * adaptive_samples == 0: no AdaptiveL.  Otherwise AdaptiveL(adaptive_samples, adaptive_scale):
+ * after the hop in which the evaluated neighbours reach adaptive_samples, L' =
+ * compute_adaptive_l(L, evaluated, accepted, adaptive_scale) (:294-310), computed on the host in
+ * the reference's f64 expression; when L' > L the list's capacity becomes L' and a longer list is
+ * cut to L' (NeighborPriorityQueue::reconfigure, neighbor/queue.rs:339-353).
+ * Checked before any device work, each failing with DAB_ERR_INVALID_ARGUMENT and a message: k >= 1,
+ * k <= l_search, 1 <= beam_width <= 64, adaptive_scale >= 1.0 (when adaptive), a label table was
+ * uploaded, l_search + n_start <= 1024 and floor(l_search * adaptive_scale) <= 1024 (when
+ * adaptive), and a CTA's shared memory fits 200 KB: 4 x (query row (f32 for float rows, the bytes
+ * for i8 / u8) + 8 * the longest list + 8 * l_search + 12 * max(beam_width * max_degree, 32) +
+ * 4 * beam_width bytes, each part rounded up to 16, the whole to 128).  Outputs as
+ * dab_search_batch; query_masks holds nq host words. */
+int dab_search_batch_filtered(dab_index* idx, const void* queries, uint32_t nq, uint32_t k,
+                              uint32_t l_search, uint32_t beam_width, const uint64_t* query_masks,
+                              uint32_t match_all, uint32_t adaptive_samples, double adaptive_scale,
+                              uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
+                              uint32_t* out_cmps, uint32_t* out_hops);
+/* the same with device buffers, d_query_masks included; returns with the outputs complete */
+int dab_search_batch_filtered_device(dab_index* idx, const void* d_queries, uint32_t nq,
+                                     uint32_t k, uint32_t l_search, uint32_t beam_width,
+                                     const uint64_t* d_query_masks, uint32_t match_all,
+                                     uint32_t adaptive_samples, double adaptive_scale,
+                                     uint32_t* d_out_ids, float* d_out_dists,
+                                     uint32_t* d_out_counts, uint32_t* d_out_cmps,
+                                     uint32_t* d_out_hops);
+
 /* ------------------------------------------------------------------ (3'''') range search */
 
 /* Range::search (diskann/src/graph/search/range_search.rs:255-469) for a whole query batch over

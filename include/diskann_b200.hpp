@@ -167,6 +167,9 @@ class Provider {
         check(dab_upload_attributes(h_, values, present, first, count));
     }
 
+    // the 64-bit label sets of ids [first, first + count) for filtered search
+    void set_labels(const uint64_t* labels, uint64_t first, uint64_t count) { check(dab_upload_labels(h_, labels, first, count)); }
+
     // index construction on the device (multi_insert semantics)
     void build(uint32_t pruned_degree, uint32_t l_build, float alpha = 1.2f, uint32_t batch = 0) {
         check(dab_build(h_, pruned_degree, l_build, alpha, batch));
@@ -369,6 +372,34 @@ class GpuDiverse {
 
     Provider<T>& p_;
     uint32_t l_, diverse_k_, beam_;
+};
+
+// InlineFilterSearch::search for a whole batch (inline_filter_search.rs:89-160): InlineFilterSearch::new(Knn::new(l_value,
+// beam_width), adaptive L), over the provider's labels (set_labels).  Query q accepts id i when labels[i] & masks[q] != 0
+// (match_all false) or == masks[q] (match_all true).  adaptive_samples == 0: no AdaptiveL.
+template <class T>
+class GpuFiltered {
+   public:
+    GpuFiltered(Provider<T>& provider, uint32_t l_value, uint32_t beam_width = 1, uint32_t adaptive_samples = 0, double adaptive_scale = 1.0)
+        : p_(provider), l_(l_value), beam_(beam_width), samples_(adaptive_samples), scale_(adaptive_scale) {}
+    KnnResults search(const T* queries, const uint64_t* masks, uint32_t nq, uint32_t k, bool match_all = false) {
+        KnnResults r;
+        r.nq = nq;
+        r.k = k;
+        r.ids.resize((size_t)nq * k);
+        r.distances.resize((size_t)nq * k);
+        std::vector<uint32_t> counts(nq), cmps(nq), hops(nq);
+        check(dab_search_batch_filtered(p_.raw(), queries, nq, k, l_, beam_, masks, match_all ? 1 : 0, samples_, scale_, r.ids.data(),
+                                        r.distances.data(), counts.data(), cmps.data(), hops.data()));
+        r.stats.resize(nq);
+        for (uint32_t i = 0; i < nq; ++i) r.stats[i] = SearchStats{cmps[i], hops[i], counts[i]};
+        return r;
+    }
+
+   private:
+    Provider<T>& p_;
+    uint32_t l_, beam_, samples_;
+    double scale_;
 };
 
 // KNN::search for a whole batch: Knn::new(l_value, beam_width) + k results per query.

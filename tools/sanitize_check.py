@@ -69,6 +69,9 @@ for dt, ddt, metric, d in ((np.float32, dab.DType.f32, dab.Metric.L2, 100), (np.
         g.upload_attributes(rng.integers(0, 7, n + 1), rng.random(n + 1) < 0.9)
         div = g.search_batch_diverse(base[:64], 5, 40, 2, 1)     # diverse_kernel
         div4 = g.search_batch_diverse(base[:64], 5, 300, 1, 4)
+        g.upload_labels(rng.integers(0, 1 << 8, n + 1).astype(np.uint64))
+        flt = g.search_batch_filtered(base[:64], 0b101, 5, 40, 1)  # filtered_kernel
+        flt4 = g.search_batch_filtered(base[:64], 0b11, 5, 40, 4, match_all=True, adaptive_l=(50, 8.0))
         rad = float(np.median(got[1][:, 4]))                     # range_kernel, range_scan, range_compact
         rng1 = g.range_search(base[:64], 20, rad, initial_slack=0.2)
         rng4 = g.range_search(base[:64], 10, rad * 2, beam_width=4, max_returned=70)
@@ -97,5 +100,6 @@ for dt, ddt, metric, d in ((np.float32, dab.DType.f32, dab.Metric.L2, 100), (np.
             g.range_search_sq(base[:32], 20, rad * 2, beam_width=4, initial_slack=0.2, rerank=rr)  # range_kernel_quant<1> and <2>
             g.range_search_minmax(base[:32], 10, rad * 2, max_returned=70, initial_slack=0.2, rerank=rr)
         print(dt.__name__, "deg max", int(adj[:, 0].max()), "search ok", int(got[2].min()), int(got4[2].min()), int(div[2].min()), int(div4[2].min()),
+              "filtered", int(flt[2].sum()), int(flt4[2].sum()),
               "finite", bool(np.isfinite(out[1:]).all() and np.isfinite(pairs).all() and np.isfinite(block).all()), knn[0].shape)
 print("sanitize_check done")
