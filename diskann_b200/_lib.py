@@ -51,6 +51,15 @@ SYMBOLS = {
     "dab_upload_labels": (_i, [_vp, _vp, _u64, _u64]),
     "dab_search_batch_filtered": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _vp, _u32, _u32, C.c_double, _vp, _vp, _vp, _vp, _vp]),
     "dab_search_batch_filtered_device": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _vp, _u32, _u32, C.c_double, _vp, _vp, _vp, _vp, _vp]),
+    "dab_search_batch_filtered_pq": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _vp, _u32, _u32, C.c_double, _i, _vp, _vp, _vp, _vp, _vp]),
+    "dab_search_batch_filtered_pq_device": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _vp, _u32, _u32, C.c_double, _i, _vp, _vp, _vp, _vp,
+                                                 _vp]),
+    "dab_search_batch_filtered_sq": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _vp, _u32, _u32, C.c_double, _i, _vp, _vp, _vp, _vp, _vp]),
+    "dab_search_batch_filtered_sq_device": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _vp, _u32, _u32, C.c_double, _i, _vp, _vp, _vp, _vp,
+                                                 _vp]),
+    "dab_search_batch_filtered_minmax": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _vp, _u32, _u32, C.c_double, _i, _vp, _vp, _vp, _vp, _vp]),
+    "dab_search_batch_filtered_minmax_device": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _vp, _u32, _u32, C.c_double, _i, _vp, _vp, _vp,
+                                                     _vp, _vp]),
     "dab_search_batch_async": (_i, [_vp, _u32, _vp, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
     "dab_search_batch_device_async": (_i, [_vp, _u32, _vp, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
     "dab_wait": (_i, [_vp, _u32]),

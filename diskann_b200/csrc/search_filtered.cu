@@ -2,9 +2,10 @@
 // inline_filter_search.rs:89-160), i.e. inline_filter_search_internal (:166-282) with its optional AdaptiveL, then the
 // default post-processing of the first L matches; and the label table it reads (dab_upload_labels).
 //
-// One warp per query on global visited tables, over full-precision rows of every type and metric of the k-NN path.  The
-// traversal is search_internal's: every evaluated neighbour enters the list, accepted or not.  Next to it the warp keeps,
-// in shared memory:
+// One warp per query on global visited tables, over full-precision rows of every type and metric of the k-NN path
+// (filtered_kernel) or the PQ, SQ and MinMax stores with the distances of their k-NN traversal and an optional
+// full-precision rerank of the first L matches (filtered_kernel_quant).  The traversal is search_internal's: every
+// evaluated neighbour enters the list, accepted or not.  Next to it the warp keeps, in shared memory:
 //   the matched list  the accepted start points and neighbours, at most L of them, ordered by distance with a later
 //                     match after an earlier one at an equal distance (-0.0 equal to +0.0, NaN after every number).
 //                     That is a stable sort of all matches followed by take(L): the reference sorts with
@@ -16,6 +17,7 @@
 // (queue.rs:339-353) cuts a longer list, so a "grown" L below L + #start shortens it.  A query whose visited set outgrows
 // its table is re-run from its start points by the job, and so takes the same decision again.
 #include "dab_common.cuh"
+#include "quant_device.cuh"
 #include "search_common.cuh"
 #include "search_filtered.cuh"
 #include "search_host.cuh"
@@ -94,7 +96,8 @@ __device__ __forceinline__ void matched_merge(float* md, uint32_t* mi, uint32_t 
 }
 
 // One warp's share of a pass.  Src is the distance source of diverse search: load(q), prepare(), distances(cid, cd, n).
-template <class Src>
+// LIST: with p.list_ids, the matched list of each query (start points included) is written for the rerank.
+template <bool LIST, class Src>
 __device__ __forceinline__ void filtered_queries(const SearchParamsFiltered& p, uint8_t* base, int lane, Src& src) {
     const int wib = threadIdx.x >> 5;
     float* bd = reinterpret_cast<float*>(base + p.off_bd);
@@ -196,6 +199,9 @@ __device__ __forceinline__ void filtered_queries(const SearchParamsFiltered& p, 
             report_overflow(p.counters, p.overflow_list, qidx, lane);
             continue;
         }
+        if constexpr (LIST) {
+            if (p.list_ids) write_list(mi, msize, p.list_ids, p.list_counts, p.list_cap, qidx, lane);
+        }
         // post-processing of matched_results.take(L): start points dropped, the first k kept
         const uint32_t count = write_results(mi, md, msize, p.n_points, p.k, p.out_ids, p.out_dists, qidx, lane);
         write_stats(p.counters, nvisited, p.out_counts, p.out_cmps, p.out_hops, qidx, count, cmps, hops, lane);
@@ -241,7 +247,51 @@ __global__ void __launch_bounds__(kFiltWarps * 32) filtered_kernel(const SearchP
             __syncwarp();
         }
     } src{p, reinterpret_cast<float*>(base), lane, (int)p.dim, 0};
-    filtered_queries(p, base, lane, src);
+    filtered_queries<false>(p, base, lane, src);
+}
+
+// The quantized accessors (MODE as search_kernel_pq: 0 PQ, 1 SQ, 2 MinMax), per candidate the code of quant_device.cuh,
+// one lane per candidate: the traversal distances of dab_search_batch_{pq,sq,minmax}.
+//   PQ: the query (index dtype, T: Into<f32>) in f32 at the front of the warp's shared memory; TableL2 / TableIP build
+//     the query's table once per query into the warp's own slice of p.luts (global memory, read through L2),
+//     DirectCosine reads the pivots directly.
+//   SQ / MinMax: the query's code words (and MinMax its four compensations), staged before the launch, copied to the
+//     front of the warp's shared memory; the SQ compensation stays in a register.
+template <int MODE>
+__global__ void __launch_bounds__(kFiltWarps * 32) filtered_kernel_quant(const SearchParamsFiltered p) {
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    uint8_t* base = smem + (size_t)wib * p.warp_smem;
+    const uint32_t entries = p.n_chunks * p.n_centers;
+    struct {
+        const SearchParamsFiltered& p;
+        float* qf;     // PQ: the f32 query
+        uint32_t* qc;  // SQ / MinMax: the query's code words, then (MinMax) {b, n, a, norm_squared}
+        float* lut;    // PQ tables: this warp's table
+        int lane, dim;
+        uint32_t entries;
+        float q_comp;
+        __device__ __forceinline__ void load(uint32_t q) {
+            if (MODE == 0) widen_query(p.dtype, p.queries, q, dim, qf, lane);
+            else load_query_codes<MODE>(p.query_codes + (size_t)q * p.code_stride, p.query_meta + q, p.code_stride >> 2, qc, q_comp, lane);
+        }
+        __device__ __forceinline__ void prepare() {
+            if (MODE == 0 && !p.direct_cosine) {
+                for (uint32_t t = lane; t < entries; t += 32) __stcg(lut + t, pq_table_entry(p, qf, dim, t));
+                __syncwarp();
+            }
+        }
+        __device__ __forceinline__ void distances(const uint32_t* cid, float* cd, uint32_t n) {
+            for (uint32_t c = lane; c < n; c += 32) {
+                if (MODE != 0) cd[c] = packed_code_distance<MODE>(p, qc, q_comp, cid[c]);
+                else if (p.direct_cosine) cd[c] = pq_direct_cosine(p, qf, dim, cid[c]);
+                else cd[c] = pq_table_distance(p, lut, cid[c]);
+            }
+            __syncwarp();
+        }
+    } src{p, reinterpret_cast<float*>(base), reinterpret_cast<uint32_t*>(base),
+          p.luts + (size_t)(blockIdx.x * kFiltWarps + wib) * entries, lane, (int)p.dim, entries, 0.0f};
+    filtered_queries<true>(p, base, lane, src);
 }
 
 template <typename S>
@@ -272,11 +322,15 @@ std::vector<uint16_t> adaptive_table(uint32_t l_search, uint32_t samples, uint32
     return t;
 }
 
-// A warp's shared memory: the query area (floats: dim f32; i8 / u8: the bytes rounded up to 16), the list's distances
-// and ids (best_max entries), the matched list's (L), a hop's candidate ids, distances and decisions, the beam
-static size_t filtered_warp_smem(const dab_index* idx, uint32_t l_search, uint32_t best_max, uint32_t beam, SearchParamsFiltered* p) {
+// A warp's shared memory: the query area (filtered_check_smem's comment), the list's distances and ids (best_max
+// entries), the matched list's (L), a hop's candidate ids, distances and decisions, the beam.  `store`: -1 full
+// precision, else a QuantStore.
+static size_t filtered_warp_smem(const dab_index* idx, uint32_t l_search, uint32_t best_max, uint32_t beam, int store,
+                                 SearchParamsFiltered* p) {
     const bool is_int = idx->dtype == DAB_I8 || idx->dtype == DAB_U8;
-    size_t off = is_int ? round_up(round_up((size_t)idx->dim, 4), 16) : round_up((size_t)idx->dim * 4, 16);
+    size_t off;
+    if (store == STORE_SQ || store == STORE_MINMAX) off = round_up((size_t)(store == STORE_SQ ? idx->sq : idx->mm).stride + 16, 16);
+    else off = is_int && store < 0 ? round_up(round_up((size_t)idx->dim, 4), 16) : round_up((size_t)idx->dim * 4, 16);
     const size_t best = round_up((size_t)best_max * 4, 16), matched = round_up((size_t)l_search * 4, 16);
     const size_t ncand = round_up(std::max<size_t>((size_t)beam * idx->max_degree, 32) * 4, 16);
     SearchParamsFiltered scratch;
@@ -292,25 +346,38 @@ static size_t filtered_warp_smem(const dab_index* idx, uint32_t l_search, uint32
     return round_up(off, 128);
 }
 
-int filtered_check_smem(const dab_index* idx, const char* api, uint32_t l_search, uint32_t best_max, uint32_t beam) {
-    const size_t smem = filtered_warp_smem(idx, l_search, best_max, beam, nullptr) * kFiltWarps;
+int filtered_check_smem(const dab_index* idx, const char* api, uint32_t l_search, uint32_t best_max, uint32_t beam, int store) {
+    const size_t smem = filtered_warp_smem(idx, l_search, best_max, beam, store, nullptr) * kFiltWarps;
     if (smem > kFilteredMaxSmem)
         return fail(DAB_ERR_INVALID_ARGUMENT, "%s: L=%u, longest list %u, beam_width=%u, dim=%u, max_degree=%u need %zu B shared memory per CTA (> %zu)",
                     api, l_search, best_max, beam, idx->dim, idx->max_degree, smem, kFilteredMaxSmem);
     return DAB_OK;
 }
 
-int filtered_plan(const dab_index* idx, uint32_t l_search, uint32_t best_max, uint32_t beam, SearchParamsFiltered& p, FilteredPlan& plan) {
-    p.warp_smem = (uint32_t)filtered_warp_smem(idx, l_search, best_max, beam, &p);
+// the grid of plan.kern at plan.smem_block bytes per CTA, at most max_per_sm CTAs per SM
+static int filtered_grid(const dab_index* idx, uint32_t l_search, uint32_t beam, int max_per_sm, FilteredPlan& plan) {
+    const int per_sm = plan.smem_block > kFilteredMaxSmem ? 0 : ctas_per_sm(plan.kern, kFiltWarps * 32, plan.smem_block);
+    if (per_sm < 1)
+        return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_filtered: L=%u, beam_width=%u, dim=%u need %zu B shared memory per CTA",
+                    l_search, beam, idx->dim, plan.smem_block);
+    plan.grid = std::min(per_sm, max_per_sm) * idx->sm_count;
+    return DAB_OK;
+}
+
+int filtered_plan(const dab_index* idx, uint32_t l_search, uint32_t best_max, uint32_t beam, int store, SearchParamsFiltered& p,
+                  FilteredPlan& plan) {
+    p.warp_smem = (uint32_t)filtered_warp_smem(idx, l_search, best_max, beam, store, &p);
     plan.smem_block = (size_t)p.warp_smem * kFiltWarps;
+    if (store >= 0) {
+        plan.kern = store == STORE_PQ ? filtered_kernel_quant<0> : store == STORE_SQ ? filtered_kernel_quant<1> : filtered_kernel_quant<2>;
+        // every resident warp owns a PQ table (n_chunks x n_centers f32: 32 KB at 32 x 256) that its lookups read
+        // through L2: the cap of search_kernel_pq keeps them L2-resident
+        const bool tables = store == STORE_PQ && idx->metric != DAB_COSINE;
+        return filtered_grid(idx, l_search, beam, tables ? 6 : INT32_MAX, plan);
+    }
     return visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) -> int {
         plan.kern = filtered_kernel_of<decltype(sc)>();
-        const int per_sm = plan.smem_block > kFilteredMaxSmem ? 0 : ctas_per_sm(plan.kern, kFiltWarps * 32, plan.smem_block);
-        if (per_sm < 1)
-            return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_filtered: L=%u, beam_width=%u, dim=%u need %zu B shared memory per CTA",
-                        l_search, beam, idx->dim, plan.smem_block);
-        plan.grid = per_sm * idx->sm_count;
-        return DAB_OK;
+        return filtered_grid(idx, l_search, beam, INT32_MAX, plan);
     });
 }
 

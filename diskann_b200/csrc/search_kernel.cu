@@ -2,8 +2,9 @@
 // any kind with its overflow re-runs and post-processing (full precision; PQ, SQ and MinMax, whose kernels and rerank
 // are in search_kernel_pq.cu and search_kernel_pqs.cu), the slots of batches in flight and the C entry points
 // (dab_search_batch[_pq|_pq_rerank|_sq|_minmax][_device][_async], dab_search_batch_diverse[_pq|_sq|_minmax][_device],
-// dab_search_batch_filtered[_device], dab_wait).  The diverse search (search_diverse.cu), over full-precision rows or a
-// quantized store, is one more kind of the job; so are the filtered search (search_filtered.cu) and the first phase of
+// dab_search_batch_filtered[_pq|_sq|_minmax][_device], dab_wait).  The diverse search (search_diverse.cu), over full-precision rows or a
+// quantized store, is one more kind of the job; so are the filtered search (search_filtered.cu), over full-precision
+// rows or a quantized store, and the first phase of
 // range search (search_range.cu), a batch over full-precision rows or a quantized store that keeps start points and
 // deleted ids.
 //
@@ -133,7 +134,7 @@ struct SlotJob {
     uint32_t diverse_k = 0;
     uint64_t pool = 0;
     Scratch* pools = nullptr;
-    // set: a filtered search over full-precision rows (FilterSpec, search_filtered.cuh)
+    // set: a filtered search over full-precision rows or `store` (FilterSpec, search_filtered.cuh)
     const FilterSpec* filt = nullptr;
     const void* d_queries = nullptr;
     uint32_t nq = 0, k = 0, l_search = 0, beam = 0, cap = 0;
@@ -198,6 +199,8 @@ struct SlotJob {
     int plan_quant();
     int plan_diverse();
     int plan_filtered();
+    template <class P>
+    int plan_store(P& p);
     int reserve_tables();
     int reserve_pools();
     int stage_queries();
@@ -384,32 +387,36 @@ int SlotJob::plan_diverse() {
     // and every larger one behaves the same
     pd.local_cap = (uint32_t)std::min<uint64_t>((uint64_t)diverse_k * l_search / k, idx->n_total());
     warps = (uint32_t)dplan.grid * kDivWarps;
-    if (store >= 0) {
-        // the quantized traversal: the store, a PQ table for every warp of the grid, the lists of the rerank (the
-        // post-processed list, at most L ids: list_cap = cap = L) and the staging of the queries
-        const QuantStore mode = (QuantStore)store;
-        pd.dtype = idx->dtype;
-        set_store_params(idx, mode, pd);
-        const size_t lut_bytes = mode == STORE_PQ && !pd.direct_cosine ? (size_t)warps * idx->pq_chunks * idx->pq_centers * 4 : 16;
-        if ((rc = luts->reserve(lut_bytes))) return rc;
-        pd.luts = (float*)luts->p;
-        if (rerank) {
-            if ((rc = lists->reserve(((size_t)nq * cap + nq) * 4))) return rc;
-            pd.list_ids = (uint32_t*)lists->p;
-            pd.list_counts = pd.list_ids + (size_t)nq * cap;
-            pd.list_cap = cap;
-        }
-        if ((rc = stage->reserve(mode == STORE_SQ ? sq_stage_bytes(idx, nq) : mode == STORE_MINMAX ? minmax_stage_bytes(idx, nq) : 0))) return rc;
-    }
+    if (store >= 0 && (rc = plan_store(pd))) return rc;
     pool = diverse_pool_first(idx, l_search);
     return reserve_pools();
 }
 
-// filtered: the kernel's plan, the label table, the masks and adaptive L's table
+// A diverse or filtered traversal over `store` (the `warps` of its grid planned): the store, a PQ table for every warp
+// of the grid, the lists of the rerank (at most L ids a query: list_cap = cap = L) and the staging of the queries
+template <class P>
+int SlotJob::plan_store(P& p) {
+    const QuantStore mode = (QuantStore)store;
+    p.dtype = idx->dtype;
+    set_store_params(idx, mode, p);
+    int rc;
+    const size_t lut_bytes = mode == STORE_PQ && !p.direct_cosine ? (size_t)warps * idx->pq_chunks * idx->pq_centers * 4 : 16;
+    if ((rc = luts->reserve(lut_bytes))) return rc;
+    p.luts = (float*)luts->p;
+    if (rerank) {
+        if ((rc = lists->reserve(((size_t)nq * cap + nq) * 4))) return rc;
+        p.list_ids = (uint32_t*)lists->p;
+        p.list_counts = p.list_ids + (size_t)nq * cap;
+        p.list_cap = cap;
+    }
+    return stage->reserve(mode == STORE_SQ ? sq_stage_bytes(idx, nq) : mode == STORE_MINMAX ? minmax_stage_bytes(idx, nq) : 0);
+}
+
+// filtered: the kernel's plan, the label table, the masks and adaptive L's table; over a store, plan_store's buffers
 int SlotJob::plan_filtered() {
     memset(&pf, 0, sizeof(pf));
     int rc;
-    if ((rc = filtered_plan(idx, l_search, filt->best_max, beam, pf, fplan))) return rc;
+    if ((rc = filtered_plan(idx, l_search, filt->best_max, beam, store, pf, fplan))) return rc;
     set_batch_params(pf);
     pf.vectors = idx->d_vectors;
     pf.row_stride = idx->row_stride;
@@ -421,7 +428,7 @@ int SlotJob::plan_filtered() {
     pf.span = beam * idx->max_degree;
     pf.adapt = filt->adapt;
     warps = (uint32_t)fplan.grid * kFiltWarps;
-    return DAB_OK;
+    return store >= 0 ? plan_store(pf) : DAB_OK;
 }
 
 // the local queues of the warps the next pass over n_work queries launches (diverse_launch's grid)
@@ -442,8 +449,8 @@ int SlotJob::reserve_tables() {
 
 // SQ and MinMax: the batch's queries compressed by the store's quantizer (MinMax: the NaN flag read back into h_counters)
 int SlotJob::stage_queries() {
-    const uint8_t** codes = diverse_k ? &pd.query_codes : &pq.query_codes;
-    const float4** meta = diverse_k ? &pd.query_meta : &pq.query_meta;
+    const uint8_t** codes = filt ? &pf.query_codes : diverse_k ? &pd.query_codes : &pq.query_codes;
+    const float4** meta = filt ? &pf.query_meta : diverse_k ? &pd.query_meta : &pq.query_meta;
     if (store == STORE_SQ) return sq_stage_queries(idx, stream, *stage, d_queries, nq, codes, meta);
     if (store == STORE_MINMAX)
         return minmax_stage_queries(idx, stream, *stage, d_queries, nq, (unsigned long long*)(h_counters + 4), codes, meta);
@@ -496,8 +503,8 @@ int SlotJob::launch_filtered() {
 // the post-processing of the whole batch: the rerank, or the filter of deleted ids
 int SlotJob::post() {
     if (rerank) {
-        const uint32_t* list_ids = diverse_k ? pd.list_ids : pq.list_ids;
-        const uint32_t* list_counts = diverse_k ? pd.list_counts : pq.list_counts;
+        const uint32_t* list_ids = filt ? pf.list_ids : diverse_k ? pd.list_ids : pq.list_ids;
+        const uint32_t* list_counts = filt ? pf.list_counts : diverse_k ? pd.list_counts : pq.list_counts;
         return launch_rerank(idx, stream, d_queries, nq, k, cap, list_ids, list_counts, out.ids, out.dists, out.counts, deleted);
     }
     if (filter) return queue_drop_deleted(idx, stream, deleted, out.ids, out.dists, cap, nq, k, filtered, idx->n_points);
@@ -679,12 +686,13 @@ static int search_diverse_quant(dab_index* idx, const char* api, bool host, cons
 
 // The checks of a filtered search, all made before any device work: InlineFilterSearch's (k >= 1 and L >= k from Knn::new,
 // scale >= 1.0 from AdaptiveL::new, which a NaN scale does not pass either), the label table, and what the kernel holds:
-// L + #start and floor(L * scale) at most kFilteredMaxL, and its shared memory.  *best_max: the longest list.
+// L + #start and floor(L * scale) at most kFilteredMaxL, and its shared memory.  *best_max: the longest list.  Over a
+// quantized store (`store` >= 0) the store checks of the synchronous quantized call follow, reported under `api`.
 static int check_filtered_args(const dab_index* idx, const char* api, uint32_t k, uint32_t l_search, uint32_t beam,
-                               uint32_t adaptive_samples, double adaptive_scale, uint32_t* best_max) {
+                               uint32_t adaptive_samples, double adaptive_scale, uint32_t* best_max, int store, bool rerank) {
     if (!idx) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: idx is NULL", api);
     int rc;
-    if ((rc = check_search_args(idx, k, l_search, beam))) return rc;
+    if ((rc = check_search_args(idx, k, l_search, beam, store < 0))) return rc;
     if (l_search < k) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: l_value (%u) must be greater than or equal to k_value (%u)", api, l_search, k);
     if (adaptive_samples && !(adaptive_scale >= 1.0)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: adaptive L scale factor must be >= 1.0", api);
     if (!idx->d_labels) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: no label table (dab_upload_labels has not been called)", api);
@@ -697,17 +705,26 @@ static int check_filtered_args(const dab_index* idx, const char* api, uint32_t k
             return fail(DAB_ERR_INVALID_ARGUMENT, "%s: floor(L * scale) = %.17g > %u", api, grown, kFilteredMaxL);
         *best_max = std::max(*best_max, (uint32_t)grown);
     }
-    return filtered_check_smem(idx, api, l_search, *best_max, beam);
+    if ((rc = filtered_check_smem(idx, api, l_search, *best_max, beam, store))) return rc;
+    if (store < 0) return DAB_OK;
+    if ((rc = check_quant_store(idx, (QuantStore)store, api, false))) return rc;
+    if (rerank) {
+        if (!idx->vectors_ready) return fail(DAB_ERR_NOT_READY, "%s: rerank needs the full-precision vectors", api);
+        if ((rc = check_rerank(idx, l_search))) return rc;
+    }
+    return DAB_OK;
 }
 
 // InlineFilterSearch::search over a batch: the checks, then the masks (host call: copied to the handle's scratch) and
-// adaptive L's table on the device, then the job.  The device form returns with its outputs complete.
+// adaptive L's table on the device, then the job.  `store` -1: full-precision rows, else the traversal reads that store
+// and `rerank` reorders the first L matches by full-precision distance.  The device form returns with its outputs
+// complete.
 static int search_filtered(dab_index* idx, const char* api, bool host, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search,
                            uint32_t beam, const uint64_t* masks, uint32_t match_all, uint32_t adaptive_samples, double adaptive_scale,
-                           const SearchOut& out) {
+                           const SearchOut& out, int store = -1, bool rerank = false) {
     uint32_t best_max = 0;
     int rc;
-    if ((rc = check_filtered_args(idx, api, k, l_search, beam, adaptive_samples, adaptive_scale, &best_max))) return rc;
+    if ((rc = check_filtered_args(idx, api, k, l_search, beam, adaptive_samples, adaptive_scale, &best_max, store, rerank))) return rc;
     if (nq == 0) return DAB_OK;
     if (!masks) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
     DAB_CUDA(cudaSetDevice(idx->device));
@@ -727,8 +744,8 @@ static int search_filtered(dab_index* idx, const char* api, bool host, const voi
         spec.adapt = (const uint16_t*)((uint8_t*)idx->s_pools.p + mask_bytes);
         DAB_CUDA(cudaMemcpyAsync((void*)spec.adapt, table.data(), table.size() * 2, cudaMemcpyHostToDevice, idx->stream));
     }
-    if (host) return search_host(idx, api, queries, nq, k, l_search, beam, out, -1, false, 0, &spec);
-    if ((rc = search_device(idx, api, queries, nq, k, l_search, beam, out, -1, false, 0, &spec))) return rc;
+    if (host) return search_host(idx, api, queries, nq, k, l_search, beam, out, store, rerank, 0, &spec);
+    if ((rc = search_device(idx, api, queries, nq, k, l_search, beam, out, store, rerank, 0, &spec))) return rc;
     DAB_CUDA(cudaStreamSynchronize(idx->stream));
     return DAB_OK;
 }
@@ -958,6 +975,62 @@ int dab_search_batch_filtered_device(dab_index* idx, const void* d_queries, uint
     return search_filtered(idx, "dab_search_batch_filtered_device", false, d_queries, nq, k, l_search, beam_width, d_query_masks,
                            match_all, adaptive_samples, adaptive_scale,
                            SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops});
+}
+
+// InlineFilterSearch::search over the PQ, SQ and MinMax stores: the traversal distances of dab_search_batch_{pq,sq,minmax};
+// rerank != 0 runs Pipeline<FilterStartPoints, Rerank> over the first L matches
+int dab_search_batch_filtered_pq(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
+                                 const uint64_t* query_masks, uint32_t match_all, uint32_t adaptive_samples, double adaptive_scale,
+                                 int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps,
+                                 uint32_t* out_hops) {
+    return search_filtered(idx, "dab_search_batch_filtered_pq", true, queries, nq, k, l_search, beam_width, query_masks, match_all,
+                           adaptive_samples, adaptive_scale, SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, STORE_PQ,
+                           rerank != 0);
+}
+
+int dab_search_batch_filtered_pq_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                                        uint32_t beam_width, const uint64_t* d_query_masks, uint32_t match_all, uint32_t adaptive_samples,
+                                        double adaptive_scale, int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
+                                        uint32_t* d_out_cmps, uint32_t* d_out_hops) {
+    return search_filtered(idx, "dab_search_batch_filtered_pq_device", false, d_queries, nq, k, l_search, beam_width, d_query_masks,
+                           match_all, adaptive_samples, adaptive_scale,
+                           SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, STORE_PQ, rerank != 0);
+}
+
+int dab_search_batch_filtered_sq(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
+                                 const uint64_t* query_masks, uint32_t match_all, uint32_t adaptive_samples, double adaptive_scale,
+                                 int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps,
+                                 uint32_t* out_hops) {
+    return search_filtered(idx, "dab_search_batch_filtered_sq", true, queries, nq, k, l_search, beam_width, query_masks, match_all,
+                           adaptive_samples, adaptive_scale, SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, STORE_SQ,
+                           rerank != 0);
+}
+
+int dab_search_batch_filtered_sq_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                                        uint32_t beam_width, const uint64_t* d_query_masks, uint32_t match_all, uint32_t adaptive_samples,
+                                        double adaptive_scale, int rerank, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
+                                        uint32_t* d_out_cmps, uint32_t* d_out_hops) {
+    return search_filtered(idx, "dab_search_batch_filtered_sq_device", false, d_queries, nq, k, l_search, beam_width, d_query_masks,
+                           match_all, adaptive_samples, adaptive_scale,
+                           SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, STORE_SQ, rerank != 0);
+}
+
+int dab_search_batch_filtered_minmax(dab_index* idx, const void* queries, uint32_t nq, uint32_t k, uint32_t l_search, uint32_t beam_width,
+                                     const uint64_t* query_masks, uint32_t match_all, uint32_t adaptive_samples, double adaptive_scale,
+                                     int rerank, uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint32_t* out_cmps,
+                                     uint32_t* out_hops) {
+    return search_filtered(idx, "dab_search_batch_filtered_minmax", true, queries, nq, k, l_search, beam_width, query_masks, match_all,
+                           adaptive_samples, adaptive_scale, SearchOut{out_ids, out_dists, out_counts, out_cmps, out_hops}, STORE_MINMAX,
+                           rerank != 0);
+}
+
+int dab_search_batch_filtered_minmax_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t k, uint32_t l_search,
+                                            uint32_t beam_width, const uint64_t* d_query_masks, uint32_t match_all,
+                                            uint32_t adaptive_samples, double adaptive_scale, int rerank, uint32_t* d_out_ids,
+                                            float* d_out_dists, uint32_t* d_out_counts, uint32_t* d_out_cmps, uint32_t* d_out_hops) {
+    return search_filtered(idx, "dab_search_batch_filtered_minmax_device", false, d_queries, nq, k, l_search, beam_width, d_query_masks,
+                           match_all, adaptive_samples, adaptive_scale,
+                           SearchOut{d_out_ids, d_out_dists, d_out_counts, d_out_cmps, d_out_hops}, STORE_MINMAX, rerank != 0);
 }
 
 // ---- asynchronous batches: launch on a slot, collect with dab_wait ---------------------------

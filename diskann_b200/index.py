@@ -566,6 +566,61 @@ class GpuIndex:
                                                           C.c_void_p(d_counts or None), C.c_void_p(d_cmps or None),
                                                           C.c_void_p(d_hops or None)))
 
+    def _filtered_quant(self, store, queries, masks, k, l_search, beam_width, match_all, adaptive_l, rerank):
+        queries = self._queries(queries)
+        nq = queries.shape[0]
+        masks = np.ascontiguousarray(np.broadcast_to(np.asarray(masks, np.uint64), (nq,)))
+        samples, scale = self._adaptive(adaptive_l)
+        ids = np.empty((nq, k), np.uint32)
+        dists = np.empty((nq, k), np.float32)
+        counts, cmps, hops = (np.empty(nq, np.uint32) for _ in range(3))
+        fn = getattr(_lib.lib(), f"dab_search_batch_filtered_{store}")
+        check(fn(self._h, _ptr(queries), nq, k, l_search, beam_width, _ptr(masks), int(bool(match_all)), samples, scale, int(bool(rerank)),
+                 _ptr(ids), _ptr(dists), _ptr(counts), _ptr(cmps), _ptr(hops)))
+        return ids, dists, counts, cmps, hops
+
+    def _filtered_quant_device(self, store, d_queries, nq, k, l_search, beam_width, d_masks, d_ids, d_dists, d_counts, d_cmps, d_hops,
+                               match_all, adaptive_l, rerank):
+        samples, scale = self._adaptive(adaptive_l)
+        fn = getattr(_lib.lib(), f"dab_search_batch_filtered_{store}_device")
+        check(fn(self._h, C.c_void_p(d_queries), nq, k, l_search, beam_width, C.c_void_p(d_masks), int(bool(match_all)), samples, scale,
+                 int(bool(rerank)), C.c_void_p(d_ids), C.c_void_p(d_dists), C.c_void_p(d_counts or None), C.c_void_p(d_cmps or None),
+                 C.c_void_p(d_hops or None)))
+
+    def search_batch_filtered_pq(self, queries, masks, k, l_search, beam_width=1, match_all=False, adaptive_l=None, rerank=False):
+        """search_batch_filtered with the traversal distances of search_batch_pq (PQ store); rerank=True reranks the
+        first L matches by full-precision distance."""
+        return self._filtered_quant("pq", queries, masks, k, l_search, beam_width, match_all, adaptive_l, rerank)
+
+    def search_batch_filtered_sq(self, queries, masks, k, l_search, beam_width=1, match_all=False, adaptive_l=None, rerank=False):
+        """search_batch_filtered with the traversal distances of search_batch_sq (scalar-quantized store)."""
+        return self._filtered_quant("sq", queries, masks, k, l_search, beam_width, match_all, adaptive_l, rerank)
+
+    def search_batch_filtered_minmax(self, queries, masks, k, l_search, beam_width=1, match_all=False, adaptive_l=None, rerank=False):
+        """search_batch_filtered with the traversal distances of search_batch_minmax (MinMax store)."""
+        return self._filtered_quant("minmax", queries, masks, k, l_search, beam_width, match_all, adaptive_l, rerank)
+
+    def search_batch_filtered_pq_device(self, d_queries, nq, k, l_search, beam_width, d_masks, d_ids, d_dists, d_counts=0, d_cmps=0,
+                                        d_hops=0, match_all=False, adaptive_l=None, rerank=False):
+        """search_batch_filtered_pq with device pointers (integers), the masks included; results stay in HBM, complete on
+        return."""
+        self._filtered_quant_device("pq", d_queries, nq, k, l_search, beam_width, d_masks, d_ids, d_dists, d_counts, d_cmps, d_hops,
+                                    match_all, adaptive_l, rerank)
+
+    def search_batch_filtered_sq_device(self, d_queries, nq, k, l_search, beam_width, d_masks, d_ids, d_dists, d_counts=0, d_cmps=0,
+                                        d_hops=0, match_all=False, adaptive_l=None, rerank=False):
+        """search_batch_filtered_sq with device pointers (integers), the masks included; results stay in HBM, complete on
+        return."""
+        self._filtered_quant_device("sq", d_queries, nq, k, l_search, beam_width, d_masks, d_ids, d_dists, d_counts, d_cmps, d_hops,
+                                    match_all, adaptive_l, rerank)
+
+    def search_batch_filtered_minmax_device(self, d_queries, nq, k, l_search, beam_width, d_masks, d_ids, d_dists, d_counts=0, d_cmps=0,
+                                            d_hops=0, match_all=False, adaptive_l=None, rerank=False):
+        """search_batch_filtered_minmax with device pointers (integers), the masks included; results stay in HBM, complete
+        on return."""
+        self._filtered_quant_device("minmax", d_queries, nq, k, l_search, beam_width, d_masks, d_ids, d_dists, d_counts, d_cmps, d_hops,
+                                    match_all, adaptive_l, rerank)
+
     def _diverse_quant(self, store, queries, k, l_search, diverse_k, beam_width, rerank):
         queries = self._queries(queries)
         nq = queries.shape[0]

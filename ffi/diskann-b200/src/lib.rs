@@ -261,6 +261,45 @@ impl<T: Element> GpuIndex<T> {
         Ok(b)
     }
 
+    /// `search_batch_filtered` with the traversal distances of `search_batch_pq` (the PQ store); `rerank`: the
+    /// full-precision `Rerank` of the first L matches.
+    #[allow(clippy::too_many_arguments)]
+    pub fn search_batch_filtered_pq(&self, queries: &[T], masks: &[u64], k: usize, l_search: u32, beam_width: u32, match_all: bool,
+                                    adaptive_l: Option<(u32, f64)>, rerank: bool) -> Result<Batch> {
+        self.filtered_quantized(sys::dab_search_batch_filtered_pq, queries, masks, k, l_search, beam_width, match_all, adaptive_l, rerank)
+    }
+
+    /// `search_batch_filtered` with the traversal distances of `search_batch_sq` (the scalar-quantized store).
+    #[allow(clippy::too_many_arguments)]
+    pub fn search_batch_filtered_sq(&self, queries: &[T], masks: &[u64], k: usize, l_search: u32, beam_width: u32, match_all: bool,
+                                    adaptive_l: Option<(u32, f64)>, rerank: bool) -> Result<Batch> {
+        self.filtered_quantized(sys::dab_search_batch_filtered_sq, queries, masks, k, l_search, beam_width, match_all, adaptive_l, rerank)
+    }
+
+    /// `search_batch_filtered` with the traversal distances of `search_batch_minmax` (the MinMax store).
+    #[allow(clippy::too_many_arguments)]
+    pub fn search_batch_filtered_minmax(&self, queries: &[T], masks: &[u64], k: usize, l_search: u32, beam_width: u32, match_all: bool,
+                                        adaptive_l: Option<(u32, f64)>, rerank: bool) -> Result<Batch> {
+        self.filtered_quantized(sys::dab_search_batch_filtered_minmax, queries, masks, k, l_search, beam_width, match_all, adaptive_l,
+                                rerank)
+    }
+
+    #[allow(clippy::too_many_arguments)]
+    fn filtered_quantized(&self, f: FilteredQuantized, queries: &[T], masks: &[u64], k: usize, l_search: u32, beam_width: u32,
+                          match_all: bool, adaptive_l: Option<(u32, f64)>, rerank: bool) -> Result<Batch> {
+        assert_eq!(queries.len() % self.dim, 0);
+        let nq = queries.len() / self.dim;
+        assert_eq!(masks.len(), nq);
+        let (samples, scale) = adaptive_l.unwrap_or((0, 1.0));
+        assert!(adaptive_l.is_none() || samples > 0, "AdaptiveL: sample count cannot be zero");
+        let mut b = Batch { k, ids: vec![0; nq * k], dists: vec![0.0; nq * k], counts: vec![0; nq], cmps: vec![0; nq], hops: vec![0; nq] };
+        check(unsafe {
+            f(self.raw, queries.as_ptr() as *const c_void, nq as u32, k as u32, l_search, beam_width, masks.as_ptr(), match_all as u32, samples,
+              scale, rerank as i32, b.ids.as_mut_ptr(), b.dists.as_mut_ptr(), b.counts.as_mut_ptr(), b.cmps.as_mut_ptr(), b.hops.as_mut_ptr())
+        })?;
+        Ok(b)
+    }
+
     /// `Range::search` (range_search.rs:255-469) for the batch: every point within `radius` of each query, query q's
     /// results at `offsets[q] .. offsets[q + 1]` in the reference's output order.
     pub fn range_search(&self, queries: &[T], l_search: u32, radius: f32, args: RangeArgs) -> Result<RangeBatch> {
@@ -496,6 +535,8 @@ type QuantizedAsync = unsafe extern "C" fn(*mut sys::dab_index, u32, *const c_vo
 /// The entry points that open a paged search over a quantized store (one signature for PQ, SQ and MinMax).
 type DiverseQuantized = unsafe extern "C" fn(*mut sys::dab_index, *const c_void, u32, u32, u32, u32, u32, std::os::raw::c_int,
                                              *mut u32, *mut f32, *mut u32, *mut u32, *mut u32) -> std::os::raw::c_int;
+type FilteredQuantized = unsafe extern "C" fn(*mut sys::dab_index, *const c_void, u32, u32, u32, u32, *const u64, u32, u32, f64,
+                                              std::os::raw::c_int, *mut u32, *mut f32, *mut u32, *mut u32, *mut u32) -> std::os::raw::c_int;
 type RangeQuantized = unsafe extern "C" fn(*mut sys::dab_index, *const c_void, u32, u32, u32, f32, std::os::raw::c_int, f32, f32, f32, u64,
                                            std::os::raw::c_int, *mut *mut sys::dab_range) -> std::os::raw::c_int;
 

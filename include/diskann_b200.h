@@ -298,6 +298,65 @@ int dab_search_batch_filtered_device(dab_index* idx, const void* d_queries, uint
                                      uint32_t* d_out_counts, uint32_t* d_out_cmps,
                                      uint32_t* d_out_hops);
 
+/* InlineFilterSearch::search over a quantized store (inline_filter_search.rs:89-160 with the
+ * quantized strategy behind graph::ext::labeled::Filtered, labeled.rs:96-129): the traversal, the
+ * matches and adaptive L are those of dab_search_batch_filtered, and the traversal distances are
+ * those of dab_search_batch_pq / _sq / _minmax on the same store (PQ: TableL2 / TableIP,
+ * DirectCosine for Metric::Cosine; SQ and MinMax: the queries compressed by the store's
+ * quantizer).
+ *   rerank == 0: the first L matches by store distance, start points and deleted ids dropped, the
+ *     first k kept, with their store distances;
+ *   rerank != 0: Pipeline<FilterStartPoints, Rerank> over the first L matches (providers
+ *     inmem/product.rs:391-400, full_precision.rs:356-399): each match that is neither a start
+ *     point nor deleted gets its full-precision distance, the matches are sorted by it (ties keep
+ *     matched-list order) and the first k are kept with their full-precision distances.
+ * A query can return fewer than k.  cmps / hops as in dab_search_batch_filtered.  Checked before
+ * any device work: the arguments of dab_search_batch_filtered (the shared memory with the query
+ * area the f32 query for PQ, the store's code row + 16 bytes for SQ and MinMax), then the store
+ * checks of the synchronous quantized call (store uploaded with rows, no Metric::Cosine on the SQ
+ * store, rerank only with the full-precision vectors uploaded); a MinMax query that holds a NaN
+ * after the transform fails the call.  Outputs as dab_search_batch; the _device forms take
+ * d_query_masks on the device and return with the outputs complete. */
+int dab_search_batch_filtered_pq(dab_index* idx, const void* queries, uint32_t nq, uint32_t k,
+                                 uint32_t l_search, uint32_t beam_width,
+                                 const uint64_t* query_masks, uint32_t match_all,
+                                 uint32_t adaptive_samples, double adaptive_scale, int rerank,
+                                 uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
+                                 uint32_t* out_cmps, uint32_t* out_hops);
+int dab_search_batch_filtered_sq(dab_index* idx, const void* queries, uint32_t nq, uint32_t k,
+                                 uint32_t l_search, uint32_t beam_width,
+                                 const uint64_t* query_masks, uint32_t match_all,
+                                 uint32_t adaptive_samples, double adaptive_scale, int rerank,
+                                 uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
+                                 uint32_t* out_cmps, uint32_t* out_hops);
+int dab_search_batch_filtered_minmax(dab_index* idx, const void* queries, uint32_t nq, uint32_t k,
+                                     uint32_t l_search, uint32_t beam_width,
+                                     const uint64_t* query_masks, uint32_t match_all,
+                                     uint32_t adaptive_samples, double adaptive_scale, int rerank,
+                                     uint32_t* out_ids, float* out_dists, uint32_t* out_counts,
+                                     uint32_t* out_cmps, uint32_t* out_hops);
+int dab_search_batch_filtered_pq_device(dab_index* idx, const void* d_queries, uint32_t nq,
+                                        uint32_t k, uint32_t l_search, uint32_t beam_width,
+                                        const uint64_t* d_query_masks, uint32_t match_all,
+                                        uint32_t adaptive_samples, double adaptive_scale,
+                                        int rerank, uint32_t* d_out_ids, float* d_out_dists,
+                                        uint32_t* d_out_counts, uint32_t* d_out_cmps,
+                                        uint32_t* d_out_hops);
+int dab_search_batch_filtered_sq_device(dab_index* idx, const void* d_queries, uint32_t nq,
+                                        uint32_t k, uint32_t l_search, uint32_t beam_width,
+                                        const uint64_t* d_query_masks, uint32_t match_all,
+                                        uint32_t adaptive_samples, double adaptive_scale,
+                                        int rerank, uint32_t* d_out_ids, float* d_out_dists,
+                                        uint32_t* d_out_counts, uint32_t* d_out_cmps,
+                                        uint32_t* d_out_hops);
+int dab_search_batch_filtered_minmax_device(dab_index* idx, const void* d_queries, uint32_t nq,
+                                            uint32_t k, uint32_t l_search, uint32_t beam_width,
+                                            const uint64_t* d_query_masks, uint32_t match_all,
+                                            uint32_t adaptive_samples, double adaptive_scale,
+                                            int rerank, uint32_t* d_out_ids, float* d_out_dists,
+                                            uint32_t* d_out_counts, uint32_t* d_out_cmps,
+                                            uint32_t* d_out_hops);
+
 /* ------------------------------------------------------------------ (3'''') range search */
 
 /* Range::search (diskann/src/graph/search/range_search.rs:255-469) for a whole query batch over

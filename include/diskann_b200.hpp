@@ -395,8 +395,35 @@ class GpuFiltered {
         for (uint32_t i = 0; i < nq; ++i) r.stats[i] = SearchStats{cmps[i], hops[i], counts[i]};
         return r;
     }
+    // The same over the quantized stores (the store must be resident): the traversal distances of
+    // dab_search_batch_pq / _sq / _minmax; `rerank`: Pipeline<FilterStartPoints, Rerank> over the first L matches
+    KnnResults search_pq(const T* queries, const uint64_t* masks, uint32_t nq, uint32_t k, bool rerank, bool match_all = false) {
+        return search_quantized(dab_search_batch_filtered_pq, queries, masks, nq, k, rerank, match_all);
+    }
+    KnnResults search_sq(const T* queries, const uint64_t* masks, uint32_t nq, uint32_t k, bool rerank, bool match_all = false) {
+        return search_quantized(dab_search_batch_filtered_sq, queries, masks, nq, k, rerank, match_all);
+    }
+    KnnResults search_minmax(const T* queries, const uint64_t* masks, uint32_t nq, uint32_t k, bool rerank, bool match_all = false) {
+        return search_quantized(dab_search_batch_filtered_minmax, queries, masks, nq, k, rerank, match_all);
+    }
 
    private:
+    using Quantized = int (*)(dab_index*, const void*, uint32_t, uint32_t, uint32_t, uint32_t, const uint64_t*, uint32_t, uint32_t, double,
+                              int, uint32_t*, float*, uint32_t*, uint32_t*, uint32_t*);
+    KnnResults search_quantized(Quantized fn, const T* queries, const uint64_t* masks, uint32_t nq, uint32_t k, bool rerank, bool match_all) {
+        KnnResults r;
+        r.nq = nq;
+        r.k = k;
+        r.ids.resize((size_t)nq * k);
+        r.distances.resize((size_t)nq * k);
+        std::vector<uint32_t> counts(nq), cmps(nq), hops(nq);
+        check(fn(p_.raw(), queries, nq, k, l_, beam_, masks, match_all ? 1 : 0, samples_, scale_, rerank ? 1 : 0, r.ids.data(),
+                 r.distances.data(), counts.data(), cmps.data(), hops.data()));
+        r.stats.resize(nq);
+        for (uint32_t i = 0; i < nq; ++i) r.stats[i] = SearchStats{cmps[i], hops[i], counts[i]};
+        return r;
+    }
+
     Provider<T>& p_;
     uint32_t l_, beam_, samples_;
     double scale_;

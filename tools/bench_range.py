@@ -49,6 +49,24 @@ def in_range_sets(base_t, bn, queries, radius, want_ids):
     return np.concatenate(counts), ids
 
 
+def build_store(g, cfg, base, store):
+    """the compressed store `store` of g over its rows `base` (fp: none): PQ-32 trained on the device, SQ-8, or MinMax-8
+    behind DoubleHadamard"""
+    n = base.shape[0]
+    if store == "sq":
+        mean, std = base.mean(0).astype(np.float32), float(base.std())
+        shift = (mean - np.float32(2.5 * std)).astype(np.float32)
+        g.upload_sq(8, shift, float(np.float32(5.0 * std)), float(np.dot(shift, shift)), 0.0)
+        g.sq_encode_all()
+    elif store == "minmax":
+        g.upload_minmax(8, 1.0, dab.Transform.double_hadamard(cfg["dim"], "same", seed=7))
+        g.minmax_encode_all()
+    elif store == "pq":
+        pick = np.sort(np.random.default_rng(bench.SEED_PQ).choice(n, size=min(100_000, n), replace=False))
+        g.pq_train(base[pick].astype(np.float32), 32, 256, 5, bench.SEED_PQ)
+        g.pq_encode_all()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--n", type=int, default=0)
@@ -69,18 +87,7 @@ def main():
     base_t = torch.from_numpy(base).cuda().double()
     bn = (base_t * base_t).sum(1)
     d_q = torch.from_numpy(queries).cuda()
-    if args.store == "sq":
-        mean, std = base.mean(0).astype(np.float32), float(base.std())
-        shift = (mean - np.float32(2.5 * std)).astype(np.float32)
-        g.upload_sq(8, shift, float(np.float32(5.0 * std)), float(np.dot(shift, shift)), 0.0)
-        g.sq_encode_all()
-    elif args.store == "minmax":
-        g.upload_minmax(8, 1.0, dab.Transform.double_hadamard(cfg["dim"], "same", seed=7))
-        g.minmax_encode_all()
-    elif args.store == "pq":
-        pick = np.sort(np.random.default_rng(bench.SEED_PQ).choice(n, size=min(100_000, n), replace=False))
-        g.pq_train(base[pick].astype(np.float32), 32, 256, 5, bench.SEED_PQ)
-        g.pq_encode_all()
+    build_store(g, cfg, base, args.store)
     stores = ["fp"] if args.store == "fp" else ["fp", args.store]
 
     def timed(call):
