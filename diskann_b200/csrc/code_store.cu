@@ -97,8 +97,12 @@ int store_alloc(dab_index* idx, CodeStore& s, int nbits, uint32_t dim, bool dim_
     s.stride = (uint32_t)round_up(code_bytes, 16);
     DAB_CUDA(cudaMalloc(&s.d_codes, total * s.stride));
     DAB_CUDA(cudaMalloc(&s.d_meta, total * meta_words * 4));
-    DAB_CUDA(cudaMemset(s.d_codes, 0, total * s.stride));
-    DAB_CUDA(cudaMemset(s.d_meta, 0, total * meta_words * 4));
+    // on the index's stream, which does not wait for the legacy default stream: a cudaMemset there could still be
+    // clearing the arrays while an encode on idx->stream writes them.  The uploads of an index's parameters (PQ table,
+    // SQ shift, MinMax transform tables) likewise copy on idx->stream.
+    DAB_CUDA(cudaMemsetAsync(s.d_codes, 0, total * s.stride, idx->stream));
+    DAB_CUDA(cudaMemsetAsync(s.d_meta, 0, total * meta_words * 4, idx->stream));
+    DAB_CUDA(cudaStreamSynchronize(idx->stream));
     s.nbits = nbits;  // set up only once both arrays exist
     return DAB_OK;
 }

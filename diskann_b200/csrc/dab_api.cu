@@ -317,12 +317,15 @@ int dab_upload_pq(dab_index* idx, const float* pivots, uint32_t n_centers, const
     DAB_CUDA(cudaMalloc(&idx->d_pivots, (size_t)n_centers * idx->dim * 4));
     DAB_CUDA(cudaMalloc(&idx->d_offsets, (size_t)(n_chunks + 1) * 4));
     DAB_CUDA(cudaMalloc(&idx->d_codes, idx->n_total() * (size_t)n_chunks));
-    DAB_CUDA(cudaMemcpy(idx->d_pivots, pivots, (size_t)n_centers * idx->dim * 4, cudaMemcpyHostToDevice));
-    DAB_CUDA(cudaMemcpy(idx->d_offsets, off32.data(), (size_t)(n_chunks + 1) * 4, cudaMemcpyHostToDevice));
+    // on the index's stream, which does not wait for the legacy default stream (where a cudaMemcpy from pageable memory
+    // may return before its DMA has landed, and a cudaMemset may still be clearing what dab_pq_encode_all writes)
+    DAB_CUDA(cudaMemcpyAsync(idx->d_pivots, pivots, (size_t)n_centers * idx->dim * 4, cudaMemcpyHostToDevice, idx->stream));
+    DAB_CUDA(cudaMemcpyAsync(idx->d_offsets, off32.data(), (size_t)(n_chunks + 1) * 4, cudaMemcpyHostToDevice, idx->stream));
     if (codes)
-        DAB_CUDA(cudaMemcpy(idx->d_codes, codes, idx->n_total() * (size_t)n_chunks, cudaMemcpyHostToDevice));
+        DAB_CUDA(cudaMemcpyAsync(idx->d_codes, codes, idx->n_total() * (size_t)n_chunks, cudaMemcpyHostToDevice, idx->stream));
     else
-        DAB_CUDA(cudaMemset(idx->d_codes, 0, idx->n_total() * (size_t)n_chunks));
+        DAB_CUDA(cudaMemsetAsync(idx->d_codes, 0, idx->n_total() * (size_t)n_chunks, idx->stream));
+    DAB_CUDA(cudaStreamSynchronize(idx->stream));
     idx->pq_chunks = n_chunks;
     idx->pq_centers = n_centers;
     idx->pq_uniform_len = off32[1] - off32[0];

@@ -133,7 +133,8 @@ int dab_upload_minmax(dab_index* idx, int nbits, float grid_scale, const dab_tra
         if (!idx->mm_transform) return fail(DAB_ERR_OUT_OF_MEMORY, "%s: out of host memory", who);
         const std::vector<uint32_t> tables = transform_tables(t);
         DAB_CUDA(cudaMalloc(&idx->d_mm_tables, tables.size() * 4));
-        DAB_CUDA(cudaMemcpy(idx->d_mm_tables, tables.data(), tables.size() * 4, cudaMemcpyHostToDevice));
+        DAB_CUDA(cudaMemcpyAsync(idx->d_mm_tables, tables.data(), tables.size() * 4, cudaMemcpyHostToDevice, idx->stream));  // see store_alloc
+        DAB_CUDA(cudaStreamSynchronize(idx->stream));
     }
     if ((rc = store_alloc(idx, idx->mm, nbits, out_dim, true, 4))) return rc;  // the header: dim, then {b, n, a, norm_squared}
     return rows ? store_upload(idx, idx->mm, rows, who) : DAB_OK;

@@ -168,7 +168,8 @@ int dab_upload_sq(dab_index* idx, int nbits, const float* shift, float scale, fl
     cudaFree(idx->d_sq_shift);
     idx->d_sq_shift = nullptr;
     DAB_CUDA(cudaMalloc(&idx->d_sq_shift, (size_t)idx->dim * 4));
-    DAB_CUDA(cudaMemcpy(idx->d_sq_shift, shift, (size_t)idx->dim * 4, cudaMemcpyHostToDevice));
+    DAB_CUDA(cudaMemcpyAsync(idx->d_sq_shift, shift, (size_t)idx->dim * 4, cudaMemcpyHostToDevice, idx->stream));  // see store_alloc
+    DAB_CUDA(cudaStreamSynchronize(idx->stream));
     idx->sq_scale = scale;
     idx->sq_shift_square_norm = shift_square_norm;
     idx->sq_mean_norm = mean_norm;
