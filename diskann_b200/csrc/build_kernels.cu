@@ -293,7 +293,6 @@ struct BackedgeParams {
     int prune_kind;
     uint32_t* adj;
     uint32_t adj_stride;
-    uint32_t* dropped;      // in-edges that did not fit the per-destination list of a batch
     // in-place deletes (inplace_backedge_kernel): the ids every visited list loses, ascending
     const uint32_t* remove;
     uint32_t n_remove;
@@ -931,7 +930,7 @@ static int launch_backedges(const dab_index* idx, BackedgeParams& p, bool remove
 // backedge_kernel takes a target's sources in the order the pairs arrive, and add_edge_and_prune takes them sorted
 // (index.rs:986-992): the ids in `batch` must be ascending.  Steps 1 and 2 do not depend on the members' order.
 struct LinkStep {
-    DevBuf batch, rec_ids, rec_d, rec_n, nbr, nbr_n, keys, vals, keys2, vals2, tmp, res_ids, res_d, dropped;
+    DevBuf batch, rec_ids, rec_d, rec_n, nbr, nbr_n, keys, vals, keys2, vals2, tmp, res_ids, res_d;
     size_t tmp_bytes = 0;
     uint32_t rec_cap = 0, pruned_degree = 0, l_build = 0;
     float alpha = 0.0f;
@@ -949,8 +948,6 @@ struct LinkStep {
             (rc = keys2.alloc(B * pruned_degree * 4)) || (rc = vals2.alloc(B * pruned_degree * 4)) || (rc = res_ids.alloc(B * 4)) ||
             (rc = res_d.alloc(B * 4)))
             return rc;
-        if ((rc = dropped.alloc(4))) return rc;
-        DAB_CUDA(cudaMemsetAsync(dropped.p, 0, 4, idx->stream));
         cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, (const uint32_t*)keys.p, (uint32_t*)keys2.p, (const uint32_t*)vals.p,
                                         (uint32_t*)vals2.p, (int)(B * pruned_degree), 0, 32, idx->stream);
         return tmp.alloc(tmp_bytes);
@@ -997,18 +994,12 @@ struct LinkStep {
         bp.n_pairs = n_pairs;
         bp.degree = pruned_degree;
         bp.alpha = alpha;
-        bp.dropped = (uint32_t*)dropped.p;
         return launch_backedges(idx, bp);
     }
 
-    // after the last step: dropped back-edges and truncated records, reported under `who`
+    // after the last step: truncated records, reported under `who`
     int report(dab_index* idx, const char* who) {
-        uint32_t n_dropped = 0;
-        DAB_CUDA(cudaMemcpyAsync(&n_dropped, dropped.p, 4, cudaMemcpyDeviceToHost, idx->stream));
         DAB_CUDA(cudaStreamSynchronize(idx->stream));
-        if (n_dropped)
-            return fail(DAB_ERR_INVALID_ARGUMENT, "%s: %u back-edges exceeded the per-destination list of a batch and were dropped "
-                        "(the graph is usable but not the reference's; use a smaller batch_size)", who, n_dropped);
         if (idx->rec_truncated)
             return fail(DAB_ERR_INVALID_ARGUMENT, "%s: %llu insert searches expanded more than %u nodes; their prune pools were cut "
                         "(the graph is usable but not the reference's)", who, (unsigned long long)idx->rec_truncated, rec_cap);
@@ -1201,7 +1192,9 @@ int dab_robust_prune(dab_index* idx, const uint32_t* pool_ids, const float* pool
     if (n_pools == 0) return DAB_OK;
     if (!pool_ids || !pool_dists || !pool_lens || !locations || !out_ids || !out_counts)
         return fail(DAB_ERR_INVALID_ARGUMENT, "dab_robust_prune: NULL argument");
-    if (degree == 0 || pool_cap == 0 || pool_cap > 4096) return fail(DAB_ERR_INVALID_ARGUMENT, "dab_robust_prune: bad degree / pool_cap");
+    // launch_prune holds a whole pool in shared memory: 20 bytes a slot, four warps a CTA, at most 200 KB
+    if (degree == 0 || pool_cap == 0 || pool_cap > 2048)
+        return fail(DAB_ERR_INVALID_ARGUMENT, "dab_robust_prune: degree must be > 0 and pool_cap in [1, 2048]");
     DAB_CUDA(cudaSetDevice(idx->device));
     DevBuf b_ids, b_d, b_len, b_loc, b_out, b_cnt;
     int rc;

@@ -761,7 +761,9 @@ int dab_search_batch_minmax_device(dab_index* idx, const void* d_queries, uint32
  * pool_ids/pool_dists[p * pool_cap ...] (any order; sorted by distance then arrival order and
  * truncated to max_occlusion_size = 750 like SortedNeighbors::new), locations[p] is the node
  * being pruned (excluded from its own pool).  Candidate x candidate distances are
- * Distance<T,T> over the uploaded rows.  out_ids [n_pools][degree] (padded UINT32_MAX). */
+ * Distance<T,T> over the uploaded rows.  out_ids [n_pools][degree] (padded UINT32_MAX).
+ * pool_cap must be in [1, 2048] (a whole pool is held in shared memory) and degree > 0;
+ * otherwise DAB_ERR_INVALID_ARGUMENT and nothing is written. */
 int dab_robust_prune(dab_index* idx, const uint32_t* pool_ids, const float* pool_dists,
                      const uint32_t* pool_lens, const uint32_t* locations, uint32_t n_pools,
                      uint32_t pool_cap, uint32_t degree, float alpha, uint32_t* out_ids,
@@ -775,7 +777,10 @@ int dab_robust_prune(dab_index* idx, const uint32_t* pool_ids, const float* pool
  * bootstrap routine (index.rs:589-747, run by the reference while a batch's back-edges reach <= 8 x batch distinct
  * targets) is NOT run: batch_size = 1 is DiskANNIndex::insert point by point, larger batches grow as inserted / 8 up
  * to batch_size (0: a default from the index size) so that no point is inserted blind.  Uses the uploaded vectors
- * (including start rows) and overwrites the adjacency. */
+ * (including start rows) and overwrites the adjacency.  A target's back-edges are not limited in number.  An insert
+ * search keeps a record of min(2048, 4 * l_build + 64) expanded nodes; when a search expands more, its prune pool is
+ * cut, the build still completes with a valid graph, and the call returns DAB_ERR_INVALID_ARGUMENT saying "their prune
+ * pools were cut" (the graph is then usable but not the reference's). */
 int dab_build(dab_index* idx, uint32_t pruned_degree, uint32_t l_build, float alpha,
               uint32_t batch_size);
 
@@ -800,9 +805,8 @@ int dab_build(dab_index* idx, uint32_t pruned_degree, uint32_t l_build, float al
  * whose vector and out-list are then replaced.  DAB_ERR_INVALID_ARGUMENT, changing nothing and naming the first
  * offending id: an id >= n_points (start points are frozen), a repeated id, a deleted id (dab_release it first); also
  * NULL pointers with n > 0, pruned_degree outside [1, max_degree], l_build == 0, alpha < 1, or any slot holding a batch
- * in flight.  DAB_ERR_NOT_READY when no vectors were uploaded.  n == 0 returns DAB_OK after these checks.  Back-edges
- * dropped and visited records cut are reported as dab_build reports them (the graph is then usable but not the
- * reference's).  Open paged sessions fail their next page; the tensor-core scan rebuilds its operand on its next use;
+ * in flight.  DAB_ERR_NOT_READY when no vectors were uploaded.  n == 0 returns DAB_OK after these checks.  Visited
+ * records cut are reported as dab_build reports them (the graph is then usable but not the reference's).  Open paged sessions fail their next page; the tensor-core scan rebuilds its operand on its next use;
  * dab_flat_knn* still scan every row. */
 int dab_insert(dab_index* idx, const uint32_t* ids, const void* rows, uint64_t n, uint32_t pruned_degree, uint32_t l_build,
                float alpha, uint32_t batch_size);
