@@ -71,6 +71,8 @@ SYMBOLS = {
     "dab_range_search_sq_device": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, _i, C.POINTER(_vp)]),
     "dab_range_search_minmax": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, _i, C.POINTER(_vp)]),
     "dab_range_search_minmax_device": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, _i, C.POINTER(_vp)]),
+    "dab_range_search_filtered": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, _vp, _u32, C.POINTER(_vp)]),
+    "dab_range_search_filtered_device": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, _vp, _u32, C.POINTER(_vp)]),
     "dab_range_offsets": (_i, [_vp, _vp, _vp, _vp, _vp]),
     "dab_range_results": (_i, [_vp, _vp, _vp]),
     "dab_range_results_device": (_i, [_vp, _vp, _vp]),

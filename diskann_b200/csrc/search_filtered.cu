@@ -21,6 +21,7 @@
 #include "search_common.cuh"
 #include "search_filtered.cuh"
 #include "search_host.cuh"
+#include "search_range.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -95,10 +96,17 @@ __device__ __forceinline__ void matched_merge(float* md, uint32_t* mi, uint32_t 
     __syncwarp();
 }
 
+// The matched list of InlineFilterSearch: the first L matches, written as the query's results
+struct MatchedTopL {
+    static constexpr bool kRange = false;
+};
+
 // One warp's share of a pass.  Src is the distance source of diverse search: load(q), prepare(), distances(cid, cd, n).
-// LIST: with p.list_ids, the matched list of each query (start points included) is written for the rerank.
-template <bool LIST, class Src>
-__device__ __forceinline__ void filtered_queries(const SearchParamsFiltered& p, uint8_t* base, int lane, Src& src) {
+// LIST: with p.list_ids, the matched list of each query (start points included) is written for the rerank.  Sink: where
+// the matches go, MatchedTopL or a sink with kRange (FilteredRangeSink), which sees every hop's candidates through
+// matches() and finishes each query that did not overflow.
+template <bool LIST, class Src, class Sink = MatchedTopL>
+__device__ __forceinline__ void filtered_queries(const SearchParamsFiltered& p, uint8_t* base, int lane, Src& src, Sink* sink = nullptr) {
     const int wib = threadIdx.x >> 5;
     float* bd = reinterpret_cast<float*>(base + p.off_bd);
     uint32_t* bi = reinterpret_cast<uint32_t*>(base + p.off_bi);
@@ -123,13 +131,15 @@ __device__ __forceinline__ void filtered_queries(const SearchParamsFiltered& p, 
         uint32_t cap = p.best_cap, size = 0, cursor = 0, msize = 0;
         uint32_t cmps = 0, hops = 0, nvisited = 0, sample_visited = 0, sample_matched = 0;
         bool adjusted = p.samples == 0, overflow = false;
+        if constexpr (Sink::kRange) sink->begin();
 
         // the candidates cid[0..n) (with their decisions in ca) into the list and the matched list, in order
         auto insert_all = [&](uint32_t n) {
             for (uint32_t c0 = 0; c0 < n; c0 += 32) {
                 const uint32_t m = min(32u, n - c0);
                 merge_round_chunked<8>(bd, bi, cap, size, cursor, cid, cd, c0, m, lane);
-                matched_merge(md, mi, p.cap, msize, cid, cd, ca, c0, m, lane);
+                if constexpr (Sink::kRange) sink->matches(cid, cd, ca, c0, m);
+                else matched_merge(md, mi, p.cap, msize, cid, cd, ca, c0, m, lane);
             }
         };
 
@@ -199,54 +209,61 @@ __device__ __forceinline__ void filtered_queries(const SearchParamsFiltered& p, 
             report_overflow(p.counters, p.overflow_list, qidx, lane);
             continue;
         }
-        if constexpr (LIST) {
-            if (p.list_ids) write_list(mi, msize, p.list_ids, p.list_counts, p.list_cap, qidx, lane);
+        if constexpr (Sink::kRange) {
+            sink->finish(qidx, bi, bd, size, mask, table, cmps, hops, nvisited);
+        } else {
+            if constexpr (LIST) {
+                if (p.list_ids) write_list(mi, msize, p.list_ids, p.list_counts, p.list_cap, qidx, lane);
+            }
+            // post-processing of matched_results.take(L): start points dropped, the first k kept
+            const uint32_t count = write_results(mi, md, msize, p.n_points, p.k, p.out_ids, p.out_dists, qidx, lane);
+            write_stats(p.counters, nvisited, p.out_counts, p.out_cmps, p.out_hops, qidx, count, cmps, hops, lane);
         }
-        // post-processing of matched_results.take(L): start points dropped, the first k kept
-        const uint32_t count = write_results(mi, md, msize, p.n_points, p.k, p.out_ids, p.out_dists, qidx, lane);
-        write_stats(p.counters, nvisited, p.out_counts, p.out_cmps, p.out_hops, qidx, count, cmps, hops, lane);
     }
 }
 
 // Full precision: rows from global memory with the shared distance schemas (distance_device.cuh), a team of lanes per row
 template <typename TD, int KIND, int POST, int NA>
+struct FullRows {
+    static constexpr bool INT = std::is_same<TD, int8_t>::value || std::is_same<TD, uint8_t>::value;
+    const SearchParamsFiltered& p;
+    float* qf;
+    int lane, dim, qq;  // qq, integer rows: Sum x^2 of the query (unused by inner product)
+    __device__ __forceinline__ void load(uint32_t q) { load_query(reinterpret_cast<const TD*>(p.queries) + (size_t)q * dim, dim, 4, qf, lane); }
+    __device__ __forceinline__ void prepare() {
+        if constexpr (INT) {
+            if (KIND != KIND_IP) qq = warp_int_self<std::is_same<TD, int8_t>::value>(reinterpret_cast<const uint8_t*>(qf), dim, lane);
+        }
+    }
+    __device__ __forceinline__ void distances(const uint32_t* cid, float* cd, uint32_t n) {
+        constexpr int S = INT ? 32 : 8 * NA, TEAMS = 32 / S, U = kFiltRows;
+        using Row = typename std::conditional<INT, uint8_t, TD>::type;
+        const int team = lane / S, slot = lane % S;
+        for (uint32_t c0 = 0; c0 < n; c0 += TEAMS * U) {
+            float r[U];
+            uint32_t cc[U];
+            const Row* rows[U];
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+                cc[u] = c0 + u * TEAMS + team;
+                rows[u] = reinterpret_cast<const Row*>(p.vectors + (size_t)cid[min(cc[u], n - 1)] * p.row_stride);
+            }
+            if constexpr (INT) warp_int_multi<std::is_same<TD, int8_t>::value, KIND, U>(reinterpret_cast<const uint8_t*>(qf), rows, dim, lane, qq, r);
+            else team_float_multi<NA, KIND, U>(qf, rows, dim, slot, r);
+#pragma unroll
+            for (int u = 0; u < U; ++u)
+                if (slot == 0 && cc[u] < n) cd[cc[u]] = post_op<POST>(r[u]);
+        }
+        __syncwarp();
+    }
+};
+
+template <typename TD, int KIND, int POST, int NA>
 __global__ void __launch_bounds__(kFiltWarps * 32) filtered_kernel(const SearchParamsFiltered p) {
-    constexpr bool INT = std::is_same<TD, int8_t>::value || std::is_same<TD, uint8_t>::value;
     extern __shared__ __align__(128) uint8_t smem[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     uint8_t* base = smem + (size_t)wib * p.warp_smem;
-    struct {
-        const SearchParamsFiltered& p;
-        float* qf;
-        int lane, dim, qq;  // qq, integer rows: Sum x^2 of the query (unused by inner product)
-        __device__ __forceinline__ void load(uint32_t q) { load_query(reinterpret_cast<const TD*>(p.queries) + (size_t)q * dim, dim, 4, qf, lane); }
-        __device__ __forceinline__ void prepare() {
-            if constexpr (INT) {
-                if (KIND != KIND_IP) qq = warp_int_self<std::is_same<TD, int8_t>::value>(reinterpret_cast<const uint8_t*>(qf), dim, lane);
-            }
-        }
-        __device__ __forceinline__ void distances(const uint32_t* cid, float* cd, uint32_t n) {
-            constexpr int S = INT ? 32 : 8 * NA, TEAMS = 32 / S, U = kFiltRows;
-            using Row = typename std::conditional<INT, uint8_t, TD>::type;
-            const int team = lane / S, slot = lane % S;
-            for (uint32_t c0 = 0; c0 < n; c0 += TEAMS * U) {
-                float r[U];
-                uint32_t cc[U];
-                const Row* rows[U];
-#pragma unroll
-                for (int u = 0; u < U; ++u) {
-                    cc[u] = c0 + u * TEAMS + team;
-                    rows[u] = reinterpret_cast<const Row*>(p.vectors + (size_t)cid[min(cc[u], n - 1)] * p.row_stride);
-                }
-                if constexpr (INT) warp_int_multi<std::is_same<TD, int8_t>::value, KIND, U>(reinterpret_cast<const uint8_t*>(qf), rows, dim, lane, qq, r);
-                else team_float_multi<NA, KIND, U>(qf, rows, dim, slot, r);
-#pragma unroll
-                for (int u = 0; u < U; ++u)
-                    if (slot == 0 && cc[u] < n) cd[cc[u]] = post_op<POST>(r[u]);
-            }
-            __syncwarp();
-        }
-    } src{p, reinterpret_cast<float*>(base), lane, (int)p.dim, 0};
+    FullRows<TD, KIND, POST, NA> src{p, reinterpret_cast<float*>(base), lane, (int)p.dim, 0};
     filtered_queries<false>(p, base, lane, src);
 }
 
@@ -292,6 +309,200 @@ __global__ void __launch_bounds__(kFiltWarps * 32) filtered_kernel_quant(const S
     } src{p, reinterpret_cast<float*>(base), reinterpret_cast<uint32_t*>(base),
           p.luts + (size_t)(blockIdx.x * kFiltWarps + wib) * entries, lane, (int)p.dim, entries, 0.0f};
     filtered_queries<true>(p, base, lane, src);
+}
+
+// ---- the filtered range search (FilteredRange::search, filtered_range_search.rs:119-248) ---------------------------
+// 64-bit keys a[0, n), n a power of two, into ascending order: a bitonic network run by one warp in global memory
+__device__ __forceinline__ void warp_sort_keys(unsigned long long* a, uint32_t n, int lane) {
+    for (uint32_t k = 2; k <= n; k <<= 1) {
+        for (uint32_t j = k >> 1; j > 0; j >>= 1) {
+            for (uint32_t i = lane; i < n; i += 32) {
+                const uint32_t l = i ^ j;
+                if (l > i) {
+                    const unsigned long long x = a[i], y = a[l];
+                    if ((x > y) == ((i & k) == 0)) a[i] = y, a[l] = x;
+                }
+            }
+            __syncwarp();
+        }
+    }
+}
+
+__device__ __forceinline__ uint32_t pow2_at_least(uint32_t n) { return n <= 1 ? 1u : 1u << (32 - __clz(n - 1)); }
+
+// The sink of filtered_queries for a filtered range search.  Phase 1 (the traversal at L + #start, no adaptive L) hands
+// it every hop's candidates: the accepted ones within the radius are appended to the warp's region of matches, in
+// evaluation order, start points first.  finish() then runs the rest of the query on the warp's frontier and key regions:
+//   matched   the matches sorted by distance, stably (order_key: -0.0 equal to +0.0; the reference's sort_unstable_by
+//             leaves exact ties open, the earlier match goes first as in InlineFilterSearch);
+//   in_range  the list's first L entries within the radius and the matches, sorted by (distance, id), each id once;
+//   round 2   iff |in_range| >= min_in_range and |matched| < max_returned: the visited table is cleared and seeded with
+//             the in_range ids, which are also the FIFO frontier.  While it is not empty and |matched| < max_returned,
+//             up to beam ids are popped and expanded one node at a time (expand_beam_filtered, the label read next to
+//             the visited probe); every neighbour with d <= radius * range_slack is pushed onto the frontier, and the
+//             accepted ones with d <= radius are appended to matched while it is below max_returned.  The cap does not
+//             cut a hop short.  cmps and hops count both phases.
+//   output    matched.take(max_returned) in order without start points, deleted ids and ids with d <= inner_radius.
+// A full region of matches or frontier stops the query, which the job re-runs on regions four times larger.
+template <class Src>
+struct FilteredRangeSink {
+    static constexpr bool kRange = true;
+    const FilteredRangeParams& fp;
+    Src& src;
+    int lane;
+    uint32_t *cid, *ca;  // the hop's candidates and their decisions (shared memory)
+    float* cd;
+    uint32_t* mid;  // the matches: region_cap ids, then dists
+    float* md;
+    uint32_t* fid;  // the frontier: front_cap ids, then dists (the sort's scratch)
+    float* fd;
+    unsigned long long* keys;
+    uint64_t m;  // matches within the radius, counted past region_cap
+
+    __device__ __forceinline__ FilteredRangeSink(const FilteredRangeParams& p, Src& s, uint8_t* base, int ln, size_t slot) : fp(p), src(s), lane(ln) {
+        cid = reinterpret_cast<uint32_t*>(base + p.f.off_cid);
+        cd = reinterpret_cast<float*>(base + p.f.off_cd);
+        ca = reinterpret_cast<uint32_t*>(base + p.f.off_ca);
+        mid = p.r.regions + slot * p.r.region_cap * 2;
+        md = reinterpret_cast<float*>(mid + p.r.region_cap);
+        fid = p.fronts + slot * p.front_cap * 2;
+        fd = reinterpret_cast<float*>(fid + p.front_cap);
+        keys = p.keys + slot * p.key_cap;
+    }
+
+    __device__ __forceinline__ void begin() { m = 0; }
+
+    // the accepted candidates within the radius among c0 .. c0+n-1 (n <= 32, lane j owns candidate j), in order
+    __device__ __forceinline__ void matches(const uint32_t* ids, const float* ds, const uint32_t* acc, uint32_t c0, uint32_t n) {
+        const uint32_t j = (uint32_t)lane;
+        const float d = j < n ? ds[c0 + j] : 0.0f;
+        const bool ok = j < n && acc[c0 + j] && d <= fp.r.radius;
+        const unsigned b = __ballot_sync(kFull, ok);
+        const uint64_t at = m + __popc(b & ((1u << lane) - 1u));
+        if (ok && at < fp.r.region_cap) mid[at] = ids[c0 + j], md[at] = d;
+        m += __popc(b);
+    }
+
+    __device__ __forceinline__ void finish(uint32_t qidx, const uint32_t* bi, const float* bd, uint32_t size, uint64_t mask, uint32_t* table,
+                                           uint32_t cmps, uint32_t hops, uint32_t nvisited) {
+        const RangeParams& p = fp.r;
+        const unsigned below = (1u << lane) - 1u;
+        const uint32_t nbk = p.n_buckets, hlimit = nbk * 7;
+        const uint64_t n_total = p.n_points + p.n_start;
+        bool region_full = m > p.region_cap, overflow = region_full, second = false;
+        uint32_t M = (uint32_t)m;
+        if (!overflow) {
+            __syncwarp();
+            // ---- matched_results sorted by (distance, evaluation order)
+            uint32_t n = pow2_at_least(M);
+            for (uint32_t i = lane; i < n; i += 32) keys[i] = i < M ? (unsigned long long)order_key(md[i]) << 32 | i : ~0ull;
+            __syncwarp();
+            warp_sort_keys(keys, n, lane);
+            for (uint32_t i = lane; i < M; i += 32) {
+                const uint32_t s = (uint32_t)keys[i];
+                fid[i] = mid[s], fd[i] = md[s];
+            }
+            __syncwarp();
+            for (uint32_t i = lane; i < M; i += 32) mid[i] = fid[i], md[i] = fd[i];
+            // ---- in_range: the list's first L entries within the radius and the matches, by (distance, id), deduplicated
+            const uint32_t n1 = min(size, p.l_search);
+            uint32_t t = 0;
+            for (uint32_t b = 0; b < n1; b += 32) {
+                const uint32_t i = b + lane;
+                const float d = i < n1 ? bd[i] : 0.0f;
+                const bool in = i < n1 && d <= p.radius;
+                const unsigned bb = __ballot_sync(kFull, in);
+                if (in) keys[t + __popc(bb & below)] = (unsigned long long)order_key(d) << 32 | (bi[i] & ~kFlagV2);  // expanded: flagged
+                t += __popc(bb);
+            }
+            __syncwarp();
+            for (uint32_t i = lane; i < M; i += 32) keys[t + i] = (unsigned long long)order_key(md[i]) << 32 | mid[i];
+            const uint32_t T = t + M;
+            n = pow2_at_least(T);
+            for (uint32_t i = T + lane; i < n; i += 32) keys[i] = ~0ull;
+            __syncwarp();
+            warp_sort_keys(keys, n, lane);
+            // an id in both sources has the same distance bits there, so its two keys are equal and adjacent
+            uint32_t F = 0;
+            for (uint32_t b = 0; b < T; b += 32) {
+                const uint32_t i = b + lane;
+                const bool first = i < T && (i == 0 || keys[i] != keys[i - 1]);
+                const unsigned bb = __ballot_sync(kFull, first);
+                if (first) fid[F + __popc(bb & below)] = (uint32_t)keys[i];
+                F += __popc(bb);
+            }
+            __syncwarp();
+            second = F >= p.min_in_range && M < p.max_returned;
+            if (second) {
+                // ---- filtered_range_search_internal
+                for (uint32_t i = lane; i < nbk; i += 32) store_empty_bucket(table + (size_t)i * 8);
+                __syncwarp();
+                for (uint32_t i = lane; i < F; i += 32) visit_global(table, nbk, fid[i]);
+                __syncwarp();  // every seed is in the table before any lane probes it for a neighbour
+                nvisited = F;
+                overflow = nvisited + p.max_degree > hlimit;
+                uint32_t head = 0;
+                while (!overflow && head < F && M < p.max_returned) {
+                    const uint32_t nb = min(p.beam, F - head), f0 = head;
+                    head += nb;
+                    hops += nb;
+                    for (uint32_t b = 0; b < nb && !overflow; ++b) {
+                        uint32_t ncand = 0;
+                        expand_node(p.adj, p.adj_stride, p.max_degree, n_total, table, nbk, fid[f0 + b], cid, ncand, nvisited, lane,
+                                    [&](bool isnew, uint32_t word, uint32_t at) {
+                                        const bool acc = isnew && label_accepts(__ldg(fp.f.labels + word), mask, fp.f.match_all);
+                                        const unsigned mn = __ballot_sync(kFull, isnew);
+                                        if (isnew) ca[at + __popc(mn & below)] = acc;
+                                    });
+                        if (nvisited + p.max_degree > hlimit) {
+                            overflow = true;
+                            break;
+                        }
+                        __syncwarp();
+                        src.distances(cid, cd, ncand);
+                        cmps += ncand;
+                        // every neighbour within the navigation radius onto the frontier; the accepted ones within the
+                        // radius into matched while it is below max_returned
+                        for (uint32_t c0 = 0; c0 < ncand; c0 += 32) {
+                            const uint32_t c = c0 + lane;
+                            const float d = c < ncand ? cd[c] : 0.0f;
+                            const bool nav = c < ncand && d <= p.bound;
+                            const bool acc = nav && d <= p.radius && ca[c];
+                            const unsigned bn = __ballot_sync(kFull, nav), ba = __ballot_sync(kFull, acc);
+                            const uint32_t take = (uint32_t)min((unsigned long long)__popc(ba), (unsigned long long)(p.max_returned - M));
+                            if (F + __popc(bn) > fp.front_cap || M + take > p.region_cap) {
+                                region_full = overflow = true;
+                                break;
+                            }
+                            if (nav) fid[F + __popc(bn & below)] = cid[c];
+                            const uint32_t rank = __popc(ba & below);
+                            if (acc && rank < take) mid[M + rank] = cid[c], md[M + rank] = d;
+                            F += __popc(bn);
+                            M += take;
+                        }
+                        __syncwarp();
+                    }
+                }
+            }
+        }
+        if (overflow) {
+            report_overflow(p.counters, p.overflow_list, qidx, lane);
+            if (region_full && lane == 0) atomicAdd(p.counters + 3, 1u);
+            return;
+        }
+        if (lane == 0) fp.out_cmps[qidx] = cmps;
+        range_emit(p, mid, md, min((uint64_t)M, p.max_returned), true, qidx, hops, second, nvisited, lane);
+    }
+};
+
+template <typename TD, int KIND, int POST, int NA>
+__global__ void __launch_bounds__(kFiltWarps * 32) filtered_range_kernel(const FilteredRangeParams p) {
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    uint8_t* base = smem + (size_t)wib * p.f.warp_smem;
+    FullRows<TD, KIND, POST, NA> src{p.f, reinterpret_cast<float*>(base), lane, (int)p.f.dim, 0};
+    FilteredRangeSink<decltype(src)> sink(p, src, base, lane, (size_t)blockIdx.x * kFiltWarps + wib);
+    filtered_queries<false>(p.f, base, lane, src, &sink);
 }
 
 template <typename S>
@@ -378,6 +589,16 @@ int filtered_plan(const dab_index* idx, uint32_t l_search, uint32_t best_max, ui
     return visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) -> int {
         plan.kern = filtered_kernel_of<decltype(sc)>();
         return filtered_grid(idx, l_search, beam, INT32_MAX, plan);
+    });
+}
+
+int filtered_range_plan(const dab_index* idx, uint32_t l_search, uint32_t beam, FilteredRangeParams& p, FilteredRangePlan& plan) {
+    p.f.warp_smem = (uint32_t)filtered_warp_smem(idx, l_search, l_search + idx->n_start, beam, -1, &p.f);
+    plan.smem_block = (size_t)p.f.warp_smem * kFiltWarps;
+    return visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) -> int {
+        using S = decltype(sc);
+        plan.kern = filtered_range_kernel<typename S::TD, S::KIND, S::POST, S::NA>;
+        return DAB_OK;
     });
 }
 

@@ -35,6 +35,7 @@
 #include "search_common.cuh"
 #include "search_host.cuh"
 #include "search_pq.cuh"
+#include "search_range.cuh"
 #include "search_smem.cuh"
 
 #include <cub/device/device_segmented_sort.cuh>
@@ -58,71 +59,15 @@ namespace dab {
 
 namespace {
 
-constexpr int kRangeWarps = 4;
 constexpr int kRangeRows = 4;                  // rows in flight per team in the distance loop
 constexpr size_t kRangeMaxSmem = 200 * 1024;   // a CTA's shared memory
 constexpr uint64_t kRegionBudget = 1ull << 31;  // bytes of in_range regions one pass may take
 
-struct RangeParams {
-    const uint32_t* adj;
-    uint32_t adj_stride;
-    uint64_t n_points;
-    uint32_t n_start;
-    uint32_t dim;
-    uint32_t max_degree;
-    const uint8_t* vectors;
-    size_t row_stride;
-    const void* queries;
-    const uint32_t* query_list;  // the queries of a re-run pass (NULL: 0 .. n_work-1)
-    uint32_t n_work;
-    uint32_t l_search, beam;
-    // phase 1: the first L list entries of every query [nq][L], their number and the hops [nq]
-    const uint32_t* list_ids;
-    const float* list_dists;
-    const uint32_t* list_counts;
-    const uint32_t* list_hops;
-    float radius, bound, inner_radius;  // bound: radius * range_slack
-    int has_inner;
-    uint64_t min_in_range;  // (f32(L) * initial_slack) as usize
-    uint64_t max_returned;  // UINT64_MAX: None
-    const uint32_t* deleted;  // NULL: nothing deleted
-    uint32_t* tables;
-    uint32_t n_buckets;
-    uint32_t* regions;  // region_cap ids then region_cap dists for every warp of the pass
-    uint32_t region_cap;
-    // counters[0] work cursor, [1] stopped queries (listed in overflow_list), [2] largest visited set, [3] the stopped
-    // queries whose region was full, [4] queries without room in the arena (listed in arena_fail)
-    uint32_t* counters;
-    uint32_t* overflow_list;
-    uint32_t* arena_fail;
-    // the arena: positions [arena_first, arena_end) are arena_ids / arena_dists [0, arena_end - arena_first);
-    // arena_ctr: the next position, the entries written, the entries of the queries that found no room
-    uint32_t* arena_ids;
-    float* arena_dists;
-    uint64_t arena_first, arena_end;
-    unsigned long long* arena_ctr;
-    uint64_t* q_pos;
-    uint32_t *q_count, *out_hops;
-    uint8_t* out_second;
-    uint32_t warp_smem, off_cid, off_cd;
-    // the quantized stores (range_kernel_quant), named as in SearchParamsPq for the per-candidate code
-    // (quant_device.cuh).  Fields of the full-precision kernel come first, so that its parameter offsets stay as they were.
-    int dtype;
-    const float* pivots;  // PQ: the table, [n_centers][dim]
-    const uint32_t* offsets;
-    const uint8_t* codes;  // [n_total][n_chunks]
-    uint32_t n_chunks, n_centers;
-    int ip_table, direct_cosine;
-    float* luts;  // PQ tables (TableL2 / TableIP): n_chunks x n_centers f32 for every resident warp
-    const uint8_t* row_codes;  // SQ / MinMax: the store's rows and the batch's staged queries
-    const float* row_meta;
-    uint32_t code_stride, code_dim;
-    int code_nbits, code_metric;
-    float sq_scale_squared, sq_shift_square_norm;
-    const uint8_t* query_codes;  // [nq][code_stride]
-    const float4* query_meta;    // [nq]
-    int rerank;  // the output keeps every in_range id but start points and deleted ids, for range_rerank
-};
+inline uint64_t round_up_pow2(uint64_t n) {
+    uint64_t p = 1;
+    while (p < n) p <<= 1;
+    return p;
+}
 
 // One warp's share of a pass: the queries of the work list it takes, whatever the distances are.  Src is the distance
 // source: load(q) brings query q into the front of the warp's shared memory, prepare() runs once the visited table is
@@ -181,17 +126,9 @@ __device__ __forceinline__ void range_queries(const RangeParams& p, uint8_t* bas
                 front += nb;
                 hops2 += nb;
                 for (uint32_t b = 0; b < nb && size < p.max_returned; ++b) {
-                    // expand_beam of one node: its unvisited, in-bounds neighbours in adjacency order
-                    const uint32_t node = rid[f0 + b];
-                    const uint32_t* row = p.adj + (size_t)node * p.adj_stride;
-                    const uint32_t deg = min(__ldg(row), p.max_degree);
                     uint32_t ncand = 0;
-                    for (uint32_t c0 = 0; c0 < deg + 1; c0 += 32) {
-                        const uint32_t j = c0 + lane;
-                        const uint32_t word = j < p.adj_stride ? __ldg(row + j) : kEmptyV2;
-                        const bool inserted = j >= 1 && j <= deg && visit_global(table, nbk, word);
-                        push_new(inserted, inserted && word < n_total, word, cid, ncand, nvisited, lane);
-                    }
+                    expand_node(p.adj, p.adj_stride, p.max_degree, n_total, table, nbk, rid[f0 + b], cid, ncand, nvisited, lane,
+                                [](bool, uint32_t, uint32_t) {});
                     if (nvisited + p.max_degree > hlimit) {
                         overflow = true;
                         break;
@@ -227,53 +164,7 @@ __device__ __forceinline__ void range_queries(const RangeParams& p, uint8_t* bas
         }
 
         // ---- the output: start points, deleted ids, the inner radius and the radius filtered out
-        auto keep = [&](uint64_t i) {
-            if (i >= size) return false;
-            const uint32_t id = rid[i];
-            const float d = rd[i];
-            if (id >= p.n_points) return false;
-            if (p.deleted && (__ldg(p.deleted + (id >> 5)) >> (id & 31) & 1u)) return false;
-            if (!radius_filter) return true;
-            if (p.has_inner && d <= p.inner_radius) return false;
-            return d <= p.radius;
-        };
-        uint32_t count = 0;
-        for (uint64_t b = 0; b < size; b += 32) count += __popc(__ballot_sync(kFull, keep(b + lane)));
-        unsigned long long pos = 0;
-        int fits = 1;
-        if (lane == 0 && count) {
-            pos = atomicAdd(p.arena_ctr, (unsigned long long)count);
-            fits = pos + count <= p.arena_end;
-            if (fits) {
-                atomicAdd(p.arena_ctr + 1, (unsigned long long)count);
-            } else {
-                p.arena_fail[atomicAdd(p.counters + 4, 1u)] = qidx;
-                atomicAdd(p.arena_ctr + 2, (unsigned long long)count);
-            }
-        }
-        pos = __shfl_sync(kFull, pos, 0);
-        fits = __shfl_sync(kFull, fits, 0);
-        if (fits && count) {
-            uint32_t w = 0;
-            for (uint64_t b = 0; b < size; b += 32) {
-                const uint64_t i = b + lane;
-                const bool k = keep(i);
-                const unsigned m = __ballot_sync(kFull, k);
-                if (k) {
-                    const uint64_t at = pos - p.arena_first + w + __popc(m & below);
-                    p.arena_ids[at] = rid[i];
-                    p.arena_dists[at] = rd[i];
-                }
-                w += __popc(m);
-            }
-        }
-        if (lane == 0) {
-            atomicMax(p.counters + 2, nvisited);
-            p.q_count[qidx] = count;
-            p.q_pos[qidx] = pos;
-            p.out_hops[qidx] = hops;
-            p.out_second[qidx] = second ? 1 : 0;
-        }
+        range_emit(p, rid, rd, size, radius_filter, qidx, hops, second, nvisited, lane);
     }
 }
 
@@ -521,9 +412,10 @@ size_t range_rerank_smem(const dab_index* idx) {
 
 // The range search's own checks, after Range::validate_and_create's (range_search.rs:91-131) in its order.  Over a
 // quantized store (`store` >= 0) the traversal reads the graph and the store only; the store checks of its k-NN call
-// follow, then those of the rerank.
+// follow, then those of the rerank.  A filtered range search (`filtered`) checks, after beam_width, the label table, the
+// filtered kernel's list (L + #start <= kFilteredMaxL) and its shared memory.
 int check_range_args(const dab_index* idx, const char* api, int store, bool rerank, uint32_t l_search, uint32_t beam, float radius,
-                     int has_inner, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned) {
+                     int has_inner, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, bool filtered = false) {
     if (store < 0 && (!idx->graph_ready || !idx->vectors_ready)) return fail(DAB_ERR_NOT_READY, "%s: vectors and graph must be uploaded first", api);
     if (store >= 0 && !idx->graph_ready) return fail(DAB_ERR_NOT_READY, "%s: graph must be uploaded first", api);
     if (beam == 0) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: beam_width must be > 0 (BeamWidthZero)", api);
@@ -537,6 +429,12 @@ int check_range_args(const dab_index* idx, const char* api, int store, bool rera
     if (has_inner && inner_radius > radius)
         return fail(DAB_ERR_INVALID_ARGUMENT, "%s: inner_radius %g must be <= radius %g (InnerRadiusValueError)", api, (double)inner_radius, (double)radius);
     if (beam > 64) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: beam_width %u > 64", api, beam);
+    if (filtered) {
+        if (!idx->d_labels) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: no label table (dab_upload_labels has not been called)", api);
+        if ((uint64_t)l_search + idx->n_start > kFilteredMaxL)
+            return fail(DAB_ERR_INVALID_ARGUMENT, "%s: L + #start = %llu > %u", api, (unsigned long long)l_search + idx->n_start, kFilteredMaxL);
+        return filtered_check_smem(idx, api, l_search, l_search + idx->n_start, beam);
+    }
     const size_t smem = range_warp_smem(idx, store, nullptr) * kRangeWarps;
     if (smem > kRangeMaxSmem)
         return fail(DAB_ERR_INVALID_ARGUMENT, "%s: dim=%u, max_degree=%u need %zu B shared memory per CTA (> %zu)", api, idx->dim, idx->max_degree,
@@ -656,10 +554,18 @@ int range_rerank(dab_index* idx, const char* api, const void* d_queries, uint32_
     return DAB_OK;
 }
 
+// A filtered range search's device masks (one per query) and mode
+struct RangeFilter {
+    const uint64_t* masks;
+    uint32_t match_all;
+};
+
 // Both phases for nq >= 1 queries (checks passed) into a new result set: over full-precision rows (`store` -1) or a
-// QuantStore, whose results `rerank` reorders by full-precision distance
+// QuantStore, whose results `rerank` reorders by full-precision distance.  With `filt` (full precision) both phases are
+// the filtered range search's, in filtered_range_kernel: its passes run the traversal too, and write cmps.
 int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t nq, uint32_t l_search, uint32_t beam, float radius, int has_inner,
-              float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, int store, bool rerank, dab_range* r) {
+              float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, int store, bool rerank, dab_range* r,
+              const RangeFilter* filt) {
     cudaStream_t st = idx->stream;
     int rc;
     // ---- the result set's statistics, then phase 1: the first L entries of every list with start points and
@@ -667,7 +573,7 @@ int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t n
     const size_t stat_bytes = ((size_t)nq + 1) * 8 + (size_t)nq * 9;
     DAB_CUDA(cudaMalloc(&r->d_stats, stat_bytes));
     DevBuf p1;
-    const size_t lq = (size_t)nq * l_search;
+    const size_t lq = filt ? 0 : (size_t)nq * l_search;
     if ((rc = p1.alloc(lq * 8 + (size_t)nq * 8, api))) return rc;
     uint32_t* list_ids = (uint32_t*)p1.p;
     float* list_dists = (float*)(list_ids + lq);
@@ -678,17 +584,23 @@ int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t n
     rec.keep_deleted = true;
     StagedQueries staged{};  // SQ / MinMax: the queries phase 1 compressed, which phase 2 reads too
     rec.staged = &staged;
-    if ((rc = run_search(idx, d_queries, nq, l_search, l_search, beam, SearchOut{list_ids, list_dists, list_counts, r->cmps(), list_hops}, store,
-                         false, &rec)))
+    if (!filt && (rc = run_search(idx, d_queries, nq, l_search, l_search, beam, SearchOut{list_ids, list_dists, list_counts, r->cmps(), list_hops},
+                                  store, false, &rec)))
         return rc;
 
     // ---- phase 2
     RangeParams p;
     memset(&p, 0, sizeof(p));
     p.warp_smem = (uint32_t)range_warp_smem(idx, store, &p);
-    const size_t smem_block = (size_t)p.warp_smem * kRangeWarps;
+    size_t smem_block = (size_t)p.warp_smem * kRangeWarps;
     void (*kern)(const RangeParams) = nullptr;
-    if (store >= 0) {
+    FilteredRangeParams fp;
+    FilteredRangePlan fplan;
+    if (filt) {
+        memset(&fp, 0, sizeof(fp));
+        if ((rc = filtered_range_plan(idx, l_search, beam, fp, fplan))) return rc;
+        smem_block = fplan.smem_block;
+    } else if (store >= 0) {
         kern = store == STORE_PQ ? range_kernel_quant<0> : store == STORE_SQ ? range_kernel_quant<1> : range_kernel_quant<2>;
     } else {
         visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) -> int {
@@ -696,7 +608,7 @@ int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t n
             return DAB_OK;
         });
     }
-    int per_sm = ctas_per_sm(kern, kRangeWarps * 32, smem_block);
+    int per_sm = filt ? ctas_per_sm(fplan.kern, kFiltWarps * 32, smem_block) : ctas_per_sm(kern, kRangeWarps * 32, smem_block);
     if (per_sm < 1) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: dim=%u needs %zu B shared memory per CTA", api, idx->dim, smem_block);
     // every resident warp owns a PQ table (n_chunks x n_centers f32: 32 KB at 32 x 256) that its lookups read through
     // L2: the cap of search_kernel_pq keeps them L2-resident
@@ -729,6 +641,20 @@ int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t n
     p.deleted = deleted_filter(idx);
     p.out_hops = r->hops();
     p.out_second = r->second();
+    if (filt) {
+        // phase 1: the filtered traversal at L + #start without adaptive L; its tables, counters and work list are p's
+        set_graph_params(idx, fp.f);
+        fp.f.vectors = idx->d_vectors;
+        fp.f.row_stride = idx->row_stride;
+        fp.f.queries = d_queries;
+        fp.f.cap = l_search;
+        fp.f.beam = beam;
+        fp.f.best_cap = l_search + idx->n_start;
+        fp.f.labels = idx->d_labels;
+        fp.f.masks = filt->masks;
+        fp.f.match_all = filt->match_all;
+        fp.out_cmps = r->cmps();
+    }
 
     DevBuf ctr, per_query, tables, regions, arena1, arena2;
     if ((rc = ctr.alloc(64 + (size_t)nq * 8, api)) || (rc = per_query.alloc((size_t)nq * 12, api))) return rc;
@@ -741,11 +667,12 @@ int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t n
     DAB_CUDA(cudaMemsetAsync(ctr.p, 0, 64, st));
     uint32_t* h = (uint32_t*)idx->h_counters.p;  // pinned: the five counters, then the three arena counters
 
-    // the in_range regions and the arena of the first pass
-    const uint64_t region_max = std::min<uint64_t>(p.max_returned, idx->n_total());
+    // the in_range regions (filtered: the matches, which max_returned does not bound in phase 1) and the arena of the
+    // first pass
+    const uint64_t region_max = filt ? idx->n_total() : std::min<uint64_t>(p.max_returned, idx->n_total());
     uint64_t region = idx->tune.test_range_list ? idx->tune.test_range_list : round_up(std::max<uint64_t>(4ull * l_search, 1024), 32);
     region = std::min(region, region_max);
-    uint64_t slots = table_slots(idx, VisitedHint{}, l_search, beam, STORE_PQ);
+    uint64_t slots = table_slots(idx, VisitedHint{}, filt ? l_search + idx->n_start : l_search, beam, STORE_PQ);
     const uint64_t limit = idx->tune.test_range_limit ? idx->tune.test_range_limit : UINT64_MAX;
     const uint64_t arena_first = std::min<uint64_t>(idx->tune.test_range_arena ? idx->tune.test_range_arena : (uint64_t)nq * l_search, limit);
     if ((rc = alloc_entries(idx, api, arena1, arena_first, arena_first))) return rc;
@@ -754,7 +681,7 @@ int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t n
     p.arena_first = 0;
     p.arena_end = arena_first;
 
-    DevBuf retry;
+    DevBuf retry, fronts, keys;
     if ((rc = retry.alloc((size_t)nq * 4, api))) return rc;
     p.n_work = nq;
     int pass = 0;
@@ -763,7 +690,10 @@ int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t n
     for (;;) {
         // the grid of this pass: one warp per query at most, and regions within kRegionBudget
         int grid = balanced_grid(p.n_work, resident, kRangeWarps);
-        const uint64_t region_grid = std::max<uint64_t>(1, kRegionBudget / (region * 8 * kRangeWarps));
+        // a filtered search's warp also holds a frontier of region + L entries and the sort keys of as many
+        const uint64_t front = region + l_search, key_cap = filt ? round_up_pow2(front) : 0;
+        const uint64_t warp_bytes = region * 8 + (filt ? front * 8 + key_cap * 8 : 0);
+        const uint64_t region_grid = std::max<uint64_t>(1, kRegionBudget / (warp_bytes * kRangeWarps));
         grid = (int)std::min<uint64_t>(grid, region_grid);
         const uint64_t warps = (uint64_t)grid * kRangeWarps;
         p.n_buckets = (uint32_t)((slots + 7) / 8);
@@ -772,8 +702,25 @@ int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t n
         p.tables = (uint32_t*)tables.p;
         p.regions = (uint32_t*)regions.p;
         DAB_CUDA(cudaMemsetAsync(p.counters, 0, 16, st));
-        DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_block));
-        kern<<<grid, kRangeWarps * 32, smem_block, st>>>(p);
+        if (filt) {
+            if ((rc = fronts.alloc(warps * front * 8, api)) || (rc = keys.alloc(warps * key_cap * 8, api))) return rc;
+            fp.r = p;
+            fp.f.query_list = p.query_list;
+            fp.f.n_work = p.n_work;
+            fp.f.tables = p.tables;
+            fp.f.n_buckets = p.n_buckets;
+            fp.f.counters = p.counters;
+            fp.f.overflow_list = p.overflow_list;
+            fp.fronts = (uint32_t*)fronts.p;
+            fp.keys = (unsigned long long*)keys.p;
+            fp.front_cap = (uint32_t)front;
+            fp.key_cap = (uint32_t)key_cap;
+            DAB_CUDA(cudaFuncSetAttribute(fplan.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_block));
+            fplan.kern<<<grid, kFiltWarps * 32, smem_block, st>>>(fp);
+        } else {
+            DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_block));
+            kern<<<grid, kRangeWarps * 32, smem_block, st>>>(p);
+        }
         DAB_LAUNCHED();
         DAB_CUDA(cudaGetLastError());
         DAB_CUDA(cudaMemcpyAsync(h, ctr.p, 64, cudaMemcpyDeviceToHost, st));
@@ -812,8 +759,8 @@ int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t n
         }
         break;
     }
-    cudaFree(tables.p), cudaFree(regions.p);
-    tables.p = regions.p = nullptr;
+    cudaFree(tables.p), cudaFree(regions.p), cudaFree(fronts.p), cudaFree(keys.p);
+    tables.p = regions.p = fronts.p = keys.p = nullptr;
 
     // ---- the result set: offsets, then the results in query order
     range_scan<<<1, 1024, 0, st>>>(p.q_count, nq, r->offsets());
@@ -853,7 +800,7 @@ int range_empty(dab_index* idx, dab_range* r) {
 // nq >= 1 queries, from the host (`host`, copied to the handle's scratch) or the device
 int range_batch(dab_index* idx, const char* api, bool host, const void* queries, uint32_t nq, uint32_t l_search, uint32_t beam, float radius,
                 int has_inner, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, int store, bool rerank,
-                dab_range* r) {
+                dab_range* r, const uint64_t* masks, uint32_t match_all) {
     const void* d_queries = queries;
     if (host) {
         const size_t qbytes = (size_t)nq * idx->dim * elem_size(idx->dtype);
@@ -862,20 +809,30 @@ int range_batch(dab_index* idx, const char* api, bool host, const void* queries,
         d_queries = idx->s_queries.p;
         DAB_CUDA(cudaMemcpyAsync(idx->s_queries.p, queries, qbytes, cudaMemcpyHostToDevice, idx->stream));
     }
+    if (!masks) return range_run(idx, api, d_queries, nq, l_search, beam, radius, has_inner, inner_radius, initial_slack, range_slack, max_returned,
+                                 store, rerank, r, nullptr);
+    RangeFilter filt{masks, match_all};
+    if (host) {
+        int rc;
+        if ((rc = idx->s_pools.reserve((size_t)nq * 8))) return rc;
+        DAB_CUDA(cudaMemcpyAsync(idx->s_pools.p, masks, (size_t)nq * 8, cudaMemcpyHostToDevice, idx->stream));
+        filt.masks = (const uint64_t*)idx->s_pools.p;
+    }
     return range_run(idx, api, d_queries, nq, l_search, beam, radius, has_inner, inner_radius, initial_slack, range_slack, max_returned, store,
-                     rerank, r);
+                     rerank, r, &filt);
 }
 
 // `store`: -1 full precision, else the QuantStore both phases read; `rerank` (a store) reorders the results by
-// full-precision distance
+// full-precision distance.  `filtered` (full precision): a filtered range search with one mask per query in `masks`
+// (host or device memory, as the queries) and the mode match_all.
 int range_search(dab_index* idx, const char* api, bool host, const void* queries, uint32_t nq, uint32_t l_search, uint32_t beam, float radius,
                  int has_inner, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, dab_range** out,
-                 int store = -1, bool rerank = false) {
-    if (!idx || !out || (nq && !queries)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
+                 int store = -1, bool rerank = false, bool filtered = false, const uint64_t* masks = nullptr, uint32_t match_all = 0) {
+    if (!idx || !out || (nq && !queries) || (nq && filtered && !masks)) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: NULL argument", api);
     *out = nullptr;
     int rc;
     if ((rc = check_range_args(idx, api, store, rerank, l_search, beam, radius, has_inner, inner_radius, initial_slack, range_slack,
-                               max_returned)))
+                               max_returned, filtered)))
         return rc;
     DAB_CUDA(cudaSetDevice(idx->device));
     if ((rc = idx->h_counters.reserve(64))) return rc;
@@ -883,7 +840,7 @@ int range_search(dab_index* idx, const char* api, bool host, const void* queries
     r->idx = idx;
     r->nq = nq;
     if ((rc = nq ? range_batch(idx, api, host, queries, nq, l_search, beam, radius, has_inner, inner_radius, initial_slack, range_slack,
-                               max_returned, store, rerank, r)
+                               max_returned, store, rerank, r, filtered ? masks : nullptr, match_all)
                  : range_empty(idx, r))) {
         cudaStreamSynchronize(idx->stream);
         range_free(r);
@@ -923,6 +880,21 @@ int dab_range_search_device(dab_index* idx, const void* d_queries, uint32_t nq, 
                             dab_range** out) {
     return range_search(idx, "dab_range_search_device", false, d_queries, nq, l_search, beam_width, radius, has_inner_radius, inner_radius,
                         initial_slack, range_slack, max_returned, out);
+}
+
+// FilteredRange::search (filtered_range_search.rs:119-248): the masks and mode of dab_search_batch_filtered
+int dab_range_search_filtered(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search, uint32_t beam_width, float radius,
+                              int has_inner_radius, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned,
+                              const uint64_t* query_masks, uint32_t match_all, dab_range** out) {
+    return range_search(idx, "dab_range_search_filtered", true, queries, nq, l_search, beam_width, radius, has_inner_radius, inner_radius,
+                        initial_slack, range_slack, max_returned, out, -1, false, true, query_masks, match_all);
+}
+
+int dab_range_search_filtered_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t l_search, uint32_t beam_width, float radius,
+                                     int has_inner_radius, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned,
+                                     const uint64_t* d_query_masks, uint32_t match_all, dab_range** out) {
+    return range_search(idx, "dab_range_search_filtered_device", false, d_queries, nq, l_search, beam_width, radius, has_inner_radius,
+                        inner_radius, initial_slack, range_slack, max_returned, out, -1, false, true, d_query_masks, match_all);
 }
 
 int dab_range_search_pq(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search, uint32_t beam_width, float radius,

@@ -493,6 +493,34 @@ class GpuIndex:
         return self._range_quant_device("minmax", d_queries, nq, l_search, radius, beam_width=beam_width, inner_radius=inner_radius,
                                         initial_slack=initial_slack, range_slack=range_slack, max_returned=max_returned, rerank=rerank)
 
+    def range_search_filtered(self, queries, masks, l_search, radius, *, match_all=False, beam_width=1, inner_radius=None,
+                              initial_slack=1.0, range_slack=1.0, max_returned=None):
+        """FilteredRange::search for the whole batch over the label table (upload_labels): every point within `radius` of
+        each query that its mask accepts (as search_batch_filtered accepts it; `masks` u64 per query, or one for all).
+        Returns range_search's (offsets, ids, dists, cmps, hops, second_round); results are in the reference's order
+        (phase 1's matches by distance, then the second round's in the order found).  max_returned=None: no limit."""
+        with self.range_search_filtered_set(queries, masks, l_search, radius, match_all=match_all, beam_width=beam_width,
+                                            inner_radius=inner_radius, initial_slack=initial_slack, range_slack=range_slack,
+                                            max_returned=max_returned) as r:
+            offsets, cmps, hops, second = r.offsets()
+            ids, dists = r.results()
+        return offsets, ids, dists, cmps, hops, second
+
+    def range_search_filtered_set(self, queries, masks, l_search, radius, *, match_all=False, **kw):
+        """range_search_filtered, keeping the result set on the device: a RangeResults"""
+        queries = self._queries(queries)
+        masks = np.ascontiguousarray(np.broadcast_to(np.asarray(masks, np.uint64), (queries.shape[0],)))
+        return RangeResults(self, _lib.lib().dab_range_search_filtered, _ptr(queries), len(queries), l_search, radius, masks=_ptr(masks),
+                            match_all=match_all, **kw)
+
+    def range_search_filtered_device(self, d_queries, d_masks, nq, l_search, radius, *, match_all=False, beam_width=1, inner_radius=None,
+                                     initial_slack=1.0, range_slack=1.0, max_returned=None):
+        """range_search_filtered of `nq` queries and masks at the device pointers `d_queries` and `d_masks` (integers): a
+        RangeResults"""
+        return RangeResults(self, _lib.lib().dab_range_search_filtered_device, C.c_void_p(d_queries), nq, l_search, radius,
+                            beam_width=beam_width, inner_radius=inner_radius, initial_slack=initial_slack, range_slack=range_slack,
+                            max_returned=max_returned, masks=C.c_void_p(d_masks), match_all=match_all)
+
     def search_batch_device(self, d_queries, nq, k, l_search, beam_width, d_ids, d_dists, d_counts=0, d_cmps=0, d_hops=0):
         """Same with device pointers (integers); results stay in HBM."""
         check(_lib.lib().dab_search_batch_device(self._h, C.c_void_p(d_queries), nq, k, l_search, beam_width,
@@ -1042,11 +1070,14 @@ class RangeResults:
     do not change.  Use as a context manager or call close(); closing the index closes it too."""
 
     def __init__(self, index, search, queries, nq, l_search, radius, beam_width=1, inner_radius=None, initial_slack=1.0,
-                 range_slack=1.0, max_returned=None, rerank=None):
-        """`rerank`: None for the full-precision call, else the rerank flag of a quantized store's call"""
+                 range_slack=1.0, max_returned=None, rerank=None, masks=None, match_all=False):
+        """`rerank`: None for the full-precision call, else the rerank flag of a quantized store's call; `masks`: None,
+        else the masks pointer of a filtered call, which takes match_all after it"""
         self._h = C.c_void_p()
         self.nq = int(nq)
         store_args = () if rerank is None else (int(bool(rerank)),)
+        if masks is not None:
+            store_args = (masks, int(bool(match_all)))
         check(search(index._h, queries, self.nq, l_search, beam_width, radius, int(inner_radius is not None),
                      0.0 if inner_radius is None else inner_radius, initial_slack, range_slack, max_returned or 0, *store_args,
                      C.byref(self._h)))

@@ -314,6 +314,22 @@ impl<T: Element> GpuIndex<T> {
         take_range(set, nq)
     }
 
+    /// `FilteredRange::search` (filtered_range_search.rs:119-248) for the batch: every point within `radius` of each
+    /// query that its mask accepts (`masks`: one per query; `match_all`: ALL, else ANY, as `search_batch_filtered`).
+    pub fn range_search_filtered(&self, queries: &[T], masks: &[u64], match_all: bool, l_search: u32, radius: f32, args: RangeArgs)
+        -> Result<RangeBatch> {
+        assert_eq!(queries.len() % self.dim, 0);
+        let nq = queries.len() / self.dim;
+        assert_eq!(masks.len(), nq);
+        let mut set: *mut sys::dab_range = std::ptr::null_mut();
+        check(unsafe {
+            sys::dab_range_search_filtered(self.raw, queries.as_ptr() as *const c_void, nq as u32, l_search, args.beam_width, radius,
+                                           args.inner_radius.is_some() as i32, args.inner_radius.unwrap_or(0.0), args.initial_slack,
+                                           args.range_slack, args.max_returned.unwrap_or(0), masks.as_ptr(), match_all as u32, &mut set)
+        })?;
+        take_range(set, nq)
+    }
+
     /// `range_search` with every distance of both phases the PQ store's (those of `search_batch_pq`); `rerank`: the
     /// in_range ids by full-precision distance, those within (inner_radius, radius] of it, sorted by it, with it.
     pub fn range_search_pq(&self, queries: &[T], l_search: u32, radius: f32, args: RangeArgs, rerank: bool) -> Result<RangeBatch> {

@@ -438,6 +438,49 @@ int dab_range_search_minmax_device(dab_index* idx, const void* d_queries, uint32
                                    int has_inner_radius, float inner_radius, float initial_slack,
                                    float range_slack, uint64_t max_returned, int rerank,
                                    dab_range** out);
+/* FilteredRange::search (diskann/src/graph/search/filtered_range_search.rs:119-248) over
+ * full-precision rows of every dtype and metric: every point within `radius` of each query that
+ * its mask accepts, with the arguments of dab_range_search plus the masks and mode of
+ * dab_search_batch_filtered (ANY: labels & mask != 0; ALL: labels & mask == mask).
+ *   phase 1: the filtered traversal of dab_search_batch_filtered (inline_filter_search_internal,
+ *     without adaptive L) with a list of l_search + n_start entries.  matched: every accepted start
+ *     point and evaluated neighbour with distance <= radius, sorted by distance (stable: among
+ *     exactly equal distances the earlier match first, the order InlineFilterSearch fixes too;
+ *     -0.0 equal to +0.0).  It is not cut to l_search.
+ *   in_range: the list's first l_search entries and matched, those with distance <= radius,
+ *     sorted by (distance, id) and each id once (:162-172).
+ *   second round iff |in_range| >= (size_t)((float)l_search * initial_slack) and
+ *     |matched| < max_returned (:182-185): the visited set is re-seeded with the in_range ids,
+ *     which also form a FIFO frontier; while it is not empty and |matched| < max_returned, up to
+ *     beam_width ids are popped and their unvisited neighbours evaluated, accepted or not
+ *     (filtered_range_search_internal, :259-322).  Every neighbour with distance <= radius *
+ *     range_slack (an f32 product) is pushed onto the frontier; an accepted one with distance
+ *     <= radius is appended to matched while |matched| < max_returned.  The cap does not cut a hop
+ *     short: the rest of the hop is still evaluated, pushed and counted.
+ *   results: matched.take(max_returned) in order (phase 1's sorted matches, then the second
+ *     round's in the order found; not sorted) without ids with distance <= inner_radius (when
+ *     has_inner_radius), start points and deleted ids.  Start points and deleted ids are walked and
+ *     count toward max_returned; they are never returned.
+ * Per query: cmps and hops are both phases' totals when the second round ran (one scratch counts
+ * both), else phase 1's; cmps do not count start points; second_round says whether it ran.
+ * max_returned == 0 means no limit.  query_masks: one u64 per query (host memory, device memory for
+ * the _device form).  Checked before any device work, each failing with DAB_ERR_INVALID_ARGUMENT
+ * and a message: the checks of dab_range_search in its order up to beam_width > 64, then a label
+ * table uploaded (dab_upload_labels), l_search + n_start <= 1024 and the shared memory of the
+ * filtered kernel (that of dab_search_batch_filtered with a list of l_search + n_start).
+ * DAB_ERR_NOT_READY without vectors and graph.  DAB_ERR_OUT_OF_MEMORY, the result set and
+ * dab_destroy as dab_range_search. */
+int dab_range_search_filtered(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search,
+                              uint32_t beam_width, float radius, int has_inner_radius,
+                              float inner_radius, float initial_slack, float range_slack,
+                              uint64_t max_returned, const uint64_t* query_masks,
+                              uint32_t match_all, dab_range** out);
+int dab_range_search_filtered_device(dab_index* idx, const void* d_queries, uint32_t nq,
+                                     uint32_t l_search, uint32_t beam_width, float radius,
+                                     int has_inner_radius, float inner_radius,
+                                     float initial_slack, float range_slack,
+                                     uint64_t max_returned, const uint64_t* d_query_masks,
+                                     uint32_t match_all, dab_range** out);
 /* offsets [nq + 1]: query q's results are entries offsets[q] .. offsets[q + 1] - 1; cmps, hops
  * [nq] u32 and second_round [nq] (0 / 1) may be NULL.  Host buffers. */
 int dab_range_offsets(const dab_range* r, uint64_t* offsets, uint32_t* cmps, uint32_t* hops,

@@ -288,6 +288,14 @@ class GpuRange {
     RangeResults search_minmax(const T* queries, uint32_t nq, bool rerank = false) {
         return search_store(dab_range_search_minmax, queries, nq, rerank);
     }
+    // FilteredRange::search over the provider's label table: every point within the radius that masks[q] accepts (one
+    // mask per query; match_all: ALL, else ANY, as GpuFiltered)
+    RangeResults search_filtered(const T* queries, uint32_t nq, const uint64_t* masks, bool match_all = false) {
+        dab_range* set = nullptr;
+        check(dab_range_search_filtered(p_.raw(), queries, nq, l_, beam_, radius_, has_inner_ ? 1 : 0, inner_, initial_slack_, range_slack_,
+                                        max_returned_, masks, match_all ? 1 : 0, &set));
+        return take(set, nq);
+    }
 
    private:
     using StoreSearch = int (*)(dab_index*, const void*, uint32_t, uint32_t, uint32_t, float, int, float, float, float, uint64_t, int, dab_range**);

@@ -15,7 +15,11 @@ sq, SQ-8; minmax, MinMax-8 behind DoubleHadamard) with dab_range_search_{pq,sq,m
 full-precision rerank.  Each radius then has a row for the store next to the full-precision row, timed the same way
 (phase 1 of the store is dab_search_batch_{pq,sq,minmax}_device at L), with its average_precision against the same exact
 full-precision in-range sets.
-usage: python tools/bench_range.py [--n N] [--nq NQ] [--reps R] [--beam B] [--store {fp,pq,sq,minmax}] [--rerank] [--json PATH]"""
+--selectivity S runs dab_range_search_filtered_device instead of the unfiltered call: bit 0 of the label table is set on
+a share S of the ids (seeded draw), every query's mask is that bit (ANY), and the exact sets are the in-range ids that
+carry it.  Its rows report the same numbers; phase 1 is not separated (the filtered traversal is part of the call).
+usage: python tools/bench_range.py [--n N] [--nq NQ] [--reps R] [--beam B] [--store {fp,pq,sq,minmax}] [--rerank]
+                                   [--selectivity S] [--json PATH]"""
 import argparse
 import json
 import os
@@ -75,6 +79,7 @@ def main():
     ap.add_argument("--beam", type=int, default=1)
     ap.add_argument("--store", choices=["fp", "pq", "sq", "minmax"], default="fp")
     ap.add_argument("--rerank", action="store_true")
+    ap.add_argument("--selectivity", type=float, default=None)
     ap.add_argument("--json", default="")
     args = ap.parse_args()
     name, power = card()
@@ -89,6 +94,12 @@ def main():
     d_q = torch.from_numpy(queries).cuda()
     build_store(g, cfg, base, args.store)
     stores = ["fp"] if args.store == "fp" else ["fp", args.store]
+    accepted = None
+    if args.selectivity is not None:
+        accepted = np.random.default_rng(bench.SEED_QUERY + 1).random(n + 1) < args.selectivity
+        g.upload_labels(accepted.astype(np.uint64))
+        d_masks = torch.ones(nq, dtype=torch.int64, device="cuda")
+        stores = ["fp_filtered"]
 
     def timed(call):
         call()
@@ -113,6 +124,8 @@ def main():
                                                                                            *(o.data_ptr() for o in outs)))
 
     def range_set(store, radius):
+        if store == "fp_filtered":
+            return g.range_search_filtered_device(d_q.data_ptr(), d_masks.data_ptr(), nq, L, radius, beam_width=args.beam)
         if store == "fp":
             return g.range_search_device(d_q.data_ptr(), nq, L, radius, beam_width=args.beam)
         return getattr(g, f"range_search_{store}_device")(d_q.data_ptr(), nq, L, radius, beam_width=args.beam, rerank=args.rerank)
@@ -129,6 +142,9 @@ def main():
                 hi = mid
         radius = float(np.float32(hi))
         exact, truth = in_range_sets(base_t, bn, queries, radius, True)
+        if accepted is not None:  # the exact matching sets
+            truth = [t[accepted[t]] for t in truth]
+            exact = np.array([len(t) for t in truth])
 
         for store in stores:
             def call():
@@ -142,7 +158,8 @@ def main():
             found = sum(len(np.intersect1d(truth[q], ids[offsets[q]:offsets[q + 1]])) for q in range(nq))
             row = dict(store=store, rerank=args.rerank and store != "fp", target_mean_count=target, radius=radius,
                        exact_mean_count=round(float(exact.mean()), 2), exact_max_count=int(exact.max()), ms_per_batch=round(ms, 3),
-                       phase1_ms=round(phase1[store], 3), phase2_ms=round(ms - phase1[store], 3), qps=round(nq / ms * 1e3, 1),
+                       phase1_ms=round(phase1.get(store, float("nan")), 3), phase2_ms=round(ms - phase1.get(store, float("nan")), 3),
+                       qps=round(nq / ms * 1e3, 1),
                        mean_count=round(float(counts.mean()), 2), max_count=int(counts.max()),
                        second_round_share=round(float(second.mean()), 4), mean_hops=round(float(hops.mean()), 1),
                        mean_cmps=round(float(cmps.mean()), 1), average_precision=round(found / max(1, int(exact.sum())), 4))
@@ -150,7 +167,7 @@ def main():
             rows.append(row)
     summary = dict(gpu=name, power_limit_max_sm_clock=power, workload="c2_1Mx128_f32_l2", n=n, nq=nq, L=L, beam=args.beam,
                    store={"fp": "full_precision", "pq": "pq32_dab_pq_train", "sq": "sq8", "minmax": "minmax8_doublehadamard"}[args.store],
-                   rerank=args.rerank, reps=args.reps, knn_batch_ms=round(knn_ms, 3), range=rows)
+                   rerank=args.rerank, selectivity=args.selectivity, reps=args.reps, knn_batch_ms=round(knn_ms, 3), range=rows)
     print(json.dumps(summary), flush=True)
     if args.json:
         os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)

@@ -75,6 +75,8 @@ for dt, ddt, metric, d in ((np.float32, dab.DType.f32, dab.Metric.L2, 100), (np.
         rad = float(np.median(got[1][:, 4]))                     # range_kernel, range_scan, range_compact
         rng1 = g.range_search(base[:64], 20, rad, initial_slack=0.2)
         rng4 = g.range_search(base[:64], 10, rad * 2, beam_width=4, max_returned=70)
+        frng = g.range_search_filtered(base[:64], 0b101, 20, rad * 2, initial_slack=0.2)  # filtered_range_kernel
+        frng4 = g.range_search_filtered(base[:64], 0b11, 10, rad * 2, match_all=True, beam_width=4, max_returned=70)
         knn = g.flat_knn(base[:16], 5)
         knn_tc = g.flat_knn_tc(base[:16], 5)                     # wgmma + TMA path
         assert np.array_equal(knn[0], knn_tc[0])
