@@ -1,7 +1,8 @@
 // quant_device.cuh — thread-serial emulation of the reference's simd_op for short f32 chunks
 // (PQ LUT entries, encode), the packed-code integer cores, the scalar quantizer and the SQ / MinMax
 // epilogues, and the per-candidate distances of the quantized traversals, shared by quant_kernels.cu, sq_index.cu,
-// search_kernel_pq.cu and search_paged.cu.
+// minmax_kernels.cu, search_kernel_pq.cu, search_kernel_pqs.cu and the StoreSource of the paged, diverse, filtered and
+// range traversals (search_source.cuh).
 #pragma once
 
 #include "distance_device.cuh"
@@ -155,7 +156,7 @@ __device__ __forceinline__ float minmax_finish(int metric, uint32_t ip, uint32_t
 
 // ------------------------------------------------------------------ per-candidate distances of the quantized traversals
 // What one lane computes for one candidate in the quantized accessor's expand_beam: search_kernel_pq.cu (one-shot and
-// in-flight batches) and search_paged.cu (paged sessions) share these, so both return the same bits.
+// in-flight batches) and StoreSource (paged, diverse, filtered and range search) share these, so all return the same bits.
 
 // the integer cores of one packed code row against the query's code words, 16 B at a time
 template <int NBITS>

@@ -3,6 +3,8 @@
 #pragma once
 
 #include "dab_common.cuh"
+#include "search_host.cuh"
+#include "search_source.cuh"
 
 namespace dab {
 
@@ -41,47 +43,23 @@ struct SearchParamsDiverse {
     uint32_t* pools;
     uint32_t pool_cap;
     uint32_t warp_smem, off_gd, off_gi, off_ga, off_cid, off_cd, off_beam;
-    // the quantized traversals (diverse_kernel_quant), named as in SearchParamsPq for the per-candidate code
-    // (quant_device.cuh).  Fields of the full-precision kernel come first, so that its parameter offsets stay as they were.
-    int dtype;
-    const float* pivots;  // PQ: the table, [n_centers][dim]
-    const uint32_t* offsets;
-    const uint8_t* codes;  // [n_total][n_chunks]
-    uint32_t n_chunks, n_centers;
-    int ip_table, direct_cosine;
-    float* luts;  // PQ tables (TableL2 / TableIP): n_chunks x n_centers f32 for every warp of the grid
-    const uint8_t* row_codes;  // SQ / MinMax: the store's rows and the batch's staged queries
-    const float* row_meta;
-    uint32_t code_stride, code_dim;
-    int code_nbits, code_metric;
-    float sq_scale_squared, sq_shift_square_norm;
-    const uint8_t* query_codes;  // [nq][code_stride]
-    const float4* query_meta;    // [nq]
+    StoreParams store;  // the quantized traversals (diverse_kernel_quant)
     // with rerank: the post-processed list of every query (at most L ids) for launch_rerank
     uint32_t* list_ids;     // [nq][list_cap]
     uint32_t* list_counts;  // [nq]
     uint32_t list_cap;
 };
 
-// A CTA's shared memory may not pass this: kDivWarps x (the query, 3 x L list words, 2 x beam_width x max_degree
-// candidate words, the beam).  The query area is the query itself over full-precision rows (i8 / u8: its bytes rounded
-// up to 16; floats: dim f32), the f32 query for PQ, and the query's code row plus 16 bytes of compensations for SQ and
-// MinMax.
+// A CTA's shared memory may not pass this: kDivWarps x (the query area of query_area_bytes, 3 x L list words,
+// 2 x beam_width x max_degree candidate words, the beam)
 constexpr size_t kDiverseMaxSmem = 200 * 1024;
 // "<api>: ... need N B shared memory per CTA" unless (L, beam_width) fit kDiverseMaxSmem on this index for a traversal
 // over `store` (-1: full precision, else a QuantStore); no device work
 int diverse_check_smem(const dab_index* idx, const char* api, uint32_t l_search, uint32_t beam, int store = -1);
 
-// The kernel of this index's schema and its shape: `grid` CTAs of kDivWarps warps are resident, each with `smem_block`
-// bytes of shared memory.  Fills p's shared-memory offsets.
-struct DiversePlan {
-    void (*kern)(const SearchParamsDiverse) = nullptr;
-    int grid = 0;
-    size_t smem_block = 0;
-};
-int diverse_plan(const dab_index* idx, uint32_t l_search, uint32_t beam, int store, SearchParamsDiverse& p, DiversePlan& plan);
-// One pass over p.n_work queries, queued on `stream`
-int diverse_launch(const SearchParamsDiverse& p, const DiversePlan& plan, cudaStream_t stream);
+// The kernel of this index's schema (store -1) or of `store`, and its shape in CTAs of kDivWarps warps; fills p's
+// shared-memory offsets
+int diverse_plan(const dab_index* idx, uint32_t l_search, uint32_t beam, int store, SearchParamsDiverse& p, WarpPlan<SearchParamsDiverse>& plan);
 // Local-queue entries per warp in the first pass at L (tests may ask for fewer), and after a pass where a query's
 // entries outgrew them
 uint64_t diverse_pool_first(const dab_index* idx, uint32_t l_search);

@@ -17,10 +17,8 @@
 // (queue.rs:339-353) cuts a longer list, so a "grown" L below L + #start shortens it.  A query whose visited set outgrows
 // its table is re-run from its start points by the job, and so takes the same decision again.
 #include "dab_common.cuh"
-#include "quant_device.cuh"
 #include "search_common.cuh"
 #include "search_filtered.cuh"
-#include "search_host.cuh"
 #include "search_range.cuh"
 
 #include <algorithm>
@@ -29,8 +27,6 @@
 namespace dab {
 
 namespace {
-
-constexpr int kFiltRows = 4;  // rows in flight per team in the distance loop
 
 __device__ __forceinline__ bool label_accepts(uint64_t labels, uint64_t mask, uint32_t match_all) {
     const uint64_t x = labels & mask;
@@ -101,7 +97,7 @@ struct MatchedTopL {
     static constexpr bool kRange = false;
 };
 
-// One warp's share of a pass.  Src is the distance source of diverse search: load(q), prepare(), distances(cid, cd, n).
+// One warp's share of a pass.  Src is a distance source (search_source.cuh).
 // LIST: with p.list_ids, the matched list of each query (start points included) is written for the rerank.  Sink: where
 // the matches go, MatchedTopL or a sink with kRange (FilteredRangeSink), which sees every hop's candidates through
 // matches() and finishes each query that did not overflow.
@@ -222,92 +218,21 @@ __device__ __forceinline__ void filtered_queries(const SearchParamsFiltered& p, 
     }
 }
 
-// Full precision: rows from global memory with the shared distance schemas (distance_device.cuh), a team of lanes per row
-template <typename TD, int KIND, int POST, int NA>
-struct FullRows {
-    static constexpr bool INT = std::is_same<TD, int8_t>::value || std::is_same<TD, uint8_t>::value;
-    const SearchParamsFiltered& p;
-    float* qf;
-    int lane, dim, qq;  // qq, integer rows: Sum x^2 of the query (unused by inner product)
-    __device__ __forceinline__ void load(uint32_t q) { load_query(reinterpret_cast<const TD*>(p.queries) + (size_t)q * dim, dim, 4, qf, lane); }
-    __device__ __forceinline__ void prepare() {
-        if constexpr (INT) {
-            if (KIND != KIND_IP) qq = warp_int_self<std::is_same<TD, int8_t>::value>(reinterpret_cast<const uint8_t*>(qf), dim, lane);
-        }
-    }
-    __device__ __forceinline__ void distances(const uint32_t* cid, float* cd, uint32_t n) {
-        constexpr int S = INT ? 32 : 8 * NA, TEAMS = 32 / S, U = kFiltRows;
-        using Row = typename std::conditional<INT, uint8_t, TD>::type;
-        const int team = lane / S, slot = lane % S;
-        for (uint32_t c0 = 0; c0 < n; c0 += TEAMS * U) {
-            float r[U];
-            uint32_t cc[U];
-            const Row* rows[U];
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                cc[u] = c0 + u * TEAMS + team;
-                rows[u] = reinterpret_cast<const Row*>(p.vectors + (size_t)cid[min(cc[u], n - 1)] * p.row_stride);
-            }
-            if constexpr (INT) warp_int_multi<std::is_same<TD, int8_t>::value, KIND, U>(reinterpret_cast<const uint8_t*>(qf), rows, dim, lane, qq, r);
-            else team_float_multi<NA, KIND, U>(qf, rows, dim, slot, r);
-#pragma unroll
-            for (int u = 0; u < U; ++u)
-                if (slot == 0 && cc[u] < n) cd[cc[u]] = post_op<POST>(r[u]);
-        }
-        __syncwarp();
-    }
-};
-
 template <typename TD, int KIND, int POST, int NA>
 __global__ void __launch_bounds__(kFiltWarps * 32) filtered_kernel(const SearchParamsFiltered p) {
     extern __shared__ __align__(128) uint8_t smem[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     uint8_t* base = smem + (size_t)wib * p.warp_smem;
-    FullRows<TD, KIND, POST, NA> src{p, reinterpret_cast<float*>(base), lane, (int)p.dim, 0};
+    FullRowSource<TD, KIND, POST, NA, SearchParamsFiltered> src(p, base, lane);
     filtered_queries<false>(p, base, lane, src);
 }
 
-// The quantized accessors (MODE as search_kernel_pq: 0 PQ, 1 SQ, 2 MinMax), per candidate the code of quant_device.cuh,
-// one lane per candidate: the traversal distances of dab_search_batch_{pq,sq,minmax}.
-//   PQ: the query (index dtype, T: Into<f32>) in f32 at the front of the warp's shared memory; TableL2 / TableIP build
-//     the query's table once per query into the warp's own slice of p.luts (global memory, read through L2),
-//     DirectCosine reads the pivots directly.
-//   SQ / MinMax: the query's code words (and MinMax its four compensations), staged before the launch, copied to the
-//     front of the warp's shared memory; the SQ compensation stays in a register.
 template <int MODE>
 __global__ void __launch_bounds__(kFiltWarps * 32) filtered_kernel_quant(const SearchParamsFiltered p) {
     extern __shared__ __align__(128) uint8_t smem[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     uint8_t* base = smem + (size_t)wib * p.warp_smem;
-    const uint32_t entries = p.n_chunks * p.n_centers;
-    struct {
-        const SearchParamsFiltered& p;
-        float* qf;     // PQ: the f32 query
-        uint32_t* qc;  // SQ / MinMax: the query's code words, then (MinMax) {b, n, a, norm_squared}
-        float* lut;    // PQ tables: this warp's table
-        int lane, dim;
-        uint32_t entries;
-        float q_comp;
-        __device__ __forceinline__ void load(uint32_t q) {
-            if (MODE == 0) widen_query(p.dtype, p.queries, q, dim, qf, lane);
-            else load_query_codes<MODE>(p.query_codes + (size_t)q * p.code_stride, p.query_meta + q, p.code_stride >> 2, qc, q_comp, lane);
-        }
-        __device__ __forceinline__ void prepare() {
-            if (MODE == 0 && !p.direct_cosine) {
-                for (uint32_t t = lane; t < entries; t += 32) __stcg(lut + t, pq_table_entry(p, qf, dim, t));
-                __syncwarp();
-            }
-        }
-        __device__ __forceinline__ void distances(const uint32_t* cid, float* cd, uint32_t n) {
-            for (uint32_t c = lane; c < n; c += 32) {
-                if (MODE != 0) cd[c] = packed_code_distance<MODE>(p, qc, q_comp, cid[c]);
-                else if (p.direct_cosine) cd[c] = pq_direct_cosine(p, qf, dim, cid[c]);
-                else cd[c] = pq_table_distance(p, lut, cid[c]);
-            }
-            __syncwarp();
-        }
-    } src{p, reinterpret_cast<float*>(base), reinterpret_cast<uint32_t*>(base),
-          p.luts + (size_t)(blockIdx.x * kFiltWarps + wib) * entries, lane, (int)p.dim, entries, 0.0f};
+    StoreSource<MODE, SearchParamsFiltered> src(p, base, lane, blockIdx.x * kFiltWarps + wib);
     filtered_queries<true>(p, base, lane, src);
 }
 
@@ -500,7 +425,7 @@ __global__ void __launch_bounds__(kFiltWarps * 32) filtered_range_kernel(const F
     extern __shared__ __align__(128) uint8_t smem[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     uint8_t* base = smem + (size_t)wib * p.f.warp_smem;
-    FullRows<TD, KIND, POST, NA> src{p.f, reinterpret_cast<float*>(base), lane, (int)p.f.dim, 0};
+    FullRowSource<TD, KIND, POST, NA, SearchParamsFiltered> src(p.f, base, lane);
     FilteredRangeSink<decltype(src)> sink(p, src, base, lane, (size_t)blockIdx.x * kFiltWarps + wib);
     filtered_queries<false>(p.f, base, lane, src, &sink);
 }
@@ -533,15 +458,11 @@ std::vector<uint16_t> adaptive_table(uint32_t l_search, uint32_t samples, uint32
     return t;
 }
 
-// A warp's shared memory: the query area (filtered_check_smem's comment), the list's distances and ids (best_max
-// entries), the matched list's (L), a hop's candidate ids, distances and decisions, the beam.  `store`: -1 full
-// precision, else a QuantStore.
+// A warp's shared memory: the query area (query_area_bytes), the list's distances and ids (best_max entries), the matched
+// list's (L), a hop's candidate ids, distances and decisions, the beam.  `store`: -1 full precision, else a QuantStore.
 static size_t filtered_warp_smem(const dab_index* idx, uint32_t l_search, uint32_t best_max, uint32_t beam, int store,
                                  SearchParamsFiltered* p) {
-    const bool is_int = idx->dtype == DAB_I8 || idx->dtype == DAB_U8;
-    size_t off;
-    if (store == STORE_SQ || store == STORE_MINMAX) off = round_up((size_t)(store == STORE_SQ ? idx->sq : idx->mm).stride + 16, 16);
-    else off = is_int && store < 0 ? round_up(round_up((size_t)idx->dim, 4), 16) : round_up((size_t)idx->dim * 4, 16);
+    size_t off = query_area_bytes(idx, store);
     const size_t best = round_up((size_t)best_max * 4, 16), matched = round_up((size_t)l_search * 4, 16);
     const size_t ncand = round_up(std::max<size_t>((size_t)beam * idx->max_degree, 32) * 4, 16);
     SearchParamsFiltered scratch;
@@ -565,34 +486,26 @@ int filtered_check_smem(const dab_index* idx, const char* api, uint32_t l_search
     return DAB_OK;
 }
 
-// the grid of plan.kern at plan.smem_block bytes per CTA, at most max_per_sm CTAs per SM
-static int filtered_grid(const dab_index* idx, uint32_t l_search, uint32_t beam, int max_per_sm, FilteredPlan& plan) {
-    const int per_sm = plan.smem_block > kFilteredMaxSmem ? 0 : ctas_per_sm(plan.kern, kFiltWarps * 32, plan.smem_block);
+int filtered_plan(const dab_index* idx, uint32_t l_search, uint32_t best_max, uint32_t beam, int store, SearchParamsFiltered& p,
+                  WarpPlan<SearchParamsFiltered>& plan) {
+    p.warp_smem = (uint32_t)filtered_warp_smem(idx, l_search, best_max, beam, store, &p);
+    plan.smem_block = (size_t)p.warp_smem * kFiltWarps;
+    int rc;
+    if (store >= 0) plan.kern = store == STORE_PQ ? filtered_kernel_quant<0> : store == STORE_SQ ? filtered_kernel_quant<1> : filtered_kernel_quant<2>;
+    else if ((rc = visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) -> int {
+                 plan.kern = filtered_kernel_of<decltype(sc)>();
+                 return DAB_OK;
+             })))
+        return rc;
+    const int per_sm = traversal_ctas_per_sm(idx, store, plan.kern, kFiltWarps, plan.smem_block, kFilteredMaxSmem);
     if (per_sm < 1)
         return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_filtered: L=%u, beam_width=%u, dim=%u need %zu B shared memory per CTA",
                     l_search, beam, idx->dim, plan.smem_block);
-    plan.grid = std::min(per_sm, max_per_sm) * idx->sm_count;
+    plan.grid = per_sm * idx->sm_count;
     return DAB_OK;
 }
 
-int filtered_plan(const dab_index* idx, uint32_t l_search, uint32_t best_max, uint32_t beam, int store, SearchParamsFiltered& p,
-                  FilteredPlan& plan) {
-    p.warp_smem = (uint32_t)filtered_warp_smem(idx, l_search, best_max, beam, store, &p);
-    plan.smem_block = (size_t)p.warp_smem * kFiltWarps;
-    if (store >= 0) {
-        plan.kern = store == STORE_PQ ? filtered_kernel_quant<0> : store == STORE_SQ ? filtered_kernel_quant<1> : filtered_kernel_quant<2>;
-        // every resident warp owns a PQ table (n_chunks x n_centers f32: 32 KB at 32 x 256) that its lookups read
-        // through L2: the cap of search_kernel_pq keeps them L2-resident
-        const bool tables = store == STORE_PQ && idx->metric != DAB_COSINE;
-        return filtered_grid(idx, l_search, beam, tables ? 6 : INT32_MAX, plan);
-    }
-    return visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) -> int {
-        plan.kern = filtered_kernel_of<decltype(sc)>();
-        return filtered_grid(idx, l_search, beam, INT32_MAX, plan);
-    });
-}
-
-int filtered_range_plan(const dab_index* idx, uint32_t l_search, uint32_t beam, FilteredRangeParams& p, FilteredRangePlan& plan) {
+int filtered_range_plan(const dab_index* idx, uint32_t l_search, uint32_t beam, FilteredRangeParams& p, WarpPlan<FilteredRangeParams>& plan) {
     p.f.warp_smem = (uint32_t)filtered_warp_smem(idx, l_search, l_search + idx->n_start, beam, -1, &p.f);
     plan.smem_block = (size_t)p.f.warp_smem * kFiltWarps;
     return visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) -> int {
@@ -600,14 +513,6 @@ int filtered_range_plan(const dab_index* idx, uint32_t l_search, uint32_t beam, 
         plan.kern = filtered_range_kernel<typename S::TD, S::KIND, S::POST, S::NA>;
         return DAB_OK;
     });
-}
-
-int filtered_launch(const SearchParamsFiltered& p, const FilteredPlan& plan, cudaStream_t stream) {
-    DAB_CUDA(cudaFuncSetAttribute(plan.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem_block));
-    plan.kern<<<balanced_grid(p.n_work, plan.grid, kFiltWarps), kFiltWarps * 32, plan.smem_block, stream>>>(p);
-    DAB_LAUNCHED();
-    DAB_CUDA(cudaGetLastError());
-    return DAB_OK;
 }
 
 // ---- the label table ---------------------------------------------------------------------------------------------

@@ -3,6 +3,8 @@
 #pragma once
 
 #include "dab_common.cuh"
+#include "search_host.cuh"
+#include "search_source.cuh"
 
 #include <vector>
 
@@ -44,22 +46,7 @@ struct SearchParamsFiltered {
     uint32_t samples, span;
     const uint16_t* adapt;
     uint32_t warp_smem, off_bd, off_bi, off_md, off_mi, off_cid, off_cd, off_ca, off_beam;
-    // the quantized traversals (filtered_kernel_quant), named as in SearchParamsPq for the per-candidate code
-    // (quant_device.cuh).  Fields of the full-precision kernel come first, so that its parameter offsets stay as they were.
-    int dtype;
-    const float* pivots;  // PQ: the table, [n_centers][dim]
-    const uint32_t* offsets;
-    const uint8_t* codes;  // [n_total][n_chunks]
-    uint32_t n_chunks, n_centers;
-    int ip_table, direct_cosine;
-    float* luts;  // PQ tables (TableL2 / TableIP): n_chunks x n_centers f32 for every warp of the grid
-    const uint8_t* row_codes;  // SQ / MinMax: the store's rows and the batch's staged queries
-    const float* row_meta;
-    uint32_t code_stride, code_dim;
-    int code_nbits, code_metric;
-    float sq_scale_squared, sq_shift_square_norm;
-    const uint8_t* query_codes;  // [nq][code_stride]
-    const float4* query_meta;    // [nq]
+    StoreParams store;  // the quantized traversals (filtered_kernel_quant)
     // with rerank: the matched list of every query (at most L ids, start points included) for launch_rerank
     uint32_t* list_ids;     // [nq][list_cap]
     uint32_t* list_counts;  // [nq]
@@ -83,20 +70,12 @@ uint32_t adaptive_l(uint32_t base_l, uint64_t visited, uint64_t matched, double 
 std::vector<uint16_t> adaptive_table(uint32_t l_search, uint32_t samples, uint32_t span, double scale);
 
 // "<api>: ... need N B shared memory per CTA" unless a list of best_max entries, L matched entries and beam_width fit
-// kFilteredMaxSmem on this index for a traversal over `store` (-1: full precision, else a QuantStore); no device work.
-// The query area is the query itself over full-precision rows (i8 / u8: its bytes rounded up to 16; floats: dim f32),
-// the f32 query for PQ, and the query's code row plus 16 bytes of compensations for SQ and MinMax.
+// kFilteredMaxSmem on this index for a traversal over `store` (-1: full precision, else a QuantStore); no device work
 int filtered_check_smem(const dab_index* idx, const char* api, uint32_t l_search, uint32_t best_max, uint32_t beam, int store = -1);
 
-struct FilteredPlan {
-    void (*kern)(const SearchParamsFiltered) = nullptr;
-    int grid = 0;
-    size_t smem_block = 0;
-};
-// The kernel of this index's schema (store -1) or of `store`, and its shape; fills p's shared-memory offsets
+// The kernel of this index's schema (store -1) or of `store`, and its shape in CTAs of kFiltWarps warps; fills p's
+// shared-memory offsets
 int filtered_plan(const dab_index* idx, uint32_t l_search, uint32_t best_max, uint32_t beam, int store, SearchParamsFiltered& p,
-                  FilteredPlan& plan);
-// One pass over p.n_work queries, queued on `stream`
-int filtered_launch(const SearchParamsFiltered& p, const FilteredPlan& plan, cudaStream_t stream);
+                  WarpPlan<SearchParamsFiltered>& plan);
 
 }  // namespace dab

@@ -1,10 +1,12 @@
 // search_host.cuh — the host side every graph search shares (defined in search_kernel.cu): argument checks, the size of
-// the per-warp visited tables in global memory, the parameter fields every traversal takes from the index, the one-shot
-// search batch and the slots of batches in flight.
+// the per-warp visited tables in global memory, the parameter fields every traversal takes from the index, the query
+// area, CTA cap, plan and launch of the one-query-per-warp traversals, the one-shot search batch and the slots of
+// batches in flight.
 #pragma once
 
 #include "dab_common.cuh"
 
+#include <algorithm>
 #include <type_traits>
 
 namespace dab {
@@ -77,9 +79,11 @@ bool set_tag_map(const dab_index* idx, uint64_t n_buckets, P& p) {
     return true;
 }
 
-// The fields a quantized traversal's parameter block (SearchParamsPq, PagedParams) takes from the store it reads
+// The fields a quantized traversal's parameter block (SearchParamsPq, or the StoreParams of the others) takes from the
+// index and the store it reads
 template <class P>
 void set_store_params(const dab_index* idx, QuantStore store, P& p) {
+    p.dtype = idx->dtype;
     if (store == STORE_PQ) {
         p.pivots = idx->d_pivots;
         p.offsets = idx->d_offsets;
@@ -101,6 +105,47 @@ void set_store_params(const dab_index* idx, QuantStore store, P& p) {
         p.sq_scale_squared = idx->sq_scale * idx->sq_scale;  // AsFunctor (scalar/quantizer.rs:316-335)
         p.sq_shift_square_norm = idx->sq_shift_square_norm;
     }
+}
+
+// The query area at the front of a warp's shared memory in a traversal over `store` (-1: full precision, else a
+// QuantStore): the query itself over full-precision rows (i8 / u8: its bytes rounded up to 16; floats: dim f32), the f32
+// query for PQ, and the query's code row plus 16 bytes of compensations for SQ and MinMax
+inline size_t query_area_bytes(const dab_index* idx, int store) {
+    if (store == STORE_SQ || store == STORE_MINMAX) return round_up((size_t)(store == STORE_SQ ? idx->sq : idx->mm).stride + 16, 16);
+    const bool is_int = idx->dtype == DAB_I8 || idx->dtype == DAB_U8;
+    return is_int && store < 0 ? round_up(round_up((size_t)idx->dim, 4), 16) : round_up((size_t)idx->dim * 4, 16);
+}
+
+// The most CTAs per SM of a traversal over `store` (-1: full precision, else a QuantStore): with a PQ table metric every
+// resident warp owns a table (n_chunks x n_centers f32: 32 KB at 32 x 256) that its lookups read through L2, and the cap
+// of search_kernel_pq keeps them L2-resident; no cap otherwise
+inline int store_ctas_cap(const dab_index* idx, int store) { return store == STORE_PQ && idx->metric != DAB_COSINE ? 6 : INT32_MAX; }
+
+// The CTAs of `kern`, `warps` warps and smem_block bytes of shared memory each, resident on one SM in a traversal over
+// `store`, at most store_ctas_cap; 0 when none fits or smem_block passes max_smem
+template <class P>
+int traversal_ctas_per_sm(const dab_index* idx, int store, void (*kern)(const P), int warps, size_t smem_block, size_t max_smem) {
+    const int per_sm = smem_block > max_smem ? 0 : ctas_per_sm(kern, warps * 32, smem_block);
+    return std::min(per_sm, store_ctas_cap(idx, store));
+}
+
+// A traversal kernel of one query per warp and its shape: `grid` CTAs are resident, each with `smem_block` bytes of
+// shared memory
+template <class P>
+struct WarpPlan {
+    void (*kern)(const P) = nullptr;
+    int grid = 0;
+    size_t smem_block = 0;
+};
+
+// One pass of plan.kern over p.n_work queries in CTAs of `warps` warps, queued on `stream`
+template <class P>
+int warp_launch(const P& p, const WarpPlan<P>& plan, int warps, cudaStream_t stream) {
+    DAB_CUDA(cudaFuncSetAttribute(plan.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem_block));
+    plan.kern<<<balanced_grid(p.n_work, plan.grid, warps), warps * 32, plan.smem_block, stream>>>(p);
+    DAB_LAUNCHED();
+    DAB_CUDA(cudaGetLastError());
+    return DAB_OK;
 }
 
 // Where a batch's results go: ids and dists [nq][k]; counts, cmps and hops [nq], optional

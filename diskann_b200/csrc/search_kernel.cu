@@ -173,10 +173,10 @@ struct SlotJob {
     size_t smem_block = 0;
     // diverse
     SearchParamsDiverse pd;
-    DiversePlan dplan;
+    WarpPlan<SearchParamsDiverse> dplan;
     // filtered
     SearchParamsFiltered pf;
-    FilteredPlan fplan;
+    WarpPlan<SearchParamsFiltered> fplan;
 
     SlotJob(dab_index* idx_, cudaStream_t stream_, Scratch& tables_, Scratch& counters_, Scratch& stage_, Scratch& luts_,
             Scratch& lists_, Scratch& pinned_)
@@ -308,7 +308,6 @@ int SlotJob::plan_quant() {
     const QuantStore mode = (QuantStore)store;
     memset(&pq, 0, sizeof(pq));
     set_batch_params(pq);
-    pq.dtype = idx->dtype;
     set_store_params(idx, mode, pq);
 
     size_t off = 0;
@@ -397,12 +396,11 @@ int SlotJob::plan_diverse() {
 template <class P>
 int SlotJob::plan_store(P& p) {
     const QuantStore mode = (QuantStore)store;
-    p.dtype = idx->dtype;
-    set_store_params(idx, mode, p);
+    set_store_params(idx, mode, p.store);
     int rc;
-    const size_t lut_bytes = mode == STORE_PQ && !p.direct_cosine ? (size_t)warps * idx->pq_chunks * idx->pq_centers * 4 : 16;
+    const size_t lut_bytes = mode == STORE_PQ && !p.store.direct_cosine ? (size_t)warps * idx->pq_chunks * idx->pq_centers * 4 : 16;
     if ((rc = luts->reserve(lut_bytes))) return rc;
-    p.luts = (float*)luts->p;
+    p.store.luts = (float*)luts->p;
     if (rerank) {
         if ((rc = lists->reserve(((size_t)nq * cap + nq) * 4))) return rc;
         p.list_ids = (uint32_t*)lists->p;
@@ -431,7 +429,7 @@ int SlotJob::plan_filtered() {
     return store >= 0 ? plan_store(pf) : DAB_OK;
 }
 
-// the local queues of the warps the next pass over n_work queries launches (diverse_launch's grid)
+// the local queues of the warps the next pass over n_work queries launches (warp_launch's grid)
 int SlotJob::reserve_pools() {
     int rc;
     const uint64_t pass_warps = (uint64_t)balanced_grid(n_work, dplan.grid, kDivWarps) * kDivWarps;
@@ -449,8 +447,8 @@ int SlotJob::reserve_tables() {
 
 // SQ and MinMax: the batch's queries compressed by the store's quantizer (MinMax: the NaN flag read back into h_counters)
 int SlotJob::stage_queries() {
-    const uint8_t** codes = filt ? &pf.query_codes : diverse_k ? &pd.query_codes : &pq.query_codes;
-    const float4** meta = filt ? &pf.query_meta : diverse_k ? &pd.query_meta : &pq.query_meta;
+    const uint8_t** codes = filt ? &pf.store.query_codes : diverse_k ? &pd.store.query_codes : &pq.query_codes;
+    const float4** meta = filt ? &pf.store.query_meta : diverse_k ? &pd.store.query_meta : &pq.query_meta;
     if (store == STORE_SQ) return sq_stage_queries(idx, stream, *stage, d_queries, nq, codes, meta);
     if (store == STORE_MINMAX)
         return minmax_stage_queries(idx, stream, *stage, d_queries, nq, (unsigned long long*)(h_counters + 4), codes, meta);
@@ -492,12 +490,12 @@ int SlotJob::launch_quant() {
 
 int SlotJob::launch_diverse() {
     set_pass_params(pd);
-    return diverse_launch(pd, dplan, stream);
+    return warp_launch(pd, dplan, kDivWarps, stream);
 }
 
 int SlotJob::launch_filtered() {
     set_pass_params(pf);
-    return filtered_launch(pf, fplan, stream);
+    return warp_launch(pf, fplan, kFiltWarps, stream);
 }
 
 // the post-processing of the whole batch: the rerank, or the filter of deleted ids

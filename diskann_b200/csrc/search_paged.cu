@@ -26,10 +26,10 @@
 // a session reads between pages lives in the index's shared scratch: the compressed SQ / MinMax queries are session
 // memory, and a PQ query's table is rebuilt at every call in the session's own table scratch.
 #include "dab_common.cuh"
-#include "quant_device.cuh"
 #include "search_common.cuh"
 #include "search_host.cuh"
 #include "search_pq.cuh"
+#include "search_source.cuh"
 
 #include <algorithm>
 #include <vector>
@@ -39,7 +39,6 @@ namespace dab {
 namespace {
 
 constexpr int kPagedWarps = 4;  // warps per CTA, one query each
-constexpr int kPagedRows = 4;   // rows in flight per team in the distance loop
 
 // where one query's growing state lives (the window and counters have fixed strides)
 struct PagedQuery {
@@ -76,21 +75,7 @@ struct PagedParams {
     float* out_dists;
     uint32_t *out_counts, *out_cmps, *out_hops;
     uint32_t warp_smem, off_cid, off_cd, off_wd, off_wi, off_ws;
-    // the quantized sessions (paged_kernel_quant), named as in SearchParamsPq for the per-candidate code
-    int dtype;
-    const float* pivots;  // PQ: the table, [n_centers][dim]
-    const uint32_t* offsets;
-    const uint8_t* codes;  // [n_total][n_chunks]
-    uint32_t n_chunks, n_centers;
-    int ip_table, direct_cosine;
-    float* luts;  // PQ tables: one table per warp of the grid
-    const uint8_t* row_codes;  // SQ / MinMax: the store's rows and the session's staged queries
-    const float* row_meta;
-    uint32_t code_stride, code_dim;
-    int code_nbits, code_metric;
-    float sq_scale_squared, sq_shift_square_norm;
-    const uint8_t* query_codes;  // [nq][code_stride]
-    const float4* query_meta;    // [nq]
+    StoreParams store;  // the quantized sessions (paged_kernel_quant); SQ / MinMax queries are the session's
 };
 
 // (distance ascending, insertion number descending) as one ascending 64-bit key; -0.0 and +0.0 compare equal
@@ -180,9 +165,8 @@ __device__ __forceinline__ void merge_paged(float* wd, uint32_t* wi, uint32_t* w
 }
 
 // One warp's share of a pass: the session logic of paged search for every query it takes, whatever the distances are.
-// Src is the distance source: load(q) brings query q into the warp's shared memory (before its window is read back),
-// prepare() runs once the window is in place (what the distances need of the loaded query), and distances(cid, cd, n)
-// writes the distances of cid[0..n) into cd[0..n) and ends with the warp converged.
+// Src is a distance source (search_source.cuh): load(q) runs before the query's window is read back, prepare() once
+// the window is in place.
 template <class Src>
 __device__ __forceinline__ void paged_queries(const PagedParams& p, uint8_t* base, int lane, Src& src) {
     uint32_t* cid = reinterpret_cast<uint32_t*>(base + p.off_cid);
@@ -356,95 +340,21 @@ __device__ __forceinline__ void paged_queries(const PagedParams& p, uint8_t* bas
 }
 
 
-// Full precision: rows from global memory with the shared distance schemas (distance_device.cuh)
 template <typename TD, int KIND, int POST, int NA>
 __global__ void __launch_bounds__(kPagedWarps * 32) paged_kernel(const PagedParams p) {
-    constexpr bool INT = std::is_same<TD, int8_t>::value || std::is_same<TD, uint8_t>::value;
     extern __shared__ __align__(128) uint8_t smem[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     uint8_t* base = smem + (size_t)wib * p.warp_smem;
-    float* qf = reinterpret_cast<float*>(base);
-    const int dim = (int)p.dim;
-    struct {
-        const PagedParams& p;
-        float* qf;
-        int lane, dim, qq;
-        __device__ __forceinline__ void load(uint32_t q) {
-            load_query(reinterpret_cast<const TD*>(p.queries) + (size_t)q * dim, dim, 4, qf, lane);
-        }
-        __device__ __forceinline__ void prepare() {
-            qq = 0;  // Sum x^2 of the query (unused by inner product)
-            if constexpr (INT) {
-                if (KIND != KIND_IP) qq = warp_int_self<std::is_same<TD, int8_t>::value>(reinterpret_cast<const uint8_t*>(qf), dim, lane);
-            }
-        }
-        // rows from global memory, a team per row
-        __device__ __forceinline__ void distances(const uint32_t* cid, float* cd, uint32_t n) {
-            constexpr int S = INT ? 32 : 8 * NA, TEAMS = 32 / S, U = kPagedRows;
-            using Row = typename std::conditional<INT, uint8_t, TD>::type;
-            const int team = lane / S, slot = lane % S;
-            for (uint32_t c0 = 0; c0 < n; c0 += TEAMS * U) {
-                float r[U];
-                uint32_t cc[U];
-                const Row* rows[U];
-#pragma unroll
-                for (int u = 0; u < U; ++u) {
-                    cc[u] = c0 + u * TEAMS + team;
-                    rows[u] = reinterpret_cast<const Row*>(p.vectors + (size_t)cid[min(cc[u], n - 1)] * p.row_stride);
-                }
-                if constexpr (INT) warp_int_multi<std::is_same<TD, int8_t>::value, KIND, U>(reinterpret_cast<const uint8_t*>(qf), rows, dim, lane, qq, r);
-                else team_float_multi<NA, KIND, U>(qf, rows, dim, slot, r);
-#pragma unroll
-                for (int u = 0; u < U; ++u)
-                    if (slot == 0 && cc[u] < n) cd[cc[u]] = post_op<POST>(r[u]);
-            }
-            __syncwarp();
-        }
-    } src{p, qf, lane, dim, 0};
+    FullRowSource<TD, KIND, POST, NA, PagedParams> src(p, base, lane);
     paged_queries(p, base, lane, src);
 }
 
-// The quantized accessors (MODE as search_kernel_pq: 0 PQ, 1 SQ, 2 MinMax), per candidate the code of quant_device.cuh.
-//   PQ: the query (index dtype, T: Into<f32>) in f32 at the front of the warp's shared memory; TableL2 / TableIP build
-//     the query's table into the warp's own slice of the session's table scratch at every call (it is not kept between
-//     calls), DirectCosine reads the pivots directly.
-//   SQ / MinMax: the query's code words (and MinMax its four compensations), staged once at begin into session memory,
-//     copied to the front of the warp's shared memory; the SQ compensation stays in a register.
 template <int MODE>
 __global__ void __launch_bounds__(kPagedWarps * 32) paged_kernel_quant(const PagedParams p) {
     extern __shared__ __align__(128) uint8_t smem[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     uint8_t* base = smem + (size_t)wib * p.warp_smem;
-    const uint32_t entries = p.n_chunks * p.n_centers;
-    struct {
-        const PagedParams& p;
-        float* qf;     // PQ: the f32 query
-        uint32_t* qc;  // SQ / MinMax: the query's code words, then (MinMax) {b, n, a, norm_squared}
-        float* lut;    // PQ tables: this warp's table
-        int lane, dim;
-        uint32_t entries;
-        float q_comp;
-        __device__ __forceinline__ void load(uint32_t q) {
-            if (MODE == 0) widen_query(p.dtype, p.queries, q, dim, qf, lane);
-            else load_query_codes<MODE>(p.query_codes + (size_t)q * p.code_stride, p.query_meta + q, p.code_stride >> 2, qc, q_comp, lane);
-        }
-        __device__ __forceinline__ void prepare() {
-            if (MODE == 0 && !p.direct_cosine) {
-                for (uint32_t t = lane; t < entries; t += 32) __stcg(lut + t, pq_table_entry(p, qf, dim, t));
-                __syncwarp();
-            }
-        }
-        // one lane per candidate
-        __device__ __forceinline__ void distances(const uint32_t* cid, float* cd, uint32_t n) {
-            for (uint32_t c = lane; c < n; c += 32) {
-                if (MODE != 0) cd[c] = packed_code_distance<MODE>(p, qc, q_comp, cid[c]);
-                else if (p.direct_cosine) cd[c] = pq_direct_cosine(p, qf, dim, cid[c]);
-                else cd[c] = pq_table_distance(p, lut, cid[c]);
-            }
-            __syncwarp();
-        }
-    } src{p, reinterpret_cast<float*>(base), reinterpret_cast<uint32_t*>(base),
-          p.luts + (size_t)(blockIdx.x * kPagedWarps + wib) * entries, lane, (int)p.dim, entries, 0.0f};
+    StoreSource<MODE, PagedParams> src(p, base, lane, blockIdx.x * kPagedWarps + wib);
     paged_queries(p, base, lane, src);
 }
 
@@ -609,12 +519,16 @@ int run_pass(dab_paged* s) {
     }
 }
 
-// the shared memory of a warp — the query area of `qbytes`, the candidates, the window — and the grid of `kern`;
-// max_per_sm caps the CTAs per SM
-int plan_kernel(dab_paged* s, void (*kern)(const PagedParams), size_t qbytes, int max_per_sm, const char* who) {
+const char* begin_name(int store) {
+    return store == STORE_PQ ? "dab_paged_search_begin_pq" : store == STORE_SQ ? "dab_paged_search_begin_sq"
+           : store == STORE_MINMAX ? "dab_paged_search_begin_minmax" : "dab_paged_search_begin";
+}
+
+// the shared memory of a warp — the query area (query_area_bytes), the candidates, the window — and the grid of `kern`
+int plan_kernel(dab_paged* s, void (*kern)(const PagedParams)) {
     const dab_index* idx = s->idx;
     PagedParams& p = s->p;
-    size_t off = qbytes;
+    size_t off = query_area_bytes(idx, s->store);
     const size_t ncand = round_up(std::max<size_t>(idx->max_degree, 1) * 4, 16), win = round_up((size_t)s->cap * 4, 16);
     p.off_cid = (uint32_t)off, off += ncand;
     p.off_cd = (uint32_t)off, off += ncand;
@@ -624,43 +538,18 @@ int plan_kernel(dab_paged* s, void (*kern)(const PagedParams), size_t qbytes, in
     p.warp_smem = (uint32_t)round_up(off, 128);
     s->smem_block = (size_t)p.warp_smem * kPagedWarps;
     s->kern = kern;
-    const int per_sm = s->smem_block > 200 * 1024 ? 0 : ctas_per_sm(s->kern, kPagedWarps * 32, s->smem_block);
+    const int per_sm = traversal_ctas_per_sm(idx, s->store, s->kern, kPagedWarps, s->smem_block, 200 * 1024);
     if (per_sm < 1)
-        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: L=%u, dim=%u need %zu B shared memory per CTA", who, s->l_search, idx->dim, s->smem_block);
-    s->grid = std::min(per_sm, max_per_sm) * idx->sm_count;
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: L=%u, dim=%u need %zu B shared memory per CTA", begin_name(s->store), s->l_search, idx->dim,
+                    s->smem_block);
+    s->grid = per_sm * idx->sm_count;
     return DAB_OK;
 }
 
-template <typename S>
-int prepare_kernel(dab_paged* s) {
-    const size_t qbytes = S::IS_INT ? round_up(round_up((size_t)s->idx->dim, 4), 16) : round_up((size_t)s->idx->dim * 4, 16);
-    return plan_kernel(s, paged_kernel_of<S>(), qbytes, INT32_MAX, "dab_paged_search_begin");
-}
-
-const char* begin_name(int store) {
-    return store == STORE_PQ ? "dab_paged_search_begin_pq" : store == STORE_SQ ? "dab_paged_search_begin_sq"
-           : store == STORE_MINMAX ? "dab_paged_search_begin_minmax" : "dab_paged_search_begin";
-}
-
-// The quantized sessions: the store's parameters into the session's PagedParams, the kernel and its plan.  The query
-// area holds the f32 query (PQ) or the query's code row and its four compensations (SQ, MinMax).
+// The quantized sessions: the store's parameters into the session's PagedParams, the kernel and its plan
 int prepare_quant_kernel(dab_paged* s) {
-    const dab_index* idx = s->idx;
-    PagedParams& p = s->p;
-    p.dtype = idx->dtype;
-    size_t qbytes;
-    int max_per_sm = INT32_MAX;
-    set_store_params(idx, (QuantStore)s->store, p);
-    if (s->store == STORE_PQ) {
-        qbytes = round_up((size_t)idx->dim * 4, 16);
-        // every resident warp owns a table (n_chunks x n_centers f32: 32 KB at 32 x 256) that its lookups read through
-        // L2: the cap of search_kernel_pq keeps them L2-resident
-        if (!p.direct_cosine) max_per_sm = 6;
-    } else {
-        qbytes = round_up((size_t)p.code_stride + 16, 16);
-    }
-    void (*kern)(const PagedParams) = s->store == STORE_PQ ? paged_kernel_quant<0> : s->store == STORE_SQ ? paged_kernel_quant<1> : paged_kernel_quant<2>;
-    return plan_kernel(s, kern, qbytes, max_per_sm, begin_name(s->store));
+    set_store_params(s->idx, (QuantStore)s->store, s->p.store);
+    return plan_kernel(s, s->store == STORE_PQ ? paged_kernel_quant<0> : s->store == STORE_SQ ? paged_kernel_quant<1> : paged_kernel_quant<2>);
 }
 
 // SQ and MinMax: the session's queries compressed by the store's quantizer into session memory (staged through the
@@ -688,8 +577,8 @@ int stage_session_queries(dab_paged* s) {
     DAB_CUDA(cudaStreamSynchronize(st));
     if (h_nan && *h_nan != ~0ull)
         return fail(DAB_ERR_INVALID_ARGUMENT, "%s: query %llu contains NaN after the transform (InputContainsNaN)", begin_name(s->store), *h_nan);
-    s->p.query_codes = s->d_qcodes;
-    s->p.query_meta = (const float4*)(s->d_qcodes + cbytes);
+    s->p.store.query_codes = s->d_qcodes;
+    s->p.store.query_meta = (const float4*)(s->d_qcodes + cbytes);
     return DAB_OK;
 }
 
@@ -703,7 +592,7 @@ int begin_session(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_s
     s->cap = l_search + idx->n_start;  // PriorityQueueConfiguration::Resizable(L + #start)
     int rc;
     if (store >= 0) rc = prepare_quant_kernel(s);
-    else rc = visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) { return prepare_kernel<decltype(sc)>(s); });
+    else rc = visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) { return plan_kernel(s, paged_kernel_of<decltype(sc)>()); });
     if (rc) return rc;
     const size_t qbytes = (size_t)nq * idx->dim * elem_size(idx->dtype), wbytes = (size_t)nq * s->cap * 4;
     const size_t n1 = std::max<uint32_t>(nq, 1);
@@ -739,9 +628,9 @@ int begin_session(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_s
         cudaFree(s->d_queries);  // the kernel reads the compressed queries only
         s->d_queries = nullptr;
     }
-    if (store == STORE_PQ && !s->p.direct_cosine) {
+    if (store == STORE_PQ && !s->p.store.direct_cosine) {
         DAB_CUDA(cudaMalloc(&s->d_luts, (size_t)s->grid * kPagedWarps * idx->pq_chunks * idx->pq_centers * 4));
-        s->p.luts = s->d_luts;
+        s->p.store.luts = s->d_luts;
     }
 
     PagedParams& p = s->p;

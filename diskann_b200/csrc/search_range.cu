@@ -31,7 +31,6 @@
 // arena has been extended by exactly what those queries need.  A scan and a compaction then lay the results out in
 // query order in the result set, which owns its memory: later writes to the index do not change it.
 #include "dab_common.cuh"
-#include "quant_device.cuh"
 #include "search_common.cuh"
 #include "search_host.cuh"
 #include "search_pq.cuh"
@@ -59,7 +58,6 @@ namespace dab {
 
 namespace {
 
-constexpr int kRangeRows = 4;                  // rows in flight per team in the distance loop
 constexpr size_t kRangeMaxSmem = 200 * 1024;   // a CTA's shared memory
 constexpr uint64_t kRegionBudget = 1ull << 31;  // bytes of in_range regions one pass may take
 
@@ -69,11 +67,9 @@ inline uint64_t round_up_pow2(uint64_t n) {
     return p;
 }
 
-// One warp's share of a pass: the queries of the work list it takes, whatever the distances are.  Src is the distance
-// source: load(q) brings query q into the front of the warp's shared memory, prepare() runs once the visited table is
-// cleared (what the distances need of the loaded query), and distances(cid, cd, n) writes the distances of cid[0..n)
-// into cd[0..n) and ends with the warp converged.  radius_filter: the output drops the ids outside (inner_radius,
-// radius]; without it only start points and deleted ids are dropped (the rerank filters on its own distances).
+// One warp's share of a pass: the queries of the work list it takes, whatever the distances are.  Src is a distance
+// source (search_source.cuh).  radius_filter: the output drops the ids outside (inner_radius, radius]; without it only
+// start points and deleted ids are dropped (the rerank filters on its own distances).
 template <class Src>
 __device__ __forceinline__ void range_queries(const RangeParams& p, uint8_t* base, int lane, Src& src, bool radius_filter) {
     const int wib = threadIdx.x >> 5;
@@ -168,89 +164,21 @@ __device__ __forceinline__ void range_queries(const RangeParams& p, uint8_t* bas
     }
 }
 
-// Full precision: rows from global memory with the shared distance schemas (distance_device.cuh), a team of lanes per row
 template <typename TD, int KIND, int POST, int NA>
 __global__ void __launch_bounds__(kRangeWarps * 32) range_kernel(const RangeParams p) {
-    constexpr bool INT = std::is_same<TD, int8_t>::value || std::is_same<TD, uint8_t>::value;
     extern __shared__ __align__(128) uint8_t smem[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     uint8_t* base = smem + (size_t)wib * p.warp_smem;
-    struct {
-        const RangeParams& p;
-        float* qf;
-        int lane, dim, qq;  // qq, integer rows: Sum x^2 of the query (unused by inner product)
-        __device__ __forceinline__ void load(uint32_t q) { load_query(reinterpret_cast<const TD*>(p.queries) + (size_t)q * dim, dim, 4, qf, lane); }
-        __device__ __forceinline__ void prepare() {
-            if constexpr (INT) {
-                if (KIND != KIND_IP) qq = warp_int_self<std::is_same<TD, int8_t>::value>(reinterpret_cast<const uint8_t*>(qf), dim, lane);
-            }
-        }
-        __device__ __forceinline__ void distances(const uint32_t* cid, float* cd, uint32_t n) {
-            constexpr int S = INT ? 32 : 8 * NA, TEAMS = 32 / S, U = kRangeRows;
-            using Row = typename std::conditional<INT, uint8_t, TD>::type;
-            const int team = lane / S, slot = lane % S;
-            for (uint32_t c0 = 0; c0 < n; c0 += TEAMS * U) {
-                float r[U];
-                uint32_t cc[U];
-                const Row* rows[U];
-#pragma unroll
-                for (int u = 0; u < U; ++u) {
-                    cc[u] = c0 + u * TEAMS + team;
-                    rows[u] = reinterpret_cast<const Row*>(p.vectors + (size_t)cid[min(cc[u], n - 1)] * p.row_stride);
-                }
-                if constexpr (INT) warp_int_multi<std::is_same<TD, int8_t>::value, KIND, U>(reinterpret_cast<const uint8_t*>(qf), rows, dim, lane, qq, r);
-                else team_float_multi<NA, KIND, U>(qf, rows, dim, slot, r);
-#pragma unroll
-                for (int u = 0; u < U; ++u)
-                    if (slot == 0 && cc[u] < n) cd[cc[u]] = post_op<POST>(r[u]);
-            }
-            __syncwarp();
-        }
-    } src{p, reinterpret_cast<float*>(base), lane, (int)p.dim, 0};
+    FullRowSource<TD, KIND, POST, NA, RangeParams> src(p, base, lane);
     range_queries(p, base, lane, src, true);
 }
 
-// The quantized accessors (MODE as search_kernel_pq: 0 PQ, 1 SQ, 2 MinMax), per candidate the code of quant_device.cuh,
-// one lane per candidate: the traversal distances of dab_search_batch_{pq,sq,minmax}.
-//   PQ: the query (index dtype, T: Into<f32>) in f32 at the front of the warp's shared memory; TableL2 / TableIP build
-//     the query's table once per query into the warp's own slice of p.luts (global memory, read through L2),
-//     DirectCosine reads the pivots directly.
-//   SQ / MinMax: the query's code words (and MinMax its four compensations), staged before phase 1, copied to the front
-//     of the warp's shared memory; the SQ compensation stays in a register.
 template <int MODE>
 __global__ void __launch_bounds__(kRangeWarps * 32) range_kernel_quant(const RangeParams p) {
     extern __shared__ __align__(128) uint8_t smem[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     uint8_t* base = smem + (size_t)wib * p.warp_smem;
-    const uint32_t entries = p.n_chunks * p.n_centers;
-    struct {
-        const RangeParams& p;
-        float* qf;     // PQ: the f32 query
-        uint32_t* qc;  // SQ / MinMax: the query's code words, then (MinMax) {b, n, a, norm_squared}
-        float* lut;    // PQ tables: this warp's table
-        int lane, dim;
-        uint32_t entries;
-        float q_comp;
-        __device__ __forceinline__ void load(uint32_t q) {
-            if (MODE == 0) widen_query(p.dtype, p.queries, q, dim, qf, lane);
-            else load_query_codes<MODE>(p.query_codes + (size_t)q * p.code_stride, p.query_meta + q, p.code_stride >> 2, qc, q_comp, lane);
-        }
-        __device__ __forceinline__ void prepare() {
-            if (MODE == 0 && !p.direct_cosine) {
-                for (uint32_t t = lane; t < entries; t += 32) __stcg(lut + t, pq_table_entry(p, qf, dim, t));
-                __syncwarp();
-            }
-        }
-        __device__ __forceinline__ void distances(const uint32_t* cid, float* cd, uint32_t n) {
-            for (uint32_t c = lane; c < n; c += 32) {
-                if (MODE != 0) cd[c] = packed_code_distance<MODE>(p, qc, q_comp, cid[c]);
-                else if (p.direct_cosine) cd[c] = pq_direct_cosine(p, qf, dim, cid[c]);
-                else cd[c] = pq_table_distance(p, lut, cid[c]);
-            }
-            __syncwarp();
-        }
-    } src{p, reinterpret_cast<float*>(base), reinterpret_cast<uint32_t*>(base),
-          p.luts + (size_t)(blockIdx.x * kRangeWarps + wib) * entries, lane, (int)p.dim, entries, 0.0f};
+    StoreSource<MODE, RangeParams> src(p, base, lane, blockIdx.x * kRangeWarps + wib);
     range_queries(p, base, lane, src, !p.rerank);
 }
 
@@ -388,14 +316,10 @@ void (*range_kernel_of())(const RangeParams) {
     return range_kernel<typename S::TD, S::KIND, S::POST, S::NA>;
 }
 
-// A warp's shared memory: the query area, then one node's candidate ids and distances.  The query area is the query
-// itself over full-precision rows (i8 / u8: its bytes rounded up to 16; floats: dim f32), the f32 query for PQ, and the
-// query's code row plus 16 bytes of compensations for SQ and MinMax.  `store`: -1 full precision, else a QuantStore.
+// A warp's shared memory: the query area (query_area_bytes), then one node's candidate ids and distances.  `store`: -1
+// full precision, else a QuantStore.
 size_t range_warp_smem(const dab_index* idx, int store, RangeParams* p) {
-    const bool is_int = idx->dtype == DAB_I8 || idx->dtype == DAB_U8;
-    size_t off;
-    if (store == STORE_SQ || store == STORE_MINMAX) off = round_up((size_t)(store == STORE_SQ ? idx->sq : idx->mm).stride + 16, 16);
-    else off = is_int && store < 0 ? round_up(round_up((size_t)idx->dim, 4), 16) : round_up((size_t)idx->dim * 4, 16);
+    size_t off = query_area_bytes(idx, store);
     const size_t ncand = round_up(std::max<size_t>(idx->max_degree, 32) * 4, 16);
     RangeParams scratch;
     RangeParams& q = p ? *p : scratch;
@@ -595,7 +519,7 @@ int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t n
     size_t smem_block = (size_t)p.warp_smem * kRangeWarps;
     void (*kern)(const RangeParams) = nullptr;
     FilteredRangeParams fp;
-    FilteredRangePlan fplan;
+    WarpPlan<FilteredRangeParams> fplan;
     if (filt) {
         memset(&fp, 0, sizeof(fp));
         if ((rc = filtered_range_plan(idx, l_search, beam, fp, fplan))) return rc;
@@ -608,22 +532,20 @@ int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t n
             return DAB_OK;
         });
     }
-    int per_sm = filt ? ctas_per_sm(fplan.kern, kFiltWarps * 32, smem_block) : ctas_per_sm(kern, kRangeWarps * 32, smem_block);
+    // (the shared memory was checked with the arguments)
+    const int per_sm = filt ? traversal_ctas_per_sm(idx, store, fplan.kern, kFiltWarps, smem_block, SIZE_MAX)
+                            : traversal_ctas_per_sm(idx, store, kern, kRangeWarps, smem_block, SIZE_MAX);
     if (per_sm < 1) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: dim=%u needs %zu B shared memory per CTA", api, idx->dim, smem_block);
-    // every resident warp owns a PQ table (n_chunks x n_centers f32: 32 KB at 32 x 256) that its lookups read through
-    // L2: the cap of search_kernel_pq keeps them L2-resident
-    const bool pq_tables = store == STORE_PQ && idx->metric != DAB_COSINE;
-    if (pq_tables) per_sm = std::min(per_sm, 6);
     const int resident = per_sm * idx->sm_count;
     DevBuf luts;
     if (store >= 0) {
-        p.dtype = idx->dtype;
-        set_store_params(idx, (QuantStore)store, p);
-        p.query_codes = staged.codes;
-        p.query_meta = staged.meta;
+        set_store_params(idx, (QuantStore)store, p.store);
+        p.store.query_codes = staged.codes;
+        p.store.query_meta = staged.meta;
         p.rerank = rerank ? 1 : 0;
+        const bool pq_tables = store == STORE_PQ && !p.store.direct_cosine;
         if ((rc = luts.alloc(pq_tables ? (size_t)resident * kRangeWarps * idx->pq_chunks * idx->pq_centers * 4 : 16, api))) return rc;
-        p.luts = (float*)luts.p;
+        p.store.luts = (float*)luts.p;
     }
     set_graph_params(idx, p);
     p.vectors = idx->d_vectors;

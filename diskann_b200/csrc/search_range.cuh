@@ -6,6 +6,8 @@
 #include "dab_common.cuh"
 #include "search_common.cuh"
 #include "search_filtered.cuh"
+#include "search_host.cuh"
+#include "search_source.cuh"
 
 namespace dab {
 
@@ -53,22 +55,7 @@ struct RangeParams {
     uint32_t *q_count, *out_hops;
     uint8_t* out_second;
     uint32_t warp_smem, off_cid, off_cd;
-    // the quantized stores (range_kernel_quant), named as in SearchParamsPq for the per-candidate code
-    // (quant_device.cuh).  Fields of the full-precision kernel come first, so that its parameter offsets stay as they were.
-    int dtype;
-    const float* pivots;  // PQ: the table, [n_centers][dim]
-    const uint32_t* offsets;
-    const uint8_t* codes;  // [n_total][n_chunks]
-    uint32_t n_chunks, n_centers;
-    int ip_table, direct_cosine;
-    float* luts;  // PQ tables (TableL2 / TableIP): n_chunks x n_centers f32 for every resident warp
-    const uint8_t* row_codes;  // SQ / MinMax: the store's rows and the batch's staged queries
-    const float* row_meta;
-    uint32_t code_stride, code_dim;
-    int code_nbits, code_metric;
-    float sq_scale_squared, sq_shift_square_norm;
-    const uint8_t* query_codes;  // [nq][code_stride]
-    const float4* query_meta;    // [nq]
+    StoreParams store;  // the quantized stores (range_kernel_quant)
     int rerank;  // the output keeps every in_range id but start points and deleted ids, for range_rerank
 };
 
@@ -160,11 +147,8 @@ __device__ __forceinline__ void range_emit(const RangeParams& p, const uint32_t*
 }
 
 // ---- host (search_filtered.cu) ----------------------------------------------------------------------------------------
-struct FilteredRangePlan {
-    void (*kern)(const FilteredRangeParams) = nullptr;
-    size_t smem_block = 0;
-};
-// The filtered range kernel of this index's schema and its shared memory; fills p.f's shared-memory offsets
-int filtered_range_plan(const dab_index* idx, uint32_t l_search, uint32_t beam, FilteredRangeParams& p, FilteredRangePlan& plan);
+// The filtered range kernel of this index's schema and its shared memory (the range search sizes the grid); fills p.f's
+// shared-memory offsets
+int filtered_range_plan(const dab_index* idx, uint32_t l_search, uint32_t beam, FilteredRangeParams& p, WarpPlan<FilteredRangeParams>& plan);
 
 }  // namespace dab
