@@ -415,19 +415,13 @@ int diverse_check_smem(const dab_index* idx, const char* api, uint32_t l_search,
 
 int diverse_plan(const dab_index* idx, uint32_t l_search, uint32_t beam, int store, SearchParamsDiverse& p, WarpPlan<SearchParamsDiverse>& plan) {
     p.warp_smem = (uint32_t)diverse_warp_smem(idx, l_search, beam, store, &p);
-    plan.smem_block = (size_t)p.warp_smem * kDivWarps;
     int rc;
-    if (store >= 0) plan.kern = store == STORE_PQ ? diverse_kernel_quant<0> : store == STORE_SQ ? diverse_kernel_quant<1> : diverse_kernel_quant<2>;
-    else if ((rc = visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) -> int {
-                 plan.kern = diverse_kernel_of<decltype(sc)>();
-                 return DAB_OK;
-             })))
+    if ((rc = traversal_kernel(idx, store, [](auto m) { return diverse_kernel_quant<decltype(m)::value>; },
+                               [](auto sc) { return diverse_kernel_of<decltype(sc)>(); }, plan.kern)))
         return rc;
-    const int per_sm = traversal_ctas_per_sm(idx, store, plan.kern, kDivWarps, plan.smem_block, kDiverseMaxSmem);
-    if (per_sm < 1)
+    if (!plan_warps(idx, store, kDivWarps, p.warp_smem, kDiverseMaxSmem, plan))
         return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_diverse: L=%u, beam_width=%u, dim=%u need %zu B shared memory per CTA",
                     l_search, beam, idx->dim, plan.smem_block);
-    plan.grid = per_sm * idx->sm_count;
     return DAB_OK;
 }
 

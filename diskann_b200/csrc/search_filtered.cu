@@ -489,30 +489,26 @@ int filtered_check_smem(const dab_index* idx, const char* api, uint32_t l_search
 int filtered_plan(const dab_index* idx, uint32_t l_search, uint32_t best_max, uint32_t beam, int store, SearchParamsFiltered& p,
                   WarpPlan<SearchParamsFiltered>& plan) {
     p.warp_smem = (uint32_t)filtered_warp_smem(idx, l_search, best_max, beam, store, &p);
-    plan.smem_block = (size_t)p.warp_smem * kFiltWarps;
     int rc;
-    if (store >= 0) plan.kern = store == STORE_PQ ? filtered_kernel_quant<0> : store == STORE_SQ ? filtered_kernel_quant<1> : filtered_kernel_quant<2>;
-    else if ((rc = visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) -> int {
-                 plan.kern = filtered_kernel_of<decltype(sc)>();
-                 return DAB_OK;
-             })))
+    if ((rc = traversal_kernel(idx, store, [](auto m) { return filtered_kernel_quant<decltype(m)::value>; },
+                               [](auto sc) { return filtered_kernel_of<decltype(sc)>(); }, plan.kern)))
         return rc;
-    const int per_sm = traversal_ctas_per_sm(idx, store, plan.kern, kFiltWarps, plan.smem_block, kFilteredMaxSmem);
-    if (per_sm < 1)
+    if (!plan_warps(idx, store, kFiltWarps, p.warp_smem, kFilteredMaxSmem, plan))
         return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_filtered: L=%u, beam_width=%u, dim=%u need %zu B shared memory per CTA",
                     l_search, beam, idx->dim, plan.smem_block);
-    plan.grid = per_sm * idx->sm_count;
     return DAB_OK;
 }
 
 int filtered_range_plan(const dab_index* idx, uint32_t l_search, uint32_t beam, FilteredRangeParams& p, WarpPlan<FilteredRangeParams>& plan) {
     p.f.warp_smem = (uint32_t)filtered_warp_smem(idx, l_search, l_search + idx->n_start, beam, -1, &p.f);
-    plan.smem_block = (size_t)p.f.warp_smem * kFiltWarps;
-    return visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) -> int {
-        using S = decltype(sc);
-        plan.kern = filtered_range_kernel<typename S::TD, S::KIND, S::POST, S::NA>;
-        return DAB_OK;
-    });
+    int rc;
+    if ((rc = full_kernel(idx, [](auto sc) {
+             using S = decltype(sc);
+             return filtered_range_kernel<typename S::TD, S::KIND, S::POST, S::NA>;
+         }, plan.kern)))
+        return rc;
+    plan_warps(idx, -1, kFiltWarps, p.f.warp_smem, SIZE_MAX, plan);
+    return DAB_OK;
 }
 
 // ---- the label table ---------------------------------------------------------------------------------------------

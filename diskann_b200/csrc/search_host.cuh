@@ -1,10 +1,11 @@
 // search_host.cuh — the host side every graph search shares (defined in search_kernel.cu): argument checks, the size of
 // the per-warp visited tables in global memory, the parameter fields every traversal takes from the index, the query
-// area, CTA cap, plan and launch of the one-query-per-warp traversals, the one-shot search batch and the slots of
-// batches in flight.
+// area, CTA cap, PQ tables, kernel choice, plan and launch of the one-query-per-warp traversals (paged, diverse,
+// filtered, range), the staging of SQ / MinMax queries, the one-shot search batch and the slots of batches in flight.
 #pragma once
 
 #include "dab_common.cuh"
+#include "distance_device.cuh"
 
 #include <algorithm>
 #include <type_traits>
@@ -117,32 +118,61 @@ inline size_t query_area_bytes(const dab_index* idx, int store) {
 }
 
 // The most CTAs per SM of a traversal over `store` (-1: full precision, else a QuantStore): with a PQ table metric every
-// resident warp owns a table (n_chunks x n_centers f32: 32 KB at 32 x 256) that its lookups read through L2, and the cap
-// of search_kernel_pq keeps them L2-resident; no cap otherwise
+// resident warp owns a table (pq_table_bytes) that its lookups read through L2, and the cap of search_kernel_pq keeps
+// them L2-resident; no cap otherwise
 inline int store_ctas_cap(const dab_index* idx, int store) { return store == STORE_PQ && idx->metric != DAB_COSINE ? 6 : INT32_MAX; }
 
-// The CTAs of `kern`, `warps` warps and smem_block bytes of shared memory each, resident on one SM in a traversal over
-// `store`, at most store_ctas_cap; 0 when none fits or smem_block passes max_smem
-template <class P>
-int traversal_ctas_per_sm(const dab_index* idx, int store, void (*kern)(const P), int warps, size_t smem_block, size_t max_smem) {
-    const int per_sm = smem_block > max_smem ? 0 : ctas_per_sm(kern, warps * 32, smem_block);
-    return std::min(per_sm, store_ctas_cap(idx, store));
+// The PQ tables of `warps` warps over `store`: n_chunks x n_centers f32 each for a PQ table metric, else 0 bytes
+// (`cosine_too`: search_kernel_pq's reservation, which keeps them under DirectCosine as well)
+inline size_t pq_table_bytes(const dab_index* idx, int store, uint64_t warps, bool cosine_too = false) {
+    return store == STORE_PQ && (cosine_too || idx->metric != DAB_COSINE) ? (size_t)warps * idx->pq_chunks * idx->pq_centers * 4 : 0;
 }
 
-// A traversal kernel of one query per warp and its shape: `grid` CTAs are resident, each with `smem_block` bytes of
-// shared memory
+// A kind's kernel over `store` into `kern`: quant(integral_constant<int, MODE>) over a store, MODE being the store
+// (STORE_PQ / SQ / MINMAX = 0 / 1 / 2), or full(S) for the index's distance schema S over full-precision rows (-1)
+template <class P, class F>
+int full_kernel(const dab_index* idx, F&& full, void (*&kern)(const P)) {
+    return visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) -> int {
+        kern = full(sc);
+        return DAB_OK;
+    });
+}
+template <class P, class Q, class F>
+int traversal_kernel(const dab_index* idx, int store, Q&& quant, F&& full, void (*&kern)(const P)) {
+    if (store < 0) return full_kernel(idx, full, kern);
+    kern = store == STORE_PQ ? quant(std::integral_constant<int, STORE_PQ>{})
+           : store == STORE_SQ ? quant(std::integral_constant<int, STORE_SQ>{})
+                               : quant(std::integral_constant<int, STORE_MINMAX>{});
+    return DAB_OK;
+}
+
+// A one-query-per-warp kernel and its shape: CTAs of `warps` warps and smem_block bytes, `grid` of them resident
 template <class P>
 struct WarpPlan {
     void (*kern)(const P) = nullptr;
+    int warps = 0;
     int grid = 0;
     size_t smem_block = 0;
+    int pass_grid(uint64_t n_work) const { return balanced_grid(n_work, grid, warps); }  // a pass over n_work queries
 };
 
-// One pass of plan.kern over p.n_work queries in CTAs of `warps` warps, queued on `stream`
+// plan.kern's shape over `store`: CTAs of `warps` warps of warp_smem bytes each, at most store_ctas_cap per SM.  Returns
+// plan.grid: 0 when no CTA fits or smem_block passes max_smem, which the caller reports.
 template <class P>
-int warp_launch(const P& p, const WarpPlan<P>& plan, int warps, cudaStream_t stream) {
+int plan_warps(const dab_index* idx, int store, int warps, size_t warp_smem, size_t max_smem, WarpPlan<P>& plan) {
+    plan.warps = warps;
+    plan.smem_block = warp_smem * warps;
+    const int per_sm = plan.smem_block > max_smem ? 0 : ctas_per_sm(plan.kern, warps * 32, plan.smem_block);
+    plan.grid = std::min(per_sm, store_ctas_cap(idx, store)) * idx->sm_count;
+    return plan.grid;
+}
+
+// One pass of plan.kern in `grid` CTAs (plan.pass_grid, or fewer), queued on `stream`; the shared-memory attribute is set
+// at every launch because it belongs to the kernel, which plans of other shapes share
+template <class P>
+int warp_launch(const P& p, const WarpPlan<P>& plan, int grid, cudaStream_t stream) {
     DAB_CUDA(cudaFuncSetAttribute(plan.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem_block));
-    plan.kern<<<balanced_grid(p.n_work, plan.grid, warps), warps * 32, plan.smem_block, stream>>>(p);
+    plan.kern<<<grid, plan.warps * 32, plan.smem_block, stream>>>(p);
     DAB_LAUNCHED();
     DAB_CUDA(cudaGetLastError());
     return DAB_OK;
@@ -168,6 +198,12 @@ struct StagedQueries {
     const uint8_t* codes;
     const float4* meta;
 };
+
+// SQ / MinMax: the nq queries compressed into `stage` on `stream` (nothing otherwise).  MinMax: staged_first_nan reads
+// the first query holding a NaN after the transform from h_counters (pinned, 24 bytes) once the stream has passed.
+int stage_store_queries(const dab_index* idx, cudaStream_t stream, Scratch& stage, int store, const void* d_queries, uint32_t nq,
+                        uint32_t* h_counters, StagedQueries& out);
+inline unsigned long long staged_first_nan(const uint32_t* h_counters) { return *(const unsigned long long*)(h_counters + 4); }
 
 // Searches whose queries are rows of the index (the build's insert searches, in-place deletes): they ignore deletions
 // and teach the visited tables nothing.  With `ids` each records the nodes it expanded; with `keep_starts` its results

@@ -94,6 +94,13 @@ static int take_overflow_list(cudaStream_t stream, const uint32_t* d_overflow, u
     return DAB_OK;
 }
 
+int stage_store_queries(const dab_index* idx, cudaStream_t stream, Scratch& stage, int store, const void* d_queries, uint32_t nq,
+                        uint32_t* h_counters, StagedQueries& out) {
+    if (store == STORE_SQ) return sq_stage_queries(idx, stream, stage, d_queries, nq, &out.codes, &out.meta);
+    if (store == STORE_MINMAX)
+        return minmax_stage_queries(idx, stream, stage, d_queries, nq, (unsigned long long*)(h_counters + 4), &out.codes, &out.meta);
+    return DAB_OK;
+}
 
 // The checks of a batch that need no plan: the arguments and, for a quantized traversal, the store, its metric and the
 // list length
@@ -164,7 +171,9 @@ struct SlotJob {
     V2Launch v2;
     V3Launch v3;
     bool on_v3 = false;  // the first pass runs on search_kernel_v3
-    // quantized
+    // quantized: staged queries and rerank lists, which each kind's launch copies into its parameter block
+    StagedQueries staged{};
+    uint32_t *list_ids = nullptr, *list_counts = nullptr;
     SearchParamsPq pq;
     PqsPlan plan;
     bool use_pqs = false;
@@ -201,9 +210,11 @@ struct SlotJob {
     int plan_filtered();
     template <class P>
     int plan_store(P& p);
+    int reserve_quant();
     int reserve_tables();
     int reserve_pools();
-    int stage_queries();
+    // SQ and MinMax: the batch's queries compressed by the store's quantizer (MinMax: the NaN flag read back into h_counters)
+    int stage_queries() { return stage_store_queries(idx, stream, *stage, store, d_queries, nq, h_counters, staged); }
     int launch_pass();
     int launch_full();
     int launch_quant();
@@ -214,7 +225,7 @@ struct SlotJob {
     // full precision keeps STORE_PQ in a hint of its own
     VisitedHint& hint() const { return store < 0 ? idx->hint : idx->pq_hint; }
     QuantStore mode() const { return store < 0 ? STORE_PQ : (QuantStore)store; }
-    unsigned long long first_nan() const { return *(const unsigned long long*)(h_counters + 4); }
+    unsigned long long first_nan() const { return staged_first_nan(h_counters); }
     int nan_error() const {
         return fail(DAB_ERR_INVALID_ARGUMENT, "dab_search_batch_minmax: query %llu contains NaN after the transform (InputContainsNaN)", first_nan());
     }
@@ -249,6 +260,12 @@ struct SlotJob {
         p.n_work = n_work;
         p.tables = (uint32_t*)tables->p;
         p.n_buckets = n_buckets;
+    }
+    // a quantized traversal's staged queries (into `q`: the block, or its StoreParams) and rerank lists
+    template <class P, class Q>
+    void set_quant_inputs(P& p, Q& q) const {
+        q.query_codes = staged.codes, q.query_meta = staged.meta;
+        p.list_ids = list_ids, p.list_counts = list_counts, p.list_cap = rerank ? cap : 0;
     }
 };
 
@@ -357,18 +374,10 @@ int SlotJob::plan_quant() {
     }
 
     int rc;
-    const size_t lut_bytes = mode == STORE_PQ && !use_pqs ? (size_t)warps * idx->pq_chunks * idx->pq_centers * 4 : 16;
-    if ((rc = luts->reserve(lut_bytes))) return rc;
+    if ((rc = luts->reserve(std::max<size_t>(use_pqs ? 0 : pq_table_bytes(idx, store, warps, true), 16)))) return rc;
     pq.luts = (float*)luts->p;
-    if (rerank) {
-        if (!idx->vectors_ready) return fail(DAB_ERR_NOT_READY, "dab_search_batch_pq: rerank needs the full-precision vectors");
-        if ((rc = check_rerank(idx, cap))) return rc;
-        if ((rc = lists->reserve(((size_t)nq * cap + nq) * 4))) return rc;
-        pq.list_ids = (uint32_t*)lists->p;
-        pq.list_counts = pq.list_ids + (size_t)nq * cap;
-        pq.list_cap = cap;
-    }
-    return stage->reserve(mode == STORE_SQ ? sq_stage_bytes(idx, nq) : mode == STORE_MINMAX ? minmax_stage_bytes(idx, nq) : 0);
+    if (rerank && (rc = check_rerank(idx, "dab_search_batch_pq", cap))) return rc;
+    return reserve_quant();
 }
 
 // diverse: the kernel's plan, the attribute table and the local queues of the first pass
@@ -385,29 +394,32 @@ int SlotJob::plan_diverse() {
     // diverse_priority_queue.rs:96 in 64 bits; a local queue holds distinct ids, so a capacity of n_total never fills
     // and every larger one behaves the same
     pd.local_cap = (uint32_t)std::min<uint64_t>((uint64_t)diverse_k * l_search / k, idx->n_total());
-    warps = (uint32_t)dplan.grid * kDivWarps;
+    warps = (uint32_t)dplan.grid * dplan.warps;
     if (store >= 0 && (rc = plan_store(pd))) return rc;
     pool = diverse_pool_first(idx, l_search);
     return reserve_pools();
 }
 
 // A diverse or filtered traversal over `store` (the `warps` of its grid planned): the store, a PQ table for every warp
-// of the grid, the lists of the rerank (at most L ids a query: list_cap = cap = L) and the staging of the queries
+// of the grid, and reserve_quant's buffers (the rerank's lists hold at most L ids a query: cap = L)
 template <class P>
 int SlotJob::plan_store(P& p) {
-    const QuantStore mode = (QuantStore)store;
-    set_store_params(idx, mode, p.store);
+    set_store_params(idx, (QuantStore)store, p.store);
     int rc;
-    const size_t lut_bytes = mode == STORE_PQ && !p.store.direct_cosine ? (size_t)warps * idx->pq_chunks * idx->pq_centers * 4 : 16;
-    if ((rc = luts->reserve(lut_bytes))) return rc;
+    if ((rc = luts->reserve(std::max<size_t>(pq_table_bytes(idx, store, warps), 16)))) return rc;
     p.store.luts = (float*)luts->p;
+    return reserve_quant();
+}
+
+// a quantized traversal's rerank lists (at most cap ids a query, then every query's count) and the staging of its queries
+int SlotJob::reserve_quant() {
+    int rc;
     if (rerank) {
         if ((rc = lists->reserve(((size_t)nq * cap + nq) * 4))) return rc;
-        p.list_ids = (uint32_t*)lists->p;
-        p.list_counts = p.list_ids + (size_t)nq * cap;
-        p.list_cap = cap;
+        list_ids = (uint32_t*)lists->p;
+        list_counts = list_ids + (size_t)nq * cap;
     }
-    return stage->reserve(mode == STORE_SQ ? sq_stage_bytes(idx, nq) : mode == STORE_MINMAX ? minmax_stage_bytes(idx, nq) : 0);
+    return stage->reserve(store == STORE_SQ ? sq_stage_bytes(idx, nq) : store == STORE_MINMAX ? minmax_stage_bytes(idx, nq) : 0);
 }
 
 // filtered: the kernel's plan, the label table, the masks and adaptive L's table; over a store, plan_store's buffers
@@ -425,14 +437,14 @@ int SlotJob::plan_filtered() {
     pf.samples = filt->adapt ? filt->samples : 0;
     pf.span = beam * idx->max_degree;
     pf.adapt = filt->adapt;
-    warps = (uint32_t)fplan.grid * kFiltWarps;
+    warps = (uint32_t)fplan.grid * fplan.warps;
     return store >= 0 ? plan_store(pf) : DAB_OK;
 }
 
 // the local queues of the warps the next pass over n_work queries launches (warp_launch's grid)
 int SlotJob::reserve_pools() {
     int rc;
-    const uint64_t pass_warps = (uint64_t)balanced_grid(n_work, dplan.grid, kDivWarps) * kDivWarps;
+    const uint64_t pass_warps = (uint64_t)dplan.pass_grid(n_work) * dplan.warps;
     if ((rc = pools->reserve((size_t)pass_warps * pool * 16))) return rc;
     pd.pools = (uint32_t*)pools->p;
     pd.pool_cap = (uint32_t)pool;
@@ -443,16 +455,6 @@ int SlotJob::reserve_pools() {
 int SlotJob::reserve_tables() {
     n_buckets = (uint32_t)((slots + 7) / 8);
     return tables->reserve((size_t)warps * n_buckets * 32);
-}
-
-// SQ and MinMax: the batch's queries compressed by the store's quantizer (MinMax: the NaN flag read back into h_counters)
-int SlotJob::stage_queries() {
-    const uint8_t** codes = filt ? &pf.store.query_codes : diverse_k ? &pd.store.query_codes : &pq.query_codes;
-    const float4** meta = filt ? &pf.store.query_meta : diverse_k ? &pd.store.query_meta : &pq.query_meta;
-    if (store == STORE_SQ) return sq_stage_queries(idx, stream, *stage, d_queries, nq, codes, meta);
-    if (store == STORE_MINMAX)
-        return minmax_stage_queries(idx, stream, *stage, d_queries, nq, (unsigned long long*)(h_counters + 4), codes, meta);
-    return DAB_OK;
 }
 
 // one traversal pass over the queries of `work` (tables reserved) and the read-back of its counters
@@ -481,6 +483,7 @@ int SlotJob::launch_full() {
 
 int SlotJob::launch_quant() {
     set_pass_params(pq);
+    set_quant_inputs(pq, pq);
     if (use_pqs) return pqs_launch(pq, plan, cap, stream);
     kern<<<grid, kPqWarps * 32, smem_block, stream>>>(pq);
     DAB_LAUNCHED();
@@ -490,21 +493,19 @@ int SlotJob::launch_quant() {
 
 int SlotJob::launch_diverse() {
     set_pass_params(pd);
-    return warp_launch(pd, dplan, kDivWarps, stream);
+    set_quant_inputs(pd, pd.store);
+    return warp_launch(pd, dplan, dplan.pass_grid(n_work), stream);
 }
 
 int SlotJob::launch_filtered() {
     set_pass_params(pf);
-    return warp_launch(pf, fplan, kFiltWarps, stream);
+    set_quant_inputs(pf, pf.store);
+    return warp_launch(pf, fplan, fplan.pass_grid(n_work), stream);
 }
 
 // the post-processing of the whole batch: the rerank, or the filter of deleted ids
 int SlotJob::post() {
-    if (rerank) {
-        const uint32_t* list_ids = filt ? pf.list_ids : diverse_k ? pd.list_ids : pq.list_ids;
-        const uint32_t* list_counts = filt ? pf.list_counts : diverse_k ? pd.list_counts : pq.list_counts;
-        return launch_rerank(idx, stream, d_queries, nq, k, cap, list_ids, list_counts, out.ids, out.dists, out.counts, deleted);
-    }
+    if (rerank) return launch_rerank(idx, stream, d_queries, nq, k, cap, list_ids, list_counts, out.ids, out.dists, out.counts, deleted);
     if (filter) return queue_drop_deleted(idx, stream, deleted, out.ids, out.dists, cap, nq, k, filtered, idx->n_points);
     return DAB_OK;
 }
@@ -576,11 +577,7 @@ static int check_diverse_args(const dab_index* idx, const char* api, uint32_t k,
     if (!idx->d_attr_values) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: no attribute table (dab_upload_attributes has not been called)", api);
     if (store < 0) return DAB_OK;
     if ((rc = check_quant_store(idx, (QuantStore)store, api, false))) return rc;
-    if (rerank) {
-        if (!idx->vectors_ready) return fail(DAB_ERR_NOT_READY, "%s: rerank needs the full-precision vectors", api);
-        if ((rc = check_rerank(idx, l_search))) return rc;
-    }
-    return DAB_OK;
+    return rerank ? check_rerank(idx, api, l_search) : DAB_OK;
 }
 
 // `diverse_k` > 0: a diverse search, whose arguments check_diverse_args has passed; `filt`: a filtered search, whose
@@ -595,7 +592,7 @@ static int run_job(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t 
     job.filt = filt;
     job.pools = &idx->s_pools;
     if ((rc = job.prepare(d_queries, nq, k, l_search, beam, d, store, rerank, rec)) || (rc = job.stage_queries())) return rc;
-    if (rec && rec->staged && store >= 0) *rec->staged = StagedQueries{job.pq.query_codes, job.pq.query_meta};
+    if (rec && rec->staged) *rec->staged = job.staged;
     if (store == STORE_MINMAX) {  // a batch with a NaN query fails before any traversal is launched
         DAB_CUDA(cudaStreamSynchronize(idx->stream));
         if (job.first_nan() != ~0ull) return job.nan_error();
@@ -706,11 +703,7 @@ static int check_filtered_args(const dab_index* idx, const char* api, uint32_t k
     if ((rc = filtered_check_smem(idx, api, l_search, *best_max, beam, store))) return rc;
     if (store < 0) return DAB_OK;
     if ((rc = check_quant_store(idx, (QuantStore)store, api, false))) return rc;
-    if (rerank) {
-        if (!idx->vectors_ready) return fail(DAB_ERR_NOT_READY, "%s: rerank needs the full-precision vectors", api);
-        if ((rc = check_rerank(idx, l_search))) return rc;
-    }
-    return DAB_OK;
+    return rerank ? check_rerank(idx, api, l_search) : DAB_OK;
 }
 
 // InlineFilterSearch::search over a batch: the checks, then the masks (host call: copied to the handle's scratch) and

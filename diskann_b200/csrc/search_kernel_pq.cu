@@ -237,7 +237,8 @@ static size_t rerank_warp_smem(bool is_int, uint32_t dim, uint32_t list_cap) {
     return (is_int ? round_up((size_t)dim, 16) : round_up((size_t)dim * 4, 16)) + 2 * round_up((size_t)list_cap * 4, 16);
 }
 
-int check_rerank(const dab_index* idx, uint32_t list_cap) {
+int check_rerank(const dab_index* idx, const char* api, uint32_t list_cap) {
+    if (!idx->vectors_ready) return fail(DAB_ERR_NOT_READY, "%s: rerank needs the full-precision vectors", api);
     return visit_schema<OPS_ROW>(idx->dtype, idx->metric, [&](auto s) -> int {
         const size_t smem = rerank_warp_smem(decltype(s)::IS_INT, idx->dim, list_cap) * kRerankWarps;
         if (smem > 200 * 1024) return fail(DAB_ERR_INVALID_ARGUMENT, "rerank: configuration needs %zu B shared memory per CTA", smem);

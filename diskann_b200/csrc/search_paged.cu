@@ -402,10 +402,8 @@ struct dab_paged {
     uint32_t nq = 0, l_search = 0, cap = 0;
     int store = -1;           // -1: full precision; else the QuantStore the traversal reads
     uint64_t store_writes = 0;  // idx->store_writes[store] when the session began
-    void (*kern)(const PagedParams) = nullptr;
     PagedParams p{};
-    size_t smem_block = 0;
-    int grid = 0;
+    WarpPlan<PagedParams> plan;
     void* d_queries = nullptr;
     float* d_wd = nullptr;
     uint32_t *d_wi = nullptr, *d_ws = nullptr, *d_ctr = nullptr;
@@ -478,13 +476,10 @@ int run_pass(dab_paged* s) {
     p.n_work = s->nq;
     std::vector<uint32_t> over;
     std::vector<PagedQuery> fresh;
-    // the attribute belongs to the kernel, which sessions of other L share
-    DAB_CUDA(cudaFuncSetAttribute(s->kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s->smem_block));
     for (int pass = 0;;) {
         DAB_CUDA(cudaMemsetAsync(s->d_counters, 0, 8, st));
-        s->kern<<<balanced_grid(p.n_work, s->grid, kPagedWarps), kPagedWarps * 32, s->smem_block, st>>>(p);
-        DAB_LAUNCHED();
-        DAB_CUDA(cudaGetLastError());
+        int rc;
+        if ((rc = warp_launch(p, s->plan, s->plan.pass_grid(p.n_work), st))) return rc;
         uint32_t n_over = 0;
         DAB_CUDA(cudaMemcpyAsync(&n_over, s->d_counters + 1, 4, cudaMemcpyDeviceToHost, st));
         DAB_CUDA(cudaStreamSynchronize(st));
@@ -493,7 +488,7 @@ int run_pass(dab_paged* s) {
         DAB_CUDA(cudaMemcpyAsync(over.data(), s->d_counters + 2, (size_t)n_over * 4, cudaMemcpyDeviceToHost, st));
         DAB_CUDA(cudaStreamSynchronize(st));
         // a table four times larger for each (grow_visited_tables), carved from one new allocation
-        int rc, next_pass = pass;
+        int next_pass = pass;
         size_t bytes = 0;
         for (uint32_t q : over) {
             int pq = pass;
@@ -524,10 +519,15 @@ const char* begin_name(int store) {
            : store == STORE_MINMAX ? "dab_paged_search_begin_minmax" : "dab_paged_search_begin";
 }
 
-// the shared memory of a warp — the query area (query_area_bytes), the candidates, the window — and the grid of `kern`
-int plan_kernel(dab_paged* s, void (*kern)(const PagedParams)) {
+// the session's kernel, the shared memory of a warp — the query area (query_area_bytes), the candidates, the window — and
+// the grid
+int plan_kernel(dab_paged* s) {
     const dab_index* idx = s->idx;
     PagedParams& p = s->p;
+    int rc;
+    if ((rc = traversal_kernel(idx, s->store, [](auto m) { return paged_kernel_quant<decltype(m)::value>; },
+                               [](auto sc) { return paged_kernel_of<decltype(sc)>(); }, s->plan.kern)))
+        return rc;
     size_t off = query_area_bytes(idx, s->store);
     const size_t ncand = round_up(std::max<size_t>(idx->max_degree, 1) * 4, 16), win = round_up((size_t)s->cap * 4, 16);
     p.off_cid = (uint32_t)off, off += ncand;
@@ -536,20 +536,10 @@ int plan_kernel(dab_paged* s, void (*kern)(const PagedParams)) {
     p.off_wi = (uint32_t)off, off += win;
     p.off_ws = (uint32_t)off, off += win;
     p.warp_smem = (uint32_t)round_up(off, 128);
-    s->smem_block = (size_t)p.warp_smem * kPagedWarps;
-    s->kern = kern;
-    const int per_sm = traversal_ctas_per_sm(idx, s->store, s->kern, kPagedWarps, s->smem_block, 200 * 1024);
-    if (per_sm < 1)
+    if (!plan_warps(idx, s->store, kPagedWarps, p.warp_smem, 200 * 1024, s->plan))
         return fail(DAB_ERR_INVALID_ARGUMENT, "%s: L=%u, dim=%u need %zu B shared memory per CTA", begin_name(s->store), s->l_search, idx->dim,
-                    s->smem_block);
-    s->grid = per_sm * idx->sm_count;
+                    s->plan.smem_block);
     return DAB_OK;
-}
-
-// The quantized sessions: the store's parameters into the session's PagedParams, the kernel and its plan
-int prepare_quant_kernel(dab_paged* s) {
-    set_store_params(s->idx, (QuantStore)s->store, s->p.store);
-    return plan_kernel(s, s->store == STORE_PQ ? paged_kernel_quant<0> : s->store == STORE_SQ ? paged_kernel_quant<1> : paged_kernel_quant<2>);
 }
 
 // SQ and MinMax: the session's queries compressed by the store's quantizer into session memory (staged through the
@@ -559,24 +549,21 @@ int stage_session_queries(dab_paged* s) {
     dab_index* idx = s->idx;
     cudaStream_t st = idx->stream;
     const CodeStore& cs = s->store == STORE_SQ ? idx->sq : idx->mm;
-    const uint8_t* qcodes;
-    const float4* qmeta;
     int rc;
-    unsigned long long* h_nan = nullptr;
-    if (s->store == STORE_SQ) {
-        if ((rc = sq_stage_queries(idx, st, idx->s_stage, s->d_queries, s->nq, &qcodes, &qmeta))) return rc;
-    } else {
+    uint32_t* h_counters = nullptr;
+    if (s->store == STORE_MINMAX) {
         if ((rc = idx->h_counters.reserve(24))) return rc;
-        h_nan = (unsigned long long*)((uint32_t*)idx->h_counters.p + 4);
-        if ((rc = minmax_stage_queries(idx, st, idx->s_stage, s->d_queries, s->nq, h_nan, &qcodes, &qmeta))) return rc;
+        h_counters = (uint32_t*)idx->h_counters.p;
     }
+    StagedQueries q{};
+    if ((rc = stage_store_queries(idx, st, idx->s_stage, s->store, s->d_queries, s->nq, h_counters, q))) return rc;
     const size_t cbytes = (size_t)s->nq * cs.stride;
     DAB_CUDA(cudaMalloc(&s->d_qcodes, cbytes + (size_t)s->nq * 16));
-    DAB_CUDA(cudaMemcpyAsync(s->d_qcodes, qcodes, cbytes, cudaMemcpyDeviceToDevice, st));
-    DAB_CUDA(cudaMemcpyAsync(s->d_qcodes + cbytes, qmeta, (size_t)s->nq * 16, cudaMemcpyDeviceToDevice, st));
+    DAB_CUDA(cudaMemcpyAsync(s->d_qcodes, q.codes, cbytes, cudaMemcpyDeviceToDevice, st));
+    DAB_CUDA(cudaMemcpyAsync(s->d_qcodes + cbytes, q.meta, (size_t)s->nq * 16, cudaMemcpyDeviceToDevice, st));
     DAB_CUDA(cudaStreamSynchronize(st));
-    if (h_nan && *h_nan != ~0ull)
-        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: query %llu contains NaN after the transform (InputContainsNaN)", begin_name(s->store), *h_nan);
+    const unsigned long long nan = h_counters ? staged_first_nan(h_counters) : ~0ull;
+    if (nan != ~0ull) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: query %llu contains NaN after the transform (InputContainsNaN)", begin_name(s->store), nan);
     s->p.store.query_codes = s->d_qcodes;
     s->p.store.query_meta = (const float4*)(s->d_qcodes + cbytes);
     return DAB_OK;
@@ -590,10 +577,9 @@ int begin_session(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_s
     s->nq = nq;
     s->l_search = l_search;
     s->cap = l_search + idx->n_start;  // PriorityQueueConfiguration::Resizable(L + #start)
+    if (store >= 0) set_store_params(idx, (QuantStore)store, s->p.store);
     int rc;
-    if (store >= 0) rc = prepare_quant_kernel(s);
-    else rc = visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) { return plan_kernel(s, paged_kernel_of<decltype(sc)>()); });
-    if (rc) return rc;
+    if ((rc = plan_kernel(s))) return rc;
     const size_t qbytes = (size_t)nq * idx->dim * elem_size(idx->dtype), wbytes = (size_t)nq * s->cap * 4;
     const size_t n1 = std::max<uint32_t>(nq, 1);
     DAB_CUDA(cudaMalloc(&s->d_queries, std::max<size_t>(qbytes, 16)));
@@ -628,8 +614,8 @@ int begin_session(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_s
         cudaFree(s->d_queries);  // the kernel reads the compressed queries only
         s->d_queries = nullptr;
     }
-    if (store == STORE_PQ && !s->p.store.direct_cosine) {
-        DAB_CUDA(cudaMalloc(&s->d_luts, (size_t)s->grid * kPagedWarps * idx->pq_chunks * idx->pq_centers * 4));
+    if (const size_t tables = pq_table_bytes(idx, store, (uint64_t)s->plan.grid * s->plan.warps)) {
+        DAB_CUDA(cudaMalloc(&s->d_luts, tables));
         s->p.store.luts = s->d_luts;
     }
 

@@ -62,8 +62,9 @@ using PqKernel = void (*)(const SearchParamsPq);
 // search_kernel_pq's instantiation for lists of `cap` entries over `store`; `keep_starts`: the one whose results keep
 // start points (search_kernel_pq_starts)
 PqKernel pq_kernel(uint32_t cap, QuantStore store, bool keep_starts = false);
-// The rerank of lists of list_cap entries fits a CTA of this index's schema
-int check_rerank(const dab_index* idx, uint32_t list_cap);
+// A quantized call's rerank can run: the full-precision vectors are uploaded (reported under `api`) and the rerank of
+// lists of list_cap entries fits a CTA of this index's schema
+int check_rerank(const dab_index* idx, const char* api, uint32_t list_cap);
 // Reranks each query's list (d_list [nq][list_cap], d_list_n [nq]) by full-precision distance, the start points and the ids
 // `deleted` marks (may be NULL) dropped: the first k into d_ids / d_dists [nq][k] and d_counts, queued on `stream`
 int launch_rerank(const dab_index* idx, cudaStream_t stream, const void* d_queries, uint32_t nq, uint32_t k, uint32_t list_cap,

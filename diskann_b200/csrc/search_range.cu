@@ -311,6 +311,12 @@ __global__ void range_rerank_gather(const uint32_t* pos, uint64_t n, const uint3
     }
 }
 
+// Instantiated here, in this order, for the module order that ptxas's register allocation of the cosine range_kernel
+// instantiations depends on (traversal_kernel alone would instantiate them at the end of the file)
+template __global__ void range_kernel_quant<STORE_SQ>(const RangeParams);
+template __global__ void range_kernel_quant<STORE_MINMAX>(const RangeParams);
+template __global__ void range_kernel_quant<STORE_PQ>(const RangeParams);
+
 template <typename S>
 void (*range_kernel_of())(const RangeParams) {
     return range_kernel<typename S::TD, S::KIND, S::POST, S::NA>;
@@ -516,35 +522,27 @@ int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t n
     RangeParams p;
     memset(&p, 0, sizeof(p));
     p.warp_smem = (uint32_t)range_warp_smem(idx, store, &p);
-    size_t smem_block = (size_t)p.warp_smem * kRangeWarps;
-    void (*kern)(const RangeParams) = nullptr;
+    WarpPlan<RangeParams> plan;
     FilteredRangeParams fp;
     WarpPlan<FilteredRangeParams> fplan;
     if (filt) {
         memset(&fp, 0, sizeof(fp));
-        if ((rc = filtered_range_plan(idx, l_search, beam, fp, fplan))) return rc;
-        smem_block = fplan.smem_block;
-    } else if (store >= 0) {
-        kern = store == STORE_PQ ? range_kernel_quant<0> : store == STORE_SQ ? range_kernel_quant<1> : range_kernel_quant<2>;
-    } else {
-        visit_schema<OPS_QUERY>(idx->dtype, idx->metric, [&](auto sc) -> int {
-            kern = range_kernel_of<decltype(sc)>();
-            return DAB_OK;
-        });
+        rc = filtered_range_plan(idx, l_search, beam, fp, fplan);
+    } else if (!(rc = traversal_kernel(idx, store, [](auto m) { return range_kernel_quant<decltype(m)::value>; },
+                                       [](auto sc) { return range_kernel_of<decltype(sc)>(); }, plan.kern))) {
+        plan_warps(idx, store, kRangeWarps, p.warp_smem, SIZE_MAX, plan);  // (the shared memory was checked with the arguments)
     }
-    // (the shared memory was checked with the arguments)
-    const int per_sm = filt ? traversal_ctas_per_sm(idx, store, fplan.kern, kFiltWarps, smem_block, SIZE_MAX)
-                            : traversal_ctas_per_sm(idx, store, kern, kRangeWarps, smem_block, SIZE_MAX);
-    if (per_sm < 1) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: dim=%u needs %zu B shared memory per CTA", api, idx->dim, smem_block);
-    const int resident = per_sm * idx->sm_count;
+    if (rc) return rc;
+    const int resident = filt ? fplan.grid : plan.grid, warps_per_cta = filt ? fplan.warps : plan.warps;
+    if (!resident)
+        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: dim=%u needs %zu B shared memory per CTA", api, idx->dim, filt ? fplan.smem_block : plan.smem_block);
     DevBuf luts;
     if (store >= 0) {
         set_store_params(idx, (QuantStore)store, p.store);
         p.store.query_codes = staged.codes;
         p.store.query_meta = staged.meta;
         p.rerank = rerank ? 1 : 0;
-        const bool pq_tables = store == STORE_PQ && !p.store.direct_cosine;
-        if ((rc = luts.alloc(pq_tables ? (size_t)resident * kRangeWarps * idx->pq_chunks * idx->pq_centers * 4 : 16, api))) return rc;
+        if ((rc = luts.alloc(std::max<size_t>(pq_table_bytes(idx, store, (uint64_t)resident * warps_per_cta), 16), api))) return rc;
         p.store.luts = (float*)luts.p;
     }
     set_graph_params(idx, p);
@@ -611,13 +609,13 @@ int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t n
     uint64_t used = 0;
     for (;;) {
         // the grid of this pass: one warp per query at most, and regions within kRegionBudget
-        int grid = balanced_grid(p.n_work, resident, kRangeWarps);
+        int grid = balanced_grid(p.n_work, resident, warps_per_cta);
         // a filtered search's warp also holds a frontier of region + L entries and the sort keys of as many
         const uint64_t front = region + l_search, key_cap = filt ? round_up_pow2(front) : 0;
         const uint64_t warp_bytes = region * 8 + (filt ? front * 8 + key_cap * 8 : 0);
-        const uint64_t region_grid = std::max<uint64_t>(1, kRegionBudget / (warp_bytes * kRangeWarps));
+        const uint64_t region_grid = std::max<uint64_t>(1, kRegionBudget / (warp_bytes * warps_per_cta));
         grid = (int)std::min<uint64_t>(grid, region_grid);
-        const uint64_t warps = (uint64_t)grid * kRangeWarps;
+        const uint64_t warps = (uint64_t)grid * warps_per_cta;
         p.n_buckets = (uint32_t)((slots + 7) / 8);
         p.region_cap = (uint32_t)region;
         if ((rc = tables.alloc(warps * p.n_buckets * 32, api)) || (rc = regions.alloc(warps * region * 8, api))) return rc;
@@ -637,14 +635,8 @@ int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t n
             fp.keys = (unsigned long long*)keys.p;
             fp.front_cap = (uint32_t)front;
             fp.key_cap = (uint32_t)key_cap;
-            DAB_CUDA(cudaFuncSetAttribute(fplan.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_block));
-            fplan.kern<<<grid, kFiltWarps * 32, smem_block, st>>>(fp);
-        } else {
-            DAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_block));
-            kern<<<grid, kRangeWarps * 32, smem_block, st>>>(p);
         }
-        DAB_LAUNCHED();
-        DAB_CUDA(cudaGetLastError());
+        if ((rc = filt ? warp_launch(fp, fplan, grid, st) : warp_launch(p, plan, grid, st))) return rc;
         DAB_CUDA(cudaMemcpyAsync(h, ctr.p, 64, cudaMemcpyDeviceToHost, st));
         DAB_CUDA(cudaStreamSynchronize(st));
         const unsigned long long* actr = (const unsigned long long*)h;

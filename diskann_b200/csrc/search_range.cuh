@@ -147,8 +147,8 @@ __device__ __forceinline__ void range_emit(const RangeParams& p, const uint32_t*
 }
 
 // ---- host (search_filtered.cu) ----------------------------------------------------------------------------------------
-// The filtered range kernel of this index's schema and its shared memory (the range search sizes the grid); fills p.f's
-// shared-memory offsets
+// The filtered range kernel of this index's schema and its shape (plan.grid 0: no CTA fits, which the range search
+// reports; its passes cap the grid); fills p.f's shared-memory offsets
 int filtered_range_plan(const dab_index* idx, uint32_t l_search, uint32_t beam, FilteredRangeParams& p, WarpPlan<FilteredRangeParams>& plan);
 
 }  // namespace dab
