@@ -73,6 +73,12 @@ SYMBOLS = {
     "dab_range_search_minmax_device": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, _i, C.POINTER(_vp)]),
     "dab_range_search_filtered": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, _vp, _u32, C.POINTER(_vp)]),
     "dab_range_search_filtered_device": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, _vp, _u32, C.POINTER(_vp)]),
+    "dab_range_search_filtered_pq": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, _vp, _u32, _i, C.POINTER(_vp)]),
+    "dab_range_search_filtered_pq_device": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, _vp, _u32, _i, C.POINTER(_vp)]),
+    "dab_range_search_filtered_sq": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, _vp, _u32, _i, C.POINTER(_vp)]),
+    "dab_range_search_filtered_sq_device": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, _vp, _u32, _i, C.POINTER(_vp)]),
+    "dab_range_search_filtered_minmax": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, _vp, _u32, _i, C.POINTER(_vp)]),
+    "dab_range_search_filtered_minmax_device": (_i, [_vp, _vp, _u32, _u32, _u32, _f, _i, _f, _f, _f, _u64, _vp, _u32, _i, C.POINTER(_vp)]),
     "dab_range_offsets": (_i, [_vp, _vp, _vp, _vp, _vp]),
     "dab_range_results": (_i, [_vp, _vp, _vp]),
     "dab_range_results_device": (_i, [_vp, _vp, _vp]),

@@ -3,7 +3,7 @@
 // default post-processing of the first L matches; and the label table it reads (dab_upload_labels).
 //
 // One warp per query on global visited tables, over full-precision rows of every type and metric of the k-NN path
-// (filtered_kernel) or the PQ, SQ and MinMax stores with the distances of their k-NN traversal and an optional
+// (filtered_kernel; filtered_range_kernel for FilteredRange::search, _quant over a store) or the PQ, SQ and MinMax stores with the distances of their k-NN traversal and an optional
 // full-precision rerank of the first L matches (filtered_kernel_quant).  The traversal is search_internal's: every
 // evaluated neighbour enters the list, accepted or not.  Next to it the warp keeps, in shared memory:
 //   the matched list  the accepted start points and neighbours, at most L of them, ordered by distance with a later
@@ -31,13 +31,6 @@ namespace {
 __device__ __forceinline__ bool label_accepts(uint64_t labels, uint64_t mask, uint32_t match_all) {
     const uint64_t x = labels & mask;
     return match_all ? x == mask : x != 0;
-}
-
-// fast_distance's order as an unsigned key: -0.0 and +0.0 equal, every NaN after every number
-__device__ __forceinline__ uint32_t order_key(float d) {
-    if (d != d) return 0xFFFFFFFFu;
-    const uint32_t u = __float_as_uint(d == 0.0f ? 0.0f : d);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 
 // The accepted ones among candidates c0 .. c0+m-1 (m <= 32; lane j owns candidate j) into the matched list of at most
@@ -267,7 +260,9 @@ __device__ __forceinline__ uint32_t pow2_at_least(uint32_t n) { return n <= 1 ? 
 //             the visited probe); every neighbour with d <= radius * range_slack is pushed onto the frontier, and the
 //             accepted ones with d <= radius are appended to matched while it is below max_returned.  The cap does not
 //             cut a hop short.  cmps and hops count both phases.
-//   output    matched.take(max_returned) in order without start points, deleted ids and ids with d <= inner_radius.
+//   output    matched.take(max_returned) in order without start points, deleted ids and ids with d <= inner_radius;
+//             without radius_filter (a store's call with rerank) only start points and deleted ids are dropped, and
+//             range_rerank applies the inner radius to the full-precision distances.
 // A full region of matches or frontier stops the query, which the job re-runs on regions four times larger.
 template <class Src>
 struct FilteredRangeSink {
@@ -283,8 +278,10 @@ struct FilteredRangeSink {
     float* fd;
     unsigned long long* keys;
     uint64_t m;  // matches within the radius, counted past region_cap
+    bool radius_filter;
 
-    __device__ __forceinline__ FilteredRangeSink(const FilteredRangeParams& p, Src& s, uint8_t* base, int ln, size_t slot) : fp(p), src(s), lane(ln) {
+    __device__ __forceinline__ FilteredRangeSink(const FilteredRangeParams& p, Src& s, uint8_t* base, int ln, size_t slot, bool rf)
+        : fp(p), src(s), lane(ln), radius_filter(rf) {
         cid = reinterpret_cast<uint32_t*>(base + p.f.off_cid);
         cd = reinterpret_cast<float*>(base + p.f.off_cd);
         ca = reinterpret_cast<uint32_t*>(base + p.f.off_ca);
@@ -416,7 +413,7 @@ struct FilteredRangeSink {
             return;
         }
         if (lane == 0) fp.out_cmps[qidx] = cmps;
-        range_emit(p, mid, md, min((uint64_t)M, p.max_returned), true, qidx, hops, second, nvisited, lane);
+        range_emit(p, mid, md, min((uint64_t)M, p.max_returned), radius_filter, qidx, hops, second, nvisited, lane);
     }
 };
 
@@ -426,9 +423,28 @@ __global__ void __launch_bounds__(kFiltWarps * 32) filtered_range_kernel(const F
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     uint8_t* base = smem + (size_t)wib * p.f.warp_smem;
     FullRowSource<TD, KIND, POST, NA, SearchParamsFiltered> src(p.f, base, lane);
-    FilteredRangeSink<decltype(src)> sink(p, src, base, lane, (size_t)blockIdx.x * kFiltWarps + wib);
+    FilteredRangeSink<decltype(src)> sink(p, src, base, lane, (size_t)blockIdx.x * kFiltWarps + wib, true);
     filtered_queries<false>(p.f, base, lane, src, &sink);
 }
+
+// Over a store: the distances of filtered_kernel_quant (p.f.store), the warp's grid index its PQ-table slot; with
+// p.r.rerank the output keeps every match but start points and deleted ids, for range_rerank
+template <int MODE>
+__global__ void __launch_bounds__(kFiltWarps * 32) filtered_range_kernel_quant(const FilteredRangeParams p) {
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    uint8_t* base = smem + (size_t)wib * p.f.warp_smem;
+    const uint32_t slot = blockIdx.x * kFiltWarps + wib;
+    StoreSource<MODE, SearchParamsFiltered> src(p.f, base, lane, slot);
+    FilteredRangeSink<decltype(src)> sink(p, src, base, lane, slot, !p.r.rerank);
+    filtered_queries<false>(p.f, base, lane, src, &sink);
+}
+
+// Instantiated here, in this order, rather than by traversal_kernel in filtered_range_plan: ptxas's register allocation
+// of some kernels depends on their order in the module, and with this placement every other kernel keeps its SASS
+template __global__ void filtered_range_kernel_quant<STORE_SQ>(const FilteredRangeParams);
+template __global__ void filtered_range_kernel_quant<STORE_MINMAX>(const FilteredRangeParams);
+template __global__ void filtered_range_kernel_quant<STORE_PQ>(const FilteredRangeParams);
 
 template <typename S>
 void (*filtered_kernel_of())(const SearchParamsFiltered) {
@@ -499,15 +515,18 @@ int filtered_plan(const dab_index* idx, uint32_t l_search, uint32_t best_max, ui
     return DAB_OK;
 }
 
-int filtered_range_plan(const dab_index* idx, uint32_t l_search, uint32_t beam, FilteredRangeParams& p, WarpPlan<FilteredRangeParams>& plan) {
-    p.f.warp_smem = (uint32_t)filtered_warp_smem(idx, l_search, l_search + idx->n_start, beam, -1, &p.f);
+int filtered_range_plan(const dab_index* idx, uint32_t l_search, uint32_t beam, int store, FilteredRangeParams& p,
+                        WarpPlan<FilteredRangeParams>& plan) {
+    p.f.warp_smem = (uint32_t)filtered_warp_smem(idx, l_search, l_search + idx->n_start, beam, store, &p.f);
     int rc;
-    if ((rc = full_kernel(idx, [](auto sc) {
-             using S = decltype(sc);
-             return filtered_range_kernel<typename S::TD, S::KIND, S::POST, S::NA>;
-         }, plan.kern)))
+    if ((rc = traversal_kernel(idx, store, [](auto m) { return filtered_range_kernel_quant<decltype(m)::value>; },
+                               [](auto sc) {
+                                   using S = decltype(sc);
+                                   return filtered_range_kernel<typename S::TD, S::KIND, S::POST, S::NA>;
+                               },
+                               plan.kern)))
         return rc;
-    plan_warps(idx, -1, kFiltWarps, p.f.warp_smem, SIZE_MAX, plan);
+    plan_warps(idx, store, kFiltWarps, p.f.warp_smem, SIZE_MAX, plan);
     return DAB_OK;
 }
 

@@ -1,7 +1,8 @@
 // search_range.cu — batched range search on the device: Range::search and range_search_internal
-// (diskann/src/graph/search/range_search.rs:255-469) over full-precision rows or the PQ, SQ and MinMax stores, and the
-// result sets it returns (dab_range_search[_pq|_sq|_minmax][_device], dab_range_offsets, dab_range_results[_device],
-// dab_range_free).
+// (diskann/src/graph/search/range_search.rs:255-469) over full-precision rows or the PQ, SQ and MinMax stores, the
+// filtered range search's pass loop (FilteredRange::search, dab_range_search_filtered[_pq|_sq|_minmax][_device]; its
+// kernels are in search_filtered.cu), and the result sets they return (dab_range_search[_pq|_sq|_minmax][_device],
+// dab_range_offsets, dab_range_results[_device], dab_range_free).
 //
 // Phase 1 is the k-NN traversal at L through run_search (search_kernel_v3 / _v2 over full-precision rows,
 // search_kernel_pq_starts over a store): with k = L and start points and deleted ids kept, it writes each query's first
@@ -275,10 +276,34 @@ __device__ __forceinline__ uint32_t sort_key(float d) {
     return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
 
-// One warp per query: the results within (inner_radius, radius], in order, from [from[q], from[q + 1]) to
-// [to[q], to[q + 1]) of ids / dists, with their sort keys and their positions
-__global__ void range_rerank_filter(const uint64_t* from, const uint64_t* to, uint32_t nq, const uint32_t* ids, const float* dists, float radius,
-                                    int has_inner, float inner_radius, uint32_t* out_ids, float* out_dists, uint32_t* keys, uint32_t* pos) {
+// The rerank's rule for a reranked distance: Range's (BOUNDED) keeps (inner_radius, radius] and no NaN reaches its sort;
+// FilteredRange's checks only the inner radius (it takes its matches to be within the radius), so distances above the
+// radius and NaN stay, and NaN sorts after every number (order_key)
+template <bool BOUNDED>
+__device__ __forceinline__ bool rerank_keeps(float d, float radius, int has_inner, float inner_radius) {
+    return BOUNDED ? in_band(d, radius, has_inner, inner_radius) : !(has_inner && d <= inner_radius);
+}
+
+// FilteredRange's rule: how many results of each query rerank_keeps, over range_rerank_kernel's counts of Range's; a
+// warp per query
+__global__ void range_rerank_count_unbounded(const uint64_t* offsets, uint32_t nq, const float* dists, int has_inner, float inner_radius,
+                                             uint32_t* counts) {
+    const int lane = threadIdx.x & 31;
+    const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x >> 5);
+    for (uint64_t q = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5; q < nq; q += warps) {
+        uint32_t count = 0;
+        for (uint64_t i = offsets[q] + lane; i < offsets[q + 1]; i += 32) count += rerank_keeps<false>(dists[i], 0.0f, has_inner, inner_radius) ? 1u : 0u;
+        count = __reduce_add_sync(kFull, count);
+        if (lane == 0) counts[q] = count;
+    }
+}
+
+// One warp per query: the results the rule keeps, in order, from [from[q], from[q + 1]) to [to[q], to[q + 1]) of ids /
+// dists, with their sort keys and their positions
+template <bool BOUNDED>
+__device__ __forceinline__ void rerank_filter(const uint64_t* from, const uint64_t* to, uint32_t nq, const uint32_t* ids, const float* dists,
+                                              float radius, int has_inner, float inner_radius, uint32_t* out_ids, float* out_dists, uint32_t* keys,
+                                              uint32_t* pos) {
     const int lane = threadIdx.x & 31;
     const unsigned below = (1u << lane) - 1u;
     const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x >> 5);
@@ -288,18 +313,29 @@ __global__ void range_rerank_filter(const uint64_t* from, const uint64_t* to, ui
         for (uint64_t i0 = b; i0 < e; i0 += 32) {
             const uint64_t i = i0 + lane;
             const float d = i < e ? dists[i] : 0.0f;
-            const bool k = i < e && in_band(d, radius, has_inner, inner_radius);
+            const bool k = i < e && rerank_keeps<BOUNDED>(d, radius, has_inner, inner_radius);
             const unsigned m = __ballot_sync(kFull, k);
             if (k) {
                 const uint64_t at = w + __popc(m & below);
                 out_ids[at] = ids[i];
                 out_dists[at] = d;
-                keys[at] = sort_key(d);
+                keys[at] = BOUNDED ? sort_key(d) : order_key(d);
                 pos[at] = (uint32_t)at;
             }
             w += __popc(m);
         }
     }
+}
+
+__global__ void range_rerank_filter(const uint64_t* from, const uint64_t* to, uint32_t nq, const uint32_t* ids, const float* dists, float radius,
+                                    int has_inner, float inner_radius, uint32_t* out_ids, float* out_dists, uint32_t* keys, uint32_t* pos) {
+    rerank_filter<true>(from, to, nq, ids, dists, radius, has_inner, inner_radius, out_ids, out_dists, keys, pos);
+}
+
+__global__ void range_rerank_filter_unbounded(const uint64_t* from, const uint64_t* to, uint32_t nq, const uint32_t* ids, const float* dists,
+                                              float radius, int has_inner, float inner_radius, uint32_t* out_ids, float* out_dists, uint32_t* keys,
+                                              uint32_t* pos) {
+    rerank_filter<false>(from, to, nq, ids, dists, radius, has_inner, inner_radius, out_ids, out_dists, keys, pos);
 }
 
 // out[i] <- in[pos[i]], ids and dists
@@ -343,7 +379,8 @@ size_t range_rerank_smem(const dab_index* idx) {
 // The range search's own checks, after Range::validate_and_create's (range_search.rs:91-131) in its order.  Over a
 // quantized store (`store` >= 0) the traversal reads the graph and the store only; the store checks of its k-NN call
 // follow, then those of the rerank.  A filtered range search (`filtered`) checks, after beam_width, the label table, the
-// filtered kernel's list (L + #start <= kFilteredMaxL) and its shared memory.
+// filtered kernel's list (L + #start <= kFilteredMaxL) and its shared memory (with the store's query area), in place of
+// the range kernel's shared memory.
 int check_range_args(const dab_index* idx, const char* api, int store, bool rerank, uint32_t l_search, uint32_t beam, float radius,
                      int has_inner, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, bool filtered = false) {
     if (store < 0 && (!idx->graph_ready || !idx->vectors_ready)) return fail(DAB_ERR_NOT_READY, "%s: vectors and graph must be uploaded first", api);
@@ -363,12 +400,14 @@ int check_range_args(const dab_index* idx, const char* api, int store, bool rera
         if (!idx->d_labels) return fail(DAB_ERR_INVALID_ARGUMENT, "%s: no label table (dab_upload_labels has not been called)", api);
         if ((uint64_t)l_search + idx->n_start > kFilteredMaxL)
             return fail(DAB_ERR_INVALID_ARGUMENT, "%s: L + #start = %llu > %u", api, (unsigned long long)l_search + idx->n_start, kFilteredMaxL);
-        return filtered_check_smem(idx, api, l_search, l_search + idx->n_start, beam);
+        int rc;
+        if ((rc = filtered_check_smem(idx, api, l_search, l_search + idx->n_start, beam, store))) return rc;
+    } else {
+        const size_t smem = range_warp_smem(idx, store, nullptr) * kRangeWarps;
+        if (smem > kRangeMaxSmem)
+            return fail(DAB_ERR_INVALID_ARGUMENT, "%s: dim=%u, max_degree=%u need %zu B shared memory per CTA (> %zu)", api, idx->dim,
+                        idx->max_degree, smem, kRangeMaxSmem);
     }
-    const size_t smem = range_warp_smem(idx, store, nullptr) * kRangeWarps;
-    if (smem > kRangeMaxSmem)
-        return fail(DAB_ERR_INVALID_ARGUMENT, "%s: dim=%u, max_degree=%u need %zu B shared memory per CTA (> %zu)", api, idx->dim, idx->max_degree,
-                    smem, kRangeMaxSmem);
     if (store < 0) return DAB_OK;
     int rc;
     if ((rc = check_quant_store(idx, (QuantStore)store, api, false))) return rc;
@@ -403,10 +442,11 @@ void range_free(dab_range* r) {
     delete r;
 }
 
-// The rerank of a result set whose results are every in_range id but start points and deleted ids: their full-precision
-// distances, then those within (inner_radius, radius] sorted per query by that distance, stably
+// The rerank of a result set whose results are every in_range id (a filtered search: every match it returns) but start
+// points and deleted ids: their full-precision distances, then those the rule keeps (`bounded`: Range's, within
+// (inner_radius, radius]; else FilteredRange's, above inner_radius) sorted per query by that distance, stably
 int range_rerank(dab_index* idx, const char* api, const void* d_queries, uint32_t nq, float radius, int has_inner, float inner_radius,
-                 dab_range* r) {
+                 bool bounded, dab_range* r) {
     cudaStream_t st = idx->stream;
     int rc;
     DevBuf counts, offsets;
@@ -438,6 +478,11 @@ int range_rerank(dab_index* idx, const char* api, const void* d_queries, uint32_
         return rc;
     DAB_LAUNCHED();
     DAB_CUDA(cudaGetLastError());
+    if (!bounded) {
+        range_rerank_count_unbounded<<<grid_for(idx, (uint64_t)nq * 32), 256, 0, st>>>(p.offsets, nq, p.dists, p.has_inner, inner_radius, p.counts);
+        DAB_LAUNCHED();
+        DAB_CUDA(cudaGetLastError());
+    }
     range_scan<<<1, 1024, 0, st>>>(p.counts, nq, (uint64_t*)offsets.p);
     DAB_LAUNCHED();
     DAB_CUDA(cudaGetLastError());
@@ -458,8 +503,8 @@ int range_rerank(dab_index* idx, const char* api, const void* d_queries, uint32_
     uint32_t* v_in = k_in + total;
     uint32_t* k_out = v_in + total;
     uint32_t* v_out = k_out + total;
-    range_rerank_filter<<<grid_for(idx, (uint64_t)nq * 32), 256, 0, st>>>(r->offsets(), (const uint64_t*)offsets.p, nq, p.ids, p.dists, radius,
-                                                                          p.has_inner, inner_radius, kept_ids, kept_dists, k_in, v_in);
+    (bounded ? range_rerank_filter : range_rerank_filter_unbounded)<<<grid_for(idx, (uint64_t)nq * 32), 256, 0, st>>>(
+        r->offsets(), (const uint64_t*)offsets.p, nq, p.ids, p.dists, radius, p.has_inner, inner_radius, kept_ids, kept_dists, k_in, v_in);
     DAB_LAUNCHED();
     DAB_CUDA(cudaGetLastError());
     if (total) {
@@ -491,8 +536,8 @@ struct RangeFilter {
 };
 
 // Both phases for nq >= 1 queries (checks passed) into a new result set: over full-precision rows (`store` -1) or a
-// QuantStore, whose results `rerank` reorders by full-precision distance.  With `filt` (full precision) both phases are
-// the filtered range search's, in filtered_range_kernel: its passes run the traversal too, and write cmps.
+// QuantStore, whose results `rerank` reorders by full-precision distance.  With `filt` both phases are the filtered range
+// search's, in filtered_range_kernel (_quant over a store): its passes run the traversal too, and write cmps.
 int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t nq, uint32_t l_search, uint32_t beam, float radius, int has_inner,
               float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, int store, bool rerank, dab_range* r,
               const RangeFilter* filt) {
@@ -517,6 +562,18 @@ int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t n
     if (!filt && (rc = run_search(idx, d_queries, nq, l_search, l_search, beam, SearchOut{list_ids, list_dists, list_counts, r->cmps(), list_hops},
                                   store, false, &rec)))
         return rc;
+    uint32_t* h = (uint32_t*)idx->h_counters.p;  // pinned: the five counters, then the three arena counters
+    if (filt && (store == STORE_SQ || store == STORE_MINMAX)) {
+        // the filtered traversal does not run through the job: the queries are compressed here, once for both phases
+        if ((rc = idx->s_stage.reserve(store == STORE_SQ ? sq_stage_bytes(idx, nq) : minmax_stage_bytes(idx, nq))) ||
+            (rc = stage_store_queries(idx, st, idx->s_stage, store, d_queries, nq, h, staged)))
+            return rc;
+        if (store == STORE_MINMAX) {  // a batch with a NaN query fails before any traversal is launched
+            DAB_CUDA(cudaStreamSynchronize(st));
+            if (staged_first_nan(h) != ~0ull)
+                return fail(DAB_ERR_INVALID_ARGUMENT, "%s: query %llu contains NaN after the transform (InputContainsNaN)", api, staged_first_nan(h));
+        }
+    }
 
     // ---- phase 2
     RangeParams p;
@@ -527,7 +584,7 @@ int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t n
     WarpPlan<FilteredRangeParams> fplan;
     if (filt) {
         memset(&fp, 0, sizeof(fp));
-        rc = filtered_range_plan(idx, l_search, beam, fp, fplan);
+        rc = filtered_range_plan(idx, l_search, beam, store, fp, fplan);
     } else if (!(rc = traversal_kernel(idx, store, [](auto m) { return range_kernel_quant<decltype(m)::value>; },
                                        [](auto sc) { return range_kernel_of<decltype(sc)>(); }, plan.kern))) {
         plan_warps(idx, store, kRangeWarps, p.warp_smem, SIZE_MAX, plan);  // (the shared memory was checked with the arguments)
@@ -573,6 +630,7 @@ int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t n
         fp.f.labels = idx->d_labels;
         fp.f.masks = filt->masks;
         fp.f.match_all = filt->match_all;
+        fp.f.store = p.store;
         fp.out_cmps = r->cmps();
     }
 
@@ -585,7 +643,6 @@ int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t n
     p.q_pos = (uint64_t*)per_query.p;
     p.q_count = (uint32_t*)(p.q_pos + nq);
     DAB_CUDA(cudaMemsetAsync(ctr.p, 0, 64, st));
-    uint32_t* h = (uint32_t*)idx->h_counters.p;  // pinned: the five counters, then the three arena counters
 
     // the in_range regions (filtered: the matches, which max_returned does not bound in phase 1) and the arena of the
     // first pass
@@ -698,7 +755,7 @@ int range_run(dab_index* idx, const char* api, const void* d_queries, uint32_t n
     if (rerank) {
         cudaFree(luts.p), cudaFree(p1.p), cudaFree(arena1.p), cudaFree(arena2.p);
         luts.p = p1.p = arena1.p = arena2.p = nullptr;
-        return range_rerank(idx, api, d_queries, nq, radius, has_inner, inner_radius, r);
+        return range_rerank(idx, api, d_queries, nq, radius, has_inner, inner_radius, !filt, r);
     }
     return DAB_OK;
 }
@@ -737,8 +794,8 @@ int range_batch(dab_index* idx, const char* api, bool host, const void* queries,
 }
 
 // `store`: -1 full precision, else the QuantStore both phases read; `rerank` (a store) reorders the results by
-// full-precision distance.  `filtered` (full precision): a filtered range search with one mask per query in `masks`
-// (host or device memory, as the queries) and the mode match_all.
+// full-precision distance.  `filtered`: a filtered range search with one mask per query in `masks` (host or device
+// memory, as the queries) and the mode match_all.
 int range_search(dab_index* idx, const char* api, bool host, const void* queries, uint32_t nq, uint32_t l_search, uint32_t beam, float radius,
                  int has_inner, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned, dab_range** out,
                  int store = -1, bool rerank = false, bool filtered = false, const uint64_t* masks = nullptr, uint32_t match_all = 0) {
@@ -809,6 +866,50 @@ int dab_range_search_filtered_device(dab_index* idx, const void* d_queries, uint
                                      const uint64_t* d_query_masks, uint32_t match_all, dab_range** out) {
     return range_search(idx, "dab_range_search_filtered_device", false, d_queries, nq, l_search, beam_width, radius, has_inner_radius,
                         inner_radius, initial_slack, range_slack, max_returned, out, -1, false, true, d_query_masks, match_all);
+}
+
+// FilteredRange::search over a store (graph::ext::labeled::Filtered over the quantized strategies, labeled.rs:118-129)
+int dab_range_search_filtered_pq(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search, uint32_t beam_width, float radius,
+                                 int has_inner_radius, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned,
+                                 const uint64_t* query_masks, uint32_t match_all, int rerank, dab_range** out) {
+    return range_search(idx, "dab_range_search_filtered_pq", true, queries, nq, l_search, beam_width, radius, has_inner_radius, inner_radius,
+                        initial_slack, range_slack, max_returned, out, STORE_PQ, rerank != 0, true, query_masks, match_all);
+}
+
+int dab_range_search_filtered_pq_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t l_search, uint32_t beam_width,
+                                        float radius, int has_inner_radius, float inner_radius, float initial_slack, float range_slack,
+                                        uint64_t max_returned, const uint64_t* d_query_masks, uint32_t match_all, int rerank, dab_range** out) {
+    return range_search(idx, "dab_range_search_filtered_pq_device", false, d_queries, nq, l_search, beam_width, radius, has_inner_radius,
+                        inner_radius, initial_slack, range_slack, max_returned, out, STORE_PQ, rerank != 0, true, d_query_masks, match_all);
+}
+
+int dab_range_search_filtered_sq(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search, uint32_t beam_width, float radius,
+                                 int has_inner_radius, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned,
+                                 const uint64_t* query_masks, uint32_t match_all, int rerank, dab_range** out) {
+    return range_search(idx, "dab_range_search_filtered_sq", true, queries, nq, l_search, beam_width, radius, has_inner_radius, inner_radius,
+                        initial_slack, range_slack, max_returned, out, STORE_SQ, rerank != 0, true, query_masks, match_all);
+}
+
+int dab_range_search_filtered_sq_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t l_search, uint32_t beam_width,
+                                        float radius, int has_inner_radius, float inner_radius, float initial_slack, float range_slack,
+                                        uint64_t max_returned, const uint64_t* d_query_masks, uint32_t match_all, int rerank, dab_range** out) {
+    return range_search(idx, "dab_range_search_filtered_sq_device", false, d_queries, nq, l_search, beam_width, radius, has_inner_radius,
+                        inner_radius, initial_slack, range_slack, max_returned, out, STORE_SQ, rerank != 0, true, d_query_masks, match_all);
+}
+
+int dab_range_search_filtered_minmax(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search, uint32_t beam_width, float radius,
+                                     int has_inner_radius, float inner_radius, float initial_slack, float range_slack, uint64_t max_returned,
+                                     const uint64_t* query_masks, uint32_t match_all, int rerank, dab_range** out) {
+    return range_search(idx, "dab_range_search_filtered_minmax", true, queries, nq, l_search, beam_width, radius, has_inner_radius, inner_radius,
+                        initial_slack, range_slack, max_returned, out, STORE_MINMAX, rerank != 0, true, query_masks, match_all);
+}
+
+int dab_range_search_filtered_minmax_device(dab_index* idx, const void* d_queries, uint32_t nq, uint32_t l_search, uint32_t beam_width,
+                                            float radius, int has_inner_radius, float inner_radius, float initial_slack, float range_slack,
+                                            uint64_t max_returned, const uint64_t* d_query_masks, uint32_t match_all, int rerank,
+                                            dab_range** out) {
+    return range_search(idx, "dab_range_search_filtered_minmax_device", false, d_queries, nq, l_search, beam_width, radius, has_inner_radius,
+                        inner_radius, initial_slack, range_slack, max_returned, out, STORE_MINMAX, rerank != 0, true, d_query_masks, match_all);
 }
 
 int dab_range_search_pq(dab_index* idx, const void* queries, uint32_t nq, uint32_t l_search, uint32_t beam_width, float radius,

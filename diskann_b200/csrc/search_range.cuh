@@ -146,9 +146,17 @@ __device__ __forceinline__ void range_emit(const RangeParams& p, const uint32_t*
     }
 }
 
+// fast_distance's order as an unsigned key: -0.0 and +0.0 equal, every NaN after every number
+__device__ __forceinline__ uint32_t order_key(float d) {
+    if (d != d) return 0xFFFFFFFFu;
+    const uint32_t u = __float_as_uint(d == 0.0f ? 0.0f : d);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
 // ---- host (search_filtered.cu) ----------------------------------------------------------------------------------------
-// The filtered range kernel of this index's schema and its shape (plan.grid 0: no CTA fits, which the range search
-// reports; its passes cap the grid); fills p.f's shared-memory offsets
-int filtered_range_plan(const dab_index* idx, uint32_t l_search, uint32_t beam, FilteredRangeParams& p, WarpPlan<FilteredRangeParams>& plan);
+// The filtered range kernel of this index's schema (store -1) or of `store`, and its shape (plan.grid 0: no CTA fits,
+// which the range search reports; its passes cap the grid); fills p.f's shared-memory offsets
+int filtered_range_plan(const dab_index* idx, uint32_t l_search, uint32_t beam, int store, FilteredRangeParams& p,
+                        WarpPlan<FilteredRangeParams>& plan);
 
 }  // namespace dab

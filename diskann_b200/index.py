@@ -521,6 +521,67 @@ class GpuIndex:
                             beam_width=beam_width, inner_radius=inner_radius, initial_slack=initial_slack, range_slack=range_slack,
                             max_returned=max_returned, masks=C.c_void_p(d_masks), match_all=match_all)
 
+    def _range_filtered_quant(self, store, queries, masks, l_search, radius, match_all=False, rerank=False, **kw):
+        queries = self._queries(queries)
+        masks = np.ascontiguousarray(np.broadcast_to(np.asarray(masks, np.uint64), (queries.shape[0],)))
+        with RangeResults(self, getattr(_lib.lib(), f"dab_range_search_filtered_{store}"), _ptr(queries), len(queries), l_search, radius,
+                          masks=_ptr(masks), match_all=match_all, rerank=bool(rerank), **kw) as r:
+            offsets, cmps, hops, second = r.offsets()
+            ids, dists = r.results()
+        return offsets, ids, dists, cmps, hops, second
+
+    def range_search_filtered_pq(self, queries, masks, l_search, radius, *, match_all=False, beam_width=1, inner_radius=None,
+                                 initial_slack=1.0, range_slack=1.0, max_returned=None, rerank=False):
+        """range_search_filtered with every distance of both phases the PQ store's (those of search_batch_pq).
+        rerank=True: the returned matches (start points and deleted ids dropped) by full-precision distance, sorted by it
+        (NaN last), those above inner_radius, with it; no outer-radius filter, as in FilteredRange::search."""
+        return self._range_filtered_quant("pq", queries, masks, l_search, radius, match_all=match_all, beam_width=beam_width,
+                                          inner_radius=inner_radius, initial_slack=initial_slack, range_slack=range_slack,
+                                          max_returned=max_returned, rerank=rerank)
+
+    def range_search_filtered_sq(self, queries, masks, l_search, radius, *, match_all=False, beam_width=1, inner_radius=None,
+                                 initial_slack=1.0, range_slack=1.0, max_returned=None, rerank=False):
+        """range_search_filtered_pq over the scalar-quantized store (the distances of search_batch_sq)"""
+        return self._range_filtered_quant("sq", queries, masks, l_search, radius, match_all=match_all, beam_width=beam_width,
+                                          inner_radius=inner_radius, initial_slack=initial_slack, range_slack=range_slack,
+                                          max_returned=max_returned, rerank=rerank)
+
+    def range_search_filtered_minmax(self, queries, masks, l_search, radius, *, match_all=False, beam_width=1, inner_radius=None,
+                                     initial_slack=1.0, range_slack=1.0, max_returned=None, rerank=False):
+        """range_search_filtered_pq over the MinMax store (the distances of search_batch_minmax).  A query holding a NaN
+        after the store's transform fails the call."""
+        return self._range_filtered_quant("minmax", queries, masks, l_search, radius, match_all=match_all, beam_width=beam_width,
+                                          inner_radius=inner_radius, initial_slack=initial_slack, range_slack=range_slack,
+                                          max_returned=max_returned, rerank=rerank)
+
+    def _range_filtered_quant_device(self, store, d_queries, d_masks, nq, l_search, radius, match_all=False, rerank=False, **kw):
+        return RangeResults(self, getattr(_lib.lib(), f"dab_range_search_filtered_{store}_device"), C.c_void_p(d_queries), nq, l_search,
+                            radius, masks=C.c_void_p(d_masks), match_all=match_all, rerank=bool(rerank), **kw)
+
+    def range_search_filtered_pq_device(self, d_queries, d_masks, nq, l_search, radius, *, match_all=False, beam_width=1,
+                                        inner_radius=None, initial_slack=1.0, range_slack=1.0, max_returned=None, rerank=False):
+        """range_search_filtered_pq of `nq` queries and masks at the device pointers `d_queries` and `d_masks` (integers):
+        a RangeResults"""
+        return self._range_filtered_quant_device("pq", d_queries, d_masks, nq, l_search, radius, match_all=match_all, beam_width=beam_width,
+                                                 inner_radius=inner_radius, initial_slack=initial_slack, range_slack=range_slack,
+                                                 max_returned=max_returned, rerank=rerank)
+
+    def range_search_filtered_sq_device(self, d_queries, d_masks, nq, l_search, radius, *, match_all=False, beam_width=1,
+                                        inner_radius=None, initial_slack=1.0, range_slack=1.0, max_returned=None, rerank=False):
+        """range_search_filtered_sq of `nq` queries and masks at the device pointers `d_queries` and `d_masks` (integers):
+        a RangeResults"""
+        return self._range_filtered_quant_device("sq", d_queries, d_masks, nq, l_search, radius, match_all=match_all, beam_width=beam_width,
+                                                 inner_radius=inner_radius, initial_slack=initial_slack, range_slack=range_slack,
+                                                 max_returned=max_returned, rerank=rerank)
+
+    def range_search_filtered_minmax_device(self, d_queries, d_masks, nq, l_search, radius, *, match_all=False, beam_width=1,
+                                            inner_radius=None, initial_slack=1.0, range_slack=1.0, max_returned=None, rerank=False):
+        """range_search_filtered_minmax of `nq` queries and masks at the device pointers `d_queries` and `d_masks`
+        (integers): a RangeResults"""
+        return self._range_filtered_quant_device("minmax", d_queries, d_masks, nq, l_search, radius, match_all=match_all,
+                                                 beam_width=beam_width, inner_radius=inner_radius, initial_slack=initial_slack,
+                                                 range_slack=range_slack, max_returned=max_returned, rerank=rerank)
+
     def search_batch_device(self, d_queries, nq, k, l_search, beam_width, d_ids, d_dists, d_counts=0, d_cmps=0, d_hops=0):
         """Same with device pointers (integers); results stay in HBM."""
         check(_lib.lib().dab_search_batch_device(self._h, C.c_void_p(d_queries), nq, k, l_search, beam_width,
@@ -1072,12 +1133,13 @@ class RangeResults:
     def __init__(self, index, search, queries, nq, l_search, radius, beam_width=1, inner_radius=None, initial_slack=1.0,
                  range_slack=1.0, max_returned=None, rerank=None, masks=None, match_all=False):
         """`rerank`: None for the full-precision call, else the rerank flag of a quantized store's call; `masks`: None,
-        else the masks pointer of a filtered call, which takes match_all after it"""
+        else the masks pointer of a filtered call, which takes match_all after it (and the rerank flag after that over a
+        store)"""
         self._h = C.c_void_p()
         self.nq = int(nq)
-        store_args = () if rerank is None else (int(bool(rerank)),)
-        if masks is not None:
-            store_args = (masks, int(bool(match_all)))
+        store_args = () if masks is None else (masks, int(bool(match_all)))
+        if rerank is not None:
+            store_args += (int(bool(rerank)),)
         check(search(index._h, queries, self.nq, l_search, beam_width, radius, int(inner_radius is not None),
                      0.0 if inner_radius is None else inner_radius, initial_slack, range_slack, max_returned or 0, *store_args,
                      C.byref(self._h)))

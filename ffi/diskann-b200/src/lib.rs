@@ -346,6 +346,41 @@ impl<T: Element> GpuIndex<T> {
         self.range_quantized(sys::dab_range_search_minmax, queries, l_search, radius, args, rerank)
     }
 
+    /// `range_search_filtered` with every distance of both phases the PQ store's (those of `search_batch_pq`); `rerank`:
+    /// the returned matches by full-precision distance, sorted by it (NaN last), those above inner_radius, with it (no
+    /// outer-radius filter, as in `FilteredRange::search`).
+    pub fn range_search_filtered_pq(&self, queries: &[T], masks: &[u64], match_all: bool, l_search: u32, radius: f32, args: RangeArgs,
+                                    rerank: bool) -> Result<RangeBatch> {
+        self.range_filtered_quantized(sys::dab_range_search_filtered_pq, queries, masks, match_all, l_search, radius, args, rerank)
+    }
+
+    /// `range_search_filtered_pq` over the scalar-quantized store (the distances of `search_batch_sq`).
+    pub fn range_search_filtered_sq(&self, queries: &[T], masks: &[u64], match_all: bool, l_search: u32, radius: f32, args: RangeArgs,
+                                    rerank: bool) -> Result<RangeBatch> {
+        self.range_filtered_quantized(sys::dab_range_search_filtered_sq, queries, masks, match_all, l_search, radius, args, rerank)
+    }
+
+    /// `range_search_filtered_pq` over the MinMax store (the distances of `search_batch_minmax`).
+    pub fn range_search_filtered_minmax(&self, queries: &[T], masks: &[u64], match_all: bool, l_search: u32, radius: f32, args: RangeArgs,
+                                        rerank: bool) -> Result<RangeBatch> {
+        self.range_filtered_quantized(sys::dab_range_search_filtered_minmax, queries, masks, match_all, l_search, radius, args, rerank)
+    }
+
+    #[allow(clippy::too_many_arguments)]
+    fn range_filtered_quantized(&self, f: RangeFilteredQuantized, queries: &[T], masks: &[u64], match_all: bool, l_search: u32, radius: f32,
+                                args: RangeArgs, rerank: bool) -> Result<RangeBatch> {
+        assert_eq!(queries.len() % self.dim, 0);
+        let nq = queries.len() / self.dim;
+        assert_eq!(masks.len(), nq);
+        let mut set: *mut sys::dab_range = std::ptr::null_mut();
+        check(unsafe {
+            f(self.raw, queries.as_ptr() as *const c_void, nq as u32, l_search, args.beam_width, radius, args.inner_radius.is_some() as i32,
+              args.inner_radius.unwrap_or(0.0), args.initial_slack, args.range_slack, args.max_returned.unwrap_or(0), masks.as_ptr(),
+              match_all as u32, rerank as i32, &mut set)
+        })?;
+        take_range(set, nq)
+    }
+
     fn range_quantized(&self, f: RangeQuantized, queries: &[T], l_search: u32, radius: f32, args: RangeArgs, rerank: bool)
         -> Result<RangeBatch> {
         assert_eq!(queries.len() % self.dim, 0);
@@ -555,6 +590,9 @@ type FilteredQuantized = unsafe extern "C" fn(*mut sys::dab_index, *const c_void
                                               std::os::raw::c_int, *mut u32, *mut f32, *mut u32, *mut u32, *mut u32) -> std::os::raw::c_int;
 type RangeQuantized = unsafe extern "C" fn(*mut sys::dab_index, *const c_void, u32, u32, u32, f32, std::os::raw::c_int, f32, f32, f32, u64,
                                            std::os::raw::c_int, *mut *mut sys::dab_range) -> std::os::raw::c_int;
+type RangeFilteredQuantized = unsafe extern "C" fn(*mut sys::dab_index, *const c_void, u32, u32, u32, f32, std::os::raw::c_int, f32, f32, f32,
+                                                   u64, *const u64, u32, std::os::raw::c_int, *mut *mut sys::dab_range)
+                                                   -> std::os::raw::c_int;
 
 /// The offsets, stats and results of a range search's result set, which is freed
 fn take_range(set: *mut sys::dab_range, nq: usize) -> Result<RangeBatch> {

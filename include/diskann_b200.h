@@ -481,6 +481,63 @@ int dab_range_search_filtered_device(dab_index* idx, const void* d_queries, uint
                                      float initial_slack, float range_slack,
                                      uint64_t max_returned, const uint64_t* d_query_masks,
                                      uint32_t match_all, dab_range** out);
+/* FilteredRange::search over the PQ, SQ or MinMax store (graph::ext::labeled::Filtered over the
+ * quantized strategies): the arguments and result set of dab_range_search_filtered, plus `rerank`.
+ * Both phases are those of dab_range_search_filtered, and every distance of both is the store's,
+ * as in dab_range_search_{pq,sq,minmax} (SQ and MinMax compress the queries once, before the
+ * launch; a MinMax query holding a NaN after the transform fails the call, naming it).
+ *   rerank == 0: the results of dab_range_search_filtered with the store's distances.
+ *   rerank != 0: matched.take(max_returned) without start points and deleted ids; each id's
+ *     full-precision distance to the query; sorted by it (stable: ties in matched order, -0.0
+ *     equal to +0.0, NaN after every number: the reference leaves the order of NaN open); the ids
+ *     with d <= inner_radius of it (when has_inner_radius) dropped.  There is no outer-radius
+ *     filter, unlike dab_range_search_pq: FilteredRange::search checks only the inner radius, so the
+ *     results may hold ids whose full-precision distance is above radius, or NaN.  The result set
+ *     holds the full-precision distances.
+ * cmps, hops and second_round are those of the traversal, with or without rerank.  Checked before
+ * any device work, in this order: every check of dab_range_search_filtered (the shared-memory
+ * bound with the store's query area; the graph must be uploaded), then the store's (its rows
+ * uploaded, SQ not under Cosine, l_search + n_start <= 1024) and, with rerank, the full-precision
+ * vectors (DAB_ERR_NOT_READY) and the rerank's shared memory.  Without rerank only the graph, the
+ * store and the label table are needed.  DAB_ERR_OUT_OF_MEMORY as dab_range_search, the rerank's
+ * sort included. */
+int dab_range_search_filtered_pq(dab_index* idx, const void* queries, uint32_t nq,
+                                 uint32_t l_search, uint32_t beam_width, float radius,
+                                 int has_inner_radius, float inner_radius, float initial_slack,
+                                 float range_slack, uint64_t max_returned,
+                                 const uint64_t* query_masks, uint32_t match_all, int rerank,
+                                 dab_range** out);
+int dab_range_search_filtered_pq_device(dab_index* idx, const void* d_queries, uint32_t nq,
+                                        uint32_t l_search, uint32_t beam_width, float radius,
+                                        int has_inner_radius, float inner_radius,
+                                        float initial_slack, float range_slack,
+                                        uint64_t max_returned, const uint64_t* d_query_masks,
+                                        uint32_t match_all, int rerank, dab_range** out);
+int dab_range_search_filtered_sq(dab_index* idx, const void* queries, uint32_t nq,
+                                 uint32_t l_search, uint32_t beam_width, float radius,
+                                 int has_inner_radius, float inner_radius, float initial_slack,
+                                 float range_slack, uint64_t max_returned,
+                                 const uint64_t* query_masks, uint32_t match_all, int rerank,
+                                 dab_range** out);
+int dab_range_search_filtered_sq_device(dab_index* idx, const void* d_queries, uint32_t nq,
+                                        uint32_t l_search, uint32_t beam_width, float radius,
+                                        int has_inner_radius, float inner_radius,
+                                        float initial_slack, float range_slack,
+                                        uint64_t max_returned, const uint64_t* d_query_masks,
+                                        uint32_t match_all, int rerank, dab_range** out);
+int dab_range_search_filtered_minmax(dab_index* idx, const void* queries, uint32_t nq,
+                                     uint32_t l_search, uint32_t beam_width, float radius,
+                                     int has_inner_radius, float inner_radius,
+                                     float initial_slack, float range_slack,
+                                     uint64_t max_returned, const uint64_t* query_masks,
+                                     uint32_t match_all, int rerank, dab_range** out);
+int dab_range_search_filtered_minmax_device(dab_index* idx, const void* d_queries, uint32_t nq,
+                                            uint32_t l_search, uint32_t beam_width, float radius,
+                                            int has_inner_radius, float inner_radius,
+                                            float initial_slack, float range_slack,
+                                            uint64_t max_returned,
+                                            const uint64_t* d_query_masks, uint32_t match_all,
+                                            int rerank, dab_range** out);
 /* offsets [nq + 1]: query q's results are entries offsets[q] .. offsets[q + 1] - 1; cmps, hops
  * [nq] u32 and second_round [nq] (0 / 1) may be NULL.  Host buffers. */
 int dab_range_offsets(const dab_range* r, uint64_t* offsets, uint32_t* cmps, uint32_t* hops,

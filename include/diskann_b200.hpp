@@ -296,6 +296,18 @@ class GpuRange {
                                         max_returned_, masks, match_all ? 1 : 0, &set));
         return take(set, nq);
     }
+    // FilteredRange::search over the provider's PQ, SQ or MinMax store: every distance of both phases the store's;
+    // `rerank`: the returned matches by full-precision distance, sorted by it (NaN last), those above inner_radius, with
+    // it (no outer-radius filter, as in FilteredRange::search)
+    RangeResults search_filtered_pq(const T* queries, uint32_t nq, const uint64_t* masks, bool match_all = false, bool rerank = false) {
+        return search_filtered_store(dab_range_search_filtered_pq, queries, nq, masks, match_all, rerank);
+    }
+    RangeResults search_filtered_sq(const T* queries, uint32_t nq, const uint64_t* masks, bool match_all = false, bool rerank = false) {
+        return search_filtered_store(dab_range_search_filtered_sq, queries, nq, masks, match_all, rerank);
+    }
+    RangeResults search_filtered_minmax(const T* queries, uint32_t nq, const uint64_t* masks, bool match_all = false, bool rerank = false) {
+        return search_filtered_store(dab_range_search_filtered_minmax, queries, nq, masks, match_all, rerank);
+    }
 
    private:
     using StoreSearch = int (*)(dab_index*, const void*, uint32_t, uint32_t, uint32_t, float, int, float, float, float, uint64_t, int, dab_range**);
@@ -303,6 +315,14 @@ class GpuRange {
         dab_range* set = nullptr;
         check(f(p_.raw(), queries, nq, l_, beam_, radius_, has_inner_ ? 1 : 0, inner_, initial_slack_, range_slack_, max_returned_, rerank ? 1 : 0,
                 &set));
+        return take(set, nq);
+    }
+    using FilteredStoreSearch = int (*)(dab_index*, const void*, uint32_t, uint32_t, uint32_t, float, int, float, float, float, uint64_t,
+                                        const uint64_t*, uint32_t, int, dab_range**);
+    RangeResults search_filtered_store(FilteredStoreSearch f, const T* queries, uint32_t nq, const uint64_t* masks, bool match_all, bool rerank) {
+        dab_range* set = nullptr;
+        check(f(p_.raw(), queries, nq, l_, beam_, radius_, has_inner_ ? 1 : 0, inner_, initial_slack_, range_slack_, max_returned_, masks,
+                match_all ? 1 : 0, rerank ? 1 : 0, &set));
         return take(set, nq);
     }
     // the offsets, stats and results of a result set, which is freed

@@ -18,6 +18,8 @@ full-precision in-range sets.
 --selectivity S runs dab_range_search_filtered_device instead of the unfiltered call: bit 0 of the label table is set on
 a share S of the ids (seeded draw), every query's mask is that bit (ANY), and the exact sets are the in-range ids that
 carry it.  Its rows report the same numbers; phase 1 is not separated (the filtered traversal is part of the call).
+With --store, each radius also has a row for dab_range_search_filtered_{pq,sq,minmax}_device (with --rerank, its
+full-precision rerank) next to the fp_filtered row, with its average_precision against the same exact matching sets.
 usage: python tools/bench_range.py [--n N] [--nq NQ] [--reps R] [--beam B] [--store {fp,pq,sq,minmax}] [--rerank]
                                    [--selectivity S] [--json PATH]"""
 import argparse
@@ -99,7 +101,7 @@ def main():
         accepted = np.random.default_rng(bench.SEED_QUERY + 1).random(n + 1) < args.selectivity
         g.upload_labels(accepted.astype(np.uint64))
         d_masks = torch.ones(nq, dtype=torch.int64, device="cuda")
-        stores = ["fp_filtered"]
+        stores = ["fp_filtered"] if args.store == "fp" else ["fp_filtered", f"{args.store}_filtered"]
 
     def timed(call):
         call()
@@ -126,6 +128,9 @@ def main():
     def range_set(store, radius):
         if store == "fp_filtered":
             return g.range_search_filtered_device(d_q.data_ptr(), d_masks.data_ptr(), nq, L, radius, beam_width=args.beam)
+        if store.endswith("_filtered"):
+            return getattr(g, f"range_search_filtered_{args.store}_device")(d_q.data_ptr(), d_masks.data_ptr(), nq, L, radius,
+                                                                            beam_width=args.beam, rerank=args.rerank)
         if store == "fp":
             return g.range_search_device(d_q.data_ptr(), nq, L, radius, beam_width=args.beam)
         return getattr(g, f"range_search_{store}_device")(d_q.data_ptr(), nq, L, radius, beam_width=args.beam, rerank=args.rerank)
@@ -156,7 +161,7 @@ def main():
                 ids, _ = r.results()
             counts = np.diff(offsets.astype(np.int64))
             found = sum(len(np.intersect1d(truth[q], ids[offsets[q]:offsets[q + 1]])) for q in range(nq))
-            row = dict(store=store, rerank=args.rerank and store != "fp", target_mean_count=target, radius=radius,
+            row = dict(store=store, rerank=args.rerank and store not in ("fp", "fp_filtered"), target_mean_count=target, radius=radius,
                        exact_mean_count=round(float(exact.mean()), 2), exact_max_count=int(exact.max()), ms_per_batch=round(ms, 3),
                        phase1_ms=round(phase1.get(store, float("nan")), 3), phase2_ms=round(ms - phase1.get(store, float("nan")), 3),
                        qps=round(nq / ms * 1e3, 1),

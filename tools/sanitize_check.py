@@ -90,6 +90,8 @@ for dt, ddt, metric, d in ((np.float32, dab.DType.f32, dab.Metric.L2, 100), (np.
                 # search_kernel_pq_starts, range_kernel_quant<0>, then range_rerank_kernel and the segmented sort
                 g.range_search_pq(base[:32], 20, rad, initial_slack=0.2, rerank=rr)
                 g.search_batch_filtered_pq(base[:32], 0b101, 5, 40, 2, adaptive_l=(30, 4.0), rerank=rr)  # filtered_kernel_quant<0>
+                # filtered_range_kernel_quant<0>, then range_rerank_kernel, its unbounded count and filter, the sort
+                g.range_search_filtered_pq(base[:32], 0b101, 20, rad * 2, initial_slack=0.2, rerank=rr)
         f32 = base.astype(np.float32)
         std = float(f32.std())
         shift = (f32.mean(0) - np.float32(2.5 * std)).astype(np.float32)
@@ -104,6 +106,9 @@ for dt, ddt, metric, d in ((np.float32, dab.DType.f32, dab.Metric.L2, 100), (np.
             g.range_search_minmax(base[:32], 10, rad * 2, max_returned=70, initial_slack=0.2, rerank=rr)
             g.search_batch_filtered_sq(base[:32], 0b11, 5, 40, 4, match_all=True, rerank=rr)  # filtered_kernel_quant<1> and <2>
             g.search_batch_filtered_minmax(base[:32], 0b101, 5, 40, 1, adaptive_l=(50, 8.0), rerank=rr)
+            # filtered_range_kernel_quant<1> and <2>
+            g.range_search_filtered_sq(base[:32], 0b11, 10, rad * 2, match_all=True, beam_width=4, max_returned=70, rerank=rr)
+            g.range_search_filtered_minmax(base[:32], 0b101, 20, rad * 2, initial_slack=0.2, rerank=rr)
         print(dt.__name__, "deg max", int(adj[:, 0].max()), "search ok", int(got[2].min()), int(got4[2].min()), int(div[2].min()), int(div4[2].min()),
               "filtered", int(flt[2].sum()), int(flt4[2].sum()),
               "finite", bool(np.isfinite(out[1:]).all() and np.isfinite(pairs).all() and np.isfinite(block).all()), knn[0].shape)
